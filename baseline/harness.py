@@ -1,6 +1,6 @@
-"""Stand-in for "the reference's own NCCL(+cuBLAS) build" (BASELINE.md §2, SURVEY §6).
+"""Stand-in for "the reference's own NCCL(+cuBLAS) build" (BASELINE.md §2).
 
-The reference (TensorFlow-1.0 + PySpark, /root/reference/src/rnn.py) has no GPU/NCCL code path and cannot run in this
+The reference (TensorFlow-1.0 + PySpark, original src/rnn.py) has no GPU/NCCL code path and cannot run in this
 image, so the bar our kernels are measured against is built here from stock library parts only — none of this
 framework's models, kernels or engine:
 

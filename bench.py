@@ -2,7 +2,7 @@
 """Headline benchmark (BASELINE.json): samples/sec of the 2-layer-1024 LSTM, seq_len 128, batch 256 per GPU, bf16,
 per-step gradient allreduce, synthetic sequences / random-init weights.
 
-    python bench.py --gpus N --steps K --warmup W [--impl ours|reference|baseline]
+    python bench.py --gpus N --steps K --warmup W [--impl ours|reference|baseline] [--dump-outputs DIR]
 
 N > 1 is launched by the driver under torchrun (RANK / LOCAL_RANK / WORLD_SIZE / MASTER_* from the env), one rank
 per GPU.  Rank 0 prints ONE JSON line.  ``value`` is the whole-job aggregate (sum over GPUs); timing is CUDA events
@@ -10,9 +10,13 @@ on the launching stream bracketed by barrier + synchronize, max over ranks.
 
   --impl ours       this framework through its public API (lstm_tensorspark_b200.engine.TrainEngine)
   --impl reference  the unmodified reference from baseline/_ref — it is Python-2 / TF-1.0 / PySpark source without
-                    packaging metadata and cannot be installed here (DESIGN.md §Reference arm) -> "unavailable"
+                    packaging metadata and cannot be installed here -> "unavailable"
   --impl baseline   our stand-in for "the reference's own NCCL(+cuBLAS) build" (BASELINE.md §2): cuDNN nn.LSTM +
                     NCCL all_reduce + torch fused Adam, same model / schedule (baseline/harness.py)
+
+--dump-outputs DIR (--impl ours): after the device-timed steps, rank 0 writes what the last timed step computed - its loss and a
+fixed, seeded sample of 2^20 entries of the updated parameters and of the gradients - as DIR/{loss,params,grads}.npy (float32).
+Inputs and initial weights are seeded, so two builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -37,6 +41,8 @@ def parse():
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference", "baseline"])
+    ap.add_argument("--dump-outputs", dest="dump_outputs", default=None, metavar="DIR",
+                    help="--impl ours only: write the last timed step's loss / parameter and gradient samples as .npy files into DIR")
     ap.add_argument("--comm", default="auto", help="ours: fused (default for N>1) | nccl")
     ap.add_argument("--optimizer", default="adam")
     ap.add_argument("--cuda_graph", type=int, default=-1, help="-1 auto (capture the step when there is one rank), 0 eager, 1 force")
@@ -53,11 +59,14 @@ def parse():
     ap.add_argument("--config", type=int, default=3, choices=[3, 4],
                     help="BASELINE.json config: 3 = 2x1024 T=128 B=256 per-step grad allreduce (headline); "
                          "4 = 4x2048 T=512 B=64 per-epoch parameter average (one average inside the timed region)")
-    return ap.parse_args()
+    args = ap.parse_args()
+    if args.dump_outputs and args.impl != "ours":
+        ap.error("--dump-outputs needs --impl ours")
+    return args
 
 
 class ClockSampler:
-    """nvidia-smi clocks + throttle reasons DURING the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi clocks + throttle reasons DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -199,13 +208,15 @@ def timed_loop(torch, dist, world, device, step_fn, steps, warmup, clocks=None):
     return ms
 
 
-def measure(torch, dist, world, device, local, step_dev, step_e2e, steps, warmup, no_e2e, B, n_gpus, h2d, d2h):
-    """Device-timed loop (+ clocks sampled during it) and the end-to-end loop of one arm."""
+def measure(torch, dist, world, device, local, step_dev, step_e2e, steps, warmup, no_e2e, B, n_gpus, h2d, d2h, after_timed=None):
+    """Device-timed loop (+ clocks sampled during it) and the end-to-end loop of one arm.  ``after_timed`` runs between them."""
     clocks = ClockSampler(local)
     clocks.start()
     time.sleep(0.3)
     ms = timed_loop(torch, dist, world, device, step_dev, steps, warmup, clocks)
     clk = clocks.stop()
+    if after_timed is not None:
+        after_timed()
     e2e = None
     if not no_e2e:
         ms_e2e = timed_loop(torch, dist, world, device, step_e2e, steps, max(3, warmup // 2))
@@ -319,14 +330,27 @@ def main():
         xs, ys = Dm.synthetic_sequences(nb * B, T, D, C, seed=1234 + rank)
         dev_x = torch.as_tensor(xs).to(device=device, dtype=torch.bfloat16)
         dev_y = torch.as_tensor(ys).to(device)
-        it = {"i": 0}
+        it = {"i": 0, "loss": None}
 
         def step_dev():
             i = it["i"] % nb
             it["i"] += 1
             loss = eng.step(dev_x[i * B:(i + 1) * B], dev_y[i * B:(i + 1) * B])
             eng.maybe_average()                       # config 4: the per-epoch parameter average (every `steps` steps)
+            it["loss"] = loss
             return loss
+
+        def dump_outputs():
+            if not args.dump_outputs or rank != 0:
+                return
+            import numpy as np
+            torch.cuda.synchronize(device)
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            n = eng.flat.data.numel()
+            idx = torch.randperm(n, generator=torch.Generator().manual_seed(0))[:min(n, 1 << 20)].sort().values.to(device)
+            out = {"loss": it["loss"].float().reshape(1), "params": eng.flat.data[idx], "grads": eng.flat.grad[idx]}
+            for name, t in out.items():
+                np.save(os.path.join(args.dump_outputs, name + ".npy"), t.detach().float().cpu().numpy())
 
         loader = Dm.PinnedHostLoader(xs, ys, B, device, dtype=torch.bfloat16, shuffle=False, seed=rank, depth=args.e2e_depth)
         e2e_dbg = os.environ.get("LSTM_TS_E2E_DEBUG", "")              # diagnostics: "nocopy" (no H2D DMA), "lagN" (read the loss N steps late)
@@ -383,7 +407,8 @@ def main():
                 eng._graph, eng._bound = None, {}
                 torch.cuda.synchronize(device)
         h2d, d2h = loader.bytes_per_batch, 4
-        ms, clk, e2e = measure(torch, dist, world, device, local, step_dev, step_e2e, args.steps, args.warmup, args.no_e2e, B, n_gpus, h2d, d2h)
+        ms, clk, e2e = measure(torch, dist, world, device, local, step_dev, step_e2e, args.steps, args.warmup, args.no_e2e, B, n_gpus, h2d, d2h,
+                               after_timed=dump_outputs)
         cuda_lstm.check_kernel_errors(device)
         if hasattr(comm, "check_errors"):
             comm.check_errors()
@@ -405,7 +430,7 @@ def main():
            "vs_baseline": None, "dtype": "bf16", "data": "synthetic", "impl": args.impl,
            "config": {"model": model_name, "global_batch": B * n_gpus, "per_gpu_batch": B, "seq_len": T, "in_features": D,
                       "num_classes": C, "parallelism": par, "sync": sync_label,
-                      "l2": "per-step working set (activations+inputs, >1 GB) exceeds the 126 MB L2; 4 rotating input batches",
+                      "l2": "per-step working set (activations+inputs, >1 GB) exceeds the 50 MB L2 of an H100; 4 rotating input batches",
                       **cfg_extra},
            "clocks": clk, "gpu_launches": launches * args.steps}
     if e2e is not None:

@@ -6,7 +6,7 @@
 For every message size: our fused kernel (one-shot / two-shot, peer-pointer / NVLS multicast) doing the in-place
 fp32 average + bf16 shadow refresh, against ``dist.all_reduce`` + the separate scale kernel the NCCL path needs.
 Device-timed with CUDA events, max over ranks.  Reports algorithm bandwidth S/t and bus bandwidth 2(N-1)/N * S/t
-against 900 GB/s/dir nominal (770 GB/s measured peer copy, B200_PROFILING.md).
+against the 450 GB/s/dir NVLink 4 nominal of an H100 (not measured here).
 """
 from __future__ import annotations
 
@@ -62,7 +62,7 @@ def main():
         if comm.arena.mc_base:
             variants.append(("two_shot_nvls", "two_shot", "force", 0, False))
         if tune and size >= (1 << 22):
-            variants += [("p2p_b128", "two_shot", "0", 128, False), ("p2p_b148", "two_shot", "0", 148, False), ("p2p_b256", "two_shot", "0", 256, False)]
+            variants += [("p2p_b128", "two_shot", "0", 128, False), ("p2p_b132", "two_shot", "0", 132, False), ("p2p_b256", "two_shot", "0", 256, False)]
         if comm.arena.mc_base:
             if tune and size >= (1 << 22):
                 variants += [("nvls_b64", "two_shot", "auto", 64, False), ("nvls_b128", "two_shot", "auto", 128, False),

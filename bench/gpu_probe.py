@@ -85,7 +85,7 @@ def check_simple():
 
 
 def check_gemm2():
-    """General tcgen05 GEMM: every operand-major combination, 1- and 2-CTA tiles, accumulate, ragged shapes, then timing
+    """General wgmma GEMM: every operand-major combination, 1- and 2-CTA tiles, accumulate, ragged shapes, then timing
     of the training-step shapes against cuBLAS."""
     import torch
     from lstm_tensorspark_b200.ops.cuda_ext import ext
@@ -177,7 +177,7 @@ def check_gemm2_dw():
     t("dW TN on transposed copies (dG^T, X^T K-major)", lambda: E.gemm2(dGT, XT, out=gw, out_fp32=True))
     t("dW A K-major (dG^T), B MN (X)", lambda: E.gemm2(dGT, X, out=gw, b_mn=True, out_fp32=True))
     t("dW A MN (dG), B K-major (X^T)", lambda: E.gemm2(dG, XT, out=gw, a_mn=True, out_fp32=True))
-    for mc in (64, 96, 128, 148):
+    for mc in (64, 96, 128, 132):
         t(f"dW NT max_ctas={mc}", lambda: E.gemm2(dG, X, out=gw, a_mn=True, b_mn=True, out_fp32=True, max_ctas=mc))
     t("dW NT 1-CTA bn256", lambda: E.gemm2(dG, X, out=gw, a_mn=True, b_mn=True, out_fp32=True, ctas=1, bn=256))
     t("dW NT 2-CTA bn128", lambda: E.gemm2(dG, X, out=gw, a_mn=True, b_mn=True, out_fp32=True, ctas=2, bn=128))

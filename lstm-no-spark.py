@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Standalone entry point (world_size = 1, CPU-capable): the counterpart of
-/root/reference/src/lstm-no-spark.py:261-288."""
+original src/lstm-no-spark.py:261-288."""
 import sys
 
 from lstm_tensorspark_b200.config import parse_args

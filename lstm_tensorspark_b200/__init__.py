@@ -1,5 +1,5 @@
 """lstm_tensorspark_b200 — a Blackwell-native distributed LSTM trainer with the capabilities, CLI and
-checkpoint layout of EmanuelOverflow/LSTM-TensorSpark (see SURVEY.md, DESIGN.md)."""
+checkpoint layout of EmanuelOverflow/LSTM-TensorSpark."""
 __version__ = "0.1.0"
 
 from .config import Config, parse_args          # noqa: F401

@@ -1,10 +1,10 @@
-"""In-tree build of the sm_100a extension (``lstm_tensorspark_b200/_C*.so``).
+"""In-tree build of the sm_90a (H100) extension (``lstm_tensorspark_b200/_C*.so``).
 
-Kernels (``csrc/*.cu``) are compiled by plain ``nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo`` —
+Kernels (``csrc/*.cu``) are compiled by plain ``nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo`` —
 they depend on the CUDA runtime only, so a file builds in seconds and ``cuobjdump -sass`` of the result is
 readable; ``csrc/bindings.cpp`` (the only translation unit that sees torch headers) is compiled by g++ and
 everything is linked into ONE shared object next to the package so it travels with the source tree.
-nvcc cross-compiles without a GPU, so this runs on the CPU-only dev box.
+nvcc cross-compiles without a GPU, so this runs on a machine without one.
 
     python -m lstm_tensorspark_b200.build [--force] [--verbose] [--sass]
 """
@@ -26,7 +26,7 @@ BUILD = os.path.join(HERE, "build")
 SO_NAME = "_C" + (sysconfig.get_config_var("EXT_SUFFIX") or ".so")
 SO_PATH = os.path.join(HERE, SO_NAME)
 
-ARCH_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ["-O3", "-std=c++17", "-lineinfo", "--use_fast_math", "-Xcompiler", "-fPIC", "-Xptxas", "-v",
               "--expt-relaxed-constexpr", "-DNDEBUG"] + ARCH_FLAGS
 
@@ -143,15 +143,13 @@ def dump_sass(out_dir: str) -> List[str]:
     return outs
 
 
-# lstm_seq_tcgen05.cu has ~30 template instantiations (ring depths, tuning variants): the committed listing keeps the
-# ones that run by default (wavefront: forward 6-stage / backward 4-stage with two batch tiles per CTA; single layer: forward
-# K-split 5-stage, backward 5-stage; streamed-weights 8-stage; prologue).
-# gemm2_tcgen05.cu has 48 (cta_group x tile x operand majors x output mode); kept: the 2-CTA x-projection / dX / dW kernels and the
-# single-CTA dataflow-gated ones of the layer wavefront.
-SASS_KEEP = {"lstm_seq_tcgen05.cu": ("ILb0ELi6ELi2ELb0ELb0E", "ILb1ELi4ELi2ELb0ELb0E", "ILb0ELi5ELi1ELb0ELb1E", "ILb1ELi5ELi1ELb0ELb0E",
-                                     "ILb0ELi8ELi1ELb1ELb0E", "seq_prologue_kernel"),
-             "gemm2_tcgen05.cu": ("ILi2ELi256ELb0ELb0ELi0E", "ILi2ELi256ELb0ELb1ELi0E", "ILi2ELi256ELb1ELb1ELi1E", "ILi2ELi256ELb1ELb1ELi2E",
-                                  "ILi1ELi256ELb0ELb0ELi0E", "ILi1ELi256ELb0ELb1ELi0E")}
+# lstm_seq_wgmma.cu has ~30 template instantiations (ring depths, tuning variants): the listing keeps the forward and backward
+# kernels with one and two batch tiles per CTA at the ring depths H = 1024 gets, the streamed-weights kernels and the prologue.
+# gemm2_wgmma.cu has 48 (cluster size x tile x operand majors x output mode); kept: the default 2-CTA 256-wide kernels of the
+# x-projection (TN, bf16 out), dX (B MN-major, bf16 out) and the weight gradients (both MN-major, fp32 accumulate).
+SASS_KEEP = {"lstm_seq_wgmma.cu": ("ILb0ELi4ELi1ELb0ELb0E", "ILb0ELi4ELi2ELb0ELb0E", "ILb1ELi3ELi1ELb0ELb0E", "ILb1ELi2ELi2ELb0ELb0E",
+                                  "ILb0ELi8ELi1ELb1ELb0E", "ILb1ELi8ELi1ELb1ELb0E", "seq_prologue_kernel"),
+             "gemm2_wgmma.cu": ("ILi2ELi256ELb0ELb0ELi0E", "ILi2ELi256ELb0ELb1ELi0E", "ILi2ELi256ELb1ELb1ELi2E")}
 
 
 def _filter_sass(text: str, keep) -> str:

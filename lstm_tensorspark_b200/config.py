@@ -1,9 +1,9 @@
 """Flag system shared by both entry points (``rnn.py`` and ``lstm-no-spark.py``).
 
 Parity targets (reference, read-only):
-  * distributed CLI  : /root/reference/src/rnn.py:306-336   (argparse, ``parse_known_args``)
-  * standalone flags : /root/reference/src/lstm-no-spark.py:9-38 (``tf.app.flags`` + ``params_str`` dump)
-  * ``net_settings``  : /root/reference/src/rnn.py:376-389
+  * distributed CLI  : original src/rnn.py:306-336   (argparse, ``parse_known_args``)
+  * standalone flags : original src/lstm-no-spark.py:9-38 (``tf.app.flags`` + ``params_str`` dump)
+  * ``net_settings``  : original src/rnn.py:376-389
 
 One dataclass, one parser.  Every reference flag keeps its name, type and default; the Spark-only flags
 (``--master``, ``--spark_exec_memory``) are accepted and ignored.  New flags are additive.
@@ -40,7 +40,7 @@ class Config:
     seq_len: int = 1                    # time steps per sample (reference == 1)
     dtype: str = "auto"                 # auto: bf16 on cuda, fp32 on cpu
     device: str = "auto"                # auto | cpu | cuda
-    backend: str = "auto"               # auto | cuda_ext (hand-written sm_100a kernels) | torch
+    backend: str = "auto"               # auto | cuda_ext (hand-written sm_90a kernels) | torch
     optimizer: str = "adam"             # adam (TF formulation) | sgd
     sync_mode: str = "param_avg"        # param_avg (reference) | grad_allreduce | none
     sync_every: int = 0                 # 0 => once at the end of training (reference); N => every N steps
@@ -163,7 +163,7 @@ _HELP = {
 
 
 def build_parser(standalone: bool = False) -> argparse.ArgumentParser:
-    desc = "RNN-LSTM on B200 (standalone)" if standalone else "RNN-LSTM on B200 (one rank per partition)"
+    desc = "RNN-LSTM on H100 (standalone)" if standalone else "RNN-LSTM on H100 (one rank per partition)"
     p = argparse.ArgumentParser(description=desc)
     defaults = Config()
     for f in dataclasses.fields(Config):

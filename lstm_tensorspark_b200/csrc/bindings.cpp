@@ -1,4 +1,4 @@
-// Python bindings for the sm_100a kernels (the only translation unit that sees torch headers).
+// Python bindings for the sm_90a kernels (the only translation unit that sees torch headers).
 // Every function validates device / dtype / contiguity, takes the CURRENT torch CUDA stream (so the kernels
 // are stream-ordered with the rest of the step and capturable in CUDA graphs) and forwards raw pointers to the
 // C-ABI launchers defined next to the kernels.
@@ -174,8 +174,8 @@ std::vector<Tensor> xent_rows(const Tensor& logits, const Tensor& labels) {
   return {dlogits, loss, correct};
 }
 
-// Tensor-core head (csrc/head_tc.cu): bf16 h [B,H] (row pitch = stride(0)), fp32 W [H,C] / bias [C] -> logits, dlogits, loss sum,
-// correct count.  Shapes the tcgen05 kernel does not take (fp32 h, C > 256, weight image > smem) run head_logits_generic +
+// Tensor-core head (csrc/head_wgmma.cu): bf16 h [B,H] (row pitch = stride(0)), fp32 W [H,C] / bias [C] -> logits, dlogits, loss sum,
+// correct count.  Shapes the wgmma kernel does not take (fp32 h, C > 256, weight image > smem) run head_logits_generic +
 // xent_rows - our own kernels, never a library GEMM.
 std::vector<Tensor> head_fwd(const Tensor& h, const Tensor& W, const Tensor& bias, const Tensor& labels) {
   TORCH_CHECK(h.is_cuda() && h.dim() == 2 && h.stride(1) == 1, "head_fwd: h [B,H] with unit inner stride");
@@ -260,7 +260,7 @@ void fused_allreduce(const Tensor& ptrs, int64_t mc_in, int64_t mc_param, int64_
         "fused_allreduce");
 }
 
-// ---- general tcgen05 GEMM (csrc/gemm2_tcgen05.cu): C[M,N] (=|+=) op(A)·op(B) (+bias) ------------------------------------
+// ---- general wgmma GEMM (csrc/gemm2_wgmma.cu): C[M,N] (=|+=) op(A)·op(B) (+bias) ------------------------------------
 // a_mn = false: A is [M,K] (K contiguous); true: A is [K,M] (M contiguous).  b_mn = false: B is [N,K]; true: B is [K,N].
 // out: optional preallocated C (fp32 for accumulate = C += A·B, or any mode); out_fp32 selects the dtype of a fresh C.
 Tensor gemm2(const Tensor& A, const Tensor& B, const std::optional<Tensor>& bias, std::optional<Tensor> out, bool a_mn, bool b_mn,
@@ -325,7 +325,7 @@ Tensor gemm_generic(const Tensor& A, const Tensor& B, const std::optional<Tensor
   return C;
 }
 
-// ---- persistent tcgen05 LSTM sequence kernels ------------------------------------------------------------------
+// ---- persistent wgmma LSTM sequence kernels ------------------------------------------------------------------
 // gx [T,B,4H] bf16 (x·Wx^T, no bias), w_h [4H,H] bf16, bias fp32 [4H], h0 bf16 [B,H], c0 fp32 [B,H]
 // -> h_seq [T+1,B,H] bf16 (row 0 = h0), c_seq [T+1,B,H] fp32, act [T,B,4H] bf16
 // in_gate (wavefront): completion counters of the GEMM that is still producing gx while this kernel runs (see SeqParams);
@@ -421,7 +421,7 @@ void lstm_seq_bwd_into(const std::optional<Tensor>& dh_seq, const Tensor& w_hT, 
 }  // namespace
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
-  m.doc() = "lstm_tensorspark_b200 sm_100a kernels";
+  m.doc() = "lstm_tensorspark_b200 sm_90a kernels";
   m.def("lstm_pointwise_fwd", &lstm_pointwise_fwd);
   m.def("transpose01", &transpose01);
   m.def("transpose2d", &transpose2d);

@@ -3,7 +3,7 @@
 // No NCCL call and no separate elementwise kernel on this path.
 //
 // Replaces: Spark reduceByKey(mean) + collect of the 8 gate-keyed weight records, once per job
-// (/root/reference/src/rnn.py:393-407; K15 in SURVEY §2.5) — and, for per-step gradient sync, the
+// (original src/rnn.py:393-407) — and, for per-step gradient sync, the
 // allreduce + ApplyAdam pair a NCCL build would run.
 //
 // Buffers are NVLink-symmetric (same offset on every rank); the host passes every rank's base pointer.
@@ -237,7 +237,7 @@ __global__ void __launch_bounds__(kThreads) ar_one_shot_kernel(const __grid_cons
 template <typename K>
 int launch_k(K kern, const ARArgs& a, int blocks, int pdl, cudaStream_t st) {
   // no shared memory of our own, but ask for the max-shared L1 split: the split the tensor-core kernels run with, so that
-  // these CTAs can be co-resident with a weight-gradient GEMM on the same SMs (see gemm2_tcgen05.cu)
+  // these CTAs can be co-resident with a weight-gradient GEMM on the same SMs (see gemm2_wgmma.cu)
   cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(blocks); cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = 0; cfg.stream = st;

@@ -1,7 +1,7 @@
 // Any-shape GEMM on the CUDA cores:  C[M,N] = beta * C + A[M,K] · B[K,N]  with arbitrary element strides (so every
-// transpose is free), bf16 or fp32 operands, fp32 accumulation.  It serves the shapes the tcgen05 kernels cannot take
+// transpose is free), bf16 or fp32 operands, fp32 accumulation.  It serves the shapes the tensor-core kernels cannot take
 // (TMA needs 16 B-aligned pitches and the tensor-core tiles 64-wide K blocks): the reference's own configuration - iris,
-// in_features = 4, hidden 16, batch 10, ONE time step (/root/reference/src/rnn.py:312-321, lstm.py:88-91) - and the fp32
+// in_features = 4, hidden 16, batch 10, ONE time step (original src/rnn.py:312-321, lstm.py:88-91) - and the fp32
 // parity path.  Performance target: none; these products are a few kFLOP.  Keeping them on our own kernel means the
 // product path never calls a library GEMM.
 #include "ts_common.cuh"

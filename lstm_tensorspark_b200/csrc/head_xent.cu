@@ -1,7 +1,7 @@
 // K-HEAD, generic half: sparse softmax cross-entropy + accuracy + dlogits over logits that are already computed (the shapes
-// the tensor-core head of head_tc.cu does not take: fp32 activations, more than 256 classes).  One warp per batch row.
+// the tensor-core head of head_wgmma.cu does not take: fp32 activations, more than 256 classes).  One warp per batch row.
 // Reference: sparse_softmax_cross_entropy_with_logits -> reduce_mean -> argmax/equal/cast/reduce_mean
-// (/root/reference/src/rnn.py:55-63, 84-92; K10-K11 in SURVEY §2.5).
+// (original src/rnn.py:55-63, 84-92).
 #include "ts_common.cuh"
 
 namespace {

@@ -1,8 +1,8 @@
 // Generic-shape LSTM cell epilogue kernels (any B, H): gate activations + c/h update (forward) and the
 // gate-gradient math (backward), each ONE launch per time step instead of the reference's ~19 elementwise
-// TF ops per layer per step (reference: /root/reference/src/models/recurrent/lstm.py:93-109, K3-K7 in SURVEY §2.5).
+// TF ops per layer per step (reference: original src/models/recurrent/lstm.py:93-109).
 // The 4-gate GEMM that feeds them is a library GEMM on this path; shapes that fit the tensor-core tiling
-// take the persistent tcgen05 kernel in lstm_seq_tcgen05.cu instead.
+// take the persistent wgmma kernel in lstm_seq_wgmma.cu instead.
 //
 // Layout: pre/act/dpre are [B, 4H] with column n = 4*j + g, g: 0=i 1=f 2=g(candidate) 3=o. c is fp32.
 #include "ts_common.cuh"
@@ -111,7 +111,7 @@ extern "C" int ts_transpose01_rows(const void* src, void* dst, int B, int T, lon
   const int vec = (int)(row_bytes / 16);
   const long long total = (long long)B * T * vec;
   int blocks = (int)((total + 255) / 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   transpose01_rows_kernel<<<blocks, 256, 0, st>>>((const uint4*)src, (uint4*)dst, B, T, vec);
   return (int)cudaGetLastError();
 }

@@ -1,7 +1,7 @@
 // K-OPT: ONE launch over the flat fp32 master buffer (Adam, TF-1.0 "epsilon-hat" formulation, or SGD) that
 // also refreshes the bf16 shadow the tensor-core kernels read.  Replaces the reference's one ApplyAdam
-// kernel per variable (14*L+2 launches per step; /root/reference/src/rnn.py:207,224; K14 in SURVEY §2.5).
-// Memory-bound: 16 B vector loads/stores, grid = 148 SMs x 8 resident CTAs, grid-stride.
+// kernel per variable (14*L+2 launches per step; original src/rnn.py:207,224).
+// Memory-bound: 16 B vector loads/stores, grid = 132 SMs (H100) x 8 resident CTAs, grid-stride.
 #include "ts_common.cuh"
 
 namespace {
@@ -69,7 +69,7 @@ __global__ void __launch_bounds__(256) cast_bf16_kernel(const float4* __restrict
 
 int grid_for(size_t n4) {
   size_t want = (n4 + 255) / 256;
-  size_t cap = 148 * 8;
+  size_t cap = 132 * 8;
   return (int)(want < cap ? (want ? want : 1) : cap);
 }
 

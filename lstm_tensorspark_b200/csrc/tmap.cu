@@ -76,7 +76,7 @@ int sm_count(int dev) {
   if (!cached[dev]) {
     int n = 0;
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    cached[dev] = n > 0 ? n : 148;
+    cached[dev] = n > 0 ? n : 132;
   }
   return cached[dev];
 }

@@ -1,4 +1,4 @@
-// Shared helpers for the sm_100a kernels of lstm_tensorspark_b200.
+// Shared helpers for the sm_90a kernels of lstm_tensorspark_b200.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>

@@ -1,13 +1,13 @@
 """Data layer: CSV reader, sharder, row parser, normaliser, batch iterators, synthetic sequences.
 
 Parity targets (reference, read-only):
-  * ``csv_to_partitions`` / ``text_to_rdd``  /root/reference/src/rnn.py:104-138
-  * ``process_batch``                         /root/reference/src/rnn.py:141-158
-  * ``next_batch``                            /root/reference/src/rnn.py:161-177
-  * ``min_max_normalizer``                    /root/reference/src/rnn.py:95-101
-  * standalone ``csv_to_batch`` / ``read_dataset_from_path``  /root/reference/src/lstm-no-spark.py:90-112,254-258
+  * ``csv_to_partitions`` / ``text_to_rdd``  original src/rnn.py:104-138
+  * ``process_batch``                         original src/rnn.py:141-158
+  * ``next_batch``                            original src/rnn.py:161-177
+  * ``min_max_normalizer``                    original src/rnn.py:95-101
+  * standalone ``csv_to_batch`` / ``read_dataset_from_path``  original src/lstm-no-spark.py:90-112,254-258
 
-Decisions where the reference is defective (SURVEY.md §2.8): Q2 (remainder shard hang) -> exactly P
+Decisions where the reference is defective: Q2 (remainder shard hang) -> exactly P
 shards of floor(N/P) rows, remainder dropped or spread; a shard smaller than the batch is an error, never
 a hang.  Q10: labels are parsed to int64 up front.  Q3: ``batch_size == 0`` means the whole shard.
 """

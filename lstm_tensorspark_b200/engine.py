@@ -5,7 +5,7 @@ This is what ``bench.py``, ``__graft_entry__.smoke`` and the per-replica trainer
     eng = TrainEngine(cfg, rank, world_size, comm, batch_size=B)
     loss = eng.step(x, y)            # forward, backward, (fused allreduce +) optimizer update
 
-One step replaces the reference's ``sess.run([train_op, loss], feed_dict=...)`` (/root/reference/src/rnn.py:264-267):
+One step replaces the reference's ``sess.run([train_op, loss], feed_dict=...)`` (original src/rnn.py:264-267):
 H2D feed, forward, backward, 14·L+2 ApplyAdam launches, D2H loss.  With ``cuda_graph=True`` the whole step is
 captured once and replayed (launch-bound inner loops belong in CUDA graphs, not in a tracing compiler).
 """
@@ -59,7 +59,7 @@ class TrainEngine:
             self.optimizer = train_optimizer(cfg.learning_rate)(self.flat)
         else:
             self.optimizer = FlatOptimizer(self.flat, cfg.learning_rate, cfg.optimizer, weight_decay=0.0)
-        # K12: the optional L2 term of create_variable (/root/reference/src/models/recurrent/lstm.py:9-11) is folded into the
+        # K12: the optional L2 term of create_variable (original src/models/recurrent/lstm.py:9-11) is folded into the
         # update kernel (g + wd * w over the LSTM weight / bias segment) instead of an autograd term over 67 MB of weights;
         # variables outside that segment that asked for decay (learned initial states) keep the autograd term
         self.optimizer.weight_decay = float(cfg.weight_decay or 0.0)
@@ -80,7 +80,7 @@ class TrainEngine:
     def _make_bucket_plan(self):
         """Gradient buckets in the order backward finishes them: [top layer (+ head)], ..., [layer 0].  A bucket = a
         contiguous element range of the flat buffer + the parameters that must have been written before it may be synced.
-        (Reference counterpart: the one-shot reduceByKey over all weights, /root/reference/src/rnn.py:393-407 - here the sync
+        (Reference counterpart: the one-shot reduceByKey over all weights, original src/rnn.py:393-407 - here the sync
         of the upper layers hides under the backward recurrence of the layers below.)"""
         flat = self.flat
         if not flat._direct:

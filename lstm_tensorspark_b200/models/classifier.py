@@ -1,5 +1,5 @@
 """RNN + dense softmax head = the network the reference trainer assembles inline
-(/root/reference/src/rnn.py:203-228): placeholders -> ``RNN.fit_layers`` -> ``Dense1`` -> loss / accuracy.
+(original src/rnn.py:203-228): placeholders -> ``RNN.fit_layers`` -> ``Dense1`` -> loss / accuracy.
 """
 from __future__ import annotations
 
@@ -77,7 +77,7 @@ class SequenceClassifier(nn.Module):
         logits, loss, correct = F.head_xent(h, self.head.weights, self.head.bias, labels)
         return loss, logits, correct
 
-    # ---- reference variable naming (SURVEY §2.7) ------------------------------------------------
+    # ---- reference variable naming ------------------------------------------------
     def named_reference_variables(self) -> List[Tuple[str, torch.Tensor]]:
         out = []
         for layer in self.rnn.layers:

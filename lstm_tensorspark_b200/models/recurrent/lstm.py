@@ -1,6 +1,6 @@
 """LSTM layer (per-timestep cell + whole-sequence fused path).
 
-Public surface mirrors the reference cell (/root/reference/src/models/recurrent/lstm.py:16-136):
+Public surface mirrors the reference cell (original src/models/recurrent/lstm.py:16-136):
 ``LSTMLayer(name, num_hidden, dim_size, batch_size)``, ``fit_next(data, train=True)``,
 ``restore_state()``, the per-gate accessors ``weight_forget / weight_input / weight_C / weight_output``
 (each ``[W_h [H,H], W_x [D,H]]``) and ``biases_*`` ``[H]``, the trainable initial ``ht`` / ``Ct``
@@ -8,7 +8,7 @@ Public surface mirrors the reference cell (/root/reference/src/models/recurrent/
 
 Storage is NOT the reference's 12 separate matrices: each layer owns three fused tensors
 (``w_x [4H,D]``, ``w_h [4H,H]``, ``bias [4H]``, gate-interleaved rows, see ops/reference.py) so one
-tcgen05 GEMM tile produces all four gates of a hidden slice; the per-gate accessors are strided views.
+wgmma GEMM tile produces all four gates of a hidden slice; the per-gate accessors are strided views.
 """
 from __future__ import annotations
 

@@ -1,6 +1,6 @@
 """Stack of LSTM layers.
 
-Public surface mirrors /root/reference/src/models/recurrent/rnn.py:5-53: ``RNN(settings)``,
+Public surface mirrors original src/models/recurrent/rnn.py:5-53: ``RNN(settings)``,
 ``fit_layers(x)``, ``map_data_by_key()``, ``add_layer(setting)``, ``add_layers(settings)``.
 ``settings`` is the list of dicts built by ``Config.net_settings`` (keys ``layer_name``, ``dim_size``,
 ``num_hidden``, ``batch_size``).  New: ``fit_layers`` also accepts a sequence ``[B,T,D]`` and unrolls it

@@ -1,4 +1,4 @@
-"""Loader for the in-tree sm_100a extension (``lstm_tensorspark_b200/_C*.so``).
+"""Loader for the in-tree sm_90a extension (``lstm_tensorspark_b200/_C*.so``).
 
 There is no eager fallback on the GPU: if a CUDA tensor reaches an op and the extension cannot be imported,
 ``ext()`` raises with the build command.  ``LSTM_TS_BUILD=1`` builds on demand (used by tests / CI)."""
@@ -48,7 +48,7 @@ def ext():
         _EXT = _Counting(importlib.import_module("lstm_tensorspark_b200._C"))
         return _EXT
     raise RuntimeError(
-        "lstm_tensorspark_b200._C (the hand-written sm_100a kernels) is not built/importable: "
+        "lstm_tensorspark_b200._C (the hand-written sm_90a kernels) is not built/importable: "
         f"{_ERR!r}.  Run `python -m lstm_tensorspark_b200.build` (or __graft_entry__.build()).  "
         "There is deliberately no PyTorch fallback on CUDA tensors.")
 

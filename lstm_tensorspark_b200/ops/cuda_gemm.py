@@ -1,9 +1,9 @@
 """Matrix products of the CUDA path: every one of them runs on this framework's own kernels.
 
-  * ``csrc/gemm2_tcgen05.cu`` - TMA + tcgen05 (2-CTA 256x256 tiles), K-major or MN-major operands, bf16 / fp32 / accumulating
+  * ``csrc/gemm2_wgmma.cu`` - TMA + wgmma (128 x 256 tiles, 2-CTA clusters sharing B), K-major or MN-major operands, bf16 / fp32 / accumulating
     fp32 output: the hoisted input projection, dX, and the weight gradients of the LSTM layers;
   * ``csrc/gemm_generic.cu``  - any shape / stride / dtype on the CUDA cores: the reference's own tiny configuration (iris:
-    in_features 4, hidden 16, /root/reference/src/rnn.py:312-321) and the fp32 parity path.
+    in_features 4, hidden 16, original src/rnn.py:312-321) and the fp32 parity path.
 
 No call in here (or anywhere on the CUDA path) reaches cuBLAS.
 """
@@ -16,7 +16,7 @@ import torch
 
 from .cuda_ext import ext
 
-GEMM_CTAS = int(os.environ.get("LSTM_TS_GEMM_CTAS", "2"))      # cta_group: 2 = CTA pairs (256x256 tiles), 1 = single CTA
+GEMM_CTAS = int(os.environ.get("LSTM_TS_GEMM_CTAS", "2"))      # 2 = 2-CTA clusters sharing the B tile (TMA multicast), 1 = single CTA
 GEMM_BN = int(os.environ.get("LSTM_TS_GEMM_BN", "256"))
 STATS = {"tc": 0, "generic": 0}
 
@@ -45,7 +45,7 @@ def _tc_ok(a_k: torch.Tensor, b_k: torch.Tensor, M: int, N: int, K: int) -> bool
 
 def folded_ok(x_bm: torch.Tensor) -> bool:
     """Can a batch-major ``[B, T, F]`` array be read in place as the time-major matrix ``[T*B, F]`` by the tensor-core GEMM
-    (see ``Gemm2Params::a_fold`` in csrc/gemm2_tcgen05.cu)?  Saves the transpose pass over the input of the first layer."""
+    (see ``Gemm2Params::a_fold`` in csrc/gemm2_wgmma.cu)?  Saves the transpose pass over the input of the first layer."""
     return (x_bm.is_cuda and x_bm.dim() == 3 and x_bm.dtype == torch.bfloat16 and x_bm.is_contiguous() and x_bm.shape[0] % 128 == 0
             and x_bm.shape[2] % max(64, GEMM_BN) == 0 and x_bm.data_ptr() % 16 == 0 and GEMM_BN in (128, 256))
 

@@ -1,7 +1,7 @@
-"""CUDA head op: dense layer + softmax cross-entropy + accuracy in ONE launch on the tensor cores (csrc/head_tc.cu:
-TMA-fed tcgen05 tile, logits in TMEM, softmax / NLL / accuracy / dlogits in the epilogue) and the whole backward
+"""CUDA head op: dense layer + softmax cross-entropy + accuracy in ONE launch on the tensor cores (csrc/head_wgmma.cu:
+TMA-fed wgmma tile, logits in registers, softmax / NLL / accuracy / dlogits in the epilogue) and the whole backward
 (dh, dW, db) in ONE launch that writes dW / db straight into the flat gradient buffer.
-Parity: /root/reference/src/rnn.py:214-221 (Dense1), :55-63 (loss), :84-92 (accuracy), :224 (autodiff)."""
+Parity: original src/rnn.py:214-221 (Dense1), :55-63 (loss), :84-92 (accuracy), :224 (autodiff)."""
 from __future__ import annotations
 
 import torch

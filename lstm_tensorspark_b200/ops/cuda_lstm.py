@@ -1,13 +1,13 @@
 """CUDA LSTM layer ops = autograd.Functions around the hand-written kernels.
 
-Fast path (bf16, H % 64 == 0, grid <= #SMs): hoisted input projection on the tcgen05 GEMM (csrc/gemm2_tcgen05.cu) + ONE
-persistent tcgen05 kernel for the whole recurrence in each direction (csrc/lstm_seq_tcgen05.cu; weights resident in SMEM
+Fast path (bf16, H % 64 == 0, grid <= #SMs): hoisted input projection on the wgmma GEMM (csrc/gemm2_wgmma.cu) + ONE
+persistent wgmma kernel for the whole recurrence in each direction (csrc/lstm_seq_wgmma.cu; weights resident in SMEM
 up to H = 1024, streamed through the ring above).  Two stacked layers run as ONE layer wavefront (``_LSTMPairFn``: both
 recurrences co-resident, the upper layer's x-projection / dX as a dataflow-gated GEMM on the idle SMs).  Generic path (any
 shape / fp32): our CUDA-core GEMM per step (csrc/gemm_generic.cu) + the fused pointwise cell kernels (csrc/lstm_pointwise.cu).
-Weight gradients are tcgen05 GEMMs over all T at once (``[4H, T·B] x [T·B, D | H]``, both operands MN-major and read in
+Weight gradients are wgmma GEMMs over all T at once (``[4H, T·B] x [T·B, D | H]``, both operands MN-major and read in
 place), fp32, written straight into the flat gradient buffer; bias gradients are deterministic column sums running next to
-them.  Nothing in here reaches cuBLAS / cuDNN.  Math parity: /root/reference/src/models/recurrent/lstm.py:88-122.
+them.  Nothing in here reaches cuBLAS / cuDNN.  Math parity: original src/models/recurrent/lstm.py:88-122.
 """
 from __future__ import annotations
 
@@ -22,7 +22,7 @@ from . import cuda_gemm as G
 _SYNC_WS = {}
 _SM_COUNT = {}
 FORCE_GENERIC = os.environ.get("LSTM_TS_FORCE_GENERIC", "0") == "1"
-# Tuning / experiment knob of the persistent kernels (0 = defaults), bit fields as decoded in csrc/lstm_seq_tcgen05.cu seq_common():
+# Tuning / experiment knob of the persistent kernels (0 = defaults), bit fields as decoded in csrc/lstm_seq_wgmma.cu seq_common():
 #   [0:4) batch tiles per CTA (2 = one CTA alternates two tiles), [4:8) ring stages, bit 8 force streamed weights,
 #   [12:15) timing-only debug mode (1 skip loads, 2 skip MMAs, 3 in-order stream, 4 half-size loads, 5 no bookkeeping stores,
 #   6 no L2 prefetch, 7 cluster-scope acquire on the exchange barriers), [16:18) sync mode (0 per-k-block dataflow counters,
@@ -107,7 +107,7 @@ def grad_sink(w_addr: int):
 
 def _accumulate_grad(w_addr: int, a_t: torch.Tensor, b: torch.Tensor, b_folded: bool = False):
     """dW = a_t @ b in fp32 (``a_t`` = dG^T as a transposed view, ``b`` = the layer input: both operands MN-major, read in
-    place by the tcgen05 GEMM; ``b_folded``: ``b`` is the batch-major [B,T,D] array standing for the time-major [T*B, D]
+    place by the wgmma GEMM; ``b_folded``: ``b`` is the batch-major [B,T,D] array standing for the time-major [T*B, D]
     matrix).  When the parameter lives in a FlatParams buffer the product lands straight in its grad
     view (overwrite on the first write of a step, accumulate afterwards) and None is returned to autograd."""
     ops = dict(a=a_t, b_t=None, b_folded=b) if b_folded else dict(a=a_t, b_t=b.t())
@@ -167,7 +167,7 @@ def _bias_grad(b_addr: int, dg2d: torch.Tensor, under_gemm: bool = False, part: 
     return G.matmul(ones, dg2d.t(), out_dtype=torch.float32).view(-1)
 
 
-SYNC_WORDS = 8192        # csrc/lstm_seq_tcgen05.cu kSyncWords; the last word is the sticky error flag
+SYNC_WORDS = 8192        # csrc/lstm_seq_wgmma.cu kSyncWords; the last word is the sticky error flag
 
 
 def _sync_ws(device) -> torch.Tensor:
@@ -181,7 +181,7 @@ def check_kernel_errors(device) -> None:
     """Raise if a persistent kernel hit its bounded-spin timeout (sticky flag, costs one D2H read)."""
     ws = _SYNC_WS.get((device.type, device.index))
     if ws is not None and int(ws[SYNC_WORDS - 1].item()) != 0:
-        raise RuntimeError("lstm_seq kernel aborted: an in-kernel wait timed out (see csrc/lstm_seq_tcgen05.cu)")
+        raise RuntimeError("lstm_seq kernel aborted: an in-kernel wait timed out (see csrc/lstm_seq_wgmma.cu)")
     for (di, _tag), ent in list(globals().get("_WS_PAIR", {}).items()):
         if di == device.index and (int(ent[SYNC_WORDS - 1].item()) != 0 or int(ent[2 * SYNC_WORDS - 1].item()) != 0):
             raise RuntimeError("lstm_seq kernel (layer wavefront) aborted: an in-kernel wait timed out")
@@ -197,38 +197,64 @@ def _sms(device) -> int:
 _CORES = {}
 
 
-def _coresident_ctas(device) -> int:
-    """CTAs of the persistent kernels that can be co-resident: the backward kernel runs in clusters of 4 (measured on
-    B200: 33 clusters = 132 CTAs of 148 SMs), the forward K-split in clusters of 2."""
-    key = device.index
+def _coresident_ctas(device, cluster: int = 4) -> int:
+    """CTAs of the persistent kernels that can be co-resident in thread-block clusters of ``cluster``: the backward kernel runs
+    in clusters of 4 (resident weights) or 2 (streamed weights), and a GPC's SM count is not always a multiple of 4 (an H100
+    co-schedules 120 CTAs in clusters of 4: fewer than the 128 of B = 256, H = 1024 at one batch tile per CTA)."""
+    key = (device.index, cluster)
     if key not in _CORES:
         n = _sms(device)
         try:
             with torch.cuda.device(device):
-                c4 = int(ext().lstm_seq_cluster_probe(4))
-            if c4 > 0:
-                n = min(n, 4 * c4)
+                c = int(ext().lstm_seq_cluster_probe(cluster))
+            if c > 0:
+                n = min(n, cluster * c)
         except Exception:                                   # noqa: BLE001
             pass
         _CORES[key] = n
     return _CORES[key]
 
 
+def _bwd_cluster(H: int) -> int:
+    """Cluster size of the backward recurrence kernel: 4 with the weight slice resident (H <= 1024), 2 once it is streamed."""
+    return 4 if H <= 1024 else 2
+
+
+def _tiles_per_cta(B: int, H: int, device) -> Optional[int]:
+    """Batch tiles per CTA of the persistent kernels (1, or 2 when one tile per CTA needs more CTAs than can be co-resident),
+    None when neither fits.  H / 16 CTAs per batch tile (pair); all of them must be co-resident (dataflow sync between CTAs),
+    in clusters for the backward pass.  Two tiles per CTA need the resident weight slice (H <= 1024); larger H streams it through
+    the ring (csrc/lstm_seq_wgmma.cu, kStream; the streamed backward takes H <= 2048)."""
+    if H > 2048:
+        return None
+    tiles_m = (B + 127) // 128
+    n = _coresident_ctas(device, _bwd_cluster(H))
+    if tiles_m * (H // 16) <= n:
+        return 1
+    if H <= 1024 and tiles_m % 2 == 0 and (tiles_m // 2) * (H // 16) <= n:
+        return 2
+    return None
+
+
+def _seq_variant(B: int, H: int, device) -> int:
+    if SEQ_VARIANT & 15 or _tiles_per_cta(B, H, device) != 2:
+        return SEQ_VARIANT
+    return SEQ_VARIANT | 2
+
+
 def fast_path_supported(B: int, H: int, dtype: torch.dtype, device) -> bool:
     if FORCE_GENERIC or dtype != torch.bfloat16 or H % 64 != 0:
         return False
-    tiles_m = (B + 127) // 128
-    # one CTA per (batch tile, 64 gate columns); all of them must be co-resident (dataflow sync between CTAs), in clusters
-    # of 4 for the backward pass.  The weight slice stays in shared memory when it fits (H <= 1024), larger H streams it
-    # through the ring (csrc/lstm_seq_tcgen05.cu, kStream)
-    return tiles_m * (H // 16) <= _coresident_ctas(device) and tiles_m <= 16
+    return (B + 127) // 128 <= 16 and _tiles_per_cta(B, H, device) is not None
 
 
 def _batch_chunk(B: int, H: int, dtype: torch.dtype, device) -> Optional[int]:
     """Largest multiple of 128 rows whose CTAs fit the device, when the whole batch does not (else None)."""
     if FORCE_GENERIC or dtype != torch.bfloat16 or H % 64 != 0 or fast_path_supported(B, H, dtype, device):
         return None
-    tiles = _coresident_ctas(device) // (H // 16)
+    if H > 2048:
+        return None
+    tiles = _coresident_ctas(device, _bwd_cluster(H)) // (H // 16) * (2 if H <= 1024 else 1)
     if tiles < 1:
         return None
     chunk = min(tiles, 16) * 128
@@ -236,7 +262,7 @@ def _batch_chunk(B: int, H: int, dtype: torch.dtype, device) -> Optional[int]:
 
 
 def _mm_f32(a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
-    """a [M,K] @ b [K,N] -> fp32 (own kernels: tcgen05 when bf16 and aligned, CUDA-core GEMM otherwise)."""
+    """a [M,K] @ b [K,N] -> fp32 (own kernels: wgmma when bf16 and aligned, CUDA-core GEMM otherwise)."""
     return G.matmul(a, b.t(), out_dtype=torch.float32)
 
 
@@ -274,7 +300,7 @@ class _LSTMSeqFn(torch.autograd.Function):
         c0f = c0.detach().float().contiguous()
         h0c = h0.detach().to(cd).contiguous()
         if fast:
-            h_seq, c_seq, act = E.lstm_seq_fwd(gx, w_h_c, bias_f, h0c, c0f, _sync_ws(x_seq.device), SEQ_VARIANT)
+            h_seq, c_seq, act = E.lstm_seq_fwd(gx, w_h_c, bias_f, h0c, c0f, _sync_ws(x_seq.device), _seq_variant(B, H, x_seq.device))
             STATS["fast_fwd"] += 1
             STATS["kernels"] += 1
         else:
@@ -320,7 +346,7 @@ class _LSTMSeqFn(torch.autograd.Function):
         if ctx.fast:
             w_hT = _transposed(w_h_c)
             _big_launch_begin()
-            dpre, dh0, dc0 = E.lstm_seq_bwd(dh_seq, w_hT, act, c_seq, dhT, dcT, _sync_ws(dev), SEQ_VARIANT)
+            dpre, dh0, dc0 = E.lstm_seq_bwd(dh_seq, w_hT, act, c_seq, dhT, dcT, _sync_ws(dev), _seq_variant(B, H, dev))
             STATS["fast_bwd"] += 1
             STATS["kernels"] += 1
             _after_big_launch()                  # finished gradient buckets of the layers above: sync them under this recurrence
@@ -374,10 +400,10 @@ def lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias):
 
 # =====================================================================================================================
 # Layer wavefront: two stacked layers' recurrences run CO-RESIDENT (64 + 64 CTAs, two batch tiles per CTA over the same resident
-# weight slice), chained through a dataflow-gated tcgen05 GEMM on the ~20 SMs they leave idle:
+# weight slice), chained through a dataflow-gated wgmma GEMM on the ~20 SMs they leave idle:
 #     forward :  L_a step t  ->  gx_b[t] = h_a[t] W_xb^T (gated GEMM)  ->  L_b step t
 #     backward:  L_b step t  ->  dh_a[t] = dG_b[t] W_xb  (gated GEMM)  ->  L_a step t
-# The reference stacks layers strictly one after the other (/root/reference/src/models/recurrent/rnn.py:38-42); here layer l+1
+# The reference stacks layers strictly one after the other (original src/models/recurrent/rnn.py:38-42); here layer l+1
 # trails layer l by a couple of time steps and the next layer's input projection leaves the critical path altogether.
 # =====================================================================================================================
 FOLDED_FEED = os.environ.get("LSTM_TS_FOLDED_FEED", "1") != "0"   # batch-major input read in place by the first layer's GEMMs
@@ -436,7 +462,7 @@ def wavefront_supported(x_seq: torch.Tensor, h_a: int, h_b: int) -> bool:
 
 
 WAVE_SYNC_MODE = int(os.environ.get("LSTM_TS_WAVE_SYNC", "1"))      # 1: one arrival counter per batch tile (measured 2.5 % faster with two
-                                                                    # tiles per CTA), 0: one per operand k-block (profiles/logs/tiles2_tune.log)
+                                                                    # tiles per CTA), 0: one per operand k-block
 
 
 def _wave_variant() -> int:
@@ -467,7 +493,7 @@ class _LSTMPairFn(torch.autograd.Function):
         Ha, Hb = w_ha.shape[1], w_hb.shape[1]
         cd = x_seq.dtype
         # a batch-major input ([B,T,D] storage behind a transposed view) is read in place by the x-projection and by the
-        # weight-gradient GEMM of the first layer (folded tensor map, csrc/gemm2_tcgen05.cu): no transpose pass
+        # weight-gradient GEMM of the first layer (folded tensor map, csrc/gemm2_wgmma.cu): no transpose pass
         x_bm = x_seq.transpose(0, 1) if not x_seq.is_contiguous() else None
         x2d = x_seq.reshape(T * B, D) if x_bm is None else x_bm
         wxa, wha, wxb, whb = _lowp(w_xa, cd), _lowp(w_ha, cd), _lowp(w_xb, cd), _lowp(w_hb, cd)

@@ -1,4 +1,4 @@
-"""Op dispatch: hand-written sm_100a kernels on CUDA tensors, pure-torch reference elsewhere.
+"""Op dispatch: hand-written sm_90a kernels on CUDA tensors, pure-torch reference elsewhere.
 
 There is exactly one GPU code path (the in-tree ``_C`` extension).  On a CUDA tensor the extension is
 mandatory: a missing/unbuilt extension raises instead of silently falling back to eager PyTorch

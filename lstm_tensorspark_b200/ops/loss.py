@@ -1,4 +1,4 @@
-"""Loss / metric ops with the reference's signatures (/root/reference/src/rnn.py:55-92):
+"""Loss / metric ops with the reference's signatures (original src/rnn.py:55-92):
 ``compute_loss(labels, logits, sparse=True)`` (+ the ``"weight_decay"`` collection terms of
 ``create_variable``), ``compute_accuracy(labels, logits, sparse=True)``.  Scalars with the reference's
 TensorBoard tags (``cross_entropy``, ``weight_decay_loss``, ``total_loss``, ``accuracy``) are pushed to the

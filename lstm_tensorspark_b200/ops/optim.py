@@ -2,7 +2,7 @@
 
 Reference: ``tf.train.AdamOptimizer(learning_rate)`` with TF defaults (beta1 .9, beta2 .999, eps 1e-8,
 "epsilon-hat" formulation), one ``ApplyAdam`` kernel per variable, injectable via ``train_optimizer``
-(/root/reference/src/rnn.py:180,207,224).  Here: ONE launch over the flat fp32 master buffer that also
+(original src/rnn.py:180,207,224).  Here: ONE launch over the flat fp32 master buffer that also
 refreshes the bf16 shadow the tensor-core kernels read (csrc/multi_tensor_opt.cu); on the CPU the same
 math runs through ops/reference.py.  In ``grad_allreduce`` mode on GPUs the update is not launched here at
 all — it is fused into the in-kernel NVLink allreduce (parallel/fused_comm.py).

@@ -1,8 +1,8 @@
-"""Pure-PyTorch reference implementations of every op that has a hand-written sm_100a kernel.
+"""Pure-PyTorch reference implementations of every op that has a hand-written sm_90a kernel.
 
 These are (a) the CPU execution path, (b) the fp32 ground truth the GPU numerics tests compare against.
-Math parity with the reference model: /root/reference/src/models/recurrent/lstm.py:88-122 (cell),
-/root/reference/src/rnn.py:55-92 (loss / accuracy), TF-1.0 ``ApplyAdam`` (optimizer).
+Math parity with the reference model: original src/models/recurrent/lstm.py:88-122 (cell),
+original src/rnn.py:55-92 (loss / accuracy), TF-1.0 ``ApplyAdam`` (optimizer).
 
 Fused parameter layout (this framework's own, chosen for the kernels): per layer
 ``w_x [4H, D]``, ``w_h [4H, H]``, ``bias [4H]`` with row ``n = 4*j + g`` = gate ``g`` of hidden unit ``j``

@@ -1,11 +1,11 @@
 """Cross-replica communication: the parameter average / gradient allreduce.
 
 Reference: ``weights_rdd.reduceByKey(mean_weights).collect()`` — a Spark shuffle keyed by the 8 gate
-names plus a driver-side collect (/root/reference/src/rnn.py:393-407), run once per job; intended semantics =
+names plus a driver-side collect (original src/rnn.py:393-407), run once per job; intended semantics =
 element-wise mean over partitions (Q1).  Here one rank per GPU; three interchangeable back ends behind one
 interface:
 
-  * ``fused`` : hand-written sm_100a kernel doing the reduction over NVLink peer / NVLS multicast pointers
+  * ``fused`` : hand-written sm_90a kernel doing the reduction over NVLink peer / NVLS multicast pointers
                 with the update (average, SGD, Adam) fused in — the product path (parallel/fused_comm.py);
   * ``nccl``  : ``dist.all_reduce`` + separate update kernels — the baseline the fused path is measured against;
   * ``gloo``  : the same on CPU, used by the multi-process tests (our analogue of Spark ``local[N]``).

@@ -7,7 +7,7 @@ multicast alias when the fabric supports it).  The sync itself is a single launc
 (average | SGD | Adam) and the bf16 shadow refresh.  NCCL is used only to bootstrap (store, rendezvous) and for
 python-object broadcasts; no NCCL collective and no separate elementwise kernel runs on the sync path.
 
-Replaces ``reduceByKey(mean_weights)`` + ``collect()`` (/root/reference/src/rnn.py:393-407).
+Replaces ``reduceByKey(mean_weights)`` + ``collect()`` (original src/rnn.py:393-407).
 """
 from __future__ import annotations
 
@@ -22,7 +22,7 @@ from ..ops.cuda_ext import ext
 from .comm import TorchDistComm
 
 MODE_AVG, MODE_SGD, MODE_ADAM = 0, 1, 2
-TWO_SHOT_BYTES = int(os.environ.get("LSTM_TS_AR_TWO_SHOT_BYTES", str(8 * 1024)))      # measured at 8 GPUs (profiles/logs/sweep8_r2.log): two-shot wins from 16 KB up, ties below
+TWO_SHOT_BYTES = int(os.environ.get("LSTM_TS_AR_TWO_SHOT_BYTES", str(8 * 1024)))      # measured at 8 GPUs: two-shot wins from 16 KB up, ties below
 AR_BLOCKS = int(os.environ.get("LSTM_TS_AR_BLOCKS", "64"))
 AR_BLOCKS_P2P_LARGE = int(os.environ.get("LSTM_TS_AR_BLOCKS_P2P_LARGE", "128"))
 AR_BLOCKS_LARGE = int(os.environ.get("LSTM_TS_AR_BLOCKS_LARGE", "64"))    # messages >= 32 MB (measured: 64 = 128 = 256 blocks, unroll irrelevant: sweep8c.log)
@@ -130,7 +130,7 @@ class FusedComm(TorchDistComm):
         A = self.arena
         two_shot = (4 * n >= TWO_SHOT_BYTES) if force is None else (force == "two_shot")
         # NVLS (in-switch reduction) pays from 3 ranks up; with 2 ranks the peer-pointer kernel is faster stand-alone (measured:
-        # profiles/logs/allreduce_sweep_n2_r2.json) - but it needs 122 registers, so a bucket that has to squeeze onto the SMs a
+        # measured) - but it needs 122 registers, so a bucket that has to squeeze onto the SMs a
         # GEMM leaves idle (pdl) keeps the 32-register multimem variant
         mc = self._multicast_on() and two_shot and (self.world_size > 2 or pdl or self.use_multicast in ("1", "on", "force"))
         if mode == MODE_AVG and not two_shot:
@@ -150,7 +150,7 @@ class FusedComm(TorchDistComm):
             m, v = m[:n], v[:n]
         if wd_numel >= 0:
             wd_numel = max(0, min(n, wd_numel - elem_off))
-        # grid: the NVLS kernel is switch-bound (64 = 128 = 256 CTAs, profiles/logs); the peer-pointer kernel is bound by bytes in
+        # grid: the NVLS kernel is switch-bound (64 = 128 = 256 CTAs); the peer-pointer kernel is bound by bytes in
         # flight per SM - 128 CTAs from 4 MB up (2 GPUs, 1 GB: 2.00 ms vs 2.57 ms with 64; NCCL 2.20 ms)
         nblk = blocks or self.blocks_override or ((AR_BLOCKS_P2P_LARGE if 4 * n >= (4 << 20) else AR_BLOCKS) if not mc
                                                   else (AR_BLOCKS_LARGE if 4 * n >= (32 << 20) else AR_BLOCKS))

@@ -1,8 +1,8 @@
 """Rank launcher: ``--partitions N`` -> N processes, one per GPU (replaces SparkConf/SparkContext +
-``local[N]`` executors, /root/reference/src/rnn.py:355-363).  Honours a torchrun environment
+``local[N]`` executors, original src/rnn.py:355-363).  Honours a torchrun environment
 (RANK / WORLD_SIZE / LOCAL_RANK / MASTER_*) when present; otherwise spawns the ranks itself on 127.0.0.1.
 
-Failure detection (SURVEY §5.3): the parent polls its children; the first abnormal exit terminates the
+Failure detection: the parent polls its children; the first abnormal exit terminates the
 remaining ranks and surfaces as ``RankFailure`` carrying every exit code — a dead peer is an error, not a hang.
 """
 from __future__ import annotations

@@ -1,11 +1,11 @@
 """Per-replica trainer + job driver.
 
 Parity targets (reference, read-only):
-  * ``train_rnn(partition, net_settings, FLAGS, train_optimizer)``   /root/reference/src/rnn.py:180-297
-  * standalone ``train_rnn(dataset, net_settings, train_optimizer)`` /root/reference/src/lstm-no-spark.py:153-251
-  * driver ``main``                                                    /root/reference/src/rnn.py:339-411
+  * ``train_rnn(partition, net_settings, FLAGS, train_optimizer)``   original src/rnn.py:180-297
+  * standalone ``train_rnn(dataset, net_settings, train_optimizer)`` original src/lstm-no-spark.py:153-251
+  * driver ``main``                                                    original src/rnn.py:339-411
 
-One implementation serves both entry points.  Differences by design (SURVEY §2.8): the cross-replica mean
+One implementation serves both entry points.  Differences by design: the cross-replica mean
 is exact and is written back into every replica and to ``--output_path`` (Q1, Q12); one run timestamp is
 shared by all ranks; a real resume path exists (Q4); replicas start from identical seeded weights unless
 ``--independent_init`` (Q9).
@@ -71,7 +71,7 @@ class ReplicaResult(dict):
 
 
 def _check_device_errors(device: torch.device, comm) -> None:
-    """Failure surfacing (SURVEY §5.3): the persistent LSTM kernels and the fused allreduce bound every in-kernel wait and
+    """Failure surfacing: the persistent LSTM kernels and the fused allreduce bound every in-kernel wait and
     raise a sticky device flag instead of hanging; turn it into a Python error at the sync points we have anyway."""
     if device.type != "cuda":
         return
@@ -117,7 +117,7 @@ def train_rnn(partition, cfg: Config, rank: int = 0, world_size: int = 1, comm: 
                       train_optimizer=train_optimizer)
     model, optimizer = eng.model, eng.optimizer
 
-    # ---- run directory (SURVEY §2.7) -----------------------------------------------------------------
+    # ---- run directory -----------------------------------------------------------------
     current_exec = run_stamp or str(time.time())
     model_save_dir = os.path.join(cfg.checkpoint_path, current_exec) if standalone else \
         os.path.join(cfg.checkpoint_path, current_exec, str(partition_key))
@@ -285,7 +285,7 @@ def _rank_main(rank: int, world_size: int, cfg: Config, shards, standalone: bool
 
 def _train_oversubscribed(mine, n_partitions: int, cfg: Config, rank: int, world_size: int, comm, stamp: str):
     """More partitions than workers (the reference runs ``--partitions`` tasks on ``local[workers]`` executor threads,
-    /root/reference/src/rnn.py:355-358: each worker takes its tasks in turn).  Every partition is still its own replica
+    original src/rnn.py:355-358: each worker takes its tasks in turn).  Every partition is still its own replica
     with its own checkpoint directory; a rank trains its partitions one after the other and the one-shot average at the
     end of the job (src/rnn.py:393-407) runs over ALL partitions: local sum -> cross-rank sum -> / partitions."""
     results = []

@@ -3,10 +3,10 @@
 Reference mechanism: ``tf.train.Saver(tf.trainable_variables())`` (default ``max_to_keep=5``), saved every
 ``evaluate_every`` steps and on the last step into ``<checkpoint_path>/<unix-time>/<partition_key>/`` with
 prefix ``spark_lstm`` (standalone: ``<checkpoint_path>/<unix-time>/``, prefix ``lstm_no_spark``), next to a
-``params_settings`` text file and a ``train/`` events dir (/root/reference/src/rnn.py:230,234-250,273-274;
-/root/reference/src/lstm-no-spark.py:182-202,230).
+``params_settings`` text file and a ``train/`` events dir (original src/rnn.py:230,234-250,273-274;
+original src/lstm-no-spark.py:182-202,230).
 
-Layout reproduced here (SURVEY §2.7):
+Layout reproduced here:
     <dir>/params_settings
     <dir>/checkpoint                       TF-style index: model_checkpoint_path + all_model_checkpoint_paths
     <dir>/<prefix>-<step>.index            json: variable name -> shape/dtype (human readable)

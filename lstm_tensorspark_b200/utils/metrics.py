@@ -1,7 +1,7 @@
 """Metrics / logging / observability.
 
 Parity (reference): TB scalars ``cross_entropy`` / ``accuracy`` (+ ``weight_decay_loss`` / ``total_loss``)
-written at eval steps to ``<ckpt dir>/train`` (/root/reference/src/rnn.py:65-68,91,249-250,276-280); tqdm bar
+written at eval steps to ``<ckpt dir>/train`` (original src/rnn.py:65-68,91,249-250,276-280); tqdm bar
 with ``Loss/t_acc`` description (:257,270-271,291-292); the human-readable timing lines (:296,410).
 New: CUDA-event device timing, NVTX ranges, JSON lines.
 """
@@ -101,7 +101,7 @@ class DeviceTimer:
 class LaggedScalar:
     """Per-step scalar for the progress bar without a per-step host sync: on CUDA the value is copied into a pinned
     buffer asynchronously and the PREVIOUS step's value is returned (its copy has long finished); on the CPU it is exact.
-    (The reference's ``sess.run([train_op, loss])`` blocks on the loss every step, /root/reference/src/rnn.py:264-271.)"""
+    (The reference's ``sess.run([train_op, loss])`` blocks on the loss every step, original src/rnn.py:264-271.)"""
 
     def __init__(self, device):
         self.cuda = torch.device(device).type == "cuda"

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Distributed entry point: ``python rnn.py --training_path dataset/iris.data --partitions 4 ...``
-(replaces ``spark-submit rnn.py ...`` of the reference, /root/reference/src/rnn.py:339-414, README.md:40).
+(replaces ``spark-submit rnn.py ...`` of the reference, original src/rnn.py:339-414, README.md:40).
 One rank per partition / GPU; also runs under torchrun."""
 import sys
 

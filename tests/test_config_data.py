@@ -1,4 +1,4 @@
-"""Unit tests for the flag system and the data layer (SURVEY §4: sharder, process_batch, next_batch, normaliser,
+"""Unit tests for the flag system and the data layer (: sharder, process_batch, next_batch, normaliser,
 flag defaults, net_settings)."""
 import numpy as np
 import pytest
@@ -10,7 +10,7 @@ from lstm_tensorspark_b200.config import Config, parse_args
 
 def test_reference_flag_defaults():
     cfg = parse_args([], standalone=False)
-    # /root/reference/src/rnn.py:310-334
+    # original src/rnn.py:310-334
     assert (cfg.master, cfg.spark_exec_memory, cfg.partitions, cfg.epochs) == ("local", "4g", 4, 1)
     assert (cfg.hidden_units, cfg.batch_size, cfg.num_classes, cfg.in_features) == ("128,256", 10, 3, 4)
     assert cfg.learning_rate == pytest.approx(1e-3) and cfg.evaluate_every == 10
@@ -20,7 +20,7 @@ def test_reference_flag_defaults():
 
 def test_standalone_defaults_and_unknown_args_ignored():
     cfg = parse_args(["--bogus", "1", "--hidden_units=16"], standalone=True)
-    assert cfg.epochs == 5                      # /root/reference/src/lstm-no-spark.py:12
+    assert cfg.epochs == 5                      # original src/lstm-no-spark.py:12
     assert cfg.partitions == 1 and cfg.hidden_units == "16"
 
 

@@ -97,7 +97,7 @@ def test_rank_failure_is_an_error_not_a_hang(tmp_path, iris_path):
 
 
 def test_more_partitions_than_workers_round_robin(tmp_path, iris_path, capfd):
-    """--partitions 4 on 2 workers (Spark local[2] with 4 tasks, /root/reference/src/rnn.py:355-358): every partition gets
+    """--partitions 4 on 2 workers (Spark local[2] with 4 tasks, original src/rnn.py:355-358): every partition gets
     its own replica + checkpoint dir, ranks take their partitions in turn, the final average runs over all 4."""
     cfg = _cfg(tmp_path, iris_path, partitions=4, max_workers=2)
     out = run_job(cfg, standalone=False)

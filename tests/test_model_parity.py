@@ -1,5 +1,5 @@
 """Numerical parity (CPU): LSTM cell / stack vs a NumPy transcription of the reference equations
-(/root/reference/src/models/recurrent/lstm.py:88-109), loss/accuracy closed forms, TF-Adam values, gradcheck."""
+(original src/models/recurrent/lstm.py:88-109), loss/accuracy closed forms, TF-Adam values, gradcheck."""
 import numpy as np
 import pytest
 import torch

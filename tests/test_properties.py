@@ -1,5 +1,5 @@
 """Property tests (hypothesis) for the data layer and the flat parameter buffer - the invariants the reference's Spark
-pipeline only held by accident (SURVEY §2.8 Q2, Q3) and the ones the fused allreduce relies on."""
+pipeline only held by accident (Q2, Q3) and the ones the fused allreduce relies on."""
 import numpy as np
 import pytest
 import torch

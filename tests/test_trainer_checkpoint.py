@@ -1,4 +1,4 @@
-"""Integration (CPU): standalone run on iris (BASELINE.json config 1), checkpoint tree (SURVEY §2.7), cadence,
+"""Integration (CPU): standalone run on iris (BASELINE.json config 1), checkpoint tree, cadence,
 retention, resume, compat step count (Q5), batch_size 0 (Q3)."""
 import glob
 import json
