@@ -38,6 +38,9 @@ class Config:
     use_pretrained_model: bool = False  # the flag the reference reads but never defines (Q4)
     resume: str = ""                    # explicit checkpoint dir/prefix to resume from
     seq_len: int = 1                    # time steps per sample (reference == 1)
+    variable_length: bool = False       # samples of 1..seq_len steps: a CSV row is k*in_features values + label (zero-padded to
+                                        # seq_len); --synthetic draws lengths in [seq_len//4, seq_len].  The final state is each
+                                        # sample's state after its own last step (padded steps hold the state)
     dtype: str = "auto"                 # auto: bf16 on cuda, fp32 on cpu
     device: str = "auto"                # auto | cpu | cuda
     backend: str = "auto"               # auto | cuda_ext (hand-written sm_90a kernels) | torch
@@ -114,6 +117,8 @@ class Config:
             raise ValueError("--batch_size must be >= 0 (0 = whole shard)")
         if self.seq_len < 1:
             raise ValueError("--seq_len must be >= 1")
+        if self.variable_length and self.seq_len < 2:
+            raise ValueError("--variable_length needs --seq_len >= 2 (the longest sample's number of steps)")
         if self.sync_mode not in ("param_avg", "grad_allreduce", "none"):
             raise ValueError(f"unknown --sync_mode {self.sync_mode}")
         if self.optimizer not in ("adam", "sgd"):

@@ -15,14 +15,15 @@
 using torch::Tensor;
 
 extern "C" {
-int ts_lstm_pointwise_fwd(const void*, const float*, const float*, void*, float*, void*, int, int, int, cudaStream_t);
+int ts_lstm_pointwise_fwd(const void*, const float*, const float*, void*, float*, void*, int, int, int, cudaStream_t, const void*,
+                          const int*, int);
 int ts_transpose01_rows(const void*, void*, int, int, long long, cudaStream_t);
 int ts_lstm_seq_cluster_probe(int);
 int ts_transpose2d_b16(const void*, void*, int, int, cudaStream_t);
 int ts_colsum_bf16(const void*, float*, void*, int, int, int, int, int, cudaStream_t);
 long long ts_colsum_scratch_bytes(int, int);
 int ts_lstm_pointwise_bwd(const void*, const float*, const float*, const void*, const float*, const float*, void*,
-                          float*, int, int, int, cudaStream_t);
+                          float*, int, int, int, cudaStream_t, const int*, int, float*);
 int ts_xent_rows(const float*, const long long*, float*, float*, int*, int, int, cudaStream_t);
 int ts_flat_adam(float*, const float*, float*, float*, void*, long long, float, float, float, float, float, float,
                  cudaStream_t, int*, long long);
@@ -43,9 +44,9 @@ int ts_gemm_generic(const void*, const void*, void*, const float*, int, int, int
 int ts_gemm2(const void*, const void*, void*, const float*, int, int, int, int, int, int, int, int, int, int, int, int, int,
              const unsigned int*, const int*, unsigned int*, int*, int, int, int, int, cudaStream_t);
 int ts_lstm_seq_fwd(const void*, const void*, const float*, const void*, const float*, void*, const float*, void*, void*, int,
-                    int, int, unsigned int*, int, cudaStream_t, const void*, const unsigned int*, int, int, int);
+                    int, int, unsigned int*, int, cudaStream_t, const void*, const unsigned int*, int, int, int, const int*);
 int ts_lstm_seq_bwd(const void*, const void*, const void*, const float*, const void*, float*, float*, void*, void*, int,
-                    int, int, unsigned int*, int, cudaStream_t, const unsigned int*, int, int, int);
+                    int, int, unsigned int*, int, cudaStream_t, const unsigned int*, int, int, int, const int*);
 int ts_lstm_seq_prologue(const void*, const float*, void*, float*, void*, unsigned int*, int, int, cudaStream_t);
 const char* ts_last_error();
 }
@@ -71,6 +72,17 @@ int is_bf16(const Tensor& t) {
   return t.scalar_type() == torch::kBFloat16 ? 1 : 0;
 }
 const float* fptr(const std::optional<Tensor>& t) { return t.has_value() ? t->data_ptr<float>() : nullptr; }
+// Per-row sequence lengths: int32 [B] on the batch's device.  The values (1 <= len <= T) are not checked here: that would
+// need a device-to-host copy on every call.
+const int* lengths_ptr(const std::optional<Tensor>& lengths, int64_t B, const Tensor& like) {
+  if (!lengths.has_value()) return nullptr;
+  const Tensor& l = *lengths;
+  TORCH_CHECK(l.is_cuda() && l.device() == like.device(), "lengths must be on the batch's device");
+  TORCH_CHECK(l.scalar_type() == torch::kInt32, "lengths must be int32");
+  TORCH_CHECK(l.dim() == 1 && l.size(0) == B, "lengths must be [B] (B = ", B, ")");
+  TORCH_CHECK(l.is_contiguous(), "lengths must be contiguous");
+  return l.data_ptr<int>();
+}
 
 // x [B,T,D] contiguous -> [T,B,D] contiguous (row permutation at copy speed)
 Tensor transpose01(const Tensor& x) {
@@ -129,34 +141,47 @@ void colsum_bf16_into(const Tensor& x, Tensor out, bool overwrite, bool pdl, int
 }
 
 // ---- generic LSTM cell epilogue -------------------------------------------------------------------------
-std::vector<Tensor> lstm_pointwise_fwd(const Tensor& pre, const Tensor& bias, const Tensor& c_prev) {
+// lengths (optional, with the step index t and h_prev [B,H] of pre's dtype): rows with t >= lengths[b] carry (h_prev, c_prev)
+std::vector<Tensor> lstm_pointwise_fwd(const Tensor& pre, const Tensor& bias, const Tensor& c_prev, const std::optional<Tensor>& h_prev,
+                                       const std::optional<Tensor>& lengths, int64_t t) {
   chk_cuda(pre, "pre"); chk_cuda(bias, "bias"); chk_cuda(c_prev, "c_prev");
   c10::cuda::CUDAGuard g(pre.device());
   int B = pre.size(0), H = pre.size(1) / 4;
   TORCH_CHECK(bias.scalar_type() == torch::kFloat32 && c_prev.scalar_type() == torch::kFloat32, "bias/c must be fp32");
   TORCH_CHECK(c_prev.numel() == (int64_t)B * H && bias.numel() == 4 * H, "shape mismatch");
+  const int* lp = lengths_ptr(lengths, B, pre);
+  if (lp) {
+    TORCH_CHECK(h_prev.has_value(), "lstm_pointwise_fwd: lengths need h_prev");
+    chk_cuda(*h_prev, "h_prev");
+    TORCH_CHECK(h_prev->scalar_type() == pre.scalar_type() && h_prev->numel() == (int64_t)B * H, "h_prev: [B,H] in pre's dtype");
+  }
   auto h = torch::empty({B, H}, pre.options());
   auto c = torch::empty({B, H}, c_prev.options());
   auto act = torch::empty_like(pre);
   check(ts_lstm_pointwise_fwd(pre.data_ptr(), bias.data_ptr<float>(), c_prev.data_ptr<float>(), h.data_ptr(),
-                              c.data_ptr<float>(), act.data_ptr(), B, H, is_bf16(pre), stream()), "lstm_pointwise_fwd");
+                              c.data_ptr<float>(), act.data_ptr(), B, H, is_bf16(pre), stream(), lp ? h_prev->data_ptr() : nullptr,
+                              lp, (int)t), "lstm_pointwise_fwd");
   return {h, c, act};
 }
 
 std::vector<Tensor> lstm_pointwise_bwd(const std::optional<Tensor>& dh_a, const std::optional<Tensor>& dh_b,
                                        const std::optional<Tensor>& dc_in, const Tensor& act, const Tensor& c_prev,
-                                       const Tensor& c_new) {
+                                       const Tensor& c_new, const std::optional<Tensor>& lengths, int64_t t) {
   chk_cuda(act, "act"); chk_cuda(c_prev, "c_prev"); chk_cuda(c_new, "c_new");
   c10::cuda::CUDAGuard g(act.device());
   int B = act.size(0), H = act.size(1) / 4;
+  const int* lp = lengths_ptr(lengths, B, act);
   if (dh_a.has_value()) { chk_cuda(*dh_a, "dh_a"); TORCH_CHECK(dh_a->scalar_type() == act.scalar_type(), "dh_a dtype"); }
   if (dh_b.has_value()) { chk_cuda(*dh_b, "dh_b"); TORCH_CHECK(dh_b->scalar_type() == torch::kFloat32, "dh_b fp32"); }
   if (dc_in.has_value()) { chk_cuda(*dc_in, "dc_in"); TORCH_CHECK(dc_in->scalar_type() == torch::kFloat32, "dc fp32"); }
   auto dpre = torch::empty_like(act);
   auto dc = torch::empty_like(c_prev);
+  // with lengths: a third output, the dh handed straight to step t-1 (the total dh of padded rows, 0 elsewhere)
+  Tensor dh_out = lp ? torch::empty_like(c_prev) : Tensor();
   check(ts_lstm_pointwise_bwd(dh_a.has_value() ? dh_a->data_ptr() : nullptr, fptr(dh_b), fptr(dc_in), act.data_ptr(),
                               c_prev.data_ptr<float>(), c_new.data_ptr<float>(), dpre.data_ptr(), dc.data_ptr<float>(),
-                              B, H, is_bf16(act), stream()), "lstm_pointwise_bwd");
+                              B, H, is_bf16(act), stream(), lp, (int)t, lp ? dh_out.data_ptr<float>() : nullptr), "lstm_pointwise_bwd");
+  if (lp) return {dpre, dc, dh_out};
   return {dpre, dc};
 }
 
@@ -332,10 +357,12 @@ Tensor gemm_generic(const Tensor& A, const Tensor& B, const std::optional<Tensor
 // extra_signal: one more arrival after the last step, for a gated GEMM that consumes h_seq.
 std::vector<Tensor> lstm_seq_fwd(const Tensor& gx, const Tensor& w_h, const Tensor& bias, const Tensor& h0,
                                  const Tensor& c0, Tensor sync_ws, int64_t variant, std::optional<Tensor> dbg,
-                                 std::optional<Tensor> in_gate, int64_t in_gate_tiles_n, bool extra_signal) {
+                                 std::optional<Tensor> in_gate, int64_t in_gate_tiles_n, bool extra_signal,
+                                 const std::optional<Tensor>& lengths) {
   chk_cuda(gx, "gx"); chk_cuda(w_h, "w_h"); chk_cuda(bias, "bias"); chk_cuda(h0, "h0"); chk_cuda(c0, "c0");
   c10::cuda::CUDAGuard gd(gx.device());
   int T = gx.size(0), B = gx.size(1), H = gx.size(2) / 4;
+  const int* lp = lengths_ptr(lengths, B, gx);
   auto h_seq = torch::empty({T + 1, B, H}, gx.options());
   auto c_seq = torch::empty({T + 1, B, H}, c0.options());
   auto act = torch::empty({T, B, 4 * H}, gx.options());
@@ -348,7 +375,7 @@ std::vector<Tensor> lstm_seq_fwd(const Tensor& gx, const Tensor& w_h, const Tens
                         act.data_ptr(), c0.data_ptr<float>(), dbg.has_value() ? dbg->data_ptr() : nullptr, tiled.data_ptr(), T, B, H,
                         (unsigned int*)sync_ws.data_ptr<int>(), (int)variant, stream(), h0.data_ptr(),
                         in_gate.has_value() ? (const unsigned int*)in_gate->data_ptr<int>() : nullptr, (int)in_gate_tiles_n,
-                        extra_signal ? 1 : 0, 0), "lstm_seq_fwd");
+                        extra_signal ? 1 : 0, 0, lp), "lstm_seq_fwd");
   return {h_seq, c_seq, act};
 }
 
@@ -357,11 +384,13 @@ std::vector<Tensor> lstm_seq_fwd(const Tensor& gx, const Tensor& w_h, const Tens
 // -> dpre [T,B,4H] bf16, dh0 fp32 [B,H], dc0 fp32 [B,H]
 std::vector<Tensor> lstm_seq_bwd(const std::optional<Tensor>& dh_seq, const Tensor& w_hT, const Tensor& act, const Tensor& c_seq,
                                  const Tensor& dhT, const Tensor& dcT, Tensor sync_ws, int64_t variant,
-                                 std::optional<Tensor> dbg, std::optional<Tensor> in_gate, int64_t in_gate_tiles_n, bool extra_signal) {
+                                 std::optional<Tensor> dbg, std::optional<Tensor> in_gate, int64_t in_gate_tiles_n, bool extra_signal,
+                                 const std::optional<Tensor>& lengths) {
   if (dh_seq.has_value()) chk_cuda(*dh_seq, "dh_seq");
   chk_cuda(w_hT, "w_hT"); chk_cuda(act, "act"); chk_cuda(c_seq, "c_seq");
   c10::cuda::CUDAGuard gd(act.device());
   int T = act.size(0), B = act.size(1), H = act.size(2) / 4;
+  const int* lp = lengths_ptr(lengths, B, act);
   auto dpre = torch::empty_like(act);
   auto dh0 = dhT.clone();
   auto dc0 = dcT.clone();
@@ -371,7 +400,7 @@ std::vector<Tensor> lstm_seq_bwd(const std::optional<Tensor>& dh_seq, const Tens
                         dh0.data_ptr<float>(), dc0.data_ptr<float>(), dbg.has_value() ? dbg->data_ptr() : nullptr, tiled.data_ptr(), T, B, H,
                         (unsigned int*)sync_ws.data_ptr<int>(), (int)variant, stream(),
                         in_gate.has_value() ? (const unsigned int*)in_gate->data_ptr<int>() : nullptr, (int)in_gate_tiles_n,
-                        extra_signal ? 1 : 0, 0), "lstm_seq_bwd");
+                        extra_signal ? 1 : 0, 0, lp), "lstm_seq_bwd");
   return {dpre, dh0, dc0};
 }
 
@@ -379,11 +408,13 @@ std::vector<Tensor> lstm_seq_bwd(const std::optional<Tensor>& dh_seq, const Tens
 // launch goes to an explicit stream - the caching allocator never sees a side stream.
 void lstm_seq_fwd_into(const Tensor& gx, const Tensor& w_h, const Tensor& bias, const Tensor& h0, const Tensor& c0, Tensor h_seq,
                        Tensor c_seq, Tensor act, Tensor tiled, Tensor sync_ws, int64_t variant, std::optional<Tensor> in_gate,
-                       int64_t in_gate_tiles_n, bool extra_signal, int64_t stream_handle, int64_t launch_flags) {
+                       int64_t in_gate_tiles_n, bool extra_signal, int64_t stream_handle, int64_t launch_flags,
+                       const std::optional<Tensor>& lengths) {
   chk_cuda(gx, "gx"); chk_cuda(w_h, "w_h"); chk_cuda(bias, "bias"); chk_cuda(h0, "h0"); chk_cuda(c0, "c0");
   chk_cuda(h_seq, "h_seq"); chk_cuda(c_seq, "c_seq"); chk_cuda(act, "act"); chk_cuda(tiled, "tiled");
   c10::cuda::CUDAGuard gd(gx.device());
   int T = gx.size(0), B = gx.size(1), H = gx.size(2) / 4;
+  const int* lp = lengths_ptr(lengths, B, gx);
   TORCH_CHECK(h_seq.numel() == (int64_t)(T + 1) * B * H && c_seq.numel() == h_seq.numel() && act.numel() == gx.numel(), "lstm_seq_fwd_into: buffer sizes");
   TORCH_CHECK(tiled.numel() == (int64_t)(T + 1) * ((B + 127) / 128) * 128 * H, "lstm_seq_fwd_into: tile-image buffer size");
   TORCH_CHECK(h0.scalar_type() == torch::kBFloat16 && c0.scalar_type() == torch::kFloat32, "h0 bf16 / c0 fp32");
@@ -391,7 +422,7 @@ void lstm_seq_fwd_into(const Tensor& gx, const Tensor& w_h, const Tensor& bias, 
                         act.data_ptr(), c0.data_ptr<float>(), nullptr, tiled.data_ptr(), T, B, H, (unsigned int*)sync_ws.data_ptr<int>(),
                         (int)variant, stream_handle ? (cudaStream_t)stream_handle : stream(), h0.data_ptr(),
                         in_gate.has_value() ? (const unsigned int*)in_gate->data_ptr<int>() : nullptr, (int)in_gate_tiles_n,
-                        extra_signal ? 1 : 0, (int)launch_flags), "lstm_seq_fwd_into");
+                        extra_signal ? 1 : 0, (int)launch_flags, lp), "lstm_seq_fwd_into");
 }
 
 // h_seq[0] <- h0, c_seq[0] <- c0, tile image of h0, step counters <- 0 (what lstm_seq_fwd does first unless launch_flags bit 0)
@@ -405,31 +436,35 @@ void lstm_seq_prologue(const Tensor& h0, const Tensor& c0, Tensor h_seq, Tensor 
 
 void lstm_seq_bwd_into(const std::optional<Tensor>& dh_seq, const Tensor& w_hT, const Tensor& act, const Tensor& c_seq, Tensor dpre,
                        Tensor dh0, Tensor dc0, Tensor tiled, Tensor sync_ws, int64_t variant, std::optional<Tensor> in_gate,
-                       int64_t in_gate_tiles_n, bool extra_signal, int64_t stream_handle, int64_t launch_flags) {
+                       int64_t in_gate_tiles_n, bool extra_signal, int64_t stream_handle, int64_t launch_flags,
+                       const std::optional<Tensor>& lengths) {
   chk_cuda(w_hT, "w_hT"); chk_cuda(act, "act"); chk_cuda(c_seq, "c_seq"); chk_cuda(dpre, "dpre"); chk_cuda(dh0, "dh0"); chk_cuda(dc0, "dc0");
   c10::cuda::CUDAGuard gd(act.device());
   int T = act.size(0), B = act.size(1), H = act.size(2) / 4;
+  const int* lp = lengths_ptr(lengths, B, act);
   TORCH_CHECK(dpre.numel() == act.numel() && tiled.numel() == (int64_t)T * ((B + 127) / 128) * 128 * 4 * H, "lstm_seq_bwd_into: buffer sizes");
   TORCH_CHECK(dh0.scalar_type() == torch::kFloat32 && dc0.scalar_type() == torch::kFloat32 && dh0.numel() == (int64_t)B * H && dc0.numel() == (int64_t)B * H, "dh0/dc0 fp32 [B,H]");
   check(ts_lstm_seq_bwd(dh_seq.has_value() ? dh_seq->data_ptr() : nullptr, w_hT.data_ptr(), act.data_ptr(), c_seq.data_ptr<float>(), dpre.data_ptr(),
                         dh0.data_ptr<float>(), dc0.data_ptr<float>(), nullptr, tiled.data_ptr(), T, B, H, (unsigned int*)sync_ws.data_ptr<int>(),
                         (int)variant, stream_handle ? (cudaStream_t)stream_handle : stream(),
                         in_gate.has_value() ? (const unsigned int*)in_gate->data_ptr<int>() : nullptr, (int)in_gate_tiles_n,
-                        extra_signal ? 1 : 0, (int)launch_flags), "lstm_seq_bwd_into");
+                        extra_signal ? 1 : 0, (int)launch_flags, lp), "lstm_seq_bwd_into");
 }
 
 }  // namespace
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.doc() = "lstm_tensorspark_b200 sm_90a kernels";
-  m.def("lstm_pointwise_fwd", &lstm_pointwise_fwd);
+  m.def("lstm_pointwise_fwd", &lstm_pointwise_fwd, py::arg("pre"), py::arg("bias"), py::arg("c_prev"), py::arg("h_prev") = py::none(),
+        py::arg("lengths") = py::none(), py::arg("t") = 0);
   m.def("transpose01", &transpose01);
   m.def("transpose2d", &transpose2d);
   m.def("colsum_bf16", &colsum_bf16);
   m.def("colsum_bf16_into", &colsum_bf16_into, py::arg("x"), py::arg("out"), py::arg("overwrite"), py::arg("pdl") = false,
         py::arg("col0") = 0, py::arg("ncols") = 0);
   m.def("lstm_seq_cluster_probe", [](int64_t c) { return ts_lstm_seq_cluster_probe((int)c); });
-  m.def("lstm_pointwise_bwd", &lstm_pointwise_bwd);
+  m.def("lstm_pointwise_bwd", &lstm_pointwise_bwd, py::arg("dh_a"), py::arg("dh_b"), py::arg("dc_in"), py::arg("act"), py::arg("c_prev"),
+        py::arg("c_new"), py::arg("lengths") = py::none(), py::arg("t") = 0);
   m.def("xent_rows", &xent_rows);
   m.def("head_fwd", &head_fwd);
   m.def("head_bwd", &head_bwd, py::arg("h"), py::arg("W"), py::arg("dlogits"), py::arg("dloss"), py::arg("dW"), py::arg("db"),
@@ -462,16 +497,17 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("fold_cols") = 0);
   m.def("lstm_seq_fwd", &lstm_seq_fwd, py::arg("gx"), py::arg("w_h"), py::arg("bias"), py::arg("h0"), py::arg("c0"),
         py::arg("sync_ws"), py::arg("variant") = 0, py::arg("dbg") = py::none(), py::arg("in_gate") = py::none(),
-        py::arg("in_gate_tiles_n") = 0, py::arg("extra_signal") = false);
+        py::arg("in_gate_tiles_n") = 0, py::arg("extra_signal") = false, py::arg("lengths") = py::none());
   m.def("lstm_seq_fwd_into", &lstm_seq_fwd_into, py::arg("gx"), py::arg("w_h"), py::arg("bias"), py::arg("h0"), py::arg("c0"),
         py::arg("h_seq"), py::arg("c_seq"), py::arg("act"), py::arg("tiled"), py::arg("sync_ws"), py::arg("variant"),
         py::arg("in_gate") = py::none(), py::arg("in_gate_tiles_n") = 0, py::arg("extra_signal") = false, py::arg("stream") = 0,
-        py::arg("launch_flags") = 0);
+        py::arg("launch_flags") = 0, py::arg("lengths") = py::none());
   m.def("lstm_seq_prologue", &lstm_seq_prologue);
   m.def("lstm_seq_bwd_into", &lstm_seq_bwd_into, py::arg("dh_seq"), py::arg("w_hT"), py::arg("act"), py::arg("c_seq"), py::arg("dpre"),
         py::arg("dh0"), py::arg("dc0"), py::arg("tiled"), py::arg("sync_ws"), py::arg("variant"), py::arg("in_gate") = py::none(),
-        py::arg("in_gate_tiles_n") = 0, py::arg("extra_signal") = false, py::arg("stream") = 0, py::arg("launch_flags") = 0);
+        py::arg("in_gate_tiles_n") = 0, py::arg("extra_signal") = false, py::arg("stream") = 0, py::arg("launch_flags") = 0,
+        py::arg("lengths") = py::none());
   m.def("lstm_seq_bwd", &lstm_seq_bwd, py::arg("dh_seq"), py::arg("w_hT"), py::arg("act"), py::arg("c_seq"), py::arg("dhT"),
         py::arg("dcT"), py::arg("sync_ws"), py::arg("variant") = 0, py::arg("dbg") = py::none(), py::arg("in_gate") = py::none(),
-        py::arg("in_gate_tiles_n") = 0, py::arg("extra_signal") = false);
+        py::arg("in_gate_tiles_n") = 0, py::arg("extra_signal") = false, py::arg("lengths") = py::none());
 }

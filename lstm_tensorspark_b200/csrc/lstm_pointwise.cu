@@ -5,17 +5,28 @@
 // take the persistent wgmma kernel in lstm_seq_wgmma.cu instead.
 //
 // Layout: pre/act/dpre are [B, 4H] with column n = 4*j + g, g: 0=i 1=f 2=g(candidate) 3=o. c is fp32.
+// kMasked (per-row lengths, right padding): at step t >= lengths[b] row b holds its state - forward h_t = h_{t-1}, c_t = c_{t-1};
+// backward dpre = 0, dc passes through and the total dh is handed on (dh_out) instead of going through W_h.
 #include "ts_common.cuh"
 
 namespace {
 
-template <typename T, bool kFast>
+template <typename T, bool kFast, bool kMasked = false>
 __global__ void lstm_pointwise_fwd_kernel(const T* __restrict__ pre, const float* __restrict__ bias,
                                           const float* __restrict__ c_prev, T* __restrict__ h_out,
-                                          float* __restrict__ c_out, T* __restrict__ act, int B, int H) {
+                                          float* __restrict__ c_out, T* __restrict__ act, int B, int H,
+                                          const T* __restrict__ h_prev = nullptr, const int* __restrict__ lengths = nullptr,
+                                          int t = 0) {
   int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= B * H) return;
   int j = idx % H;
+  if constexpr (kMasked) {
+    if (t >= lengths[idx / H]) {               // padded step: carry the state (act is never read back)
+      c_out[idx] = c_prev[idx];
+      h_out[idx] = h_prev[idx];
+      return;
+    }
+  }
   const T* p = pre + (size_t)idx * 4;
   float pi = ts::Cvt<T>::to_f(p[0]) + bias[4 * j + 0];
   float pf = ts::Cvt<T>::to_f(p[1]) + bias[4 * j + 1];
@@ -37,16 +48,29 @@ __global__ void lstm_pointwise_fwd_kernel(const T* __restrict__ pre, const float
 }
 
 // dh_a / dh_b: the two sources of dL/dh_t (layer above, and the recurrent term); either may be null.
-template <typename T, bool kFast>
+// kMasked: dh_out [B,H] fp32 = the dh handed to step t-1 directly (the total dh at a padded step, 0 otherwise); the caller
+// adds dpre W_h to it.
+template <typename T, bool kFast, bool kMasked = false>
 __global__ void lstm_pointwise_bwd_kernel(const T* __restrict__ dh_a, const float* __restrict__ dh_b,
                                           const float* __restrict__ dc_in, const T* __restrict__ act,
                                           const float* __restrict__ c_prev, const float* __restrict__ c_new,
-                                          T* __restrict__ dpre, float* __restrict__ dc_out, int B, int H) {
+                                          T* __restrict__ dpre, float* __restrict__ dc_out, int B, int H,
+                                          const int* __restrict__ lengths = nullptr, int t = 0, float* __restrict__ dh_out = nullptr) {
   int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= B * H) return;
   float dh = 0.f;
   if (dh_a) dh += ts::Cvt<T>::to_f(dh_a[idx]);
   if (dh_b) dh += dh_b[idx];
+  if constexpr (kMasked) {
+    const bool pad = t >= lengths[idx / H];
+    dh_out[idx] = pad ? dh : 0.f;
+    if (pad) {
+      dc_out[idx] = dc_in ? dc_in[idx] : 0.f;
+      T* d = dpre + (size_t)idx * 4;
+      d[0] = d[1] = d[2] = d[3] = ts::Cvt<T>::from_f(0.f);
+      return;
+    }
+  }
   const T* a = act + (size_t)idx * 4;
   float i = ts::Cvt<T>::to_f(a[0]), f = ts::Cvt<T>::to_f(a[1]);
   float g = ts::Cvt<T>::to_f(a[2]), o = ts::Cvt<T>::to_f(a[3]);
@@ -65,9 +89,17 @@ __global__ void lstm_pointwise_bwd_kernel(const T* __restrict__ dh_a, const floa
 }  // namespace
 
 extern "C" int ts_lstm_pointwise_fwd(const void* pre, const float* bias, const float* c_prev, void* h_out,
-                                     float* c_out, void* act, int B, int H, int is_bf16, cudaStream_t st) {
+                                     float* c_out, void* act, int B, int H, int is_bf16, cudaStream_t st,
+                                     const void* h_prev, const int* lengths, int t) {
   int n = B * H, thr = 256, blk = (n + thr - 1) / thr;
-  if (is_bf16)
+  if (lengths && is_bf16)
+    lstm_pointwise_fwd_kernel<__nv_bfloat16, true, true><<<blk, thr, 0, st>>>(
+        (const __nv_bfloat16*)pre, bias, c_prev, (__nv_bfloat16*)h_out, c_out, (__nv_bfloat16*)act, B, H,
+        (const __nv_bfloat16*)h_prev, lengths, t);
+  else if (lengths)
+    lstm_pointwise_fwd_kernel<float, false, true><<<blk, thr, 0, st>>>((const float*)pre, bias, c_prev, (float*)h_out,
+                                                                       c_out, (float*)act, B, H, (const float*)h_prev, lengths, t);
+  else if (is_bf16)
     lstm_pointwise_fwd_kernel<__nv_bfloat16, true><<<blk, thr, 0, st>>>(
         (const __nv_bfloat16*)pre, bias, c_prev, (__nv_bfloat16*)h_out, c_out, (__nv_bfloat16*)act, B, H);
   else
@@ -78,9 +110,16 @@ extern "C" int ts_lstm_pointwise_fwd(const void* pre, const float* bias, const f
 
 extern "C" int ts_lstm_pointwise_bwd(const void* dh_a, const float* dh_b, const float* dc_in, const void* act,
                                      const float* c_prev, const float* c_new, void* dpre, float* dc_out, int B,
-                                     int H, int is_bf16, cudaStream_t st) {
+                                     int H, int is_bf16, cudaStream_t st, const int* lengths, int t, float* dh_out) {
   int n = B * H, thr = 256, blk = (n + thr - 1) / thr;
-  if (is_bf16)
+  if (lengths && is_bf16)
+    lstm_pointwise_bwd_kernel<__nv_bfloat16, true, true><<<blk, thr, 0, st>>>(
+        (const __nv_bfloat16*)dh_a, dh_b, dc_in, (const __nv_bfloat16*)act, c_prev, c_new, (__nv_bfloat16*)dpre,
+        dc_out, B, H, lengths, t, dh_out);
+  else if (lengths)
+    lstm_pointwise_bwd_kernel<float, false, true><<<blk, thr, 0, st>>>((const float*)dh_a, dh_b, dc_in, (const float*)act,
+                                                                       c_prev, c_new, (float*)dpre, dc_out, B, H, lengths, t, dh_out);
+  else if (is_bf16)
     lstm_pointwise_bwd_kernel<__nv_bfloat16, true><<<blk, thr, 0, st>>>(
         (const __nv_bfloat16*)dh_a, dh_b, dc_in, (const __nv_bfloat16*)act, c_prev, c_new, (__nv_bfloat16*)dpre,
         dc_out, B, H);

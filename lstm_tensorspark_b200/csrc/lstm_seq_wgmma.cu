@@ -217,6 +217,9 @@ struct SeqParams {
   int no_trap;                 // debugging: the watchdog only records the abort (variant bit 20) instead of killing the kernel
   int extra_signal;            // one more arrival on this CTA's k-block counter after the LAST step's bookkeeping stores (a gated
                                // GEMM consumes h_seq / dpre in the natural layout, which is written after the per-step signal)
+  const int* lengths;          // [B] valid steps per row (right padding, 1 <= len <= T); null = every row runs all T steps.  Read
+                               // only by the kMasked instantiations: at a step t >= len the cell holds its state (h, c carried
+                               // over) and the backward pass emits a zero gate gradient and passes dh / dc through unchanged.
 };
 
 // Work decomposition
@@ -238,7 +241,9 @@ struct SeqParams {
 // k-blocks per step at H = 1024) against a [128 x H/2] weight slice, and the two partial [128 x 128] accumulators are
 // reduce-scattered through DSMEM: every member ends up with the same 64 gate columns = 16 hidden units it owns in the
 // unsplit kernel.  Used when the larger accumulator stage still leaves >= 3 ring stages (smaller H).
-template <bool kBwd, int kStages, int kTiles, bool kStream, bool kFSplit = false>
+// kMasked: per-row sequence lengths (SeqParams::lengths).  A separate instantiation, so the unmasked kernels - at the register
+// cap - carry no extra state; the dataflow, the exchange and the signalling are the same (a padded row still signals every step).
+template <bool kBwd, int kStages, int kTiles, bool kStream, bool kFSplit = false, bool kMasked = false>
 __global__ void __launch_bounds__(384, 1)
 lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
   static_assert(!(kFSplit && (kBwd || kStream || kTiles != 1)), "forward K-split: one tile, resident weights");
@@ -564,6 +569,18 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
 #pragma unroll
         for (int i = 0; i < 8; ++i) cst[tile][i] = row < B ? p.c_seq[(size_t)row * H + j0 + i] : 0.f;     // c_0 (written by the prologue)
       }
+      // kMasked: this thread's row length per tile, and its last emitted h (8 bf16) - a padded step re-emits it without a load.
+      // Step 0 is never padded (len >= 1), so hprev needs no initial value.
+      int len[kTiles];
+      uint4 hprev[kTiles];
+      if constexpr (kMasked) {
+#pragma unroll
+        for (int tile = 0; tile < kTiles; ++tile) {
+          const int row = (mb0 + tile) * BM + rloc;
+          len[tile] = row < B ? p.lengths[row] : p.T;
+          hprev[tile] = make_uint4(0u, 0u, 0u, 0u);
+        }
+      }
       for (int t = 0; t < p.T && ok; ++t) {
 #pragma unroll
         for (int tile = 0; tile < kTiles; ++tile) {
@@ -625,6 +642,7 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
             acc_ld32(32 * half, v);
           }
           if (dbg_thread && t == 8 && tile == 0) p.dbg[4 * (p.T + 2) + 0] = gtime();
+          const bool pad = kMasked && t >= len[tile];   // padded step: the cell holds (the activations are computed but unused)
           float cn[8], hv[8];
           uint32_t apk[16];
 #pragma unroll
@@ -636,13 +654,22 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
             const float po = __uint_as_float(v[4 * jj + 3]) + bf_hi(gb) + bs[4 * jj + 3];
             const float ig = ts::sigmoidf_fast(pi), fg = ts::sigmoidf_fast(pf), gg = ts::tanhf_fast(pg), og = ts::sigmoidf_fast(po);
             const float c = fg * cst[tile][jj] + ig * gg;
-            cst[tile][jj] = c;                        // the cell state never leaves the registers of its thread
-            cn[jj] = c;
+            if constexpr (kMasked) {
+              if (!pad) cst[tile][jj] = c;
+              cn[jj] = cst[tile][jj];
+            } else {
+              cst[tile][jj] = c;                      // the cell state never leaves the registers of its thread
+              cn[jj] = c;
+            }
             hv[jj] = og * ts::tanhf_fast(c);
             apk[2 * jj] = pack_bf2(ig, fg);
             apk[2 * jj + 1] = pack_bf2(gg, og);
           }
-          const uint4 h8 = make_uint4(pack_bf2(hv[0], hv[1]), pack_bf2(hv[2], hv[3]), pack_bf2(hv[4], hv[5]), pack_bf2(hv[6], hv[7]));
+          uint4 h8 = make_uint4(pack_bf2(hv[0], hv[1]), pack_bf2(hv[2], hv[3]), pack_bf2(hv[4], hv[5]), pack_bf2(hv[6], hv[7]));
+          if constexpr (kMasked) {
+            if (pad) h8 = hprev[tile];
+            hprev[tile] = h8;
+          }
           {
             // next step's operand first (the only thing other CTAs wait for): 8 values = one 16 B chunk of the swizzled
             // tile image; chunk c of row r sits at position c ^ (r & 7)
@@ -714,6 +741,16 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
         }
       }
       U8 c_carry[kTiles];                       // c_t of the previous iteration = c_{t+1} of this one (one load per step, not two)
+      // kMasked: right padding makes a row's padded steps the FIRST backward iterations.  There dG = 0, dc passes through and
+      // dh[tile] keeps the total dh (carry + dh_seq[t]): the next exchange sum adds the (exactly zero) recurrent term to it.
+      int len[kTiles];
+      if constexpr (kMasked) {
+#pragma unroll
+        for (int tile = 0; tile < kTiles; ++tile) {
+          const int row = (mb0 + tile) * BM + rloc;
+          len[tile] = row < B ? p.lengths[row] : p.T;
+        }
+      }
       for (int s = 0; s <= p.T && ok; ++s) {
         const int t = p.T - 1 - s;
 #pragma unroll
@@ -721,6 +758,8 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
           const int mb = mb0 + tile;
           const int row = mb * BM + rloc;
           const bool valid = row < B;
+          const bool pad = kMasked && s < p.T && t >= len[tile];           // step t is padding for this row
+          const bool prev_pad = kMasked && s > 0 && t + 1 >= len[tile];    // step t + 1 was: dh carries, c_carry is not set
           uint8_t* xbuf = smem_x + tile * kXchgBytes;               // [kSplit src][128 rows][16 bf16]
           const uint32_t xbase = tc::smem_u32(xbuf);
           const uint32_t xbar = tc::smem_u32(&ss->xchg_full[tile]);
@@ -733,18 +772,20 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
           }
           if (valid && s < p.T) {
             const __nv_bfloat16* ap = p.act + ((size_t)t * B + row) * (4 * H) + 4 * j0;
-            avw[0] = ldg_nc32(ap); avw[1] = ldg_nc32(ap + 16);
+            if (!pad) { avw[0] = ldg_nc32(ap); avw[1] = ldg_nc32(ap + 16); }
             dhv = p.dh_seq ? (p.in_gate ? ldg_cg16(p.dh_seq + ((size_t)t * B + row) * H + j0) : ldg_nc16(p.dh_seq + ((size_t)t * B + row) * H + j0))
                            : make_uint4(0u, 0u, 0u, 0u);
             const float* c0p = p.c_seq + ((size_t)t * B + row) * H + j0;
             const float* c1p = p.c_seq + ((size_t)(t + 1) * B + row) * H + j0;
-            cpv = ldg_nc32(c0p);
-            cnv = (s == 0) ? ldg_nc32(c1p) : c_carry[tile];
-            c_carry[tile] = cpv;
-            if (t >= 2) {                                                      // saved activations come from HBM: pull t-2 into L2 early
-              prefetch_l2(ap - (size_t)2 * B * (4 * H));
-              prefetch_l2(c0p - (size_t)2 * B * H);
-              if (p.dh_seq && !p.in_gate) prefetch_l2(p.dh_seq + ((size_t)(t - 2) * B + row) * H + j0);
+            if (!pad) {
+              cpv = ldg_nc32(c0p);
+              cnv = (s == 0 || prev_pad) ? ldg_nc32(c1p) : c_carry[tile];
+              c_carry[tile] = cpv;
+              if (t >= 2) {                                                    // saved activations come from HBM: pull t-2 into L2 early
+                prefetch_l2(ap - (size_t)2 * B * (4 * H));
+                prefetch_l2(c0p - (size_t)2 * B * H);
+                if (p.dh_seq && !p.in_gate) prefetch_l2(p.dh_seq + ((size_t)(t - 2) * B + row) * H + j0);
+              }
             }
           }
           if (s > 0) {
@@ -772,8 +813,10 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
             }
             ok = xwait(&ss->xchg_full[tile], xphase, abort_flag);
             if (!ok) break;
+            if (!prev_pad) {
 #pragma unroll
-            for (int i = 0; i < 8; ++i) dh[tile][i] = 0.f;
+              for (int i = 0; i < 8; ++i) dh[tile][i] = 0.f;
+            }
 #pragma unroll
             for (int src = 0; src < kSplit; ++src) {
               const uint4 x4 = *reinterpret_cast<const uint4*>(xbuf + (size_t)(src * BM + rloc) * 32 + 16 * half);
@@ -808,11 +851,20 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
             const float dht = dh[tile][jj] + ((jj & 1) ? bf_hi(dw) : bf_lo(dw));
             const float cprev = __uint_as_float(cpv.v[jj]);
             const float tcn = ts::tanhf_fast(__uint_as_float(cnv.v[jj]));
-            const float dct = dc[tile][jj] + dht * og * (1.f - tcn * tcn);
+            const float dc_in = dc[tile][jj];
+            const float dct = dc_in + dht * og * (1.f - tcn * tcn);
             const float d_o = dht * tcn, d_i = dct * gg, d_f = dct * cprev, d_g = dct * ig;
             dc[tile][jj] = dct * fg;
             gpk[2 * jj] = pack_bf2(d_i * ig * (1.f - ig), d_f * fg * (1.f - fg));
             gpk[2 * jj + 1] = pack_bf2(d_g * (1.f - gg * gg), d_o * og * (1.f - og));
+            if constexpr (kMasked) {
+              if (pad) {                          // (the loads above were skipped: everything but dht is discarded)
+                dc[tile][jj] = dc_in;
+                dh[tile][jj] = dht;
+                gpk[2 * jj] = 0u;
+                gpk[2 * jj + 1] = 0u;
+              }
+            }
           }
           {
             // next iteration's operand first: this thread's 32 gate columns = 4 chunks of row rloc of k-block j0/16
@@ -898,9 +950,9 @@ size_t smem_bytes(int H, bool bwd, int stages, int tiles, bool stream = false, b
   return (stream ? 0 : (size_t)(H / BK) * kWBlockBytes) + ring + ((bwd || fsplit) ? tiles * kXchgBytes : 0) + acc_stage + sizeof(SeqSmem) + 1024;
 }
 
-template <bool kBwd, int kStages, int kTiles, bool kStream = false, bool kFSplit = false>
+template <bool kBwd, int kStages, int kTiles, bool kStream = false, bool kFSplit = false, bool kMasked = false>
 int launch_cfg(const CUtensorMap& tw, const SeqParams& p, int grid, cudaStream_t st) {
-  auto kern = lstm_seq_kernel<kBwd, kStages, kTiles, kStream, kFSplit>;
+  auto kern = lstm_seq_kernel<kBwd, kStages, kTiles, kStream, kFSplit, kMasked>;
   const size_t smem = smem_bytes(p.H, kBwd, kStages, kTiles, kStream, kFSplit);
   constexpr int kClusterDim = kBwd ? (kStream ? 2 : 4) : (kFSplit ? 2 : 1);
   if (smem > 227 * 1024) return -4;
@@ -927,42 +979,42 @@ int launch_cfg(const CUtensorMap& tw, const SeqParams& p, int grid, cudaStream_t
   return (int)e;
 }
 
-template <bool kBwd>
+template <bool kBwd, bool kMasked>
 int dispatch(const CUtensorMap& tw, const SeqParams& p, int grid, int stages, int tiles, bool stream, bool fsplit, cudaStream_t st) {
   if constexpr (!kBwd) {
     if (fsplit) {                                  // forward K-split (cluster of 2), one batch tile per CTA
       switch (stages) {
-        case 3: return launch_cfg<false, 3, 1, false, true>(tw, p, grid, st);
-        case 4: return launch_cfg<false, 4, 1, false, true>(tw, p, grid, st);
-        case 5: return launch_cfg<false, 5, 1, false, true>(tw, p, grid, st);
-        case 6: return launch_cfg<false, 6, 1, false, true>(tw, p, grid, st);
+        case 3: return launch_cfg<false, 3, 1, false, true, kMasked>(tw, p, grid, st);
+        case 4: return launch_cfg<false, 4, 1, false, true, kMasked>(tw, p, grid, st);
+        case 5: return launch_cfg<false, 5, 1, false, true, kMasked>(tw, p, grid, st);
+        case 6: return launch_cfg<false, 6, 1, false, true, kMasked>(tw, p, grid, st);
       }
       return -5;
     }
   }
   if (stream) {                                    // streamed weights: 24 KB stages, one batch tile per CTA
     switch (stages) {
-      case 4: return launch_cfg<kBwd, 4, 1, true>(tw, p, grid, st);
-      case 6: return launch_cfg<kBwd, 6, 1, true>(tw, p, grid, st);
-      case 8: return launch_cfg<kBwd, 8, 1, true>(tw, p, grid, st);
+      case 4: return launch_cfg<kBwd, 4, 1, true, false, kMasked>(tw, p, grid, st);
+      case 6: return launch_cfg<kBwd, 6, 1, true, false, kMasked>(tw, p, grid, st);
+      case 8: return launch_cfg<kBwd, 8, 1, true, false, kMasked>(tw, p, grid, st);
     }
     return -5;
   }
   if (tiles == 2) {
     switch (stages) {
-      case 2: return launch_cfg<kBwd, 2, 2>(tw, p, grid, st);
-      case 3: return launch_cfg<kBwd, 3, 2>(tw, p, grid, st);
-      case 4: return launch_cfg<kBwd, 4, 2>(tw, p, grid, st);
-      case 5: return launch_cfg<kBwd, 5, 2>(tw, p, grid, st);
-      case 6: return launch_cfg<kBwd, 6, 2>(tw, p, grid, st);
+      case 2: return launch_cfg<kBwd, 2, 2, false, false, kMasked>(tw, p, grid, st);
+      case 3: return launch_cfg<kBwd, 3, 2, false, false, kMasked>(tw, p, grid, st);
+      case 4: return launch_cfg<kBwd, 4, 2, false, false, kMasked>(tw, p, grid, st);
+      case 5: return launch_cfg<kBwd, 5, 2, false, false, kMasked>(tw, p, grid, st);
+      case 6: return launch_cfg<kBwd, 6, 2, false, false, kMasked>(tw, p, grid, st);
     }
   } else {
     switch (stages) {
-      case 2: return launch_cfg<kBwd, 2, 1>(tw, p, grid, st);
-      case 3: return launch_cfg<kBwd, 3, 1>(tw, p, grid, st);
-      case 4: return launch_cfg<kBwd, 4, 1>(tw, p, grid, st);
-      case 5: return launch_cfg<kBwd, 5, 1>(tw, p, grid, st);
-      case 6: return launch_cfg<kBwd, 6, 1>(tw, p, grid, st);
+      case 2: return launch_cfg<kBwd, 2, 1, false, false, kMasked>(tw, p, grid, st);
+      case 3: return launch_cfg<kBwd, 3, 1, false, false, kMasked>(tw, p, grid, st);
+      case 4: return launch_cfg<kBwd, 4, 1, false, false, kMasked>(tw, p, grid, st);
+      case 5: return launch_cfg<kBwd, 5, 1, false, false, kMasked>(tw, p, grid, st);
+      case 6: return launch_cfg<kBwd, 6, 1, false, false, kMasked>(tw, p, grid, st);
     }
   }
   return -5;
@@ -1017,14 +1069,16 @@ static int seq_common(SeqParams& p, const void* w_base, int variant, cudaStream_
   if (int rc = ts::make_tmap_2d_bf16(&tw, w_base, (uint64_t)N, (uint64_t)K, (uint64_t)K, BK, fsplit ? 2 * BN : ((kBwd && stream) ? BN / 2 : BN))) return rc;
   p.tiles_n = tiles_n;
   p.tiles_m = tiles_m;
-  int rc = dispatch<kBwd>(tw, p, grid, stages, tiles, stream, fsplit, st);
+  int rc = p.lengths ? dispatch<kBwd, true>(tw, p, grid, stages, tiles, stream, fsplit, st)
+                     : dispatch<kBwd, false>(tw, p, grid, stages, tiles, stream, fsplit, st);
   if (rc == -21) ts::set_last_error("lstm_seq: the thread-block clusters are not co-resident on this device");
   return rc;
 }
 
 extern "C" int ts_lstm_seq_fwd(const void* gx, const void* w_h, const float* bias, const void* h_seq, const float* c_seq,
                                void* act, const float* c0, void* dbg, void* a_tiled, int T, int B, int H, unsigned int* sync_ws, int variant,
-                               cudaStream_t st, const void* h0, const unsigned int* in_gate, int in_gate_tiles_n, int extra_signal, int launch_flags) {
+                               cudaStream_t st, const void* h0, const unsigned int* in_gate, int in_gate_tiles_n, int extra_signal, int launch_flags,
+                               const int* lengths) {
   if (!(launch_flags & 1)) {           // bit 0: the caller has run ts_lstm_seq_prologue itself (wavefront: all prologues precede the chain)
     const int tiles_m = (B + BM - 1) / BM;
     const int total = tiles_m * BM * (H / 8);
@@ -1039,6 +1093,7 @@ extern "C" int ts_lstm_seq_fwd(const void* gx, const void* w_h, const float* bia
   p.act = (__nv_bfloat16*)act; p.sync = sync_ws; p.T = T; p.B = B; p.H = H; p.dbg = (unsigned long long*)dbg;
   p.in_gate = in_gate; p.in_gate_tiles_n = in_gate_tiles_n; p.extra_signal = extra_signal;
   p.pdl_wait = (launch_flags >> 1) & 1;
+  p.lengths = lengths;
   return seq_common<false>(p, w_h, variant, st);
 }
 
@@ -1054,7 +1109,8 @@ extern "C" int ts_lstm_seq_prologue(const void* h0, const float* c0, void* h_seq
 
 extern "C" int ts_lstm_seq_bwd(const void* dh_seq, const void* w_hT, const void* act, const float* c_seq, const void* dpre,
                                float* dh0, float* dc0, void* dbg, void* a_tiled, int T, int B, int H, unsigned int* sync_ws, int variant,
-                               cudaStream_t st, const unsigned int* in_gate, int in_gate_tiles_n, int extra_signal, int launch_flags) {
+                               cudaStream_t st, const unsigned int* in_gate, int in_gate_tiles_n, int extra_signal, int launch_flags,
+                               const int* lengths) {
   if (!(launch_flags & 1)) cudaMemsetAsync(sync_ws, 0, kSyncErr * sizeof(unsigned int), st);      // arrival counters restart at 0 every launch
   SeqParams p{};
   p.a_tiled = (__nv_bfloat16*)a_tiled;
@@ -1062,6 +1118,7 @@ extern "C" int ts_lstm_seq_bwd(const void* dh_seq, const void* w_hT, const void*
   p.dh0 = dh0; p.dc0 = dc0; p.sync = sync_ws; p.T = T; p.B = B; p.H = H; p.dbg = (unsigned long long*)dbg;
   p.in_gate = in_gate; p.in_gate_tiles_n = in_gate_tiles_n; p.extra_signal = extra_signal;
   p.pdl_wait = (launch_flags >> 1) & 1;
+  p.lengths = lengths;
   return seq_common<true>(p, w_hT, variant, st);
 }
 

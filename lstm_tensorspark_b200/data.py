@@ -120,6 +120,37 @@ def process_batch(train_xy: Sequence[Sequence[str]], normalize: bool = False,
     return x, y
 
 
+def process_batch_ragged(train_xy: Sequence[Sequence[str]], seq_len: int, in_features: int,
+                         normalize: bool = False) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+    """Variable-length rows -> ``(x float32 [N, seq_len, in_features], y int64 [N], lengths int32 [N])``.
+
+    A row is ``k * in_features`` values followed by the label, ``1 <= k <= seq_len``; it is zero-padded on the right to
+    ``seq_len`` steps and ``lengths = k``.  ``normalize``: global min-max over the real values only (padding excluded)."""
+    if seq_len < 1 or in_features < 1:
+        raise ValueError("variable-length rows need seq_len >= 1 and in_features >= 1")
+    xs, ys, ls = [], [], []
+    for n, row in enumerate(train_xy):
+        if len(row) <= 1:
+            continue
+        width = len(row) - 1
+        if width % in_features != 0 or not (1 <= width // in_features <= seq_len):
+            raise ValueError(f"row {n}: {width} values is not a whole number of 1..{seq_len} steps of "
+                             f"{in_features} features")
+        xs.append([float(v) for v in row[:-1]])
+        ys.append(int(float(row[-1])))
+        ls.append(width // in_features)
+    if not xs:
+        raise ValueError("empty partition: no parsable rows")
+    if normalize:
+        flat = min_max_normalizer(np.concatenate([np.asarray(r, dtype=np.float64) for r in xs]))
+        off = np.cumsum([0] + [len(r) for r in xs])
+        xs = [flat[off[i]:off[i + 1]] for i in range(len(xs))]
+    x = np.zeros((len(xs), seq_len, in_features), dtype=np.float32)
+    for i, r in enumerate(xs):
+        x[i, :ls[i]] = np.asarray(r, dtype=np.float32).reshape(ls[i], in_features)
+    return x, np.asarray(ys, dtype=np.int64), np.asarray(ls, dtype=np.int32)
+
+
 def resolve_batch_size(batch_size: int, shard_rows: int) -> int:
     """``--batch_size 0`` = whole shard (reference intent, src/rnn.py:193-199, Q3)."""
     bs = shard_rows if not batch_size else batch_size
@@ -152,8 +183,11 @@ def next_batch(train_x, train_y, batch_size: int = 10, shuffle: bool = True,
 # synthetic sequences (benchmark configs of BASELINE.json)
 # ------------------------------------------------------------------------------------------------
 def synthetic_sequences(n: int, seq_len: int, in_features: int, num_classes: int, seed: int = 0,
-                        dtype=np.float32) -> Tuple[np.ndarray, np.ndarray]:
-    """Class-dependent gaussian sequences (learnable, so loss curves are meaningful)."""
+                        dtype=np.float32, variable_length: bool = False):
+    """Class-dependent gaussian sequences (learnable, so loss curves are meaningful).  -> ``(x, y)``.
+
+    ``variable_length``: -> ``(x, y, lengths)``, the same ``x`` / ``y`` with per-sample lengths drawn uniformly from
+    ``[max(1, seq_len // 4), seq_len]`` (int32) by a generator of their own, and the padded steps zeroed."""
     rng = np.random.default_rng(seed)
     y = rng.integers(0, num_classes, size=n).astype(np.int64)
     centers = rng.standard_normal((num_classes, in_features)).astype(np.float32)
@@ -161,7 +195,19 @@ def synthetic_sequences(n: int, seq_len: int, in_features: int, num_classes: int
         x = rng.standard_normal((n, seq_len, in_features), dtype=np.float32) * 0.5 + centers[y][:, None, :]
     else:
         x = rng.standard_normal((n, in_features), dtype=np.float32) * 0.5 + centers[y]
-    return x.astype(dtype), y
+    if not variable_length:
+        return x.astype(dtype), y
+    if seq_len < 2:
+        raise ValueError("variable-length sequences need seq_len >= 2")
+    lengths = synthetic_lengths(n, seq_len, seed)
+    x[np.arange(seq_len)[None, :] >= lengths[:, None]] = 0.0
+    return x.astype(dtype), y, lengths
+
+
+def synthetic_lengths(n: int, seq_len: int, seed: int = 0) -> np.ndarray:
+    """Per-sample lengths, uniform in ``[max(1, seq_len // 4), seq_len]``, int32, from a generator seeded apart from the data's."""
+    rng = np.random.default_rng([seed, 0x6C656E])
+    return rng.integers(max(1, seq_len // 4), seq_len + 1, size=n).astype(np.int32)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -172,9 +218,11 @@ class DeviceShard:
     (replaces the per-step feed_dict copy, src/rnn.py:264-267)."""
 
     def __init__(self, x: np.ndarray, y: np.ndarray, batch_size: int, device, dtype=torch.float32,
-                 shuffle: bool = True, seed: int = 0):
+                 shuffle: bool = True, seed: int = 0, lengths: Optional[np.ndarray] = None):
+        """``lengths``: optional per-row sequence lengths; they follow their rows and ``next()`` returns them third."""
         self.x = torch.as_tensor(x).to(device=device, dtype=dtype)
         self.y = torch.as_tensor(y).to(device=device)
+        self.lengths = None if lengths is None else torch.as_tensor(lengths).to(device=device, dtype=torch.int32)
         self.n = self.x.shape[0]
         self.batch_size = resolve_batch_size(batch_size, self.n)
         self.per_epoch = self.n // self.batch_size
@@ -191,19 +239,27 @@ class DeviceShard:
             self._perm = torch.arange(self.n, device=self.x.device)
         self._i = 0
 
-    def next(self, out=None) -> Tuple[torch.Tensor, torch.Tensor]:
-        """``out = (x_buf, y_buf)``: gather the batch straight into these buffers (the input buffers of a captured CUDA graph:
-        ``TrainEngine.graph_inputs()``) instead of into fresh tensors that then have to be copied there."""
+    def next(self, out=None) -> Tuple[torch.Tensor, ...]:
+        """-> ``(x, y)``, or ``(x, y, lengths)`` for a shard with lengths.  ``out = (x_buf, y_buf[, lengths_buf])``: gather the
+        batch straight into these buffers (the input buffers of a captured CUDA graph: ``TrainEngine.graph_inputs()``)
+        instead of into fresh tensors that then have to be copied there."""
         if self._perm is None or self._i >= self.per_epoch:
             self._reshuffle()
         lo = self._i * self.batch_size
         idx = self._perm[lo:lo + self.batch_size]
         self._i += 1
-        if out is not None and out[0].shape[0] == idx.numel() and out[0].dtype == self.x.dtype:
+        out_l = out[2] if (out is not None and len(out) > 2) else None
+        if out is not None and out[0].shape[0] == idx.numel() and out[0].dtype == self.x.dtype \
+                and (self.lengths is None or out_l is not None):
             torch.index_select(self.x, 0, idx, out=out[0])
             torch.index_select(self.y, 0, idx, out=out[1])
-            return out[0], out[1]
-        return self.x.index_select(0, idx), self.y.index_select(0, idx)
+            if self.lengths is None:
+                return out[0], out[1]
+            torch.index_select(self.lengths, 0, idx, out=out_l)
+            return out[0], out[1], out_l
+        if self.lengths is None:
+            return self.x.index_select(0, idx), self.y.index_select(0, idx)
+        return self.x.index_select(0, idx), self.y.index_select(0, idx), self.lengths.index_select(0, idx)
 
     def state_dict(self):
         return {"gen": self.gen.get_state(), "i": self._i,
@@ -221,8 +277,10 @@ class PinnedHostLoader:
     Shuffling permutes the pinned copy once per pass (not per step), so a step is exactly one H2D DMA per tensor."""
 
     def __init__(self, x: np.ndarray, y: np.ndarray, batch_size: int, device, dtype=torch.float32,
-                 shuffle: bool = True, seed: int = 0, depth: int = 2):
-        """``depth``: device staging slots (the copy of a batch is enqueued ``depth - 1`` calls before it is handed out)."""
+                 shuffle: bool = True, seed: int = 0, depth: int = 2, lengths: Optional[np.ndarray] = None):
+        """``depth``: device staging slots (the copy of a batch is enqueued ``depth - 1`` calls before it is handed out).
+        ``lengths``: optional per-row sequence lengths, permuted and copied with their rows; ``next()`` returns them third
+        and every staging slot of ``dev`` is an ``(x, y, lengths)`` triple."""
         assert depth >= 2
         self.device = torch.device(device)
         self.dtype = dtype
@@ -236,12 +294,17 @@ class PinnedHostLoader:
         cuda = self.device.type == "cuda"
         self.x_host = torch.as_tensor(x).to(dtype).contiguous()
         self.y_host = torch.as_tensor(y).contiguous()
+        self.l_host = None if lengths is None else torch.as_tensor(lengths).to(torch.int32).contiguous()
         if cuda:
             self.x_host = self.x_host.pin_memory()
             self.y_host = self.y_host.pin_memory()
+            if self.l_host is not None:
+                self.l_host = self.l_host.pin_memory()
         shape_x = (self.batch_size,) + tuple(self.x_host.shape[1:])
         self.dev = [(torch.empty(shape_x, dtype=dtype, device=self.device),
-                     torch.empty((self.batch_size,), dtype=torch.int64, device=self.device)) for _ in range(depth)]
+                     torch.empty((self.batch_size,), dtype=torch.int64, device=self.device))
+                    + (() if self.l_host is None else (torch.empty((self.batch_size,), dtype=torch.int32, device=self.device),))
+                    for _ in range(depth)]
         self._slot = 0
         self._pending = []
         self._copy_stream = None
@@ -256,7 +319,8 @@ class PinnedHostLoader:
         if not shuffle:
             self._pass_start[1] = (self.gen.get_state(), self._order.clone())
         self._consumed = (self._pass, 0)
-        self.bytes_per_batch = self.dev[0][0].numel() * self.dev[0][0].element_size() + self.batch_size * 8
+        self.bytes_per_batch = self.dev[0][0].numel() * self.dev[0][0].element_size() + self.batch_size * 8 \
+            + (0 if self.l_host is None else self.batch_size * 4)
 
     def _reshuffle(self):
         # the async H2D copy of the last batch of the previous pass may not have run yet (the host is ahead of the GPU):
@@ -272,6 +336,8 @@ class PinnedHostLoader:
         xs, ys = self.x_host[idx], self.y_host[idx]
         self.x_host.copy_(xs)
         self.y_host.copy_(ys)
+        if self.l_host is not None:
+            self.l_host.copy_(self.l_host[idx])
         self._order = perm
 
     def _advance(self) -> int:
@@ -304,6 +370,8 @@ class PinnedHostLoader:
         order = st["order"]
         self.x_host.copy_(self.x_host[order])
         self.y_host.copy_(self.y_host[order])
+        if self.l_host is not None:
+            self.l_host.copy_(self.l_host[order])
         self._order = order.clone()
         self.gen.set_state(st["gen"])
         self._pass = 0
@@ -317,12 +385,15 @@ class PinnedHostLoader:
         """Enqueue the H2D copy of the next batch on the copy stream into the free staging slot."""
         lo = self._advance()
         tag = (self._pass, self._i)                      # handing this batch out makes it the consumed position
-        dx, dy = self.dev[self._slot]
+        slot = self.dev[self._slot]
+        dx, dy = slot[0], slot[1]
         self._slot = (self._slot + 1) % self.depth
         if self.device.type != "cuda":
             dx.copy_(self.x_host[lo:lo + self.batch_size])
             dy.copy_(self.y_host[lo:lo + self.batch_size])
-            return dx, dy, None, tag
+            if self.l_host is not None:
+                slot[2].copy_(self.l_host[lo:lo + self.batch_size])
+            return slot, None, tag
         if self._copy_stream is None:
             self._copy_stream = torch.cuda.Stream(device=self.device)
         # the slot being overwritten was consumed by compute work already enqueued on the current stream
@@ -331,18 +402,21 @@ class PinnedHostLoader:
             if not self.debug_skip_copy:                  # (bench diagnostics only: how much of a step is the DMA's interference?)
                 dx.copy_(self.x_host[lo:lo + self.batch_size], non_blocking=True)
                 dy.copy_(self.y_host[lo:lo + self.batch_size], non_blocking=True)
+                if self.l_host is not None:
+                    slot[2].copy_(self.l_host[lo:lo + self.batch_size], non_blocking=True)
             ev = torch.cuda.Event()
             ev.record(self._copy_stream)
-        return dx, dy, ev, tag
+        return slot, ev, tag
 
-    def next(self) -> Tuple[torch.Tensor, torch.Tensor]:
-        """Returns this step's batch (its H2D copy was enqueued one call earlier, so it overlaps the previous step's
-        compute) and enqueues the copy of the following one.  Every step still moves its own inputs host->device."""
+    def next(self) -> Tuple[torch.Tensor, ...]:
+        """Returns this step's batch - ``(x, y)``, or ``(x, y, lengths)`` with lengths - (its H2D copy was enqueued one call
+        earlier, so it overlaps the previous step's compute) and enqueues the copy of the following one.  Every step still
+        moves its own inputs host->device."""
         while len(self._pending) < self.depth - 1:
             self._pending.append(self._issue())
-        dx, dy, ev, self._consumed = self._pending.pop(0)
+        slot, ev, self._consumed = self._pending.pop(0)
         if ev is not None:
             torch.cuda.current_stream(self.device).wait_event(ev)
         # refill: the slot this copy overwrites was handed out depth - 1 calls ago; the step that consumed it is enqueued
         self._pending.append(self._issue())
-        return dx, dy
+        return slot

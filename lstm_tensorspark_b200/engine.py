@@ -4,6 +4,7 @@ This is what ``bench.py``, ``__graft_entry__.smoke`` and the per-replica trainer
 
     eng = TrainEngine(cfg, rank, world_size, comm, batch_size=B)
     loss = eng.step(x, y)            # forward, backward, (fused allreduce +) optimizer update
+    loss = eng.step(x, y, lengths)   # variable-length batch: int32 [B] per-sample lengths, x right-padded
 
 One step replaces the reference's ``sess.run([train_op, loss], feed_dict=...)`` (original src/rnn.py:264-267):
 H2D feed, forward, backward, 14·L+2 ApplyAdam launches, D2H loss.  With ``cuda_graph=True`` the whole step is
@@ -72,7 +73,7 @@ class TrainEngine:
                                                          and cfg.grad_buckets) else None
         self._graph = None
         self._static = None
-        self._bound = {}                        # (x ptr, y ptr, shape) -> (graph captured on that buffer, its loss tensor)
+        self._bound = {}                        # (x ptr, y ptr, lengths ptr, shape) -> (graph captured on those buffers, its loss)
         self._bound_keepalive = []
         self.steps_done = 0
 
@@ -132,9 +133,9 @@ class TrainEngine:
         for b in plan[state["next"]:]:
             comm.launch_bucket(b["lo"], b["hi"])
 
-    def _step_eager(self, x: torch.Tensor, y: torch.Tensor) -> torch.Tensor:
+    def _step_eager(self, x: torch.Tensor, y: torch.Tensor, lengths: Optional[torch.Tensor] = None) -> torch.Tensor:
         self.flat.zero_grad()
-        loss, _logits, _correct = self.model(x, y)
+        loss, _logits, _correct = self.model(x, y, lengths)
         if self._wd_autograd:
             loss = loss + torch.stack([fn(v) * wd for (v, fn, wd) in self._wd_autograd]).sum()
         l2 = None
@@ -154,29 +155,35 @@ class TrainEngine:
             loss = loss.detach() + l2
         return loss.detach()
 
-    def step(self, x: torch.Tensor, y: torch.Tensor) -> torch.Tensor:
-        """One full training step on this replica; returns the (detached, device) loss."""
+    def step(self, x: torch.Tensor, y: torch.Tensor, lengths: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """One full training step on this replica; returns the (detached, device) loss.  ``lengths``: optional int32 ``[B]``
+        per-sample sequence lengths of a right-padded ``x`` (a captured graph must have been captured with lengths too)."""
         self.steps_done += 1
         if self._graph is None:
-            return self._step_eager(x, y)
-        bound = self._bound.get((x.data_ptr(), y.data_ptr(), tuple(x.shape)))
+            return self._step_eager(x, y, lengths)
+        if (lengths is None) != (self._static[2] is None):
+            raise ValueError("the captured step was captured " + ("with" if lengths is None else "without") + " lengths")
+        bound = self._bound.get((x.data_ptr(), y.data_ptr(), 0 if lengths is None else lengths.data_ptr(), tuple(x.shape)))
         if bound is not None:                   # the batch already sits in a buffer a graph was captured on: no staging copy
             g, sloss = bound
         else:
-            sx, sy, sloss = self._static
+            sx, sy, sl, sloss = self._static
             if x.data_ptr() != sx.data_ptr():       # (a loader may have gathered the batch straight into graph_inputs())
                 sx.copy_(x, non_blocking=True)
             if y.data_ptr() != sy.data_ptr():
                 sy.copy_(y, non_blocking=True)
+            if lengths is not None and lengths.data_ptr() != sl.data_ptr():
+                sl.copy_(lengths, non_blocking=True)
             g = self._graph
         g.replay()
         self.optimizer.step_count += 1          # host mirror; the kernels use the device-resident counter
         return sloss
 
     def graph_inputs(self):
-        """(x, y) input buffers of the captured graph, or None: a loader that assembles batches on the device can write them
-        here directly (``DeviceShard.next(out=...)``) and ``step()`` then skips its staging copy."""
-        return None if self._graph is None else self._static[:2]
+        """(x, y, lengths) input buffers of the captured graph (lengths None when captured without), or None: a loader that
+        assembles batches on the device can write them here directly (``DeviceShard.next(out=...)``) and ``step()`` then skips
+        its staging copy."""
+        return None if self._graph is None else self._static[:3]
 
     def maybe_average(self, force: bool = False):
         """Parameter-average sync point (reference semantics: once, at the end; or every ``sync_every`` steps)."""
@@ -187,16 +194,20 @@ class TrainEngine:
             self.comm.average_params_(self.flat, cfg.average_scope)
 
     # ---------------------------------------------------------------------------------------------------
-    def capture(self, x: torch.Tensor, y: torch.Tensor, warmup: int = 3, bind=()):
+    def capture(self, x: torch.Tensor, y: torch.Tensor, warmup: int = 3, bind=(), lengths: Optional[torch.Tensor] = None):
         """Capture fwd+bwd+update into one CUDA graph (static shapes).  Adam's bias correction is derived in-kernel from
         a device-resident step counter, so replays are exact.
 
         ``bind``: ``(x, y)`` pairs of LONG-LIVED device buffers that batches will be handed over in (the two staging slots of
         ``PinnedHostLoader``, fixed slices of a device-resident shard).  One more graph is captured directly on each of them,
         and ``step()`` replays it when it is given exactly that buffer - the 67 MB copy into the graph's own input buffer
-        (27 us of a 4 ms step) disappears.  Any other tensor still goes through the staging copy."""
+        (27 us of a 4 ms step) disappears.  Any other tensor still goes through the staging copy.
+
+        ``lengths`` (int32 ``[B]``): variable-length batches - a third static graph input; ``bind`` then takes
+        ``(x, y, lengths)`` triples."""
         assert self.device.type == "cuda"
         sx, sy = x.clone(), y.clone()
+        sl = None if lengths is None else lengths.clone()
         # warm-up / capture run real updates: snapshot the training state and put it back, so capturing is not
         # `warmup` uncounted optimizer steps on one batch and the host / device Adam step counters stay equal
         opt = self.optimizer
@@ -207,19 +218,21 @@ class TrainEngine:
         s.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(s):
             for _ in range(warmup):
-                self._step_eager(sx, sy)
+                self._step_eager(sx, sy, sl)
         torch.cuda.current_stream().wait_stream(s)
         g = torch.cuda.CUDAGraph()
         with torch.cuda.graph(g):
-            sloss = self._step_eager(sx, sy)
+            sloss = self._step_eager(sx, sy, sl)
         bound = {}
-        for bx, by in bind:
+        for b in bind:
+            bx, by, bl = (tuple(b) + (None,))[:3]
             assert bx.shape == sx.shape and bx.dtype == sx.dtype and by.shape == sy.shape and bx.is_contiguous() and by.is_contiguous()
+            assert (bl is None) == (sl is None) and (bl is None or (bl.shape == sl.shape and bl.dtype == sl.dtype and bl.is_contiguous()))
             gb = torch.cuda.CUDAGraph()
             with torch.cuda.graph(gb):
-                lb = self._step_eager(bx, by)
-            bound[(bx.data_ptr(), by.data_ptr(), tuple(bx.shape))] = (gb, lb)
-            self._bound_keepalive.append((bx, by))          # the graphs hold raw pointers into these buffers
+                lb = self._step_eager(bx, by, bl)
+            bound[(bx.data_ptr(), by.data_ptr(), 0 if bl is None else bl.data_ptr(), tuple(bx.shape))] = (gb, lb)
+            self._bound_keepalive.append((bx, by, bl))      # the graphs hold raw pointers into these buffers
         with torch.no_grad():
             self.flat.data.copy_(snap["data"])
             self.flat.refresh_shadow()
@@ -228,12 +241,12 @@ class TrainEngine:
             if snap["step_dev"] is not None:
                 opt.step_dev.copy_(snap["step_dev"])
             opt.step_count = snap["step_count"]
-        self._graph, self._static, self._bound = g, (sx, sy, sloss), bound
+        self._graph, self._static, self._bound = g, (sx, sy, sl, sloss), bound
         return g
 
     @torch.no_grad()
-    def evaluate(self, x: torch.Tensor, y: torch.Tensor):
-        h = self.model.features(x)
+    def evaluate(self, x: torch.Tensor, y: torch.Tensor, lengths: Optional[torch.Tensor] = None):
+        h = self.model.features(x, lengths)
         logits = self.model.head(h)
         from .ops import reference as ref
         return ref.softmax_xent(logits, y), ref.accuracy(logits, y)

@@ -67,13 +67,14 @@ class SequenceClassifier(nn.Module):
                 # zero_grad() then has nothing to memset
                 self.flat.enable_direct_grads(self.rnn.averaged_parameters() + [self.head.weights, self.head.bias])
 
-    def features(self, x: torch.Tensor) -> torch.Tensor:
+    def features(self, x: torch.Tensor, lengths: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """``lengths``: optional int32 ``[B]`` per-sample sequence lengths (right-padded ``x``)."""
         self.rnn.reset_state(x.shape[0])
-        return self.rnn.fit_layers(x.to(self.compute_dtype) if x.is_floating_point() else x)
+        return self.rnn.fit_layers(x.to(self.compute_dtype) if x.is_floating_point() else x, lengths=lengths)
 
-    def forward(self, x: torch.Tensor, labels: torch.Tensor):
+    def forward(self, x: torch.Tensor, labels: torch.Tensor, lengths: Optional[torch.Tensor] = None):
         """-> (loss, logits, correct_count)"""
-        h = self.features(x)
+        h = self.features(x, lengths)
         logits, loss, correct = F.head_xent(h, self.head.weights, self.head.bias, labels)
         return loss, logits, correct
 

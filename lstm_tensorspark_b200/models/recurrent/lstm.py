@@ -157,12 +157,13 @@ class LSTMLayer(nn.Module):
         return out
 
     # ---- whole-sequence path (the thing the persistent kernel implements) ----------------------
-    def fit_sequence(self, x_seq: torch.Tensor) -> torch.Tensor:
-        """``x_seq [T,B,D]`` -> ``h_seq [T,B,H]``; final (ht, Ct) stored on the layer."""
+    def fit_sequence(self, x_seq: torch.Tensor, lengths: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """``x_seq [T,B,D]`` -> ``h_seq [T,B,H]``; final (ht, Ct) stored on the layer.  ``lengths`` (int32 ``[B]``, right
+        padding): the final state is each row's state after its own last step; padded positions of ``h_seq`` carry it."""
         B = x_seq.shape[1]
         if B != self.ht.shape[0]:
             self.reset_state(B)
-        h_seq, h_T, c_T = F.lstm_layer_sequence(x_seq, self.ht, self.Ct, self.w_x, self.w_h, self.bias)
+        h_seq, h_T, c_T = F.lstm_layer_sequence(x_seq, self.ht, self.Ct, self.w_x, self.w_h, self.bias, lengths=lengths)
         self._set_state(h_T, c_T)
         self.state.append((h_T, c_T))
         return h_seq

@@ -41,9 +41,10 @@ class RNN(nn.Module):
         for layer in self.layers:
             layer.reset_state(batch_size)
 
-    def fit_layers(self, input_data: torch.Tensor, train: bool = True) -> torch.Tensor:
-        """``[B,D]``: one step per layer (reference semantics, rnn.py:38-42).
-        ``[B,T,D]``: full unroll; returns the last layer's h at the last step, ``[B,H_last]``."""
+    def fit_layers(self, input_data: torch.Tensor, train: bool = True, lengths: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """``[B,D]``: one step per layer (reference semantics, rnn.py:38-42; ``lengths`` is ignored).
+        ``[B,T,D]``: full unroll; returns the last layer's h at the last step, ``[B,H_last]`` - with ``lengths`` (int32 ``[B]``,
+        right padding) at each row's own last step."""
         if input_data.dim() == 2:
             state = input_data
             for layer in self.layers:
@@ -51,14 +52,14 @@ class RNN(nn.Module):
             return state
         if input_data.dim() != 3:
             raise ValueError(f"expected [B,D] or [B,T,D], got {tuple(input_data.shape)}")
-        self._run_stack(input_data.transpose(0, 1))  # time-major [T,B,D]; the kernels index (t, b)
+        self._run_stack(input_data.transpose(0, 1), lengths)  # time-major [T,B,D]; the kernels index (t, b)
         return self.layers[-1].ht                   # = seq[-1], as a separate autograd edge (no [T,B,H] gradient for the top layer)
 
-    def fit_sequence_all(self, input_data: torch.Tensor) -> torch.Tensor:
-        """``[B,T,D]`` -> last layer's full ``h_seq [T,B,H]``."""
-        return self._run_stack(input_data.transpose(0, 1))
+    def fit_sequence_all(self, input_data: torch.Tensor, lengths: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """``[B,T,D]`` -> last layer's full ``h_seq [T,B,H]`` (padded positions hold the carried state)."""
+        return self._run_stack(input_data.transpose(0, 1), lengths)
 
-    def _run_stack(self, seq: torch.Tensor) -> torch.Tensor:
+    def _run_stack(self, seq: torch.Tensor, lengths: Optional[torch.Tensor] = None) -> torch.Tensor:
         """Layers bottom-up; adjacent pairs run as ONE layer-wavefront op where the GPU path supports it (both recurrences
         co-resident, the upper layer trailing by a couple of time steps), single layers otherwise."""
         from ...ops import functional as F
@@ -72,12 +73,12 @@ class RNN(nn.Module):
                     if B != l.ht.shape[0]:
                         l.reset_state(B)
                 seq, hT_a, cT_a, hT_b, cT_b = F.lstm_pair_sequence(seq, (la.ht, la.Ct, la.w_x, la.w_h, la.bias),
-                                                                     (lb.ht, lb.Ct, lb.w_x, lb.w_h, lb.bias))
+                                                                     (lb.ht, lb.Ct, lb.w_x, lb.w_h, lb.bias), lengths=lengths)
                 la._set_state(hT_a, cT_a); la.state.append((hT_a, cT_a))
                 lb._set_state(hT_b, cT_b); lb.state.append((hT_b, cT_b))
                 i += 2
             else:
-                seq = la.fit_sequence(seq)
+                seq = la.fit_sequence(seq, lengths)
                 i += 1
         return seq
 

@@ -284,9 +284,17 @@ def _gemm_tn(a: torch.Tensor, w: torch.Tensor) -> torch.Tensor:
 _CHUNKING = {"on": False}      # True while lstm_layer_sequence feeds batch chunks (weight gradients then accumulate over calls)
 
 
+def _check_lengths_arg(lengths: Optional[torch.Tensor], B: int, device) -> None:
+    """Shape / dtype / device of per-row lengths; the values are not read (that would synchronise with the device)."""
+    if lengths is not None and (lengths.dtype != torch.int32 or lengths.shape != (B,) or lengths.device != device
+                                or not lengths.is_contiguous()):
+        raise ValueError(f"lengths must be a contiguous int32 [{B}] tensor on {device}, got {lengths.dtype} "
+                         f"{tuple(lengths.shape)} on {lengths.device}")
+
+
 class _LSTMSeqFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x_seq, h0, c0, w_x, w_h, bias):
+    def forward(ctx, x_seq, h0, c0, w_x, w_h, bias, lengths=None):
         E = ext()
         T, B, D = x_seq.shape
         H = w_h.shape[1]
@@ -300,7 +308,8 @@ class _LSTMSeqFn(torch.autograd.Function):
         c0f = c0.detach().float().contiguous()
         h0c = h0.detach().to(cd).contiguous()
         if fast:
-            h_seq, c_seq, act = E.lstm_seq_fwd(gx, w_h_c, bias_f, h0c, c0f, _sync_ws(x_seq.device), _seq_variant(B, H, x_seq.device))
+            h_seq, c_seq, act = E.lstm_seq_fwd(gx, w_h_c, bias_f, h0c, c0f, _sync_ws(x_seq.device), _seq_variant(B, H, x_seq.device),
+                                               lengths=lengths)
             STATS["fast_fwd"] += 1
             STATS["kernels"] += 1
         else:
@@ -313,7 +322,7 @@ class _LSTMSeqFn(torch.autograd.Function):
             for t in range(T):
                 pre.copy_(gx[t])
                 G.matmul(h_seq[t], w_h_c, out=pre, accumulate=True)       # pre = gx[t] + h_{t-1} W_h^T
-                h, c, a = E.lstm_pointwise_fwd(pre, bias_f, c_seq[t])
+                h, c, a = E.lstm_pointwise_fwd(pre, bias_f, c_seq[t], h_seq[t], lengths, t)
                 h_seq[t + 1].copy_(h)
                 c_seq[t + 1].copy_(c)
                 act[t].copy_(a)
@@ -322,6 +331,7 @@ class _LSTMSeqFn(torch.autograd.Function):
         ctx.save_for_backward(x2d, h_seq, c_seq, act, w_x_c, w_h_c)
         ctx.set_materialize_grads(False)       # an unused output must arrive as None, not as a zero-filled [T,B,H] tensor
         ctx.fast = fast
+        ctx.lengths = lengths
         ctx.whole_batch = not _CHUNKING["on"]
         ctx.dims = (T, B, D, H)
         ctx.w_addrs = (w_x.data_ptr(), w_h.data_ptr(), bias.data_ptr())
@@ -346,7 +356,8 @@ class _LSTMSeqFn(torch.autograd.Function):
         if ctx.fast:
             w_hT = _transposed(w_h_c)
             _big_launch_begin()
-            dpre, dh0, dc0 = E.lstm_seq_bwd(dh_seq, w_hT, act, c_seq, dhT, dcT, _sync_ws(dev), _seq_variant(B, H, dev))
+            dpre, dh0, dc0 = E.lstm_seq_bwd(dh_seq, w_hT, act, c_seq, dhT, dcT, _sync_ws(dev), _seq_variant(B, H, dev),
+                                            lengths=ctx.lengths)
             STATS["fast_bwd"] += 1
             STATS["kernels"] += 1
             _after_big_launch()                  # finished gradient buckets of the layers above: sync them under this recurrence
@@ -355,9 +366,14 @@ class _LSTMSeqFn(torch.autograd.Function):
             dh_rec: Optional[torch.Tensor] = dhT if dh_T is not None else None
             dc = dcT
             for t in range(T - 1, -1, -1):
-                dp, dc = E.lstm_pointwise_bwd(dh_seq[t], dh_rec, dc, act[t], c_seq[t], c_seq[t + 1])
+                if ctx.lengths is None:
+                    dp, dc = E.lstm_pointwise_bwd(dh_seq[t], dh_rec, dc, act[t], c_seq[t], c_seq[t + 1])
+                    dh_rec = _mm_f32(dp, w_h_c)
+                else:                            # padded rows hand their dh on directly (dh_pass), the others through W_h
+                    dp, dc, dh_pass = E.lstm_pointwise_bwd(dh_seq[t], dh_rec, dc, act[t], c_seq[t], c_seq[t + 1], ctx.lengths, t)
+                    G.matmul(dp, w_h_c.t(), out=dh_pass, accumulate=True)
+                    dh_rec = dh_pass
                 dpre[t].copy_(dp)
-                dh_rec = _mm_f32(dp, w_h_c)
             dh0, dc0 = dh_rec, dc
             STATS["generic_bwd"] += 1
             STATS["kernels"] += T
@@ -371,31 +387,34 @@ class _LSTMSeqFn(torch.autograd.Function):
             dx = G.matmul(dg2d, w_x_c.t(), out_dtype=cd).view(T, B, D)        # dG · W_x: W_x read in place as an MN-major operand
             STATS["kernels"] += 1
         h0_dt, c0_dt = ctx.in_dtypes
-        return dx, dh0.to(h0_dt), dc0.to(c0_dt), dw_x, dw_h, db
+        return dx, dh0.to(h0_dt), dc0.to(c0_dt), dw_x, dw_h, db, None
 
 
-def lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias):
-    """``x_seq [T,B,D]`` (bf16 or fp32) -> ``(h_seq [T,B,H], h_T, c_T)``."""
+def lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths=None):
+    """``x_seq [T,B,D]`` (bf16 or fp32) -> ``(h_seq [T,B,H], h_T, c_T)``.  ``lengths``: optional int32 ``[B]`` on the batch's
+    device, right padding (``ops/reference.py``); the persistent kernels then run their masked instantiations."""
     if (not x_seq.is_contiguous() and not x_seq.requires_grad and x_seq.transpose(0, 1).is_contiguous()
             and (x_seq.shape[2] * x_seq.element_size()) % 16 == 0):
         x_seq = ext().transpose01(x_seq.transpose(0, 1))     # batch-major feed -> time-major, a row permutation at copy speed
         STATS["kernels"] += 1
     T, B, _ = x_seq.shape
     H = w_h.shape[1]
+    _check_lengths_arg(lengths, B, x_seq.device)
     chunk = _batch_chunk(B, H, x_seq.dtype, x_seq.device)
     if chunk is not None:
         # more batch tiles than the persistent kernels can keep co-resident: the sequences are independent, so run the fast
         # path per batch chunk (weight-gradient contributions accumulate across chunks) instead of the per-step generic path
         _CHUNKING["on"] = True
         try:
-            outs = [_LSTMSeqFn.apply(x_seq[:, b0:b0 + chunk].contiguous(), h0[b0:b0 + chunk], c0[b0:b0 + chunk], w_x, w_h, bias)
+            outs = [_LSTMSeqFn.apply(x_seq[:, b0:b0 + chunk].contiguous(), h0[b0:b0 + chunk], c0[b0:b0 + chunk], w_x, w_h, bias,
+                                     None if lengths is None else lengths[b0:b0 + chunk])
                     for b0 in range(0, B, chunk)]
         finally:
             _CHUNKING["on"] = False
         STATS["batch_chunks"] = STATS.get("batch_chunks", 0) + len(outs)
         return (torch.cat([o[0] for o in outs], dim=1), torch.cat([o[1] for o in outs], dim=0),
                 torch.cat([o[2] for o in outs], dim=0))
-    return _LSTMSeqFn.apply(x_seq.contiguous(), h0, c0, w_x, w_h, bias)
+    return _LSTMSeqFn.apply(x_seq.contiguous(), h0, c0, w_x, w_h, bias, lengths)
 
 
 # =====================================================================================================================
@@ -486,7 +505,7 @@ def _gate_cfg(var: int, tiles_m: int, nkb: int, per_kb_step: int, ctas_per_tile:
 
 class _LSTMPairFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x_seq, h0a, c0a, w_xa, w_ha, b_a, h0b, c0b, w_xb, w_hb, b_b):
+    def forward(ctx, x_seq, h0a, c0a, w_xa, w_ha, b_a, h0b, c0b, w_xb, w_hb, b_b, lengths=None):
         E = ext()
         dev = x_seq.device
         T, B, D = x_seq.shape
@@ -522,8 +541,8 @@ class _LSTMPairFn(torch.autograd.Function):
         # Everything the later kernels need up front (prologues, zeroed counters) is enqueued before the chain head.
         E.lstm_seq_prologue(h0a_c, c0a_f, h_seq_a, c_seq_a, til_a, ws_a)
         E.lstm_seq_prologue(h0b_c, c0b_f, h_seq_b, c_seq_b, til_b, ws_b)
-        E.lstm_seq_fwd_into(gx_a, wha, ba_f, h0a_c, c0a_f, h_seq_a, c_seq_a, act_a, til_a, ws_a, var, None, 0, True, 0, 1)
-        E.lstm_seq_fwd_into(gx_b, whb, bb_f, h0b_c, c0b_f, h_seq_b, c_seq_b, act_b, til_b, ws_b, var, done, tn, False, 0, 3)
+        E.lstm_seq_fwd_into(gx_a, wha, ba_f, h0a_c, c0a_f, h_seq_a, c_seq_a, act_a, til_a, ws_a, var, None, 0, True, 0, 1, lengths)
+        E.lstm_seq_fwd_into(gx_b, whb, bb_f, h0b_c, c0b_f, h_seq_b, c_seq_b, act_b, til_b, ws_b, var, done, tn, False, 0, 3, lengths)
         # single-CTA tiles: the recurrences' CTAs are spread one per TPC, the SMs they leave free rarely form CTA pairs
         free_ctas = max(1, _sms(dev) - Ha // 16 - Hb // 16)
         E.gemm2(h_seq_a[1:].view(T * B, Ha), wxb, out=gx_b.view(T * B, 4 * Hb), ctas=1, bn=256, max_ctas=free_ctas,
@@ -535,6 +554,7 @@ class _LSTMPairFn(torch.autograd.Function):
         ctx.save_for_backward(x2d, h_seq_a, c_seq_a, act_a, h_seq_b, c_seq_b, act_b, wxa, wha, wxb, whb)
         ctx.set_materialize_grads(False)
         ctx.dims = (T, B, D, Ha, Hb)
+        ctx.lengths = lengths
         ctx.x_folded = x_bm is not None
         ctx.addrs = (w_xa.data_ptr(), w_ha.data_ptr(), b_a.data_ptr(), w_xb.data_ptr(), w_hb.data_ptr(), b_b.data_ptr())
         ctx.in_dtypes = (h0a.dtype, c0a.dtype, h0b.dtype, c0b.dtype)
@@ -560,8 +580,8 @@ class _LSTMPairFn(torch.autograd.Function):
         ws_a[:SYNC_WORDS - 1].zero_(); ws_b[:SYNC_WORDS - 1].zero_(); done.zero_()
         var = _wave_variant()
         # programmatic-dependent-launch chain on one stream (see forward): L_b -> L_a -> gated dX GEMM
-        E.lstm_seq_bwd_into(dh_seq_b, whT_b, act_b, c_seq_b, dpre_b, dh0b, dc0b, til_b, ws_b, var, None, 0, True, 0, 1)
-        E.lstm_seq_bwd_into(dx_b, whT_a, act_a, c_seq_a, dpre_a, dh0a, dc0a, til_a, ws_a, var, done, tn, False, 0, 3)
+        E.lstm_seq_bwd_into(dh_seq_b, whT_b, act_b, c_seq_b, dpre_b, dh0b, dc0b, til_b, ws_b, var, None, 0, True, 0, 1, ctx.lengths)
+        E.lstm_seq_bwd_into(dx_b, whT_a, act_a, c_seq_a, dpre_a, dh0a, dc0a, til_a, ws_a, var, done, tn, False, 0, 3, ctx.lengths)
         free_ctas = max(1, _sms(dev) - Ha // 16 - Hb // 16)
         E.gemm2(dpre_b.view(T * B, 4 * Hb), wxb, out=dx_b.view(T * B, Ha), b_mn=True, ctas=1, bn=256, max_ctas=free_ctas,
                 gate=ws_b[_gate_off(var):], gate_cfg=_gate_cfg(var, 2, 4 * Hb // 64, 1, 4 * Hb // 64, T + 1, -1, B, True), done=done,
@@ -587,15 +607,17 @@ class _LSTMPairFn(torch.autograd.Function):
             dx = G.matmul(dg_a, wxa.t(), out_dtype=cd).view(T, B, D)
             STATS["kernels"] += 1
         t = ctx.in_dtypes
-        return dx, dh0a.to(t[0]), dc0a.to(t[1]), dw_xa, dw_ha, db_a, dh0b.to(t[2]), dc0b.to(t[3]), dw_xb, dw_hb, db_b
+        return dx, dh0a.to(t[0]), dc0a.to(t[1]), dw_xa, dw_ha, db_a, dh0b.to(t[2]), dc0b.to(t[3]), dw_xb, dw_hb, db_b, None
 
 
-def lstm_pair_sequence(x_seq, la, lb):
-    """Two stacked layers as one wavefront op.  ``la`` / ``lb`` = (h0, c0, w_x, w_h, bias).  -> (h_seq_b, hT_a, cT_a, hT_b, cT_b)."""
+def lstm_pair_sequence(x_seq, la, lb, lengths=None):
+    """Two stacked layers as one wavefront op.  ``la`` / ``lb`` = (h0, c0, w_x, w_h, bias).  -> (h_seq_b, hT_a, cT_a, hT_b, cT_b).
+    ``lengths``: optional int32 ``[B]`` per-row lengths (both layers run their masked kernels; the gated GEMM is unchanged)."""
+    _check_lengths_arg(lengths, x_seq.shape[1], x_seq.device)
     if (not x_seq.is_contiguous() and not x_seq.requires_grad and x_seq.transpose(0, 1).is_contiguous()
             and (x_seq.shape[2] * x_seq.element_size()) % 16 == 0):
         if FOLDED_FEED and G.folded_ok(x_seq.transpose(0, 1)):
-            return _LSTMPairFn.apply(x_seq, *la, *lb)                     # read in place (see forward)
+            return _LSTMPairFn.apply(x_seq, *la, *lb, lengths)            # read in place (see forward)
         x_seq = ext().transpose01(x_seq.transpose(0, 1))
         STATS["kernels"] += 1
-    return _LSTMPairFn.apply(x_seq.contiguous(), *la, *lb)
+    return _LSTMPairFn.apply(x_seq.contiguous(), *la, *lb, lengths)

@@ -42,11 +42,12 @@ def lstm_cell_step(x, h, c, w_x, w_h, bias):
     return ref.lstm_cell_step(x, h, c, w_x, w_h, bias)
 
 
-def lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias):
+def lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths=None):
+    """``lengths``: optional int32 ``[B]`` per-row sequence lengths (right padding, see ``reference.lstm_layer_sequence``)."""
     if _use_ext(x_seq):
         from . import cuda_lstm
-        return cuda_lstm.lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias)
-    return ref.lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias)
+        return cuda_lstm.lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths=lengths)
+    return ref.lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths=lengths)
 
 
 def head_xent(h, weights, bias, labels):
@@ -65,6 +66,6 @@ def lstm_pair_supported(x_seq, h_a: int, h_b: int) -> bool:
     return cuda_lstm.wavefront_supported(x_seq, h_a, h_b)
 
 
-def lstm_pair_sequence(x_seq, la, lb):
+def lstm_pair_sequence(x_seq, la, lb, lengths=None):
     from . import cuda_lstm
-    return cuda_lstm.lstm_pair_sequence(x_seq, la, lb)
+    return cuda_lstm.lstm_pair_sequence(x_seq, la, lb, lengths=lengths)

@@ -40,9 +40,26 @@ def lstm_cell_step(x, h, c, w_x, w_h, bias):
     return h_new, c_new
 
 
-def lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias):
-    """Unrolled layer: ``x_seq [T,B,D]`` -> ``(h_seq [T,B,H], h_T, c_T)``."""
+def check_lengths(lengths: torch.Tensor, B: int, T: int) -> None:
+    """Per-row sequence lengths: int32 ``[B]`` with ``1 <= lengths[b] <= T`` (costs a device-to-host read on a GPU tensor)."""
+    if lengths.dtype != torch.int32 or lengths.dim() != 1 or lengths.shape[0] != B:
+        raise ValueError(f"lengths must be int32 [{B}], got {lengths.dtype} {tuple(lengths.shape)}")
+    lo, hi = int(lengths.min()), int(lengths.max())
+    if lo < 1 or hi > T:
+        raise ValueError(f"lengths must lie in [1, {T}], got [{lo}, {hi}]")
+
+
+def lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths: Optional[torch.Tensor] = None):
+    """Unrolled layer: ``x_seq [T,B,D]`` -> ``(h_seq [T,B,H], h_T, c_T)``.
+
+    ``lengths`` (int32 ``[B]``, right padding): at a step ``t >= lengths[b]`` row ``b`` holds its state (``h_t = h_{t-1}``,
+    ``c_t = c_{t-1}``), so ``h_T`` / ``c_T`` are the state after the row's last real step - ``h_n`` / ``c_n`` of ``nn.LSTM`` on
+    a packed sequence - and padded inputs get no gradient."""
     T = x_seq.shape[0]
+    keep = None
+    if lengths is not None:
+        check_lengths(lengths, x_seq.shape[1], T)
+        keep = lengths.to(x_seq.device).long().view(-1, 1) > torch.arange(T, device=x_seq.device).view(1, -1)   # [B,T]
     h, c = h0, c0
     outs = []
     # hoisted input projection (same arithmetic as per-step x·W_x)
@@ -50,8 +67,13 @@ def lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias):
     for t in range(T):
         pre = gx[t] + h @ w_h.t() + bias
         i, f, g, o = lstm_gates(pre)
-        c = f * c + i * g
-        h = o * torch.tanh(c)
+        c_new = f * c + i * g
+        h_new = o * torch.tanh(c_new)
+        if keep is None:
+            c, h = c_new, h_new
+        else:
+            k = keep[:, t:t + 1]
+            c, h = torch.where(k, c_new, c), torch.where(k, h_new, h)
         outs.append(h)
     return torch.stack(outs, 0), h, c
 

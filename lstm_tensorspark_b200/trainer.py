@@ -104,8 +104,12 @@ def train_rnn(partition, cfg: Config, rank: int = 0, world_size: int = 1, comm: 
     dtype = resolve_dtype(cfg, device)
     F.set_backend(cfg.backend if cfg.backend != "auto" else "auto")
 
+    train_lengths = None
     if isinstance(rows, tuple):
-        train_x, train_y = rows
+        train_x, train_y = rows[0], rows[1]
+        train_lengths = rows[2] if len(rows) > 2 else None
+    elif cfg.variable_length:
+        train_x, train_y, train_lengths = D.process_batch_ragged(rows, cfg.seq_len, cfg.in_features, normalize=cfg.normalize)
     else:
         train_x, train_y = D.process_batch(rows, normalize=cfg.normalize, seq_len=cfg.seq_len,
                                            in_features=cfg.in_features)
@@ -129,10 +133,10 @@ def train_rnn(partition, cfg: Config, rank: int = 0, world_size: int = 1, comm: 
     if cfg.data_residency == "host":
         # the reference's feed (src/rnn.py:264-267: every batch travels host -> device), as an asynchronous DMA pipeline
         loader = D.PinnedHostLoader(train_x, train_y, batch_size, device, dtype=torch.float32, shuffle=True,
-                                    seed=cfg.seed + 17 * (rank + 1), depth=3)
+                                    seed=cfg.seed + 17 * (rank + 1), depth=3, lengths=train_lengths)
     else:
         loader = D.DeviceShard(train_x, train_y, batch_size, device, dtype=torch.float32, shuffle=True,
-                               seed=cfg.seed + 17 * (rank + 1))
+                               seed=cfg.seed + 17 * (rank + 1), lengths=train_lengths)
     start_step = 0
     if cfg.resume or cfg.use_pretrained_model:
         src = cfg.resume or ckpt.find_latest_run(cfg.checkpoint_path, None if standalone else str(partition_key))
@@ -193,13 +197,16 @@ def train_rnn(partition, cfg: Config, rank: int = 0, world_size: int = 1, comm: 
             os._exit(17)
         # with a captured step the batch is gathered straight into the graph's input buffers (no second copy)
         gi = eng.graph_inputs() if isinstance(loader, D.DeviceShard) else None
-        train_input, train_labels = loader.next(out=gi) if gi is not None else loader.next()
+        batch = loader.next(out=gi) if gi is not None else loader.next()
+        train_input, train_labels = batch[0], batch[1]
+        batch_lengths = batch[2] if len(batch) > 2 else None      # variable-length samples: int32 [B]
 
         with M.nvtx_range("step", cfg.nvtx):
             if cfg.cuda_graph and device.type == "cuda" and eng._graph is None and step == start_step + 3:
                 # static shapes: replay the captured step from here on (host feed: one graph per staging slot, no extra copy)
-                eng.capture(train_input, train_labels, bind=list(loader.dev) if isinstance(loader, D.PinnedHostLoader) else ())
-            loss = eng.step(train_input, train_labels)
+                eng.capture(train_input, train_labels, bind=list(loader.dev) if isinstance(loader, D.PinnedHostLoader) else (),
+                            lengths=batch_lengths)
+            loss = eng.step(train_input, train_labels, batch_lengths)
         samples += batch_size
 
         with M.nvtx_range("param_avg", cfg.nvtx):
@@ -221,7 +228,7 @@ def train_rnn(partition, cfg: Config, rank: int = 0, world_size: int = 1, comm: 
                                   "loss": t_loss, "config": cfg.__dict__},
                            opt_state={"optimizer": comm.optimizer_state(optimizer), "loader": loader.state_dict()})
                 with torch.no_grad(), M.capture(sink):
-                    h = model.features(train_input)      # same batch, from the initial state (src/rnn.py:276-279)
+                    h = model.features(train_input, batch_lengths)   # same batch, from the initial state (src/rnn.py:276-279)
                     logits = model.head(h)
                     e_loss = compute_loss(labels=train_labels, logits=logits)
                     e_acc = compute_accuracy(labels=train_labels, logits=logits)
@@ -334,8 +341,8 @@ def load_shards(cfg: Config, world_size: int, standalone: bool):
         n_per = cfg.synthetic // world_size
         shards = []
         for r in range(world_size):
-            x, y = D.synthetic_sequences(n_per, cfg.seq_len, cfg.in_features, cfg.num_classes, seed=cfg.seed + r)
-            shards.append((r, (x, y)))
+            shards.append((r, D.synthetic_sequences(n_per, cfg.seq_len, cfg.in_features, cfg.num_classes, seed=cfg.seed + r,
+                                                    variable_length=cfg.variable_length)))
         return shards
     if standalone:
         return [(0, D.read_dataset_from_path(cfg.training_path))]
@@ -370,8 +377,15 @@ def evaluate_job(cfg: Config, standalone: bool = False) -> Dict:
     only ``train`` and the averaged model is thrown away, src/rnn.py:371,407-408); it closes the train -> average -> use loop."""
     from .engine import TrainEngine
     variables, src = _find_trained_model(cfg, standalone)
+    lengths = None
     if cfg.synthetic:
-        x, y = D.synthetic_sequences(cfg.synthetic, cfg.seq_len, cfg.in_features, cfg.num_classes, seed=cfg.seed)
+        data = D.synthetic_sequences(cfg.synthetic, cfg.seq_len, cfg.in_features, cfg.num_classes, seed=cfg.seed,
+                                     variable_length=cfg.variable_length)
+        x, y = data[0], data[1]
+        lengths = data[2] if cfg.variable_length else None
+    elif cfg.variable_length:
+        x, y, lengths = D.process_batch_ragged(D.read_dataset_from_path(cfg.training_path), cfg.seq_len, cfg.in_features,
+                                               normalize=cfg.normalize)
     else:
         rows = D.read_dataset_from_path(cfg.training_path)
         x, y = D.process_batch(rows, normalize=cfg.normalize, seq_len=cfg.seq_len, in_features=cfg.in_features)
@@ -393,15 +407,17 @@ def evaluate_job(cfg: Config, standalone: bool = False) -> Dict:
     eng.flat.refresh_shadow()
     xs = torch.as_tensor(x).to(device=device, dtype=torch.float32)
     ys = torch.as_tensor(y).to(device)
+    ls = None if lengths is None else torch.as_tensor(lengths).to(device=device, dtype=torch.int32)
+    sl = lambda a, b: None if ls is None else ls[a:b]
     loss_sum, correct, seen = 0.0, 0.0, 0
     start = time.time()
     for lo in range(0, n - bs + 1, bs):                 # full batches (static shapes for the kernels); the tail is scored below
-        l, a = eng.evaluate(xs[lo:lo + bs], ys[lo:lo + bs])
+        l, a = eng.evaluate(xs[lo:lo + bs], ys[lo:lo + bs], sl(lo, lo + bs))
         loss_sum += float(l) * bs; correct += float(a) * bs; seen += bs
     if seen < n:                                        # remainder: the last `bs` rows, counting only the ones not seen yet
         from .ops import reference as ref
         with torch.no_grad():
-            logits = eng.model.head(eng.model.features(xs[n - bs:]))[bs - (n - seen):]
+            logits = eng.model.head(eng.model.features(xs[n - bs:], sl(n - bs, n)))[bs - (n - seen):]
         tail_y = ys[seen:]
         loss_sum += float(ref.softmax_xent(logits.float(), tail_y)) * (n - seen)
         correct += float(ref.accuracy(logits.float(), tail_y)) * (n - seen)
