@@ -27,21 +27,24 @@ import torch.nn.functional as F
 
 
 class CudnnLSTMClassifier(nn.Module):
-    def __init__(self, hidden, in_features, num_classes, time_major=False):
+    def __init__(self, hidden, in_features, num_classes, time_major=False, bidirectional=False):
         super().__init__()
         assert len(set(hidden)) == 1, "nn.LSTM stacks equal-width layers"
         self.time_major = time_major
-        self.lstm = nn.LSTM(in_features, hidden[0], num_layers=len(hidden), batch_first=not time_major)
-        self.head = nn.Linear(hidden[-1], num_classes)
+        self.bidirectional = bidirectional
+        self.lstm = nn.LSTM(in_features, hidden[0], num_layers=len(hidden), batch_first=not time_major, bidirectional=bidirectional)
+        self.head = nn.Linear(hidden[-1] * (2 if bidirectional else 1), num_classes)
 
     def forward(self, x):
-        out, _ = self.lstm(x)
+        out, (h_n, _) = self.lstm(x)
+        if self.bidirectional:                          # [forward final | reverse final (after time 0)], as the framework's model
+            return self.head(torch.cat([h_n[-2], h_n[-1]], 1))
         return self.head(out[-1] if self.time_major else out[:, -1, :])
 
 
 class BaselineRunner:
     def __init__(self, hidden, in_features, num_classes, batch, seq_len, rank, world, device, optimizer="adam", lr=1e-3,
-                 variant="stock"):
+                 variant="stock", bidirectional=False):
         self.rank, self.world, self.device = rank, world, device
         self.B, self.T, self.D, self.C = batch, seq_len, in_features, num_classes
         self.variant = variant
@@ -52,7 +55,7 @@ class BaselineRunner:
         torch.manual_seed(0)
         if world > 1 and not dist.is_initialized():
             dist.init_process_group("nccl", rank=rank, world_size=world, device_id=device)
-        model = CudnnLSTMClassifier(hidden, in_features, num_classes, time_major=self.tuned).to(device)
+        model = CudnnLSTMClassifier(hidden, in_features, num_classes, time_major=self.tuned, bidirectional=bidirectional).to(device)
         if self.tuned:
             model = model.to(torch.bfloat16)
             model.lstm.flatten_parameters()

@@ -50,20 +50,22 @@ def _card():
 
 
 def ours(args, xs, ys, ls, dev):
+    """``ls`` None: fixed-length batches.  ``args.bidirectional`` (absent = False): bench/bidirectional.py."""
     from lstm_tensorspark_b200.config import Config
     from lstm_tensorspark_b200.engine import TrainEngine
     from lstm_tensorspark_b200.ops import cuda_lstm
     B, T, D, C, nb = args.batch_size, args.seq_len, args.in_features, args.num_classes, 4
     cfg = Config(hidden_units=args.hidden_units, in_features=D, seq_len=T, batch_size=B, num_classes=C, partitions=1,
                  sync_mode="none", init="scaled", learn_initial_state=False, dtype="bf16", device="cuda", learning_rate=1e-3,
-                 quiet=True, variable_length=True)
+                 quiet=True, variable_length=ls is not None, bidirectional=getattr(args, "bidirectional", False))
     eng = TrainEngine(cfg, 0, 1, None, batch_size=B, device=dev, dtype=torch.bfloat16)
     dx = torch.as_tensor(xs).to(dev, torch.bfloat16)
-    dy, dl = torch.as_tensor(ys).to(dev), torch.as_tensor(ls).to(dev)
-    batches = [(dx[i * B:(i + 1) * B], dy[i * B:(i + 1) * B], dl[i * B:(i + 1) * B]) for i in range(nb)]
+    dy = torch.as_tensor(ys).to(dev)
+    dl = None if ls is None else torch.as_tensor(ls).to(dev)
+    batches = [(dx[i * B:(i + 1) * B], dy[i * B:(i + 1) * B], None if dl is None else dl[i * B:(i + 1) * B]) for i in range(nb)]
     eng.step(*batches[0])
     if args.cuda_graph:
-        eng.capture(*batches[0][:2], lengths=batches[0][2], bind=batches[1:])
+        eng.capture(*batches[0][:2], lengths=batches[0][2], bind=batches[1:] if dl is not None else [b[:2] for b in batches[1:]])
     it = {"i": 0}
 
     def step():
@@ -72,7 +74,8 @@ def ours(args, xs, ys, ls, dev):
     ms = _timed(step, args.steps, args.warmup)
     cuda_lstm.check_kernel_errors(dev)
     return {"ms_per_step": ms, "value": B * 1e3 / ms, "cuda_graph": bool(args.cuda_graph),
-            "fast_path": cuda_lstm.STATS["fast_fwd"] > 0, "generic_path": cuda_lstm.STATS["generic_fwd"] > 0}
+            "fast_path": cuda_lstm.STATS["fast_fwd"] > 0, "generic_path": cuda_lstm.STATS["generic_fwd"] > 0,
+            "wavefront": cuda_lstm.STATS.get("wavefront_fwd", 0) > 0}
 
 
 def packed_cudnn(args, xs, ys, ls, dev):
@@ -81,10 +84,12 @@ def packed_cudnn(args, xs, ys, ls, dev):
     from torch.nn.utils.rnn import pack_padded_sequence
     B, T, D, C, nb = args.batch_size, args.seq_len, args.in_features, args.num_classes, 4
     hidden = [int(h) for h in args.hidden_units.split(",")]
+    bidir = getattr(args, "bidirectional", False)
     torch.manual_seed(0)
-    lstm = nn.LSTM(D, hidden[0], num_layers=len(hidden), device=dev, dtype=torch.bfloat16)    # weights in one cuDNN buffer
+    lstm = nn.LSTM(D, hidden[0], num_layers=len(hidden), device=dev, dtype=torch.bfloat16,     # weights in one cuDNN buffer
+                   bidirectional=bidir)
     lstm.flatten_parameters()
-    head = nn.Linear(hidden[-1], C, device=dev, dtype=torch.bfloat16)
+    head = nn.Linear(hidden[-1] * (2 if bidir else 1), C, device=dev, dtype=torch.bfloat16)
     params = list(lstm.parameters()) + list(head.parameters())
     masters = [p.detach().float().clone().requires_grad_(True) for p in params]
     for m in masters:
@@ -101,7 +106,8 @@ def packed_cudnn(args, xs, ys, ls, dev):
         for p in params:
             p.grad = None
         _, (h_n, _) = lstm(pack_padded_sequence(dx[:, i * B:(i + 1) * B], lens[i], enforce_sorted=False))
-        loss = Fn.cross_entropy(head(h_n[-1]).float(), dy[i * B:(i + 1) * B])
+        feat = torch.cat([h_n[-2], h_n[-1]], 1) if bidir else h_n[-1]
+        loss = Fn.cross_entropy(head(feat).float(), dy[i * B:(i + 1) * B])
         loss.backward()
         with torch.no_grad():
             torch._foreach_copy_([m.grad for m in masters], [p.grad for p in params])       # bf16 grads -> fp32 masters

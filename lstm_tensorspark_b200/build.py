@@ -143,13 +143,13 @@ def dump_sass(out_dir: str) -> List[str]:
     return outs
 
 
-# lstm_seq_wgmma.cu has ~60 template instantiations (ring depths, tuning variants, each with and without per-row lengths): the
-# listing keeps the unmasked forward and backward kernels with one and two batch tiles per CTA at the ring depths H = 1024 gets,
-# the streamed-weights kernels and the prologue.
+# lstm_seq_wgmma.cu has ~120 template instantiations (ring depths, tuning variants, each with and without per-row lengths, in both
+# time directions): the listing keeps the unmasked forward-time forward and backward kernels with one and two batch tiles per CTA
+# at the ring depths H = 1024 gets, the streamed-weights kernels and the prologue.
 # gemm2_wgmma.cu has 48 (cluster size x tile x operand majors x output mode); kept: the default 2-CTA 256-wide kernels of the
 # x-projection (TN, bf16 out), dX (B MN-major, bf16 out) and the weight gradients (both MN-major, fp32 accumulate).
-SASS_KEEP = {"lstm_seq_wgmma.cu": ("ILb0ELi4ELi1ELb0ELb0ELb0E", "ILb0ELi4ELi2ELb0ELb0ELb0E", "ILb1ELi3ELi1ELb0ELb0ELb0E",
-                                  "ILb1ELi2ELi2ELb0ELb0ELb0E", "ILb0ELi8ELi1ELb1ELb0ELb0E", "ILb1ELi8ELi1ELb1ELb0ELb0E",
+SASS_KEEP = {"lstm_seq_wgmma.cu": ("ILb0ELi4ELi1ELb0ELb0ELb0ELb0E", "ILb0ELi4ELi2ELb0ELb0ELb0ELb0E", "ILb1ELi3ELi1ELb0ELb0ELb0ELb0E",
+                                  "ILb1ELi2ELi2ELb0ELb0ELb0ELb0E", "ILb0ELi8ELi1ELb1ELb0ELb0ELb0E", "ILb1ELi8ELi1ELb1ELb0ELb0ELb0E",
                                   "seq_prologue_kernel"),
              "gemm2_wgmma.cu": ("ILi2ELi256ELb0ELb0ELi0E", "ILi2ELi256ELb0ELb1ELi0E", "ILi2ELi256ELb1ELb1ELi2E")}
 

@@ -41,6 +41,8 @@ class Config:
     variable_length: bool = False       # samples of 1..seq_len steps: a CSV row is k*in_features values + label (zero-padded to
                                         # seq_len); --synthetic draws lengths in [seq_len//4, seq_len].  The final state is each
                                         # sample's state after its own last step (padded steps hold the state)
+    bidirectional: bool = False         # every layer also runs a reverse-time LSTM; layer l+1 and the classifier read
+                                        # [forward | reverse] (2 H wide), as nn.LSTM(bidirectional=True) on a packed sequence
     dtype: str = "auto"                 # auto: bf16 on cuda, fp32 on cpu
     device: str = "auto"                # auto | cpu | cuda
     backend: str = "auto"               # auto | cuda_ext (hand-written sm_90a kernels) | torch
@@ -97,7 +99,7 @@ class Config:
         for i, h in enumerate(hidden):
             settings.append({
                 "layer_name": f"LSTMLayer{i}",
-                "dim_size": self.in_features if i == 0 else hidden[i - 1],
+                "dim_size": self.in_features if i == 0 else (2 if self.bidirectional else 1) * hidden[i - 1],
                 "num_hidden": h,
                 "batch_size": bs,
                 "normalize": True,      # present in the reference dict, never read there either
@@ -119,6 +121,8 @@ class Config:
             raise ValueError("--seq_len must be >= 1")
         if self.variable_length and self.seq_len < 2:
             raise ValueError("--variable_length needs --seq_len >= 2 (the longest sample's number of steps)")
+        if self.bidirectional and self.seq_len < 2:
+            raise ValueError("--bidirectional needs --seq_len >= 2 (the reverse direction runs over a whole sequence)")
         if self.sync_mode not in ("param_avg", "grad_allreduce", "none"):
             raise ValueError(f"unknown --sync_mode {self.sync_mode}")
         if self.optimizer not in ("adam", "sgd"):

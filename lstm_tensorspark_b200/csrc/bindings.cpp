@@ -44,9 +44,9 @@ int ts_gemm_generic(const void*, const void*, void*, const float*, int, int, int
 int ts_gemm2(const void*, const void*, void*, const float*, int, int, int, int, int, int, int, int, int, int, int, int, int,
              const unsigned int*, const int*, unsigned int*, int*, int, int, int, int, cudaStream_t);
 int ts_lstm_seq_fwd(const void*, const void*, const float*, const void*, const float*, void*, const float*, void*, void*, int,
-                    int, int, unsigned int*, int, cudaStream_t, const void*, const unsigned int*, int, int, int, const int*);
+                    int, int, unsigned int*, int, cudaStream_t, const void*, const unsigned int*, int, int, int, const int*, int);
 int ts_lstm_seq_bwd(const void*, const void*, const void*, const float*, const void*, float*, float*, void*, void*, int,
-                    int, int, unsigned int*, int, cudaStream_t, const unsigned int*, int, int, int, const int*);
+                    int, int, unsigned int*, int, cudaStream_t, const unsigned int*, int, int, int, const int*, int);
 int ts_lstm_seq_prologue(const void*, const float*, void*, float*, void*, unsigned int*, int, int, cudaStream_t);
 const char* ts_last_error();
 }
@@ -82,6 +82,12 @@ const int* lengths_ptr(const std::optional<Tensor>& lengths, int64_t B, const Te
   TORCH_CHECK(l.dim() == 1 && l.size(0) == B, "lengths must be [B] (B = ", B, ")");
   TORCH_CHECK(l.is_contiguous(), "lengths must be contiguous");
   return l.data_ptr<int>();
+}
+// Direction of a persistent-kernel launch: reverse = the reverse-time half of a bidirectional layer (h_seq / c_seq row T holds
+// the initial state).  The layer wavefront's dataflow gating (in_gate / extra_signal) is forward-only.
+int direction_flag(bool reverse, const std::optional<Tensor>& in_gate, bool extra_signal) {
+  TORCH_CHECK(!reverse || (!in_gate.has_value() && !extra_signal), "reverse: the layer wavefront (in_gate / extra_signal) is forward-only");
+  return reverse ? 1 : 0;
 }
 
 // x [B,T,D] contiguous -> [T,B,D] contiguous (row permutation at copy speed)
@@ -353,16 +359,18 @@ Tensor gemm_generic(const Tensor& A, const Tensor& B, const std::optional<Tensor
 // ---- persistent wgmma LSTM sequence kernels ------------------------------------------------------------------
 // gx [T,B,4H] bf16 (x·Wx^T, no bias), w_h [4H,H] bf16, bias fp32 [4H], h0 bf16 [B,H], c0 fp32 [B,H]
 // -> h_seq [T+1,B,H] bf16 (row 0 = h0), c_seq [T+1,B,H] fp32, act [T,B,4H] bf16
+// reverse: time runs from T-1 down to 0; h_seq / c_seq row t = the state after time t, row T = h0 / c0.
 // in_gate (wavefront): completion counters of the GEMM that is still producing gx while this kernel runs (see SeqParams);
 // extra_signal: one more arrival after the last step, for a gated GEMM that consumes h_seq.
 std::vector<Tensor> lstm_seq_fwd(const Tensor& gx, const Tensor& w_h, const Tensor& bias, const Tensor& h0,
                                  const Tensor& c0, Tensor sync_ws, int64_t variant, std::optional<Tensor> dbg,
                                  std::optional<Tensor> in_gate, int64_t in_gate_tiles_n, bool extra_signal,
-                                 const std::optional<Tensor>& lengths) {
+                                 const std::optional<Tensor>& lengths, bool reverse) {
   chk_cuda(gx, "gx"); chk_cuda(w_h, "w_h"); chk_cuda(bias, "bias"); chk_cuda(h0, "h0"); chk_cuda(c0, "c0");
   c10::cuda::CUDAGuard gd(gx.device());
   int T = gx.size(0), B = gx.size(1), H = gx.size(2) / 4;
   const int* lp = lengths_ptr(lengths, B, gx);
+  const int rev = direction_flag(reverse, in_gate, extra_signal);
   auto h_seq = torch::empty({T + 1, B, H}, gx.options());
   auto c_seq = torch::empty({T + 1, B, H}, c0.options());
   auto act = torch::empty({T, B, 4 * H}, gx.options());
@@ -375,7 +383,7 @@ std::vector<Tensor> lstm_seq_fwd(const Tensor& gx, const Tensor& w_h, const Tens
                         act.data_ptr(), c0.data_ptr<float>(), dbg.has_value() ? dbg->data_ptr() : nullptr, tiled.data_ptr(), T, B, H,
                         (unsigned int*)sync_ws.data_ptr<int>(), (int)variant, stream(), h0.data_ptr(),
                         in_gate.has_value() ? (const unsigned int*)in_gate->data_ptr<int>() : nullptr, (int)in_gate_tiles_n,
-                        extra_signal ? 1 : 0, 0, lp), "lstm_seq_fwd");
+                        extra_signal ? 1 : 0, 0, lp, rev), "lstm_seq_fwd");
   return {h_seq, c_seq, act};
 }
 
@@ -385,12 +393,13 @@ std::vector<Tensor> lstm_seq_fwd(const Tensor& gx, const Tensor& w_h, const Tens
 std::vector<Tensor> lstm_seq_bwd(const std::optional<Tensor>& dh_seq, const Tensor& w_hT, const Tensor& act, const Tensor& c_seq,
                                  const Tensor& dhT, const Tensor& dcT, Tensor sync_ws, int64_t variant,
                                  std::optional<Tensor> dbg, std::optional<Tensor> in_gate, int64_t in_gate_tiles_n, bool extra_signal,
-                                 const std::optional<Tensor>& lengths) {
+                                 const std::optional<Tensor>& lengths, bool reverse) {
   if (dh_seq.has_value()) chk_cuda(*dh_seq, "dh_seq");
   chk_cuda(w_hT, "w_hT"); chk_cuda(act, "act"); chk_cuda(c_seq, "c_seq");
   c10::cuda::CUDAGuard gd(act.device());
   int T = act.size(0), B = act.size(1), H = act.size(2) / 4;
   const int* lp = lengths_ptr(lengths, B, act);
+  const int rev = direction_flag(reverse, in_gate, extra_signal);
   auto dpre = torch::empty_like(act);
   auto dh0 = dhT.clone();
   auto dc0 = dcT.clone();
@@ -400,7 +409,7 @@ std::vector<Tensor> lstm_seq_bwd(const std::optional<Tensor>& dh_seq, const Tens
                         dh0.data_ptr<float>(), dc0.data_ptr<float>(), dbg.has_value() ? dbg->data_ptr() : nullptr, tiled.data_ptr(), T, B, H,
                         (unsigned int*)sync_ws.data_ptr<int>(), (int)variant, stream(),
                         in_gate.has_value() ? (const unsigned int*)in_gate->data_ptr<int>() : nullptr, (int)in_gate_tiles_n,
-                        extra_signal ? 1 : 0, 0, lp), "lstm_seq_bwd");
+                        extra_signal ? 1 : 0, 0, lp, rev), "lstm_seq_bwd");
   return {dpre, dh0, dc0};
 }
 
@@ -409,12 +418,13 @@ std::vector<Tensor> lstm_seq_bwd(const std::optional<Tensor>& dh_seq, const Tens
 void lstm_seq_fwd_into(const Tensor& gx, const Tensor& w_h, const Tensor& bias, const Tensor& h0, const Tensor& c0, Tensor h_seq,
                        Tensor c_seq, Tensor act, Tensor tiled, Tensor sync_ws, int64_t variant, std::optional<Tensor> in_gate,
                        int64_t in_gate_tiles_n, bool extra_signal, int64_t stream_handle, int64_t launch_flags,
-                       const std::optional<Tensor>& lengths) {
+                       const std::optional<Tensor>& lengths, bool reverse) {
   chk_cuda(gx, "gx"); chk_cuda(w_h, "w_h"); chk_cuda(bias, "bias"); chk_cuda(h0, "h0"); chk_cuda(c0, "c0");
   chk_cuda(h_seq, "h_seq"); chk_cuda(c_seq, "c_seq"); chk_cuda(act, "act"); chk_cuda(tiled, "tiled");
   c10::cuda::CUDAGuard gd(gx.device());
   int T = gx.size(0), B = gx.size(1), H = gx.size(2) / 4;
   const int* lp = lengths_ptr(lengths, B, gx);
+  const int rev = direction_flag(reverse, in_gate, extra_signal);
   TORCH_CHECK(h_seq.numel() == (int64_t)(T + 1) * B * H && c_seq.numel() == h_seq.numel() && act.numel() == gx.numel(), "lstm_seq_fwd_into: buffer sizes");
   TORCH_CHECK(tiled.numel() == (int64_t)(T + 1) * ((B + 127) / 128) * 128 * H, "lstm_seq_fwd_into: tile-image buffer size");
   TORCH_CHECK(h0.scalar_type() == torch::kBFloat16 && c0.scalar_type() == torch::kFloat32, "h0 bf16 / c0 fp32");
@@ -422,33 +432,38 @@ void lstm_seq_fwd_into(const Tensor& gx, const Tensor& w_h, const Tensor& bias, 
                         act.data_ptr(), c0.data_ptr<float>(), nullptr, tiled.data_ptr(), T, B, H, (unsigned int*)sync_ws.data_ptr<int>(),
                         (int)variant, stream_handle ? (cudaStream_t)stream_handle : stream(), h0.data_ptr(),
                         in_gate.has_value() ? (const unsigned int*)in_gate->data_ptr<int>() : nullptr, (int)in_gate_tiles_n,
-                        extra_signal ? 1 : 0, (int)launch_flags, lp), "lstm_seq_fwd_into");
+                        extra_signal ? 1 : 0, (int)launch_flags, lp, rev), "lstm_seq_fwd_into");
 }
 
-// h_seq[0] <- h0, c_seq[0] <- c0, tile image of h0, step counters <- 0 (what lstm_seq_fwd does first unless launch_flags bit 0)
-void lstm_seq_prologue(const Tensor& h0, const Tensor& c0, Tensor h_seq, Tensor c_seq, Tensor tiled, Tensor sync_ws) {
+// h_seq[0] <- h0, c_seq[0] <- c0 (reverse: row T), tile image of h0, step counters <- 0 (what lstm_seq_fwd does first unless
+// launch_flags bit 0)
+void lstm_seq_prologue(const Tensor& h0, const Tensor& c0, Tensor h_seq, Tensor c_seq, Tensor tiled, Tensor sync_ws, bool reverse) {
   chk_cuda(h0, "h0"); chk_cuda(c0, "c0"); chk_cuda(h_seq, "h_seq"); chk_cuda(c_seq, "c_seq"); chk_cuda(tiled, "tiled");
   c10::cuda::CUDAGuard gd(h0.device());
   TORCH_CHECK(h0.scalar_type() == torch::kBFloat16 && c0.scalar_type() == torch::kFloat32 && h0.dim() == 2, "h0 bf16 [B,H] / c0 fp32");
-  check(ts_lstm_seq_prologue(h0.data_ptr(), c0.data_ptr<float>(), h_seq.data_ptr(), c_seq.data_ptr<float>(), tiled.data_ptr(),
+  TORCH_CHECK(h_seq.scalar_type() == torch::kBFloat16 && h_seq.numel() % h0.numel() == 0 && h_seq.numel() >= h0.numel() &&
+              c_seq.numel() == h_seq.numel(), "lstm_seq_prologue: h_seq bf16 / c_seq [T+1,B,H]");
+  const int64_t init_off = reverse ? h_seq.numel() - h0.numel() : 0;       // row T
+  check(ts_lstm_seq_prologue(h0.data_ptr(), c0.data_ptr<float>(), (at::BFloat16*)h_seq.data_ptr() + init_off, c_seq.data_ptr<float>() + init_off, tiled.data_ptr(),
                              (unsigned int*)sync_ws.data_ptr<int>(), (int)h0.size(0), (int)h0.size(1), stream()), "lstm_seq_prologue");
 }
 
 void lstm_seq_bwd_into(const std::optional<Tensor>& dh_seq, const Tensor& w_hT, const Tensor& act, const Tensor& c_seq, Tensor dpre,
                        Tensor dh0, Tensor dc0, Tensor tiled, Tensor sync_ws, int64_t variant, std::optional<Tensor> in_gate,
                        int64_t in_gate_tiles_n, bool extra_signal, int64_t stream_handle, int64_t launch_flags,
-                       const std::optional<Tensor>& lengths) {
+                       const std::optional<Tensor>& lengths, bool reverse) {
   chk_cuda(w_hT, "w_hT"); chk_cuda(act, "act"); chk_cuda(c_seq, "c_seq"); chk_cuda(dpre, "dpre"); chk_cuda(dh0, "dh0"); chk_cuda(dc0, "dc0");
   c10::cuda::CUDAGuard gd(act.device());
   int T = act.size(0), B = act.size(1), H = act.size(2) / 4;
   const int* lp = lengths_ptr(lengths, B, act);
+  const int rev = direction_flag(reverse, in_gate, extra_signal);
   TORCH_CHECK(dpre.numel() == act.numel() && tiled.numel() == (int64_t)T * ((B + 127) / 128) * 128 * 4 * H, "lstm_seq_bwd_into: buffer sizes");
   TORCH_CHECK(dh0.scalar_type() == torch::kFloat32 && dc0.scalar_type() == torch::kFloat32 && dh0.numel() == (int64_t)B * H && dc0.numel() == (int64_t)B * H, "dh0/dc0 fp32 [B,H]");
   check(ts_lstm_seq_bwd(dh_seq.has_value() ? dh_seq->data_ptr() : nullptr, w_hT.data_ptr(), act.data_ptr(), c_seq.data_ptr<float>(), dpre.data_ptr(),
                         dh0.data_ptr<float>(), dc0.data_ptr<float>(), nullptr, tiled.data_ptr(), T, B, H, (unsigned int*)sync_ws.data_ptr<int>(),
                         (int)variant, stream_handle ? (cudaStream_t)stream_handle : stream(),
                         in_gate.has_value() ? (const unsigned int*)in_gate->data_ptr<int>() : nullptr, (int)in_gate_tiles_n,
-                        extra_signal ? 1 : 0, (int)launch_flags, lp), "lstm_seq_bwd_into");
+                        extra_signal ? 1 : 0, (int)launch_flags, lp, rev), "lstm_seq_bwd_into");
 }
 
 }  // namespace
@@ -497,17 +512,18 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("fold_cols") = 0);
   m.def("lstm_seq_fwd", &lstm_seq_fwd, py::arg("gx"), py::arg("w_h"), py::arg("bias"), py::arg("h0"), py::arg("c0"),
         py::arg("sync_ws"), py::arg("variant") = 0, py::arg("dbg") = py::none(), py::arg("in_gate") = py::none(),
-        py::arg("in_gate_tiles_n") = 0, py::arg("extra_signal") = false, py::arg("lengths") = py::none());
+        py::arg("in_gate_tiles_n") = 0, py::arg("extra_signal") = false, py::arg("lengths") = py::none(), py::arg("reverse") = false);
   m.def("lstm_seq_fwd_into", &lstm_seq_fwd_into, py::arg("gx"), py::arg("w_h"), py::arg("bias"), py::arg("h0"), py::arg("c0"),
         py::arg("h_seq"), py::arg("c_seq"), py::arg("act"), py::arg("tiled"), py::arg("sync_ws"), py::arg("variant"),
         py::arg("in_gate") = py::none(), py::arg("in_gate_tiles_n") = 0, py::arg("extra_signal") = false, py::arg("stream") = 0,
-        py::arg("launch_flags") = 0, py::arg("lengths") = py::none());
-  m.def("lstm_seq_prologue", &lstm_seq_prologue);
+        py::arg("launch_flags") = 0, py::arg("lengths") = py::none(), py::arg("reverse") = false);
+  m.def("lstm_seq_prologue", &lstm_seq_prologue, py::arg("h0"), py::arg("c0"), py::arg("h_seq"), py::arg("c_seq"), py::arg("tiled"),
+        py::arg("sync_ws"), py::arg("reverse") = false);
   m.def("lstm_seq_bwd_into", &lstm_seq_bwd_into, py::arg("dh_seq"), py::arg("w_hT"), py::arg("act"), py::arg("c_seq"), py::arg("dpre"),
         py::arg("dh0"), py::arg("dc0"), py::arg("tiled"), py::arg("sync_ws"), py::arg("variant"), py::arg("in_gate") = py::none(),
         py::arg("in_gate_tiles_n") = 0, py::arg("extra_signal") = false, py::arg("stream") = 0, py::arg("launch_flags") = 0,
-        py::arg("lengths") = py::none());
+        py::arg("lengths") = py::none(), py::arg("reverse") = false);
   m.def("lstm_seq_bwd", &lstm_seq_bwd, py::arg("dh_seq"), py::arg("w_hT"), py::arg("act"), py::arg("c_seq"), py::arg("dhT"),
         py::arg("dcT"), py::arg("sync_ws"), py::arg("variant") = 0, py::arg("dbg") = py::none(), py::arg("in_gate") = py::none(),
-        py::arg("in_gate_tiles_n") = 0, py::arg("extra_signal") = false, py::arg("lengths") = py::none());
+        py::arg("in_gate_tiles_n") = 0, py::arg("extra_signal") = false, py::arg("lengths") = py::none(), py::arg("reverse") = false);
 }

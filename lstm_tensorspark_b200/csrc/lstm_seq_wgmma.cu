@@ -243,7 +243,14 @@ struct SeqParams {
 // unsplit kernel.  Used when the larger accumulator stage still leaves >= 3 ring stages (smaller H).
 // kMasked: per-row sequence lengths (SeqParams::lengths).  A separate instantiation, so the unmasked kernels - at the register
 // cap - carry no extra state; the dataflow, the exchange and the signalling are the same (a padded row still signals every step).
-template <bool kBwd, int kStages, int kTiles, bool kStream, bool kFSplit = false, bool kMasked = false>
+// kRev: the reverse-time direction of a bidirectional layer.  Forward step s processes time tau = T-1-s, the backward pass visits
+// tau ascending.  The saved sequences stay in time order with the initial state in the LAST slot: h_seq / c_seq row tau < T = the
+// state after processing time tau, row T = h0 / c0; act / dpre row tau = time tau.  The output is h_seq[0:T], the final state
+// row 0, and dW_h pairs dpre with h_seq[1:T+1].  Only the time index of those arrays changes: the swizzled operand images
+// (a_tiled), the dataflow counters and the exchange stay in processing order.  With kMasked a row's padded steps
+// (tau >= len) come FIRST in the forward pass (the cell holds h0 / c0 there) and LAST in the backward pass (dh / dc carry
+// through them into dh0 / dc0).  Not combined with the layer wavefront (in_gate / extra_signal; the host rejects it).
+template <bool kBwd, int kStages, int kTiles, bool kStream, bool kFSplit = false, bool kMasked = false, bool kRev = false>
 __global__ void __launch_bounds__(384, 1)
 lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
   static_assert(!(kFSplit && (kBwd || kStream || kTiles != 1)), "forward K-split: one tile, resident weights");
@@ -563,14 +570,16 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
       const uint32_t xbar = tc::smem_u32(&ss->xchg_full[0]), fbar = tc::smem_u32(&ss->xchg_free[0]);
       const uint32_t pbar = kFSplit ? mapa(xbar, (uint32_t)(1 - ks)) : 0u;      // the peer's exchange barrier
       float cst[kTiles][8];
+      const size_t init_row = kRev ? (size_t)p.T * B : 0;     // the prologue wrote h0 / c0 to row 0 (forward) or row T (kRev)
 #pragma unroll
       for (int tile = 0; tile < kTiles; ++tile) {
         const int row = (mb0 + tile) * BM + rloc;
 #pragma unroll
-        for (int i = 0; i < 8; ++i) cst[tile][i] = row < B ? p.c_seq[(size_t)row * H + j0 + i] : 0.f;     // c_0 (written by the prologue)
+        for (int i = 0; i < 8; ++i) cst[tile][i] = row < B ? p.c_seq[(init_row + row) * H + j0 + i] : 0.f;     // c_0 (written by the prologue)
       }
       // kMasked: this thread's row length per tile, and its last emitted h (8 bf16) - a padded step re-emits it without a load.
-      // Step 0 is never padded (len >= 1), so hprev needs no initial value.
+      // Forward order: step 0 is never padded (len >= 1), so hprev needs no initial value.  kRev: the padded steps come first
+      // and re-emit h0.
       int len[kTiles];
       uint4 hprev[kTiles];
       if constexpr (kMasked) {
@@ -579,9 +588,11 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
           const int row = (mb0 + tile) * BM + rloc;
           len[tile] = row < B ? p.lengths[row] : p.T;
           hprev[tile] = make_uint4(0u, 0u, 0u, 0u);
+          if (kRev && row < B) hprev[tile] = *reinterpret_cast<const uint4*>(p.h_seq + (init_row + row) * H + j0);
         }
       }
       for (int t = 0; t < p.T && ok; ++t) {
+        const int tt = kRev ? p.T - 1 - t : t;        // the time step that processing step t handles
 #pragma unroll
         for (int tile = 0; tile < kTiles; ++tile) {
           const int mb = mb0 + tile;
@@ -598,9 +609,10 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
               gxw[0] = ldg_cg32(gp); gxw[1] = ldg_cg32(gp + 16);
             }
           } else if (valid) {
-            const __nv_bfloat16* gp = p.gx + ((size_t)t * B + row) * (4 * H) + n0;
+            const __nv_bfloat16* gp = p.gx + ((size_t)tt * B + row) * (4 * H) + n0;
             gxw[0] = ldg_nc32(gp); gxw[1] = ldg_nc32(gp + 16);
-            if (t + 2 < p.T && p.debug_mode != 6) prefetch_l2(gp + (size_t)2 * B * (4 * H));     // the x-projection comes from HBM: pull it into L2 early
+            if (t + 2 < p.T && p.debug_mode != 6)      // the x-projection comes from HBM: pull it into L2 early
+              prefetch_l2(kRev ? gp - (size_t)2 * B * (4 * H) : gp + (size_t)2 * B * (4 * H));
           }
           ok = mma_tile();
           if (!ok) break;
@@ -642,7 +654,7 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
             acc_ld32(32 * half, v);
           }
           if (dbg_thread && t == 8 && tile == 0) p.dbg[4 * (p.T + 2) + 0] = gtime();
-          const bool pad = kMasked && t >= len[tile];   // padded step: the cell holds (the activations are computed but unused)
+          const bool pad = kMasked && tt >= len[tile];  // padded step: the cell holds (the activations are computed but unused)
           float cn[8], hv[8];
           uint32_t apk[16];
 #pragma unroll
@@ -698,11 +710,12 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
           }
           signal_sent_bar();
           if (valid && p.debug_mode != 5) {              // everything below is off the critical path
-            stg16(p.h_seq + ((size_t)(t + 1) * B + row) * H + j0, h8);
-            float* cp = p.c_seq + ((size_t)(t + 1) * B + row) * H + j0;
+            const size_t srow = kRev ? (size_t)tt : (size_t)(t + 1);      // state row written by this step
+            stg16(p.h_seq + (srow * B + row) * H + j0, h8);
+            float* cp = p.c_seq + (srow * B + row) * H + j0;
             stg32(cp, __float_as_uint(cn[0]), __float_as_uint(cn[1]), __float_as_uint(cn[2]), __float_as_uint(cn[3]),
                   __float_as_uint(cn[4]), __float_as_uint(cn[5]), __float_as_uint(cn[6]), __float_as_uint(cn[7]));
-            __nv_bfloat16* ap = p.act + ((size_t)t * B + row) * (4 * H) + n0;
+            __nv_bfloat16* ap = p.act + ((size_t)tt * B + row) * (4 * H) + n0;
 #pragma unroll
             for (int i = 0; i < 2; ++i)
               stg32(ap + 16 * i, apk[8 * i], apk[8 * i + 1], apk[8 * i + 2], apk[8 * i + 3], apk[8 * i + 4], apk[8 * i + 5], apk[8 * i + 6], apk[8 * i + 7]);
@@ -741,8 +754,9 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
         }
       }
       U8 c_carry[kTiles];                       // c_t of the previous iteration = c_{t+1} of this one (one load per step, not two)
-      // kMasked: right padding makes a row's padded steps the FIRST backward iterations.  There dG = 0, dc passes through and
-      // dh[tile] keeps the total dh (carry + dh_seq[t]): the next exchange sum adds the (exactly zero) recurrent term to it.
+      // kMasked: right padding makes a row's padded steps the FIRST backward iterations (kRev: the LAST ones).  There dG = 0, dc
+      // passes through and dh[tile] keeps the total dh (carry + dh_seq[t]): the next exchange sum adds the (exactly zero)
+      // recurrent term to it.  With kRev the values carried through the trailing padded steps are dh0 / dc0.
       int len[kTiles];
       if constexpr (kMasked) {
 #pragma unroll
@@ -752,14 +766,16 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
         }
       }
       for (int s = 0; s <= p.T && ok; ++s) {
-        const int t = p.T - 1 - s;
+        const int t = p.T - 1 - s;                    // operand-image slot (processing order)
+        const int tt = kRev ? s : t;                  // the time step of this iteration
 #pragma unroll
         for (int tile = 0; tile < kTiles; ++tile) {
           const int mb = mb0 + tile;
           const int row = mb * BM + rloc;
           const bool valid = row < B;
-          const bool pad = kMasked && s < p.T && t >= len[tile];           // step t is padding for this row
-          const bool prev_pad = kMasked && s > 0 && t + 1 >= len[tile];    // step t + 1 was: dh carries, c_carry is not set
+          const bool pad = kMasked && s < p.T && tt >= len[tile];          // step tt is padding for this row
+          // the previous iteration's step was: dh carries, c_carry is not set
+          const bool prev_pad = kMasked && s > 0 && (kRev ? tt - 1 : t + 1) >= len[tile];
           uint8_t* xbuf = smem_x + tile * kXchgBytes;               // [kSplit src][128 rows][16 bf16]
           const uint32_t xbase = tc::smem_u32(xbuf);
           const uint32_t xbar = tc::smem_u32(&ss->xchg_full[tile]);
@@ -771,20 +787,27 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
             if (!ok) break;
           }
           if (valid && s < p.T) {
-            const __nv_bfloat16* ap = p.act + ((size_t)t * B + row) * (4 * H) + 4 * j0;
+            const __nv_bfloat16* ap = p.act + ((size_t)tt * B + row) * (4 * H) + 4 * j0;
             if (!pad) { avw[0] = ldg_nc32(ap); avw[1] = ldg_nc32(ap + 16); }
-            dhv = p.dh_seq ? (p.in_gate ? ldg_cg16(p.dh_seq + ((size_t)t * B + row) * H + j0) : ldg_nc16(p.dh_seq + ((size_t)t * B + row) * H + j0))
+            dhv = p.dh_seq ? (p.in_gate ? ldg_cg16(p.dh_seq + ((size_t)t * B + row) * H + j0) : ldg_nc16(p.dh_seq + ((size_t)tt * B + row) * H + j0))
                            : make_uint4(0u, 0u, 0u, 0u);
-            const float* c0p = p.c_seq + ((size_t)t * B + row) * H + j0;
-            const float* c1p = p.c_seq + ((size_t)(t + 1) * B + row) * H + j0;
+            // c_prev / c_new of step tt (kRev: rows tt + 1 / tt).  c_new is the previous iteration's c_prev in both directions.
+            const float* c0p = p.c_seq + ((size_t)(kRev ? tt + 1 : t) * B + row) * H + j0;
+            const float* c1p = p.c_seq + ((size_t)(kRev ? tt : t + 1) * B + row) * H + j0;
             if (!pad) {
               cpv = ldg_nc32(c0p);
               cnv = (s == 0 || prev_pad) ? ldg_nc32(c1p) : c_carry[tile];
               c_carry[tile] = cpv;
-              if (t >= 2) {                                                    // saved activations come from HBM: pull t-2 into L2 early
-                prefetch_l2(ap - (size_t)2 * B * (4 * H));
-                prefetch_l2(c0p - (size_t)2 * B * H);
-                if (p.dh_seq && !p.in_gate) prefetch_l2(p.dh_seq + ((size_t)(t - 2) * B + row) * H + j0);
+              if (t >= 2) {                          // saved activations come from HBM: pull the step two iterations ahead into L2
+                if constexpr (kRev) {
+                  prefetch_l2(ap + (size_t)2 * B * (4 * H));
+                  prefetch_l2(c0p + (size_t)2 * B * H);
+                  if (p.dh_seq) prefetch_l2(p.dh_seq + ((size_t)(tt + 2) * B + row) * H + j0);
+                } else {
+                  prefetch_l2(ap - (size_t)2 * B * (4 * H));
+                  prefetch_l2(c0p - (size_t)2 * B * H);
+                  if (p.dh_seq && !p.in_gate) prefetch_l2(p.dh_seq + ((size_t)(t - 2) * B + row) * H + j0);
+                }
               }
             }
           }
@@ -897,7 +920,7 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
           }
           signal_sent_bar();
           if (valid) {                                   // the [T,B,4H] copy for the weight-gradient GEMMs: off the critical path
-            __nv_bfloat16* gp = p.dpre + ((size_t)t * B + row) * (4 * H) + 4 * j0;
+            __nv_bfloat16* gp = p.dpre + ((size_t)tt * B + row) * (4 * H) + 4 * j0;
 #pragma unroll
             for (int i = 0; i < 2; ++i)
               stg32(gp + 16 * i, gpk[8 * i], gpk[8 * i + 1], gpk[8 * i + 2], gpk[8 * i + 3], gpk[8 * i + 4], gpk[8 * i + 5], gpk[8 * i + 6], gpk[8 * i + 7]);
@@ -918,8 +941,8 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
   if (threadIdx.x == 0 && ss->abort_flag) atomicExch(reinterpret_cast<int*>(p.sync + kSyncErr), 1);
 }
 
-// One small launch instead of ~12 framework ops: h_seq[0] <- h0, c_seq[0] <- c0, the swizzled tile image of h0 (slot 0
-// of the streamed operand, zero rows beyond B), and the step counters <- 0.
+// One small launch instead of ~12 framework ops: h_seq[0] <- h0, c_seq[0] <- c0 (the reverse direction passes row T), the
+// swizzled tile image of h0 (slot 0 of the streamed operand, zero rows beyond B), and the step counters <- 0.
 __global__ void seq_prologue_kernel(const __nv_bfloat16* __restrict__ h0, const float* __restrict__ c0,
                                     __nv_bfloat16* __restrict__ h_seq0, float* __restrict__ c_seq0,
                                     __nv_bfloat16* __restrict__ tiled0, unsigned int* __restrict__ sync, int B, int H, int tiles_m) {
@@ -950,9 +973,9 @@ size_t smem_bytes(int H, bool bwd, int stages, int tiles, bool stream = false, b
   return (stream ? 0 : (size_t)(H / BK) * kWBlockBytes) + ring + ((bwd || fsplit) ? tiles * kXchgBytes : 0) + acc_stage + sizeof(SeqSmem) + 1024;
 }
 
-template <bool kBwd, int kStages, int kTiles, bool kStream = false, bool kFSplit = false, bool kMasked = false>
+template <bool kBwd, int kStages, int kTiles, bool kStream = false, bool kFSplit = false, bool kMasked = false, bool kRev = false>
 int launch_cfg(const CUtensorMap& tw, const SeqParams& p, int grid, cudaStream_t st) {
-  auto kern = lstm_seq_kernel<kBwd, kStages, kTiles, kStream, kFSplit, kMasked>;
+  auto kern = lstm_seq_kernel<kBwd, kStages, kTiles, kStream, kFSplit, kMasked, kRev>;
   const size_t smem = smem_bytes(p.H, kBwd, kStages, kTiles, kStream, kFSplit);
   constexpr int kClusterDim = kBwd ? (kStream ? 2 : 4) : (kFSplit ? 2 : 1);
   if (smem > 227 * 1024) return -4;
@@ -979,42 +1002,42 @@ int launch_cfg(const CUtensorMap& tw, const SeqParams& p, int grid, cudaStream_t
   return (int)e;
 }
 
-template <bool kBwd, bool kMasked>
+template <bool kBwd, bool kMasked, bool kRev>
 int dispatch(const CUtensorMap& tw, const SeqParams& p, int grid, int stages, int tiles, bool stream, bool fsplit, cudaStream_t st) {
   if constexpr (!kBwd) {
     if (fsplit) {                                  // forward K-split (cluster of 2), one batch tile per CTA
       switch (stages) {
-        case 3: return launch_cfg<false, 3, 1, false, true, kMasked>(tw, p, grid, st);
-        case 4: return launch_cfg<false, 4, 1, false, true, kMasked>(tw, p, grid, st);
-        case 5: return launch_cfg<false, 5, 1, false, true, kMasked>(tw, p, grid, st);
-        case 6: return launch_cfg<false, 6, 1, false, true, kMasked>(tw, p, grid, st);
+        case 3: return launch_cfg<false, 3, 1, false, true, kMasked, kRev>(tw, p, grid, st);
+        case 4: return launch_cfg<false, 4, 1, false, true, kMasked, kRev>(tw, p, grid, st);
+        case 5: return launch_cfg<false, 5, 1, false, true, kMasked, kRev>(tw, p, grid, st);
+        case 6: return launch_cfg<false, 6, 1, false, true, kMasked, kRev>(tw, p, grid, st);
       }
       return -5;
     }
   }
   if (stream) {                                    // streamed weights: 24 KB stages, one batch tile per CTA
     switch (stages) {
-      case 4: return launch_cfg<kBwd, 4, 1, true, false, kMasked>(tw, p, grid, st);
-      case 6: return launch_cfg<kBwd, 6, 1, true, false, kMasked>(tw, p, grid, st);
-      case 8: return launch_cfg<kBwd, 8, 1, true, false, kMasked>(tw, p, grid, st);
+      case 4: return launch_cfg<kBwd, 4, 1, true, false, kMasked, kRev>(tw, p, grid, st);
+      case 6: return launch_cfg<kBwd, 6, 1, true, false, kMasked, kRev>(tw, p, grid, st);
+      case 8: return launch_cfg<kBwd, 8, 1, true, false, kMasked, kRev>(tw, p, grid, st);
     }
     return -5;
   }
   if (tiles == 2) {
     switch (stages) {
-      case 2: return launch_cfg<kBwd, 2, 2, false, false, kMasked>(tw, p, grid, st);
-      case 3: return launch_cfg<kBwd, 3, 2, false, false, kMasked>(tw, p, grid, st);
-      case 4: return launch_cfg<kBwd, 4, 2, false, false, kMasked>(tw, p, grid, st);
-      case 5: return launch_cfg<kBwd, 5, 2, false, false, kMasked>(tw, p, grid, st);
-      case 6: return launch_cfg<kBwd, 6, 2, false, false, kMasked>(tw, p, grid, st);
+      case 2: return launch_cfg<kBwd, 2, 2, false, false, kMasked, kRev>(tw, p, grid, st);
+      case 3: return launch_cfg<kBwd, 3, 2, false, false, kMasked, kRev>(tw, p, grid, st);
+      case 4: return launch_cfg<kBwd, 4, 2, false, false, kMasked, kRev>(tw, p, grid, st);
+      case 5: return launch_cfg<kBwd, 5, 2, false, false, kMasked, kRev>(tw, p, grid, st);
+      case 6: return launch_cfg<kBwd, 6, 2, false, false, kMasked, kRev>(tw, p, grid, st);
     }
   } else {
     switch (stages) {
-      case 2: return launch_cfg<kBwd, 2, 1, false, false, kMasked>(tw, p, grid, st);
-      case 3: return launch_cfg<kBwd, 3, 1, false, false, kMasked>(tw, p, grid, st);
-      case 4: return launch_cfg<kBwd, 4, 1, false, false, kMasked>(tw, p, grid, st);
-      case 5: return launch_cfg<kBwd, 5, 1, false, false, kMasked>(tw, p, grid, st);
-      case 6: return launch_cfg<kBwd, 6, 1, false, false, kMasked>(tw, p, grid, st);
+      case 2: return launch_cfg<kBwd, 2, 1, false, false, kMasked, kRev>(tw, p, grid, st);
+      case 3: return launch_cfg<kBwd, 3, 1, false, false, kMasked, kRev>(tw, p, grid, st);
+      case 4: return launch_cfg<kBwd, 4, 1, false, false, kMasked, kRev>(tw, p, grid, st);
+      case 5: return launch_cfg<kBwd, 5, 1, false, false, kMasked, kRev>(tw, p, grid, st);
+      case 6: return launch_cfg<kBwd, 6, 1, false, false, kMasked, kRev>(tw, p, grid, st);
     }
   }
   return -5;
@@ -1032,9 +1055,13 @@ int pick_stages(int H, bool bwd, int tiles) {
 // variant (tuning knob, 0 = defaults) = tiles_per_cta + 16*stages + 4096*debug_mode:  tiles_per_cta 0 -> 1 (set 2 to let a
 // CTA alternate two batch tiles);  stages 0 -> deepest ring that fits next to the resident weight slice.
 template <bool kBwd>
-static int seq_common(SeqParams& p, const void* w_base, int variant, cudaStream_t st) {
+static int seq_common(SeqParams& p, const void* w_base, int variant, cudaStream_t st, bool reverse) {
   const int H = p.H, B = p.B;
   if (H % 64 != 0) { ts::set_last_error("lstm_seq: H must be a multiple of 64"); return -2; }
+  if (reverse && (p.in_gate != nullptr || p.extra_signal)) {
+    ts::set_last_error("lstm_seq: the reverse direction does not run in the layer wavefront (in_gate / extra_signal)");
+    return -2;
+  }
   const int tiles_m = (B + BM - 1) / BM, tiles_n = kBwd ? (H / BN) * 4 : 4 * H / BN;
   int stages = (variant >> 4) & 15, tiles = variant & 15;
   p.debug_mode = (variant >> 12) & 7;
@@ -1069,8 +1096,10 @@ static int seq_common(SeqParams& p, const void* w_base, int variant, cudaStream_
   if (int rc = ts::make_tmap_2d_bf16(&tw, w_base, (uint64_t)N, (uint64_t)K, (uint64_t)K, BK, fsplit ? 2 * BN : ((kBwd && stream) ? BN / 2 : BN))) return rc;
   p.tiles_n = tiles_n;
   p.tiles_m = tiles_m;
-  int rc = p.lengths ? dispatch<kBwd, true>(tw, p, grid, stages, tiles, stream, fsplit, st)
-                     : dispatch<kBwd, false>(tw, p, grid, stages, tiles, stream, fsplit, st);
+  int rc = reverse ? (p.lengths ? dispatch<kBwd, true, true>(tw, p, grid, stages, tiles, stream, fsplit, st)
+                                : dispatch<kBwd, false, true>(tw, p, grid, stages, tiles, stream, fsplit, st))
+                   : (p.lengths ? dispatch<kBwd, true, false>(tw, p, grid, stages, tiles, stream, fsplit, st)
+                                : dispatch<kBwd, false, false>(tw, p, grid, stages, tiles, stream, fsplit, st));
   if (rc == -21) ts::set_last_error("lstm_seq: the thread-block clusters are not co-resident on this device");
   return rc;
 }
@@ -1078,13 +1107,14 @@ static int seq_common(SeqParams& p, const void* w_base, int variant, cudaStream_
 extern "C" int ts_lstm_seq_fwd(const void* gx, const void* w_h, const float* bias, const void* h_seq, const float* c_seq,
                                void* act, const float* c0, void* dbg, void* a_tiled, int T, int B, int H, unsigned int* sync_ws, int variant,
                                cudaStream_t st, const void* h0, const unsigned int* in_gate, int in_gate_tiles_n, int extra_signal, int launch_flags,
-                               const int* lengths) {
+                               const int* lengths, int reverse) {
   if (!(launch_flags & 1)) {           // bit 0: the caller has run ts_lstm_seq_prologue itself (wavefront: all prologues precede the chain)
     const int tiles_m = (B + BM - 1) / BM;
     const int total = tiles_m * BM * (H / 8);
     int blocks = (total + 255) / 256;
     if (blocks > 592) blocks = 592;
-    seq_prologue_kernel<<<blocks, 256, 0, st>>>((const __nv_bfloat16*)h0, c0, (__nv_bfloat16*)h_seq, (float*)c_seq,
+    const size_t init_off = reverse ? (size_t)T * B * H : 0;      // h0 / c0 go to row T of the reverse direction
+    seq_prologue_kernel<<<blocks, 256, 0, st>>>((const __nv_bfloat16*)h0, c0, (__nv_bfloat16*)h_seq + init_off, (float*)c_seq + init_off,
                                                 (__nv_bfloat16*)a_tiled, sync_ws, B, H, tiles_m);
   }
   SeqParams p{};
@@ -1094,7 +1124,7 @@ extern "C" int ts_lstm_seq_fwd(const void* gx, const void* w_h, const float* bia
   p.in_gate = in_gate; p.in_gate_tiles_n = in_gate_tiles_n; p.extra_signal = extra_signal;
   p.pdl_wait = (launch_flags >> 1) & 1;
   p.lengths = lengths;
-  return seq_common<false>(p, w_h, variant, st);
+  return seq_common<false>(p, w_h, variant, st, reverse != 0);
 }
 
 extern "C" int ts_lstm_seq_prologue(const void* h0, const float* c0, void* h_seq, float* c_seq, void* a_tiled, unsigned int* sync_ws,
@@ -1110,7 +1140,7 @@ extern "C" int ts_lstm_seq_prologue(const void* h0, const float* c0, void* h_seq
 extern "C" int ts_lstm_seq_bwd(const void* dh_seq, const void* w_hT, const void* act, const float* c_seq, const void* dpre,
                                float* dh0, float* dc0, void* dbg, void* a_tiled, int T, int B, int H, unsigned int* sync_ws, int variant,
                                cudaStream_t st, const unsigned int* in_gate, int in_gate_tiles_n, int extra_signal, int launch_flags,
-                               const int* lengths) {
+                               const int* lengths, int reverse) {
   if (!(launch_flags & 1)) cudaMemsetAsync(sync_ws, 0, kSyncErr * sizeof(unsigned int), st);      // arrival counters restart at 0 every launch
   SeqParams p{};
   p.a_tiled = (__nv_bfloat16*)a_tiled;
@@ -1119,7 +1149,7 @@ extern "C" int ts_lstm_seq_bwd(const void* dh_seq, const void* w_hT, const void*
   p.in_gate = in_gate; p.in_gate_tiles_n = in_gate_tiles_n; p.extra_signal = extra_signal;
   p.pdl_wait = (launch_flags >> 1) & 1;
   p.lengths = lengths;
-  return seq_common<true>(p, w_hT, variant, st);
+  return seq_common<true>(p, w_hT, variant, st, reverse != 0);
 }
 
 

@@ -82,12 +82,13 @@ class TrainEngine:
         """Gradient buckets in the order backward finishes them: [top layer (+ head)], ..., [layer 0].  A bucket = a
         contiguous element range of the flat buffer + the parameters that must have been written before it may be synced.
         (Reference counterpart: the one-shot reduceByKey over all weights, original src/rnn.py:393-407 - here the sync
-        of the upper layers hides under the backward recurrence of the layers below.)"""
+        of the upper layers hides under the backward recurrence of the layers below.)  Bidirectional: every direction of a layer
+        is a layer here (flat order: forward, reverse per depth; backward finishes the reverse direction first)."""
         flat = self.flat
         if not flat._direct:
             return None
         off = {id(p): o for p, o in zip(flat.params, flat.offsets)}
-        layers = list(self.model.rnn.layers)
+        layers = self.model.rnn.directions()
         others = [p for p in flat.params[len(self.model.rnn.averaged_parameters()):]]
         others_direct = all(p.data_ptr() in flat._direct for p in others)
         end = [off[id(l.w_x)] for l in layers[1:]] + [flat.lstm_numel]        # end of each layer's segment

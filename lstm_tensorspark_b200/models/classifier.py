@@ -16,7 +16,7 @@ from .recurrent.rnn import RNN
 
 
 class DenseHead(nn.Module):
-    """``Dense1``: weights ``[H_last, C]``, bias ``[C]`` (truncated normal, src/rnn.py:214-221)."""
+    """``Dense1``: weights ``[H_last, C]`` (bidirectional: ``[2 H_last, C]``), bias ``[C]`` (truncated normal, src/rnn.py:214-221)."""
 
     def __init__(self, in_features: int, num_classes: int, init_std: float = 1.0, device=None, generator=None):
         super().__init__()
@@ -41,11 +41,14 @@ class SequenceClassifier(nn.Module):
         self.cfg = cfg
         bs = cfg.batch_size if batch_size is None else batch_size
         settings = cfg.net_settings(bs)
-        head_std = cfg.init_std if cfg.init != "scaled" else cfg.init_std / (settings[-1]["num_hidden"] ** 0.5)
+        head_in = settings[-1]["num_hidden"] * (2 if cfg.bidirectional else 1)
+        head_std = cfg.init_std if cfg.init != "scaled" else cfg.init_std / (head_in ** 0.5)
         self.rnn = RNN(settings, learn_initial_state=cfg.resolved_learn_initial_state(), init_std=cfg.init_std,
                        init=cfg.init, weight_decay=(cfg.weight_decay or None), device=device, generator=generator)
-        self.head = DenseHead(settings[-1]["num_hidden"], cfg.num_classes, init_std=head_std, device=device,
-                              generator=generator)
+        self.head = DenseHead(head_in, cfg.num_classes, init_std=head_std, device=device, generator=generator)
+        if cfg.bidirectional:
+            # drawn after every parameter of the unidirectional model, which therefore keeps its initial weights
+            self.rnn.add_reverse_layers()
         self.flat: Optional[FlatParams] = None
         self._allocator = allocator
         self.compute_dtype = torch.float32
@@ -81,11 +84,20 @@ class SequenceClassifier(nn.Module):
     # ---- reference variable naming ------------------------------------------------
     def named_reference_variables(self) -> List[Tuple[str, torch.Tensor]]:
         out = []
-        for layer in self.rnn.layers:
+        for layer in self.rnn.directions():
             out += layer.named_reference_variables()
         out.append(("Dense1/weights", self.head.weights))
         out.append(("Dense1/bias", self.head.bias))
         return out
+
+    def check_directions(self, variables: Dict[str, torch.Tensor], what: str = "checkpoint") -> None:
+        """A checkpoint loads with ``strict=False``: a unidirectional one would leave a bidirectional model's reverse weights at
+        their initial values (and the other way round silently drop them).  Raise unless both have the same directions."""
+        saved = any("_reverse/" in k for k in variables)
+        if saved != self.rnn.bidirectional:
+            raise ValueError(f"{what} was written by a {'bidirectional' if saved else 'unidirectional'} model, this run is "
+                             f"{'bidirectional' if self.rnn.bidirectional else 'unidirectional'}: "
+                             f"{'add' if saved else 'drop'} --bidirectional")
 
     def reference_state_dict(self) -> Dict[str, torch.Tensor]:
         return {k: v.detach().clone().contiguous().cpu() for k, v in self.named_reference_variables()}

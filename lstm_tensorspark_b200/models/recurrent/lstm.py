@@ -68,8 +68,9 @@ class LSTMLayer(nn.Module):
     def __init__(self, name: str, num_hidden: int, dim_size: int, batch_size: int,
                  learn_initial_state: bool = True, init_std: float = 1.0, init: str = "truncated_normal",
                  weight_decay: Optional[float] = None, device=None,
-                 generator: Optional[torch.Generator] = None):
+                 generator: Optional[torch.Generator] = None, reverse: bool = False):
         super().__init__()
+        self.reverse = reverse                  # reverse-time direction of a bidirectional layer (whole sequences only)
         self.shape = [batch_size, num_hidden, dim_size]
         self.batch_size = batch_size
         self.num_hidden = num_hidden
@@ -159,11 +160,14 @@ class LSTMLayer(nn.Module):
     # ---- whole-sequence path (the thing the persistent kernel implements) ----------------------
     def fit_sequence(self, x_seq: torch.Tensor, lengths: Optional[torch.Tensor] = None) -> torch.Tensor:
         """``x_seq [T,B,D]`` -> ``h_seq [T,B,H]``; final (ht, Ct) stored on the layer.  ``lengths`` (int32 ``[B]``, right
-        padding): the final state is each row's state after its own last step; padded positions of ``h_seq`` carry it."""
+        padding): the final state is each row's state after its own last step; padded positions of ``h_seq`` carry it.
+        A reverse layer runs from the last step to the first: its final state is the one after step 0, and its padded
+        positions hold the initial state."""
         B = x_seq.shape[1]
         if B != self.ht.shape[0]:
             self.reset_state(B)
-        h_seq, h_T, c_T = F.lstm_layer_sequence(x_seq, self.ht, self.Ct, self.w_x, self.w_h, self.bias, lengths=lengths)
+        h_seq, h_T, c_T = F.lstm_layer_sequence(x_seq, self.ht, self.Ct, self.w_x, self.w_h, self.bias, lengths=lengths,
+                                                reverse=self.reverse)
         self._set_state(h_T, c_T)
         self.state.append((h_T, c_T))
         return h_seq

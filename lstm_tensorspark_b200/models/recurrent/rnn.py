@@ -4,7 +4,8 @@ Public surface mirrors original src/models/recurrent/rnn.py:5-53: ``RNN(settings
 ``fit_layers(x)``, ``map_data_by_key()``, ``add_layer(setting)``, ``add_layers(settings)``.
 ``settings`` is the list of dicts built by ``Config.net_settings`` (keys ``layer_name``, ``dim_size``,
 ``num_hidden``, ``batch_size``).  New: ``fit_layers`` also accepts a sequence ``[B,T,D]`` and unrolls it
-through time on the fused per-layer sequence op (the reference only ever takes one step).
+through time on the fused per-layer sequence op (the reference only ever takes one step), and
+``add_reverse_layers()`` makes the stack bidirectional.
 """
 from __future__ import annotations
 
@@ -22,15 +23,42 @@ class RNN(nn.Module):
     def __init__(self, settings: Iterable[dict], **layer_kw):
         super().__init__()
         self.layers = nn.ModuleList()
+        self.reverse_layers = nn.ModuleList()      # empty, or one reverse-time layer per entry of ``layers``
         self._layer_kw = layer_kw
         self.add_layers(settings)
 
-    def _make(self, setting: dict) -> LSTMLayer:
-        return LSTMLayer(name=setting["layer_name"], num_hidden=setting["num_hidden"],
-                         dim_size=setting["dim_size"], batch_size=setting["batch_size"], **self._layer_kw)
+    def _make(self, setting: dict, reverse: bool = False) -> LSTMLayer:
+        name = setting["layer_name"] + ("_reverse" if reverse else "")
+        return LSTMLayer(name=name, num_hidden=setting["num_hidden"], dim_size=setting["dim_size"],
+                         batch_size=setting["batch_size"], reverse=reverse, **self._layer_kw)
 
     def add_layer(self, setting: dict):
+        if self.bidirectional:
+            raise ValueError("add_layer: add every layer before add_reverse_layers()")
         self.layers.append(self._make(setting))
+
+    def add_reverse_layers(self):
+        """Make the stack bidirectional: a reverse-time twin ``<layer_name>_reverse`` of every layer, with its own weights (drawn
+        now, after everything drawn so far).  Layer ``l + 1`` then reads ``[h_fwd(t) | h_rev(t)]``, so its ``dim_size`` must be
+        ``2 H_l`` (``Config.net_settings`` with ``bidirectional``)."""
+        if self.bidirectional:
+            raise ValueError("the stack is already bidirectional")
+        for i, layer in enumerate(self.layers):
+            if i > 0 and layer.dim_size != 2 * self.layers[i - 1].num_hidden:
+                raise ValueError(f"{layer.node_name}: a bidirectional stack needs dim_size = 2 * {self.layers[i - 1].num_hidden}, "
+                                 f"got {layer.dim_size}")
+            self.reverse_layers.append(self._make({"layer_name": layer.node_name, "num_hidden": layer.num_hidden,
+                                                   "dim_size": layer.dim_size, "batch_size": layer.batch_size}, reverse=True))
+
+    @property
+    def bidirectional(self) -> bool:
+        return len(self.reverse_layers) > 0
+
+    def directions(self) -> List[LSTMLayer]:
+        """Every layer, forward and reverse of each depth in turn (the order of the averaged / flat parameter set)."""
+        if not self.bidirectional:
+            return list(self.layers)
+        return [l for pair in zip(self.layers, self.reverse_layers) for l in pair]
 
     def add_layers(self, settings: Iterable[dict]):
         for setting in settings:
@@ -38,14 +66,17 @@ class RNN(nn.Module):
 
     # --------------------------------------------------------------------------------------------
     def reset_state(self, batch_size: Optional[int] = None):
-        for layer in self.layers:
+        for layer in self.directions():
             layer.reset_state(batch_size)
 
     def fit_layers(self, input_data: torch.Tensor, train: bool = True, lengths: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """``[B,D]``: one step per layer (reference semantics, rnn.py:38-42; ``lengths`` is ignored).
+        """``[B,D]``: one step per layer (reference semantics, rnn.py:38-42; ``lengths`` is ignored; not bidirectional).
         ``[B,T,D]``: full unroll; returns the last layer's h at the last step, ``[B,H_last]`` - with ``lengths`` (int32 ``[B]``,
-        right padding) at each row's own last step."""
+        right padding) at each row's own last step.  Bidirectional: ``[h_fwd_final | h_rev_final]``, ``[B, 2 H_last]``, the
+        reverse half being the state after step 0."""
         if input_data.dim() == 2:
+            if self.bidirectional:
+                raise ValueError("a bidirectional stack needs whole sequences [B,T,D]: the one-step [B,D] path runs forward only")
             state = input_data
             for layer in self.layers:
                 state = layer.fit_next(state, train=train)
@@ -53,16 +84,25 @@ class RNN(nn.Module):
         if input_data.dim() != 3:
             raise ValueError(f"expected [B,D] or [B,T,D], got {tuple(input_data.shape)}")
         self._run_stack(input_data.transpose(0, 1), lengths)  # time-major [T,B,D]; the kernels index (t, b)
+        if self.bidirectional:
+            return torch.cat([self.layers[-1].ht, self.reverse_layers[-1].ht], 1)
         return self.layers[-1].ht                   # = seq[-1], as a separate autograd edge (no [T,B,H] gradient for the top layer)
 
     def fit_sequence_all(self, input_data: torch.Tensor, lengths: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """``[B,T,D]`` -> last layer's full ``h_seq [T,B,H]`` (padded positions hold the carried state)."""
+        """``[B,T,D]`` -> last layer's full ``h_seq [T,B,H]`` (padded positions hold the carried state); bidirectional:
+        ``[T,B,2H]``, forward half first."""
         return self._run_stack(input_data.transpose(0, 1), lengths)
 
     def _run_stack(self, seq: torch.Tensor, lengths: Optional[torch.Tensor] = None) -> torch.Tensor:
         """Layers bottom-up; adjacent pairs run as ONE layer-wavefront op where the GPU path supports it (both recurrences
-        co-resident, the upper layer trailing by a couple of time steps), single layers otherwise."""
+        co-resident, the upper layer trailing by a couple of time steps), single layers otherwise.  Bidirectional: both
+        directions of a layer run one after the other on the same input, and their outputs are joined into ``[T,B,2H]``
+        (one concatenation) for the next layer; no wavefront."""
         from ...ops import functional as F
+        if self.bidirectional:
+            for la, lr in zip(self.layers, self.reverse_layers):
+                seq = torch.cat([la.fit_sequence(seq, lengths), lr.fit_sequence(seq, lengths)], 2)
+            return seq
         i, n = 0, len(self.layers)
         while i < n:
             la = self.layers[i]
@@ -87,7 +127,7 @@ class RNN(nn.Module):
         """The record set that is averaged across partitions (reference rnn.py:14-36): 8 ``(key, list)``
         pairs; ``w*`` -> per layer ``[W_h [H,H], W_x [D,H]]``; ``b*`` -> per layer ``[H]``."""
         rec: Dict[str, list] = {k: [] for k in EXPORT_KEYS}
-        for layer in self.layers:
+        for layer in self.directions():
             rec["wf"].append(layer.weight_forget)
             rec["wi"].append(layer.weight_input)
             rec["wo"].append(layer.weight_output)
@@ -101,6 +141,6 @@ class RNN(nn.Module):
     def averaged_parameters(self) -> List[nn.Parameter]:
         """The same set as ``map_data_by_key`` in fused storage (what the allreduce kernel touches)."""
         out = []
-        for layer in self.layers:
+        for layer in self.directions():
             out += [layer.w_x, layer.w_h, layer.bias]
         return out

@@ -294,7 +294,7 @@ def _check_lengths_arg(lengths: Optional[torch.Tensor], B: int, device) -> None:
 
 class _LSTMSeqFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x_seq, h0, c0, w_x, w_h, bias, lengths=None):
+    def forward(ctx, x_seq, h0, c0, w_x, w_h, bias, lengths=None, reverse=False):
         E = ext()
         T, B, D = x_seq.shape
         H = w_h.shape[1]
@@ -309,22 +309,24 @@ class _LSTMSeqFn(torch.autograd.Function):
         h0c = h0.detach().to(cd).contiguous()
         if fast:
             h_seq, c_seq, act = E.lstm_seq_fwd(gx, w_h_c, bias_f, h0c, c0f, _sync_ws(x_seq.device), _seq_variant(B, H, x_seq.device),
-                                               lengths=lengths)
+                                               lengths=lengths, reverse=reverse)
             STATS["fast_fwd"] += 1
             STATS["kernels"] += 1
         else:
             h_seq = torch.empty(T + 1, B, H, dtype=cd, device=x_seq.device)
             c_seq = torch.empty(T + 1, B, H, dtype=torch.float32, device=x_seq.device)
             act = torch.empty(T, B, 4 * H, dtype=cd, device=x_seq.device)
-            h_seq[0].copy_(h0c)
-            c_seq[0].copy_(c0f)
+            s0 = T if reverse else 0                                      # state row of h0 / c0 (see lstm_layer_sequence)
+            h_seq[s0].copy_(h0c)
+            c_seq[s0].copy_(c0f)
             pre = torch.empty(B, 4 * H, dtype=cd, device=x_seq.device)
-            for t in range(T):
+            for t in (range(T - 1, -1, -1) if reverse else range(T)):
+                sp, sn = (t + 1, t) if reverse else (t, t + 1)            # state rows before / after step t
                 pre.copy_(gx[t])
-                G.matmul(h_seq[t], w_h_c, out=pre, accumulate=True)       # pre = gx[t] + h_{t-1} W_h^T
-                h, c, a = E.lstm_pointwise_fwd(pre, bias_f, c_seq[t], h_seq[t], lengths, t)
-                h_seq[t + 1].copy_(h)
-                c_seq[t + 1].copy_(c)
+                G.matmul(h_seq[sp], w_h_c, out=pre, accumulate=True)      # pre = gx[t] + h_prev W_h^T
+                h, c, a = E.lstm_pointwise_fwd(pre, bias_f, c_seq[sp], h_seq[sp], lengths, t)
+                h_seq[sn].copy_(h)
+                c_seq[sn].copy_(c)
                 act[t].copy_(a)
             STATS["generic_fwd"] += 1
             STATS["kernels"] += T
@@ -332,12 +334,15 @@ class _LSTMSeqFn(torch.autograd.Function):
         ctx.set_materialize_grads(False)       # an unused output must arrive as None, not as a zero-filled [T,B,H] tensor
         ctx.fast = fast
         ctx.lengths = lengths
+        ctx.reverse = reverse
         ctx.whole_batch = not _CHUNKING["on"]
         ctx.dims = (T, B, D, H)
         ctx.w_addrs = (w_x.data_ptr(), w_h.data_ptr(), bias.data_ptr())
         ctx.in_dtypes = (h0.dtype, c0.dtype)
         # h_T is its own output (not a slice of the first one taken by the caller): a consumer of the final state only - the
         # classifier on top of the stack - then sends back a [B,H] gradient instead of a zero-filled [T,B,H] one
+        if reverse:
+            return h_seq[:T], h_seq[0], c_seq[0]
         return h_seq[1:], h_seq[T], c_seq[T]
 
     @staticmethod
@@ -357,7 +362,7 @@ class _LSTMSeqFn(torch.autograd.Function):
             w_hT = _transposed(w_h_c)
             _big_launch_begin()
             dpre, dh0, dc0 = E.lstm_seq_bwd(dh_seq, w_hT, act, c_seq, dhT, dcT, _sync_ws(dev), _seq_variant(B, H, dev),
-                                            lengths=ctx.lengths)
+                                            lengths=ctx.lengths, reverse=ctx.reverse)
             STATS["fast_bwd"] += 1
             STATS["kernels"] += 1
             _after_big_launch()                  # finished gradient buckets of the layers above: sync them under this recurrence
@@ -365,12 +370,13 @@ class _LSTMSeqFn(torch.autograd.Function):
             dpre = torch.empty_like(act)
             dh_rec: Optional[torch.Tensor] = dhT if dh_T is not None else None
             dc = dcT
-            for t in range(T - 1, -1, -1):
+            for t in (range(T) if ctx.reverse else range(T - 1, -1, -1)):
+                sp, sn = (t + 1, t) if ctx.reverse else (t, t + 1)
                 if ctx.lengths is None:
-                    dp, dc = E.lstm_pointwise_bwd(dh_seq[t], dh_rec, dc, act[t], c_seq[t], c_seq[t + 1])
+                    dp, dc = E.lstm_pointwise_bwd(dh_seq[t], dh_rec, dc, act[t], c_seq[sp], c_seq[sn])
                     dh_rec = _mm_f32(dp, w_h_c)
                 else:                            # padded rows hand their dh on directly (dh_pass), the others through W_h
-                    dp, dc, dh_pass = E.lstm_pointwise_bwd(dh_seq[t], dh_rec, dc, act[t], c_seq[t], c_seq[t + 1], ctx.lengths, t)
+                    dp, dc, dh_pass = E.lstm_pointwise_bwd(dh_seq[t], dh_rec, dc, act[t], c_seq[sp], c_seq[sn], ctx.lengths, t)
                     G.matmul(dp, w_h_c.t(), out=dh_pass, accumulate=True)
                     dh_rec = dh_pass
                 dpre[t].copy_(dp)
@@ -380,19 +386,21 @@ class _LSTMSeqFn(torch.autograd.Function):
         dg2d = dpre.view(T * B, 4 * H)
         dg_t = dg2d.t()
         dw_x = _accumulate_grad(ctx.w_addrs[0], dg_t, x2d)
-        dw_h = _accumulate_grad(ctx.w_addrs[1], dg_t, h_seq[:T].reshape(T * B, H))
+        h_prev = h_seq[1:] if ctx.reverse else h_seq[:T]          # the h each step's dG pairs with
+        dw_h = _accumulate_grad(ctx.w_addrs[1], dg_t, h_prev.reshape(T * B, H))
         db = _bias_grad(ctx.w_addrs[2], dg2d)
         dx = None
         if ctx.needs_input_grad[0]:
             dx = G.matmul(dg2d, w_x_c.t(), out_dtype=cd).view(T, B, D)        # dG · W_x: W_x read in place as an MN-major operand
             STATS["kernels"] += 1
         h0_dt, c0_dt = ctx.in_dtypes
-        return dx, dh0.to(h0_dt), dc0.to(c0_dt), dw_x, dw_h, db, None
+        return dx, dh0.to(h0_dt), dc0.to(c0_dt), dw_x, dw_h, db, None, None
 
 
-def lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths=None):
+def lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths=None, reverse=False):
     """``x_seq [T,B,D]`` (bf16 or fp32) -> ``(h_seq [T,B,H], h_T, c_T)``.  ``lengths``: optional int32 ``[B]`` on the batch's
-    device, right padding (``ops/reference.py``); the persistent kernels then run their masked instantiations."""
+    device, right padding (``ops/reference.py``); the persistent kernels then run their masked instantiations.  ``reverse``:
+    the reverse-time direction (time T-1 down to 0; ``h_T`` / ``c_T`` are then the state after time 0)."""
     if (not x_seq.is_contiguous() and not x_seq.requires_grad and x_seq.transpose(0, 1).is_contiguous()
             and (x_seq.shape[2] * x_seq.element_size()) % 16 == 0):
         x_seq = ext().transpose01(x_seq.transpose(0, 1))     # batch-major feed -> time-major, a row permutation at copy speed
@@ -407,14 +415,14 @@ def lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths=None):
         _CHUNKING["on"] = True
         try:
             outs = [_LSTMSeqFn.apply(x_seq[:, b0:b0 + chunk].contiguous(), h0[b0:b0 + chunk], c0[b0:b0 + chunk], w_x, w_h, bias,
-                                     None if lengths is None else lengths[b0:b0 + chunk])
+                                     None if lengths is None else lengths[b0:b0 + chunk], reverse)
                     for b0 in range(0, B, chunk)]
         finally:
             _CHUNKING["on"] = False
         STATS["batch_chunks"] = STATS.get("batch_chunks", 0) + len(outs)
         return (torch.cat([o[0] for o in outs], dim=1), torch.cat([o[1] for o in outs], dim=0),
                 torch.cat([o[2] for o in outs], dim=0))
-    return _LSTMSeqFn.apply(x_seq.contiguous(), h0, c0, w_x, w_h, bias, lengths)
+    return _LSTMSeqFn.apply(x_seq.contiguous(), h0, c0, w_x, w_h, bias, lengths, reverse)
 
 
 # =====================================================================================================================

@@ -42,12 +42,13 @@ def lstm_cell_step(x, h, c, w_x, w_h, bias):
     return ref.lstm_cell_step(x, h, c, w_x, w_h, bias)
 
 
-def lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths=None):
-    """``lengths``: optional int32 ``[B]`` per-row sequence lengths (right padding, see ``reference.lstm_layer_sequence``)."""
+def lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths=None, reverse=False):
+    """``lengths``: optional int32 ``[B]`` per-row sequence lengths (right padding, see ``reference.lstm_layer_sequence``).
+    ``reverse``: the reverse-time direction of a bidirectional layer (same reference)."""
     if _use_ext(x_seq):
         from . import cuda_lstm
-        return cuda_lstm.lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths=lengths)
-    return ref.lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths=lengths)
+        return cuda_lstm.lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths=lengths, reverse=reverse)
+    return ref.lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths=lengths, reverse=reverse)
 
 
 def head_xent(h, weights, bias, labels):

@@ -49,12 +49,17 @@ def check_lengths(lengths: torch.Tensor, B: int, T: int) -> None:
         raise ValueError(f"lengths must lie in [1, {T}], got [{lo}, {hi}]")
 
 
-def lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths: Optional[torch.Tensor] = None):
+def lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths: Optional[torch.Tensor] = None, reverse: bool = False):
     """Unrolled layer: ``x_seq [T,B,D]`` -> ``(h_seq [T,B,H], h_T, c_T)``.
 
     ``lengths`` (int32 ``[B]``, right padding): at a step ``t >= lengths[b]`` row ``b`` holds its state (``h_t = h_{t-1}``,
     ``c_t = c_{t-1}``), so ``h_T`` / ``c_T`` are the state after the row's last real step - ``h_n`` / ``c_n`` of ``nn.LSTM`` on
-    a packed sequence - and padded inputs get no gradient."""
+    a packed sequence - and padded inputs get no gradient.
+
+    ``reverse``: the reverse-time direction of a bidirectional layer.  Steps run from ``t = T-1`` down to 0, ``h_seq[t]`` is the
+    state after step ``t`` (still in time order) and ``h_T`` / ``c_T`` are the state after step 0.  With ``lengths`` the padded
+    steps come first and hold ``h0`` / ``c0``, so each row starts from ``h0`` at its own last real step - the reverse half of
+    ``nn.LSTM(bidirectional=True)`` on a packed sequence."""
     T = x_seq.shape[0]
     keep = None
     if lengths is not None:
@@ -64,7 +69,7 @@ def lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths: Optional[torch.T
     outs = []
     # hoisted input projection (same arithmetic as per-step x·W_x)
     gx = (x_seq.reshape(-1, x_seq.shape[-1]) @ w_x.t()).view(T, x_seq.shape[1], -1)
-    for t in range(T):
+    for t in (range(T - 1, -1, -1) if reverse else range(T)):
         pre = gx[t] + h @ w_h.t() + bias
         i, f, g, o = lstm_gates(pre)
         c_new = f * c + i * g
@@ -75,6 +80,8 @@ def lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths: Optional[torch.T
             k = keep[:, t:t + 1]
             c, h = torch.where(k, c_new, c), torch.where(k, h_new, h)
         outs.append(h)
+    if reverse:
+        outs.reverse()
     return torch.stack(outs, 0), h, c
 
 

@@ -146,6 +146,7 @@ def train_rnn(partition, cfg: Config, rank: int = 0, world_size: int = 1, comm: 
             src = ckpt.latest_checkpoint(src)
         if src:
             variables, meta, opt_state = ckpt.load(src)
+            model.check_directions(variables, f"checkpoint {src}")
             model.load_reference_state_dict(variables, strict=False)
             eng.flat.refresh_shadow()
             if opt_state is not None:
@@ -399,6 +400,7 @@ def evaluate_job(cfg: Config, standalone: bool = False) -> Dict:
     # scoring with another batch size uses the mean learned row for every sample
     shapes = {k: tuple(v.shape) for k, v in eng.model.named_reference_variables()}
     variables = dict(variables)
+    eng.model.check_directions(variables, f"model {src}")
     for k, v in list(variables.items()):
         want = shapes.get(k)
         if want is not None and tuple(v.shape) != want and v.dim() == 2 and len(want) == 2 and v.shape[1] == want[1]:
