@@ -20,7 +20,7 @@ int ts_lstm_pointwise_fwd(const void*, const float*, const float*, void*, float*
 int ts_transpose01_rows(const void*, void*, int, int, long long, cudaStream_t);
 int ts_lstm_seq_cluster_probe(int);
 int ts_transpose2d_b16(const void*, void*, int, int, cudaStream_t);
-int ts_colsum_bf16(const void*, float*, void*, int, int, int, int, int, cudaStream_t);
+int ts_colsum_bf16(const void*, float*, void*, int, int, int, int, int, int, cudaStream_t);
 long long ts_colsum_scratch_bytes(int, int);
 int ts_lstm_pointwise_bwd(const void*, const float*, const float*, const void*, const float*, const float*, void*,
                           float*, int, int, int, cudaStream_t, const int*, int, float*);
@@ -129,13 +129,14 @@ Tensor colsum_bf16(const Tensor& x) {
   TORCH_CHECK(x.dim() == 2 && x.is_contiguous() && is_bf16(x) && x.size(1) % 256 == 0, "colsum_bf16: contiguous bf16 [rows, cols], cols % 256 == 0");
   c10::cuda::CUDAGuard g(x.device());
   auto out = torch::empty({x.size(1)}, x.options().dtype(torch::kFloat32));
-  check(ts_colsum_bf16(x.data_ptr(), out.data_ptr<float>(), colsum_scratch(x), (int)x.size(0), (int)x.size(1), (int)x.size(1), 0, 0, stream()), "colsum_bf16");
+  check(ts_colsum_bf16(x.data_ptr(), out.data_ptr<float>(), colsum_scratch(x), (int)x.size(0), (int)x.size(1), (int)x.size(1), 0, 0, 0, stream()), "colsum_bf16");
   return out;
 }
 
 // column sums written (overwrite) or accumulated into an existing fp32 [cols] tensor; pdl: launch as a programmatic dependent of
-// the previous kernel of the stream (a weight-gradient GEMM that reads the same matrix and leaves SMs idle)
-void colsum_bf16_into(const Tensor& x, Tensor out, bool overwrite, bool pdl, int64_t col0, int64_t ncols) {
+// the previous kernel of the stream (a weight-gradient GEMM that reads the same matrix and leaves SMs idle); max_ctas > 0 caps
+// the grid (the same sums, computed by fewer CTAs)
+void colsum_bf16_into(const Tensor& x, Tensor out, bool overwrite, bool pdl, int64_t col0, int64_t ncols, int64_t max_ctas) {
   chk_cuda(x, "x"); chk_cuda(out, "out");
   TORCH_CHECK(x.dim() == 2 && is_bf16(x) && x.size(1) % 256 == 0 && out.scalar_type() == torch::kFloat32 && out.numel() == x.size(1),
               "colsum_bf16_into: bf16 [rows, cols % 256 == 0] -> fp32 [cols]");
@@ -143,7 +144,7 @@ void colsum_bf16_into(const Tensor& x, Tensor out, bool overwrite, bool pdl, int
   TORCH_CHECK(col0 % 256 == 0 && ncols % 256 == 0 && col0 + ncols <= x.size(1), "colsum_bf16_into: 256-aligned column range");
   c10::cuda::CUDAGuard g(x.device());
   check(ts_colsum_bf16((const char*)x.data_ptr() + 2 * col0, out.data_ptr<float>() + col0, colsum_scratch(x), (int)x.size(0), (int)ncols,
-                       (int)x.size(1), overwrite ? 0 : 1, pdl ? 1 : 0, stream()), "colsum_bf16_into");
+                       (int)x.size(1), overwrite ? 0 : 1, pdl ? 1 : 0, (int)max_ctas, stream()), "colsum_bf16_into");
 }
 
 // ---- generic LSTM cell epilogue -------------------------------------------------------------------------
@@ -476,7 +477,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("transpose2d", &transpose2d);
   m.def("colsum_bf16", &colsum_bf16);
   m.def("colsum_bf16_into", &colsum_bf16_into, py::arg("x"), py::arg("out"), py::arg("overwrite"), py::arg("pdl") = false,
-        py::arg("col0") = 0, py::arg("ncols") = 0);
+        py::arg("col0") = 0, py::arg("ncols") = 0, py::arg("max_ctas") = 0);
   m.def("lstm_seq_cluster_probe", [](int64_t c) { return ts_lstm_seq_cluster_probe((int)c); });
   m.def("lstm_pointwise_bwd", &lstm_pointwise_bwd, py::arg("dh_a"), py::arg("dh_b"), py::arg("dc_in"), py::arg("act"), py::arg("c_prev"),
         py::arg("c_new"), py::arg("lengths") = py::none(), py::arg("t") = 0);

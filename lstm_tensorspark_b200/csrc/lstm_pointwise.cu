@@ -195,52 +195,58 @@ extern "C" int ts_transpose2d_b16(const void* src, void* dst, int R, int C, cuda
 // 8 fp32 accumulators per thread, warps stride over rows, one shared-memory reduction and one atomicAdd per column per block.
 // cols % 256 == 0.  Deterministic: every row slab writes its partial sums to a scratch row, the LAST slab to finish (ticket
 // counter per column block) adds the slabs in fixed order and accumulates the result into out (beta = 1).
+// The work is a grid of nx = cols / 256 column blocks x ny row slabs; a launch with fewer CTAs than that walks it in a
+// grid-stride loop (same slabs, same order of additions: the result does not depend on the CTA count).
 namespace {
 __global__ void colsum_bf16_kernel(const uint4* __restrict__ src, float* __restrict__ out, float* __restrict__ partial,
                                    unsigned int* __restrict__ tickets, int rows, int cols, int rows_per_block, int accumulate, int pdl,
-                                   int pitch_cols) {
+                                   int pitch_cols, int nx, int ny) {
   __shared__ float red[8][256];
   __shared__ unsigned int ticket_s;
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int cv = blockIdx.x * 32 + lane;                       // 16 B column-vector index (8 columns)
   const int vec_per_row = pitch_cols / 8;                      // (src / out already point at the first column of this launch)
-  const int r_begin = blockIdx.y * rows_per_block;
-  const int r_end = min(rows, r_begin + rows_per_block);
-  float acc[8];
+  for (int vb = blockIdx.x; vb < nx * ny; vb += gridDim.x) {
+    const int bx = vb % nx, by = vb / nx;
+    const int cv = bx * 32 + lane;                             // 16 B column-vector index (8 columns)
+    const int r_begin = by * rows_per_block;
+    const int r_end = min(rows, r_begin + rows_per_block);
+    float acc[8];
 #pragma unroll
-  for (int i = 0; i < 8; ++i) acc[i] = 0.f;
-  for (int r = r_begin + warp; r < r_end; r += 8) {
-    const uint4 v = src[(size_t)r * vec_per_row + cv];
-    const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+    for (int i = 0; i < 8; ++i) acc[i] = 0.f;
+    for (int r = r_begin + warp; r < r_end; r += 8) {
+      const uint4 v = src[(size_t)r * vec_per_row + cv];
+      const uint32_t w[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      acc[2 * i] += __uint_as_float(w[i] << 16);
-      acc[2 * i + 1] += __uint_as_float(w[i] & 0xffff0000u);
+      for (int i = 0; i < 4; ++i) {
+        acc[2 * i] += __uint_as_float(w[i] << 16);
+        acc[2 * i + 1] += __uint_as_float(w[i] & 0xffff0000u);
+      }
     }
-  }
 #pragma unroll
-  for (int i = 0; i < 8; ++i) red[warp][lane * 8 + i] = acc[i];
-  __syncthreads();
-  float s = 0.f;
+    for (int i = 0; i < 8; ++i) red[warp][lane * 8 + i] = acc[i];
+    __syncthreads();
+    float s = 0.f;
 #pragma unroll
-  for (int w = 0; w < 8; ++w) s += red[w][threadIdx.x];
-  const int col = blockIdx.x * 256 + threadIdx.x;
-  if (gridDim.y == 1) {
-    out[col] = accumulate ? out[col] + s : s;
-  } else {
-    partial[(size_t)blockIdx.y * cols + col] = s;
-    __threadfence();
-    __syncthreads();
-    if (threadIdx.x == 0) ticket_s = atomicAdd(tickets + blockIdx.x, 1u);
-    __syncthreads();
-    if (ticket_s == gridDim.y - 1) {
+    for (int w = 0; w < 8; ++w) s += red[w][threadIdx.x];
+    const int col = bx * 256 + threadIdx.x;
+    if (ny == 1) {
+      out[col] = accumulate ? out[col] + s : s;
+    } else {
+      partial[(size_t)by * cols + col] = s;
       __threadfence();
-      float t = 0.f;
-      for (unsigned int y = 0; y < gridDim.y; ++y) t += __ldcg(partial + (size_t)y * cols + col);     // fixed order
-      out[col] = accumulate ? out[col] + t : t;
-      if (threadIdx.x == 0) tickets[blockIdx.x] = 0u;            // ready for the next launch
+      __syncthreads();
+      if (threadIdx.x == 0) ticket_s = atomicAdd(tickets + bx, 1u);
+      __syncthreads();
+      if (ticket_s == (unsigned int)ny - 1) {
+        __threadfence();
+        float t = 0.f;
+        for (int y = 0; y < ny; ++y) t += __ldcg(partial + (size_t)y * cols + col);     // fixed order
+        out[col] = accumulate ? out[col] + t : t;
+        if (threadIdx.x == 0) tickets[bx] = 0u;                  // ready for the next launch
+      }
     }
+    __syncthreads();                                             // red / ticket_s are reused by the next work item
   }
   // launched as a programmatic dependent of a weight-gradient GEMM (it runs on the SMs that GEMM leaves idle and reads the same
   // dG): do not let anything behind us start before that GEMM has completed
@@ -258,19 +264,24 @@ extern "C" long long ts_colsum_scratch_bytes(int rows, int cols) {
 }
 
 // cols = columns summed by this launch (a 256-aligned sub-range of a matrix with row pitch pitch_cols; src / out point at its first column)
+// max_ctas > 0 caps the grid: a programmatic dependent that runs next to kernels holding most SMs then gets all of its CTAs
+// resident on the SMs left to it (a CTA that has finished waits for the previous kernel before it exits, so CTAs that do not
+// fit would only start once that kernel is complete).
 extern "C" int ts_colsum_bf16(const void* src, float* out, void* scratch, int rows, int cols, int pitch_cols, int accumulate, int pdl,
-                              cudaStream_t st) {
+                              int max_ctas, cudaStream_t st) {
   if (cols % 256 != 0 || cols / 256 > kColsumTickets) return -2;
   const int rows_per_block = 512;
-  dim3 grid(cols / 256, (rows + rows_per_block - 1) / rows_per_block);
+  const int nx = cols / 256, ny = (rows + rows_per_block - 1) / rows_per_block;
+  int grid = nx * ny;
+  if (max_ctas > 0 && max_ctas < grid) grid = max_ctas;
   unsigned int* tickets = (unsigned int*)scratch;
   float* partial = (float*)((char*)scratch + (size_t)kColsumTickets * 4);
   cudaLaunchConfig_t cfg{};
-  cfg.gridDim = grid; cfg.blockDim = dim3(256); cfg.dynamicSmemBytes = 0; cfg.stream = st;
+  cfg.gridDim = dim3(grid); cfg.blockDim = dim3(256); cfg.dynamicSmemBytes = 0; cfg.stream = st;
   cudaLaunchAttribute at[1];
   at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   at[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = at; cfg.numAttrs = pdl ? 1 : 0;
   return (int)cudaLaunchKernelEx(&cfg, colsum_bf16_kernel, (const uint4*)src, out, partial, tickets, rows, cols, rows_per_block, accumulate, pdl,
-                                 pitch_cols);
+                                 pitch_cols, nx, ny);
 }

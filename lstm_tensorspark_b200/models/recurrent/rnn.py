@@ -94,8 +94,9 @@ class RNN(nn.Module):
         return self._run_stack(input_data.transpose(0, 1), lengths)
 
     def _run_stack(self, seq: torch.Tensor, lengths: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """Layers bottom-up; adjacent pairs run as ONE layer-wavefront op where the GPU path supports it (both recurrences
-        co-resident, the upper layer trailing by a couple of time steps), single layers otherwise.  Bidirectional: both
+        """Layers bottom-up; adjacent pairs run as ONE op where the GPU path supports it (``cuda_lstm.pair_schedule``: a layer
+        wavefront with both recurrences co-resident, or, where they do not fit side by side, the recurrences one after the other
+        with the upper layer's GEMMs next to them), single layers otherwise.  Bidirectional: both
         directions of a layer run one after the other on the same input, and their outputs are joined into ``[T,B,2H]``
         (one concatenation) for the next layer; no wavefront."""
         from ...ops import functional as F

@@ -52,13 +52,18 @@ def folded_ok(x_bm: torch.Tensor) -> bool:
 
 def matmul(a: Optional[torch.Tensor], b_t: Optional[torch.Tensor], out: Optional[torch.Tensor] = None, accumulate: bool = False,
            out_dtype: Optional[torch.dtype] = None, bias: Optional[torch.Tensor] = None, max_ctas: int = 0,
-           a_folded: Optional[torch.Tensor] = None, b_folded: Optional[torch.Tensor] = None) -> torch.Tensor:
+           a_folded: Optional[torch.Tensor] = None, b_folded: Optional[torch.Tensor] = None, pdl: bool = False,
+           ctas: int = 0) -> torch.Tensor:
     """``a [M,K] @ b_t[N,K]^T`` (+ bias[N]); either operand may be a transposed view (then it is MN-major and is read in
     place).  ``out`` fp32 + ``accumulate`` -> ``out += a @ b_t^T``.
 
     ``a_folded`` / ``b_folded`` (instead of ``a`` / ``b_t``): a batch-major ``[B, T, F]`` array (``folded_ok``) standing for the
-    time-major matrix ``X = [T*B, F]``: ``a = X`` resp. ``b_t = X^T``."""
+    time-major matrix ``X = [T*B, F]``: ``a = X`` resp. ``b_t = X^T``.
+
+    ``pdl``: programmatic dependent launch of the tensor-core GEMM (it starts once every CTA of the previous kernel is resident
+    and waits for that kernel before it exits).  ``ctas``: CTAs per tile cluster, 1 or 2 (0 = ``LSTM_TS_GEMM_CTAS``)."""
     E = ext()
+    ctas = ctas or GEMM_CTAS
     if a_folded is not None or b_folded is not None:
         xb = a_folded if a_folded is not None else b_folded
         Bsz, T, F = xb.shape
@@ -70,10 +75,10 @@ def matmul(a: Optional[torch.Tensor], b_t: Optional[torch.Tensor], out: Optional
         STATS["tc"] += 1
         if a_folded is not None:
             return E.gemm2(store, other[1], bias=bias, out=out, a_mn=False, b_mn=other[0], out_fp32=out_dtype == torch.float32,
-                           accumulate=accumulate, ctas=GEMM_CTAS, bn=GEMM_BN if b_t.shape[0] > 128 else 128, max_ctas=max_ctas,
+                           accumulate=accumulate, ctas=ctas, bn=GEMM_BN if b_t.shape[0] > 128 else 128, max_ctas=max_ctas, pdl=pdl,
                            a_fold=Bsz, fold_cols=F)
         return E.gemm2(other[1], store, bias=bias, out=out, a_mn=other[0], b_mn=True, out_fp32=out_dtype == torch.float32,
-                       accumulate=accumulate, ctas=GEMM_CTAS, bn=GEMM_BN, max_ctas=max_ctas, b_fold=Bsz, fold_cols=F)
+                       accumulate=accumulate, ctas=ctas, bn=GEMM_BN, max_ctas=max_ctas, pdl=pdl, b_fold=Bsz, fold_cols=F)
     M, K = a.shape
     N = b_t.shape[0]
     assert b_t.shape[1] == K, (a.shape, b_t.shape)
@@ -85,7 +90,7 @@ def matmul(a: Optional[torch.Tensor], b_t: Optional[torch.Tensor], out: Optional
             and (out is None or (out.stride(1) == 1 and out.stride(0) % 4 == 0 and out.data_ptr() % 16 == 0)):
         STATS["tc"] += 1
         return E.gemm2(ma[1], mb[1], bias=bias, out=out, a_mn=ma[0], b_mn=mb[0], out_fp32=out_dtype == torch.float32,
-                       accumulate=accumulate, ctas=GEMM_CTAS, bn=GEMM_BN if N > 128 else 128, max_ctas=max_ctas)
+                       accumulate=accumulate, ctas=ctas, bn=GEMM_BN if N > 128 else 128, max_ctas=max_ctas, pdl=pdl)
     assert a_folded is None and b_folded is None, "folded operands need the tensor-core path (check folded_ok first)"
     STATS["generic"] += 1
     a_g = a if a.dtype in (torch.float32, torch.bfloat16) else a.float()

@@ -105,17 +105,25 @@ def grad_sink(w_addr: int):
     return ent[1], owner.take_sink(w_addr)
 
 
-def _accumulate_grad(w_addr: int, a_t: torch.Tensor, b: torch.Tensor, b_folded: bool = False):
+def _accumulate_grad(w_addr: int, a_t: torch.Tensor, b: torch.Tensor, b_folded: bool = False, pdl: bool = False,
+                     max_ctas: int = 0):
     """dW = a_t @ b in fp32 (``a_t`` = dG^T as a transposed view, ``b`` = the layer input: both operands MN-major, read in
     place by the wgmma GEMM; ``b_folded``: ``b`` is the batch-major [B,T,D] array standing for the time-major [T*B, D]
     matrix).  When the parameter lives in a FlatParams buffer the product lands straight in its grad
-    view (overwrite on the first write of a step, accumulate afterwards) and None is returned to autograd."""
+    view (overwrite on the first write of a step, accumulate afterwards) and None is returned to autograd.
+    ``pdl``: launch as a programmatic dependent of the previous kernel (single-CTA tiles on at most ``max_ctas`` SMs, next to a
+    recurrence that is still running).  Such a GEMM is no "big launch" for the gradient buckets: what precedes it in the stream
+    may still be running when it starts, so no bucket's allreduce is launched under it."""
     ops = dict(a=a_t, b_t=None, b_folded=b) if b_folded else dict(a=a_t, b_t=b.t())
+    if pdl:
+        ops.update(pdl=True, ctas=1, max_ctas=max_ctas)
     sink = grad_sink(w_addr)
     if sink is not None:
-        _big_launch_begin()
+        if not pdl:
+            _big_launch_begin()
         G.matmul(out=sink[0], accumulate=sink[1], **ops)
-        _after_big_launch()                  # finished buckets of earlier gradients: allreduce them under this GEMM
+        if not pdl:
+            _after_big_launch()              # finished buckets of earlier gradients: allreduce them under this GEMM
         _grads_written()
         return None
     return G.matmul(out_dtype=torch.float32, **ops)
@@ -124,11 +132,12 @@ def _accumulate_grad(w_addr: int, a_t: torch.Tensor, b: torch.Tensor, b_folded: 
 _BIAS_SPLIT = {}
 
 
-def _bias_grad(b_addr: int, dg2d: torch.Tensor, under_gemm: bool = False, part: int = -1):
+def _bias_grad(b_addr: int, dg2d: torch.Tensor, under_gemm: bool = False, part: int = -1, max_ctas: int = 0):
     """db = column sums of dG; straight into the flat grad view when there is one.  ``under_gemm``: the previous launch of the
     stream is a weight-gradient GEMM over the same dG that leaves SMs idle - run next to it (programmatic dependent launch).
     ``part`` 0 / 1: only the first / second half of the columns (one half under each of the layer's two weight-gradient GEMMs:
-    on the ~20 idle SMs a half takes about as long as the GEMM it hides under); the value for autograd comes from part 1."""
+    on the ~20 idle SMs a half takes about as long as the GEMM it hides under); the value for autograd comes from part 1.
+    ``max_ctas`` (whole-column launches): at most that many CTAs, each walking several slabs (the same sums)."""
     fast = dg2d.is_cuda and dg2d.dtype == torch.bfloat16 and dg2d.shape[1] % 512 == 0 and dg2d.is_contiguous()
     if part == 0:
         if not fast:
@@ -155,7 +164,7 @@ def _bias_grad(b_addr: int, dg2d: torch.Tensor, under_gemm: bool = False, part: 
     if fast:
         STATS["kernels"] += 1
         if sink is not None:
-            ext().colsum_bf16_into(dg2d, sink[0], not sink[1], under_gemm and part < 0)
+            ext().colsum_bf16_into(dg2d, sink[0], not sink[1], under_gemm and part < 0, max_ctas=max_ctas)
             _grads_written()
             return None
         return ext().colsum_bf16(dg2d)
@@ -432,6 +441,10 @@ def lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths=None, reverse=Fal
 #     backward:  L_b step t  ->  dh_a[t] = dG_b[t] W_xb  (gated GEMM)  ->  L_a step t
 # The reference stacks layers strictly one after the other (original src/models/recurrent/rnn.py:38-42); here layer l+1
 # trails layer l by a couple of time steps and the next layer's input projection leaves the critical path altogether.
+# Where both recurrences do not fit side by side (an H100 at H = 1024: 64 + 64 + 8 > 132 SMs), the pair is PIPELINED instead:
+# the recurrences run one after the other and the GEMMs that do not feed the running recurrence move onto the SMs it leaves idle
+#     forward :  L_a  || gx_b (gated)                    ->  L_b
+#     backward:  L_b  || dx_b (gated)                    ->  L_a  || dW_xb, dW_hb, db_b
 # =====================================================================================================================
 FOLDED_FEED = os.environ.get("LSTM_TS_FOLDED_FEED", "1") != "0"   # batch-major input read in place by the first layer's GEMMs
 WAVEFRONT = os.environ.get("LSTM_TS_WAVEFRONT", "1") == "1"
@@ -474,18 +487,38 @@ def _pair_ws(device, tag: str, n_done: int):
     return ent[:SYNC_WORDS], ent[SYNC_WORDS:2 * SYNC_WORDS], ent[2 * SYNC_WORDS:2 * SYNC_WORDS + n_done]
 
 
-def wavefront_supported(x_seq: torch.Tensor, h_a: int, h_b: int) -> bool:
-    """Two co-resident layers need: bf16 fast path, B = 256 (two batch tiles per CTA, one GEMM tile per time step), resident
-    weights (H <= 1024), 256-aligned widths, and 2 * H/16 CTAs + a few GEMM CTAs within the device."""
+def pair_schedule(T: int, B: int, D: int, h_a: int, h_b: int, sms: int, coresident: int) -> Optional[str]:
+    """How two stacked layers run as one op on a device with ``sms`` SMs, ``coresident`` of which hold backward-kernel CTAs in
+    clusters of 4 (``_coresident_ctas``).  Every recurrence runs two batch tiles per CTA, H/16 CTAs.  Both schedules need
+    B = 256 (one GEMM tile row per time step), resident weights (H <= 1024) and 256-aligned widths.
+      "wavefront": both recurrences co-resident, the gated GEMM on the SMs they leave free (H_a/16 + H_b/16 + 8 SMs).
+      "pipelined": the recurrences run one after the other; next to each runs a GEMM that does not feed it (forward: L_a with
+                   gx_b; backward: L_b with dx_b, then L_a with dW_xb, dW_hb and db_b).  Needs max(H)/16 + 8 SMs.
+      None: two separate layers."""
+    if B != 256 or T < 2 or D % 8 != 0 or any(h % 256 != 0 or h > 1024 for h in (h_a, h_b)):
+        return None
+    both = h_a // 16 + h_b // 16 + 8
+    if both <= coresident + 16 and both <= sms:
+        return "wavefront"
+    if max(h_a, h_b) // 16 <= coresident and max(h_a, h_b) // 16 + 8 <= sms:
+        return "pipelined"
+    return None
+
+
+def _pair_schedule_of(x_seq: torch.Tensor, h_a: int, h_b: int) -> Optional[str]:
+    """``pair_schedule`` for an input on its device; None off the bf16 fast path, with ``LSTM_TS_WAVEFRONT=0`` (serial layers,
+    for tools that serialise kernels) or with a tile-count override in ``LSTM_TS_SEQ_VARIANT``."""
     if not (WAVEFRONT and x_seq.is_cuda and x_seq.dtype == torch.bfloat16 and not FORCE_GENERIC and x_seq.dim() == 3):
-        return False
+        return None
+    if (SEQ_VARIANT & 15) > 2:
+        return None
     T, B, D = x_seq.shape
-    if B != 256 or T < 2 or D % 8 != 0 or (SEQ_VARIANT & 15) > 2:
-        return False
-    for h in (h_a, h_b):
-        if h % 256 != 0 or h > 1024:
-            return False
-    return h_a // 16 + h_b // 16 + 8 <= _coresident_ctas(x_seq.device) + 16 and h_a // 16 + h_b // 16 + 8 <= _sms(x_seq.device)
+    return pair_schedule(T, B, D, h_a, h_b, _sms(x_seq.device), _coresident_ctas(x_seq.device))
+
+
+def wavefront_supported(x_seq: torch.Tensor, h_a: int, h_b: int) -> bool:
+    """Can two stacked layers run as one pair op (``lstm_pair_sequence``, either schedule of ``pair_schedule``)?"""
+    return _pair_schedule_of(x_seq, h_a, h_b) is not None
 
 
 WAVE_SYNC_MODE = int(os.environ.get("LSTM_TS_WAVE_SYNC", "1"))      # 1: one arrival counter per batch tile (measured 2.5 % faster with two
@@ -494,6 +527,16 @@ WAVE_SYNC_MODE = int(os.environ.get("LSTM_TS_WAVE_SYNC", "1"))      # 1: one arr
 
 def _wave_variant() -> int:
     return (SEQ_VARIANT & ~(15 | (3 << 16))) | 2 | ((WAVE_SYNC_MODE & 1) << 16)
+
+
+_COLSUM_SMS = 4            # pipelined backward: SMs kept for layer b's bias column sums (4 CTAs of 256 threads each)
+
+
+def _pair_variant(schedule: str) -> int:
+    """Variant of the four recurrences of a layer pair.  Pipelined: per-k-block counters (sync mode 0), the layout a single
+    layer's recurrence uses; one counter per batch tile only pays off when two recurrences are co-resident."""
+    var = _wave_variant()
+    return var & ~(3 << 16) if schedule == "pipelined" else var
 
 
 def _gate_off(var: int) -> int:
@@ -513,8 +556,9 @@ def _gate_cfg(var: int, tiles_m: int, nkb: int, per_kb_step: int, ctas_per_tile:
 
 class _LSTMPairFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x_seq, h0a, c0a, w_xa, w_ha, b_a, h0b, c0b, w_xb, w_hb, b_b, lengths=None):
+    def forward(ctx, x_seq, h0a, c0a, w_xa, w_ha, b_a, h0b, c0b, w_xb, w_hb, b_b, lengths=None, schedule="wavefront"):
         E = ext()
+        pipelined = schedule == "pipelined"
         dev = x_seq.device
         T, B, D = x_seq.shape
         Ha, Hb = w_ha.shape[1], w_hb.shape[1]
@@ -542,27 +586,33 @@ class _LSTMPairFn(torch.autograd.Function):
         tn = 4 * Hb // 256
         ws_a, ws_b, done = _pair_ws(dev, "fwd", T * tn * 2)
         done.zero_()                                                     # (the prologue kernels zero ws_a / ws_b)
-        var = _wave_variant()                                            # two batch tiles per CTA: 64 CTAs per layer at H = 1024
+        var = _pair_variant(schedule)                                    # two batch tiles per CTA: 64 CTAs per layer at H = 1024
         # ONE stream, a programmatic-dependent-launch chain: L_a -> L_b (starts once every CTA of L_a is resident) -> gated GEMM
         # (starts once every CTA of L_b is resident, on the SMs that are left).  The order in which the three grids take their
         # SMs is thereby fixed (a kernel that is still queueing could otherwise starve the chain head of co-resident SMs).
         # Everything the later kernels need up front (prologues, zeroed counters) is enqueued before the chain head.
+        # Pipelined: L_a -> gated GEMM (programmatic dependent, on the SMs L_a leaves free) -> L_b, an ordinary launch that
+        # starts once both are complete (the GEMM waits for L_a before it exits).
         E.lstm_seq_prologue(h0a_c, c0a_f, h_seq_a, c_seq_a, til_a, ws_a)
         E.lstm_seq_prologue(h0b_c, c0b_f, h_seq_b, c_seq_b, til_b, ws_b)
         E.lstm_seq_fwd_into(gx_a, wha, ba_f, h0a_c, c0a_f, h_seq_a, c_seq_a, act_a, til_a, ws_a, var, None, 0, True, 0, 1, lengths)
-        E.lstm_seq_fwd_into(gx_b, whb, bb_f, h0b_c, c0b_f, h_seq_b, c_seq_b, act_b, til_b, ws_b, var, done, tn, False, 0, 3, lengths)
+        if not pipelined:
+            E.lstm_seq_fwd_into(gx_b, whb, bb_f, h0b_c, c0b_f, h_seq_b, c_seq_b, act_b, til_b, ws_b, var, done, tn, False, 0, 3, lengths)
         # single-CTA tiles: the recurrences' CTAs are spread one per TPC, the SMs they leave free rarely form CTA pairs
-        free_ctas = max(1, _sms(dev) - Ha // 16 - Hb // 16)
+        free_ctas = max(1, _sms(dev) - Ha // 16 - (0 if pipelined else Hb // 16))
         E.gemm2(h_seq_a[1:].view(T * B, Ha), wxb, out=gx_b.view(T * B, 4 * Hb), ctas=1, bn=256, max_ctas=free_ctas,
                 gate=ws_a[_gate_off(var):], gate_cfg=_gate_cfg(var, 2, Ha // 64, 4, 4 * Ha // 64, 2, 1, B, False), done=done,
                 gate_err=ws_a[SYNC_WORDS - 1:], pdl=True)
+        if pipelined:
+            E.lstm_seq_fwd_into(gx_b, whb, bb_f, h0b_c, c0b_f, h_seq_b, c_seq_b, act_b, til_b, ws_b, var, None, 0, False, 0, 1, lengths)
         STATS["fast_fwd"] += 2
         STATS["kernels"] += 3
-        STATS["wavefront_fwd"] = STATS.get("wavefront_fwd", 0) + 1
+        STATS[schedule + "_fwd"] = STATS.get(schedule + "_fwd", 0) + 1
         ctx.save_for_backward(x2d, h_seq_a, c_seq_a, act_a, h_seq_b, c_seq_b, act_b, wxa, wha, wxb, whb)
         ctx.set_materialize_grads(False)
         ctx.dims = (T, B, D, Ha, Hb)
         ctx.lengths = lengths
+        ctx.pipelined = pipelined
         ctx.x_folded = x_bm is not None
         ctx.addrs = (w_xa.data_ptr(), w_ha.data_ptr(), b_a.data_ptr(), w_xb.data_ptr(), w_hb.data_ptr(), b_b.data_ptr())
         ctx.in_dtypes = (h0a.dtype, c0a.dtype, h0b.dtype, c0b.dtype)
@@ -586,25 +636,45 @@ class _LSTMPairFn(torch.autograd.Function):
         tn = Ha // 256
         ws_b, ws_a, done = _pair_ws(dev, "bwd", T * tn * 2)               # head of the backward chain is layer b
         ws_a[:SYNC_WORDS - 1].zero_(); ws_b[:SYNC_WORDS - 1].zero_(); done.zero_()
-        var = _wave_variant()
-        # programmatic-dependent-launch chain on one stream (see forward): L_b -> L_a -> gated dX GEMM
+        var = _pair_variant("pipelined" if ctx.pipelined else "wavefront")
+        # programmatic-dependent-launch chain on one stream (see forward): L_b -> L_a -> gated dX GEMM.  Pipelined: L_b -> gated
+        # dX GEMM -> L_a (ordinary launch: dx_b is complete when it starts)
+        pipelined = ctx.pipelined
         E.lstm_seq_bwd_into(dh_seq_b, whT_b, act_b, c_seq_b, dpre_b, dh0b, dc0b, til_b, ws_b, var, None, 0, True, 0, 1, ctx.lengths)
-        E.lstm_seq_bwd_into(dx_b, whT_a, act_a, c_seq_a, dpre_a, dh0a, dc0a, til_a, ws_a, var, done, tn, False, 0, 3, ctx.lengths)
-        free_ctas = max(1, _sms(dev) - Ha // 16 - Hb // 16)
+        if not pipelined:
+            E.lstm_seq_bwd_into(dx_b, whT_a, act_a, c_seq_a, dpre_a, dh0a, dc0a, til_a, ws_a, var, done, tn, False, 0, 3, ctx.lengths)
+        free_ctas = max(1, _sms(dev) - Hb // 16 - (0 if pipelined else Ha // 16))
         E.gemm2(dpre_b.view(T * B, 4 * Hb), wxb, out=dx_b.view(T * B, Ha), b_mn=True, ctas=1, bn=256, max_ctas=free_ctas,
                 gate=ws_b[_gate_off(var):], gate_cfg=_gate_cfg(var, 2, 4 * Hb // 64, 1, 4 * Hb // 64, T + 1, -1, B, True), done=done,
                 gate_err=ws_b[SYNC_WORDS - 1:], pdl=True)
+        if pipelined:
+            E.lstm_seq_bwd_into(dx_b, whT_a, act_a, c_seq_a, dpre_a, dh0a, dc0a, til_a, ws_a, var, None, 0, False, 0, 1, ctx.lengths)
         STATS["fast_bwd"] += 2
         STATS["kernels"] += 5
         a = ctx.addrs
         dg_b = dpre_b.view(T * B, 4 * Hb)
-        # the bias column sums run NEXT TO the first weight-gradient GEMM of their layer (same dG, idle SMs), not after it
-        # (each GEMM is followed by: finished gradient buckets [programmatic dependents of the GEMM], then half of the layer's
-        # bias column sums [programmatic dependent of whatever was launched last] - all three run side by side)
-        dw_xb = _accumulate_grad(a[3], dg_b.t(), h_seq_a[1:].reshape(T * B, Ha))
-        _bias_grad(a[5], dg_b, under_gemm=dw_xb is None, part=0)
-        dw_hb = _accumulate_grad(a[4], dg_b.t(), h_seq_b[:T].reshape(T * B, Hb))
-        db_b = _bias_grad(a[5], dg_b, under_gemm=dw_hb is None, part=1)
+        if pipelined:
+            # layer b's weight and bias gradients read nothing L_a writes: programmatic dependents of L_a, next to it on the SMs it
+            # leaves free.  dW_xb and dW_hb split those SMs between them: a dependent that has finished its tiles stays resident
+            # until L_a ends (it waits for its predecessor before exiting), so a second GEMM behind it would get no SMs.  A GEMM
+            # CTA holds nearly all registers of its SM, so the bias column sums get SMs of their own (_COLSUM_SMS; at H = 1024
+            # the GEMMs still take 4 rounds of tiles on 32 instead of 34 CTAs): ONE launch of a few CTAs that all stay resident
+            # and walk every slab while L_a runs (with one CTA per slab, the CTAs that find no SM would start after L_a; two
+            # concurrent column-sum launches would share the slab scratch).  Gradient buckets are launched under the next
+            # ordinary launch (dW_xa), not under these: a programmatic dependent may start before the kernels ahead of it in
+            # the stream are complete.
+            side = max(1, (_sms(dev) - Ha // 16 - _COLSUM_SMS) // 2)
+            dw_xb = _accumulate_grad(a[3], dg_b.t(), h_seq_a[1:].reshape(T * B, Ha), pdl=True, max_ctas=side)
+            dw_hb = _accumulate_grad(a[4], dg_b.t(), h_seq_b[:T].reshape(T * B, Hb), pdl=True, max_ctas=side)
+            db_b = _bias_grad(a[5], dg_b, under_gemm=True, max_ctas=4 * _COLSUM_SMS)
+        else:
+            # the bias column sums run NEXT TO the first weight-gradient GEMM of their layer (same dG, idle SMs), not after it
+            # (each GEMM is followed by: finished gradient buckets [programmatic dependents of the GEMM], then half of the layer's
+            # bias column sums [programmatic dependent of whatever was launched last] - all three run side by side)
+            dw_xb = _accumulate_grad(a[3], dg_b.t(), h_seq_a[1:].reshape(T * B, Ha))
+            _bias_grad(a[5], dg_b, under_gemm=dw_xb is None, part=0)
+            dw_hb = _accumulate_grad(a[4], dg_b.t(), h_seq_b[:T].reshape(T * B, Hb))
+            db_b = _bias_grad(a[5], dg_b, under_gemm=dw_hb is None, part=1)
         dg_a = dpre_a.view(T * B, 4 * Ha)
         dw_xa = _accumulate_grad(a[0], dg_a.t(), x2d, b_folded=ctx.x_folded)
         _bias_grad(a[2], dg_a, under_gemm=dw_xa is None, part=0)
@@ -615,17 +685,23 @@ class _LSTMPairFn(torch.autograd.Function):
             dx = G.matmul(dg_a, wxa.t(), out_dtype=cd).view(T, B, D)
             STATS["kernels"] += 1
         t = ctx.in_dtypes
-        return dx, dh0a.to(t[0]), dc0a.to(t[1]), dw_xa, dw_ha, db_a, dh0b.to(t[2]), dc0b.to(t[3]), dw_xb, dw_hb, db_b, None
+        return dx, dh0a.to(t[0]), dc0a.to(t[1]), dw_xa, dw_ha, db_a, dh0b.to(t[2]), dc0b.to(t[3]), dw_xb, dw_hb, db_b, None, None
 
 
-def lstm_pair_sequence(x_seq, la, lb, lengths=None):
-    """Two stacked layers as one wavefront op.  ``la`` / ``lb`` = (h0, c0, w_x, w_h, bias).  -> (h_seq_b, hT_a, cT_a, hT_b, cT_b).
-    ``lengths``: optional int32 ``[B]`` per-row lengths (both layers run their masked kernels; the gated GEMM is unchanged)."""
+def lstm_pair_sequence(x_seq, la, lb, lengths=None, schedule=None):
+    """Two stacked layers as one op.  ``la`` / ``lb`` = (h0, c0, w_x, w_h, bias).  -> (h_seq_b, hT_a, cT_a, hT_b, cT_b).
+    ``lengths``: optional int32 ``[B]`` per-row lengths (both layers run their masked kernels; the gated GEMM is unchanged).
+    ``schedule``: "wavefront" or "pipelined" (see ``pair_schedule``); None = the one ``pair_schedule`` picks for the device."""
     _check_lengths_arg(lengths, x_seq.shape[1], x_seq.device)
+    if schedule is None:
+        schedule = _pair_schedule_of(x_seq, la[3].shape[1], lb[3].shape[1])
+    if schedule not in ("wavefront", "pipelined"):
+        raise ValueError(f"no layer-pair schedule for x {tuple(x_seq.shape)} {x_seq.dtype}, H = {la[3].shape[1]}, "
+                         f"{lb[3].shape[1]} (schedule={schedule!r}); check wavefront_supported first")
     if (not x_seq.is_contiguous() and not x_seq.requires_grad and x_seq.transpose(0, 1).is_contiguous()
             and (x_seq.shape[2] * x_seq.element_size()) % 16 == 0):
         if FOLDED_FEED and G.folded_ok(x_seq.transpose(0, 1)):
-            return _LSTMPairFn.apply(x_seq, *la, *lb, lengths)            # read in place (see forward)
+            return _LSTMPairFn.apply(x_seq, *la, *lb, lengths, schedule)  # read in place (see forward)
         x_seq = ext().transpose01(x_seq.transpose(0, 1))
         STATS["kernels"] += 1
-    return _LSTMPairFn.apply(x_seq.contiguous(), *la, *lb, lengths)
+    return _LSTMPairFn.apply(x_seq.contiguous(), *la, *lb, lengths, schedule)

@@ -60,7 +60,7 @@ def head_xent(h, weights, bias, labels):
 
 
 def lstm_pair_supported(x_seq, h_a: int, h_b: int) -> bool:
-    """Can two stacked layers run as one layer-wavefront op (both recurrences co-resident on the GPU)?"""
+    """Can two stacked layers run as one pair op on the GPU (layer wavefront or pipelined, ``cuda_lstm.pair_schedule``)?"""
     if not x_seq.is_cuda or _BACKEND == "torch":
         return False
     from . import cuda_lstm
