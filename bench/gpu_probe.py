@@ -452,6 +452,49 @@ def check_tiles2_tune():
     _emit("tiles1_bwd", us_per_step=ms * 1e3 / (T + 1))
 
 
+def check_tiles2_phase():
+    """Per-step phase split of the two-tiles-per-CTA kernels (64 CTAs per layer, the headline's recurrences), from the time
+    stamps of CTA 0's first tile: first operand block ready -> accumulator ready (load_mma_us), accumulator ready -> dataflow
+    signal sent (epi_us), signal -> next step's first block ready (sync_us).  debug_mode 1 skips the operand loads (garbage
+    results): how much of the step the operand stream costs."""
+    import torch
+    from lstm_tensorspark_b200.ops import cuda_lstm
+    from lstm_tensorspark_b200.ops.cuda_ext import ext
+    E = ext()
+    dev = torch.device("cuda")
+    T, B, H = 128, 256, 1024
+    torch.manual_seed(0)
+    gx = (torch.randn(T, B, 4 * H, device=dev) * 0.5).bfloat16()
+    whb = (torch.randn(4 * H, H, device=dev) / H ** 0.5).bfloat16()
+    whT = whb.t().contiguous()
+    bias = torch.zeros(4 * H, device=dev)
+    h0 = torch.zeros(B, H, device=dev).bfloat16(); c0 = torch.zeros(B, H, device=dev)
+    ws = cuda_lstm._sync_ws(dev)
+    _, cseq, act = E.lstm_seq_fwd(gx, whb, bias, h0, c0, ws, 2)
+    dh = (torch.randn(T, B, H, device=dev) * 0.1).bfloat16()
+    z = torch.zeros(B, H, device=dev)
+    runs = {"fwd": lambda v, dbg=None: E.lstm_seq_fwd(gx, whb, bias, h0, c0, ws, v, dbg),
+            "bwd": lambda v, dbg=None: E.lstm_seq_bwd(dh, whT, act, cseq, z, z, ws, v, dbg)}
+    for direction, run in runs.items():
+        steps = T if direction == "fwd" else T + 1
+        first = 8 if direction == "fwd" else 9              # skip the first steps (the backward pass stamps from s = 1)
+        for mode in (0, 1):
+            v = 2 + 4096 * mode
+            try:
+                ms = _time_ms(lambda: run(v), iters=5, warm=2)
+                dbg = torch.zeros(4 * (T + 2) + 64 + 512, dtype=torch.int64, device=dev)
+                run(v, dbg)
+                torch.cuda.synchronize()
+                cuda_lstm.check_kernel_errors(dev)
+                d = dbg[:4 * (T + 2)].view(-1, 4)[first:steps - 8].cpu()
+                waited, accum, sig = d[:, 0], d[:, 1], d[:, 2]
+                _emit("tiles2_phase", direction=direction, debug_mode=mode, us_per_step=ms * 1e3 / steps,
+                      load_mma_us=float((accum - waited).float().mean()) / 1e3, epi_us=float((sig - accum).float().mean()) / 1e3,
+                      sync_us=float((waited[1:] - sig[:-1]).float().mean()) / 1e3)
+            except Exception as e:                     # noqa: BLE001
+                _emit("tiles2_phase", direction=direction, debug_mode=mode, error=repr(e)[:300])
+
+
 def check_bwd_tune():
     """Backward kernel: per-phase timestamps of CTA 0 (first operand block ready / accumulator ready / signalled)."""
     import torch
@@ -581,7 +624,7 @@ def check_iris_gpu():
     _emit("iris_gpu_standalone", rc=r.returncode, tail=(r.stdout + r.stderr)[-600:])
 
 
-CHECKS = {"tiles2": check_tiles2_tune, "wave": check_wave, "wave_bwd": check_wave_bwd, "gemm2": check_gemm2, "gemm2_dw": check_gemm2_dw, "seq_h2048": check_seq_h2048, "bwd_tune": check_bwd_tune, "skew": check_skew, "seq_tiles": check_seq_tiles, "seq_tune": check_seq_tune, "env": check_env, "simple": check_simple, "generic": check_generic, "seq_small": check_seq_small,
+CHECKS = {"tiles2": check_tiles2_tune, "tiles2_phase": check_tiles2_phase,"wave": check_wave, "wave_bwd": check_wave_bwd, "gemm2": check_gemm2, "gemm2_dw": check_gemm2_dw, "seq_h2048": check_seq_h2048, "bwd_tune": check_bwd_tune, "skew": check_skew, "seq_tiles": check_seq_tiles, "seq_tune": check_seq_tune, "env": check_env, "simple": check_simple, "generic": check_generic, "seq_small": check_seq_small,
           "seq_big": check_seq_big, "engine": check_engine, "iris_gpu": check_iris_gpu}
 
 

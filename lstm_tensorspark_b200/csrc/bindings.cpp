@@ -19,6 +19,7 @@ int ts_lstm_pointwise_fwd(const void*, const float*, const float*, void*, float*
                           const int*, int);
 int ts_transpose01_rows(const void*, void*, int, int, long long, cudaStream_t);
 int ts_lstm_seq_cluster_probe(int);
+int ts_lstm_seq_config(int, int, int, int, int*);
 int ts_transpose2d_b16(const void*, void*, int, int, cudaStream_t);
 int ts_colsum_bf16(const void*, float*, void*, int, int, int, int, int, int, cudaStream_t);
 long long ts_colsum_scratch_bytes(int, int);
@@ -479,6 +480,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("colsum_bf16_into", &colsum_bf16_into, py::arg("x"), py::arg("out"), py::arg("overwrite"), py::arg("pdl") = false,
         py::arg("col0") = 0, py::arg("ncols") = 0, py::arg("max_ctas") = 0);
   m.def("lstm_seq_cluster_probe", [](int64_t c) { return ts_lstm_seq_cluster_probe((int)c); });
+  // (ring stages, batch tiles per CTA, streamed weights, forward K-split) of the persistent kernel for these arguments
+  m.def("lstm_seq_config", [](bool bwd, int64_t H, int64_t B, int64_t variant) {
+    int out[4];
+    check(ts_lstm_seq_config(bwd ? 1 : 0, (int)H, (int)B, (int)variant, out), "lstm_seq_config");
+    return std::make_tuple(out[0], out[1], out[2] != 0, out[3] != 0);
+  }, py::arg("bwd"), py::arg("H"), py::arg("B"), py::arg("variant") = 0);
   m.def("lstm_pointwise_bwd", &lstm_pointwise_bwd, py::arg("dh_a"), py::arg("dh_b"), py::arg("dc_in"), py::arg("act"), py::arg("c_prev"),
         py::arg("c_new"), py::arg("lengths") = py::none(), py::arg("t") = 0);
   m.def("xent_rows", &xent_rows);

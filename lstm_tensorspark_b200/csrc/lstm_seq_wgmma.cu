@@ -10,9 +10,10 @@
 //     owns a row slice owns complete (i,f,g,o) quadruples: the gate epilogue needs no cross-CTA traffic.
 //   * Per step a CTA streams a 128-row batch tile of h_{t-1} (forward) / dG_{t+1} (backward) through a bulk-copy ->
 //     mbarrier ring (the operand is kept in global memory as ready-made 128B-swizzled tile images, 16 KB contiguous per
-//     k-block).  Two consumer warpgroups issue wgmma (m64n32k16, bf16 -> fp32 accumulators in registers), one per 32
-//     accumulator columns over all 128 rows, stage the accumulator through shared memory and do the whole cell with one
-//     thread per batch row (the cell state never leaves its registers).
+//     k-block).  Two consumer warpgroups issue wgmma (m64n64k16, bf16 -> fp32 accumulators in registers), one per 64 batch
+//     rows over all accumulator columns, stage the accumulator through shared memory - in their own half of the ring stages
+//     they have just drained, so the ring gets that space - and do the whole cell with one thread per batch row (the cell
+//     state never leaves its registers).  At H = 1024 with two batch tiles per CTA the ring holds 6 stages forward, 4 backward.
 //   * The forward pass can split K across a cluster of 2 CTAs and the backward pass does across 4 (one gate-column quarter
 //     each); the partial accumulators are reduce-scattered through DISTRIBUTED SHARED MEMORY with st.async (bytes are
 //     counted on the receiver's mbarrier: no release/acquire fences).  Every member then owns 16 hidden units.
@@ -229,8 +230,9 @@ struct SeqParams {
 //             streamed weights (kNarrow): columns [32 nb2, +32) over gate-column half ks (K = 2H), clusters of 2; member ks
 //                                 then owns hidden [32 nb2 + 16 ks, +16) - the same 16 hidden units per CTA.
 // Warps: 0 = producer, 1..2 = idle, 3 = watchdog, 4..11 = two consumer warpgroups.  Consumer warpgroup `half` = (warp-4)/4
-// computes accumulator columns [32 half, +32) (+64: forward K-split) of all 128 rows with wgmma and stages them in shared
-// memory; then warp % 4 = row quarter, and one thread = one batch row x 8 hidden units (32 accumulator columns).
+// computes batch rows [64 half, +64) x all accumulator columns with one wgmma per k16 (it reads only its half of each A tile)
+// and stages them in shared memory; then warp q = warp % 4 reads rows 64 half + 32 (q & 1) + lane, column half q >> 1, and one
+// thread = one batch row x 8 hidden units (32 accumulator columns).
 // The producer warp runs CONVERGED and issues under elect.sync so addresses stay in uniform registers.
 // kTiles = 2: the CTA alternates TWO independent 128-row batch tiles (same resident weight slice): while one tile sits
 // in its epilogue + dataflow wait (latency), the other one's operand streams in.  Half as many CTAs are needed (64 for
@@ -262,7 +264,7 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
   constexpr int kSplit = kBwd ? (kNarrow ? 2 : 4) : (kFSplit ? 2 : 1);     // cluster size = K-split factor
   constexpr bool kCluster = kSplit > 1;
   constexpr int kBNm = kFSplit ? 2 * BN : (kNarrow ? BN / 2 : BN);        // accumulator columns per CTA
-  constexpr int kCW = kNarrow ? 16 : 32;                     // accumulator columns per wgmma (warpgroup `half`: [kCW half, +kCW))
+  constexpr int kCW = kNarrow ? 16 : 32;                     // backward: accumulator columns per epilogue thread ([kCW chalf, +kCW))
   constexpr int kWBlk = kBNm * BK * 2;                       // bytes of one weight k-block
   // operand k-blocks this CTA contracts over per step (backward: K = 4H split kSplit ways)
   const int num_kb = kFSplit ? p.H / (2 * BK) : (kBwd ? 4 * p.H / (kSplit * BK) : p.H / BK);
@@ -272,10 +274,17 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
   uint8_t* smem_w = smem;                                    // resident weight slice: num_kb blocks of [kBNm x 64] (not kStream)
   uint8_t* smem_a = smem + (kStream ? 0 : (size_t)num_kb * kWBlk);    // kStages x (16 KB [+ 8 KB weight block])
   uint8_t* smem_x = smem_a + kStages * kStageBytes;          // DSMEM exchange buffer (bf16 partial sums)
-  // staged fp32 accumulator [BM][kBNm]: 16 B chunk q of row r sits at q ^ (r & 7) (conflict-free row-per-thread reads)
-  float* acc_s = reinterpret_cast<float*>(smem_x + (kCluster ? kTiles * kXchgBytes : 0));
-  auto acc_idx = [](int r, int c) { return r * kBNm + ((((c >> 2) ^ r) & 7) | ((c >> 2) & ~7)) * 4 + (c & 3); };
-  SeqSmem* ss = reinterpret_cast<SeqSmem*>(acc_s + BM * kBNm);
+
+  // The fp32 accumulator is staged in shared memory so that one thread can read a whole row.  A warpgroup's 64 rows take
+  // kAccPieces 8 KB pieces; they go into the A-operand halves of the ring stages it consumed last (see mma_tile), except in
+  // the forward K-split (32 KB per warpgroup) and when a tile has fewer k-blocks than pieces (H = 64): there a dedicated
+  // buffer holds them (smem_bytes() sizes it for exactly these cases).
+  constexpr int kAccRowBytes = kBNm * 4;
+  constexpr int kAccPieces = 64 * kAccRowBytes / (kABytes / 2);               // 2; kNarrow 1; kFSplit 4
+  constexpr int kAccRowsPer = kFSplit ? 64 : (kABytes / 2) / kAccRowBytes;    // rows per piece (kFSplit: contiguous buffer)
+  const bool ring_acc = !kFSplit && num_kb >= kAccPieces;
+  uint8_t* acc_s = smem_x + (kCluster ? kTiles * kXchgBytes : 0);             // dedicated staging buffer [BM][kBNm] fp32
+  SeqSmem* ss = reinterpret_cast<SeqSmem*>(acc_s + (ring_acc ? 0 : BM * kAccRowBytes));
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   // Programmatic dependent launch: a kernel queued behind this one WITH the PDL attribute (the fused allreduce + update of a
@@ -472,21 +481,34 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
     // ======================================================================== consumers (8 warps, serve the tiles in turn)
     const int ewi = warp - kEpiWarp0;
     const int quarter = ewi & 3, half = ewi >> 2;
-    const int rloc = quarter * 32 + lane;
+    // epilogue thread: row rl of its warpgroup's 64 (= batch row rloc of the tile), accumulator column half chalf
+    const int rl = 32 * (quarter & 1) + lane, chalf = quarter >> 1;
+    const int rloc = 64 * half + rl;
     const int etid = ewi * 32 + lane;
     const int H = p.H, B = p.B;
     bool ok = true;
     // wgmma over one batch tile's operand k-blocks of the current step (ring order; the stage carries its k-block id): this
-    // warpgroup's accumulator columns {kCW half + 2 kCW j} of all 128 rows, m64 x kCW x k16 per (row half, column chunk), then
-    // staged in acc_s so that every thread can read its own row
-    constexpr int kNAcc = 2 * (kBNm / (2 * kCW));
+    // warpgroup's batch rows [64 half, +64) x all kBNm accumulator columns, m64 x kBNm x k16, then staged in shared memory so
+    // that every thread can read its own row.  Each warpgroup reads only its own half of every A tile.
     const uint32_t full0 = tc::smem_u32(&ss->full[0]), empty0 = tc::smem_u32(&ss->empty[0]);
     const uint64_t desc_a0 = tc::desc_kmajor_sw128(tc::smem_u32(smem_a));      // + stage * (kStageBytes >> 4)
     const uint64_t desc_w0 = tc::desc_kmajor_sw128(tc::smem_u32(smem_w));      // + kb * (kWBlk >> 4)
     uint32_t stage = 0, phase = 0;
+    // Ring staging: the tile's last kAccPieces stages (the ones `stage` has just moved past) hold the staged rows, pieces
+    // 0 / 1 = rows [0, kAccRowsPer) / the rest, and receive this warp's empty arrival only once it has read its row.
+    auto stage_back = [&](int back) -> uint32_t { return stage >= (uint32_t)back ? stage - back : stage + kStages - back; };
+    auto acc_row_ptr = [&](int r) -> float* {           // staged row r of this warpgroup's 64 (a warp's rows share one piece)
+      uint8_t* pc = ring_acc ? smem_a + stage_back(kAccPieces - r / kAccRowsPer) * kStageBytes + half * (kABytes / 2)
+                             : acc_s + (half * 64 + r / kAccRowsPer * kAccRowsPer) * kAccRowBytes;
+      return reinterpret_cast<float*>(pc + (r % kAccRowsPer) * kAccRowBytes);
+    };
+    // 16 B chunk q of a staged row r sits at q ^ (r & 7) (conflict-free row-per-thread reads)
+    auto acc_swz = [](int r, int c) { return ((((c >> 2) ^ r) & 7) | ((c >> 2) & ~7)) * 4 + (c & 3); };
     auto wg_bar = [&]() { asm volatile("bar.sync %0, 128;" ::"r"(3 + half) : "memory"); };
     auto mma_tile = [&]() -> bool {
-      float acc[kNAcc][kCW / 2];
+      float acc[kBNm / 2];
+      // ring staging: the last kAccPieces stages of the tile stay borrowed (no empty arrival) until acc_release
+      const int borrow = ring_acc ? kAccPieces : 0;
       uint32_t prev = 0;
       for (int kb = 0; kb < num_kb; ++kb) {
         if (!tc::mbar_try_wait_u32(full0 + 8 * stage, phase) && !wait_bar<false>(&ss->full[stage], phase, abort_flag)) {
@@ -494,55 +516,65 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
           return false;
         }
         const uint32_t kbi = kStream ? 0u : (p.sync_mode == 1 ? (uint32_t)kb : ss->kb_idx[stage]);
-        const uint64_t da = desc_a0 + (uint64_t)(stage * (kStageBytes >> 4));
-        const uint64_t dw = kStream ? da + (uint64_t)(kABytes >> 4) : desc_w0 + (uint64_t)(kbi * (kWBlk >> 4));
-#pragma unroll
-        for (int a = 0; a < kNAcc; ++a) tc::fence_regs(acc[a]);
+        const uint64_t ds = desc_a0 + (uint64_t)(stage * (kStageBytes >> 4));
+        const uint64_t da = ds + (uint64_t)(half * ((kABytes / 2) >> 4));           // A rows [64 half, +64)
+        const uint64_t dw = kStream ? ds + (uint64_t)(kABytes >> 4) : desc_w0 + (uint64_t)(kbi * (kWBlk >> 4));
+        tc::fence_regs(acc);
         tc::wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < BK / 16; ++k)
-#pragma unroll
-          for (int a = 0; a < kNAcc; ++a)       // A rows [64 (a & 1), +64), weight rows [kCW half + 2 kCW (a >> 1), +kCW)
-            tc::Wgmma<kCW, 0, 0>::mma(acc[a], da + (uint64_t)((a & 1) * (8192 >> 4) + 2 * k),
-                                      dw + (uint64_t)((kCW * half + 2 * kCW * (a >> 1)) * (128 >> 4) + 2 * k), (kb > 0 || k > 0) ? 1u : 0u);
+        for (int k = 0; k < BK / 16; ++k) tc::Wgmma<kBNm, 0, 0>::mma(acc, da + (uint64_t)(2 * k), dw + (uint64_t)(2 * k), (kb > 0 || k > 0) ? 1u : 0u);
         tc::wgmma_commit();
-#pragma unroll
-        for (int a = 0; a < kNAcc; ++a) tc::fence_regs(acc[a]);
+        tc::fence_regs(acc);
         // Hand a stage back once its MMAs have retired.  With >= 3 stages that is the previous one (its MMAs overlap this
         // stage's wait); with 2 the producer waits for both stages of a k-block pair, so each stage is released at once.
         if (kStages >= 3) {
           if (kb > 0) {
             tc::wgmma_wait<1>();
-            if (lane == 0) tc::mbar_arrive_u32(empty0 + 8 * prev);
+            if (lane == 0 && kb - 1 < num_kb - borrow) tc::mbar_arrive_u32(empty0 + 8 * prev);
           }
         } else {
           tc::wgmma_wait<0>();
-          if (lane == 0) tc::mbar_arrive_u32(empty0 + 8 * stage);
+          if (lane == 0 && kb < num_kb - borrow) tc::mbar_arrive_u32(empty0 + 8 * stage);
         }
         prev = stage;
         if (++stage == kStages) { stage = 0; phase ^= 1; }
       }
       tc::wgmma_wait<0>();
+      tc::fence_regs(acc);
+      // Ring staging: the MMAs that read this warpgroup's A half of the last stages have retired and only this warpgroup reads
+      // that half, so the accumulator goes there.  The borrowed stages were refilled only after every warp had released them
+      // the previous time: no reader of an earlier staging is left.
+      if (!ring_acc) {
+        if (kStages >= 3 && lane == 0) tc::mbar_arrive_u32(empty0 + 8 * prev);
+        wg_bar();                                        // this warpgroup has read the previously staged accumulator
+      }
+      float* wb = acc_row_ptr(16 * quarter);           // this warp's 16 fragment rows
 #pragma unroll
-      for (int a = 0; a < kNAcc; ++a) tc::fence_regs(acc[a]);
-      if (kStages >= 3 && lane == 0) tc::mbar_arrive_u32(empty0 + 8 * prev);
-      wg_bar();                                          // this warpgroup has read the previously staged accumulator
-#pragma unroll
-      for (int a = 0; a < kNAcc; ++a)
-#pragma unroll
-        for (int i = 0; i < kCW / 2; i += 2) {
-          const int r = 64 * (a & 1) + tc::acc_row(i, quarter, lane), c = kCW * half + 2 * kCW * (a >> 1) + tc::acc_col(i, lane);
-          *reinterpret_cast<float2*>(acc_s + acc_idx(r, c)) = make_float2(acc[a][i], acc[a][i + 1]);
-        }
+      for (int i = 0; i < kBNm / 2; i += 2) {
+        const int r = tc::acc_row(i, 0, lane), c = tc::acc_col(i, lane);
+        *reinterpret_cast<float2*>(wb + r * kBNm + acc_swz(r, c)) = make_float2(acc[i], acc[i + 1]);
+      }
       wg_bar();
       return true;
     };
     auto acc_ld32 = [&](int col, uint32_t (&v)[32], bool only16 = false) {   // staged accumulator: row rloc, columns [col, +32 | +16)
+      const float* rb = acc_row_ptr(rl);
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
         if (only16 && i >= 4) break;
-        const float4 f = *reinterpret_cast<const float4*>(acc_s + acc_idx(rloc, col + 4 * i));
+        const float4 f = *reinterpret_cast<const float4*>(rb + acc_swz(rl, col + 4 * i));
         v[4 * i] = __float_as_uint(f.x); v[4 * i + 1] = __float_as_uint(f.y); v[4 * i + 2] = __float_as_uint(f.z); v[4 * i + 3] = __float_as_uint(f.w);
+      }
+    };
+    // This warp has read its staged rows: the borrowed stages go back to the producer.  The proxy fence orders the generic
+    // accesses to them before the bulk copies that refill them.
+    auto acc_release = [&]() {
+      if (!ring_acc) return;
+      tc::fence_proxy_async();
+      __syncwarp();
+      if (lane == 0) {
+        tc::mbar_arrive_u32(empty0 + 8 * stage_back(1));
+        if (kAccPieces == 2) tc::mbar_arrive_u32(empty0 + 8 * stage_back(2));
       }
     };
     const bool dbg_thread = p.dbg && blockIdx.x == 0 && etid == 0;
@@ -562,9 +594,9 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
     // (~0.8 us) and three of them used to dominate the epilogue; the generic->async proxy fence is on the consumer side.
 
     if (!kBwd) {
-      const int j0 = in_mb * 16 + 8 * half;         // this thread's 8 hidden units
-      const int n0 = in_mb * 64 + 32 * half;        // = its 32 gate columns
-      const float* bs = ss->bias + 32 * half;
+      const int j0 = in_mb * 16 + 8 * chalf;         // this thread's 8 hidden units
+      const int n0 = in_mb * 64 + 32 * chalf;        // = its 32 gate columns
+      const float* bs = ss->bias + 32 * chalf;
       uint32_t xphase = 0;
       const uint32_t xbase = tc::smem_u32(smem_x);
       const uint32_t xbar = tc::smem_u32(&ss->xchg_full[0]), fbar = tc::smem_u32(&ss->xchg_free[0]);
@@ -623,8 +655,8 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
           if constexpr (kFSplit) {
             // partial sums over this member's K half: columns [64 ks, +64) are mine, the other 64 go to the peer (bf16, DSMEM)
             uint32_t u[32];
-            acc_ld32(32 * half + 64 * (1 - ks), u);
-            acc_ld32(32 * half + 64 * ks, v);
+            acc_ld32(32 * chalf + 64 * (1 - ks), u);
+            acc_ld32(32 * chalf + 64 * ks, v);
             if (t > 0) {                                               // the peer has consumed last step's partial
               ok = xwait(&ss->xchg_free[0], (uint32_t)((t - 1) & 1), abort_flag);
               if (!ok) break;
@@ -635,14 +667,14 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
               uint32_t pk[4];
 #pragma unroll
               for (int k = 0; k < 4; ++k) pk[k] = pack_bf2(__uint_as_float(u[8 * i + 2 * k]), __uint_as_float(u[8 * i + 2 * k + 1]));
-              st_async_u4(drow + (uint32_t)((((4 * half + i) ^ (rloc & 7))) * 16), make_uint4(pk[0], pk[1], pk[2], pk[3]), pbar);
+              st_async_u4(drow + (uint32_t)((((4 * chalf + i) ^ (rloc & 7))) * 16), make_uint4(pk[0], pk[1], pk[2], pk[3]), pbar);
             }
             ok = xwait(&ss->xchg_full[0], xphase, abort_flag);
             if (!ok) break;
             xphase ^= 1;
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
-              const uint4 x4 = *reinterpret_cast<const uint4*>(smem_x + (size_t)rloc * 128 + (((4 * half + i) ^ (rloc & 7)) * 16));
+              const uint4 x4 = *reinterpret_cast<const uint4*>(smem_x + (size_t)rloc * 128 + (((4 * chalf + i) ^ (rloc & 7)) * 16));
               const uint32_t w[4] = {x4.x, x4.y, x4.z, x4.w};
 #pragma unroll
               for (int k = 0; k < 4; ++k) {
@@ -651,7 +683,8 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
               }
             }
           } else {
-            acc_ld32(32 * half, v);
+            acc_ld32(32 * chalf, v);
+            acc_release();
           }
           if (dbg_thread && t == 8 && tile == 0) p.dbg[4 * (p.T + 2) + 0] = gtime();
           const bool pad = kMasked && tt >= len[tile];  // padded step: the cell holds (the activations are computed but unused)
@@ -734,7 +767,7 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
       }
     } else {
       // after the reduce-scatter this cluster member owns hidden [64 nb + 16 ks, +16); this thread 8 of them
-      const int j0 = nb * kBNm + ks * 16 + 8 * half;
+      const int j0 = nb * kBNm + ks * 16 + 8 * chalf;
       uint32_t xphase = 0;
       float dc[kTiles][8], dh[kTiles][8];
 #pragma unroll
@@ -816,7 +849,8 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
             if (!ok) break;
             if (dbg_thread && tile == 0) p.dbg[4 * s + 1] = gtime();
             uint32_t v[32];
-            acc_ld32(kCW * half, v, kCW == 16);
+            acc_ld32(kCW * chalf, v, kCW == 16);
+            acc_release();
             // A member only needs the dG blocks of ITS K-quarter, so nothing in the dataflow stops a fast member from being a
             // whole step ahead of a slow one: explicit back-pressure before overwriting anybody's exchange buffer.
             if (s > 1) {
@@ -826,11 +860,11 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
             // reduce-scatter over the kSplit K parts: column chunk q (16 wide, bf16) goes to member q's slot [ks] (DSMEM)
 #pragma unroll
             for (int qq = 0; qq < kCW / 16; ++qq) {
-              const uint32_t dst = mapa(xbase + (uint32_t)((ks * BM + rloc) * 32), (uint32_t)((kCW / 16) * half + qq));
+              const uint32_t dst = mapa(xbase + (uint32_t)((ks * BM + rloc) * 32), (uint32_t)((kCW / 16) * chalf + qq));
               uint32_t pk[8];
 #pragma unroll
               for (int i = 0; i < 8; ++i) pk[i] = pack_bf2(__uint_as_float(v[16 * qq + 2 * i]), __uint_as_float(v[16 * qq + 2 * i + 1]));
-              const uint32_t dbar = mapa(xbar, (uint32_t)((kCW / 16) * half + qq));
+              const uint32_t dbar = mapa(xbar, (uint32_t)((kCW / 16) * chalf + qq));
               st_async_u4(dst, make_uint4(pk[0], pk[1], pk[2], pk[3]), dbar);
               st_async_u4(dst + 16, make_uint4(pk[4], pk[5], pk[6], pk[7]), dbar);
             }
@@ -842,7 +876,7 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
             }
 #pragma unroll
             for (int src = 0; src < kSplit; ++src) {
-              const uint4 x4 = *reinterpret_cast<const uint4*>(xbuf + (size_t)(src * BM + rloc) * 32 + 16 * half);
+              const uint4 x4 = *reinterpret_cast<const uint4*>(xbuf + (size_t)(src * BM + rloc) * 32 + 16 * chalf);
               const uint32_t w[4] = {x4.x, x4.y, x4.z, x4.w};
 #pragma unroll
               for (int i = 0; i < 4; ++i) { dh[tile][2 * i] += bf_lo(w[i]); dh[tile][2 * i + 1] += bf_hi(w[i]); }
@@ -898,7 +932,7 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
             const bool swp = rloc & 1;
 #pragma unroll
             for (int k = 0; k < 2; ++k) {
-              const int sp = (2 * half + k) ^ ((rloc & 7) >> 1);
+              const int sp = (2 * chalf + k) ^ ((rloc & 7) >> 1);
               const uint32_t* a = gpk + 8 * k;
               stg32(tp + sp * 16, swp ? a[4] : a[0], swp ? a[5] : a[1], swp ? a[6] : a[2], swp ? a[7] : a[3],
                     swp ? a[0] : a[4], swp ? a[1] : a[5], swp ? a[2] : a[6], swp ? a[3] : a[7]);
@@ -969,7 +1003,10 @@ size_t smem_bytes(int H, bool bwd, int stages, int tiles, bool stream = false, b
   const bool narrow = bwd && stream;                       // streamed backward: 32 accumulator columns per CTA (kNarrow)
   const size_t ring = (size_t)stages * (stream ? kABytes + (narrow ? kWBlockBytes / 2 : kWBlockBytes) : kABytes);
   // resident weights: H/64 blocks of [64 x 64] (forward K-split: H/128 blocks of [128 x 64] = the same bytes)
-  const size_t acc_stage = (size_t)BM * (fsplit ? 2 * BN : (narrow ? BN / 2 : BN)) * sizeof(float);     // staged fp32 accumulator
+  // The staged fp32 accumulator lives in drained ring stages, except for the forward K-split and H = 64 (one k-block per
+  // tile, two 8 KB pieces per warpgroup): those keep a dedicated [128 x columns] buffer (lstm_seq_kernel, ring_acc).
+  const bool dedicated = fsplit || (!narrow && H / BK < 2);
+  const size_t acc_stage = dedicated ? (size_t)BM * (fsplit ? 2 * BN : BN) * sizeof(float) : 0;
   return (stream ? 0 : (size_t)(H / BK) * kWBlockBytes) + ring + ((bwd || fsplit) ? tiles * kXchgBytes : 0) + acc_stage + sizeof(SeqSmem) + 1024;
 }
 
@@ -1054,43 +1091,61 @@ int pick_stages(int H, bool bwd, int tiles) {
 // sync_ws: kSyncWords u32 (layout above); everything but the sticky error flag in the last word is zeroed before every launch.
 // variant (tuning knob, 0 = defaults) = tiles_per_cta + 16*stages + 4096*debug_mode:  tiles_per_cta 0 -> 1 (set 2 to let a
 // CTA alternate two batch tiles);  stages 0 -> deepest ring that fits next to the resident weight slice.
-template <bool kBwd>
-static int seq_common(SeqParams& p, const void* w_base, int variant, cudaStream_t st, bool reverse) {
-  const int H = p.H, B = p.B;
+struct SeqCfg {
+  int stages, tiles;
+  bool stream, fsplit;
+};
+
+// The launch configuration seq_common() uses for H, B and variant (no device needed): 0, or a negative code with the error
+// message set.
+static int seq_config(bool bwd, int H, int B, int variant, SeqCfg& c) {
   if (H % 64 != 0) { ts::set_last_error("lstm_seq: H must be a multiple of 64"); return -2; }
-  if (reverse && (p.in_gate != nullptr || p.extra_signal)) {
-    ts::set_last_error("lstm_seq: the reverse direction does not run in the layer wavefront (in_gate / extra_signal)");
-    return -2;
-  }
-  const int tiles_m = (B + BM - 1) / BM, tiles_n = kBwd ? (H / BN) * 4 : 4 * H / BN;
+  const int tiles_m = (B + BM - 1) / BM;
   int stages = (variant >> 4) & 15, tiles = variant & 15;
-  p.debug_mode = (variant >> 12) & 7;
-  p.sync_mode = (variant >> 16) & 3;
-  p.poll_acquire = (variant >> 18) & 1;
-  p.no_trap = (variant >> 20) & 1;
   if (tiles != 2 || tiles_m % 2 != 0) tiles = 1;
-  // resident weight slice if it fits next to >= 3 ring stages, else stream the weights through the ring
-  const bool stream = smem_bytes(H, kBwd, 3, 1) > 227 * 1024 || ((variant >> 8) & 1);
+  // resident weight slice up to H = 1152 (forward) / 1024 (backward; cuda_lstm._bwd_cluster and _tiles_per_cta assume this
+  // boundary), else stream the weights through the ring
+  const bool stream = H > (bwd ? 1024 : 1152) || ((variant >> 8) & 1);
   if (stream) tiles = 1;
-  if (kBwd && stream && 4 * H / (2 * BK) > 64) { ts::set_last_error("lstm_seq: streamed backward needs H <= 2048"); return -2; }
+  if (bwd && stream && 4 * H / (2 * BK) > 64) { ts::set_last_error("lstm_seq: streamed backward needs H <= 2048"); return -2; }
   // forward: 2-way K split (cluster of 2) unless disabled by variant bit 19
-  const bool fsplit = !kBwd && !stream && tiles == 1 && H % 128 == 0 && !((variant >> 19) & 1) &&
+  const bool fsplit = !bwd && !stream && tiles == 1 && H % 128 == 0 && !((variant >> 19) & 1) &&
                       smem_bytes(H, false, 3, 1, false, true) <= 227 * 1024;
-  int dev = 0;
-  cudaGetDevice(&dev);
-  const int grid = (tiles_m / tiles) * tiles_n;
-  if (grid > ts::sm_count(dev)) { ts::set_last_error("lstm_seq: grid exceeds SM count (not co-resident)"); return -3; }
   if (stream) {
-    if (stages != 4 && stages != 6 && stages != 8) stages = smem_bytes(H, kBwd, 8, 1, true) <= 227 * 1024 ? 8 : 6;
+    if (stages != 4 && stages != 6 && stages != 8) stages = smem_bytes(H, bwd, 8, 1, true) <= 227 * 1024 ? 8 : 6;
   } else if (fsplit) {
     if (stages < 3 || stages > 6 || smem_bytes(H, false, stages, 1, false, true) > 227 * 1024) {
       stages = 6;
       while (stages > 3 && smem_bytes(H, false, stages, 1, false, true) > 227 * 1024) --stages;
     }
   } else {
-    if (stages == 0) stages = pick_stages(H, kBwd, tiles);
-    if (stages < 2 || smem_bytes(H, kBwd, stages, tiles) > 227 * 1024) { ts::set_last_error("lstm_seq: weight slice does not fit in shared memory"); return -4; }
+    if (stages == 0) stages = pick_stages(H, bwd, tiles);
+    if (stages < 2 || smem_bytes(H, bwd, stages, tiles) > 227 * 1024) { ts::set_last_error("lstm_seq: weight slice does not fit in shared memory"); return -4; }
   }
+  c = SeqCfg{stages, tiles, stream, fsplit};
+  return 0;
+}
+
+template <bool kBwd>
+static int seq_common(SeqParams& p, const void* w_base, int variant, cudaStream_t st, bool reverse) {
+  const int H = p.H, B = p.B;
+  if (reverse && (p.in_gate != nullptr || p.extra_signal)) {
+    ts::set_last_error("lstm_seq: the reverse direction does not run in the layer wavefront (in_gate / extra_signal)");
+    return -2;
+  }
+  SeqCfg cfg;
+  if (int rc = seq_config(kBwd, H, B, variant, cfg)) return rc;
+  const int stages = cfg.stages, tiles = cfg.tiles;
+  const bool stream = cfg.stream, fsplit = cfg.fsplit;
+  const int tiles_m = (B + BM - 1) / BM, tiles_n = kBwd ? (H / BN) * 4 : 4 * H / BN;
+  p.debug_mode = (variant >> 12) & 7;
+  p.sync_mode = (variant >> 16) & 3;
+  p.poll_acquire = (variant >> 18) & 1;
+  p.no_trap = (variant >> 20) & 1;
+  int dev = 0;
+  cudaGetDevice(&dev);
+  const int grid = (tiles_m / tiles) * tiles_n;
+  if (grid > ts::sm_count(dev)) { ts::set_last_error("lstm_seq: grid exceeds SM count (not co-resident)"); return -3; }
   const int K = kBwd ? 4 * H : H, N = kBwd ? H : 4 * H;
   CUtensorMap tw;
   if (int rc = ts::make_tmap_2d_bf16(&tw, w_base, (uint64_t)N, (uint64_t)K, (uint64_t)K, BK, fsplit ? 2 * BN : ((kBwd && stream) ? BN / 2 : BN))) return rc;
@@ -1125,6 +1180,15 @@ extern "C" int ts_lstm_seq_fwd(const void* gx, const void* w_h, const float* bia
   p.pdl_wait = (launch_flags >> 1) & 1;
   p.lengths = lengths;
   return seq_common<false>(p, w_h, variant, st, reverse != 0);
+}
+
+// The launch configuration ts_lstm_seq_fwd / _bwd choose for H, B and variant, without a device: out = {ring stages, batch
+// tiles per CTA, streamed weights, forward K-split}.  0, or a negative code with ts_last_error set.
+extern "C" int ts_lstm_seq_config(int bwd, int H, int B, int variant, int* out) {
+  SeqCfg c;
+  if (int rc = seq_config(bwd != 0, H, B, variant, c)) return rc;
+  out[0] = c.stages; out[1] = c.tiles; out[2] = c.stream; out[3] = c.fsplit;
+  return 0;
 }
 
 extern "C" int ts_lstm_seq_prologue(const void* h0, const float* c0, void* h_seq, float* c_seq, void* a_tiled, unsigned int* sync_ws,
