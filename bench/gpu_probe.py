@@ -456,7 +456,9 @@ def check_tiles2_phase():
     """Per-step phase split of the two-tiles-per-CTA kernels (64 CTAs per layer, the headline's recurrences), from the time
     stamps of CTA 0's first tile: first operand block ready -> accumulator ready (load_mma_us), accumulator ready -> dataflow
     signal sent (epi_us), signal -> next step's first block ready (sync_us).  debug_mode 1 skips the operand loads (garbage
-    results): how much of the step the operand stream costs."""
+    results): how much of the step the operand stream costs.
+    Per warpgroup (= tile, ping-pong schedule): MMA start -> accumulator ready (wgN_mma_us), accumulator ready -> signal
+    (wgN_epi_us), and how much of warpgroup 1's MMA window falls inside warpgroup 0's epilogue (wg1_mma_in_wg0_epi_us)."""
     import torch
     from lstm_tensorspark_b200.ops import cuda_lstm
     from lstm_tensorspark_b200.ops.cuda_ext import ext
@@ -482,15 +484,23 @@ def check_tiles2_phase():
             v = 2 + 4096 * mode
             try:
                 ms = _time_ms(lambda: run(v), iters=5, warm=2)
-                dbg = torch.zeros(4 * (T + 2) + 64 + 512, dtype=torch.int64, device=dev)
+                tile1 = 4 * (T + 2) + 64 + 512                # the second tile's [steps][4] stamps start here
+                dbg = torch.zeros(tile1 + 4 * (T + 2), dtype=torch.int64, device=dev)
                 run(v, dbg)
                 torch.cuda.synchronize()
                 cuda_lstm.check_kernel_errors(dev)
                 d = dbg[:4 * (T + 2)].view(-1, 4)[first:steps - 8].cpu()
+                d1 = dbg[tile1:].view(-1, 4)[first:steps - 8].cpu()
                 waited, accum, sig = d[:, 0], d[:, 1], d[:, 2]
+
+                def us(x):
+                    return float(x.double().mean()) / 1e3
+                overlap = (torch.minimum(d1[:, 1], d[:, 2]) - torch.maximum(d1[:, 3], d[:, 1])).clamp(min=0)
                 _emit("tiles2_phase", direction=direction, debug_mode=mode, us_per_step=ms * 1e3 / steps,
-                      load_mma_us=float((accum - waited).float().mean()) / 1e3, epi_us=float((sig - accum).float().mean()) / 1e3,
-                      sync_us=float((waited[1:] - sig[:-1]).float().mean()) / 1e3)
+                      load_mma_us=us(accum - waited), epi_us=us(sig - accum), sync_us=us(waited[1:] - sig[:-1]),
+                      wg0_mma_us=us(d[:, 1] - d[:, 3]), wg0_epi_us=us(d[:, 2] - d[:, 1]),
+                      wg1_mma_us=us(d1[:, 1] - d1[:, 3]), wg1_epi_us=us(d1[:, 2] - d1[:, 1]),
+                      wg1_mma_start_after_wg0_acc_us=us(d1[:, 3] - d[:, 1]), wg1_mma_in_wg0_epi_us=us(overlap))
             except Exception as e:                     # noqa: BLE001
                 _emit("tiles2_phase", direction=direction, debug_mode=mode, error=repr(e)[:300])
 
