@@ -51,7 +51,8 @@ constexpr long long kSpinLimit = 6000000000LL;   // ~3 s of SM clocks: a bug sur
 constexpr long long kAbortGrace = 1000000000LL;  // ~0.5 s for the role loops to drain after an abort before the watchdog traps
 
 // sync workspace (u32 words): [0,16) grid-barrier counters, [64,320) per-CTA step flags, [512 + 32 i) k-block arrival
-// counters (one 128 B line each, i < tiles_m * 4H/64), [kSyncWords-1] sticky error flag
+// counters (one 128 B line each, i < tiles_m * 4H/64; seq_config rejects layouts that reach the last word), [kSyncWords-1]
+// sticky error flag
 constexpr int kSyncWords = 8192;
 constexpr int kSyncErr = kSyncWords - 1;
 constexpr int kSyncFlags = 64;
@@ -1231,6 +1232,13 @@ static int seq_config(bool bwd, int H, int B, int variant, SeqCfg& c) {
   const bool stream = H > (bwd ? 1024 : 1152) || ((variant >> 8) & 1);
   if (stream) tiles = 1;
   if (bwd && stream && 4 * H / (2 * BK) > 64) { ts::set_last_error("lstm_seq: streamed backward needs H <= 2048"); return -2; }
+  // one arrival counter per operand k-block of every batch tile, at word kSyncKb + 32 i: the last one must stay below the
+  // sticky error word (a layout with more counters would count its arrivals into the error flag)
+  const int counters = tiles_m * (bwd ? 4 * H : H) / BK;
+  if (kSyncKb + 32 * (counters - 1) >= kSyncErr) {
+    ts::set_last_error("lstm_seq: the k-block arrival counters of this layout do not fit in the sync workspace");
+    return -2;
+  }
   // forward: 2-way K split (cluster of 2) unless disabled by variant bit 19
   const bool fsplit = !bwd && !stream && tiles == 1 && H % 128 == 0 && !((variant >> 19) & 1) &&
                       smem_bytes(H, false, 3, 1, false, true) <= 227 * 1024;

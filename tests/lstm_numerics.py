@@ -1,0 +1,255 @@
+"""A reference for the persistent LSTM kernels (csrc/lstm_seq_wgmma.cu) that knows where their fast path rounds.
+
+``layer`` / ``pair`` run one layer / a stacked pair forward AND backward with a hand-written backward loop (no autograd: at
+T = 512, B = 64, H = 2048 a single fp64 [T, B, 4H] tensor is 2.1 GB, and the rounding points sit inside the backward):
+  * ``rounding=None``: fp64 - the exact result of the operation on the inputs the kernels get;
+  * ``rounding=Bf16(...)``: fp32 with every bf16 rounding of the fast path in its place - what an ideal kernel with those
+    rounding points computes.  Its distance from fp64 is the error the bf16 storage alone explains.
+``check_budget`` then holds a kernel's error against fp64 to ALPHA x the emulation's error (plus a small floor), per time step
+for the sequences, so that a defect confined to one step of hundreds cannot hide in a global norm.
+
+Rounding points of the fast path (ops/cuda_lstm.py, csrc/lstm_seq_wgmma.cu), all round-to-nearest-even:
+  forward   gx = x W_x^T is stored bf16 (_gemm_tn); with the forward K-split (cluster of 2) a member adds the PEER's half of the
+            recurrent product as bf16 to its own fp32 half; pre = rec + gx + bias (fp32 bias); h and the saved activations
+            (i, f, g, o) are stored bf16, c stays fp32; h0 enters as bf16, c0 as fp32.
+  backward  dh_seq enters as bf16, dh_T / dc_T as fp32; the recurrent product dG W_h is split into ``bwd_split`` K parts (4 with
+            the weights resident, 2 streamed), each an fp32 partial sum rounded to bf16 for the DSMEM exchange and summed in
+            fp32; the cell backward reads the bf16 activations and fp32 c, and stores dG as bf16; dW_x / dW_h are fp32 products
+            of bf16 operands, db the fp32 column sum of the bf16 dG, dx = dG W_x is stored bf16.
+  pair      h_seq of layer a (bf16) is layer b's input; dx of layer b (bf16) is layer a's dh_seq (ops/cuda_lstm._LSTMPairFn).
+"""
+from __future__ import annotations
+
+import dataclasses
+from typing import NamedTuple, Optional
+
+import torch
+
+KB = 64            # columns of one operand k-block of the persistent kernels
+ROWS = 16          # rows of one wgmma row group
+
+# The kernel's error may be at most ALPHA times the emulation's (both measured against fp64) ...
+ALPHA = 2.0
+# ... plus FLOOR x |fp64|.  The emulation computes tanh / sigmoid exactly; the kernels use tanh.approx.f32 (relative error
+# <= 2^-11; sigmoid(x) = 0.5 tanh(x / 2) + 0.5).  One step's h = o * tanh(c) carries two such approximations, so a kernel
+# that is exact up to them may sit 2 x 2^-11 away from the emulation where the emulation itself happens to be exact.
+FLOOR = 2.0 * 2.0 ** -11
+
+
+@dataclasses.dataclass(frozen=True)
+class Bf16:
+    """The fast path's rounding: ``fwd_split`` K parts of the forward recurrent product (2 = forward K-split), ``bwd_split``
+    K parts of the backward one (4 resident weights, 2 streamed).  ``approx``: relative error put on every tanh (a
+    deterministic function of its argument, like tanh.approx's) - only for stand-ins of a kernel in tests of this module."""
+    fwd_split: int = 1
+    bwd_split: int = 4
+    approx: float = 0.0
+
+    @classmethod
+    def for_layer(cls, H: int, B: int, variant: int = 0) -> "Bf16":
+        """The splits the kernels use for H, B and a variant (``lstm_seq_config``: no device needed)."""
+        from lstm_tensorspark_b200.ops.cuda_ext import ext
+        fwd = ext().lstm_seq_config(False, H, B, variant)
+        bwd = ext().lstm_seq_config(True, H, B, variant)
+        return cls(fwd_split=2 if fwd[3] else 1, bwd_split=2 if bwd[2] else 4)
+
+
+@dataclasses.dataclass(frozen=True)
+class Defect:
+    """A defect to plant into a run (tests of the budget's sensitivity).  ``step``: processing step (0 = the first step of
+    the direction); ``index``: the k-block (``drop_kblock``: of h in the forward recurrent product; ``zero_dg``: of dG) or the
+    16-row group (``stale_rows``: its recurrent operand is h from one step earlier)."""
+    kind: str
+    step: int
+    index: int
+
+
+class LayerOut(NamedTuple):
+    h_seq: torch.Tensor
+    h_T: torch.Tensor
+    c_T: torch.Tensor
+    dx: torch.Tensor
+    dh0: torch.Tensor
+    dc0: torch.Tensor
+    dw_x: torch.Tensor
+    dw_h: torch.Tensor
+    db: torch.Tensor
+
+
+def _round(r: Optional[Bf16], x: torch.Tensor) -> torch.Tensor:
+    return x if r is None else x.to(torch.bfloat16).to(x.dtype)
+
+
+def _tanh(r: Optional[Bf16], x: torch.Tensor) -> torch.Tensor:
+    y = torch.tanh(x)
+    if r is not None and r.approx:
+        y = y * (1.0 + r.approx * torch.sin(x * 4099.0))
+    return y
+
+
+def _sigmoid(r: Optional[Bf16], x: torch.Tensor) -> torch.Tensor:
+    return torch.sigmoid(x) if r is None else 0.5 * _tanh(r, 0.5 * x) + 0.5
+
+
+def _keep(lengths, T, B, device):
+    if lengths is None:
+        return None
+    return lengths.to(device).long().view(B, 1) > torch.arange(T, device=device).view(1, T)      # [B, T]
+
+
+def _rec_fwd(r, h, w_h):
+    """h_{t-1} W_h^T.  Forward K-split: gate column n belongs to cluster member m = (n % 128) // 64, which contracts K half m
+    itself (fp32) and receives the other half from its peer as bf16."""
+    if r is None or r.fwd_split == 1:
+        return h @ w_h.t()
+    hk = h.shape[1] // 2
+    p0 = h[:, :hk] @ w_h[:, :hk].t()
+    p1 = h[:, hk:] @ w_h[:, hk:].t()
+    own0 = (torch.arange(w_h.shape[0], device=h.device) % (2 * KB)) < KB
+    return torch.where(own0, p0 + _round(r, p1), p1 + _round(r, p0))
+
+
+def _rec_bwd(r, dg, w_h):
+    """dG W_h: ``bwd_split`` fp32 partial sums over K quarters / halves, each rounded to bf16, summed in fp32."""
+    if r is None:
+        return dg @ w_h
+    q = dg.shape[1] // r.bwd_split
+    out = None
+    for s in range(r.bwd_split):
+        part = _round(r, dg[:, s * q:(s + 1) * q] @ w_h[s * q:(s + 1) * q])
+        out = part if out is None else out + part
+    return out
+
+
+def _forward(x, h0, c0, w_x, w_h, bias, keep, reverse, r, defect):
+    dt = torch.float64 if r is None else torch.float32
+    T, B, D = x.shape
+    H = w_h.shape[1]
+    w_h = w_h.to(dt)
+    gx = _round(r, x.reshape(T * B, D).to(dt) @ w_x.to(dt).t()).view(T, B, 4 * H)
+    bias = bias.to(dt)
+    h, c = _round(r, h0.to(dt)), c0.to(dt)
+    hs = torch.empty(T + 1, B, H, dtype=dt, device=x.device)
+    cs = torch.empty(T + 1, B, H, dtype=dt, device=x.device)
+    acts = torch.empty(T, B, H, 4, dtype=dt, device=x.device)
+    s0 = T if reverse else 0
+    hs[s0], cs[s0] = h, c
+    h_before = h
+    for n, t in enumerate(range(T - 1, -1, -1) if reverse else range(T)):
+        hin = h
+        if defect is not None and defect.step == n and defect.kind in ("drop_kblock", "stale_rows"):
+            hin = h.clone()
+            if defect.kind == "drop_kblock":
+                hin[:, KB * defect.index:KB * (defect.index + 1)] = 0
+            else:
+                rows = slice(ROWS * defect.index, ROWS * (defect.index + 1))
+                hin[rows] = h_before[rows]
+        pre = (_rec_fwd(r, hin, w_h) + gx[t] + bias).view(B, H, 4)
+        i, f = _sigmoid(r, pre[..., 0]), _sigmoid(r, pre[..., 1])
+        g, o = _tanh(r, pre[..., 2]), _sigmoid(r, pre[..., 3])
+        c_new = f * c + i * g
+        h_new = _round(r, o * _tanh(r, c_new))
+        acts[t] = _round(r, torch.stack((i, f, g, o), -1))
+        if keep is not None:
+            k = keep[:, t:t + 1]
+            c_new, h_new = torch.where(k, c_new, c), torch.where(k, h_new, h)
+        h_before = h
+        h, c = h_new, c_new
+        sn = t if reverse else t + 1
+        hs[sn], cs[sn] = h, c
+    return hs, cs, acts
+
+
+def _backward(fw, x, w_x, w_h, dh_seq, dh_T, dc_T, keep, reverse, r, defect):
+    hs, cs, acts = fw
+    dt = hs.dtype
+    T, B, H = acts.shape[:3]
+    D = x.shape[2]
+    w_h = w_h.to(dt)
+    zeros = lambda: torch.zeros(B, H, dtype=dt, device=hs.device)
+    dh = dh_T.to(dt) if dh_T is not None else zeros()
+    dc = dc_T.to(dt) if dc_T is not None else zeros()
+    dgs = torch.empty(T, B, 4 * H, dtype=dt, device=hs.device)
+    for n, t in enumerate(range(T) if reverse else range(T - 1, -1, -1)):
+        sp, sn = (t + 1, t) if reverse else (t, t + 1)
+        dht = dh if dh_seq is None else dh + _round(r, dh_seq[t].to(dt))
+        i, f, g, o = acts[t].unbind(-1)
+        tcn = _tanh(r, cs[sn])
+        dct = dc + dht * o * (1 - tcn * tcn)
+        dg = torch.stack((dct * g * i * (1 - i), dct * cs[sp] * f * (1 - f), dct * i * (1 - g * g), dht * tcn * o * (1 - o)), -1)
+        dg = _round(r, dg.view(B, 4 * H))
+        if defect is not None and defect.step == n and defect.kind == "zero_dg":
+            dg[:, KB * defect.index:KB * (defect.index + 1)] = 0
+        if keep is None:
+            dc = dct * f
+            dh = _rec_bwd(r, dg, w_h)
+        else:                                 # padded step: no gate gradient, dh / dc pass through to the step before
+            k = keep[:, t:t + 1]
+            dg = torch.where(k, dg, 0.0)
+            dc = torch.where(k, dct * f, dc)
+            dh = torch.where(k, 0.0, dht) + _rec_bwd(r, dg, w_h)
+        dgs[t] = dg
+    dg2d = dgs.view(T * B, 4 * H)
+    h_prev = hs[1:] if reverse else hs[:T]
+    dw_x = dg2d.t() @ x.reshape(T * B, D).to(dt)
+    dw_h = dg2d.t() @ h_prev.reshape(T * B, H)
+    dx = _round(r, dg2d @ w_x.to(dt)).view(T, B, D)
+    return dx, dh, dc, dw_x, dw_h, dg2d.sum(0)
+
+
+def _state_out(fw, reverse):
+    hs, cs, _ = fw
+    T = hs.shape[0] - 1
+    return (hs[:T], hs[0], cs[0]) if reverse else (hs[1:], hs[T], cs[T])
+
+
+def layer(x, h0, c0, w_x, w_h, bias, dh_seq, dh_T, dc_T, lengths=None, reverse=False, rounding: Optional[Bf16] = None,
+          defect: Optional[Defect] = None) -> LayerOut:
+    """One layer forward and backward (``ops/reference.lstm_layer_sequence`` semantics, masking and reverse included) for
+    the loss whose gradients into h_seq / h_T / c_T are ``dh_seq`` / ``dh_T`` / ``dc_T`` (each may be None = zero)."""
+    T, B, _ = x.shape
+    keep = _keep(lengths, T, B, x.device)
+    fw = _forward(x, h0, c0, w_x, w_h, bias, keep, reverse, rounding, defect)
+    return LayerOut(*_state_out(fw, reverse), *_backward(fw, x, w_x, w_h, dh_seq, dh_T, dc_T, keep, reverse, rounding, defect))
+
+
+def pair(x, la, lb, dh_seq, dh_T_a, dc_T_a, dh_T_b, dc_T_b, lengths=None, rounding=None):
+    """Two stacked layers as ``ops/cuda_lstm._LSTMPairFn`` composes them; ``la`` / ``lb`` = (h0, c0, w_x, w_h, bias).
+    ``rounding``: None, one Bf16 for both layers or a (layer a, layer b) tuple.  -> (LayerOut of a, LayerOut of b): the
+    pair's outputs are b.h_seq, a.h_T, a.c_T, b.h_T, b.c_T; its input gradient is a.dx (b.dx is the gradient into a.h_seq)."""
+    ra, rb = rounding if isinstance(rounding, tuple) else (rounding, rounding)
+    T, B, _ = x.shape
+    keep = _keep(lengths, T, B, x.device)
+    fa = _forward(x, *la, keep, False, ra, None)
+    h_seq_a = fa[0][1:]
+    fb = _forward(h_seq_a, *lb, keep, False, rb, None)
+    gb = _backward(fb, h_seq_a, lb[2], lb[3], dh_seq, dh_T_b, dc_T_b, keep, False, rb, None)
+    ga = _backward(fa, x, la[2], la[3], gb[0], dh_T_a, dc_T_a, keep, False, ra, None)
+    return LayerOut(*_state_out(fa, False), *ga), LayerOut(*_state_out(fb, False), *gb)
+
+
+def check_budget(name: str, got: torch.Tensor, fp64: torch.Tensor, emulated: torch.Tensor, per_step: bool = False,
+                 alpha: float = ALPHA, floor: float = FLOOR) -> float:
+    """Assert |got - fp64| <= alpha |emulated - fp64| + floor |fp64| (L2 norms: per time step along dim 0 with
+    ``per_step``, else over the whole tensor) and return the worst ratio of the left side to the right side."""
+    ref = fp64.double()
+    g = got.detach().double().to(ref.device)
+    e = emulated.double().to(ref.device)
+    if not per_step:
+        ref, g, e = ref.reshape(1, -1), g.reshape(1, -1), e.reshape(1, -1)
+    dims = tuple(range(1, ref.dim()))
+    ek = torch.linalg.vector_norm(g - ref, dim=dims)
+    ee = torch.linalg.vector_norm(e - ref, dim=dims)
+    sc = torch.linalg.vector_norm(ref, dim=dims)
+    bound = alpha * ee + floor * sc
+    ratio = torch.where(bound > 0, ek / bound.clamp_min(1e-300), torch.where(ek > 0, float("inf"), 0.0))
+    ratio = torch.where(torch.isnan(ratio), float("inf"), ratio)
+    s = int(ratio.argmax())
+    worst = float(ratio[s])
+    if not worst <= 1.0:
+        where = f" at step {s}" if per_step else ""
+        raise AssertionError(
+            f"{name}{where}: error vs fp64 {float(ek[s]):.3e} exceeds {alpha} x the bf16 emulation's {float(ee[s]):.3e} + "
+            f"{floor:.2e} x |fp64| {float(sc[s]):.3e} (ratio {worst:.2f}; kernel / emulation error "
+            f"{float(ek[s]) / max(float(ee[s]), 1e-300):.2f})")
+    return worst
