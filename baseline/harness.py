@@ -27,12 +27,13 @@ import torch.nn.functional as F
 
 
 class CudnnLSTMClassifier(nn.Module):
-    def __init__(self, hidden, in_features, num_classes, time_major=False, bidirectional=False):
+    def __init__(self, hidden, in_features, num_classes, time_major=False, bidirectional=False, dropout=0.0):
         super().__init__()
         assert len(set(hidden)) == 1, "nn.LSTM stacks equal-width layers"
         self.time_major = time_major
         self.bidirectional = bidirectional
-        self.lstm = nn.LSTM(in_features, hidden[0], num_layers=len(hidden), batch_first=not time_major, bidirectional=bidirectional)
+        self.lstm = nn.LSTM(in_features, hidden[0], num_layers=len(hidden), batch_first=not time_major, bidirectional=bidirectional,
+                            dropout=dropout)
         self.head = nn.Linear(hidden[-1] * (2 if bidirectional else 1), num_classes)
 
     def forward(self, x):
@@ -44,7 +45,7 @@ class CudnnLSTMClassifier(nn.Module):
 
 class BaselineRunner:
     def __init__(self, hidden, in_features, num_classes, batch, seq_len, rank, world, device, optimizer="adam", lr=1e-3,
-                 variant="stock", bidirectional=False):
+                 variant="stock", bidirectional=False, dropout=0.0):
         self.rank, self.world, self.device = rank, world, device
         self.B, self.T, self.D, self.C = batch, seq_len, in_features, num_classes
         self.variant = variant
@@ -55,7 +56,8 @@ class BaselineRunner:
         torch.manual_seed(0)
         if world > 1 and not dist.is_initialized():
             dist.init_process_group("nccl", rank=rank, world_size=world, device_id=device)
-        model = CudnnLSTMClassifier(hidden, in_features, num_classes, time_major=self.tuned, bidirectional=bidirectional).to(device)
+        model = CudnnLSTMClassifier(hidden, in_features, num_classes, time_major=self.tuned, bidirectional=bidirectional,
+                                    dropout=dropout).to(device)
         if self.tuned:
             model = model.to(torch.bfloat16)
             model.lstm.flatten_parameters()

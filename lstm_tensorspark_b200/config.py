@@ -12,6 +12,7 @@ from __future__ import annotations
 
 import argparse
 import dataclasses
+import warnings
 from dataclasses import dataclass, field
 from typing import List, Optional, Sequence
 
@@ -43,6 +44,8 @@ class Config:
                                         # sample's state after its own last step (padded steps hold the state)
     bidirectional: bool = False         # every layer also runs a reverse-time LSTM; layer l+1 and the classifier read
                                         # [forward | reverse] (2 H wide), as nn.LSTM(bidirectional=True) on a packed sequence
+    dropout: float = 0.0                # nn.LSTM(dropout=P): in training, the output sequence of every layer but the last is
+                                        # multiplied by a Bernoulli(1-P) mask / (1-P) before the next layer reads it
     dtype: str = "auto"                 # auto: bf16 on cuda, fp32 on cpu
     device: str = "auto"                # auto | cpu | cuda
     backend: str = "auto"               # auto | cuda_ext (hand-written sm_90a kernels) | torch
@@ -123,6 +126,11 @@ class Config:
             raise ValueError("--variable_length needs --seq_len >= 2 (the longest sample's number of steps)")
         if self.bidirectional and self.seq_len < 2:
             raise ValueError("--bidirectional needs --seq_len >= 2 (the reverse direction runs over a whole sequence)")
+        if not 0.0 <= self.dropout < 1.0:
+            raise ValueError(f"--dropout must satisfy 0 <= P < 1, got {self.dropout}")
+        if self.dropout > 0 and len(self.hidden_list()) == 1:
+            warnings.warn(f"--dropout {self.dropout} has no effect with one layer: dropout applies between stacked layers "
+                          "(it drops the output of every layer but the last)")
         if self.sync_mode not in ("param_avg", "grad_allreduce", "none"):
             raise ValueError(f"unknown --sync_mode {self.sync_mode}")
         if self.optimizer not in ("adam", "sgd"):

@@ -45,9 +45,12 @@ int ts_gemm_generic(const void*, const void*, void*, const float*, int, int, int
 int ts_gemm2(const void*, const void*, void*, const float*, int, int, int, int, int, int, int, int, int, int, int, int, int,
              const unsigned int*, const int*, unsigned int*, int*, int, int, int, int, cudaStream_t);
 int ts_lstm_seq_fwd(const void*, const void*, const float*, const void*, const float*, void*, const float*, void*, void*, int,
-                    int, int, unsigned int*, int, cudaStream_t, const void*, const unsigned int*, int, int, int, const int*, int);
+                    int, int, unsigned int*, int, cudaStream_t, const void*, const unsigned int*, int, int, int, const int*, int,
+                    void*, const int*, const unsigned int*);
 int ts_lstm_seq_bwd(const void*, const void*, const void*, const float*, const void*, float*, float*, void*, void*, int,
-                    int, int, unsigned int*, int, cudaStream_t, const unsigned int*, int, int, int, const int*, int);
+                    int, int, unsigned int*, int, cudaStream_t, const unsigned int*, int, int, int, const int*, int,
+                    const int*, const unsigned int*);
+int ts_dropout(const void*, void*, int, int, int, int, int, const int*, const unsigned int*, cudaStream_t);
 int ts_lstm_seq_prologue(const void*, const float*, void*, float*, void*, unsigned int*, int, int, cudaStream_t);
 const char* ts_last_error();
 }
@@ -84,6 +87,18 @@ const int* lengths_ptr(const std::optional<Tensor>& lengths, int64_t B, const Te
   TORCH_CHECK(l.is_contiguous(), "lengths must be contiguous");
   return l.data_ptr<int>();
 }
+// Dropout between stacked layers (ts_common.cuh DropSpec): step = the device-resident int32 step counter [1] (None = no
+// dropout), desc = {key0, key1, thr, c2, row0}.  -> counter pointer (null without dropout); desc is converted into `out`.
+const int* drop_args(const std::optional<Tensor>& step, const std::vector<int64_t>& desc, const Tensor& like, unsigned int (&out)[5]) {
+  if (!step.has_value()) return nullptr;
+  TORCH_CHECK(step->is_cuda() && step->device() == like.device() && step->scalar_type() == torch::kInt32 && step->numel() == 1,
+              "dropout: the step counter must be an int32 [1] tensor on the batch's device");
+  TORCH_CHECK(desc.size() == 5, "dropout: desc = {key0, key1, thr, c2, row0}");
+  TORCH_CHECK(desc[2] >= 1 && desc[2] <= 65535 && desc[4] >= 0, "dropout: thr in [1, 65535], row0 >= 0");
+  for (int i = 0; i < 5; ++i) out[i] = (unsigned int)(uint32_t)desc[i];
+  return step->data_ptr<int>();
+}
+
 // Direction of a persistent-kernel launch: reverse = the reverse-time half of a bidirectional layer (h_seq / c_seq row T holds
 // the initial state).  The layer wavefront's dataflow gating (in_gate / extra_signal) is forward-only.
 int direction_flag(bool reverse, const std::optional<Tensor>& in_gate, bool extra_signal) {
@@ -191,6 +206,20 @@ std::vector<Tensor> lstm_pointwise_bwd(const std::optional<Tensor>& dh_a, const 
                               B, H, is_bf16(act), stream(), lp, (int)t, lp ? dh_out.data_ptr<float>() : nullptr), "lstm_pointwise_bwd");
   if (lp) return {dpre, dc, dh_out};
   return {dpre, dc};
+}
+
+// x [..., B, H] (bf16 / fp32, contiguous; the leading dims are time steps t0, t0 + 1, ...) -> x * mask * scale (same dtype):
+// the dropout of the generic path and of the one-step path, forward (x = h) and backward (x = the gradient).
+Tensor dropout(const Tensor& x, const Tensor& step, const std::vector<int64_t>& desc, int64_t t0) {
+  chk_cuda(x, "x");
+  TORCH_CHECK(x.dim() >= 2, "dropout: x must be [..., B, H]");
+  c10::cuda::CUDAGuard g(x.device());
+  unsigned int dd[5];
+  const int* ds = drop_args(step, desc, x, dd);
+  const int64_t B = x.size(-2), H = x.size(-1), steps = B * H ? x.numel() / (B * H) : 0;
+  auto y = torch::empty_like(x);
+  check(ts_dropout(x.data_ptr(), y.data_ptr(), (int)steps, (int)B, (int)H, (int)t0, is_bf16(x), ds, dd, stream()), "dropout");
+  return y;
 }
 
 // ---- head ---------------------------------------------------------------------------------------------------
@@ -367,12 +396,16 @@ Tensor gemm_generic(const Tensor& A, const Tensor& B, const std::optional<Tensor
 std::vector<Tensor> lstm_seq_fwd(const Tensor& gx, const Tensor& w_h, const Tensor& bias, const Tensor& h0,
                                  const Tensor& c0, Tensor sync_ws, int64_t variant, std::optional<Tensor> dbg,
                                  std::optional<Tensor> in_gate, int64_t in_gate_tiles_n, bool extra_signal,
-                                 const std::optional<Tensor>& lengths, bool reverse) {
+                                 const std::optional<Tensor>& lengths, bool reverse, const std::optional<Tensor>& drop_step,
+                                 const std::vector<int64_t>& drop_desc) {
   chk_cuda(gx, "gx"); chk_cuda(w_h, "w_h"); chk_cuda(bias, "bias"); chk_cuda(h0, "h0"); chk_cuda(c0, "c0");
   c10::cuda::CUDAGuard gd(gx.device());
   int T = gx.size(0), B = gx.size(1), H = gx.size(2) / 4;
   const int* lp = lengths_ptr(lengths, B, gx);
   const int rev = direction_flag(reverse, in_gate, extra_signal);
+  unsigned int dd[5];
+  const int* ds = drop_args(drop_step, drop_desc, gx, dd);
+  Tensor h_drop = ds ? torch::empty({T, B, H}, gx.options()) : Tensor();
   auto h_seq = torch::empty({T + 1, B, H}, gx.options());
   auto c_seq = torch::empty({T + 1, B, H}, c0.options());
   auto act = torch::empty({T, B, 4 * H}, gx.options());
@@ -385,7 +418,8 @@ std::vector<Tensor> lstm_seq_fwd(const Tensor& gx, const Tensor& w_h, const Tens
                         act.data_ptr(), c0.data_ptr<float>(), dbg.has_value() ? dbg->data_ptr() : nullptr, tiled.data_ptr(), T, B, H,
                         (unsigned int*)sync_ws.data_ptr<int>(), (int)variant, stream(), h0.data_ptr(),
                         in_gate.has_value() ? (const unsigned int*)in_gate->data_ptr<int>() : nullptr, (int)in_gate_tiles_n,
-                        extra_signal ? 1 : 0, 0, lp, rev), "lstm_seq_fwd");
+                        extra_signal ? 1 : 0, 0, lp, rev, ds ? h_drop.data_ptr() : nullptr, ds, dd), "lstm_seq_fwd");
+  if (ds) return {h_seq, c_seq, act, h_drop};
   return {h_seq, c_seq, act};
 }
 
@@ -395,13 +429,16 @@ std::vector<Tensor> lstm_seq_fwd(const Tensor& gx, const Tensor& w_h, const Tens
 std::vector<Tensor> lstm_seq_bwd(const std::optional<Tensor>& dh_seq, const Tensor& w_hT, const Tensor& act, const Tensor& c_seq,
                                  const Tensor& dhT, const Tensor& dcT, Tensor sync_ws, int64_t variant,
                                  std::optional<Tensor> dbg, std::optional<Tensor> in_gate, int64_t in_gate_tiles_n, bool extra_signal,
-                                 const std::optional<Tensor>& lengths, bool reverse) {
+                                 const std::optional<Tensor>& lengths, bool reverse, const std::optional<Tensor>& drop_step,
+                                 const std::vector<int64_t>& drop_desc) {
   if (dh_seq.has_value()) chk_cuda(*dh_seq, "dh_seq");
   chk_cuda(w_hT, "w_hT"); chk_cuda(act, "act"); chk_cuda(c_seq, "c_seq");
   c10::cuda::CUDAGuard gd(act.device());
   int T = act.size(0), B = act.size(1), H = act.size(2) / 4;
   const int* lp = lengths_ptr(lengths, B, act);
   const int rev = direction_flag(reverse, in_gate, extra_signal);
+  unsigned int dd[5];
+  const int* ds = drop_args(drop_step, drop_desc, act, dd);
   auto dpre = torch::empty_like(act);
   auto dh0 = dhT.clone();
   auto dc0 = dcT.clone();
@@ -411,7 +448,7 @@ std::vector<Tensor> lstm_seq_bwd(const std::optional<Tensor>& dh_seq, const Tens
                         dh0.data_ptr<float>(), dc0.data_ptr<float>(), dbg.has_value() ? dbg->data_ptr() : nullptr, tiled.data_ptr(), T, B, H,
                         (unsigned int*)sync_ws.data_ptr<int>(), (int)variant, stream(),
                         in_gate.has_value() ? (const unsigned int*)in_gate->data_ptr<int>() : nullptr, (int)in_gate_tiles_n,
-                        extra_signal ? 1 : 0, 0, lp, rev), "lstm_seq_bwd");
+                        extra_signal ? 1 : 0, 0, lp, rev, ds, dd), "lstm_seq_bwd");
   return {dpre, dh0, dc0};
 }
 
@@ -420,7 +457,8 @@ std::vector<Tensor> lstm_seq_bwd(const std::optional<Tensor>& dh_seq, const Tens
 void lstm_seq_fwd_into(const Tensor& gx, const Tensor& w_h, const Tensor& bias, const Tensor& h0, const Tensor& c0, Tensor h_seq,
                        Tensor c_seq, Tensor act, Tensor tiled, Tensor sync_ws, int64_t variant, std::optional<Tensor> in_gate,
                        int64_t in_gate_tiles_n, bool extra_signal, int64_t stream_handle, int64_t launch_flags,
-                       const std::optional<Tensor>& lengths, bool reverse) {
+                       const std::optional<Tensor>& lengths, bool reverse, const std::optional<Tensor>& h_drop,
+                       const std::optional<Tensor>& drop_step, const std::vector<int64_t>& drop_desc) {
   chk_cuda(gx, "gx"); chk_cuda(w_h, "w_h"); chk_cuda(bias, "bias"); chk_cuda(h0, "h0"); chk_cuda(c0, "c0");
   chk_cuda(h_seq, "h_seq"); chk_cuda(c_seq, "c_seq"); chk_cuda(act, "act"); chk_cuda(tiled, "tiled");
   c10::cuda::CUDAGuard gd(gx.device());
@@ -430,11 +468,18 @@ void lstm_seq_fwd_into(const Tensor& gx, const Tensor& w_h, const Tensor& bias, 
   TORCH_CHECK(h_seq.numel() == (int64_t)(T + 1) * B * H && c_seq.numel() == h_seq.numel() && act.numel() == gx.numel(), "lstm_seq_fwd_into: buffer sizes");
   TORCH_CHECK(tiled.numel() == (int64_t)(T + 1) * ((B + 127) / 128) * 128 * H, "lstm_seq_fwd_into: tile-image buffer size");
   TORCH_CHECK(h0.scalar_type() == torch::kBFloat16 && c0.scalar_type() == torch::kFloat32, "h0 bf16 / c0 fp32");
+  unsigned int dd[5];
+  const int* ds = drop_args(drop_step, drop_desc, gx, dd);
+  if (ds) {
+    TORCH_CHECK(h_drop.has_value(), "lstm_seq_fwd_into: dropout needs h_drop");
+    chk_cuda(*h_drop, "h_drop");
+    TORCH_CHECK(h_drop->scalar_type() == gx.scalar_type() && h_drop->numel() == (int64_t)T * B * H, "lstm_seq_fwd_into: h_drop [T,B,H]");
+  }
   check(ts_lstm_seq_fwd(gx.data_ptr(), w_h.data_ptr(), bias.data_ptr<float>(), h_seq.data_ptr(), c_seq.data_ptr<float>(),
                         act.data_ptr(), c0.data_ptr<float>(), nullptr, tiled.data_ptr(), T, B, H, (unsigned int*)sync_ws.data_ptr<int>(),
                         (int)variant, stream_handle ? (cudaStream_t)stream_handle : stream(), h0.data_ptr(),
                         in_gate.has_value() ? (const unsigned int*)in_gate->data_ptr<int>() : nullptr, (int)in_gate_tiles_n,
-                        extra_signal ? 1 : 0, (int)launch_flags, lp, rev), "lstm_seq_fwd_into");
+                        extra_signal ? 1 : 0, (int)launch_flags, lp, rev, ds ? h_drop->data_ptr() : nullptr, ds, dd), "lstm_seq_fwd_into");
 }
 
 // h_seq[0] <- h0, c_seq[0] <- c0 (reverse: row T), tile image of h0, step counters <- 0 (what lstm_seq_fwd does first unless
@@ -453,7 +498,8 @@ void lstm_seq_prologue(const Tensor& h0, const Tensor& c0, Tensor h_seq, Tensor 
 void lstm_seq_bwd_into(const std::optional<Tensor>& dh_seq, const Tensor& w_hT, const Tensor& act, const Tensor& c_seq, Tensor dpre,
                        Tensor dh0, Tensor dc0, Tensor tiled, Tensor sync_ws, int64_t variant, std::optional<Tensor> in_gate,
                        int64_t in_gate_tiles_n, bool extra_signal, int64_t stream_handle, int64_t launch_flags,
-                       const std::optional<Tensor>& lengths, bool reverse) {
+                       const std::optional<Tensor>& lengths, bool reverse, const std::optional<Tensor>& drop_step,
+                       const std::vector<int64_t>& drop_desc) {
   chk_cuda(w_hT, "w_hT"); chk_cuda(act, "act"); chk_cuda(c_seq, "c_seq"); chk_cuda(dpre, "dpre"); chk_cuda(dh0, "dh0"); chk_cuda(dc0, "dc0");
   c10::cuda::CUDAGuard gd(act.device());
   int T = act.size(0), B = act.size(1), H = act.size(2) / 4;
@@ -461,11 +507,13 @@ void lstm_seq_bwd_into(const std::optional<Tensor>& dh_seq, const Tensor& w_hT, 
   const int rev = direction_flag(reverse, in_gate, extra_signal);
   TORCH_CHECK(dpre.numel() == act.numel() && tiled.numel() == (int64_t)T * ((B + 127) / 128) * 128 * 4 * H, "lstm_seq_bwd_into: buffer sizes");
   TORCH_CHECK(dh0.scalar_type() == torch::kFloat32 && dc0.scalar_type() == torch::kFloat32 && dh0.numel() == (int64_t)B * H && dc0.numel() == (int64_t)B * H, "dh0/dc0 fp32 [B,H]");
+  unsigned int dd[5];
+  const int* ds = drop_args(drop_step, drop_desc, act, dd);
   check(ts_lstm_seq_bwd(dh_seq.has_value() ? dh_seq->data_ptr() : nullptr, w_hT.data_ptr(), act.data_ptr(), c_seq.data_ptr<float>(), dpre.data_ptr(),
                         dh0.data_ptr<float>(), dc0.data_ptr<float>(), nullptr, tiled.data_ptr(), T, B, H, (unsigned int*)sync_ws.data_ptr<int>(),
                         (int)variant, stream_handle ? (cudaStream_t)stream_handle : stream(),
                         in_gate.has_value() ? (const unsigned int*)in_gate->data_ptr<int>() : nullptr, (int)in_gate_tiles_n,
-                        extra_signal ? 1 : 0, (int)launch_flags, lp, rev), "lstm_seq_bwd_into");
+                        extra_signal ? 1 : 0, (int)launch_flags, lp, rev, ds, dd), "lstm_seq_bwd_into");
 }
 
 }  // namespace
@@ -520,18 +568,23 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("fold_cols") = 0);
   m.def("lstm_seq_fwd", &lstm_seq_fwd, py::arg("gx"), py::arg("w_h"), py::arg("bias"), py::arg("h0"), py::arg("c0"),
         py::arg("sync_ws"), py::arg("variant") = 0, py::arg("dbg") = py::none(), py::arg("in_gate") = py::none(),
-        py::arg("in_gate_tiles_n") = 0, py::arg("extra_signal") = false, py::arg("lengths") = py::none(), py::arg("reverse") = false);
+        py::arg("in_gate_tiles_n") = 0, py::arg("extra_signal") = false, py::arg("lengths") = py::none(), py::arg("reverse") = false,
+        py::arg("drop_step") = py::none(), py::arg("drop_desc") = std::vector<int64_t>{});
   m.def("lstm_seq_fwd_into", &lstm_seq_fwd_into, py::arg("gx"), py::arg("w_h"), py::arg("bias"), py::arg("h0"), py::arg("c0"),
         py::arg("h_seq"), py::arg("c_seq"), py::arg("act"), py::arg("tiled"), py::arg("sync_ws"), py::arg("variant"),
         py::arg("in_gate") = py::none(), py::arg("in_gate_tiles_n") = 0, py::arg("extra_signal") = false, py::arg("stream") = 0,
-        py::arg("launch_flags") = 0, py::arg("lengths") = py::none(), py::arg("reverse") = false);
+        py::arg("launch_flags") = 0, py::arg("lengths") = py::none(), py::arg("reverse") = false, py::arg("h_drop") = py::none(),
+        py::arg("drop_step") = py::none(), py::arg("drop_desc") = std::vector<int64_t>{});
   m.def("lstm_seq_prologue", &lstm_seq_prologue, py::arg("h0"), py::arg("c0"), py::arg("h_seq"), py::arg("c_seq"), py::arg("tiled"),
         py::arg("sync_ws"), py::arg("reverse") = false);
   m.def("lstm_seq_bwd_into", &lstm_seq_bwd_into, py::arg("dh_seq"), py::arg("w_hT"), py::arg("act"), py::arg("c_seq"), py::arg("dpre"),
         py::arg("dh0"), py::arg("dc0"), py::arg("tiled"), py::arg("sync_ws"), py::arg("variant"), py::arg("in_gate") = py::none(),
         py::arg("in_gate_tiles_n") = 0, py::arg("extra_signal") = false, py::arg("stream") = 0, py::arg("launch_flags") = 0,
-        py::arg("lengths") = py::none(), py::arg("reverse") = false);
+        py::arg("lengths") = py::none(), py::arg("reverse") = false, py::arg("drop_step") = py::none(),
+        py::arg("drop_desc") = std::vector<int64_t>{});
   m.def("lstm_seq_bwd", &lstm_seq_bwd, py::arg("dh_seq"), py::arg("w_hT"), py::arg("act"), py::arg("c_seq"), py::arg("dhT"),
         py::arg("dcT"), py::arg("sync_ws"), py::arg("variant") = 0, py::arg("dbg") = py::none(), py::arg("in_gate") = py::none(),
-        py::arg("in_gate_tiles_n") = 0, py::arg("extra_signal") = false, py::arg("lengths") = py::none(), py::arg("reverse") = false);
+        py::arg("in_gate_tiles_n") = 0, py::arg("extra_signal") = false, py::arg("lengths") = py::none(), py::arg("reverse") = false,
+        py::arg("drop_step") = py::none(), py::arg("drop_desc") = std::vector<int64_t>{});
+  m.def("dropout", &dropout, py::arg("x"), py::arg("step"), py::arg("desc"), py::arg("t0") = 0);
 }

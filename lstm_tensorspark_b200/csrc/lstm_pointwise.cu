@@ -130,6 +130,47 @@ extern "C" int ts_lstm_pointwise_bwd(const void* dh_a, const float* dh_b, const 
 }
 
 
+// Dropout between stacked layers, standalone: y = x * mask * scale over [T,B,H] (time t0 + t), the mask of ts::dropout_keep8.
+// The same launch serves the forward (x = h, stored in x's dtype) and the backward (x = dL/dy) of the shapes the persistent
+// kernels do not fuse it into: the generic path (fp32, H % 64 != 0), the one-step [B,D] path and anything else.  One thread
+// per Philox group (8 units of one row).
+namespace {
+template <typename T>
+__global__ void dropout_kernel(const T* __restrict__ x, T* __restrict__ y, int steps, int B, int H, int t0, ts::DropSpec d) {
+  const int groups = (H + 7) / 8;
+  const long long total = (long long)steps * B * groups;
+  const uint32_t step = (uint32_t)__ldg(d.step);
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int g = (int)(i % groups);
+    const long long tb = i / groups;
+    const int b = (int)(tb % B), t = (int)(tb / B);
+    const uint32_t keep = ts::dropout_keep8(d, step, b, 8 * g, t0 + t, H);
+    const size_t base = (size_t)tb * H + 8 * g;
+#pragma unroll
+    for (int u = 0; u < 8; ++u) {
+      if (8 * g + u >= H) break;
+      y[base + u] = ((keep >> u) & 1u) ? ts::Cvt<T>::from_f(__fmul_rn(ts::Cvt<T>::to_f(x[base + u]), d.scale)) : ts::Cvt<T>::from_f(0.f);
+    }
+  }
+}
+}  // namespace
+
+extern "C" int ts_dropout(const void* x, void* y, int steps, int B, int H, int t0, int is_bf16, const int* drop_step,
+                          const unsigned int* drop_desc, cudaStream_t st) {
+  if (drop_step == nullptr) return -2;
+  const ts::DropSpec d = ts::make_drop_spec(drop_step, drop_desc);
+  const long long total = (long long)steps * B * ((H + 7) / 8);
+  int blocks = (int)((total + 255) / 256);
+  if (blocks > 132 * 8) blocks = 132 * 8;
+  if (blocks < 1) return 0;
+  if (is_bf16)
+    dropout_kernel<__nv_bfloat16><<<blocks, 256, 0, st>>>((const __nv_bfloat16*)x, (__nv_bfloat16*)y, steps, B, H, t0, d);
+  else
+    dropout_kernel<float><<<blocks, 256, 0, st>>>((const float*)x, (float*)y, steps, B, H, t0, d);
+  return (int)cudaGetLastError();
+}
+
+
 // [B,T,D] -> [T,B,D] for a row-contiguous tensor (row = D elements, row_bytes % 16 == 0): a pure row permutation, so it
 // runs at copy speed with 16 B vectors (the framework's generic strided copy of the transposed view takes 3.5x longer).
 // Replaces the batch-major -> time-major feed conversion in front of the first layer's x-projection GEMM.

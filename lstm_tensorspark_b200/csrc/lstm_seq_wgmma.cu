@@ -228,6 +228,10 @@ struct SeqParams {
   const int* lengths;          // [B] valid steps per row (right padding, 1 <= len <= T); null = every row runs all T steps.  Read
                                // only by the kMasked instantiations: at a step t >= len the cell holds its state (h, c carried
                                // over) and the backward pass emits a zero gate gradient and passes dh / dc through unchanged.
+  // Dropout between stacked layers (kDrop instantiations only): the forward pass also writes h_drop [T,B,H] (time order, mask
+  // drop applied to the stored bf16 h), the backward pass applies the same mask to dh_seq as it loads it.
+  __nv_bfloat16* h_drop;
+  ts::DropSpec drop;
 };
 
 // Work decomposition
@@ -279,7 +283,12 @@ struct SeqParams {
 // (a_tiled), the dataflow counters and the exchange stay in processing order.  With kMasked a row's padded steps
 // (tau >= len) come FIRST in the forward pass (the cell holds h0 / c0 there) and LAST in the backward pass (dh / dc carry
 // through them into dh0 / dc0).  Not combined with the layer wavefront (in_gate / extra_signal; the host rejects it).
-template <bool kBwd, int kStages, int kTiles, bool kStream, bool kFSplit = false, bool kMasked = false, bool kRev = false>
+// kDrop: dropout on this layer's output sequence (SeqParams::drop).  Forward: h_drop is stored in the bookkeeping block, next to
+// h_seq, so whatever gates on h_seq's natural-layout rows (the pair's gx_b GEMM, extra_signal) covers it too.  Backward: the
+// dropped units of dh_seq are zeroed as it is loaded (before the MMAs of the step) and the kept ones scaled in fp32 where dh
+// joins the carry.  A separate instantiation: the kernels without it are those of a build without dropout.
+template <bool kBwd, int kStages, int kTiles, bool kStream, bool kFSplit = false, bool kMasked = false, bool kRev = false,
+          bool kDrop = false>
 __global__ void __launch_bounds__(384, 1)
 lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
   static_assert(!(kFSplit && (kBwd || kStream || kTiles != 1)), "forward K-split: one tile, resident weights");
@@ -849,6 +858,10 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
 #pragma unroll
           for (int u = 0; u < kPass; ++u) {
             stg16(p.h_seq + (srow * B + row) * H + j0(u), h8[u]);
+            if constexpr (kDrop) {                     // this thread's 8 units of row `row` are one Philox group
+              const uint32_t keep = ts::dropout_keep8(p.drop, (uint32_t)__ldg(p.drop.step), row, j0(u), tt, H);
+              stg16(p.h_drop + ((size_t)tt * B + row) * H + j0(u), ts::dropout_bf16x8(h8[u], keep, p.drop.scale));
+            }
             float* cp = p.c_seq + (srow * B + row) * H + j0(u);
             stg32(cp, __float_as_uint(cn[u][0]), __float_as_uint(cn[u][1]), __float_as_uint(cn[u][2]), __float_as_uint(cn[u][3]),
                   __float_as_uint(cn[u][4]), __float_as_uint(cn[u][5]), __float_as_uint(cn[u][6]), __float_as_uint(cn[u][7]));
@@ -919,6 +932,8 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
             if (!pad) { avw[u][0] = ldg_nc32(ap); avw[u][1] = ldg_nc32(ap + 16); }
             dhv[u] = p.dh_seq ? (p.in_gate ? ldg_cg16(p.dh_seq + ((size_t)t * B + row) * H + j0(u)) : ldg_nc16(p.dh_seq + ((size_t)tt * B + row) * H + j0(u)))
                               : make_uint4(0u, 0u, 0u, 0u);
+            if constexpr (kDrop)                       // dropped units of dh_seq[tt] -> 0; kept ones are scaled where dh joins the carry
+              dhv[u] = ts::dropout_zero_bf16x8(dhv[u], ts::dropout_keep8(p.drop, (uint32_t)__ldg(p.drop.step), row, j0(u), tt, H));
             // c_prev / c_new of step tt (kRev: rows tt + 1 / tt).  c_new is the previous iteration's c_prev in both directions.
             const float* c0p = p.c_seq + ((size_t)(kRev ? tt + 1 : t) * B + row) * H + j0(u);
             const float* c1p = p.c_seq + ((size_t)(kRev ? tt : t + 1) * B + row) * H + j0(u);
@@ -1026,7 +1041,8 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
             const uint32_t aa = avw[u][jj >> 2].v[2 * (jj & 3)], ab = avw[u][jj >> 2].v[2 * (jj & 3) + 1];
             const float ig = bf_lo(aa), fg = bf_hi(aa), gg = bf_lo(ab), og = bf_hi(ab);
             const uint32_t dw = (jj >> 1) == 0 ? dhv[u].x : (jj >> 1) == 1 ? dhv[u].y : (jj >> 1) == 2 ? dhv[u].z : dhv[u].w;
-            const float dht = dh[u][jj] + ((jj & 1) ? bf_hi(dw) : bf_lo(dw));
+            const float dsj = (jj & 1) ? bf_hi(dw) : bf_lo(dw);
+            const float dht = dh[u][jj] + (kDrop ? __fmul_rn(dsj, p.drop.scale) : dsj);
             const float cprev = __uint_as_float(cpv[u].v[jj]);
             const float tcn = ts::tanhf_fast(__uint_as_float(cnv[u].v[jj]));
             const float dc_in = dc[u][jj];
@@ -1134,9 +1150,10 @@ size_t smem_bytes(int H, bool bwd, int stages, int tiles, bool stream = false, b
   return (stream ? 0 : (size_t)(H / BK) * kWBlockBytes) + ring + ((bwd || fsplit) ? tiles * kXchgBytes : 0) + acc_stage + sizeof(SeqSmem) + 1024;
 }
 
-template <bool kBwd, int kStages, int kTiles, bool kStream = false, bool kFSplit = false, bool kMasked = false, bool kRev = false>
+template <bool kBwd, int kStages, int kTiles, bool kStream = false, bool kFSplit = false, bool kMasked = false, bool kRev = false,
+          bool kDrop = false>
 int launch_cfg(const CUtensorMap& tw, const SeqParams& p, int grid, cudaStream_t st) {
-  auto kern = lstm_seq_kernel<kBwd, kStages, kTiles, kStream, kFSplit, kMasked, kRev>;
+  auto kern = lstm_seq_kernel<kBwd, kStages, kTiles, kStream, kFSplit, kMasked, kRev, kDrop>;
   const size_t smem = smem_bytes(p.H, kBwd, kStages, kTiles, kStream, kFSplit);
   constexpr int kClusterDim = kBwd ? (kStream ? 2 : 4) : (kFSplit ? 2 : 1);
   if (smem > 227 * 1024) return -4;
@@ -1163,45 +1180,54 @@ int launch_cfg(const CUtensorMap& tw, const SeqParams& p, int grid, cudaStream_t
   return (int)e;
 }
 
-template <bool kBwd, bool kMasked, bool kRev>
+template <bool kBwd, bool kMasked, bool kRev, bool kDrop>
 int dispatch(const CUtensorMap& tw, const SeqParams& p, int grid, int stages, int tiles, bool stream, bool fsplit, cudaStream_t st) {
   if constexpr (!kBwd) {
     if (fsplit) {                                  // forward K-split (cluster of 2), one batch tile per CTA
       switch (stages) {
-        case 3: return launch_cfg<false, 3, 1, false, true, kMasked, kRev>(tw, p, grid, st);
-        case 4: return launch_cfg<false, 4, 1, false, true, kMasked, kRev>(tw, p, grid, st);
-        case 5: return launch_cfg<false, 5, 1, false, true, kMasked, kRev>(tw, p, grid, st);
-        case 6: return launch_cfg<false, 6, 1, false, true, kMasked, kRev>(tw, p, grid, st);
+        case 3: return launch_cfg<false, 3, 1, false, true, kMasked, kRev, kDrop>(tw, p, grid, st);
+        case 4: return launch_cfg<false, 4, 1, false, true, kMasked, kRev, kDrop>(tw, p, grid, st);
+        case 5: return launch_cfg<false, 5, 1, false, true, kMasked, kRev, kDrop>(tw, p, grid, st);
+        case 6: return launch_cfg<false, 6, 1, false, true, kMasked, kRev, kDrop>(tw, p, grid, st);
       }
       return -5;
     }
   }
   if (stream) {                                    // streamed weights: 24 KB stages, one batch tile per CTA
     switch (stages) {
-      case 4: return launch_cfg<kBwd, 4, 1, true, false, kMasked, kRev>(tw, p, grid, st);
-      case 6: return launch_cfg<kBwd, 6, 1, true, false, kMasked, kRev>(tw, p, grid, st);
-      case 8: return launch_cfg<kBwd, 8, 1, true, false, kMasked, kRev>(tw, p, grid, st);
+      case 4: return launch_cfg<kBwd, 4, 1, true, false, kMasked, kRev, kDrop>(tw, p, grid, st);
+      case 6: return launch_cfg<kBwd, 6, 1, true, false, kMasked, kRev, kDrop>(tw, p, grid, st);
+      case 8: return launch_cfg<kBwd, 8, 1, true, false, kMasked, kRev, kDrop>(tw, p, grid, st);
     }
     return -5;
   }
   if (tiles == 2) {
     switch (stages) {
-      case 2: return launch_cfg<kBwd, 2, 2, false, false, kMasked, kRev>(tw, p, grid, st);
-      case 3: return launch_cfg<kBwd, 3, 2, false, false, kMasked, kRev>(tw, p, grid, st);
-      case 4: return launch_cfg<kBwd, 4, 2, false, false, kMasked, kRev>(tw, p, grid, st);
-      case 5: return launch_cfg<kBwd, 5, 2, false, false, kMasked, kRev>(tw, p, grid, st);
-      case 6: return launch_cfg<kBwd, 6, 2, false, false, kMasked, kRev>(tw, p, grid, st);
+      case 2: return launch_cfg<kBwd, 2, 2, false, false, kMasked, kRev, kDrop>(tw, p, grid, st);
+      case 3: return launch_cfg<kBwd, 3, 2, false, false, kMasked, kRev, kDrop>(tw, p, grid, st);
+      case 4: return launch_cfg<kBwd, 4, 2, false, false, kMasked, kRev, kDrop>(tw, p, grid, st);
+      case 5: return launch_cfg<kBwd, 5, 2, false, false, kMasked, kRev, kDrop>(tw, p, grid, st);
+      case 6: return launch_cfg<kBwd, 6, 2, false, false, kMasked, kRev, kDrop>(tw, p, grid, st);
     }
   } else {
     switch (stages) {
-      case 2: return launch_cfg<kBwd, 2, 1, false, false, kMasked, kRev>(tw, p, grid, st);
-      case 3: return launch_cfg<kBwd, 3, 1, false, false, kMasked, kRev>(tw, p, grid, st);
-      case 4: return launch_cfg<kBwd, 4, 1, false, false, kMasked, kRev>(tw, p, grid, st);
-      case 5: return launch_cfg<kBwd, 5, 1, false, false, kMasked, kRev>(tw, p, grid, st);
-      case 6: return launch_cfg<kBwd, 6, 1, false, false, kMasked, kRev>(tw, p, grid, st);
+      case 2: return launch_cfg<kBwd, 2, 1, false, false, kMasked, kRev, kDrop>(tw, p, grid, st);
+      case 3: return launch_cfg<kBwd, 3, 1, false, false, kMasked, kRev, kDrop>(tw, p, grid, st);
+      case 4: return launch_cfg<kBwd, 4, 1, false, false, kMasked, kRev, kDrop>(tw, p, grid, st);
+      case 5: return launch_cfg<kBwd, 5, 1, false, false, kMasked, kRev, kDrop>(tw, p, grid, st);
+      case 6: return launch_cfg<kBwd, 6, 1, false, false, kMasked, kRev, kDrop>(tw, p, grid, st);
     }
   }
   return -5;
+}
+
+template <bool kBwd, bool kDrop>
+int dispatch_dir(const CUtensorMap& tw, const SeqParams& p, int grid, int stages, int tiles, bool stream, bool fsplit, cudaStream_t st,
+                 bool reverse) {
+  return reverse ? (p.lengths ? dispatch<kBwd, true, true, kDrop>(tw, p, grid, stages, tiles, stream, fsplit, st)
+                              : dispatch<kBwd, false, true, kDrop>(tw, p, grid, stages, tiles, stream, fsplit, st))
+                 : (p.lengths ? dispatch<kBwd, true, false, kDrop>(tw, p, grid, stages, tiles, stream, fsplit, st)
+                              : dispatch<kBwd, false, false, kDrop>(tw, p, grid, stages, tiles, stream, fsplit, st));
 }
 
 int pick_stages(int H, bool bwd, int tiles) {
@@ -1282,10 +1308,8 @@ static int seq_common(SeqParams& p, const void* w_base, int variant, cudaStream_
   if (int rc = ts::make_tmap_2d_bf16(&tw, w_base, (uint64_t)N, (uint64_t)K, (uint64_t)K, BK, fsplit ? 2 * BN : ((kBwd && stream) ? BN / 2 : BN))) return rc;
   p.tiles_n = tiles_n;
   p.tiles_m = tiles_m;
-  int rc = reverse ? (p.lengths ? dispatch<kBwd, true, true>(tw, p, grid, stages, tiles, stream, fsplit, st)
-                                : dispatch<kBwd, false, true>(tw, p, grid, stages, tiles, stream, fsplit, st))
-                   : (p.lengths ? dispatch<kBwd, true, false>(tw, p, grid, stages, tiles, stream, fsplit, st)
-                                : dispatch<kBwd, false, false>(tw, p, grid, stages, tiles, stream, fsplit, st));
+  int rc = p.drop.step ? dispatch_dir<kBwd, true>(tw, p, grid, stages, tiles, stream, fsplit, st, reverse)
+                       : dispatch_dir<kBwd, false>(tw, p, grid, stages, tiles, stream, fsplit, st, reverse);
   if (rc == -21) ts::set_last_error("lstm_seq: the thread-block clusters are not co-resident on this device");
   return rc;
 }
@@ -1293,7 +1317,7 @@ static int seq_common(SeqParams& p, const void* w_base, int variant, cudaStream_
 extern "C" int ts_lstm_seq_fwd(const void* gx, const void* w_h, const float* bias, const void* h_seq, const float* c_seq,
                                void* act, const float* c0, void* dbg, void* a_tiled, int T, int B, int H, unsigned int* sync_ws, int variant,
                                cudaStream_t st, const void* h0, const unsigned int* in_gate, int in_gate_tiles_n, int extra_signal, int launch_flags,
-                               const int* lengths, int reverse) {
+                               const int* lengths, int reverse, void* h_drop, const int* drop_step, const unsigned int* drop_desc) {
   if (!(launch_flags & 1)) {           // bit 0: the caller has run ts_lstm_seq_prologue itself (wavefront: all prologues precede the chain)
     const int tiles_m = (B + BM - 1) / BM;
     const int total = tiles_m * BM * (H / 8);
@@ -1310,6 +1334,8 @@ extern "C" int ts_lstm_seq_fwd(const void* gx, const void* w_h, const float* bia
   p.in_gate = in_gate; p.in_gate_tiles_n = in_gate_tiles_n; p.extra_signal = extra_signal;
   p.pdl_wait = (launch_flags >> 1) & 1;
   p.lengths = lengths;
+  p.h_drop = (__nv_bfloat16*)h_drop;
+  p.drop = ts::make_drop_spec(drop_step, drop_desc);
   return seq_common<false>(p, w_h, variant, st, reverse != 0);
 }
 
@@ -1335,7 +1361,7 @@ extern "C" int ts_lstm_seq_prologue(const void* h0, const float* c0, void* h_seq
 extern "C" int ts_lstm_seq_bwd(const void* dh_seq, const void* w_hT, const void* act, const float* c_seq, const void* dpre,
                                float* dh0, float* dc0, void* dbg, void* a_tiled, int T, int B, int H, unsigned int* sync_ws, int variant,
                                cudaStream_t st, const unsigned int* in_gate, int in_gate_tiles_n, int extra_signal, int launch_flags,
-                               const int* lengths, int reverse) {
+                               const int* lengths, int reverse, const int* drop_step, const unsigned int* drop_desc) {
   if (!(launch_flags & 1)) cudaMemsetAsync(sync_ws, 0, kSyncErr * sizeof(unsigned int), st);      // arrival counters restart at 0 every launch
   SeqParams p{};
   p.a_tiled = (__nv_bfloat16*)a_tiled;
@@ -1344,6 +1370,7 @@ extern "C" int ts_lstm_seq_bwd(const void* dh_seq, const void* w_hT, const void*
   p.in_gate = in_gate; p.in_gate_tiles_n = in_gate_tiles_n; p.extra_signal = extra_signal;
   p.pdl_wait = (launch_flags >> 1) & 1;
   p.lengths = lengths;
+  p.drop = ts::make_drop_spec(drop_step, drop_desc);
   return seq_common<true>(p, w_hT, variant, st, reverse != 0);
 }
 

@@ -32,7 +32,7 @@ _BUCKET_PDL = _os.environ.get("LSTM_TS_BUCKET_PDL", "1") == "1"      # 0: bucket
 class TrainEngine:
     def __init__(self, cfg: Config, rank: int = 0, world_size: int = 1, comm: Optional[Communicator] = None,
                  batch_size: Optional[int] = None, device: Optional[torch.device] = None,
-                 dtype: Optional[torch.dtype] = None, train_optimizer=None):
+                 dtype: Optional[torch.dtype] = None, train_optimizer=None, partition_key: Optional[int] = None):
         self.cfg = cfg
         self.rank, self.world_size = rank, world_size
         self.comm = comm or Communicator(0, 1)
@@ -76,6 +76,13 @@ class TrainEngine:
         self._bound = {}                        # (x ptr, y ptr, lengths ptr, shape) -> (graph captured on those buffers, its loss)
         self._bound_keepalive = []
         self.steps_done = 0
+        # dropout between layers: the mask is keyed on (seed, partition) and on the number of training steps this engine has
+        # completed - a counter of its own, device-resident on the GPU (a captured graph advances it; the optimizer's step_dev is
+        # bumped before backward by the fused allreduce and never by SGD), a host int on the CPU
+        rnn = self.model.rnn
+        self._dropout_on = rnn.dropout > 0 and len(rnn.layers) > 1
+        rnn.dropout_key = (cfg.seed & 0xFFFFFFFF, rank if partition_key is None else int(partition_key))
+        rnn.dropout_step = torch.zeros(1, dtype=torch.int32, device=device) if device.type == "cuda" else 0
 
     # ---------------------------------------------------------------------------------------------------
     def _make_bucket_plan(self):
@@ -154,7 +161,25 @@ class TrainEngine:
                 self.optimizer.step()
         if l2 is not None:
             loss = loss.detach() + l2
+        if self._dropout_on:
+            self._bump_dropout_step()
         return loss.detach()
+
+    def _bump_dropout_step(self):
+        rnn = self.model.rnn
+        if isinstance(rnn.dropout_step, torch.Tensor):
+            from .ops.cuda_ext import ext
+            ext().ar_bump_step(rnn.dropout_step)          # a one-thread kernel: inside a captured step it runs on every replay
+        else:
+            rnn.dropout_step += 1
+
+    def set_dropout_step(self, n: int):
+        """Steps completed, for the dropout masks (a resumed run draws the masks the uninterrupted run would have)."""
+        rnn = self.model.rnn
+        if isinstance(rnn.dropout_step, torch.Tensor):
+            rnn.dropout_step.fill_(int(n))
+        else:
+            rnn.dropout_step = int(n)
 
     def step(self, x: torch.Tensor, y: torch.Tensor, lengths: Optional[torch.Tensor] = None) -> torch.Tensor:
         """One full training step on this replica; returns the (detached, device) loss.  ``lengths``: optional int32 ``[B]``
@@ -214,7 +239,8 @@ class TrainEngine:
         opt = self.optimizer
         snap = {"data": self.flat.data.clone(), "step_count": opt.step_count,
                 "m": None if opt.m is None else opt.m.clone(), "v": None if opt.v is None else opt.v.clone(),
-                "step_dev": None if opt.step_dev is None else opt.step_dev.clone()}
+                "step_dev": None if opt.step_dev is None else opt.step_dev.clone(),
+                "dropout_step": self.model.rnn.dropout_step.clone()}
         s = torch.cuda.Stream()
         s.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(s):
@@ -241,13 +267,20 @@ class TrainEngine:
                 opt.m.copy_(snap["m"]); opt.v.copy_(snap["v"])
             if snap["step_dev"] is not None:
                 opt.step_dev.copy_(snap["step_dev"])
+            self.model.rnn.dropout_step.copy_(snap["dropout_step"])
             opt.step_count = snap["step_count"]
         self._graph, self._static, self._bound = g, (sx, sy, sl, sloss), bound
         return g
 
     @torch.no_grad()
     def evaluate(self, x: torch.Tensor, y: torch.Tensor, lengths: Optional[torch.Tensor] = None):
-        h = self.model.features(x, lengths)
-        logits = self.model.head(h)
+        """Loss and accuracy of a batch with the model in eval mode (no dropout)."""
+        was_training = self.model.training
+        self.model.eval()
+        try:
+            h = self.model.features(x, lengths)
+            logits = self.model.head(h)
+        finally:
+            self.model.train(was_training)
         from .ops import reference as ref
         return ref.softmax_xent(logits, y), ref.accuracy(logits, y)

@@ -43,7 +43,7 @@ class SequenceClassifier(nn.Module):
         settings = cfg.net_settings(bs)
         head_in = settings[-1]["num_hidden"] * (2 if cfg.bidirectional else 1)
         head_std = cfg.init_std if cfg.init != "scaled" else cfg.init_std / (head_in ** 0.5)
-        self.rnn = RNN(settings, learn_initial_state=cfg.resolved_learn_initial_state(), init_std=cfg.init_std,
+        self.rnn = RNN(settings, dropout=cfg.dropout, learn_initial_state=cfg.resolved_learn_initial_state(), init_std=cfg.init_std,
                        init=cfg.init, weight_decay=(cfg.weight_decay or None), device=device, generator=generator)
         self.head = DenseHead(head_in, cfg.num_classes, init_std=head_std, device=device, generator=generator)
         if cfg.bidirectional:

@@ -147,27 +147,30 @@ class LSTMLayer(nn.Module):
     def restore_state(self):
         self._set_state(self.state[-1][0], self.state[-1][1])
 
-    def fit_next(self, data: torch.Tensor, train: bool = True) -> torch.Tensor:
+    def fit_next(self, data: torch.Tensor, train: bool = True, dropout=None) -> torch.Tensor:
+        """One step.  ``dropout``: optional ``ops.reference.DropoutSpec`` of the returned output (time 0); the carried state
+        is not dropped."""
         self.train_layer(data)
+        out = F.dropout(self.ht, dropout)
         if train:
             self.state.append((self.ht, self.Ct))
-            return self.ht
-        out = self.ht
+            return out
         if self.state:
             self.restore_state()       # roll back: a non-train step must not advance the recurrence
         return out
 
     # ---- whole-sequence path (the thing the persistent kernel implements) ----------------------
-    def fit_sequence(self, x_seq: torch.Tensor, lengths: Optional[torch.Tensor] = None) -> torch.Tensor:
+    def fit_sequence(self, x_seq: torch.Tensor, lengths: Optional[torch.Tensor] = None, dropout=None) -> torch.Tensor:
         """``x_seq [T,B,D]`` -> ``h_seq [T,B,H]``; final (ht, Ct) stored on the layer.  ``lengths`` (int32 ``[B]``, right
         padding): the final state is each row's state after its own last step; padded positions of ``h_seq`` carry it.
         A reverse layer runs from the last step to the first: its final state is the one after step 0, and its padded
-        positions hold the initial state."""
+        positions hold the initial state.  ``dropout``: optional ``ops.reference.DropoutSpec``; the returned sequence is then
+        the dropped one (the final state is not dropped)."""
         B = x_seq.shape[1]
         if B != self.ht.shape[0]:
             self.reset_state(B)
         h_seq, h_T, c_T = F.lstm_layer_sequence(x_seq, self.ht, self.Ct, self.w_x, self.w_h, self.bias, lengths=lengths,
-                                                reverse=self.reverse)
+                                                reverse=self.reverse, dropout=dropout)
         self._set_state(h_T, c_T)
         self.state.append((h_T, c_T))
         return h_seq

@@ -5,7 +5,8 @@ Public surface mirrors original src/models/recurrent/rnn.py:5-53: ``RNN(settings
 ``settings`` is the list of dicts built by ``Config.net_settings`` (keys ``layer_name``, ``dim_size``,
 ``num_hidden``, ``batch_size``).  New: ``fit_layers`` also accepts a sequence ``[B,T,D]`` and unrolls it
 through time on the fused per-layer sequence op (the reference only ever takes one step), and
-``add_reverse_layers()`` makes the stack bidirectional.
+``add_reverse_layers()`` makes the stack bidirectional, and ``dropout`` drops the output of every layer but the last while
+the module is in training mode (``nn.LSTM(dropout=...)``).
 """
 from __future__ import annotations
 
@@ -14,18 +15,32 @@ from typing import Dict, Iterable, List, Optional
 import torch
 from torch import nn
 
+from ...ops.reference import DropoutSpec
 from .lstm import LSTMLayer
 
 EXPORT_KEYS = ("wf", "wi", "wo", "wc", "bf", "bi", "bc", "bo")
 
 
 class RNN(nn.Module):
-    def __init__(self, settings: Iterable[dict], **layer_kw):
+    def __init__(self, settings: Iterable[dict], dropout: float = 0.0, **layer_kw):
         super().__init__()
+        if not 0.0 <= dropout < 1.0:
+            raise ValueError(f"dropout must satisfy 0 <= P < 1, got {dropout}")
         self.layers = nn.ModuleList()
         self.reverse_layers = nn.ModuleList()      # empty, or one reverse-time layer per entry of ``layers``
         self._layer_kw = layer_kw
+        self.dropout = float(dropout)
+        # the mask's key (seed, partition) and step counter (training steps completed: an int32 [1] device tensor on the GPU,
+        # an int on the CPU); a TrainEngine sets and advances them
+        self.dropout_key = (0, 0)
+        self.dropout_step = 0
         self.add_layers(settings)
+
+    def dropout_spec(self, layer: int, reverse: bool = False) -> Optional[DropoutSpec]:
+        """The dropout of layer ``layer``'s output in this forward pass: None for the top layer, with P = 0 and in eval mode."""
+        if not self.training or self.dropout == 0 or layer >= len(self.layers) - 1:
+            return None
+        return DropoutSpec(self.dropout, self.dropout_key, layer, reverse, self.dropout_step)
 
     def _make(self, setting: dict, reverse: bool = False) -> LSTMLayer:
         name = setting["layer_name"] + ("_reverse" if reverse else "")
@@ -78,8 +93,8 @@ class RNN(nn.Module):
             if self.bidirectional:
                 raise ValueError("a bidirectional stack needs whole sequences [B,T,D]: the one-step [B,D] path runs forward only")
             state = input_data
-            for layer in self.layers:
-                state = layer.fit_next(state, train=train)
+            for i, layer in enumerate(self.layers):
+                state = layer.fit_next(state, train=train, dropout=self.dropout_spec(i))
             return state
         if input_data.dim() != 3:
             raise ValueError(f"expected [B,D] or [B,T,D], got {tuple(input_data.shape)}")
@@ -101,8 +116,9 @@ class RNN(nn.Module):
         (one concatenation) for the next layer; no wavefront."""
         from ...ops import functional as F
         if self.bidirectional:
-            for la, lr in zip(self.layers, self.reverse_layers):
-                seq = torch.cat([la.fit_sequence(seq, lengths), lr.fit_sequence(seq, lengths)], 2)
+            for i, (la, lr) in enumerate(zip(self.layers, self.reverse_layers)):
+                seq = torch.cat([la.fit_sequence(seq, lengths, self.dropout_spec(i)),
+                                 lr.fit_sequence(seq, lengths, self.dropout_spec(i, True))], 2)
             return seq
         i, n = 0, len(self.layers)
         while i < n:
@@ -114,12 +130,13 @@ class RNN(nn.Module):
                     if B != l.ht.shape[0]:
                         l.reset_state(B)
                 seq, hT_a, cT_a, hT_b, cT_b = F.lstm_pair_sequence(seq, (la.ht, la.Ct, la.w_x, la.w_h, la.bias),
-                                                                     (lb.ht, lb.Ct, lb.w_x, lb.w_h, lb.bias), lengths=lengths)
+                                                                     (lb.ht, lb.Ct, lb.w_x, lb.w_h, lb.bias), lengths=lengths,
+                                                                     dropouts=(self.dropout_spec(i), self.dropout_spec(i + 1)))
                 la._set_state(hT_a, cT_a); la.state.append((hT_a, cT_a))
                 lb._set_state(hT_b, cT_b); lb.state.append((hT_b, cT_b))
                 i += 2
             else:
-                seq = la.fit_sequence(seq, lengths)
+                seq = la.fit_sequence(seq, lengths, self.dropout_spec(i))
                 i += 1
         return seq
 

@@ -301,9 +301,44 @@ def _check_lengths_arg(lengths: Optional[torch.Tensor], B: int, device) -> None:
                          f"{tuple(lengths.shape)} on {lengths.device}")
 
 
+def _drop_args(spec, device) -> dict:
+    """Keyword arguments of the kernels for a ``reference.DropoutSpec`` (none for None / P = 0): the device-resident step
+    counter and the descriptor {key0, key1, thr, c2, row0}."""
+    if spec is None or spec.p == 0:
+        return {}
+    step = spec.step
+    if not isinstance(step, torch.Tensor):                       # (a caller without an engine: no graph capture to honour)
+        step = torch.tensor([int(step)], dtype=torch.int32, device=device)
+    return {"drop_step": step, "drop_desc": spec.desc()}
+
+
+class _DropoutFn(torch.autograd.Function):
+    """Standalone dropout (csrc/lstm_pointwise.cu ts_dropout), forward and backward with the same mask: the one-step path and
+    the shapes the persistent kernels do not fuse it into.  ``x [..., B, H]``, leading dims = times t0, t0 + 1, ..."""
+    @staticmethod
+    def forward(ctx, x, spec, t0):
+        ctx.spec, ctx.t0 = spec, t0
+        STATS["kernels"] += 1
+        d = _drop_args(spec, x.device)
+        return ext().dropout(x.contiguous(), d["drop_step"], d["drop_desc"], t0)
+
+    @staticmethod
+    def backward(ctx, g):
+        STATS["kernels"] += 1
+        d = _drop_args(ctx.spec, g.device)
+        return ext().dropout(g.contiguous(), d["drop_step"], d["drop_desc"], ctx.t0), None, None
+
+
+def dropout(x: torch.Tensor, spec, t0: int = 0) -> torch.Tensor:
+    """``x * mask * scale`` (``reference.dropout``) on our own kernel; ``spec`` None or P = 0: x itself, no launch."""
+    if spec is None or spec.p == 0:
+        return x
+    return _DropoutFn.apply(x, spec, t0)
+
+
 class _LSTMSeqFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x_seq, h0, c0, w_x, w_h, bias, lengths=None, reverse=False):
+    def forward(ctx, x_seq, h0, c0, w_x, w_h, bias, lengths=None, reverse=False, dropout=None):
         E = ext()
         T, B, D = x_seq.shape
         H = w_h.shape[1]
@@ -316,9 +351,14 @@ class _LSTMSeqFn(torch.autograd.Function):
         fast = fast_path_supported(B, H, cd, x_seq.device)
         c0f = c0.detach().float().contiguous()
         h0c = h0.detach().to(cd).contiguous()
+        drop = _drop_args(dropout, x_seq.device)
+        h_drop = None
         if fast:
-            h_seq, c_seq, act = E.lstm_seq_fwd(gx, w_h_c, bias_f, h0c, c0f, _sync_ws(x_seq.device), _seq_variant(B, H, x_seq.device),
-                                               lengths=lengths, reverse=reverse)
+            outs = E.lstm_seq_fwd(gx, w_h_c, bias_f, h0c, c0f, _sync_ws(x_seq.device), _seq_variant(B, H, x_seq.device),
+                                  lengths=lengths, reverse=reverse, **drop)
+            h_seq, c_seq, act = outs[:3]
+            if drop:
+                h_drop = outs[3]                                          # written next to h_seq by the recurrence kernel
             STATS["fast_fwd"] += 1
             STATS["kernels"] += 1
         else:
@@ -339,6 +379,10 @@ class _LSTMSeqFn(torch.autograd.Function):
                 act[t].copy_(a)
             STATS["generic_fwd"] += 1
             STATS["kernels"] += T
+            if drop:
+                h_drop = E.dropout(h_seq[:T] if reverse else h_seq[1:], drop["drop_step"], drop["drop_desc"], 0)
+                STATS["kernels"] += 1
+        ctx.drop = drop
         ctx.save_for_backward(x2d, h_seq, c_seq, act, w_x_c, w_h_c)
         ctx.set_materialize_grads(False)       # an unused output must arrive as None, not as a zero-filled [T,B,H] tensor
         ctx.fast = fast
@@ -351,8 +395,8 @@ class _LSTMSeqFn(torch.autograd.Function):
         # h_T is its own output (not a slice of the first one taken by the caller): a consumer of the final state only - the
         # classifier on top of the stack - then sends back a [B,H] gradient instead of a zero-filled [T,B,H] one
         if reverse:
-            return h_seq[:T], h_seq[0], c_seq[0]
-        return h_seq[1:], h_seq[T], c_seq[T]
+            return (h_seq[:T] if h_drop is None else h_drop), h_seq[0], c_seq[0]
+        return (h_seq[1:] if h_drop is None else h_drop), h_seq[T], c_seq[T]
 
     @staticmethod
     def backward(ctx, dh_seq, dh_T, dc_T):
@@ -361,8 +405,12 @@ class _LSTMSeqFn(torch.autograd.Function):
         T, B, D, H = ctx.dims
         cd = act.dtype
         dev = act.device
+        drop = ctx.drop if dh_seq is not None else {}          # (the mask only matters where a gradient arrives)
         if dh_seq is not None:
             dh_seq = dh_seq.to(cd).contiguous()
+            if drop and not ctx.fast:
+                dh_seq = E.dropout(dh_seq, drop["drop_step"], drop["drop_desc"], 0)
+                STATS["kernels"] += 1
         elif not ctx.fast:
             dh_seq = torch.zeros(T, B, H, dtype=cd, device=dev)
         dcT = (dc_T.float().contiguous() if dc_T is not None else torch.zeros(B, H, dtype=torch.float32, device=dev))
@@ -371,7 +419,7 @@ class _LSTMSeqFn(torch.autograd.Function):
             w_hT = _transposed(w_h_c)
             _big_launch_begin()
             dpre, dh0, dc0 = E.lstm_seq_bwd(dh_seq, w_hT, act, c_seq, dhT, dcT, _sync_ws(dev), _seq_variant(B, H, dev),
-                                            lengths=ctx.lengths, reverse=ctx.reverse)
+                                            lengths=ctx.lengths, reverse=ctx.reverse, **drop)
             STATS["fast_bwd"] += 1
             STATS["kernels"] += 1
             _after_big_launch()                  # finished gradient buckets of the layers above: sync them under this recurrence
@@ -403,13 +451,15 @@ class _LSTMSeqFn(torch.autograd.Function):
             dx = G.matmul(dg2d, w_x_c.t(), out_dtype=cd).view(T, B, D)        # dG · W_x: W_x read in place as an MN-major operand
             STATS["kernels"] += 1
         h0_dt, c0_dt = ctx.in_dtypes
-        return dx, dh0.to(h0_dt), dc0.to(c0_dt), dw_x, dw_h, db, None, None
+        return dx, dh0.to(h0_dt), dc0.to(c0_dt), dw_x, dw_h, db, None, None, None
 
 
-def lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths=None, reverse=False):
+def lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths=None, reverse=False, dropout=None):
     """``x_seq [T,B,D]`` (bf16 or fp32) -> ``(h_seq [T,B,H], h_T, c_T)``.  ``lengths``: optional int32 ``[B]`` on the batch's
     device, right padding (``ops/reference.py``); the persistent kernels then run their masked instantiations.  ``reverse``:
-    the reverse-time direction (time T-1 down to 0; ``h_T`` / ``c_T`` are then the state after time 0)."""
+    the reverse-time direction (time T-1 down to 0; ``h_T`` / ``c_T`` are then the state after time 0).  ``dropout``: a
+    ``reference.DropoutSpec``; the first output is then the dropped sequence (the persistent kernels store it next to h_seq
+    and mask the incoming gradient as they load it; other shapes run the standalone dropout kernel)."""
     if (not x_seq.is_contiguous() and not x_seq.requires_grad and x_seq.transpose(0, 1).is_contiguous()
             and (x_seq.shape[2] * x_seq.element_size()) % 16 == 0):
         x_seq = ext().transpose01(x_seq.transpose(0, 1))     # batch-major feed -> time-major, a row permutation at copy speed
@@ -424,14 +474,15 @@ def lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths=None, reverse=Fal
         _CHUNKING["on"] = True
         try:
             outs = [_LSTMSeqFn.apply(x_seq[:, b0:b0 + chunk].contiguous(), h0[b0:b0 + chunk], c0[b0:b0 + chunk], w_x, w_h, bias,
-                                     None if lengths is None else lengths[b0:b0 + chunk], reverse)
+                                     None if lengths is None else lengths[b0:b0 + chunk], reverse,
+                                     None if dropout is None else dropout.at_rows(b0))
                     for b0 in range(0, B, chunk)]
         finally:
             _CHUNKING["on"] = False
         STATS["batch_chunks"] = STATS.get("batch_chunks", 0) + len(outs)
         return (torch.cat([o[0] for o in outs], dim=1), torch.cat([o[1] for o in outs], dim=0),
                 torch.cat([o[2] for o in outs], dim=0))
-    return _LSTMSeqFn.apply(x_seq.contiguous(), h0, c0, w_x, w_h, bias, lengths, reverse)
+    return _LSTMSeqFn.apply(x_seq.contiguous(), h0, c0, w_x, w_h, bias, lengths, reverse, dropout)
 
 
 # =====================================================================================================================
@@ -556,7 +607,8 @@ def _gate_cfg(var: int, tiles_m: int, nkb: int, per_kb_step: int, ctas_per_tile:
 
 class _LSTMPairFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x_seq, h0a, c0a, w_xa, w_ha, b_a, h0b, c0b, w_xb, w_hb, b_b, lengths=None, schedule="wavefront"):
+    def forward(ctx, x_seq, h0a, c0a, w_xa, w_ha, b_a, h0b, c0b, w_xb, w_hb, b_b, lengths=None, schedule="wavefront", drop_a=None,
+                drop_b=None):
         E = ext()
         pipelined = schedule == "pipelined"
         dev = x_seq.device
@@ -583,6 +635,11 @@ class _LSTMPairFn(torch.autograd.Function):
         h_seq_b = torch.empty(T + 1, B, Hb, **opt); c_seq_b = torch.empty(T + 1, B, Hb, dtype=torch.float32, device=dev)
         act_b = torch.empty(T, B, 4 * Hb, **opt); til_b = torch.empty((T + 1) * 2 * 128 * Hb, **opt)
         gx_b = torch.empty(T, B, 4 * Hb, **opt)
+        # dropout: L_a stores h_drop_a next to h_seq_a (the gated gx_b GEMM reads it), L_b stores h_drop_b (the pair's output)
+        dra, drb = _drop_args(drop_a, dev), _drop_args(drop_b, dev)
+        h_drop_a = torch.empty(T, B, Ha, **opt) if dra else None
+        h_drop_b = torch.empty(T, B, Hb, **opt) if drb else None
+        hin_b = h_seq_a[1:] if h_drop_a is None else h_drop_a            # layer b's input sequence
         tn = 4 * Hb // 256
         ws_a, ws_b, done = _pair_ws(dev, "fwd", T * tn * 2)
         done.zero_()                                                     # (the prologue kernels zero ws_a / ws_b)
@@ -595,33 +652,40 @@ class _LSTMPairFn(torch.autograd.Function):
         # starts once both are complete (the GEMM waits for L_a before it exits).
         E.lstm_seq_prologue(h0a_c, c0a_f, h_seq_a, c_seq_a, til_a, ws_a)
         E.lstm_seq_prologue(h0b_c, c0b_f, h_seq_b, c_seq_b, til_b, ws_b)
-        E.lstm_seq_fwd_into(gx_a, wha, ba_f, h0a_c, c0a_f, h_seq_a, c_seq_a, act_a, til_a, ws_a, var, None, 0, True, 0, 1, lengths)
+        E.lstm_seq_fwd_into(gx_a, wha, ba_f, h0a_c, c0a_f, h_seq_a, c_seq_a, act_a, til_a, ws_a, var, None, 0, True, 0, 1, lengths,
+                            h_drop=h_drop_a, **dra)
         if not pipelined:
-            E.lstm_seq_fwd_into(gx_b, whb, bb_f, h0b_c, c0b_f, h_seq_b, c_seq_b, act_b, til_b, ws_b, var, done, tn, False, 0, 3, lengths)
+            E.lstm_seq_fwd_into(gx_b, whb, bb_f, h0b_c, c0b_f, h_seq_b, c_seq_b, act_b, til_b, ws_b, var, done, tn, False, 0, 3, lengths,
+                                h_drop=h_drop_b, **drb)
         # single-CTA tiles: the recurrences' CTAs are spread one per TPC, the SMs they leave free rarely form CTA pairs
         free_ctas = max(1, _sms(dev) - Ha // 16 - (0 if pipelined else Hb // 16))
-        E.gemm2(h_seq_a[1:].view(T * B, Ha), wxb, out=gx_b.view(T * B, 4 * Hb), ctas=1, bn=256, max_ctas=free_ctas,
+        E.gemm2(hin_b.view(T * B, Ha), wxb, out=gx_b.view(T * B, 4 * Hb), ctas=1, bn=256, max_ctas=free_ctas,
                 gate=ws_a[_gate_off(var):], gate_cfg=_gate_cfg(var, 2, Ha // 64, 4, 4 * Ha // 64, 2, 1, B, False), done=done,
                 gate_err=ws_a[SYNC_WORDS - 1:], pdl=True)
         if pipelined:
-            E.lstm_seq_fwd_into(gx_b, whb, bb_f, h0b_c, c0b_f, h_seq_b, c_seq_b, act_b, til_b, ws_b, var, None, 0, False, 0, 1, lengths)
+            E.lstm_seq_fwd_into(gx_b, whb, bb_f, h0b_c, c0b_f, h_seq_b, c_seq_b, act_b, til_b, ws_b, var, None, 0, False, 0, 1, lengths,
+                                h_drop=h_drop_b, **drb)
         STATS["fast_fwd"] += 2
         STATS["kernels"] += 3
         STATS[schedule + "_fwd"] = STATS.get(schedule + "_fwd", 0) + 1
-        ctx.save_for_backward(x2d, h_seq_a, c_seq_a, act_a, h_seq_b, c_seq_b, act_b, wxa, wha, wxb, whb)
+        ctx.save_for_backward(x2d, h_seq_a, c_seq_a, act_a, h_seq_b, c_seq_b, act_b, wxa, wha, wxb, whb, hin_b)
         ctx.set_materialize_grads(False)
+        ctx.drop = (dra, drb)
         ctx.dims = (T, B, D, Ha, Hb)
         ctx.lengths = lengths
         ctx.pipelined = pipelined
         ctx.x_folded = x_bm is not None
         ctx.addrs = (w_xa.data_ptr(), w_ha.data_ptr(), b_a.data_ptr(), w_xb.data_ptr(), w_hb.data_ptr(), b_b.data_ptr())
         ctx.in_dtypes = (h0a.dtype, c0a.dtype, h0b.dtype, c0b.dtype)
-        return h_seq_b[1:], h_seq_a[T], c_seq_a[T], h_seq_b[T], c_seq_b[T]
+        return (h_seq_b[1:] if h_drop_b is None else h_drop_b), h_seq_a[T], c_seq_a[T], h_seq_b[T], c_seq_b[T]
 
     @staticmethod
     def backward(ctx, dh_seq_b, dhT_a, dcT_a, dhT_b, dcT_b):
         E = ext()
-        x2d, h_seq_a, c_seq_a, act_a, h_seq_b, c_seq_b, act_b, wxa, wha, wxb, whb = ctx.saved_tensors
+        x2d, h_seq_a, c_seq_a, act_a, h_seq_b, c_seq_b, act_b, wxa, wha, wxb, whb, hin_b = ctx.saved_tensors
+        dra, drb = ctx.drop
+        if dh_seq_b is None:
+            drb = {}
         T, B, D, Ha, Hb = ctx.dims
         cd, dev = act_a.dtype, act_a.device
         if dh_seq_b is not None:
@@ -640,15 +704,17 @@ class _LSTMPairFn(torch.autograd.Function):
         # programmatic-dependent-launch chain on one stream (see forward): L_b -> L_a -> gated dX GEMM.  Pipelined: L_b -> gated
         # dX GEMM -> L_a (ordinary launch: dx_b is complete when it starts)
         pipelined = ctx.pipelined
-        E.lstm_seq_bwd_into(dh_seq_b, whT_b, act_b, c_seq_b, dpre_b, dh0b, dc0b, til_b, ws_b, var, None, 0, True, 0, 1, ctx.lengths)
+        # dropout: each recurrence masks the gradient into its output sequence as it loads it (dx_b stays the raw dL/dh_drop_a)
+        E.lstm_seq_bwd_into(dh_seq_b, whT_b, act_b, c_seq_b, dpre_b, dh0b, dc0b, til_b, ws_b, var, None, 0, True, 0, 1, ctx.lengths, **drb)
         if not pipelined:
-            E.lstm_seq_bwd_into(dx_b, whT_a, act_a, c_seq_a, dpre_a, dh0a, dc0a, til_a, ws_a, var, done, tn, False, 0, 3, ctx.lengths)
+            E.lstm_seq_bwd_into(dx_b, whT_a, act_a, c_seq_a, dpre_a, dh0a, dc0a, til_a, ws_a, var, done, tn, False, 0, 3, ctx.lengths,
+                                **dra)
         free_ctas = max(1, _sms(dev) - Hb // 16 - (0 if pipelined else Ha // 16))
         E.gemm2(dpre_b.view(T * B, 4 * Hb), wxb, out=dx_b.view(T * B, Ha), b_mn=True, ctas=1, bn=256, max_ctas=free_ctas,
                 gate=ws_b[_gate_off(var):], gate_cfg=_gate_cfg(var, 2, 4 * Hb // 64, 1, 4 * Hb // 64, T + 1, -1, B, True), done=done,
                 gate_err=ws_b[SYNC_WORDS - 1:], pdl=True)
         if pipelined:
-            E.lstm_seq_bwd_into(dx_b, whT_a, act_a, c_seq_a, dpre_a, dh0a, dc0a, til_a, ws_a, var, None, 0, False, 0, 1, ctx.lengths)
+            E.lstm_seq_bwd_into(dx_b, whT_a, act_a, c_seq_a, dpre_a, dh0a, dc0a, til_a, ws_a, var, None, 0, False, 0, 1, ctx.lengths, **dra)
         STATS["fast_bwd"] += 2
         STATS["kernels"] += 5
         a = ctx.addrs
@@ -664,14 +730,14 @@ class _LSTMPairFn(torch.autograd.Function):
             # ordinary launch (dW_xa), not under these: a programmatic dependent may start before the kernels ahead of it in
             # the stream are complete.
             side = max(1, (_sms(dev) - Ha // 16 - _COLSUM_SMS) // 2)
-            dw_xb = _accumulate_grad(a[3], dg_b.t(), h_seq_a[1:].reshape(T * B, Ha), pdl=True, max_ctas=side)
+            dw_xb = _accumulate_grad(a[3], dg_b.t(), hin_b.reshape(T * B, Ha), pdl=True, max_ctas=side)
             dw_hb = _accumulate_grad(a[4], dg_b.t(), h_seq_b[:T].reshape(T * B, Hb), pdl=True, max_ctas=side)
             db_b = _bias_grad(a[5], dg_b, under_gemm=True, max_ctas=4 * _COLSUM_SMS)
         else:
             # the bias column sums run NEXT TO the first weight-gradient GEMM of their layer (same dG, idle SMs), not after it
             # (each GEMM is followed by: finished gradient buckets [programmatic dependents of the GEMM], then half of the layer's
             # bias column sums [programmatic dependent of whatever was launched last] - all three run side by side)
-            dw_xb = _accumulate_grad(a[3], dg_b.t(), h_seq_a[1:].reshape(T * B, Ha))
+            dw_xb = _accumulate_grad(a[3], dg_b.t(), hin_b.reshape(T * B, Ha))
             _bias_grad(a[5], dg_b, under_gemm=dw_xb is None, part=0)
             dw_hb = _accumulate_grad(a[4], dg_b.t(), h_seq_b[:T].reshape(T * B, Hb))
             db_b = _bias_grad(a[5], dg_b, under_gemm=dw_hb is None, part=1)
@@ -685,13 +751,16 @@ class _LSTMPairFn(torch.autograd.Function):
             dx = G.matmul(dg_a, wxa.t(), out_dtype=cd).view(T, B, D)
             STATS["kernels"] += 1
         t = ctx.in_dtypes
-        return dx, dh0a.to(t[0]), dc0a.to(t[1]), dw_xa, dw_ha, db_a, dh0b.to(t[2]), dc0b.to(t[3]), dw_xb, dw_hb, db_b, None, None
+        return (dx, dh0a.to(t[0]), dc0a.to(t[1]), dw_xa, dw_ha, db_a, dh0b.to(t[2]), dc0b.to(t[3]), dw_xb, dw_hb, db_b, None, None,
+                None, None)
 
 
-def lstm_pair_sequence(x_seq, la, lb, lengths=None, schedule=None):
+def lstm_pair_sequence(x_seq, la, lb, lengths=None, schedule=None, dropouts=(None, None)):
     """Two stacked layers as one op.  ``la`` / ``lb`` = (h0, c0, w_x, w_h, bias).  -> (h_seq_b, hT_a, cT_a, hT_b, cT_b).
     ``lengths``: optional int32 ``[B]`` per-row lengths (both layers run their masked kernels; the gated GEMM is unchanged).
-    ``schedule``: "wavefront" or "pipelined" (see ``pair_schedule``); None = the one ``pair_schedule`` picks for the device."""
+    ``schedule``: "wavefront" or "pipelined" (see ``pair_schedule``); None = the one ``pair_schedule`` picks for the device.
+    ``dropouts``: ``reference.DropoutSpec`` (or None) of layer a's output (the input of layer b) and of layer b's output (the
+    first result)."""
     _check_lengths_arg(lengths, x_seq.shape[1], x_seq.device)
     if schedule is None:
         schedule = _pair_schedule_of(x_seq, la[3].shape[1], lb[3].shape[1])
@@ -701,7 +770,7 @@ def lstm_pair_sequence(x_seq, la, lb, lengths=None, schedule=None):
     if (not x_seq.is_contiguous() and not x_seq.requires_grad and x_seq.transpose(0, 1).is_contiguous()
             and (x_seq.shape[2] * x_seq.element_size()) % 16 == 0):
         if FOLDED_FEED and G.folded_ok(x_seq.transpose(0, 1)):
-            return _LSTMPairFn.apply(x_seq, *la, *lb, lengths, schedule)  # read in place (see forward)
+            return _LSTMPairFn.apply(x_seq, *la, *lb, lengths, schedule, *dropouts)  # read in place (see forward)
         x_seq = ext().transpose01(x_seq.transpose(0, 1))
         STATS["kernels"] += 1
-    return _LSTMPairFn.apply(x_seq.contiguous(), *la, *lb, lengths, schedule)
+    return _LSTMPairFn.apply(x_seq.contiguous(), *la, *lb, lengths, schedule, *dropouts)

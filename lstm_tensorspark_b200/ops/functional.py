@@ -42,13 +42,22 @@ def lstm_cell_step(x, h, c, w_x, w_h, bias):
     return ref.lstm_cell_step(x, h, c, w_x, w_h, bias)
 
 
-def lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths=None, reverse=False):
+def lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths=None, reverse=False, dropout=None):
     """``lengths``: optional int32 ``[B]`` per-row sequence lengths (right padding, see ``reference.lstm_layer_sequence``).
-    ``reverse``: the reverse-time direction of a bidirectional layer (same reference)."""
+    ``reverse``: the reverse-time direction of a bidirectional layer (same reference).  ``dropout``: optional
+    ``reference.DropoutSpec``: the first output is then the dropped sequence."""
     if _use_ext(x_seq):
         from . import cuda_lstm
-        return cuda_lstm.lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths=lengths, reverse=reverse)
-    return ref.lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths=lengths, reverse=reverse)
+        return cuda_lstm.lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths=lengths, reverse=reverse, dropout=dropout)
+    return ref.lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths=lengths, reverse=reverse, dropout=dropout)
+
+
+def dropout(x, spec, t0: int = 0):
+    """``x [B,H]`` (time t0) or ``[T,B,H]`` -> ``x * mask * scale`` of ``spec`` (``reference.dropout``); None / P = 0: x."""
+    if _use_ext(x):
+        from . import cuda_lstm
+        return cuda_lstm.dropout(x, spec, t0)
+    return ref.dropout(x, spec, t0)
 
 
 def head_xent(h, weights, bias, labels):
@@ -67,6 +76,6 @@ def lstm_pair_supported(x_seq, h_a: int, h_b: int) -> bool:
     return cuda_lstm.wavefront_supported(x_seq, h_a, h_b)
 
 
-def lstm_pair_sequence(x_seq, la, lb, lengths=None):
+def lstm_pair_sequence(x_seq, la, lb, lengths=None, dropouts=(None, None)):
     from . import cuda_lstm
-    return cuda_lstm.lstm_pair_sequence(x_seq, la, lb, lengths=lengths)
+    return cuda_lstm.lstm_pair_sequence(x_seq, la, lb, lengths=lengths, dropouts=dropouts)

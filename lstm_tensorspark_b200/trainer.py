@@ -118,7 +118,7 @@ def train_rnn(partition, cfg: Config, rank: int = 0, world_size: int = 1, comm: 
     # ---- model + optimizer + sync = one TrainEngine (the same object bench.py drives) ----------------------
     from .engine import TrainEngine
     eng = TrainEngine(cfg, rank, world_size, comm, batch_size=batch_size, device=device, dtype=dtype,
-                      train_optimizer=train_optimizer)
+                      train_optimizer=train_optimizer, partition_key=partition_key)
     model, optimizer = eng.model, eng.optimizer
 
     # ---- run directory -----------------------------------------------------------------
@@ -151,6 +151,7 @@ def train_rnn(partition, cfg: Config, rank: int = 0, world_size: int = 1, comm: 
             eng.flat.refresh_shadow()
             if opt_state is not None:
                 comm.load_optimizer_state(optimizer, opt_state["optimizer"])
+                eng.set_dropout_step(optimizer.step_count)       # the masks continue where the interrupted run's would have
                 if opt_state.get("loader") is not None:
                     st = opt_state["loader"]
                     if bool(st.get("pinned")) == isinstance(loader, D.PinnedHostLoader):
@@ -228,11 +229,13 @@ def train_rnn(partition, cfg: Config, rank: int = 0, world_size: int = 1, comm: 
                            extra={"rank": rank, "world_size": world_size, "partition_key": partition_key,
                                   "loss": t_loss, "config": cfg.__dict__},
                            opt_state={"optimizer": comm.optimizer_state(optimizer), "loader": loader.state_dict()})
+                model.eval()                                         # no dropout while scoring
                 with torch.no_grad(), M.capture(sink):
                     h = model.features(train_input, batch_lengths)   # same batch, from the initial state (src/rnn.py:276-279)
                     logits = model.head(h)
                     e_loss = compute_loss(labels=train_labels, logits=logits)
                     e_acc = compute_accuracy(labels=train_labels, logits=logits)
+                model.train()
                 t_loss, t_acc = float(e_loss.item()), float(e_acc.item())
                 sink.flush(step)
                 jlog.write(step=step, loss=t_loss, acc=t_acc, rank=rank)
@@ -396,6 +399,7 @@ def evaluate_job(cfg: Config, standalone: bool = False) -> Dict:
     n = x.shape[0]
     bs = D.resolve_batch_size(cfg.batch_size if cfg.batch_size and cfg.batch_size <= n else 0, n)
     eng = TrainEngine(cfg, 0, 1, Communicator(0, 1), batch_size=bs, device=device, dtype=dtype)
+    eng.model.eval()                                    # scoring: no dropout
     # the reference's trainable initial state is one row PER BATCH ROW ([batch_size, H], src/models/recurrent/lstm.py:24-33):
     # scoring with another batch size uses the mean learned row for every sample
     shapes = {k: tuple(v.shape) for k, v in eng.model.named_reference_variables()}
