@@ -247,8 +247,10 @@ struct SeqParams {
 // half q >> 1: one thread = one batch row x 8 hidden units (32 accumulator columns).  The two warpgroups share the tile's
 // epilogue barriers (256 threads).
 // kTiles = 2 (ping-pong): the CTA serves TWO independent 128-row batch tiles with the same resident weight slice, and
-// warpgroup `half` owns tile mb0 + half for the whole launch.  Per k16 it issues two m64n64k16 (rows [0, 64) and [64, 128) of
-// the A tile, 64 accumulator registers), stages the whole tile and runs its epilogue with one thread per batch row (row
+// warpgroup `half` owns tile mb0 + half for the whole launch.  Per k16 it issues ONE m64n128k16 of the transposed product
+// (A = the [64 gate columns x 64] weight block, B = the 128-row operand stage, 64 accumulator registers): 6 KB of shared
+// memory per k16 instead of 8 KB for two m64n64k16 that each read the weight block.  It stages the whole tile (transposing
+// the fragment on the way) and runs its epilogue with one thread per batch row (row
 // 32 q + lane) over all 64 accumulator columns, as two passes of the 32-column body (index [column half] of the per-thread
 // state).  Its barriers are its own (128 threads), so while one warpgroup is in its cell math, exchange and dataflow
 // signal, the other one's MMAs keep the tensor cores busy.  The producer still fills the ring strictly in order - per step
@@ -578,7 +580,10 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
     const bool dbg_wg = p.dbg && blockIdx.x == 0 && gtid == 0;
     auto dbg_stamp = [&](int step, int slot) { p.dbg[(kPP && half ? dbg_tile1(p.T) : 0) + 4 * step + slot] = gtime(); };
     auto mma_tile = [&](int dstep) -> bool {
-      float acc[kPP ? 2 : 1][kBNm / 2];
+      // kPP computes the TRANSPOSED product, D[64 gate columns][128 batch rows] = W_slice x tile^T: one m64n128k16 per k16 with
+      // the weight block as A and the operand stage as B reads 6 KB of shared memory instead of the 8 KB of two m64n64k16 with
+      // the weight block read twice.  acc[0] then holds gate column acc_row(i) x batch row acc_col(i).
+      float acc[1][kPP ? kBNm : kBNm / 2];               // kPP: 64 x 128 over 128 threads
       // kPP: take the MMA turn.  A full barrier's parity only tells whether its LAST completed phase matches, so a warpgroup
       // must not wait for a stage's fill n before fill n - 1 - possibly the other warpgroup's - has landed.  Warpgroup 1's
       // tile-step n waits until warpgroup 0 has seen all its stages of step n, and warpgroup 0's step n + 1 until warpgroup 1
@@ -599,20 +604,19 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
         const uint32_t kbi = kStream ? 0u : (p.sync_mode == 1 ? (uint32_t)kb : ss->kb_idx[stage]);
         const uint64_t ds = desc_a0 + (uint64_t)(stage * (kStageBytes >> 4));
         const uint64_t dw = kStream ? ds + (uint64_t)(kABytes >> 4) : desc_w0 + (uint64_t)(kbi * (kWBlk >> 4));
-#pragma unroll
-        for (int m = 0; m < (kPP ? 2 : 1); ++m) tc::fence_regs(acc[m]);
+        tc::fence_regs(acc[0]);
         tc::wgmma_fence();
 #pragma unroll
         for (int k = 0; k < BK / 16; ++k) {
-#pragma unroll
-          for (int m = 0; m < (kPP ? 2 : 1); ++m) {       // A rows [64 m, +64) (kPP) / [64 half, +64)
-            const uint64_t da = ds + (uint64_t)((kPP ? m : half) * ((kABytes / 2) >> 4));
-            tc::Wgmma<kBNm, 0, 0>::mma(acc[m], da + (uint64_t)(2 * k), dw + (uint64_t)(2 * k), (kb > 0 || k > 0) ? 1u : 0u);
+          if constexpr (kPP) {                           // A = weight block [64 x 64], B = the whole 128-row stage
+            tc::Wgmma<BM, 0, 0>::mma(acc[0], dw + (uint64_t)(2 * k), ds + (uint64_t)(2 * k), (kb > 0 || k > 0) ? 1u : 0u);
+          } else {                                       // A rows [64 half, +64)
+            const uint64_t da = ds + (uint64_t)(half * ((kABytes / 2) >> 4));
+            tc::Wgmma<kBNm, 0, 0>::mma(acc[0], da + (uint64_t)(2 * k), dw + (uint64_t)(2 * k), (kb > 0 || k > 0) ? 1u : 0u);
           }
         }
         tc::wgmma_commit();
-#pragma unroll
-        for (int m = 0; m < (kPP ? 2 : 1); ++m) tc::fence_regs(acc[m]);
+        tc::fence_regs(acc[0]);
         // Hand a stage back once its MMAs have retired.  With >= 3 stages that is the previous one (its MMAs overlap this
         // stage's wait); with 2 the producer waits for both stages of a k-block pair, so each stage is released at once.
         if (kStages >= 3) {
@@ -629,8 +633,7 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
       }
       if (kPP && lane == 0) tc::mbar_arrive(&ss->mma_turn[1 - half]);    // every stage of this tile-step has landed
       tc::wgmma_wait<0>();
-#pragma unroll
-      for (int m = 0; m < (kPP ? 2 : 1); ++m) tc::fence_regs(acc[m]);
+      tc::fence_regs(acc[0]);
       // Ring staging: the MMAs that read the last stages have retired and only this warpgroup reads them (its A half; kPP: its
       // tile's stages), so the accumulator goes there.  The borrowed stages were refilled only after every warp had released
       // them the previous time: no reader of an earlier staging is left.
@@ -638,16 +641,29 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
         if (kStages >= 3 && lane == 0) tc::mbar_arrive_u32(empty0 + 8 * prev);
         wg_bar();                                        // this warpgroup has read the previously staged accumulator
       }
+      if constexpr (kPP) {
+        // transposed fragment: element i = gate column g of batch row b; this warp's 16 gate columns of all 128 rows, rows
+        // [8 (i / 4), +8) per group of four elements (one piece each).  Conflict-free: a warp's 32 stores of one element
+        // index hit 4 rows x 8 columns, and the row swizzle puts each row's columns in different 16 B chunks.
+        uint8_t* pb[kAccPieces];
 #pragma unroll
-      for (int m = 0; m < (kPP ? 2 : 1); ++m) {
-        uint8_t* wb = acc_row_ptr(64 * m + 16 * quarter);  // this warp's 16 fragment rows (one piece)
+        for (int pc = 0; pc < kAccPieces; ++pc) pb[pc] = acc_row_ptr(pc * kAccRowsPer);
+#pragma unroll
+        for (int i = 0; i < kBNm; ++i) {
+          const int pc = 8 * (i >> 2) / kAccRowsPer;
+          const int g = tc::acc_row(i, quarter, lane), b = tc::acc_col(i, lane);
+          uint8_t* rp = pb[pc] + (b - pc * kAccRowsPer) * kAccRowBytes;
+          if constexpr (kBwd)                            // bf16: 2 B of the row's 16 B chunk (g / 8) ^ (b & 7)
+            *reinterpret_cast<__nv_bfloat16*>(rp + (((g >> 3) ^ b) & 7) * 16 + (g & 7) * 2) = __float2bfloat16_rn(acc[0][i]);
+          else
+            *reinterpret_cast<float*>(rp + acc_swz(b, g) * 4) = acc[0][i];
+        }
+      } else {
+        uint8_t* wb = acc_row_ptr(16 * quarter);         // this warp's 16 fragment rows (one piece)
 #pragma unroll
         for (int i = 0; i < kBNm / 2; i += 2) {
           const int r = tc::acc_row(i, 0, lane), c = tc::acc_col(i, lane);
-          if constexpr (kPP && kBwd)                     // bf16 pair: 4 B of the row's 16 B chunk (c / 8) ^ (r & 7)
-            *reinterpret_cast<uint32_t*>(wb + r * kAccRowBytes + (((c >> 3) ^ r) & 7) * 16 + (c & 7) * 2) = pack_bf2(acc[m][i], acc[m][i + 1]);
-          else
-            *reinterpret_cast<float2*>(wb + r * kAccRowBytes + acc_swz(r, c) * 4) = make_float2(acc[m][i], acc[m][i + 1]);
+          *reinterpret_cast<float2*>(wb + r * kAccRowBytes + acc_swz(r, c) * 4) = make_float2(acc[0][i], acc[0][i + 1]);
         }
       }
       wg_bar();
