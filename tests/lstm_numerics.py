@@ -6,7 +6,8 @@ T = 512, B = 64, H = 2048 a single fp64 [T, B, 4H] tensor is 2.1 GB, and the rou
   * ``rounding=Bf16(...)``: fp32 with every bf16 rounding of the fast path in its place - what an ideal kernel with those
     rounding points computes.  Its distance from fp64 is the error the bf16 storage alone explains.
 ``check_budget`` then holds a kernel's error against fp64 to ALPHA x the emulation's error (plus a small floor), per time step
-for the sequences, so that a defect confined to one step of hundreds cannot hide in a global norm.
+for the sequences, so that a defect confined to one step of hundreds cannot hide in a global norm.  ``model`` composes the
+layers into the whole classifier (stacked, bidirectional, dropout, head) with the same two arms.
 
 Rounding points of the fast path (ops/cuda_lstm.py, csrc/lstm_seq_wgmma.cu), all round-to-nearest-even:
   forward   gx = x W_x^T is stored bf16 (_gemm_tn); with the forward K-split (cluster of 2) a member adds the PEER's half of the
@@ -58,7 +59,12 @@ class Bf16:
 class Defect:
     """A defect to plant into a run (tests of the budget's sensitivity).  ``step``: processing step (0 = the first step of
     the direction); ``index``: the k-block (``drop_kblock``: of h in the forward recurrent product; ``zero_dg``: of dG) or the
-    16-row group (``stale_rows``: its recurrent operand is h from one step earlier)."""
+    16-row group (``stale_rows``: its recurrent operand is h from one step earlier).
+    Defects of the model composition (``model``; every layer / layer boundary):
+      ``fwd_dx_only``      at time ``step`` the lower layer's incoming gradient is the forward upper direction's dx alone;
+      ``mask_next_step``   the backward masks dropout with the mask of training step ``step + 1``;
+      ``lost_chunk``       weight and bias gradients lose batch rows [0, ``index``) (a second batch chunk overwrote the sink);
+      ``reverse_unmasked`` the reverse direction ignores ``lengths`` and starts at T - 1."""
     kind: str
     step: int
     index: int
@@ -160,7 +166,8 @@ def _forward(x, h0, c0, w_x, w_h, bias, keep, reverse, r, defect):
     return hs, cs, acts
 
 
-def _backward(fw, x, w_x, w_h, dh_seq, dh_T, dc_T, keep, reverse, r, defect):
+def _backward(fw, x, w_x, w_h, dh_seq, dh_T, dc_T, keep, reverse, r, defect, dh_scale=None):
+    """``dh_scale`` [T,B,H]: dropout's mask x scale on this layer's output, applied to the bf16 dh_seq as it is loaded."""
     hs, cs, acts = fw
     dt = hs.dtype
     T, B, H = acts.shape[:3]
@@ -172,7 +179,12 @@ def _backward(fw, x, w_x, w_h, dh_seq, dh_T, dc_T, keep, reverse, r, defect):
     dgs = torch.empty(T, B, 4 * H, dtype=dt, device=hs.device)
     for n, t in enumerate(range(T) if reverse else range(T - 1, -1, -1)):
         sp, sn = (t + 1, t) if reverse else (t, t + 1)
-        dht = dh if dh_seq is None else dh + _round(r, dh_seq[t].to(dt))
+        if dh_seq is None:
+            dht = dh
+        elif dh_scale is None:
+            dht = dh + _round(r, dh_seq[t].to(dt))
+        else:
+            dht = dh + _round(r, dh_seq[t].to(dt)) * dh_scale[t]
         i, f, g, o = acts[t].unbind(-1)
         tcn = _tanh(r, cs[sn])
         dct = dc + dht * o * (1 - tcn * tcn)
@@ -191,10 +203,12 @@ def _backward(fw, x, w_x, w_h, dh_seq, dh_T, dc_T, keep, reverse, r, defect):
         dgs[t] = dg
     dg2d = dgs.view(T * B, 4 * H)
     h_prev = hs[1:] if reverse else hs[:T]
-    dw_x = dg2d.t() @ x.reshape(T * B, D).to(dt)
-    dw_h = dg2d.t() @ h_prev.reshape(T * B, H)
+    rows = slice(defect.index, None) if defect is not None and defect.kind == "lost_chunk" else slice(None)
+    dg_w = dgs[:, rows].reshape(-1, 4 * H)
+    dw_x = dg_w.t() @ x[:, rows].reshape(-1, D).to(dt)
+    dw_h = dg_w.t() @ h_prev[:, rows].reshape(-1, H)
     dx = _round(r, dg2d @ w_x.to(dt)).view(T, B, D)
-    return dx, dh, dc, dw_x, dw_h, dg2d.sum(0)
+    return dx, dh, dc, dw_x, dw_h, dg_w.sum(0)
 
 
 def _state_out(fw, reverse):
@@ -226,6 +240,121 @@ def pair(x, la, lb, dh_seq, dh_T_a, dc_T_a, dh_T_b, dc_T_b, lengths=None, roundi
     gb = _backward(fb, h_seq_a, lb[2], lb[3], dh_seq, dh_T_b, dc_T_b, keep, False, rb, None)
     ga = _backward(fa, x, la[2], la[3], gb[0], dh_T_a, dc_T_a, keep, False, ra, None)
     return LayerOut(*_state_out(fa, False), *ga), LayerOut(*_state_out(fb, False), *gb)
+
+
+class Dropout(NamedTuple):
+    """Dropout between stacked layers in one training step: ``RNN.dropout_spec``'s P, (seed, partition) key and step count."""
+    p: float
+    key: tuple
+    step: int
+
+
+class ModelOut(NamedTuple):
+    loss: Optional[torch.Tensor]     # mean cross-entropy (None without a head)
+    h_T: torch.Tensor                # the classifier's input [B, H_last] (bidirectional: [B, 2 H_last], forward half first)
+    grads: dict                      # "LSTMLayer<l>[_reverse]/<h0|c0|w_x|w_h|bias>", "Dense1/weights", "Dense1/bias" -> gradient
+
+
+def _drop_scale(dropout, layer, reverse, T, B, H, dt, device):
+    """mask x scale [T,B,H] of one layer direction's output (``reference.dropout_mask``, keyed as ``RNN.dropout_spec``)."""
+    from lstm_tensorspark_b200.ops import reference as ref
+    spec = ref.DropoutSpec(dropout.p, tuple(dropout.key), layer, reverse, int(dropout.step))
+    keep = ref.dropout_mask(spec, T, B, H, device=device)
+    return keep.to(dt) * ref.dropout_scale(dropout.p).to(dt).to(device)
+
+
+def model(x, layers, head, labels, lengths=None, bidirectional=False, dropout: Optional[Dropout] = None, rounding=None,
+          defect: Optional[Defect] = None, dh_T=None, backward=True) -> ModelOut:
+    """The whole classifier (``models.classifier.SequenceClassifier`` in training mode on the CUDA path) forward and backward,
+    composed from the layer loops above.  ``x [B,T,D]`` batch-major; ``layers``: per layer (h0, c0, w_x, w_h, bias) - for a
+    bidirectional stack a (forward, reverse) pair of them; ``head``: (W [H_in, C], b [C]) and ``labels`` [B] - or None and
+    ``dh_T``, the gradient into h_T; ``dropout``: None or ``Dropout``.  ``rounding``: None (fp64) or the fast path's: one
+    Bf16 for every layer, or one per layer (each a Bf16 or a (forward, reverse) pair).  ``backward=False``: loss and h_T only.
+
+    Rounding points on top of the layers' (module docstring), all in the emulation only:
+      between layers  the next layer reads the bf16 h_seq; with dropout bf16(h * scale) under the mask, and the lower layer
+                      multiplies the bf16 dx it receives by the same mask x scale in fp32 as it loads it;
+      bidirectional   the next layer reads [h_fwd | h_rev]; the lower layer's incoming gradient is the sum of the two upper
+                      directions' bf16 dx, rounded to bf16 once (autograd adds the two bf16 gradients of the shared input);
+      head            logits = bf16 h_T x bf16(W) in fp32 + fp32 bias; softmax, NLL, dlogits = (p - onehot) / B in fp32;
+                      dh = dlogits W^T with the fp32 W, stored bf16; dW = h_T^T dlogits and db in fp32.  The top layer
+                      receives dh as dh_T (no dh_seq, dc_T = 0)."""
+    dt = torch.float64 if rounding is None else torch.float32
+    dev = x.device
+    B, T, _ = x.shape
+    L = len(layers)
+    dirs = (False, True) if bidirectional else (False,)
+    keep = _keep(lengths, T, B, dev)
+
+    def rnd(l, d):
+        r = rounding[l] if isinstance(rounding, (list, tuple)) else rounding
+        return r[d] if isinstance(r, tuple) else r
+
+    def params(l, d):
+        return layers[l][d] if bidirectional else layers[l]
+
+    def name(l, d):
+        return f"LSTMLayer{l}" + ("_reverse" if dirs[d] else "")
+
+    seq = x.transpose(0, 1).to(dt)                                          # time-major [T,B,D], as RNN.fit_layers feeds it
+    saved = []                                                              # per layer: [(forward state, input, keep, scale)]
+    for l in range(L):
+        outs, sv = [], []
+        for d, rev in enumerate(dirs):
+            r, p = rnd(l, d), params(l, d)
+            kp = None if rev and defect is not None and defect.kind == "reverse_unmasked" else keep
+            fw = _forward(seq, *p, kp, rev, r, None)
+            h_seq = _state_out(fw, rev)[0]
+            sc = None
+            if dropout is not None and dropout.p > 0 and l < L - 1:
+                sc = _drop_scale(dropout, l, rev, T, B, h_seq.shape[2], dt, dev)
+                h_seq = _round(r, h_seq * sc)
+            outs.append(h_seq)
+            sv.append((fw, seq, kp, sc))
+        saved.append(sv)
+        seq = torch.cat(outs, 2) if bidirectional else outs[0]
+    r_top = rnd(L - 1, 0)
+    h_T = torch.cat([_state_out(saved[L - 1][d][0], rev)[1] for d, rev in enumerate(dirs)], 1)
+    loss = None
+    grads = {}
+    if head is not None:
+        W, b = head[0].to(dt), head[1].to(dt)
+        logits = h_T @ _round(r_top, W) + b
+        logp = torch.log_softmax(logits, 1)
+        lab = labels.long().view(-1, 1).to(dev)
+        loss = -logp.gather(1, lab).mean()
+        if backward:
+            dlogits = (logp.exp() - torch.zeros_like(logp).scatter_(1, lab, 1.0)) / B
+            dh_T = _round(r_top, dlogits @ W.t())
+            grads["Dense1/weights"] = h_T.t() @ dlogits
+            grads["Dense1/bias"] = dlogits.sum(0)
+    if not backward:
+        return ModelOut(loss, h_T, grads)
+    H_top = h_T.shape[1] // len(dirs)
+    incoming = [None] * len(dirs)                       # the gradient into each direction's output sequence (bf16 dx above)
+    for l in range(L - 1, -1, -1):
+        dxs = []
+        for d, rev in enumerate(dirs):
+            fw, x_in, kp, sc = saved[l][d]
+            p, r = params(l, d), rnd(l, d)
+            if sc is not None and defect is not None and defect.kind == "mask_next_step":
+                sc = _drop_scale(dropout._replace(step=dropout.step + 1), l, rev, T, B, sc.shape[2], dt, dev)
+            top = dh_T[:, d * H_top:(d + 1) * H_top] if l == L - 1 else None
+            g = _backward(fw, x_in, p[2], p[3], incoming[d], top, None, kp, rev, r, defect, dh_scale=sc)
+            for k, v in zip(("h0", "c0", "w_x", "w_h", "bias"), g[1:]):
+                grads[f"{name(l, d)}/{k}"] = v
+            dxs.append(g[0])
+        if l == 0:
+            break
+        if bidirectional:
+            total = _round(rnd(l, 0), dxs[0] + dxs[1])
+            if defect is not None and defect.kind == "fwd_dx_only":
+                total[defect.step] = dxs[0][defect.step]
+            H_low = total.shape[2] // 2
+            incoming = [total[..., :H_low], total[..., H_low:]]
+        else:
+            incoming = [dxs[0]]
+    return ModelOut(loss, h_T, grads)
 
 
 def check_budget(name: str, got: torch.Tensor, fp64: torch.Tensor, emulated: torch.Tensor, per_step: bool = False,

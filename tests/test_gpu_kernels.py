@@ -45,10 +45,18 @@ def test_pointwise_cell_fwd_bwd(E, dev, dtype, tol):
 
 
 @pytest.mark.parametrize("B,H,C,dtype", [(50, 96, 7, torch.bfloat16), (256, 1024, 10, torch.bfloat16), (300, 512, 40, torch.bfloat16),
-                                         (130, 256, 200, torch.bfloat16), (50, 96, 7, torch.float32), (10, 16, 3, torch.float32)])
+                                         (130, 256, 200, torch.bfloat16), (50, 96, 7, torch.float32), (10, 16, 3, torch.float32),
+                                         # backward in 32-row slabs with fp32 atomics (B > 640 at C <= 16, B > 256 at C <= 32)
+                                         (1024, 1024, 10, torch.bfloat16), (257, 256, 32, torch.bfloat16),
+                                         # the widest tensor-core head (NP = 256), and one class past each NP boundary
+                                         (200, 64, 256, torch.bfloat16), (150, 128, 17, torch.bfloat16), (150, 128, 33, torch.bfloat16),
+                                         (150, 128, 65, torch.bfloat16), (150, 128, 129, torch.bfloat16),
+                                         # bf16 h the tensor-core kernel does not take (C > 256, H % 8 != 0): logits on CUDA cores
+                                         (130, 64, 300, torch.bfloat16), (128, 100, 10, torch.bfloat16)])
 def test_head_forward_and_backward(E, dev, B, H, C, dtype):
-    """Tensor-core head (bf16 h: TMA + wgmma, epilogue from the accumulator registers) / generic head (fp32 h) vs the fp32 reference, and the fused
-    backward kernel (dh, dW, db in one launch, overwrite and accumulate)."""
+    """Tensor-core head (bf16 h: TMA + wgmma, epilogue from the accumulator registers) / generic head (fp32 h, or shapes the
+    tensor-core kernel does not take) vs the fp32 reference, and the fused backward kernel (dh, dW, db in one launch, overwrite and
+    accumulate)."""
     ref = _ref()
     torch.manual_seed(0)
     h = (torch.randn(B, H, device=dev) * 0.5).to(dtype)
@@ -56,7 +64,8 @@ def test_head_forward_and_backward(E, dev, B, H, C, dtype):
     b = torch.randn(C, device=dev)
     y = torch.randint(0, C, (B,), device=dev)
     logits, dlog, loss, corr = E.head_fwd(h, W, b, y)
-    Wr = W.bfloat16().float() if dtype == torch.bfloat16 else W          # the tensor-core path rounds W to bf16
+    tensor_cores = dtype == torch.bfloat16 and C <= 256 and H % 8 == 0
+    Wr = W.bfloat16().float() if tensor_cores else W                     # the tensor-core path rounds W to bf16, the others do not
     hr = h.float().requires_grad_(True)
     Wq = Wr.clone().requires_grad_(True)
     bq = b.clone().requires_grad_(True)
@@ -81,6 +90,54 @@ def test_head_forward_and_backward(E, dev, B, H, C, dtype):
     dW2, db2 = dW.clone(), db.clone()
     E.head_bwd(h.contiguous(), W, dlog, one, dW2, db2, True)                 # accumulate
     assert (dW2 - 2 * dW).abs().max() <= 1e-4 * max(1.0, float(dW.abs().max())) and (db2 - 2 * db).abs().max() < 1e-5
+
+
+@pytest.mark.parametrize("C", [10, 300])                  # the tensor-core head, and the CUDA-core logits + xent_rows
+def test_head_edges_against_fp64(E, dev, C):
+    """Integer-valued h and W, so the logits are exact in fp32 and the fp64 log_softmax is the reference: logits near +-80
+    (the loss and dlogits stay finite), exact ties (``correct`` follows torch.argmax's first index), the label C - 1 in the
+    padded last batch tile, and a dloss of 0.37 that scales dh, dW and db."""
+    B, H = 200, 64
+    g = torch.Generator().manual_seed(3)
+    h = torch.randint(-1, 2, (B, H), generator=g).double()
+    W = torch.randint(-3, 4, (H, C), generator=g).double()
+    b = torch.zeros(C, dtype=torch.float64)
+    b[0], b[1] = 80.0, -80.0
+    W[0] = 0.0
+    W[0, 3] = W[0, 7] = 4.0                               # classes 3 and 7 tie everywhere ...
+    W[:, 7] = W[:, 3]
+    b[7] = b[3]
+    h[: B // 2, 0] = 40.0                                 # ... and win in the first half of the rows (+160)
+    y = torch.randint(0, C, (B,), generator=g)
+    y[: B // 4], y[B // 4: B // 2] = 3, 7
+    y[B // 2: B // 2 + 8] = 1                             # labels at -80: a loss of about 160 per row
+    y[-16:] = C - 1
+    hd, Wd, bd, yd = h.to(dev, torch.bfloat16), W.float().to(dev), b.float().to(dev), y.to(dev)
+    logits, dlog, loss, corr = E.head_fwd(hd, Wd, bd, yd)
+    l64 = h @ W + b
+    assert torch.equal(logits.double().cpu(), l64)
+    logp = torch.log_softmax(l64, 1)
+    nll = -logp.gather(1, y.view(-1, 1)).squeeze(1)
+    assert torch.isfinite(loss).all() and torch.isfinite(dlog).all()
+    assert abs(float(loss) - float(nll.sum())) <= 1e-5 * float(nll.sum())
+    assert int(corr) == int((torch.argmax(l64, 1) == y).sum())
+    assert int((torch.argmax(l64, 1)[: B // 2] == 3).sum()) == B // 2          # (the ties are real and argmax takes 3)
+    d64 = (logp.exp() - torch.nn.functional.one_hot(y, C).double()) / B
+    assert float((dlog.double().cpu() - d64).abs().max()) * B <= 1e-5
+    dloss = 0.37
+    dW = torch.full((H, C), 7.0, device=dev)
+    db = torch.full((C,), 7.0, device=dev)
+    dh = E.head_bwd(hd, Wd, dlog, torch.tensor([dloss], device=dev), dW, db, False)
+    # the backward against fp64 products of the dlogits it is given: where the classes tie at logits near 160, fp32's
+    # lse = max + log(sum) carries an absolute error of up to half an ulp of 160, so dlogits (checked above) sit up to
+    # ~1e-5 relative from fp64, and dW[0, 3] = 0.37 x 40 x sum over 100 rows cancels to 0 in fp64 but not in that error
+    dk = dlog.double().cpu()
+    dh64, dW64, db64 = dloss * dk @ W.t(), dloss * h.t() @ dk, dloss * dk.sum(0)
+    assert float((dh.double().cpu() - dh64).abs().max()) <= 2.0 ** -8 * float(dh64.abs().max())
+    # fp32 sums of B terms that cancel: the worst-case bound (B + 2) u sum |terms|, element by element
+    u = (B + 2) * 2.0 ** -24
+    assert bool(((dW.double().cpu() - dW64).abs() <= u * dloss * (h.abs().t() @ dk.abs()) + 1e-30).all())
+    assert bool(((db.double().cpu() - db64).abs() <= u * dloss * dk.abs().sum(0) + 1e-30).all())
 
 
 def test_flat_adam_and_sgd(E, dev):

@@ -1,6 +1,7 @@
 """The rounding-aware LSTM reference (tests/lstm_numerics.py) on the CPU: its fp64 arm against autograd, its pair against two
-chained layers, and the error budget's sensitivity to defects confined to one step of a long sequence.  Also the sync-workspace
-guard of the persistent kernels' launch configuration."""
+chained layers, and the error budget's sensitivity to defects confined to one step of a long sequence; its whole-model arm
+against autograd on the plain composition of ops/reference, against ``pair``, and the budget's sensitivity to defects of the
+model's composition.  Also the sync-workspace guard of the persistent kernels' launch configuration."""
 import pytest
 import torch
 
@@ -125,6 +126,149 @@ def test_a_defect_at_one_step_breaks_the_budget(long_case, defect, tensor):
         rel = {n: _rel(getattr(got, n), getattr(fp64, n)) for n in ("dx", "dh0", "dc0", "dw_x", "dw_h", "db")}
         assert max(rel.values()) < 2e-2, rel
         assert _rel(got.dx[t], fp64.dx[t]) > 0.1
+
+
+# --- the whole model ----------------------------------------------------------------------------------------------------
+def _model_inputs(hidden, T, B, D, C, seed, bidirectional=False, initial_state=False, dtype=torch.float64):
+    """x [B,T,D], per-layer (direction) (h0, c0, w_x, w_h, bias), head (W, b), labels: bf16-representable where the kernels
+    read bf16.  ``initial_state``: nonzero h0 / c0 (learned), else zeros (the engine's default)."""
+    g = torch.Generator().manual_seed(seed)
+    rn = lambda *s: torch.randn(*s, generator=g, dtype=torch.float64)
+    x = _bf(rn(B, T, D) * 0.5)
+    layers, d_in = [], D
+    for H in hidden:
+        def one():
+            z = torch.zeros(B, H, dtype=torch.float64)
+            h0, c0 = (_bf(rn(B, H) * 0.3), _bf(rn(B, H) * 0.3)) if initial_state else (z, z.clone())
+            return (h0, c0, _bf(rn(4 * H, d_in) / d_in ** 0.5), _bf(rn(4 * H, H) / H ** 0.5), _bf(rn(4 * H) * 0.1))
+        layers.append((one(), one()) if bidirectional else one())
+        d_in = H * (2 if bidirectional else 1)
+    W, b = _bf(rn(d_in, C) / d_in ** 0.5), _bf(rn(C) * 0.1)
+    labels = torch.randint(0, C, (B,), generator=g)
+    cast = lambda t: t.to(dtype)
+    layers = [tuple(tuple(map(cast, p)) for p in l) if bidirectional else tuple(map(cast, l)) for l in layers]
+    return cast(x), layers, (cast(W), cast(b)), labels
+
+
+def _autograd_model(x, layers, head, labels, lengths, bidirectional, dropout):
+    """The same classifier as a plain composition of ops/reference under autograd -> (loss, h_T, {name: grad})."""
+    from lstm_tensorspark_b200.ops import reference as ref
+    dirs = (False, True) if bidirectional else (False,)
+    leaves = {}
+    for l, lp in enumerate(layers):
+        for d, rev in enumerate(dirs):
+            p = lp[d] if bidirectional else lp
+            for k, v in zip(("h0", "c0", "w_x", "w_h", "bias"), p):
+                leaves[f"LSTMLayer{l}{'_reverse' if rev else ''}/{k}"] = v.clone().requires_grad_(True)
+    leaves["Dense1/weights"], leaves["Dense1/bias"] = (t.clone().requires_grad_(True) for t in head)
+    seq = x.transpose(0, 1)
+    for l in range(len(layers)):
+        outs, finals = [], []
+        for rev in dirs:
+            n = f"LSTMLayer{l}{'_reverse' if rev else ''}/"
+            spec = None
+            if dropout is not None and l < len(layers) - 1:
+                spec = ref.DropoutSpec(dropout.p, dropout.key, l, rev, dropout.step)
+            hs, hT, _ = ref.lstm_layer_sequence(seq, *(leaves[n + k] for k in ("h0", "c0", "w_x", "w_h", "bias")),
+                                                lengths=lengths, reverse=rev, dropout=spec)
+            outs.append(hs)
+            finals.append(hT)
+        seq = torch.cat(outs, 2)
+    h_T = torch.cat(finals, 1)
+    logits = ref.dense_head(h_T, leaves["Dense1/weights"], leaves["Dense1/bias"])
+    # ref.softmax_xent, in fp64 (it casts the logits to fp32)
+    loss = -torch.log_softmax(logits, -1).gather(1, labels.view(-1, 1).long()).mean()
+    loss.backward()
+    return loss, h_T, {k: v.grad for k, v in leaves.items()}
+
+
+@pytest.mark.parametrize("case", ["three layers", "bidirectional lengths", "dropout", "bidirectional dropout",
+                                  "learned initial state"])
+def test_fp64_model_matches_autograd_on_the_reference(case):
+    T, B, D, C = 6, 5, 4, 3
+    bidir = case.startswith("bidirectional")
+    hidden = [8, 12, 8] if case == "three layers" else [8, 12]
+    x, layers, head, labels = _model_inputs(hidden, T, B, D, C, seed=11, bidirectional=bidir,
+                                            initial_state=case == "learned initial state")
+    lengths = _lengths(T, B, 12) if case == "bidirectional lengths" else None
+    dropout = N.Dropout(0.3, (5, 1), 3) if "dropout" in case else None
+    loss, h_T, want = _autograd_model(x, layers, head, labels, lengths, bidir, dropout)
+    got = N.model(x, layers, head, labels, lengths=lengths, bidirectional=bidir, dropout=dropout)
+    assert _rel(got.loss, loss) < 1e-10 and _rel(got.h_T, h_T) < 1e-10
+    assert set(got.grads) == set(want)
+    for k, v in want.items():
+        assert got.grads[k].dtype == torch.float64 and _rel(got.grads[k], v) < 1e-10, (k, _rel(got.grads[k], v))
+    if dropout is not None:                           # the masks drop something, and the step count selects them
+        other = N.model(x, layers, head, labels, bidirectional=bidir, dropout=dropout._replace(step=4), lengths=lengths)
+        assert _rel(other.loss, loss) > 1e-6
+
+
+@pytest.mark.parametrize("rounding", [None, Bf16(fwd_split=1, bwd_split=4)])
+def test_model_without_dropout_or_head_equals_pair(rounding):
+    T, B, D = 7, 6, 4
+    x, layers, _, _ = _model_inputs([8, 12], T, B, D, 3, seed=13, initial_state=True,
+                                    dtype=torch.float64 if rounding is None else torch.float32)
+    dh_T = _bf(torch.randn(B, 12, generator=torch.Generator().manual_seed(14), dtype=torch.float64)).to(x.dtype)
+    lengths = _lengths(T, B, 15)
+    got = N.model(x, layers, None, None, lengths=lengths, dh_T=dh_T, rounding=rounding)
+    a, b = N.pair(x.transpose(0, 1), layers[0], layers[1], None, None, None, dh_T, None, lengths=lengths, rounding=rounding)
+    assert torch.equal(got.h_T, b.h_T)
+    for l, out in enumerate((a, b)):
+        for k in ("dh0", "dc0", "dw_x", "dw_h", "db"):
+            n = {"dh0": "h0", "dc0": "c0", "dw_x": "w_x", "dw_h": "w_h", "db": "bias"}[k]
+            assert torch.allclose(got.grads[f"LSTMLayer{l}/{n}"], getattr(out, k), rtol=1e-12, atol=1e-14), (l, k)
+
+
+# --- the budget against defects of the model's composition --------------------------------------------------------------
+M_T, M_B, M_H, M_D, M_C = 64, 64, 256, 128, 10
+M_DROP = N.Dropout(0.2, (7, 0), 2)
+M_LOST = 40                          # rows of the first batch chunk, 256 of B = 400 scaled to B = 64
+
+
+@pytest.fixture(scope="module")
+def model_case():
+    """A bidirectional 2-layer stack with lengths (1 and T included) and dropout: fp64, the emulation and a stand-in run."""
+    x, layers, head, labels = _model_inputs([M_H, M_H], M_T, M_B, M_D, M_C, seed=17, bidirectional=True)
+    lengths = _lengths(M_T, M_B, 18)
+    f32 = lambda t: t.float()
+    l32 = [tuple(tuple(map(f32, p)) for p in l) for l in layers]
+    kw = dict(lengths=lengths, bidirectional=True, dropout=M_DROP)
+    fp64 = N.model(x, layers, head, labels, **kw)
+    emu = N.model(x.float(), l32, tuple(map(f32, head)), labels, rounding=Bf16(fwd_split=1, bwd_split=4), **kw)
+    run = lambda defect=None: N.model(x.float(), l32, tuple(map(f32, head)), labels, rounding=STANDIN, defect=defect, **kw)
+    return fp64, emu, run
+
+
+def _model_budget(got, fp64, emu):
+    """Loss, h_T per row and every gradient; raises on the first one over budget."""
+    ratios = {"loss": N.check_budget("loss", got.loss, fp64.loss, emu.loss),
+              "h_T": N.check_budget("h_T", got.h_T, fp64.h_T, emu.h_T, per_step=True)}
+    for k in fp64.grads:
+        ratios[k] = N.check_budget(k, got.grads[k], fp64.grads[k], emu.grads[k])
+    return ratios
+
+
+def test_model_emulation_sits_inside_the_budget_of_a_second_realisation(model_case):
+    fp64, emu, run = model_case
+    ratios = _model_budget(run(), fp64, emu)
+    assert max(ratios.values()) <= 1.0, ratios
+    assert 1e-4 < _rel(emu.grads["LSTMLayer0/w_x"], fp64.grads["LSTMLayer0/w_x"]) < 2e-2
+
+
+@pytest.mark.parametrize("defect,tensor", [
+    (Defect("fwd_dx_only", 1, 0), "LSTMLayer0"),                   # the reverse upper direction's dx lost at t = 1 (near its h_T)
+    (Defect("mask_next_step", 0, 0), "LSTMLayer0"),                # backward masks drawn for the next training step
+    (Defect("lost_chunk", 0, M_LOST), "LSTMLayer"),                # the second batch chunk overwrote the weight sinks
+    (Defect("reverse_unmasked", 0, 0), ""),                        # the reverse direction runs over the padding
+])
+def test_a_composition_defect_breaks_the_model_budget(model_case, defect, tensor):
+    fp64, emu, run = model_case
+    got = run(defect)
+    with pytest.raises(AssertionError, match=rf"^{tensor}[^:]*: error vs fp64 .*ratio"):
+        _model_budget(got, fp64, emu)
+    grads = {k: v for k, v in got.grads.items() if k in fp64.grads}
+    over = sorted(k for k in grads if not _rel(grads[k], fp64.grads[k]) <= 1e-2)
+    print(f"\n{defect.kind}: the per-gradient relative L2 <= 1e-2 criterion {'catches it on ' + ', '.join(over) if over else 'misses it'}")
 
 
 # --- launch configuration -----------------------------------------------------------------------------------------------
