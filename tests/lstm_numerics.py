@@ -18,10 +18,31 @@ Rounding points of the fast path (ops/cuda_lstm.py, csrc/lstm_seq_wgmma.cu), all
             fp32; the cell backward reads the bf16 activations and fp32 c, and stores dG as bf16; dW_x / dW_h are fp32 products
             of bf16 operands, db the fp32 column sum of the bf16 dG, dx = dG W_x is stored bf16.
   pair      h_seq of layer a (bf16) is layer b's input; dx of layer b (bf16) is layer a's dh_seq (ops/cuda_lstm._LSTMPairFn).
+
+The optimizer update (csrc/multi_tensor_opt.cu, TF-1.0 Adam with "epsilon-hat" or SGD over the flat fp32 master buffer) has no
+bf16 rounding point and no emulation arm: ``adam_update`` / ``sgd_update`` compute it in fp64 from the kernel's own fp32
+inputs, and ``check_update`` holds each element of the kernel's p, m, v to a worst-case bound built from sums of magnitudes
+(m and gg = g s + wd p can cancel, so a bound relative to the result would not hold).  With u = 2^-24:
+  gg        fp32 product and sum: <= 2u (|g| s + wd |p|) =: 2u |gg|_abs;
+  m         b1 m + (1 - b1) gg (1 - b1 is exact in fp32, Sterbenz): three roundings on top of gg's, 8u (b1 |m| + (1 - b1) |gg|_abs);
+  v         b2 v + (1 - b2) gg^2 likewise, 8u (b2 v + (1 - b2) |gg|_abs^2);
+  p         p - D with D = lr_t m' / (sqrt(v') + eps): 2u |p| for the subtraction, RHO |D| for the relative error of D itself,
+            and lr_t (bound on m') / (sqrt(v') + eps) for the error m' brings along;
+  floor     2^-100 absolute everywhere: build.py compiles with --use_fast_math, which flushes denormals to zero.
+RHO = 2^-11 is D's relative error under --use_fast_math, derived from the documented intrinsic bounds (not measured):
+  lr_t = lr sqrt(1 - b2^t) / (1 - b1^t) from step_dev: powf becomes __powf = ex2.approx(t __log2f(b2)).  __log2f's absolute
+            error of about 2^-21.4 becomes a relative error of t ln2 2^-21.4 in b2^t, and ex2.approx adds 2^-22.5; 1 - b2^t
+            magnifies it by b2^t / (1 - b2^t), whose product with t is largest at t = 1 (1 / (1 - b2) = 1000): <= 4.2e-4 in
+            1 - b2^t, 2.1e-4 in its square root.  The same term for b1 (1 / (1 - b1) = 10) is below 2e-6;
+  D         sqrt.approx and the approximate division add a few ulp (< 1e-6).
+So D is within 2.2e-4 of its exact value and RHO leaves a factor of 2.2.  SGD (p - lr (g s + wd p)) has no approximate
+operation: 2u |p| + 4u lr |gg|_abs.  The bf16 shadow the update kernels write has no tolerance: it must be the master rounded
+to nearest even, bit for bit (``check_shadow``).
 """
 from __future__ import annotations
 
 import dataclasses
+import math
 from typing import NamedTuple, Optional
 
 import torch
@@ -382,3 +403,90 @@ def check_budget(name: str, got: torch.Tensor, fp64: torch.Tensor, emulated: tor
             f"{floor:.2e} x |fp64| {float(sc[s]):.3e} (ratio {worst:.2f}; kernel / emulation error "
             f"{float(ek[s]) / max(float(ee[s]), 1e-300):.2f})")
     return worst
+
+
+# ---- the optimizer update (module docstring) -------------------------------------------------------------------------------
+U = 2.0 ** -24
+RHO = 2.0 ** -11
+UPDATE_FLOOR = 2.0 ** -100
+
+
+class Update(NamedTuple):
+    """One update in fp64 and the element-wise bound on a kernel's error in each tensor (m / v None for SGD)."""
+    p: torch.Tensor
+    m: Optional[torch.Tensor]
+    v: Optional[torch.Tensor]
+    bound_p: torch.Tensor
+    bound_m: Optional[torch.Tensor]
+    bound_v: Optional[torch.Tensor]
+
+
+def f32(x: float) -> float:
+    """``x`` as the fp32 value a ``float`` kernel argument receives."""
+    return float(torch.tensor(float(x), dtype=torch.float32))
+
+
+def _decayed(p, g, wd, grad_scale, wd_numel):
+    """gg = g s + wd p in fp64, the weight decay on flat elements [0, ``wd_numel``) only (-1: all), and |g| s + wd |p|."""
+    p, g = p.double(), g.double()
+    w = torch.zeros_like(p)
+    w.view(-1)[:p.numel() if wd_numel < 0 else wd_numel] = f32(wd)
+    s = f32(grad_scale)
+    return g * s + w * p, g.abs() * s + w * p.abs()
+
+
+def adam_update(p, m, v, g, t: Optional[int], lr: float, b1: float = 0.9, b2: float = 0.999, eps: float = 1e-8,
+                wd: float = 0.0, grad_scale: float = 1.0, wd_numel: int = -1) -> Update:
+    """``flat_adam_kernel`` (``ops/reference.adam_step_``'s math) on the kernel's fp32 ``p``, ``m``, ``v`` before the step and
+    gradient ``g`` (flat, contiguous).  ``t``: the step count the kernel reads from ``step_dev`` after its increment - ``lr``
+    is then the base learning rate; None: ``lr`` is the host-computed lr_t.  The scalars are taken as the fp32 values the
+    kernel receives."""
+    lr, b1, b2, eps = f32(lr), f32(b1), f32(b2), f32(eps)
+    gg, ga = _decayed(p, g, wd, grad_scale, wd_numel)
+    m, v = m.double(), v.double()
+    lr_t = lr if t is None else lr * math.sqrt(1.0 - b2 ** t) / (1.0 - b1 ** t)
+    m1 = b1 * m + (1.0 - b1) * gg
+    v1 = b2 * v + (1.0 - b2) * gg * gg
+    den = v1.sqrt() + eps
+    step = lr_t * m1 / den
+    bm = 8 * U * (b1 * m.abs() + (1.0 - b1) * ga) + UPDATE_FLOOR
+    bv = 8 * U * (b2 * v + (1.0 - b2) * ga * ga) + UPDATE_FLOOR
+    bp = 2 * U * p.double().abs() + RHO * step.abs() + lr_t * bm / den + UPDATE_FLOOR
+    return Update(p.double() - step, m1, v1, bp, bm, bv)
+
+
+def sgd_update(p, g, lr: float, wd: float = 0.0, grad_scale: float = 1.0, wd_numel: int = -1) -> Update:
+    """``flat_sgd_kernel`` (``ops/reference.sgd_step_``'s math), as ``adam_update``."""
+    lr = f32(lr)
+    gg, ga = _decayed(p, g, wd, grad_scale, wd_numel)
+    bp = 2 * U * p.double().abs() + 4 * U * lr * ga + UPDATE_FLOOR
+    return Update(p.double() - lr * gg, None, None, bp, None, None)
+
+
+def check_update(name: str, got: torch.Tensor, ref: torch.Tensor, bound: torch.Tensor) -> float:
+    """Assert |got - ref| <= bound element by element and return the worst ratio of the two sides."""
+    g = got.detach().double().to(ref.device).reshape(-1)
+    r, b = ref.reshape(-1), bound.reshape(-1)
+    ratio = (g - r).abs() / b
+    ratio = torch.where(torch.isnan(ratio), float("inf"), ratio)
+    i = int(ratio.argmax())
+    worst = float(ratio[i])
+    if not worst <= 1.0:
+        at = tuple(int(k) for k in torch.unravel_index(torch.tensor(i), tuple(ref.shape)))
+        over = int((~(ratio <= 1.0)).sum())
+        raise AssertionError(
+            f"{name}: element {at}: {float(g[i]):.9e} vs fp64 {float(r[i]):.9e}, error {abs(float(g[i]) - float(r[i])):.3e} "
+            f"exceeds the bound {float(b[i]):.3e} (ratio {worst:.2f}; {over} of {r.numel()} elements over)")
+    return worst
+
+
+def check_shadow(name: str, shadow: torch.Tensor, master: torch.Tensor) -> None:
+    """Assert the bf16 ``shadow`` is ``master`` rounded to nearest even, bit for bit."""
+    want = master.detach().to(torch.bfloat16).reshape(-1)
+    got = shadow.detach().reshape(-1)
+    bad = got.view(torch.int16) != want.view(torch.int16)
+    if bool(bad.any()):
+        i = int(bad.nonzero()[0])
+        raise AssertionError(f"{name}: the bf16 shadow differs from the rounded master at {int(bad.sum())} of {bad.numel()} "
+                             f"elements; first at {i}: {float(got[i]):.6e} vs {float(want[i]):.6e} (master "
+                             f"{float(master.reshape(-1)[i]):.9e})")

@@ -140,28 +140,81 @@ def test_head_edges_against_fp64(E, dev, C):
     assert bool(((db.double().cpu() - db64).abs() <= u * dloss * dk.abs().sum(0) + 1e-30).all())
 
 
+N_HEADLINE = 1025 * 16384        # about the headline flat buffer (2 x 1024 LSTM + head): 16 grid-stride passes of the kernels
+
+
+def _update_state(n, dev, seed):
+    """fp32 p, m, v and a gradient with magnitudes from 1e-4 to 1; the last 64 elements (alignment padding) all zero."""
+    gen = torch.Generator(device=dev).manual_seed(seed)
+    scale = 10.0 ** (torch.rand(n, generator=gen, device=dev) * 4 - 4)
+    p = torch.randn(n, generator=gen, device=dev) * 0.05
+    g = torch.randn(n, generator=gen, device=dev) * scale
+    m = torch.randn(n, generator=gen, device=dev) * scale * 0.3
+    v = scale * scale * (0.5 + torch.rand(n, generator=gen, device=dev))
+    for x in (p, g, m, v):
+        x[-64:] = 0
+    return p, g, m, v
+
+
+def _flat_steps(E, dev, p, m, v, grads, kind, lr, t0=None, wd=0.0, gscale=1.0, wd_numel=-1):
+    """One update per gradient of ``grads`` (in place on p, m, v), each against the fp64 update of the state before it
+    (lstm_numerics.adam_update / sgd_update), element by element; the bf16 shadow bit for bit, the zero padding (the last 64
+    elements) left at 0.  Adam: ``t0`` None = the host's lr_t of steps 1, 2, ...; else the bias correction from step_dev,
+    preset to ``t0`` - 1 as a resumed run's.  -> the worst update ratio."""
+    import lstm_numerics as N
+    sh = torch.empty_like(p, dtype=torch.bfloat16)
+    step_dev = None if t0 is None else torch.full((1,), t0 - 1, dtype=torch.int32, device=dev)
+    worst = 0.0
+    for k, g in enumerate(grads):
+        p0, m0, v0 = p.clone(), m.clone(), v.clone()
+        if kind == "sgd":
+            E.flat_sgd(p, g, sh, lr, wd, gscale, wd_numel)
+            ref = N.sgd_update(p0, g, lr, wd, gscale, wd_numel)
+        elif t0 is None:
+            t = k + 1
+            lr_t = lr * (1 - 0.999 ** t) ** 0.5 / (1 - 0.9 ** t)
+            E.flat_adam(p, g, m, v, sh, lr_t, 0.9, 0.999, 1e-8, wd, gscale, None, wd_numel)
+            ref = N.adam_update(p0, m0, v0, g, None, lr_t, wd=wd, grad_scale=gscale, wd_numel=wd_numel)
+        else:
+            E.flat_adam(p, g, m, v, sh, lr, 0.9, 0.999, 1e-8, wd, gscale, step_dev, wd_numel)
+            assert int(step_dev) == t0 + k
+            ref = N.adam_update(p0, m0, v0, g, t0 + k, lr, wd=wd, grad_scale=gscale, wd_numel=wd_numel)
+        worst = max(worst, N.check_update(f"step {k} p", p, ref.p, ref.bound_p))
+        if kind == "adam":
+            worst = max(worst, N.check_update(f"step {k} m", m, ref.m, ref.bound_m),
+                        N.check_update(f"step {k} v", v, ref.v, ref.bound_v))
+        N.check_shadow(f"step {k}", sh, p)
+        assert not bool(p[-64:].any() or m[-64:].any() or v[-64:].any())
+    return worst
+
+
 def test_flat_adam_and_sgd(E, dev):
-    ref = _ref()
+    """Three Adam steps with the host's lr_t and a gradient scale of 0.5 from zero moments, then SGD without and with weight
+    decay over the first 4096 elements, against the fp64 update."""
     torch.manual_seed(0)
     n = 16384
     p = torch.randn(n, device=dev); g = torch.randn(n, device=dev)
+    p[-64:] = 0; g[-64:] = 0
     m = torch.zeros(n, device=dev); v = torch.zeros(n, device=dev)
-    p2, m2, v2 = p.clone(), m.clone(), v.clone()
-    sh = torch.empty(n, dtype=torch.bfloat16, device=dev)
-    for step in (1, 2, 3):
-        lr_t = 1e-3 * (1 - 0.999 ** step) ** 0.5 / (1 - 0.9 ** step)
-        E.flat_adam(p, g, m, v, sh, lr_t, 0.9, 0.999, 1e-8, 0.0, 0.5)
-        ref.adam_step_(p2, g, m2, v2, step, 1e-3, grad_scale=0.5)
-    assert (p - p2).abs().max() < 1e-5 and (sh.float() - p).abs().max() < 2e-2
-    q = p.clone()
-    E.flat_sgd(p, g, None, 0.1, 0.0, 1.0)
-    assert torch.allclose(p, q - 0.1 * g, atol=1e-6)
-    # weight decay (K12) folded into the update, restricted to the first wd_numel elements
-    q = p.clone()
-    E.flat_sgd(p, g, None, 0.1, 0.5, 1.0, 4096)
-    exp = q - 0.1 * g
-    exp[:4096] -= 0.1 * 0.5 * q[:4096]
-    assert torch.allclose(p, exp, atol=1e-6)
+    _flat_steps(E, dev, p, m, v, [g] * 3, "adam", 1e-3, gscale=0.5)
+    _flat_steps(E, dev, p, m, v, [g], "sgd", 0.1)
+    _flat_steps(E, dev, p, m, v, [g], "sgd", 0.1, wd=0.5, wd_numel=4096)
+
+
+@pytest.mark.parametrize("wd,gscale", [(0.0, 1.0), (0.1, 0.37)], ids=["plain", "wd-gscale"])
+@pytest.mark.parametrize("kind,t0", [("adam", None), ("adam", 1), ("adam", 2), ("adam", 1000), ("adam", 100000), ("sgd", None)],
+                         ids=["adam-host-lr_t", "adam-t1", "adam-t2", "adam-t1000", "adam-t100000", "sgd"])
+@pytest.mark.parametrize("n", [16384, N_HEADLINE])
+def test_flat_update_kernels_against_fp64(E, dev, n, kind, t0, wd, gscale):
+    """Two consecutive updates over the flat buffer against the fp64 update: one grid-stride pass or about the headline's 16,
+    Adam with the host's lr_t or its bias correction from step_dev (preset as a resumed run's), SGD, weight decay over
+    [0, wd_numel) with wd_numel inside a grid-stride pass, a gradient scale."""
+    p, g, m, v = _update_state(n, dev, seed=n % 1000 + (t0 or 0))
+    g2 = g.roll(4096)                                                        # the second step's gradient
+    g2[-64:] = 0
+    wd_numel = (n * 3 // 4) // 64 * 64 + 20
+    worst = _flat_steps(E, dev, p, m, v, [g, g2], kind, 0.05 if kind == "sgd" else 1e-3, t0, wd, gscale, wd_numel)
+    print(f"\nflat {kind} n={n} t0={t0} wd={wd}: worst update ratio {worst:.3f}")
 
 
 @pytest.mark.parametrize("ctas,bn", [(1, 128), (1, 256), (2, 128), (2, 256)])

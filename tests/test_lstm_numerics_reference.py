@@ -284,3 +284,111 @@ def test_seq_config_rejects_layouts_whose_arrival_counters_overflow_the_sync_wor
     assert E.lstm_seq_config(False, 256, 2048, 2)[1] == 2     # the forward has a quarter of the counters
     assert E.lstm_seq_config(True, 1024, 256, 2) == (4, 2, False, False)
     assert E.lstm_seq_config(True, 2048, 64, 0)[2] is True
+
+
+# --- the optimizer update -----------------------------------------------------------------------------------------------
+STRIDE = 132 * 8 * 256 * 4           # floats one grid-stride pass of the update kernels covers (grid_for, multi_tensor_opt.cu)
+U_N = 2 * STRIDE + 300 * 1024        # a flat buffer of three passes, the last one partial
+U_WD = 2 * STRIDE + 128 * 1024       # end of the LSTM segment: weight decay covers [0, U_WD)
+U_BIAS = 4096                        # the last LSTM variable, a bias, ends at U_WD; a dense head follows it
+U_PAD = 64                           # trailing alignment padding: every value 0
+LR_T_APPROX = 2.2e-4                 # the worst relative error of the in-kernel lr_t under --use_fast_math (lstm_numerics)
+ADAM = dict(lr=1e-3, b1=0.9, b2=0.999, eps=1e-8, wd=0.1, grad_scale=0.37, wd_numel=U_WD)
+
+
+def _update_state(seed, n=U_N):
+    """fp32 p, m, v and two consecutive gradients with magnitudes from 1e-4 to 1 (padding all zero)."""
+    gen = torch.Generator().manual_seed(seed)
+    scale = 10.0 ** (torch.rand(n, generator=gen) * 4 - 4)
+    p = torch.randn(n, generator=gen) * 0.05
+    g = torch.randn(n, generator=gen) * scale
+    g_prev = torch.randn(n, generator=gen) * scale
+    m = torch.randn(n, generator=gen) * scale * 0.3
+    v = scale * scale * (0.5 + torch.rand(n, generator=gen))
+    for t in (p, g, g_prev, m, v):
+        t[-U_PAD:] = 0
+    return p, m, v, g, g_prev
+
+
+def _adam_f32(p, m, v, g, t, lr, b1, b2, eps, wd, grad_scale, wd_numel, defect=None):
+    """flat_adam_kernel with the bias correction from step_dev, in fp32 arithmetic with lr_t off by the worst fast-math
+    error - and ``defect`` planted."""
+    f = lambda x: torch.tensor(x, dtype=torch.float32)
+    if defect == "b1 b2 swapped":
+        b1, b2 = b2, b1
+    tt = t + 1 if defect == "lr_t of t + 1" else t
+    lr_t = f(lr) * torch.sqrt(1 - f(b2) ** tt) / (1 - f(b1) ** tt) * f(1 + LR_T_APPROX)
+    hi = {"wd missing on the bias": wd_numel - U_BIAS, "wd past wd_numel": wd_numel + 64}.get(defect, wd_numel)
+    w = torch.zeros_like(p)
+    w[:hi] = f(wd)
+    gg = g * f(grad_scale) + w * p
+    m1 = f(b1) * m + (1 - f(b1)) * gg
+    v1 = f(b2) * v + (1 - f(b2)) * gg * gg
+    p1 = p - lr_t * m1 / (torch.sqrt(v1) + f(eps))
+    skip = {"last float4 not updated": slice(p.numel() - U_PAD - 4, p.numel() - U_PAD),
+            "one grid-stride pass not updated": slice(STRIDE, 2 * STRIDE)}.get(defect)
+    if skip is not None:
+        p1[skip], m1[skip], v1[skip] = p[skip], m[skip], v[skip]
+    return p1, m1, v1
+
+
+def _check_adam(got, ref):
+    return max(N.check_update(k, a, b, bnd) for k, a, b, bnd in zip("pmv", got, ref[:3], ref[3:]))
+
+
+@pytest.mark.parametrize("t", [1, 2, 1000, 100000])
+def test_fp64_update_matches_the_reference_optimizer(t):
+    """adam_update / sgd_update == ops/reference.adam_step_ / sgd_step_ run in fp64 on the fp32 scalars, the weight decay over
+    [0, wd_numel) as FlatOptimizer applies it."""
+    from lstm_tensorspark_b200.ops import reference as ref
+    p, m, v, g, _ = _update_state(7, n=1 << 16)
+    wd_n = 40000
+    f = N.f32
+    got = N.adam_update(p, m, v, g, t, **{**ADAM, "wd_numel": wd_n})
+    p64, m64, v64, g64 = (x.double() for x in (p, m, v, g))
+    for lo, hi, wd in ((0, wd_n, f(0.1)), (wd_n, p.numel(), 0.0)):
+        ref.adam_step_(p64[lo:hi], g64[lo:hi], m64[lo:hi], v64[lo:hi], t, f(1e-3), f(0.9), f(0.999), f(1e-8), wd, f(0.37))
+    for a, b, bound in ((got.p, p64, got.bound_p), (got.m, m64, got.bound_m), (got.v, v64, got.bound_v)):
+        assert bool(((a - b).abs() <= 1e-8 * bound).all())            # fp64 rounding only: 1e-8 of the fp32 bound
+    sgd = N.sgd_update(p, g, 0.05, 0.1, 0.37, wd_n)
+    q64 = p.double()
+    for lo, hi, wd in ((0, wd_n, f(0.1)), (wd_n, p.numel(), 0.0)):
+        ref.sgd_step_(q64[lo:hi], g64[lo:hi], f(0.05), wd, f(0.37))
+    assert bool(((sgd.p - q64).abs() <= 1e-8 * sgd.bound_p).all())
+    assert bool((got.p[-U_PAD:] == 0).all()) and bool((sgd.p[-U_PAD:] == 0).all())
+
+
+@pytest.mark.parametrize("t", [1, 2, 5, 100, 1000, 100000])
+def test_fp32_update_sits_inside_the_bound(t):
+    """An fp32 realisation of the update kernels (Adam's lr_t off by its worst fast-math error) passes check_update."""
+    p, m, v, g, _ = _update_state(3)
+    worst = _check_adam(_adam_f32(p, m, v, g, t, **ADAM), N.adam_update(p, m, v, g, t, **ADAM))
+    lr, wd, gs = N.f32(0.05), N.f32(0.1), N.f32(0.37)
+    w = torch.zeros_like(p)
+    w[:U_WD] = wd
+    q = p - torch.tensor(lr) * (g * torch.tensor(gs) + w * p)
+    ref = N.sgd_update(p, g, 0.05, 0.1, 0.37, U_WD)
+    worst_sgd = N.check_update("p", q, ref.p, ref.bound_p)
+    assert 0.05 < worst <= 1.0 and worst_sgd <= 1.0, (worst, worst_sgd)
+
+
+@pytest.mark.parametrize("defect,t", [("lr_t of t + 1", 1), ("lr_t of t + 1", 5), ("lr_t of t + 1", 100),
+                                      ("wd missing on the bias", 1000), ("wd past wd_numel", 1000), ("b1 b2 swapped", 1000),
+                                      ("previous gradient", 1000), ("last float4 not updated", 1000),
+                                      ("one grid-stride pass not updated", 1000)])
+def test_an_update_defect_breaks_the_bound(defect, t):
+    p, m, v, g, g_prev = _update_state(5)
+    got = _adam_f32(p, m, v, g_prev if defect == "previous gradient" else g, t, defect=defect, **ADAM)
+    with pytest.raises(AssertionError, match=r"^[pmv]: element .* exceeds the bound"):
+        _check_adam(got, N.adam_update(p, m, v, g, t, **ADAM))
+
+
+def test_shadow_is_checked_bit_for_bit():
+    p = torch.randn(4096) * 0.05
+    N.check_shadow("shadow", p.bfloat16(), p)
+    sh = p.bfloat16()
+    sh.view(torch.int16)[1000] += 1                     # one ulp off at one element
+    with pytest.raises(AssertionError, match=r"^shadow: .* at 1 of 4096 elements; first at 1000"):
+        N.check_shadow("shadow", sh, p)
+    with pytest.raises(AssertionError, match="shadow"):
+        N.check_shadow("shadow", (p * (1 + 2.0 ** -10)).bfloat16(), p)      # the shadow of the weights before a step
