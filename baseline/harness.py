@@ -27,8 +27,9 @@ import torch.nn.functional as F
 
 
 class CudnnLSTMClassifier(nn.Module):
-    def __init__(self, hidden, in_features, num_classes, time_major=False, bidirectional=False, dropout=0.0):
+    def __init__(self, hidden, in_features, num_classes, time_major=False, bidirectional=False, dropout=0.0, per_step=False):
         super().__init__()
+        self.per_step = per_step
         assert len(set(hidden)) == 1, "nn.LSTM stacks equal-width layers"
         self.time_major = time_major
         self.bidirectional = bidirectional
@@ -38,6 +39,8 @@ class CudnnLSTMClassifier(nn.Module):
 
     def forward(self, x):
         out, (h_n, _) = self.lstm(x)
+        if self.per_step:                               # nn.Linear over every output: logits [B,T,C] (time-major: [T,B,C])
+            return self.head(out)
         if self.bidirectional:                          # [forward final | reverse final (after time 0)], as the framework's model
             return self.head(torch.cat([h_n[-2], h_n[-1]], 1))
         return self.head(out[-1] if self.time_major else out[:, -1, :])
@@ -45,10 +48,13 @@ class CudnnLSTMClassifier(nn.Module):
 
 class BaselineRunner:
     def __init__(self, hidden, in_features, num_classes, batch, seq_len, rank, world, device, optimizer="adam", lr=1e-3,
-                 variant="stock", bidirectional=False, dropout=0.0):
+                 variant="stock", bidirectional=False, dropout=0.0, per_step=False):
+        """``per_step``: sequence labelling - labels ``[B,T]``, the head over every output and the mean cross-entropy over all
+        ``T·B`` positions (default: classify the final state, labels ``[B]``)."""
         self.rank, self.world, self.device = rank, world, device
         self.B, self.T, self.D, self.C = batch, seq_len, in_features, num_classes
         self.variant = variant
+        self.per_step = per_step
         self.tuned = variant == "tuned"
         self.graph = None
         self.bound = {}
@@ -57,7 +63,7 @@ class BaselineRunner:
         if world > 1 and not dist.is_initialized():
             dist.init_process_group("nccl", rank=rank, world_size=world, device_id=device)
         model = CudnnLSTMClassifier(hidden, in_features, num_classes, time_major=self.tuned, bidirectional=bidirectional,
-                                    dropout=dropout).to(device)
+                                    dropout=dropout, per_step=per_step).to(device)
         if self.tuned:
             model = model.to(torch.bfloat16)
             model.lstm.flatten_parameters()
@@ -79,7 +85,10 @@ class BaselineRunner:
         self.opt.zero_grad(set_to_none=True)
         with torch.autocast("cuda", dtype=torch.bfloat16):
             logits = self.model(x)
-        loss = F.cross_entropy(logits.float(), y)
+        if self.per_step:
+            loss = F.cross_entropy(logits.float().reshape(-1, self.C), y.reshape(-1))
+        else:
+            loss = F.cross_entropy(logits.float(), y)
         loss.backward()
         self.opt.step()
         return loss.detach()
@@ -89,7 +98,10 @@ class BaselineRunner:
         for p in self.params:
             p.grad = None
         logits = self.model(x.transpose(0, 1))
-        loss = F.cross_entropy(logits.float(), y)
+        if self.per_step:                                # time-major logits [T,B,C] against labels [B,T]
+            loss = F.cross_entropy(logits.float().reshape(-1, self.C), y.t().reshape(-1))
+        else:
+            loss = F.cross_entropy(logits.float(), y)
         loss.backward()
         with torch.no_grad():
             torch._foreach_copy_([m.grad for m in self.masters], [p.grad for p in self.params])  # bf16 grads -> fp32
@@ -147,13 +159,13 @@ class BaselineRunner:
         rng = np.random.default_rng(1234 + self.rank)
         nb = 4
         xs = rng.standard_normal((nb * B, T, D), dtype=np.float32)
-        ys = rng.integers(0, C, size=nb * B).astype(np.int64)
+        ys = rng.integers(0, C, size=(nb * B, T) if self.per_step else nb * B).astype(np.int64)
         dev_x = torch.as_tensor(xs).to(self.device, dtype=torch.bfloat16)
         dev_y = torch.as_tensor(ys).to(self.device)
         host_x = torch.as_tensor(xs).to(torch.bfloat16).pin_memory()
         host_y = torch.as_tensor(ys).pin_memory()
         stage = [(torch.empty(B, T, D, dtype=torch.bfloat16, device=self.device),
-                  torch.empty(B, dtype=torch.int64, device=self.device)) for _ in range(2)]
+                  torch.empty((B, T) if self.per_step else (B,), dtype=torch.int64, device=self.device)) for _ in range(2)]
         loss_host = torch.empty(2, dtype=torch.float32, pin_memory=True)
         loss_evt = [torch.cuda.Event(), torch.cuda.Event()]
         it = {"i": 0, "slot": 0, "pending": None, "k": 0, "last": float("nan")}
@@ -198,6 +210,6 @@ class BaselineRunner:
         if self.tuned:
             graphed = self.capture(dev_x[:B], dev_y[:B], bind=[(dev_x[i * B:(i + 1) * B], dev_y[i * B:(i + 1) * B]) for i in range(nb)] + stage
                                    if self.bind_inputs else ())
-        h2d = B * T * D * 2 + B * 8
+        h2d = B * T * D * 2 + B * (T if self.per_step else 1) * 8
         return step_dev, step_e2e, h2d, 4, 0, {"lstm": "cudnn", "comm": "nccl-ddp" if self.world > 1 else "none",
                                               "variant": self.variant, "cuda_graph": graphed}

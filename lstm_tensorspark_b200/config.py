@@ -46,6 +46,9 @@ class Config:
                                         # [forward | reverse] (2 H wide), as nn.LSTM(bidirectional=True) on a packed sequence
     dropout: float = 0.0                # nn.LSTM(dropout=P): in training, the output sequence of every layer but the last is
                                         # multiplied by a Bernoulli(1-P) mask / (1-P) before the next layer reads it
+    per_step_labels: bool = False       # sequence labelling: a label at every time step ([B,T]), the head scores the top layer's
+                                        # output at each step (nn.LSTM -> nn.Linear -> cross_entropy over the real positions); a CSV
+                                        # row is k*in_features values followed by k labels
     dtype: str = "auto"                 # auto: bf16 on cuda, fp32 on cpu
     device: str = "auto"                # auto | cpu | cuda
     backend: str = "auto"               # auto | cuda_ext (hand-written sm_90a kernels) | torch
@@ -126,6 +129,9 @@ class Config:
             raise ValueError("--variable_length needs --seq_len >= 2 (the longest sample's number of steps)")
         if self.bidirectional and self.seq_len < 2:
             raise ValueError("--bidirectional needs --seq_len >= 2 (the reverse direction runs over a whole sequence)")
+        if self.per_step_labels and self.seq_len < 2:
+            raise ValueError("--per_step_labels needs --seq_len >= 2 (one label per time step of a sequence; the one-step [B,D] "
+                             "path classifies the last state only)")
         if not 0.0 <= self.dropout < 1.0:
             raise ValueError(f"--dropout must satisfy 0 <= P < 1, got {self.dropout}")
         if self.dropout > 0 and len(self.hidden_list()) == 1:
@@ -176,6 +182,8 @@ _HELP = {
     "output_path": "Path for store network state",
     "mode": "Execution mode",
     "checkpoint_path": "Directory where to save network model and logs",
+    "per_step_labels": "Label every time step (sequence labelling): labels [B,T], loss and accuracy over the real positions; "
+                       "a CSV row is k*in_features values followed by k labels",
 }
 
 

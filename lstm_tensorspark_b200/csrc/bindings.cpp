@@ -40,6 +40,13 @@ int ts_ar_slots();
 int ts_head_fwd_tc(const void*, int, const float*, const float*, const long long*, float*, float*, float*, int*, int, int, int, cudaStream_t);
 int ts_head_logits_generic(const void*, const float*, const float*, float*, int, int, int, int, cudaStream_t);
 int ts_head_bwd(const void*, const float*, const float*, const float*, void*, float*, float*, int, int, int, int, int, cudaStream_t);
+int ts_head_step_fwd_generic_parts(int);
+int ts_head_step_fwd(const void*, int, int, const float*, const float*, const long long*, const int*, float*, float*, float*, int*,
+                     unsigned int*, float*, int*, int*, int, int, int, int, int*, cudaStream_t);
+long long ts_head_step_bwd_scratch(int, int, int);
+int ts_head_step_bwd_tickets(int);
+int ts_head_step_bwd(const void*, const float*, const float*, const float*, void*, float*, float*, float*, unsigned int*, int, int, int,
+                     int, int, cudaStream_t);
 int ts_gemm_generic(const void*, const void*, void*, const float*, int, int, int, long long, long long, long long, long long, long long,
                     int, int, int, float, cudaStream_t);
 int ts_gemm2(const void*, const void*, void*, const float*, int, int, int, int, int, int, int, int, int, int, int, int, int,
@@ -277,6 +284,71 @@ Tensor head_bwd(const Tensor& h, const Tensor& W, const Tensor& dlogits, const s
   auto dh = torch::empty_like(h);
   check(ts_head_bwd(h.data_ptr(), W.data_ptr<float>(), dlogits.data_ptr<float>(), fptr(dloss), dh.data_ptr(), dW.data_ptr<float>(),
                     db.data_ptr<float>(), B, H, C, is_bf16(h), accumulate ? 1 : 0, stream()), "head_bwd");
+  return dh;
+}
+
+// Per-step head (csrc/head_wgmma.cu): h [T·B, H] = the rows of h_seq [T,B,H] (row pitch = stride(0)), labels int64 [B,T], optional
+// lengths int32 [B] -> logits [B,T,C], dlogits [T·B,C] (row order of h), loss (mean over counted rows), correct, N, and whether the
+// tensor-core kernel ran.  Nothing is read back to the host.
+std::vector<Tensor> head_step_fwd(const Tensor& h, const Tensor& W, const Tensor& bias, const Tensor& labels,
+                                  const std::optional<Tensor>& lengths, int64_t T) {
+  TORCH_CHECK(h.is_cuda() && h.dim() == 2 && h.stride(1) == 1, "head_step_fwd: h [T*B,H] with unit inner stride");
+  chk_cuda(W, "W"); chk_cuda(bias, "bias"); chk_cuda(labels, "labels");
+  c10::cuda::CUDAGuard g(h.device());
+  const int R = h.size(0), H = h.size(1), C = W.size(1);
+  TORCH_CHECK(T >= 1 && R % T == 0, "head_step_fwd: rows must be T*B");
+  const int B = R / (int)T;
+  TORCH_CHECK(W.size(0) == H && W.scalar_type() == torch::kFloat32 && bias.scalar_type() == torch::kFloat32 && bias.numel() == C, "head W/b");
+  TORCH_CHECK(labels.scalar_type() == torch::kInt64 && labels.dim() == 2 && labels.size(0) == B && labels.size(1) == T, "labels int64 [B,T]");
+  const int* lp = nullptr;
+  if (lengths.has_value()) {
+    chk_cuda(*lengths, "lengths");
+    TORCH_CHECK(lengths->scalar_type() == torch::kInt32 && lengths->numel() == B, "lengths int32 [B]");
+    lp = lengths->data_ptr<int>();
+  }
+  auto fo = torch::TensorOptions().device(h.device()).dtype(torch::kFloat32);
+  auto io = fo.dtype(torch::kInt32);
+  auto logits = torch::empty({B, (int64_t)T, C}, fo), dlogits = torch::empty({R, C}, fo);
+  const int parts = ts_head_step_fwd_generic_parts(R);         // the larger of the two paths' grids
+  auto part_loss = torch::empty({parts}, fo);
+  auto ints = torch::zeros({parts + 4}, io);                   // [parts] per-CTA counts, ticket, correct, N
+  auto loss = torch::empty({1}, fo);
+  Tensor hc = h;
+  if (h.scalar_type() != torch::kBFloat16 && h.stride(0) != H) hc = h.contiguous();
+  int used_tc = 0;
+  int rc = ts_head_step_fwd(hc.data_ptr(), (int)hc.stride(0), is_bf16(hc), W.data_ptr<float>(), bias.data_ptr<float>(),
+                            (const long long*)labels.data_ptr<int64_t>(), lp, logits.data_ptr<float>(), dlogits.data_ptr<float>(),
+                            part_loss.data_ptr<float>(), ints.data_ptr<int>(), (unsigned int*)(ints.data_ptr<int>() + parts),
+                            loss.data_ptr<float>(), ints.data_ptr<int>() + parts + 1, ints.data_ptr<int>() + parts + 2, (int)T, B, H, C,
+                            &used_tc, stream());
+  if (rc == -2) {                                              // a strided bf16 h the tensor-core kernel did not take
+    hc = h.contiguous();
+    rc = ts_head_step_fwd(hc.data_ptr(), H, 1, W.data_ptr<float>(), bias.data_ptr<float>(), (const long long*)labels.data_ptr<int64_t>(),
+                          lp, logits.data_ptr<float>(), dlogits.data_ptr<float>(), part_loss.data_ptr<float>(), ints.data_ptr<int>(),
+                          (unsigned int*)(ints.data_ptr<int>() + parts), loss.data_ptr<float>(), ints.data_ptr<int>() + parts + 1,
+                          ints.data_ptr<int>() + parts + 2, (int)T, B, H, C, &used_tc, stream());
+  }
+  check(rc, "head_step_fwd");
+  return {logits, dlogits, loss, ints.narrow(0, parts + 1, 1), ints.narrow(0, parts + 2, 1),
+          torch::full({1}, used_tc, torch::TensorOptions().dtype(torch::kInt32))};
+}
+
+// dh = (dloss * dlogits) W^T [T·B,H] (dtype of h), dW (+)= h^T (dloss * dlogits), db (+)= column sums: one launch, reduced in a
+// fixed order (bitwise reproducible).
+Tensor head_step_bwd(const Tensor& h, const Tensor& W, const Tensor& dlogits, const std::optional<Tensor>& dloss, Tensor dW, Tensor db,
+                     bool accumulate) {
+  chk_cuda(h, "h"); chk_cuda(W, "W"); chk_cuda(dlogits, "dlogits"); chk_cuda(dW, "dW"); chk_cuda(db, "db");
+  c10::cuda::CUDAGuard g(h.device());
+  const int R = h.size(0), H = h.size(1), C = W.size(1);
+  TORCH_CHECK(dW.scalar_type() == torch::kFloat32 && db.scalar_type() == torch::kFloat32 && dW.numel() == (int64_t)H * C && db.numel() == C, "head_step_bwd: dW/db");
+  TORCH_CHECK(dlogits.scalar_type() == torch::kFloat32 && dlogits.numel() == (int64_t)R * C, "head_step_bwd: dlogits fp32 [R,C]");
+  auto dh = torch::empty_like(h);
+  auto fo = torch::TensorOptions().device(h.device()).dtype(torch::kFloat32);
+  auto scratch = torch::empty({std::max<long long>(1, ts_head_step_bwd_scratch(R, H, C))}, fo);
+  auto tickets = torch::zeros({ts_head_step_bwd_tickets(H)}, fo.dtype(torch::kInt32));
+  check(ts_head_step_bwd(h.data_ptr(), W.data_ptr<float>(), dlogits.data_ptr<float>(), fptr(dloss), dh.data_ptr(), dW.data_ptr<float>(),
+                         db.data_ptr<float>(), scratch.data_ptr<float>(), (unsigned int*)tickets.data_ptr<int>(), R, H, C, is_bf16(h),
+                         accumulate ? 1 : 0, stream()), "head_step_bwd");
   return dh;
 }
 
@@ -538,6 +610,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("c_new"), py::arg("lengths") = py::none(), py::arg("t") = 0);
   m.def("xent_rows", &xent_rows);
   m.def("head_fwd", &head_fwd);
+  m.def("head_step_fwd", &head_step_fwd, py::arg("h"), py::arg("W"), py::arg("bias"), py::arg("labels"), py::arg("lengths"), py::arg("T"));
+  m.def("head_step_bwd", &head_step_bwd, py::arg("h"), py::arg("W"), py::arg("dlogits"), py::arg("dloss"), py::arg("dW"), py::arg("db"),
+        py::arg("accumulate"));
   m.def("head_bwd", &head_bwd, py::arg("h"), py::arg("W"), py::arg("dlogits"), py::arg("dloss"), py::arg("dW"), py::arg("db"),
         py::arg("accumulate") = false);
   m.def("flat_adam", &flat_adam, py::arg("p"), py::arg("g"), py::arg("m"), py::arg("v"), py::arg("shadow"), py::arg("lr_t"),

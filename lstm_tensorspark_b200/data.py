@@ -151,6 +151,49 @@ def process_batch_ragged(train_xy: Sequence[Sequence[str]], seq_len: int, in_fea
     return x, np.asarray(ys, dtype=np.int64), np.asarray(ls, dtype=np.int32)
 
 
+def process_batch_per_step(train_xy: Sequence[Sequence[str]], seq_len: int, in_features: int, num_classes: int,
+                           variable_length: bool = False, normalize: bool = False):
+    """Rows with a label at every step (``--per_step_labels``) -> ``(x float32 [N, seq_len, in_features], y int64 [N, seq_len])``,
+    plus ``lengths`` int32 [N] with ``variable_length``.
+
+    A row is ``k * in_features`` values followed by ``k`` labels, the label of step t being the t-th of them; ``k = seq_len``, or
+    ``1 <= k <= seq_len`` with ``variable_length`` (then zero-padded on the right to ``seq_len`` steps, padded labels 0 and never
+    read).  A row that does not split this way, or a label outside ``[0, num_classes)``, is an error naming the row.
+    ``normalize``: global min-max over the real feature values only."""
+    if seq_len < 2 or in_features < 1:
+        raise ValueError("per-step labels need seq_len >= 2 and in_features >= 1")
+    xs, ys, ls = [], [], []
+    for n, row in enumerate(train_xy):
+        if len(row) <= 1:
+            continue
+        k, rem = divmod(len(row), in_features + 1)
+        if rem or not (k == seq_len or (variable_length and 1 <= k <= seq_len)):
+            want = f"1..{seq_len}" if variable_length else f"{seq_len}"
+            raise ValueError(f"row {n}: {len(row)} fields is not {want} steps of {in_features} features followed by one "
+                             "label per step")
+        lab = [int(float(v)) for v in row[k * in_features:]]
+        bad = [v for v in lab if not 0 <= v < num_classes]
+        if bad:
+            raise ValueError(f"row {n}: label {bad[0]} outside [0, {num_classes})")
+        xs.append([float(v) for v in row[:k * in_features]])
+        ys.append(lab)
+        ls.append(k)
+    if not xs:
+        raise ValueError("empty partition: no parsable rows")
+    if normalize:
+        flat = min_max_normalizer(np.concatenate([np.asarray(r, dtype=np.float64) for r in xs]))
+        off = np.cumsum([0] + [len(r) for r in xs])
+        xs = [flat[off[i]:off[i + 1]] for i in range(len(xs))]
+    x = np.zeros((len(xs), seq_len, in_features), dtype=np.float32)
+    y = np.zeros((len(xs), seq_len), dtype=np.int64)
+    for i, r in enumerate(xs):
+        x[i, :ls[i]] = np.asarray(r, dtype=np.float32).reshape(ls[i], in_features)
+        y[i, :ls[i]] = ys[i]
+    if variable_length:
+        return x, y, np.asarray(ls, dtype=np.int32)
+    return x, y
+
+
 def resolve_batch_size(batch_size: int, shard_rows: int) -> int:
     """``--batch_size 0`` = whole shard (reference intent, src/rnn.py:193-199, Q3)."""
     bs = shard_rows if not batch_size else batch_size
@@ -201,6 +244,27 @@ def synthetic_sequences(n: int, seq_len: int, in_features: int, num_classes: int
         raise ValueError("variable-length sequences need seq_len >= 2")
     lengths = synthetic_lengths(n, seq_len, seed)
     x[np.arange(seq_len)[None, :] >= lengths[:, None]] = 0.0
+    return x.astype(dtype), y, lengths
+
+
+def synthetic_per_step(n: int, seq_len: int, in_features: int, num_classes: int, seed: int = 0, dtype=np.float32,
+                       variable_length: bool = False):
+    """A learnable sequence-labelling task (``--per_step_labels``): every step has its own class, and its input is drawn around
+    that class's centre.  -> ``(x [n, T, D], y int64 [n, T])``, plus ``lengths`` with ``variable_length`` (the lengths of
+    ``synthetic_lengths``, padded steps zeroed and labelled 0).  Drawn by a generator of its own: the draws of
+    ``synthetic_sequences`` are untouched."""
+    if seq_len < 2:
+        raise ValueError("per-step labels need seq_len >= 2")
+    rng = np.random.default_rng([seed, 0x737465])
+    centers = rng.standard_normal((num_classes, in_features)).astype(np.float32)
+    y = rng.integers(0, num_classes, size=(n, seq_len)).astype(np.int64)
+    x = rng.standard_normal((n, seq_len, in_features), dtype=np.float32) * 0.5 + centers[y]
+    if not variable_length:
+        return x.astype(dtype), y
+    lengths = synthetic_lengths(n, seq_len, seed)
+    pad = np.arange(seq_len)[None, :] >= lengths[:, None]
+    x[pad] = 0.0
+    y[pad] = 0
     return x.astype(dtype), y, lengths
 
 
@@ -301,8 +365,9 @@ class PinnedHostLoader:
             if self.l_host is not None:
                 self.l_host = self.l_host.pin_memory()
         shape_x = (self.batch_size,) + tuple(self.x_host.shape[1:])
+        shape_y = (self.batch_size,) + tuple(self.y_host.shape[1:])          # [B], or [B,T] with a label per step
         self.dev = [(torch.empty(shape_x, dtype=dtype, device=self.device),
-                     torch.empty((self.batch_size,), dtype=torch.int64, device=self.device))
+                     torch.empty(shape_y, dtype=torch.int64, device=self.device))
                     + (() if self.l_host is None else (torch.empty((self.batch_size,), dtype=torch.int32, device=self.device),))
                     for _ in range(depth)]
         self._slot = 0
@@ -319,7 +384,7 @@ class PinnedHostLoader:
         if not shuffle:
             self._pass_start[1] = (self.gen.get_state(), self._order.clone())
         self._consumed = (self._pass, 0)
-        self.bytes_per_batch = self.dev[0][0].numel() * self.dev[0][0].element_size() + self.batch_size * 8 \
+        self.bytes_per_batch = self.dev[0][0].numel() * self.dev[0][0].element_size() + self.dev[0][1].numel() * 8 \
             + (0 if self.l_host is None else self.batch_size * 4)
 
     def _reshuffle(self):

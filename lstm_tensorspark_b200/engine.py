@@ -274,10 +274,14 @@ class TrainEngine:
 
     @torch.no_grad()
     def evaluate(self, x: torch.Tensor, y: torch.Tensor, lengths: Optional[torch.Tensor] = None):
-        """Loss and accuracy of a batch with the model in eval mode (no dropout)."""
+        """Loss and accuracy of a batch with the model in eval mode (no dropout); ``--per_step_labels``: over the counted
+        positions of ``y [B,T]``."""
         was_training = self.model.training
         self.model.eval()
         try:
+            if self.model.per_step:
+                loss, correct, n = self.model.score_per_step(x, y, lengths)
+                return loss, correct.float() / n.float()
             h = self.model.features(x, lengths)
             logits = self.model.head(h)
         finally:

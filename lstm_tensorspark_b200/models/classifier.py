@@ -75,11 +75,44 @@ class SequenceClassifier(nn.Module):
         self.rnn.reset_state(x.shape[0])
         return self.rnn.fit_layers(x.to(self.compute_dtype) if x.is_floating_point() else x, lengths=lengths)
 
+    def check_labels(self, labels: torch.Tensor) -> None:
+        """``[B]`` labels classify whole sequences, ``[B,T]`` label every step (``--per_step_labels``): the wrong one is an error."""
+        if self.per_step and labels.dim() != 2:
+            raise ValueError(f"--per_step_labels needs labels [B,T], got {tuple(labels.shape)}")
+        if not self.per_step and labels.dim() == 2 and labels.shape[1] > 1:
+            raise ValueError(f"labels {tuple(labels.shape)} of one class per step need --per_step_labels; without it they are [B]")
+
+    @property
+    def per_step(self) -> bool:
+        return bool(getattr(self.cfg, "per_step_labels", False))
+
+    def sequence_features(self, x: torch.Tensor, lengths: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """The top layer's whole output ``[T,B,H_last]`` (bidirectional ``[T,B,2 H_last]``) of ``x [B,T,D]``."""
+        if x.dim() != 3:
+            raise ValueError(f"--per_step_labels needs sequences [B,T,D], got {tuple(x.shape)}")
+        self.rnn.reset_state(x.shape[0])
+        return self.rnn.fit_sequence_all(x.to(self.compute_dtype) if x.is_floating_point() else x, lengths=lengths)
+
     def forward(self, x: torch.Tensor, labels: torch.Tensor, lengths: Optional[torch.Tensor] = None):
-        """-> (loss, logits, correct_count)"""
+        """-> (loss, logits, correct_count); with ``--per_step_labels`` logits are ``[B,T,C]`` and the loss and the count run over
+        the counted positions (``ops.reference.head_xent_per_step``)."""
+        self.check_labels(labels)
+        if self.per_step:
+            h_seq = self.sequence_features(x, lengths)
+            logits, loss, correct, _n = F.head_xent_per_step(h_seq, self.head.weights, self.head.bias, labels, lengths)
+            return loss, logits, correct
         h = self.features(x, lengths)
         logits, loss, correct = F.head_xent(h, self.head.weights, self.head.bias, labels)
         return loss, logits, correct
+
+    def score_per_step(self, x: torch.Tensor, labels: torch.Tensor, lengths: Optional[torch.Tensor] = None):
+        """Per-step evaluation without gradients (call in eval mode): -> (mean loss, correct count, N) over the counted
+        positions, device tensors (no host sync)."""
+        self.check_labels(labels)
+        with torch.no_grad():
+            h_seq = self.sequence_features(x, lengths)
+            _logits, loss, correct, n = F.head_xent_per_step(h_seq, self.head.weights, self.head.bias, labels, lengths)
+        return loss, correct, n
 
     # ---- reference variable naming ------------------------------------------------
     def named_reference_variables(self) -> List[Tuple[str, torch.Tensor]]:

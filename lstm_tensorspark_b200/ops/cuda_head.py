@@ -56,3 +56,57 @@ class _HeadXentFn(torch.autograd.Function):
 
 def head_xent(h, weights, bias, labels):
     return _HeadXentFn.apply(h, weights, bias, labels)
+
+
+class _HeadXentStepFn(torch.autograd.Function):
+    """The head at every time step of ``h_seq [T,B,H]`` (read in place as ``T·B`` time-major rows): one forward launch (logits,
+    loss over the counted positions, correct count, N, dlogits) and one backward launch (dh_seq, dW, db).  N stays on the
+    device, so a captured graph holds across batches with different lengths."""
+
+    @staticmethod
+    def forward(ctx, h_seq, weights, bias, labels, lengths):
+        from .cuda_lstm import STATS
+        E = ext()
+        T, B, H = h_seq.shape
+        hc = h_seq.detach()
+        if hc.dtype not in (torch.bfloat16, torch.float32):
+            hc = hc.float()
+        h2 = hc.reshape(T * B, H) if hc.is_contiguous() else hc.contiguous().view(T * B, H)
+        w = weights.detach().float().contiguous()
+        b = bias.detach().float().contiguous()
+        lab = labels.long().contiguous()
+        ln = None if lengths is None else lengths.contiguous()
+        logits, dlogits, loss, correct, count, used_tc = E.head_step_fwd(h2, w, b, lab, ln, T)
+        STATS["head_per_step"] = STATS.get("head_per_step", 0) + 1
+        if int(used_tc[0]):
+            STATS["head_per_step_tc"] = STATS.get("head_per_step_tc", 0) + 1
+        ctx.save_for_backward(h2, w, dlogits)
+        ctx.shape, ctx.h_dtype = (T, B, H), h_seq.dtype
+        ctx.addrs = (weights.data_ptr(), bias.data_ptr())
+        ctx.mark_non_differentiable(logits, correct, count)
+        return logits, loss.squeeze(0), correct.squeeze(0), count.squeeze(0)
+
+    @staticmethod
+    def backward(ctx, _dlogits_unused, dloss, _dcorrect_unused, _dcount_unused):
+        from .cuda_lstm import grad_sink
+        E = ext()
+        h2, w, dlogits = ctx.saved_tensors
+        sw, sb = grad_sink(ctx.addrs[0]), grad_sink(ctx.addrs[1])
+        dl = dloss.detach().float().reshape(1).contiguous()
+        dw = db = None
+        if sw is not None and sb is not None:
+            if sw[1] != sb[1]:                             # one of the two already holds a gradient: bring both to "accumulate"
+                if not sw[1]:
+                    sw[0].zero_()
+                if not sb[1]:
+                    sb[0].zero_()
+            dh = E.head_step_bwd(h2, w, dlogits, dl, sw[0], sb[0], bool(sw[1] or sb[1]))
+        else:
+            dw = torch.empty_like(w)
+            db = torch.empty(w.shape[1], dtype=torch.float32, device=w.device)
+            dh = E.head_step_bwd(h2, w, dlogits, dl, dw, db, False)
+        return dh.view(ctx.shape).to(ctx.h_dtype), dw, db, None, None
+
+
+def head_xent_per_step(h_seq, weights, bias, labels, lengths=None):
+    return _HeadXentStepFn.apply(h_seq, weights, bias, labels, lengths)

@@ -68,6 +68,15 @@ def head_xent(h, weights, bias, labels):
     return ref.head_xent(h, weights, bias, labels)
 
 
+def head_xent_per_step(h_seq, weights, bias, labels, lengths=None):
+    """The head at every time step: ``h_seq [T,B,H]``, ``labels`` int64 ``[B,T]``, ``lengths`` optional int32 ``[B]`` ->
+    (logits ``[B,T,C]`` fp32, mean loss over the counted positions, correct count, N = number of counted positions)."""
+    if _use_ext(h_seq):
+        from . import cuda_head
+        return cuda_head.head_xent_per_step(h_seq, weights, bias, labels, lengths)
+    return ref.head_xent_per_step(h_seq, weights, bias, labels, lengths)
+
+
 def lstm_pair_supported(x_seq, h_a: int, h_b: int) -> bool:
     """Can two stacked layers run as one pair op on the GPU (layer wavefront or pipelined, ``cuda_lstm.pair_schedule``)?"""
     if not x_seq.is_cuda or _BACKEND == "torch":

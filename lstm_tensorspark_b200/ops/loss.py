@@ -13,7 +13,11 @@ from ..utils import metrics as _metrics
 
 
 def compute_loss(labels, logits, sparse: bool = True):
-    xent = ref.softmax_xent(logits, labels, sparse=sparse)
+    return report_loss(ref.softmax_xent(logits, labels, sparse=sparse))
+
+
+def report_loss(xent):
+    """The reference's loss scalars for an already computed mean cross-entropy (also the per-step head's)."""
     _metrics.scalar("cross_entropy", xent)
     from ..models.recurrent.lstm import weight_decay_terms
     wd = weight_decay_terms()
@@ -27,6 +31,9 @@ def compute_loss(labels, logits, sparse: bool = True):
 
 
 def compute_accuracy(labels, logits, sparse: bool = True):
-    acc = ref.accuracy(logits, labels, sparse=sparse)
+    return report_accuracy(ref.accuracy(logits, labels, sparse=sparse))
+
+
+def report_accuracy(acc):
     _metrics.scalar("accuracy", acc)
     return acc

@@ -222,6 +222,35 @@ def head_xent(h, weights, bias, labels):
     return logits, loss, correct
 
 
+def step_mask(lengths: Optional[torch.Tensor], B: int, T: int, device=None) -> torch.Tensor:
+    """``[B,T]`` bool: position (b, t) counts iff ``t < lengths[b]`` (every position without lengths)."""
+    if lengths is None:
+        return torch.ones(B, T, dtype=torch.bool, device=device)
+    return lengths.to(device).long().view(B, 1) > torch.arange(T, device=device).view(1, T)
+
+
+def head_xent_per_step(h_seq, weights, bias, labels, lengths=None):
+    """The head at every time step (sequence labelling): ``h_seq [T,B,H]``, ``labels`` int64 ``[B,T]`` -> (logits ``[B,T,C]``,
+    loss, correct, N).  Only counted positions (``step_mask``) enter the loss and the accuracy, and their labels alone are
+    read; loss = the summed NLL / N, N = the number of counted positions: ``F.cross_entropy`` over the packed outputs."""
+    T, B, _ = h_seq.shape
+    dt = torch.float64 if h_seq.dtype == torch.float64 else torch.float32
+    logits = dense_head(h_seq.to(dt), weights.to(dt), bias.to(dt)).transpose(0, 1)         # [B,T,C]
+    keep = step_mask(lengths, B, T, device=h_seq.device)
+    lg, lab = logits[keep], labels.to(h_seq.device)[keep].long()
+    loss = torch.nn.functional.cross_entropy(lg, lab, reduction="sum") / keep.sum()
+    correct = (lg.argmax(1) == lab).sum()
+    return logits, loss, correct, keep.sum()
+
+
+def softmax_xent_per_step(logits, labels, lengths=None):
+    """``logits [B,T,C]``, ``labels [B,T]`` -> (mean NLL over counted positions, accuracy over them, N)."""
+    keep = step_mask(lengths, logits.shape[0], logits.shape[1], device=logits.device)
+    lg, lab = logits[keep].float(), labels.to(logits.device)[keep].long()
+    n = keep.sum()
+    return (torch.nn.functional.cross_entropy(lg, lab, reduction="sum") / n, (lg.argmax(1) == lab).float().sum() / n, n)
+
+
 def adam_step_(p, g, m, v, step: int, lr: float, beta1: float = 0.9, beta2: float = 0.999,
                eps: float = 1e-8, weight_decay: float = 0.0, grad_scale: float = 1.0):
     """TF-1.0 Adam ("epsilon-hat"): lr_t = lr*sqrt(1-b2^t)/(1-b1^t); w -= lr_t*m/(sqrt(v)+eps)."""

@@ -26,7 +26,7 @@ from .config import Config
 from .models.classifier import SequenceClassifier
 from .models.recurrent.lstm import clear_weight_decay_collection
 from .ops import functional as F
-from .ops.loss import compute_accuracy, compute_loss
+from .ops.loss import compute_accuracy, compute_loss, report_accuracy, report_loss
 from .ops.optim import FlatOptimizer
 from .parallel.comm import Communicator, make_communicator
 from .utils import checkpoint as ckpt
@@ -108,6 +108,11 @@ def train_rnn(partition, cfg: Config, rank: int = 0, world_size: int = 1, comm: 
     if isinstance(rows, tuple):
         train_x, train_y = rows[0], rows[1]
         train_lengths = rows[2] if len(rows) > 2 else None
+    elif cfg.per_step_labels:
+        parsed = D.process_batch_per_step(rows, cfg.seq_len, cfg.in_features, cfg.num_classes,
+                                          variable_length=cfg.variable_length, normalize=cfg.normalize)
+        train_x, train_y = parsed[0], parsed[1]
+        train_lengths = parsed[2] if cfg.variable_length else None
     elif cfg.variable_length:
         train_x, train_y, train_lengths = D.process_batch_ragged(rows, cfg.seq_len, cfg.in_features, normalize=cfg.normalize)
     else:
@@ -231,10 +236,15 @@ def train_rnn(partition, cfg: Config, rank: int = 0, world_size: int = 1, comm: 
                            opt_state={"optimizer": comm.optimizer_state(optimizer), "loader": loader.state_dict()})
                 model.eval()                                         # no dropout while scoring
                 with torch.no_grad(), M.capture(sink):
-                    h = model.features(train_input, batch_lengths)   # same batch, from the initial state (src/rnn.py:276-279)
-                    logits = model.head(h)
-                    e_loss = compute_loss(labels=train_labels, logits=logits)
-                    e_acc = compute_accuracy(labels=train_labels, logits=logits)
+                    if model.per_step:                               # over the counted positions of the batch
+                        xent, ok, n = model.score_per_step(train_input, train_labels, batch_lengths)
+                        e_loss = report_loss(xent)
+                        e_acc = report_accuracy(ok.float() / n.float())
+                    else:
+                        h = model.features(train_input, batch_lengths)   # same batch, from the initial state (src/rnn.py:276-279)
+                        logits = model.head(h)
+                        e_loss = compute_loss(labels=train_labels, logits=logits)
+                        e_acc = compute_accuracy(labels=train_labels, logits=logits)
                 model.train()
                 t_loss, t_acc = float(e_loss.item()), float(e_acc.item())
                 sink.flush(step)
@@ -345,6 +355,10 @@ def load_shards(cfg: Config, world_size: int, standalone: bool):
         n_per = cfg.synthetic // world_size
         shards = []
         for r in range(world_size):
+            if cfg.per_step_labels:
+                shards.append((r, D.synthetic_per_step(n_per, cfg.seq_len, cfg.in_features, cfg.num_classes, seed=cfg.seed + r,
+                                                       variable_length=cfg.variable_length)))
+                continue
             shards.append((r, D.synthetic_sequences(n_per, cfg.seq_len, cfg.in_features, cfg.num_classes, seed=cfg.seed + r,
                                                     variable_length=cfg.variable_length)))
         return shards
@@ -382,7 +396,17 @@ def evaluate_job(cfg: Config, standalone: bool = False) -> Dict:
     from .engine import TrainEngine
     variables, src = _find_trained_model(cfg, standalone)
     lengths = None
-    if cfg.synthetic:
+    if cfg.synthetic and cfg.per_step_labels:
+        data = D.synthetic_per_step(cfg.synthetic, cfg.seq_len, cfg.in_features, cfg.num_classes, seed=cfg.seed,
+                                    variable_length=cfg.variable_length)
+        x, y = data[0], data[1]
+        lengths = data[2] if cfg.variable_length else None
+    elif cfg.per_step_labels:
+        data = D.process_batch_per_step(D.read_dataset_from_path(cfg.training_path), cfg.seq_len, cfg.in_features,
+                                        cfg.num_classes, variable_length=cfg.variable_length, normalize=cfg.normalize)
+        x, y = data[0], data[1]
+        lengths = data[2] if cfg.variable_length else None
+    elif cfg.synthetic:
         data = D.synthetic_sequences(cfg.synthetic, cfg.seq_len, cfg.in_features, cfg.num_classes, seed=cfg.seed,
                                      variable_length=cfg.variable_length)
         x, y = data[0], data[1]
@@ -415,6 +439,8 @@ def evaluate_job(cfg: Config, standalone: bool = False) -> Dict:
     ys = torch.as_tensor(y).to(device)
     ls = None if lengths is None else torch.as_tensor(lengths).to(device=device, dtype=torch.int32)
     sl = lambda a, b: None if ls is None else ls[a:b]
+    if eng.model.per_step:
+        return _evaluate_per_step(cfg, eng, src, xs, ys, ls, bs)
     loss_sum, correct, seen = 0.0, 0.0, 0
     start = time.time()
     for lo in range(0, n - bs + 1, bs):                 # full batches (static shapes for the kernels); the tail is scored below
@@ -432,6 +458,36 @@ def evaluate_job(cfg: Config, standalone: bool = False) -> Dict:
            "seconds": time.time() - start}
     if not cfg.quiet:
         print("RNN-LSTM - eval: model {model}, {samples} samples, loss {loss:.6f}, accuracy {accuracy:.4f}".format(**out))
+    if cfg.json_log:
+        jl = M.JsonLog(cfg.json_log); jl.write(**out); jl.close()
+    return out
+
+
+def _evaluate_per_step(cfg: Config, eng, src: str, xs, ys, ls, bs: int) -> Dict:
+    """``--mode eval`` with ``--per_step_labels``: loss and accuracy over every counted position of the file, each batch weighted
+    by its number of positions.  The tail runs as the last ``bs`` rows (static shapes for the kernels), of which only the rows
+    not seen yet are scored."""
+    n = xs.shape[0]
+    sl = lambda a, b: None if ls is None else ls[a:b]
+    loss_sum, correct, positions = 0.0, 0.0, 0
+    start = time.time()
+    seen = 0
+    for lo in range(0, n - bs + 1, bs):
+        loss, ok, cnt = eng.model.score_per_step(xs[lo:lo + bs], ys[lo:lo + bs], sl(lo, lo + bs))
+        loss_sum += float(loss) * int(cnt); correct += float(ok); positions += int(cnt); seen += bs
+    if seen < n:                                        # remainder: score the tail rows alone, in one smaller batch
+        from .ops import reference as ref
+        with torch.no_grad():
+            h_seq = eng.model.sequence_features(xs[n - bs:], sl(n - bs, n))[:, bs - (n - seen):]
+            logits = eng.model.head(h_seq.reshape(-1, h_seq.shape[2])).float().view(h_seq.shape[0], n - seen, -1)
+        loss, acc, cnt = ref.softmax_xent_per_step(logits.transpose(0, 1), ys[seen:], sl(seen, n))
+        loss_sum += float(loss) * int(cnt); correct += float(acc) * int(cnt); positions += int(cnt)
+        seen = n
+    out = {"mode": "eval", "model": src, "samples": seen, "positions": positions, "loss": loss_sum / positions,
+           "accuracy": correct / positions, "seconds": time.time() - start}
+    if not cfg.quiet:
+        print("RNN-LSTM - eval: model {model}, {samples} samples, {positions} positions, loss {loss:.6f}, "
+              "accuracy {accuracy:.4f}".format(**out))
     if cfg.json_log:
         jl = M.JsonLog(cfg.json_log); jl.write(**out); jl.close()
     return out
