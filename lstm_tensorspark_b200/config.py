@@ -12,9 +12,14 @@ from __future__ import annotations
 
 import argparse
 import dataclasses
+import math
 import warnings
 from dataclasses import dataclass, field
 from typing import List, Optional, Sequence
+
+
+FUSED_CLIP_ERROR = ("--clip_grad_norm with --sync_mode grad_allreduce needs the norm of the averaged gradient before any update, "
+                    "which --comm fused does not compute (it updates each gradient bucket as soon as it is reduced): use --comm nccl")
 
 
 @dataclass
@@ -66,6 +71,7 @@ class Config:
     init_std: float = 1.0
     normalize: bool = False             # global min-max normalisation (Q11)
     weight_decay: float = 0.0           # L2 term of create_variable (never enabled in the reference)
+    clip_grad_norm: float = 0.0         # >0: clip the gradient by its global norm to this value before the update (0 = off)
     synthetic: int = 0                  # >0: use N synthetic sequences instead of a CSV
     remainder: str = "drop"             # drop | spread : rows beyond floor(N/P)*P (Q2)
     cuda_graph: bool = False
@@ -112,6 +118,10 @@ class Config:
             })
         return settings
 
+    def clips_synced_grads(self) -> bool:
+        """Gradient clipping on the averaged gradient of several replicas (``--sync_mode grad_allreduce``)."""
+        return self.clip_grad_norm > 0 and self.sync_mode == "grad_allreduce" and self.partitions > 1
+
     def params_str(self) -> str:
         """``KEY = value`` per flag, sorted, upper-cased (reference: src/lstm-no-spark.py:33-37)."""
         items = sorted(dataclasses.asdict(self).items())
@@ -139,6 +149,10 @@ class Config:
                           "(it drops the output of every layer but the last)")
         if self.sync_mode not in ("param_avg", "grad_allreduce", "none"):
             raise ValueError(f"unknown --sync_mode {self.sync_mode}")
+        if not (math.isfinite(self.clip_grad_norm) and self.clip_grad_norm >= 0):
+            raise ValueError(f"--clip_grad_norm must be a finite number >= 0 (0 = off), got {self.clip_grad_norm}")
+        if self.clips_synced_grads() and self.comm == "fused":
+            raise ValueError(FUSED_CLIP_ERROR)
         if self.optimizer not in ("adam", "sgd"):
             raise ValueError(f"unknown --optimizer {self.optimizer}")
         if self.average_scope not in ("lstm", "all"):
@@ -182,6 +196,9 @@ _HELP = {
     "output_path": "Path for store network state",
     "mode": "Execution mode",
     "checkpoint_path": "Directory where to save network model and logs",
+    "clip_grad_norm": "Clip the gradient by its global L2 norm to this value before the update, as "
+                      "torch.nn.utils.clip_grad_norm_ (0 = off); the norm includes the --weight_decay term and, with "
+                      "--sync_mode grad_allreduce, is that of the averaged gradient (--comm nccl or gloo)",
     "per_step_labels": "Label every time step (sequence labelling): labels [B,T], loss and accuracy over the real positions; "
                        "a CSV row is k*in_features values followed by k labels",
 }

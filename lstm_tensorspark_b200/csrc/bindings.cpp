@@ -27,8 +27,10 @@ int ts_lstm_pointwise_bwd(const void*, const float*, const float*, const void*, 
                           float*, int, int, int, cudaStream_t, const int*, int, float*);
 int ts_xent_rows(const float*, const long long*, float*, float*, int*, int, int, cudaStream_t);
 int ts_flat_adam(float*, const float*, float*, float*, void*, long long, float, float, float, float, float, float,
-                 cudaStream_t, int*, long long);
-int ts_flat_sgd(float*, const float*, void*, long long, float, float, float, cudaStream_t, long long);
+                 cudaStream_t, int*, long long, const float*);
+int ts_flat_sgd(float*, const float*, void*, long long, float, float, float, cudaStream_t, long long, const float*);
+long long ts_flat_grad_norm_scratch(long long);
+int ts_flat_grad_norm(const float*, const float*, long long, float, float, long long, float, double*, float*, cudaStream_t);
 int ts_cast_bf16(const float*, void*, long long, cudaStream_t);
 int ts_fused_allreduce(const unsigned long long*, unsigned long long, unsigned long long, unsigned long long, float*,
                        float*, unsigned int*, int*, long long, int, int, int, int, int, int, float, float, float, float,
@@ -353,21 +355,44 @@ Tensor head_step_bwd(const Tensor& h, const Tensor& W, const Tensor& dlogits, co
 }
 
 // ---- optimizer ----------------------------------------------------------------------------------------------
+// clip: the fp32 [2] {norm, coef} flat_grad_norm wrote on this stream; the update then uses coef * g_total.
+const float* clip_ptr(const std::optional<Tensor>& clip, const Tensor& p) {
+  if (!clip.has_value()) return nullptr;
+  TORCH_CHECK(clip->is_cuda() && clip->device() == p.device() && clip->scalar_type() == torch::kFloat32 && clip->numel() == 2 &&
+              clip->is_contiguous(), "clip must be a contiguous fp32 [2] tensor on p's device (flat_grad_norm's out)");
+  return clip->data_ptr<float>();
+}
 void flat_adam(Tensor p, const Tensor& g, Tensor m, Tensor v, std::optional<Tensor> shadow, double lr_t, double b1,
-               double b2, double eps, double wd, double gscale, std::optional<Tensor> step_dev, int64_t wd_numel) {
+               double b2, double eps, double wd, double gscale, std::optional<Tensor> step_dev, int64_t wd_numel,
+               std::optional<Tensor> clip) {
   chk_cuda(p, "p"); chk_cuda(g, "g"); chk_cuda(m, "m"); chk_cuda(v, "v");
   c10::cuda::CUDAGuard gd(p.device());
   TORCH_CHECK(p.numel() == g.numel() && p.numel() == m.numel() && p.numel() == v.numel(), "numel mismatch");
   check(ts_flat_adam(p.data_ptr<float>(), g.data_ptr<float>(), m.data_ptr<float>(), v.data_ptr<float>(),
                      shadow.has_value() ? shadow->data_ptr() : nullptr, p.numel(), lr_t, b1, b2, eps, wd, gscale, stream(),
-                     step_dev.has_value() ? step_dev->data_ptr<int>() : nullptr, (long long)wd_numel),
+                     step_dev.has_value() ? step_dev->data_ptr<int>() : nullptr, (long long)wd_numel, clip_ptr(clip, p)),
         "flat_adam");
 }
-void flat_sgd(Tensor p, const Tensor& g, std::optional<Tensor> shadow, double lr, double wd, double gscale, int64_t wd_numel) {
+void flat_sgd(Tensor p, const Tensor& g, std::optional<Tensor> shadow, double lr, double wd, double gscale, int64_t wd_numel,
+              std::optional<Tensor> clip) {
   chk_cuda(p, "p"); chk_cuda(g, "g");
   c10::cuda::CUDAGuard gd(p.device());
   check(ts_flat_sgd(p.data_ptr<float>(), g.data_ptr<float>(), shadow.has_value() ? shadow->data_ptr() : nullptr,
-                    p.numel(), lr, wd, gscale, stream(), (long long)wd_numel), "flat_sgd");
+                    p.numel(), lr, wd, gscale, stream(), (long long)wd_numel, clip_ptr(clip, p)), "flat_sgd");
+}
+// out = {||g_total||_2, min(max_norm / (norm + 1e-6), 1)} with g_total = g * gscale + wd * p over [0, wd_numel) (-1: all) and
+// g * gscale beyond; scratch: float64 [flat_grad_norm_scratch(n)], zeroed before its first use (each call leaves its ticket 0).
+void flat_grad_norm(const Tensor& g, const Tensor& p, Tensor out, Tensor scratch, double max_norm, double wd, double gscale,
+                    int64_t wd_numel) {
+  chk_cuda(g, "g"); chk_cuda(p, "p"); chk_cuda(out, "out"); chk_cuda(scratch, "scratch");
+  c10::cuda::CUDAGuard gd(g.device());
+  TORCH_CHECK(g.scalar_type() == torch::kFloat32 && p.scalar_type() == torch::kFloat32 && p.numel() == g.numel(), "flat_grad_norm: g, p fp32 of one size");
+  TORCH_CHECK(out.scalar_type() == torch::kFloat32 && out.numel() == 2, "flat_grad_norm: out fp32 [2]");
+  TORCH_CHECK(scratch.scalar_type() == torch::kFloat64 && scratch.numel() >= ts_flat_grad_norm_scratch(g.numel()),
+              "flat_grad_norm: scratch float64 [flat_grad_norm_scratch(n)]");
+  TORCH_CHECK(p.device() == g.device() && out.device() == g.device() && scratch.device() == g.device(), "flat_grad_norm: one device");
+  check(ts_flat_grad_norm(g.data_ptr<float>(), p.data_ptr<float>(), g.numel(), wd, gscale, (long long)wd_numel, max_norm,
+                          scratch.data_ptr<double>(), out.data_ptr<float>(), stream()), "flat_grad_norm");
 }
 void cast_bf16(const Tensor& p, Tensor shadow) {
   chk_cuda(p, "p"); chk_cuda(shadow, "shadow");
@@ -617,9 +642,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("accumulate") = false);
   m.def("flat_adam", &flat_adam, py::arg("p"), py::arg("g"), py::arg("m"), py::arg("v"), py::arg("shadow"), py::arg("lr_t"),
         py::arg("b1"), py::arg("b2"), py::arg("eps"), py::arg("wd"), py::arg("gscale"), py::arg("step_dev") = py::none(),
-        py::arg("wd_numel") = -1);
+        py::arg("wd_numel") = -1, py::arg("clip") = py::none());
   m.def("flat_sgd", &flat_sgd, py::arg("p"), py::arg("g"), py::arg("shadow"), py::arg("lr"), py::arg("wd"), py::arg("gscale"),
-        py::arg("wd_numel") = -1);
+        py::arg("wd_numel") = -1, py::arg("clip") = py::none());
+  m.def("flat_grad_norm", &flat_grad_norm, py::arg("g"), py::arg("p"), py::arg("out"), py::arg("scratch"), py::arg("max_norm"),
+        py::arg("wd") = 0.0, py::arg("gscale") = 1.0, py::arg("wd_numel") = -1);
+  m.def("flat_grad_norm_scratch", [](int64_t n) { return ts_flat_grad_norm_scratch((long long)n); });
   m.def("cast_bf16", &cast_bf16);
   m.def("fused_allreduce", &fused_allreduce, py::arg("ptrs"), py::arg("mc_in"), py::arg("mc_param"), py::arg("mc_shadow"), py::arg("m"),
         py::arg("v"), py::arg("epochs"), py::arg("err"), py::arg("n"), py::arg("rank"), py::arg("world"), py::arg("mode"),

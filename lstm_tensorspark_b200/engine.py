@@ -5,6 +5,7 @@ This is what ``bench.py``, ``__graft_entry__.smoke`` and the per-replica trainer
     eng = TrainEngine(cfg, rank, world_size, comm, batch_size=B)
     loss = eng.step(x, y)            # forward, backward, (fused allreduce +) optimizer update
     loss = eng.step(x, y, lengths)   # variable-length batch: int32 [B] per-sample lengths, x right-padded
+    norm = eng.grad_norm()           # --clip_grad_norm: the last step's gradient norm before clipping (None without)
 
 One step replaces the reference's ``sess.run([train_op, loss], feed_dict=...)`` (original src/rnn.py:264-267):
 H2D feed, forward, backward, 14·L+2 ApplyAdam launches, D2H loss.  With ``cuda_graph=True`` the whole step is
@@ -16,7 +17,7 @@ from typing import Optional
 
 import torch
 
-from .config import Config
+from .config import FUSED_CLIP_ERROR, Config
 from .models.classifier import SequenceClassifier
 from .models.recurrent.lstm import clear_weight_decay_collection, weight_decay_collection
 from .ops import functional as F
@@ -69,6 +70,9 @@ class TrainEngine:
         self._wd_in_kernel = [(v, fn, wd) for (v, fn, wd) in weight_decay_collection() if id(v) in seg_ids]
         self._wd_autograd = [(v, fn, wd) for (v, fn, wd) in weight_decay_collection() if id(v) not in seg_ids]
         self.sync_grads = cfg.sync_mode == "grad_allreduce" and world_size > 1
+        self.optimizer.clip_norm = float(cfg.clip_grad_norm or 0.0)
+        if self.optimizer.clip_norm > 0 and self.sync_grads and getattr(self.comm, "name", "") == "fused":
+            raise ValueError(FUSED_CLIP_ERROR)
         self._bucket_plan = self._make_bucket_plan() if (self.sync_grads and hasattr(self.comm, "launch_bucket")
                                                          and cfg.grad_buckets) else None
         self._graph = None
@@ -204,6 +208,13 @@ class TrainEngine:
         g.replay()
         self.optimizer.step_count += 1          # host mirror; the kernels use the device-resident counter
         return sloss
+
+    def grad_norm(self) -> Optional[torch.Tensor]:
+        """``--clip_grad_norm``: the global norm of the last step's gradient before clipping (a 0-dim fp32 tensor on the
+        engine's device; read it without a host sync until you need the value), else None."""
+        if self.optimizer.clip_norm <= 0:
+            return None
+        return self.optimizer.clip_out[0].clone()
 
     def graph_inputs(self):
         """(x, y, lengths) input buffers of the captured graph (lengths None when captured without), or None: a loader that

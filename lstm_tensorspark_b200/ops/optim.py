@@ -25,6 +25,9 @@ class FlatOptimizer:
         self.kind = kind
         self.lr, self.beta1, self.beta2, self.eps, self.weight_decay = lr, beta1, beta2, eps, weight_decay
         self.wd_numel = -1          # weight decay covers flat elements [0, wd_numel); -1 = all (K12: the LSTM variables only)
+        self.clip_out = None        # clipping: {norm, coef} of the last step (fp32 [2], on the flat buffer's device)
+        self.clip_scratch = None    # the norm kernel's fp64 CTA partials and ticket (allocated by its first launch)
+        self.clip_norm = 0.0
         self.step_count = 0
         # device-resident mirror of step_count: the Adam kernels derive the bias correction from it, so a captured
         # CUDA graph of the training step stays exact across replays
@@ -36,6 +39,19 @@ class FlatOptimizer:
             self.m = self.v = None
         else:
             raise ValueError(f"unknown optimizer {kind!r}")
+
+    @property
+    def clip_norm(self) -> float:
+        """Clip the gradient by its global norm to this value before the update (0 = off).  The norm is that of the gradient
+        the update uses - ``g * grad_scale`` plus the weight-decay term over ``[0, wd_numel)`` - and the update uses
+        ``coef * g`` with ``coef = min(clip_norm / (norm + 1e-6), 1)``; ``clip_out`` holds {norm, coef} of the last step."""
+        return self._clip_norm
+
+    @clip_norm.setter
+    def clip_norm(self, value: float):
+        self._clip_norm = float(value)
+        if self._clip_norm > 0 and self.clip_out is None:
+            self.clip_out = torch.zeros(2, dtype=torch.float32, device=self.flat.data.device)
 
     def minimize(self, loss: torch.Tensor):
         """``optimizer.minimize(loss)`` of the reference: backward + apply."""
@@ -53,14 +69,19 @@ class FlatOptimizer:
         with torch.no_grad():
             n = fl.data.numel()
             cut = n if (self.wd_numel < 0 or not self.weight_decay) else min(self.wd_numel, n)
-            for lo, hi, wd in ((0, cut, self.weight_decay), (cut, n, 0.0)):
-                if hi <= lo:
-                    continue
+            segs = [(lo, hi, wd) for lo, hi, wd in ((0, cut, self.weight_decay), (cut, n, 0.0)) if hi > lo]
+            coef = None
+            if self.clip_norm > 0:
+                g_total = [fl.grad[lo:hi] * grad_scale + wd * fl.data[lo:hi] if wd else fl.grad[lo:hi] * grad_scale
+                           for lo, hi, wd in segs]
+                norm, coef = ref.clip_coefficient(g_total, self.clip_norm)
+                self.clip_out[0], self.clip_out[1] = norm, coef
+            for lo, hi, wd in segs:
                 if self.kind == "adam":
                     ref.adam_step_(fl.data[lo:hi], fl.grad[lo:hi], self.m[lo:hi], self.v[lo:hi], self.step_count, self.lr,
-                                   self.beta1, self.beta2, self.eps, wd, grad_scale)
+                                   self.beta1, self.beta2, self.eps, wd, grad_scale, coef)
                 else:
-                    ref.sgd_step_(fl.data[lo:hi], fl.grad[lo:hi], self.lr, wd, grad_scale)
+                    ref.sgd_step_(fl.data[lo:hi], fl.grad[lo:hi], self.lr, wd, grad_scale, coef)
             fl.refresh_shadow()
 
     def bias_corrected_lr(self, step: Optional[int] = None) -> float:

@@ -251,12 +251,27 @@ def softmax_xent_per_step(logits, labels, lengths=None):
     return (torch.nn.functional.cross_entropy(lg, lab, reduction="sum") / n, (lg.argmax(1) == lab).float().sum() / n, n)
 
 
+def clip_coefficient(g_total_segments, max_norm: float):
+    """Clipping by the global norm (``torch.nn.utils.clip_grad_norm_``): ``norm = ||g_total||_2`` over all segments, summed in
+    fp64 and rounded to the segments' dtype, and ``coef = min(max_norm / (norm + 1e-6), 1)`` in that dtype (a NaN norm gives a
+    NaN coef, an infinite one 0).  -> (norm, coef), 0-dim tensors."""
+    segs = [s.reshape(-1) for s in g_total_segments]
+    dtype = segs[0].dtype
+    sq = sum(s.double().square().sum() for s in segs)
+    norm = sq.sqrt().to(dtype)
+    coef = torch.clamp(max_norm / (norm + 1e-6), max=1.0)
+    return norm, coef
+
+
 def adam_step_(p, g, m, v, step: int, lr: float, beta1: float = 0.9, beta2: float = 0.999,
-               eps: float = 1e-8, weight_decay: float = 0.0, grad_scale: float = 1.0):
-    """TF-1.0 Adam ("epsilon-hat"): lr_t = lr*sqrt(1-b2^t)/(1-b1^t); w -= lr_t*m/(sqrt(v)+eps)."""
+               eps: float = 1e-8, weight_decay: float = 0.0, grad_scale: float = 1.0, clip_coef=None):
+    """TF-1.0 Adam ("epsilon-hat"): lr_t = lr*sqrt(1-b2^t)/(1-b1^t); w -= lr_t*m/(sqrt(v)+eps).  ``clip_coef``: the update
+    uses clip_coef * (g * grad_scale + weight_decay * p)."""
     gg = g * grad_scale if grad_scale != 1.0 else g
     if weight_decay:
         gg = gg + weight_decay * p
+    if clip_coef is not None:
+        gg = gg * clip_coef
     m.mul_(beta1).add_(gg, alpha=1.0 - beta1)
     v.mul_(beta2).addcmul_(gg, gg, value=1.0 - beta2)
     lr_t = lr * (1.0 - beta2 ** step) ** 0.5 / (1.0 - beta1 ** step)
@@ -264,9 +279,11 @@ def adam_step_(p, g, m, v, step: int, lr: float, beta1: float = 0.9, beta2: floa
     return p
 
 
-def sgd_step_(p, g, lr: float, weight_decay: float = 0.0, grad_scale: float = 1.0):
+def sgd_step_(p, g, lr: float, weight_decay: float = 0.0, grad_scale: float = 1.0, clip_coef=None):
     gg = g * grad_scale if grad_scale != 1.0 else g
     if weight_decay:
         gg = gg + weight_decay * p
+    if clip_coef is not None:
+        gg = gg * clip_coef
     p.add_(gg, alpha=-lr)
     return p

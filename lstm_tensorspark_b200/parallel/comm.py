@@ -140,11 +140,21 @@ class TorchDistComm(Communicator):
                 pass
 
 
-def make_communicator(kind: str, rank: int, world_size: int, device: torch.device, timeout_s: float = 600.0) -> Communicator:
+def resolve_comm(kind: str, device: torch.device, clip_synced_grads: bool = False) -> str:
+    """``auto``: the fused NVLink allreduce on GPUs, gloo on the CPU; nccl on GPUs when the gradient is clipped by the norm of
+    the averaged gradient (the fused allreduce updates each gradient bucket before that norm is known)."""
+    if kind != "auto":
+        return kind
+    if device.type != "cuda":
+        return "gloo"
+    return "nccl" if clip_synced_grads else "fused"
+
+
+def make_communicator(kind: str, rank: int, world_size: int, device: torch.device, timeout_s: float = 600.0,
+                      clip_synced_grads: bool = False) -> Communicator:
     if world_size == 1 and kind in ("auto", "gloo", "nccl"):
         return Communicator(0, 1)
-    if kind == "auto":
-        kind = "fused" if device.type == "cuda" else "gloo"
+    kind = resolve_comm(kind, device, clip_synced_grads)
     if kind == "gloo":
         return TorchDistComm(rank, world_size, "gloo", device, timeout_s)
     if kind == "nccl":

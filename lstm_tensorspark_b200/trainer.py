@@ -222,6 +222,7 @@ def train_rnn(partition, cfg: Config, rank: int = 0, world_size: int = 1, comm: 
         is_eval = (step % cfg.evaluate_every == 0) or (step + 1) == max_steps
         if is_eval:
             t_loss = float(loss.detach().float().item())
+            g_norm = float(eng.grad_norm().item()) if cfg.clip_grad_norm > 0 else None
         elif use_bar:
             t_loss = bar_loss.push(loss)         # CUDA: the previous step's loss, read back asynchronously (no host sync)
         if use_bar:
@@ -247,8 +248,12 @@ def train_rnn(partition, cfg: Config, rank: int = 0, world_size: int = 1, comm: 
                         e_acc = compute_accuracy(labels=train_labels, logits=logits)
                 model.train()
                 t_loss, t_acc = float(e_loss.item()), float(e_acc.item())
+                extra = {}
+                if g_norm is not None:                               # the pre-clip norm of this step's gradient
+                    sink.add("grad_norm", g_norm)
+                    extra["grad_norm"] = g_norm
                 sink.flush(step)
-                jlog.write(step=step, loss=t_loss, acc=t_acc, rank=rank)
+                jlog.write(step=step, loss=t_loss, acc=t_acc, rank=rank, **extra)
             if use_bar:
                 total_steps.set_description("Loss: {:.4f} - t_acc {:.3f}".format(t_loss, t_acc))
 
@@ -286,7 +291,7 @@ def train_rnn(partition, cfg: Config, rank: int = 0, world_size: int = 1, comm: 
 # ====================================================================================================
 def _rank_main(rank: int, world_size: int, cfg: Config, shards, standalone: bool):
     device = resolve_device(cfg, rank)
-    comm = make_communicator(cfg.comm, rank, world_size, device, cfg.timeout_s)
+    comm = make_communicator(cfg.comm, rank, world_size, device, cfg.timeout_s, clip_synced_grads=cfg.clips_synced_grads())
     try:
         stamp = comm.broadcast_object(str(time.time()), src=0)
         mine = list(shards[rank::world_size]) if shards is not None else [None]
