@@ -27,20 +27,42 @@ import torch.nn.functional as F
 
 
 class CudnnLSTMClassifier(nn.Module):
-    def __init__(self, hidden, in_features, num_classes, time_major=False, bidirectional=False, dropout=0.0, per_step=False):
+    def __init__(self, hidden, in_features, num_classes, time_major=False, bidirectional=False, dropout=0.0, per_step=False,
+                 pooling="last", attention_units=128):
         super().__init__()
         self.per_step = per_step
+        self.pooling = pooling
         assert len(set(hidden)) == 1, "nn.LSTM stacks equal-width layers"
         self.time_major = time_major
         self.bidirectional = bidirectional
         self.lstm = nn.LSTM(in_features, hidden[0], num_layers=len(hidden), batch_first=not time_major, bidirectional=bidirectional,
                             dropout=dropout)
         self.head = nn.Linear(hidden[-1] * (2 if bidirectional else 1), num_classes)
+        if pooling == "attention":                      # u_t = tanh(W_a h_t + b_a), e_t = u_t . v
+            self.att = nn.Linear(hidden[-1] * (2 if bidirectional else 1), attention_units)
+            self.context = nn.Parameter(torch.randn(attention_units) / attention_units ** 0.5)
 
-    def forward(self, x):
+    def pool(self, out, lengths=None):
+        """``--pooling mean | max | attention`` over the outputs ``out`` (time-major [T,B,H] or batch-major [B,T,H]) at each row's
+        steps t < lengths[b] (every step without lengths)."""
+        seq = out if self.time_major else out.transpose(0, 1)            # [T,B,H]
+        T = seq.shape[0]
+        keep = torch.ones(T, seq.shape[1], dtype=torch.bool, device=seq.device) if lengths is None else \
+            torch.arange(T, device=seq.device).view(T, 1) < lengths.view(1, -1)
+        hm = seq.masked_fill(~keep.unsqueeze(2), 0)
+        if self.pooling == "mean":
+            return hm.sum(0) / keep.sum(0, keepdim=True).t().to(hm.dtype)
+        if self.pooling == "max":
+            return seq.masked_fill(~keep.unsqueeze(2), float("-inf")).max(0).values
+        e = (torch.tanh(self.att(hm)) @ self.context.to(hm.dtype)).masked_fill(~keep, float("-inf"))
+        return (torch.softmax(e.float(), 0).to(hm.dtype).unsqueeze(2) * hm).sum(0)
+
+    def forward(self, x, lengths=None):
         out, (h_n, _) = self.lstm(x)
         if self.per_step:                               # nn.Linear over every output: logits [B,T,C] (time-major: [T,B,C])
             return self.head(out)
+        if self.pooling != "last":
+            return self.head(self.pool(out, lengths))
         if self.bidirectional:                          # [forward final | reverse final (after time 0)], as the framework's model
             return self.head(torch.cat([h_n[-2], h_n[-1]], 1))
         return self.head(out[-1] if self.time_major else out[:, -1, :])
@@ -48,9 +70,10 @@ class CudnnLSTMClassifier(nn.Module):
 
 class BaselineRunner:
     def __init__(self, hidden, in_features, num_classes, batch, seq_len, rank, world, device, optimizer="adam", lr=1e-3,
-                 variant="stock", bidirectional=False, dropout=0.0, per_step=False):
+                 variant="stock", bidirectional=False, dropout=0.0, per_step=False, pooling="last"):
         """``per_step``: sequence labelling - labels ``[B,T]``, the head over every output and the mean cross-entropy over all
-        ``T·B`` positions (default: classify the final state, labels ``[B]``)."""
+        ``T·B`` positions (default: classify the final state, labels ``[B]``).  ``pooling``: classify the mean / max / attention
+        pooling of the top layer's outputs (``nn.LSTM`` + masked pool + ``nn.Linear``); a step then takes ``lengths``."""
         self.rank, self.world, self.device = rank, world, device
         self.B, self.T, self.D, self.C = batch, seq_len, in_features, num_classes
         self.variant = variant
@@ -63,7 +86,7 @@ class BaselineRunner:
         if world > 1 and not dist.is_initialized():
             dist.init_process_group("nccl", rank=rank, world_size=world, device_id=device)
         model = CudnnLSTMClassifier(hidden, in_features, num_classes, time_major=self.tuned, bidirectional=bidirectional,
-                                    dropout=dropout, per_step=per_step).to(device)
+                                    dropout=dropout, per_step=per_step, pooling=pooling).to(device)
         if self.tuned:
             model = model.to(torch.bfloat16)
             model.lstm.flatten_parameters()

@@ -22,6 +22,9 @@ FUSED_CLIP_ERROR = ("--clip_grad_norm with --sync_mode grad_allreduce needs the 
                     "which --comm fused does not compute (it updates each gradient bucket as soon as it is reduced): use --comm nccl")
 
 
+ATTENTION_UNITS_DEFAULT = 128
+
+
 @dataclass
 class Config:
     # ---- reference flags (rnn.py:310-334) -------------------------------------------------------
@@ -54,6 +57,9 @@ class Config:
     per_step_labels: bool = False       # sequence labelling: a label at every time step ([B,T]), the head scores the top layer's
                                         # output at each step (nn.LSTM -> nn.Linear -> cross_entropy over the real positions); a CSV
                                         # row is k*in_features values followed by k labels
+    pooling: str = "last"               # what the classifier reads: last (the top layer's state after each sample's last step) |
+                                        # mean | max | attention over the top layer's outputs at the sample's real steps
+    attention_units: int = ATTENTION_UNITS_DEFAULT  # A of --pooling attention: u_t = tanh(h_t W_a + b_a) [A], score u_t . v
     dtype: str = "auto"                 # auto: bf16 on cuda, fp32 on cpu
     device: str = "auto"                # auto | cpu | cuda
     backend: str = "auto"               # auto | cuda_ext (hand-written sm_90a kernels) | torch
@@ -142,6 +148,18 @@ class Config:
         if self.per_step_labels and self.seq_len < 2:
             raise ValueError("--per_step_labels needs --seq_len >= 2 (one label per time step of a sequence; the one-step [B,D] "
                              "path classifies the last state only)")
+        if self.pooling not in ("last", "mean", "max", "attention"):
+            raise ValueError(f"unknown --pooling {self.pooling!r}: one of last, mean, max, attention")
+        if self.attention_units < 1:
+            raise ValueError(f"--attention_units must be >= 1, got {self.attention_units}")
+        if self.pooling != "last" and self.seq_len < 2:
+            raise ValueError(f"--pooling {self.pooling} needs --seq_len >= 2 (it pools the top layer's outputs over the time steps "
+                             "of a sequence)")
+        if self.pooling != "last" and self.per_step_labels:
+            raise ValueError(f"--pooling {self.pooling} does not combine with --per_step_labels: per-step labels score every "
+                             "step's output, there is nothing to pool (use --pooling last)")
+        if self.attention_units != ATTENTION_UNITS_DEFAULT and self.pooling != "attention":
+            warnings.warn(f"--attention_units {self.attention_units} has no effect without --pooling attention")
         if not 0.0 <= self.dropout < 1.0:
             raise ValueError(f"--dropout must satisfy 0 <= P < 1, got {self.dropout}")
         if self.dropout > 0 and len(self.hidden_list()) == 1:
@@ -199,6 +217,9 @@ _HELP = {
     "clip_grad_norm": "Clip the gradient by its global L2 norm to this value before the update, as "
                       "torch.nn.utils.clip_grad_norm_ (0 = off); the norm includes the --weight_decay term and, with "
                       "--sync_mode grad_allreduce, is that of the averaged gradient (--comm nccl or gloo)",
+    "pooling": "What the classifier reads: last (the top layer's final state, default), or mean / max / attention pooling of "
+               "the top layer's outputs over each sample's real steps",
+    "attention_units": "Units A of --pooling attention (score = tanh(h_t W_a + b_a) . v)",
     "per_step_labels": "Label every time step (sequence labelling): labels [B,T], loss and accuracy over the real positions; "
                        "a CSV row is k*in_features values followed by k labels",
 }

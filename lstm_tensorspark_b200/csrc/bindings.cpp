@@ -61,6 +61,11 @@ int ts_lstm_seq_bwd(const void*, const void*, const void*, const float*, const v
                     const int*, const unsigned int*);
 int ts_dropout(const void*, void*, int, int, int, int, int, const int*, const unsigned int*, cudaStream_t);
 int ts_lstm_seq_prologue(const void*, const float*, void*, float*, void*, unsigned int*, int, int, cudaStream_t);
+int ts_seq_pool_fwd(const void*, int, const int*, const float*, int, int, int, int, float*, int*, cudaStream_t);
+int ts_seq_pool_attn_scores(float*, const float*, const float*, const int*, int, int, int, float*, cudaStream_t);
+int ts_seq_pool_attn_bwd(const void*, int, const float*, const float*, const float*, const float*, const int*, int, int, int, int,
+                         float*, void*, float*, unsigned int*, float*, float*, int, int, cudaStream_t);
+int ts_seq_pool_bwd(const float*, const int*, const int*, const float*, const float*, int, int, int, int, void*, int, cudaStream_t);
 const char* ts_last_error();
 }
 
@@ -354,6 +359,90 @@ Tensor head_step_bwd(const Tensor& h, const Tensor& W, const Tensor& dlogits, co
   return dh;
 }
 
+// ---- pooling over time (csrc/seq_pool.cu) ---------------------------------------------------------------------
+// h: the top layer's h_seq as contiguous [T·B, H] time-major rows (bf16 or fp32); mode 0 mean, 1 max, 2 attention.
+void chk_f32(const Tensor& t, int64_t numel, const char* n) {
+  chk_cuda(t, n);
+  TORCH_CHECK(t.scalar_type() == torch::kFloat32 && t.numel() == numel, n, ": fp32 with ", numel, " elements");
+}
+
+// -> (s fp32 [B,H], argmax int32 [B,H] (max; else empty)); alpha fp32 [T,B] for attention.
+std::vector<Tensor> seq_pool_fwd(const Tensor& h, const std::optional<Tensor>& lengths, int64_t T, int64_t mode,
+                                 const std::optional<Tensor>& alpha) {
+  chk_cuda(h, "h");
+  TORCH_CHECK(h.dim() == 2 && T >= 1 && h.size(0) % T == 0, "seq_pool_fwd: h [T·B, H]");
+  TORCH_CHECK(mode >= 0 && mode <= 2, "seq_pool_fwd: mode 0 mean, 1 max, 2 attention");
+  c10::cuda::CUDAGuard g(h.device());
+  const int B = h.size(0) / T, H = h.size(1);
+  if (mode == 2) {
+    TORCH_CHECK(alpha.has_value(), "seq_pool_fwd: attention needs alpha");
+    chk_f32(*alpha, (int64_t)T * B, "alpha");
+  }
+  auto fo = h.options().dtype(torch::kFloat32);
+  auto s = torch::empty({B, H}, fo);
+  auto am = mode == 1 ? torch::empty({B, H}, fo.dtype(torch::kInt32)) : torch::empty({0}, fo.dtype(torch::kInt32));
+  check(ts_seq_pool_fwd(h.data_ptr(), is_bf16(h), lengths_ptr(lengths, B, h), fptr(alpha), (int)mode, (int)T, B, H,
+                        s.data_ptr<float>(), mode == 1 ? am.data_ptr<int>() : nullptr, stream()), "seq_pool_fwd");
+  return {s, am};
+}
+
+// u fp32 [T·B, A]: h W_a in, tanh(h W_a + b_a) out (0 at uncounted steps) -> alpha fp32 [T,B], the softmax over counted steps.
+Tensor seq_pool_attn_scores(Tensor u, const Tensor& ba, const Tensor& v, const std::optional<Tensor>& lengths, int64_t T) {
+  chk_cuda(u, "u");
+  TORCH_CHECK(u.dim() == 2 && u.scalar_type() == torch::kFloat32 && T >= 1 && u.size(0) % T == 0, "seq_pool_attn_scores: u fp32 [T·B, A]");
+  c10::cuda::CUDAGuard g(u.device());
+  const int B = u.size(0) / T, A = u.size(1);
+  chk_f32(ba, A, "b_a"); chk_f32(v, A, "v");
+  auto alpha = torch::empty({T, B}, u.options());
+  check(ts_seq_pool_attn_scores(u.data_ptr<float>(), ba.data_ptr<float>(), v.data_ptr<float>(), lengths_ptr(lengths, B, u), (int)T, B, A,
+                                alpha.data_ptr<float>(), stream()), "seq_pool_attn_scores");
+  return alpha;
+}
+
+// -> dU [T·B, A] (dtype of h; 0 at uncounted steps); dv, dba fp32 [A] written (or accumulated into, acc_*) in a fixed order.
+Tensor seq_pool_attn_bwd(const Tensor& h, const Tensor& ds, const Tensor& alpha, const Tensor& u, const Tensor& v,
+                         const std::optional<Tensor>& lengths, int64_t T, Tensor dv, Tensor dba, bool acc_dv, bool acc_dba) {
+  chk_cuda(h, "h");
+  TORCH_CHECK(h.dim() == 2 && T >= 1 && h.size(0) % T == 0, "seq_pool_attn_bwd: h [T·B, H]");
+  c10::cuda::CUDAGuard g(h.device());
+  const int B = h.size(0) / T, H = h.size(1), A = u.size(1);
+  chk_f32(ds, (int64_t)B * H, "ds"); chk_f32(alpha, (int64_t)T * B, "alpha"); chk_f32(u, (int64_t)T * B * A, "u");
+  chk_f32(v, A, "v"); chk_f32(dv, A, "dv"); chk_f32(dba, A, "dba");
+  auto fo = h.options().dtype(torch::kFloat32);
+  auto dU = torch::empty({h.size(0), A}, h.options());
+  auto dalpha = torch::empty({T, B}, fo);
+  auto partial = torch::empty({B, 2 * A}, fo);
+  auto ticket = torch::zeros({1}, fo.dtype(torch::kInt32));
+  check(ts_seq_pool_attn_bwd(h.data_ptr(), is_bf16(h), ds.data_ptr<float>(), alpha.data_ptr<float>(), u.data_ptr<float>(),
+                             v.data_ptr<float>(), lengths_ptr(lengths, B, h), (int)T, B, H, A, dalpha.data_ptr<float>(), dU.data_ptr(),
+                             partial.data_ptr<float>(), (unsigned int*)ticket.data_ptr<int>(), dv.data_ptr<float>(), dba.data_ptr<float>(),
+                             acc_dv ? 1 : 0, acc_dba ? 1 : 0, stream()), "seq_pool_attn_bwd");
+  return dU;
+}
+
+// ds fp32 [B,H] -> dh_seq [T·B, H] (bf16 when out_bf16, else fp32), 0 at uncounted steps.  max: argmax int32 [B,H];
+// attention: alpha fp32 [T,B] and G = dU W_a^T fp32 [T·B, H] (added before the one rounding).
+Tensor seq_pool_bwd(const Tensor& ds, const std::optional<Tensor>& lengths, int64_t T, int64_t mode, const std::optional<Tensor>& argmax,
+                    const std::optional<Tensor>& alpha, const std::optional<Tensor>& G, bool out_bf16) {
+  chk_cuda(ds, "ds");
+  TORCH_CHECK(ds.dim() == 2 && ds.scalar_type() == torch::kFloat32 && T >= 1, "seq_pool_bwd: ds fp32 [B,H]");
+  TORCH_CHECK(mode >= 0 && mode <= 2, "seq_pool_bwd: mode 0 mean, 1 max, 2 attention");
+  c10::cuda::CUDAGuard g(ds.device());
+  const int B = ds.size(0), H = ds.size(1);
+  if (mode == 1) {
+    TORCH_CHECK(argmax.has_value() && argmax->scalar_type() == torch::kInt32 && argmax->numel() == (int64_t)B * H, "seq_pool_bwd: argmax int32 [B,H]");
+    chk_cuda(*argmax, "argmax");
+  }
+  if (mode == 2) {
+    TORCH_CHECK(alpha.has_value() && G.has_value(), "seq_pool_bwd: attention needs alpha and G");
+    chk_f32(*alpha, (int64_t)T * B, "alpha"); chk_f32(*G, (int64_t)T * B * H, "G");
+  }
+  auto dh = torch::empty({T * B, H}, ds.options().dtype(out_bf16 ? torch::kBFloat16 : torch::kFloat32));
+  check(ts_seq_pool_bwd(ds.data_ptr<float>(), lengths_ptr(lengths, B, ds), mode == 1 ? argmax->data_ptr<int>() : nullptr, fptr(alpha),
+                        fptr(G), (int)mode, (int)T, B, H, dh.data_ptr(), out_bf16 ? 1 : 0, stream()), "seq_pool_bwd");
+  return dh;
+}
+
 // ---- optimizer ----------------------------------------------------------------------------------------------
 // clip: the fp32 [2] {norm, coef} flat_grad_norm wrote on this stream; the update then uses coef * g_total.
 const float* clip_ptr(const std::optional<Tensor>& clip, const Tensor& p) {
@@ -635,6 +724,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("c_new"), py::arg("lengths") = py::none(), py::arg("t") = 0);
   m.def("xent_rows", &xent_rows);
   m.def("head_fwd", &head_fwd);
+  m.def("seq_pool_fwd", &seq_pool_fwd, py::arg("h"), py::arg("lengths"), py::arg("T"), py::arg("mode"), py::arg("alpha"));
+  m.def("seq_pool_attn_scores", &seq_pool_attn_scores, py::arg("u"), py::arg("b_a"), py::arg("v"), py::arg("lengths"), py::arg("T"));
+  m.def("seq_pool_attn_bwd", &seq_pool_attn_bwd, py::arg("h"), py::arg("ds"), py::arg("alpha"), py::arg("u"), py::arg("v"),
+        py::arg("lengths"), py::arg("T"), py::arg("dv"), py::arg("dba"), py::arg("acc_dv"), py::arg("acc_dba"));
+  m.def("seq_pool_bwd", &seq_pool_bwd, py::arg("ds"), py::arg("lengths"), py::arg("T"), py::arg("mode"), py::arg("argmax"),
+        py::arg("alpha"), py::arg("G"), py::arg("out_bf16"));
   m.def("head_step_fwd", &head_step_fwd, py::arg("h"), py::arg("W"), py::arg("bias"), py::arg("labels"), py::arg("lengths"), py::arg("T"));
   m.def("head_step_bwd", &head_step_bwd, py::arg("h"), py::arg("W"), py::arg("dlogits"), py::arg("dloss"), py::arg("dW"), py::arg("db"),
         py::arg("accumulate"));

@@ -33,6 +33,27 @@ class DenseHead(nn.Module):
         return h2.float() @ self.weights + self.bias
 
 
+class Attention(nn.Module):
+    """Attention pooling over time (``--pooling attention``): ``W_a [H_in, A]``, ``b_a [A]`` and the context vector ``v [A]``
+    score every step as ``tanh(h_t W_a + b_a) . v`` (``ops.reference.pool_sequence``).  ``--init scaled``: W_a has std
+    init_std / sqrt(H_in), b_a = 0 and v std init_std / sqrt(A); otherwise all three are truncated normal with init_std."""
+
+    def __init__(self, in_features: int, units: int, init_std: float = 1.0, scaled: bool = False, device=None, generator=None):
+        super().__init__()
+        w_std = init_std / in_features ** 0.5 if scaled else init_std
+        v_std = init_std / units ** 0.5 if scaled else init_std
+        self.weights = create_variable("weights", (in_features, units), device=device, generator=generator,
+                                       initializer=lambda t, generator=None: truncated_normal_(t, w_std, generator))
+        self.bias = create_variable("bias", (units,), device=device, generator=generator,
+                                    initializer=(lambda t, generator=None: nn.init.zeros_(t)) if scaled
+                                    else (lambda t, generator=None: truncated_normal_(t, init_std, generator)))
+        self.context = create_variable("context", (units,), device=device, generator=generator,
+                                       initializer=lambda t, generator=None: truncated_normal_(t, v_std, generator))
+
+    def params(self) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+        return self.weights, self.bias, self.context
+
+
 class SequenceClassifier(nn.Module):
     def __init__(self, cfg: Config, batch_size: Optional[int] = None, device=None,
                  generator: Optional[torch.Generator] = None,
@@ -49,6 +70,12 @@ class SequenceClassifier(nn.Module):
         if cfg.bidirectional:
             # drawn after every parameter of the unidirectional model, which therefore keeps its initial weights
             self.rnn.add_reverse_layers()
+        self.pooling = getattr(cfg, "pooling", "last")
+        self.attention: Optional[Attention] = None
+        if self.pooling == "attention":
+            # drawn after everything else (the reverse layers included): every other configuration keeps its initial weights
+            self.attention = Attention(head_in, cfg.attention_units, init_std=cfg.init_std, scaled=cfg.init == "scaled",
+                                       device=device, generator=generator)
         self.flat: Optional[FlatParams] = None
         self._allocator = allocator
         self.compute_dtype = torch.float32
@@ -68,10 +95,19 @@ class SequenceClassifier(nn.Module):
             if self.flat.data.is_cuda and F.get_backend() != "torch":
                 # the CUDA ops write these gradients straight into the flat buffer (first write of a step overwrites):
                 # zero_grad() then has nothing to memset
-                self.flat.enable_direct_grads(self.rnn.averaged_parameters() + [self.head.weights, self.head.bias])
+                self.flat.enable_direct_grads(self.rnn.averaged_parameters() + [self.head.weights, self.head.bias] +
+                                              ([] if self.attention is None else list(self.attention.params())))
 
     def features(self, x: torch.Tensor, lengths: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """``lengths``: optional int32 ``[B]`` per-sample sequence lengths (right-padded ``x``)."""
+        """``lengths``: optional int32 ``[B]`` per-sample sequence lengths (right-padded ``x``).  The top layer's last state, or
+        with ``--pooling mean | max | attention`` its outputs pooled over each sample's steps (``ops.reference.pool_sequence``),
+        rounded once to the compute dtype."""
+        if self.pooling != "last":
+            if x.dim() != 3:
+                raise ValueError(f"--pooling {self.pooling} needs sequences [B,T,D], got {tuple(x.shape)}")
+            h_seq = self.sequence_features(x, lengths)
+            s = F.pool_sequence(h_seq, lengths, self.pooling, None if self.attention is None else self.attention.params())
+            return s.to(h_seq.dtype)
         self.rnn.reset_state(x.shape[0])
         return self.rnn.fit_layers(x.to(self.compute_dtype) if x.is_floating_point() else x, lengths=lengths)
 
@@ -89,7 +125,8 @@ class SequenceClassifier(nn.Module):
     def sequence_features(self, x: torch.Tensor, lengths: Optional[torch.Tensor] = None) -> torch.Tensor:
         """The top layer's whole output ``[T,B,H_last]`` (bidirectional ``[T,B,2 H_last]``) of ``x [B,T,D]``."""
         if x.dim() != 3:
-            raise ValueError(f"--per_step_labels needs sequences [B,T,D], got {tuple(x.shape)}")
+            flag = "--per_step_labels" if self.per_step else f"--pooling {self.pooling}"
+            raise ValueError(f"{flag} needs sequences [B,T,D], got {tuple(x.shape)}")
         self.rnn.reset_state(x.shape[0])
         return self.rnn.fit_sequence_all(x.to(self.compute_dtype) if x.is_floating_point() else x, lengths=lengths)
 
@@ -121,6 +158,10 @@ class SequenceClassifier(nn.Module):
             out += layer.named_reference_variables()
         out.append(("Dense1/weights", self.head.weights))
         out.append(("Dense1/bias", self.head.bias))
+        if self.attention is not None:
+            out.append(("Attention/weights", self.attention.weights))
+            out.append(("Attention/bias", self.attention.bias))
+            out.append(("Attention/context", self.attention.context))
         return out
 
     def check_directions(self, variables: Dict[str, torch.Tensor], what: str = "checkpoint") -> None:
@@ -131,6 +172,19 @@ class SequenceClassifier(nn.Module):
             raise ValueError(f"{what} was written by a {'bidirectional' if saved else 'unidirectional'} model, this run is "
                              f"{'bidirectional' if self.rnn.bidirectional else 'unidirectional'}: "
                              f"{'add' if saved else 'drop'} --bidirectional")
+
+    def check_pooling(self, variables: Dict[str, torch.Tensor], recorded: Optional[str] = None, what: str = "checkpoint") -> None:
+        """Raise unless ``variables`` (and the pooling ``recorded`` beside them; nothing recorded counts as ``last``) were written
+        under this model's ``--pooling``: a checkpoint loads with ``strict=False`` and would otherwise drop or leave behind the
+        attention weights, or silently score another model."""
+        saved = recorded or "last"
+        has_attn = any(k.startswith("Attention/") for k in variables)
+        if saved == self.pooling and has_attn == (self.pooling == "attention"):
+            return
+        if saved == self.pooling:
+            saved = "attention" if has_attn else f"{saved} (without the Attention/* variables)"
+        raise ValueError(f"{what} was written with --pooling {saved}, this run uses --pooling {self.pooling}: "
+                         f"pass the --pooling it was trained with")
 
     def reference_state_dict(self) -> Dict[str, torch.Tensor]:
         return {k: v.detach().clone().contiguous().cpu() for k, v in self.named_reference_variables()}

@@ -77,6 +77,15 @@ def head_xent_per_step(h_seq, weights, bias, labels, lengths=None):
     return ref.head_xent_per_step(h_seq, weights, bias, labels, lengths)
 
 
+def pool_sequence(h_seq, lengths=None, mode: str = "mean", attention=None):
+    """Pool ``h_seq [T,B,H]`` over each row's counted steps -> ``s [B,H]`` fp32 (``reference.pool_sequence``); ``mode`` mean,
+    max or attention (``attention = (W_a, b_a, v)``)."""
+    if _use_ext(h_seq):
+        from . import cuda_pool
+        return cuda_pool.pool_sequence(h_seq, lengths, mode, attention)
+    return ref.pool_sequence(h_seq, lengths, mode, attention)
+
+
 def lstm_pair_supported(x_seq, h_a: int, h_b: int) -> bool:
     """Can two stacked layers run as one pair op on the GPU (layer wavefront or pipelined, ``cuda_lstm.pair_schedule``)?"""
     if not x_seq.is_cuda or _BACKEND == "torch":

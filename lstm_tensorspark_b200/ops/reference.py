@@ -251,6 +251,39 @@ def softmax_xent_per_step(logits, labels, lengths=None):
     return (torch.nn.functional.cross_entropy(lg, lab, reduction="sum") / n, (lg.argmax(1) == lab).float().sum() / n, n)
 
 
+POOLING_MODES = ("last", "mean", "max", "attention")
+
+
+def pool_sequence(h_seq, lengths=None, mode: str = "mean", attention=None):
+    """Pool the top layer's output over the counted steps (``step_mask``): ``h_seq [T,B,H]`` -> ``s [B,H]`` (fp32; fp64 for
+    fp64 ``h_seq``).  ``mean``: the mean over t < len_b.  ``max``: the per-unit max; its gradient goes to the smallest t that
+    attains it.  ``attention`` with ``attention = (W_a [H,A], b_a [A], v [A])``: u = tanh(h W_a + b_a), e = u . v, alpha =
+    softmax over the counted t (0 elsewhere), s = sum_t alpha_t h_t.  Uncounted positions are replaced by zeros before anything
+    reads them, so their values reach neither the result nor a gradient (theirs is 0)."""
+    T, B, _ = h_seq.shape
+    dt = torch.float64 if h_seq.dtype == torch.float64 else torch.float32
+    keep = step_mask(lengths, B, T, device=h_seq.device).t()                                 # [T,B]
+    h = torch.where(keep.unsqueeze(2), h_seq.to(dt), torch.zeros((), dtype=dt, device=h_seq.device))
+    if mode == "mean":
+        n = keep.sum(0).to(dt)
+        return h.sum(0) / n.unsqueeze(1)
+    if mode == "max":
+        hm = torch.where(keep.unsqueeze(2), h, torch.full((), float("-inf"), dtype=dt, device=h.device))
+        top = hm.max(0, keepdim=True).values
+        t_idx = torch.arange(T, device=h.device).view(T, 1, 1).expand_as(hm)
+        first = torch.where(hm == top, t_idx, T).min(0, keepdim=True).values                  # the smallest t at the max
+        return h.gather(0, first).squeeze(0)
+    if mode == "attention":
+        if attention is None:
+            raise ValueError("attention pooling needs its parameters (W_a, b_a, v)")
+        w_a, b_a, v = (p.to(dt) for p in attention)
+        u = torch.tanh(h @ w_a + b_a)
+        e = torch.where(keep, u @ v, torch.full((), float("-inf"), dtype=dt, device=h.device))
+        alpha = torch.softmax(e, 0)
+        return (alpha.unsqueeze(2) * h).sum(0)
+    raise ValueError(f"unknown pooling {mode!r}: one of {', '.join(POOLING_MODES)}")
+
+
 def clip_coefficient(g_total_segments, max_norm: float):
     """Clipping by the global norm (``torch.nn.utils.clip_grad_norm_``): ``norm = ||g_total||_2`` over all segments, summed in
     fp64 and rounded to the segments' dtype, and ``coef = min(max_norm / (norm + 1e-6), 1)`` in that dtype (a NaN norm gives a

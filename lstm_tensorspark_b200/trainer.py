@@ -152,6 +152,7 @@ def train_rnn(partition, cfg: Config, rank: int = 0, world_size: int = 1, comm: 
         if src:
             variables, meta, opt_state = ckpt.load(src)
             model.check_directions(variables, f"checkpoint {src}")
+            model.check_pooling(variables, (meta.get("config") or {}).get("pooling"), f"checkpoint {src}")
             model.load_reference_state_dict(variables, strict=False)
             eng.flat.refresh_shadow()
             if opt_state is not None:
@@ -374,7 +375,7 @@ def load_shards(cfg: Config, world_size: int, standalone: bool):
 
 def _find_trained_model(cfg: Config, standalone: bool):
     """--resume <file | dir>, else <output_path>/averaged_model.pt (distributed job), else the latest checkpoint under
-    --checkpoint_path.  -> (variables in the reference's names, description)."""
+    --checkpoint_path.  -> (variables in the reference's names, description, the --pooling the file records or None)."""
     src = cfg.resume
     if not src and not standalone and cfg.output_path and os.path.isfile(os.path.join(cfg.output_path, "averaged_model.pt")):
         src = os.path.join(cfg.output_path, "averaged_model.pt")
@@ -384,13 +385,14 @@ def _find_trained_model(cfg: Config, standalone: bool):
         src = os.path.join(src, "averaged_model.pt")
     if src and os.path.isfile(src) and src.endswith(".pt"):
         blob = torch.load(src, map_location="cpu", weights_only=False)
-        return blob["variables"], src
+        return blob["variables"], src, (blob.get("meta") or {}).get("pooling")
     if src and os.path.isdir(src):
         if ckpt.latest_checkpoint(src) is None and os.path.isdir(os.path.join(src, "0")):
             src = os.path.join(src, "0")
         last = ckpt.latest_checkpoint(src)
         if last:
-            return ckpt.load(last)[0], last
+            variables, meta, _ = ckpt.load(last)
+            return variables, last, (meta.get("config") or {}).get("pooling")
     raise FileNotFoundError("--mode eval: no trained model found (give --resume <averaged_model.pt | checkpoint dir>)")
 
 
@@ -399,7 +401,7 @@ def evaluate_job(cfg: Config, standalone: bool = False) -> Dict:
     file in batches of ``--batch_size``, forward kernels only, one device.  Not in the reference (its ``--mode`` flag knows
     only ``train`` and the averaged model is thrown away, src/rnn.py:371,407-408); it closes the train -> average -> use loop."""
     from .engine import TrainEngine
-    variables, src = _find_trained_model(cfg, standalone)
+    variables, src, pooling = _find_trained_model(cfg, standalone)
     lengths = None
     if cfg.synthetic and cfg.per_step_labels:
         data = D.synthetic_per_step(cfg.synthetic, cfg.seq_len, cfg.in_features, cfg.num_classes, seed=cfg.seed,
@@ -434,6 +436,7 @@ def evaluate_job(cfg: Config, standalone: bool = False) -> Dict:
     shapes = {k: tuple(v.shape) for k, v in eng.model.named_reference_variables()}
     variables = dict(variables)
     eng.model.check_directions(variables, f"model {src}")
+    eng.model.check_pooling(variables, pooling, f"model {src}")
     for k, v in list(variables.items()):
         want = shapes.get(k)
         if want is not None and tuple(v.shape) != want and v.dim() == 2 and len(want) == 2 and v.shape[1] == want[1]:
@@ -523,7 +526,8 @@ def run_job(cfg: Config, standalone: bool = False) -> Dict:
     if res0 is not None and cfg.output_path:
         ckpt.save_averaged_model(cfg.output_path, res0["records"], res0["variables"],
                                  {"world_size": world_size, "sync_mode": cfg.sync_mode, "average_scope": cfg.average_scope,
-                                  "hidden_units": cfg.hidden_units, "seconds": total})
+                                  "hidden_units": cfg.hidden_units, "pooling": cfg.pooling,
+                                  "attention_units": cfg.attention_units, "seconds": total})
     if not cfg.quiet:
         print("RNN-LSTM - Total Processing Time {}s".format(total))
     return {"results": results, "seconds": total, "world_size": world_size, "partitions": n_shards}
