@@ -28,7 +28,7 @@ import torch.nn.functional as F
 
 class CudnnLSTMClassifier(nn.Module):
     def __init__(self, hidden, in_features, num_classes, time_major=False, bidirectional=False, dropout=0.0, per_step=False,
-                 pooling="last", attention_units=128):
+                 pooling="last", attention_units=128, vocab_size=0):
         super().__init__()
         self.per_step = per_step
         self.pooling = pooling
@@ -41,6 +41,8 @@ class CudnnLSTMClassifier(nn.Module):
         if pooling == "attention":                      # u_t = tanh(W_a h_t + b_a), e_t = u_t . v
             self.att = nn.Linear(hidden[-1] * (2 if bidirectional else 1), attention_units)
             self.context = nn.Parameter(torch.randn(attention_units) / attention_units ** 0.5)
+        # vocab_size > 0: token ids [B,T] (time-major [T,B]) through nn.Embedding(V, in_features) in front of the stack
+        self.embed = nn.Embedding(vocab_size, in_features) if vocab_size > 0 else None
 
     def pool(self, out, lengths=None):
         """``--pooling mean | max | attention`` over the outputs ``out`` (time-major [T,B,H] or batch-major [B,T,H]) at each row's
@@ -58,6 +60,8 @@ class CudnnLSTMClassifier(nn.Module):
         return (torch.softmax(e.float(), 0).to(hm.dtype).unsqueeze(2) * hm).sum(0)
 
     def forward(self, x, lengths=None):
+        if self.embed is not None:
+            x = self.embed(x)
         out, (h_n, _) = self.lstm(x)
         if self.per_step:                               # nn.Linear over every output: logits [B,T,C] (time-major: [T,B,C])
             return self.head(out)
@@ -70,10 +74,11 @@ class CudnnLSTMClassifier(nn.Module):
 
 class BaselineRunner:
     def __init__(self, hidden, in_features, num_classes, batch, seq_len, rank, world, device, optimizer="adam", lr=1e-3,
-                 variant="stock", bidirectional=False, dropout=0.0, per_step=False, pooling="last"):
+                 variant="stock", bidirectional=False, dropout=0.0, per_step=False, pooling="last", vocab_size=0):
         """``per_step``: sequence labelling - labels ``[B,T]``, the head over every output and the mean cross-entropy over all
         ``T·B`` positions (default: classify the final state, labels ``[B]``).  ``pooling``: classify the mean / max / attention
-        pooling of the top layer's outputs (``nn.LSTM`` + masked pool + ``nn.Linear``); a step then takes ``lengths``."""
+        pooling of the top layer's outputs (``nn.LSTM`` + masked pool + ``nn.Linear``); a step then takes ``lengths``.
+        ``vocab_size`` > 0: a step takes int token ids ``[B,T]`` read through ``nn.Embedding(vocab_size, in_features)``."""
         self.rank, self.world, self.device = rank, world, device
         self.B, self.T, self.D, self.C = batch, seq_len, in_features, num_classes
         self.variant = variant
@@ -86,7 +91,7 @@ class BaselineRunner:
         if world > 1 and not dist.is_initialized():
             dist.init_process_group("nccl", rank=rank, world_size=world, device_id=device)
         model = CudnnLSTMClassifier(hidden, in_features, num_classes, time_major=self.tuned, bidirectional=bidirectional,
-                                    dropout=dropout, per_step=per_step, pooling=pooling).to(device)
+                                    dropout=dropout, per_step=per_step, pooling=pooling, vocab_size=vocab_size).to(device)
         if self.tuned:
             model = model.to(torch.bfloat16)
             model.lstm.flatten_parameters()

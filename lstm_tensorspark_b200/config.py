@@ -60,6 +60,9 @@ class Config:
     pooling: str = "last"               # what the classifier reads: last (the top layer's state after each sample's last step) |
                                         # mean | max | attention over the top layer's outputs at the sample's real steps
     attention_units: int = ATTENTION_UNITS_DEFAULT  # A of --pooling attention: u_t = tanh(h_t W_a + b_a) [A], score u_t . v
+    vocab_size: int = 0                 # V > 0: the input is int token ids [B,T] (one step: [B]) and the first layer reads
+                                        # x_t = Embedding[tok_t], a learned [V, in_features] table (nn.Embedding); a CSV row is k ids
+                                        # followed by the label (--per_step_labels: by k labels).  0 = float features
     dtype: str = "auto"                 # auto: bf16 on cuda, fp32 on cpu
     device: str = "auto"                # auto | cpu | cuda
     backend: str = "auto"               # auto | cuda_ext (hand-written sm_90a kernels) | torch
@@ -160,6 +163,10 @@ class Config:
                              "step's output, there is nothing to pool (use --pooling last)")
         if self.attention_units != ATTENTION_UNITS_DEFAULT and self.pooling != "attention":
             warnings.warn(f"--attention_units {self.attention_units} has no effect without --pooling attention")
+        if self.vocab_size < 0:
+            raise ValueError(f"--vocab_size must be >= 0 (0 = float features), got {self.vocab_size}")
+        if self.vocab_size > 0 and self.normalize:
+            raise ValueError("--normalize does not combine with --vocab_size: token ids are not feature values to scale")
         if not 0.0 <= self.dropout < 1.0:
             raise ValueError(f"--dropout must satisfy 0 <= P < 1, got {self.dropout}")
         if self.dropout > 0 and len(self.hidden_list()) == 1:
@@ -220,6 +227,9 @@ _HELP = {
     "pooling": "What the classifier reads: last (the top layer's final state, default), or mean / max / attention pooling of "
                "the top layer's outputs over each sample's real steps",
     "attention_units": "Units A of --pooling attention (score = tanh(h_t W_a + b_a) . v)",
+    "vocab_size": "Read token ids through a learned embedding table of V rows and --in_features columns (nn.Embedding in front "
+                  "of the first layer); a CSV row is k ids followed by the label (or by k labels with --per_step_labels). "
+                  "0 = float features",
     "per_step_labels": "Label every time step (sequence labelling): labels [B,T], loss and accuracy over the real positions; "
                        "a CSV row is k*in_features values followed by k labels",
 }

@@ -66,6 +66,10 @@ int ts_seq_pool_attn_scores(float*, const float*, const float*, const int*, int,
 int ts_seq_pool_attn_bwd(const void*, int, const float*, const float*, const float*, const float*, const int*, int, int, int, int,
                          float*, void*, float*, unsigned int*, float*, float*, int, int, cudaStream_t);
 int ts_seq_pool_bwd(const float*, const int*, const int*, const float*, const float*, int, int, int, int, void*, int, cudaStream_t);
+void ts_embed_scratch_numel(long long, long long, long long, long long*);
+int ts_embed_fwd(const void*, int, const int*, const int*, int, int, int, int, void*, cudaStream_t);
+int ts_embed_bwd(const void*, int, const int*, const int*, int, int, int, int, float*, int, int*, int*, float*, cudaStream_t);
+int ts_embed_bwd_launches();
 const char* ts_last_error();
 }
 
@@ -443,6 +447,59 @@ Tensor seq_pool_bwd(const Tensor& ds, const std::optional<Tensor>& lengths, int6
   return dh;
 }
 
+// ---- token embedding (csrc/embedding.cu) ------------------------------------------------------------------------
+void chk_tokens(const Tensor& tok, const Tensor& like) {
+  chk_cuda(tok, "tokens");
+  TORCH_CHECK(tok.device() == like.device() && tok.scalar_type() == torch::kInt32 && tok.dim() == 2,
+              "tokens must be int32 [B,T] on the table's device");
+}
+
+// table [V,E] (bf16 or fp32), tokens int32 [B,T] -> x [T,B,E] of the table's dtype, time-major
+Tensor embed_fwd(const Tensor& table, const Tensor& tokens, const std::optional<Tensor>& lengths) {
+  chk_cuda(table, "table");
+  TORCH_CHECK(table.dim() == 2, "embed_fwd: table [V,E]");
+  chk_tokens(tokens, table);
+  c10::cuda::CUDAGuard g(table.device());
+  const int B = tokens.size(0), T = tokens.size(1), V = table.size(0), E = table.size(1);
+  auto x = torch::empty({T, B, E}, table.options());
+  check(ts_embed_fwd(table.data_ptr(), is_bf16(table), tokens.data_ptr<int>(), lengths_ptr(lengths, B, table), T, B, E, V,
+                     x.data_ptr(), stream()), "embed_fwd");
+  return x;
+}
+
+// Per-device scratch of the backward pass: {zeroed (2 V int32 words that are zero between calls, the kernels restore them),
+// working ints, partial floats}.  A buffer only grows, and a replaced one is kept alive: a captured graph holds its pointers.
+struct EmbedScratch { int* zeroed; int* ints; float* floats; };
+EmbedScratch embed_scratch(const Tensor& like, int64_t N, int64_t V, int64_t E) {
+  static std::vector<std::vector<Tensor>> bufs(64, std::vector<Tensor>(3));
+  static std::vector<Tensor> retired;
+  auto& b = bufs[like.device().index()];
+  long long need[2];
+  ts_embed_scratch_numel(N, V, E, need);
+  const int64_t sizes[3] = {2 * V, need[0], need[1]};
+  for (int i = 0; i < 3; ++i) {
+    if (b[i].defined() && b[i].numel() >= sizes[i]) continue;
+    if (b[i].defined()) retired.push_back(b[i]);
+    auto opt = torch::TensorOptions().device(like.device()).dtype(i == 2 ? torch::kFloat32 : torch::kInt32);
+    b[i] = i == 0 ? torch::zeros({sizes[i]}, opt) : torch::empty({sizes[i]}, opt);
+  }
+  return {b[0].data_ptr<int>(), b[1].data_ptr<int>(), b[2].data_ptr<float>()};
+}
+
+// dx [T·B, E] (bf16 or fp32) -> dW fp32 [V,E]: every row written (accumulate false) or added to the rows of ids present
+void embed_bwd(const Tensor& dx, const Tensor& tokens, const std::optional<Tensor>& lengths, Tensor dW, bool accumulate) {
+  chk_cuda(dx, "dx"); chk_cuda(dW, "dW");
+  chk_tokens(tokens, dx);
+  const int B = tokens.size(0), T = tokens.size(1);
+  TORCH_CHECK(dW.dim() == 2 && dW.scalar_type() == torch::kFloat32 && dW.device() == dx.device(), "embed_bwd: dW fp32 [V,E]");
+  const int V = dW.size(0), E = dW.size(1);
+  TORCH_CHECK(dx.numel() == (int64_t)T * B * E, "embed_bwd: dx [T·B, E]");
+  c10::cuda::CUDAGuard g(dx.device());
+  auto s = embed_scratch(dx, (int64_t)T * B, V, E);
+  check(ts_embed_bwd(dx.data_ptr(), is_bf16(dx), tokens.data_ptr<int>(), lengths_ptr(lengths, B, dx), T, B, E, V,
+                     dW.data_ptr<float>(), accumulate ? 1 : 0, s.zeroed, s.ints, s.floats, stream()), "embed_bwd");
+}
+
 // ---- optimizer ----------------------------------------------------------------------------------------------
 // clip: the fp32 [2] {norm, coef} flat_grad_norm wrote on this stream; the update then uses coef * g_total.
 const float* clip_ptr(const std::optional<Tensor>& clip, const Tensor& p) {
@@ -730,6 +787,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("lengths"), py::arg("T"), py::arg("dv"), py::arg("dba"), py::arg("acc_dv"), py::arg("acc_dba"));
   m.def("seq_pool_bwd", &seq_pool_bwd, py::arg("ds"), py::arg("lengths"), py::arg("T"), py::arg("mode"), py::arg("argmax"),
         py::arg("alpha"), py::arg("G"), py::arg("out_bf16"));
+  m.def("embed_fwd", &embed_fwd, py::arg("table"), py::arg("tokens"), py::arg("lengths"));
+  m.def("embed_bwd", &embed_bwd, py::arg("dx"), py::arg("tokens"), py::arg("lengths"), py::arg("dW"), py::arg("accumulate"));
+  m.attr("EMBED_BWD_LAUNCHES") = ts_embed_bwd_launches();
   m.def("head_step_fwd", &head_step_fwd, py::arg("h"), py::arg("W"), py::arg("bias"), py::arg("labels"), py::arg("lengths"), py::arg("T"));
   m.def("head_step_bwd", &head_step_bwd, py::arg("h"), py::arg("W"), py::arg("dlogits"), py::arg("dloss"), py::arg("dW"), py::arg("db"),
         py::arg("accumulate"));

@@ -194,6 +194,62 @@ def process_batch_per_step(train_xy: Sequence[Sequence[str]], seq_len: int, in_f
     return x, y
 
 
+def process_tokens(train_xy: Sequence[Sequence[str]], seq_len: int, vocab_size: int, num_classes: int = 0,
+                   variable_length: bool = False, per_step_labels: bool = False):
+    """Rows of token ids (``--vocab_size``) -> ``(x int32 [N, seq_len] ([N] when seq_len == 1), y int64 [N] or [N, seq_len])``,
+    plus ``lengths`` int32 [N] with ``variable_length``.
+
+    A row is ``k`` ids followed by the label, or with ``per_step_labels`` by ``k`` labels; ``k = seq_len``, or
+    ``1 <= k <= seq_len`` with ``variable_length`` (then padded on the right with id 0, label 0, never read).  A non-integer id,
+    an id outside ``[0, vocab_size)``, a per-step label outside ``[0, num_classes)`` or a row that does not split this way is an
+    error naming the row."""
+    if seq_len < 1 or vocab_size < 1:
+        raise ValueError("token rows need seq_len >= 1 and vocab_size >= 1")
+    want = f"1..{seq_len}" if variable_length else f"{seq_len}"
+    xs, ys, ls = [], [], []
+    for n, row in enumerate(train_xy):
+        if len(row) <= 1:
+            continue
+        if per_step_labels:
+            k, rem = divmod(len(row), 2)
+        else:
+            k, rem = len(row) - 1, 0
+        if rem or not (k == seq_len or (variable_length and 1 <= k <= seq_len)):
+            raise ValueError(f"row {n}: {len(row)} fields is not {want} token ids followed by "
+                             f"{'one label per step' if per_step_labels else 'the label'}")
+        ids = []
+        for v in row[:k]:
+            s = str(v).strip()
+            try:
+                i = int(s)
+            except ValueError:
+                raise ValueError(f"row {n}: token id {s!r} is not an integer") from None
+            if not 0 <= i < vocab_size:
+                raise ValueError(f"row {n}: token id {i} outside [0, {vocab_size}) (--vocab_size {vocab_size})")
+            ids.append(i)
+        lab = [int(float(v)) for v in row[k:]]
+        if per_step_labels:
+            bad = [v for v in lab if not 0 <= v < num_classes]
+            if bad:
+                raise ValueError(f"row {n}: label {bad[0]} outside [0, {num_classes})")
+        xs.append(ids)
+        ys.append(lab if per_step_labels else lab[0])
+        ls.append(k)
+    if not xs:
+        raise ValueError("empty partition: no parsable rows")
+    x = np.zeros((len(xs), seq_len), dtype=np.int32)
+    y = np.zeros((len(xs), seq_len), dtype=np.int64) if per_step_labels else np.asarray(ys, dtype=np.int64)
+    for i, r in enumerate(xs):
+        x[i, :ls[i]] = r
+        if per_step_labels:
+            y[i, :ls[i]] = ys[i]
+    if seq_len == 1:
+        x = x[:, 0].copy()
+    if variable_length:
+        return x, y, np.asarray(ls, dtype=np.int32)
+    return x, y
+
+
 def resolve_batch_size(batch_size: int, shard_rows: int) -> int:
     """``--batch_size 0`` = whole shard (reference intent, src/rnn.py:193-199, Q3)."""
     bs = shard_rows if not batch_size else batch_size
@@ -266,6 +322,45 @@ def synthetic_per_step(n: int, seq_len: int, in_features: int, num_classes: int,
     x[pad] = 0.0
     y[pad] = 0
     return x.astype(dtype), y, lengths
+
+
+def synthetic_tokens(n: int, seq_len: int, vocab_size: int, num_classes: int, seed: int = 0, variable_length: bool = False,
+                     per_step_labels: bool = False, p_class: float = 0.5, ids_per_class: int = 8):
+    """A learnable token task (``--vocab_size``): every class owns ``ids_per_class`` indicative ids (distinct while the vocabulary
+    allows); a step draws from its class's ids with probability ``p_class`` and from a Zipf(1.1) background over the whole
+    vocabulary otherwise.  The class of a step is its sample's label, or with ``per_step_labels`` the step's own label.
+    -> ``(x int32 [n, T] ([n] when T == 1), y int64 [n] or [n, T])``, plus ``lengths`` with ``variable_length`` (those of
+    ``synthetic_lengths``; padded steps hold id 0 and label 0).  Drawn by a generator of its own: the draws of
+    ``synthetic_sequences`` and ``synthetic_per_step`` are untouched."""
+    if vocab_size < 1:
+        raise ValueError("synthetic tokens need vocab_size >= 1")
+    rng = np.random.default_rng([seed, 0x746F6B])
+    own = rng.permutation(vocab_size)[:num_classes * ids_per_class] if vocab_size >= num_classes * ids_per_class \
+        else rng.integers(0, vocab_size, size=num_classes * ids_per_class)
+    own = own.reshape(num_classes, ids_per_class)
+    if per_step_labels:
+        y = rng.integers(0, num_classes, size=(n, seq_len)).astype(np.int64)
+        cls = y
+    else:
+        y = rng.integers(0, num_classes, size=n).astype(np.int64)
+        cls = np.broadcast_to(y[:, None], (n, seq_len))
+    pick = own[cls, rng.integers(0, ids_per_class, size=(n, seq_len))]
+    background = (rng.zipf(1.1, size=(n, seq_len)) - 1) % vocab_size
+    x = np.where(rng.random((n, seq_len)) < p_class, pick, background).astype(np.int32)
+    lengths = None
+    if variable_length:
+        if seq_len < 2:
+            raise ValueError("variable-length sequences need seq_len >= 2")
+        lengths = synthetic_lengths(n, seq_len, seed)
+        pad = np.arange(seq_len)[None, :] >= lengths[:, None]
+        x[pad] = 0
+        if per_step_labels:
+            y[pad] = 0
+    if seq_len == 1:
+        x = x[:, 0].copy()
+        if per_step_labels:
+            y = y[:, 0].copy()
+    return (x, y) if lengths is None else (x, y, lengths)
 
 
 def synthetic_lengths(n: int, seq_len: int, seed: int = 0) -> np.ndarray:

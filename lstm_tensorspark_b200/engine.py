@@ -102,6 +102,10 @@ class TrainEngine:
         layers = self.model.rnn.directions()
         others = [p for p in flat.params[len(self.model.rnn.averaged_parameters()):]]
         others_direct = all(p.data_ptr() in flat._direct for p in others)
+        # --vocab_size: the table's gradient is the last one backward writes (after layer 0's), and it is the last parameter of
+        # the flat buffer - a bucket of its own, so the top layer's bucket does not wait for the whole backward pass
+        table = None if self.model.embedding is None else self.model.embedding.weights
+        top_others = [p for p in others if p is not table]
         end = [off[id(l.w_x)] for l in layers[1:]] + [flat.lstm_numel]        # end of each layer's segment
         plan = []
         for li in reversed(range(len(layers))):
@@ -111,10 +115,13 @@ class TrainEngine:
             lo_x, lo_h, hi = off[id(l.w_x)], off[id(l.w_h)], end[li]
             need_h = [l.w_h, l.bias]
             if li == len(layers) - 1 and others_direct:
-                hi = flat.padded_numel                     # head weights / bias follow the last layer in the flat buffer
-                need_h = need_h + others
+                # head weights / bias (and the attention weights) follow the last layer in the flat buffer
+                hi = flat.padded_numel if table is None else off[id(table)]
+                need_h = need_h + top_others
             plan.append({"lo": lo_x, "hi": lo_h, "need": {l.w_x.data_ptr()}})
             plan.append({"lo": lo_h, "hi": hi, "need": {p.data_ptr() for p in need_h}})
+        if table is not None and others_direct:
+            plan.append({"lo": off[id(table)], "hi": flat.padded_numel, "need": {table.data_ptr()}})
         if not others_direct:
             plan.append({"lo": flat.lstm_numel, "hi": flat.padded_numel, "need": None})    # autograd-accumulated: only final at the end
         return plan

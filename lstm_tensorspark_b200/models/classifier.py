@@ -54,6 +54,19 @@ class Attention(nn.Module):
         return self.weights, self.bias, self.context
 
 
+class Embedding(nn.Module):
+    """Token embedding in front of the first layer (``--vocab_size V``): ``weights [V, E]``, truncated normal with ``init_std``
+    under both ``--init`` modes (the fan-in of a one-hot input is 1)."""
+
+    def __init__(self, vocab_size: int, dim: int, init_std: float = 1.0, device=None, generator=None):
+        super().__init__()
+        self.weights = create_variable("weights", (vocab_size, dim), device=device, generator=generator,
+                                       initializer=lambda t, generator=None: truncated_normal_(t, init_std, generator))
+
+    def forward(self, tokens: torch.Tensor, lengths: Optional[torch.Tensor] = None, dtype=None) -> torch.Tensor:
+        return F.embedding(tokens, self.weights, lengths, dtype)
+
+
 class SequenceClassifier(nn.Module):
     def __init__(self, cfg: Config, batch_size: Optional[int] = None, device=None,
                  generator: Optional[torch.Generator] = None,
@@ -76,6 +89,11 @@ class SequenceClassifier(nn.Module):
             # drawn after everything else (the reverse layers included): every other configuration keeps its initial weights
             self.attention = Attention(head_in, cfg.attention_units, init_std=cfg.init_std, scaled=cfg.init == "scaled",
                                        device=device, generator=generator)
+        self.vocab_size = int(getattr(cfg, "vocab_size", 0) or 0)
+        self.embedding: Optional[Embedding] = None
+        if self.vocab_size > 0:
+            # drawn last (after the reverse layers and the attention weights): every run without it keeps its initial weights
+            self.embedding = Embedding(self.vocab_size, cfg.in_features, init_std=cfg.init_std, device=device, generator=generator)
         self.flat: Optional[FlatParams] = None
         self._allocator = allocator
         self.compute_dtype = torch.float32
@@ -96,20 +114,35 @@ class SequenceClassifier(nn.Module):
                 # the CUDA ops write these gradients straight into the flat buffer (first write of a step overwrites):
                 # zero_grad() then has nothing to memset
                 self.flat.enable_direct_grads(self.rnn.averaged_parameters() + [self.head.weights, self.head.bias] +
-                                              ([] if self.attention is None else list(self.attention.params())))
+                                              ([] if self.attention is None else list(self.attention.params())) +
+                                              ([] if self.embedding is None else [self.embedding.weights]))
+
+    def _is_sequence(self, x: torch.Tensor) -> bool:
+        """Whole sequences: ``[B,T,D]`` features, or ``[B,T]`` token ids with ``--vocab_size``."""
+        return x.dim() == (2 if self.embedding is not None else 3)
+
+    def _input(self, x: torch.Tensor, lengths: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """What the stack reads, batch-major: the features in the compute dtype, or with ``--vocab_size`` the embedded tokens
+        (``[B,T,E]``, a view of the time-major ``[T,B,E]`` the embedding writes; ``[B,E]`` for one-step ``[B]`` tokens)."""
+        if self.embedding is None:
+            return x.to(self.compute_dtype) if x.is_floating_point() else x
+        if x.is_floating_point() or x.dim() not in (1, 2):
+            raise ValueError(f"--vocab_size needs integer token ids [B,T] (one step: [B]), got {x.dtype} {tuple(x.shape)}")
+        e = self.embedding(x, lengths if x.dim() == 2 else None, self.compute_dtype)
+        return e[0] if x.dim() == 1 else e.transpose(0, 1)
 
     def features(self, x: torch.Tensor, lengths: Optional[torch.Tensor] = None) -> torch.Tensor:
         """``lengths``: optional int32 ``[B]`` per-sample sequence lengths (right-padded ``x``).  The top layer's last state, or
         with ``--pooling mean | max | attention`` its outputs pooled over each sample's steps (``ops.reference.pool_sequence``),
-        rounded once to the compute dtype."""
+        rounded once to the compute dtype.  With ``--vocab_size`` ``x`` holds token ids (``[B,T]``, or ``[B]`` for one step)."""
         if self.pooling != "last":
-            if x.dim() != 3:
-                raise ValueError(f"--pooling {self.pooling} needs sequences [B,T,D], got {tuple(x.shape)}")
+            if not self._is_sequence(x):
+                raise ValueError(f"--pooling {self.pooling} needs sequences [B,T,D] (token ids: [B,T]), got {tuple(x.shape)}")
             h_seq = self.sequence_features(x, lengths)
             s = F.pool_sequence(h_seq, lengths, self.pooling, None if self.attention is None else self.attention.params())
             return s.to(h_seq.dtype)
         self.rnn.reset_state(x.shape[0])
-        return self.rnn.fit_layers(x.to(self.compute_dtype) if x.is_floating_point() else x, lengths=lengths)
+        return self.rnn.fit_layers(self._input(x, lengths), lengths=lengths)
 
     def check_labels(self, labels: torch.Tensor) -> None:
         """``[B]`` labels classify whole sequences, ``[B,T]`` label every step (``--per_step_labels``): the wrong one is an error."""
@@ -124,11 +157,11 @@ class SequenceClassifier(nn.Module):
 
     def sequence_features(self, x: torch.Tensor, lengths: Optional[torch.Tensor] = None) -> torch.Tensor:
         """The top layer's whole output ``[T,B,H_last]`` (bidirectional ``[T,B,2 H_last]``) of ``x [B,T,D]``."""
-        if x.dim() != 3:
+        if not self._is_sequence(x):
             flag = "--per_step_labels" if self.per_step else f"--pooling {self.pooling}"
-            raise ValueError(f"{flag} needs sequences [B,T,D], got {tuple(x.shape)}")
+            raise ValueError(f"{flag} needs sequences [B,T,D] (token ids: [B,T]), got {tuple(x.shape)}")
         self.rnn.reset_state(x.shape[0])
-        return self.rnn.fit_sequence_all(x.to(self.compute_dtype) if x.is_floating_point() else x, lengths=lengths)
+        return self.rnn.fit_sequence_all(self._input(x, lengths), lengths=lengths)
 
     def forward(self, x: torch.Tensor, labels: torch.Tensor, lengths: Optional[torch.Tensor] = None):
         """-> (loss, logits, correct_count); with ``--per_step_labels`` logits are ``[B,T,C]`` and the loss and the count run over
@@ -162,7 +195,24 @@ class SequenceClassifier(nn.Module):
             out.append(("Attention/weights", self.attention.weights))
             out.append(("Attention/bias", self.attention.bias))
             out.append(("Attention/context", self.attention.context))
+        if self.embedding is not None:
+            out.append(("Embedding/weights", self.embedding.weights))
         return out
+
+    def check_vocab(self, variables: Dict[str, torch.Tensor], recorded: Optional[int] = None, what: str = "checkpoint") -> None:
+        """Raise unless ``variables`` (and the vocabulary ``recorded`` beside them; nothing recorded: the table's row count, or 0
+        without a table) were written with this model's ``--vocab_size``: a checkpoint loads with ``strict=False`` and would
+        otherwise drop or leave behind the embedding table, or read ids against another vocabulary."""
+        table = variables.get("Embedding/weights")
+        saved = int(recorded) if recorded is not None else (0 if table is None else int(table.shape[0]))
+        has_table = table is not None
+        if saved == self.vocab_size and has_table == (self.vocab_size > 0) \
+                and (table is None or int(table.shape[0]) == self.vocab_size):
+            return
+        desc = f"--vocab_size {saved}" if has_table == (saved > 0) else \
+            f"--vocab_size {saved} ({'with' if has_table else 'without'} an Embedding/weights table)"
+        raise ValueError(f"{what} was written with {desc}, this run uses --vocab_size {self.vocab_size}: "
+                         f"pass the --vocab_size it was trained with")
 
     def check_directions(self, variables: Dict[str, torch.Tensor], what: str = "checkpoint") -> None:
         """A checkpoint loads with ``strict=False``: a unidirectional one would leave a bidirectional model's reverse weights at

@@ -284,6 +284,24 @@ def pool_sequence(h_seq, lengths=None, mode: str = "mean", attention=None):
     raise ValueError(f"unknown pooling {mode!r}: one of {', '.join(POOLING_MODES)}")
 
 
+def embedding(tokens, table, lengths=None):
+    """Token embedding in front of the first layer (``--vocab_size``): ``nn.Embedding`` read time-major.  ``tokens`` int ``[B,T]``
+    (or ``[B]``, one step), ``table [V,E]``, ``lengths`` optional int ``[B]`` -> ``x [T,B,E]`` of the table's dtype with
+    ``x[t,b] = table[tokens[b,t]]`` at counted positions (``t < lengths[b]``, id in ``[0, V)``) and 0 elsewhere.  Uncounted
+    positions give the table no gradient; a counted one adds its ``dx`` to its id's row."""
+    tok = tokens.long()
+    if tok.dim() == 1:
+        tok = tok.unsqueeze(1)
+    tok = tok.t()                                                    # [T,B]
+    T, B = tok.shape
+    V = table.shape[0]
+    keep = (tok >= 0) & (tok < V)
+    if lengths is not None:
+        keep = keep & (torch.arange(T, device=tok.device).unsqueeze(1) < lengths.to(tok.device).long().unsqueeze(0))
+    rows = table[torch.where(keep, tok, torch.zeros_like(tok))]       # [T,B,E]
+    return rows * keep.unsqueeze(2).to(table.dtype)
+
+
 def clip_coefficient(g_total_segments, max_norm: float):
     """Clipping by the global norm (``torch.nn.utils.clip_grad_norm_``): ``norm = ||g_total||_2`` over all segments, summed in
     fp64 and rounded to the segments' dtype, and ``coef = min(max_norm / (norm + 1e-6), 1)`` in that dtype (a NaN norm gives a

@@ -108,6 +108,10 @@ def train_rnn(partition, cfg: Config, rank: int = 0, world_size: int = 1, comm: 
     if isinstance(rows, tuple):
         train_x, train_y = rows[0], rows[1]
         train_lengths = rows[2] if len(rows) > 2 else None
+    elif cfg.vocab_size > 0:
+        parsed = _parse_tokens(cfg, rows)
+        train_x, train_y = parsed[0], parsed[1]
+        train_lengths = parsed[2] if cfg.variable_length else None
     elif cfg.per_step_labels:
         parsed = D.process_batch_per_step(rows, cfg.seq_len, cfg.in_features, cfg.num_classes,
                                           variable_length=cfg.variable_length, normalize=cfg.normalize)
@@ -135,12 +139,13 @@ def train_rnn(partition, cfg: Config, rank: int = 0, world_size: int = 1, comm: 
     sink = M.SummarySink(os.path.join(model_save_dir, "train"))
     jlog = M.JsonLog(cfg.json_log)
 
+    x_dtype = _input_dtype(cfg)                      # token ids stay int32 (4 B per position on the host -> device copy)
     if cfg.data_residency == "host":
         # the reference's feed (src/rnn.py:264-267: every batch travels host -> device), as an asynchronous DMA pipeline
-        loader = D.PinnedHostLoader(train_x, train_y, batch_size, device, dtype=torch.float32, shuffle=True,
+        loader = D.PinnedHostLoader(train_x, train_y, batch_size, device, dtype=x_dtype, shuffle=True,
                                     seed=cfg.seed + 17 * (rank + 1), depth=3, lengths=train_lengths)
     else:
-        loader = D.DeviceShard(train_x, train_y, batch_size, device, dtype=torch.float32, shuffle=True,
+        loader = D.DeviceShard(train_x, train_y, batch_size, device, dtype=x_dtype, shuffle=True,
                                seed=cfg.seed + 17 * (rank + 1), lengths=train_lengths)
     start_step = 0
     if cfg.resume or cfg.use_pretrained_model:
@@ -153,6 +158,7 @@ def train_rnn(partition, cfg: Config, rank: int = 0, world_size: int = 1, comm: 
             variables, meta, opt_state = ckpt.load(src)
             model.check_directions(variables, f"checkpoint {src}")
             model.check_pooling(variables, (meta.get("config") or {}).get("pooling"), f"checkpoint {src}")
+            model.check_vocab(variables, (meta.get("config") or {}).get("vocab_size"), f"checkpoint {src}")
             model.load_reference_state_dict(variables, strict=False)
             eng.flat.refresh_shadow()
             if opt_state is not None:
@@ -356,11 +362,28 @@ def resolve_workers(cfg: Config, standalone: bool) -> int:
     return max(1, min(cfg.partitions, cap))
 
 
+def _input_dtype(cfg: Config) -> torch.dtype:
+    return torch.int32 if cfg.vocab_size > 0 else torch.float32
+
+
+def _parse_tokens(cfg: Config, rows):
+    return D.process_tokens(rows, cfg.seq_len, cfg.vocab_size, cfg.num_classes, variable_length=cfg.variable_length,
+                            per_step_labels=cfg.per_step_labels)
+
+
+def _synthetic_tokens(cfg: Config, n: int, seed: int):
+    return D.synthetic_tokens(n, cfg.seq_len, cfg.vocab_size, cfg.num_classes, seed=seed, variable_length=cfg.variable_length,
+                              per_step_labels=cfg.per_step_labels)
+
+
 def load_shards(cfg: Config, world_size: int, standalone: bool):
     if cfg.synthetic:
         n_per = cfg.synthetic // world_size
         shards = []
         for r in range(world_size):
+            if cfg.vocab_size > 0:
+                shards.append((r, _synthetic_tokens(cfg, n_per, cfg.seed + r)))
+                continue
             if cfg.per_step_labels:
                 shards.append((r, D.synthetic_per_step(n_per, cfg.seq_len, cfg.in_features, cfg.num_classes, seed=cfg.seed + r,
                                                        variable_length=cfg.variable_length)))
@@ -375,7 +398,8 @@ def load_shards(cfg: Config, world_size: int, standalone: bool):
 
 def _find_trained_model(cfg: Config, standalone: bool):
     """--resume <file | dir>, else <output_path>/averaged_model.pt (distributed job), else the latest checkpoint under
-    --checkpoint_path.  -> (variables in the reference's names, description, the --pooling the file records or None)."""
+    --checkpoint_path.  -> (variables in the reference's names, description, the --pooling and the --vocab_size the file
+    records, each or None)."""
     src = cfg.resume
     if not src and not standalone and cfg.output_path and os.path.isfile(os.path.join(cfg.output_path, "averaged_model.pt")):
         src = os.path.join(cfg.output_path, "averaged_model.pt")
@@ -385,14 +409,16 @@ def _find_trained_model(cfg: Config, standalone: bool):
         src = os.path.join(src, "averaged_model.pt")
     if src and os.path.isfile(src) and src.endswith(".pt"):
         blob = torch.load(src, map_location="cpu", weights_only=False)
-        return blob["variables"], src, (blob.get("meta") or {}).get("pooling")
+        meta = blob.get("meta") or {}
+        return blob["variables"], src, meta.get("pooling"), meta.get("vocab_size")
     if src and os.path.isdir(src):
         if ckpt.latest_checkpoint(src) is None and os.path.isdir(os.path.join(src, "0")):
             src = os.path.join(src, "0")
         last = ckpt.latest_checkpoint(src)
         if last:
             variables, meta, _ = ckpt.load(last)
-            return variables, last, (meta.get("config") or {}).get("pooling")
+            recorded = meta.get("config") or {}
+            return variables, last, recorded.get("pooling"), recorded.get("vocab_size")
     raise FileNotFoundError("--mode eval: no trained model found (give --resume <averaged_model.pt | checkpoint dir>)")
 
 
@@ -401,9 +427,14 @@ def evaluate_job(cfg: Config, standalone: bool = False) -> Dict:
     file in batches of ``--batch_size``, forward kernels only, one device.  Not in the reference (its ``--mode`` flag knows
     only ``train`` and the averaged model is thrown away, src/rnn.py:371,407-408); it closes the train -> average -> use loop."""
     from .engine import TrainEngine
-    variables, src, pooling = _find_trained_model(cfg, standalone)
+    variables, src, pooling, vocab = _find_trained_model(cfg, standalone)
     lengths = None
-    if cfg.synthetic and cfg.per_step_labels:
+    if cfg.vocab_size > 0:
+        data = _synthetic_tokens(cfg, cfg.synthetic, cfg.seed) if cfg.synthetic else \
+            _parse_tokens(cfg, D.read_dataset_from_path(cfg.training_path))
+        x, y = data[0], data[1]
+        lengths = data[2] if cfg.variable_length else None
+    elif cfg.synthetic and cfg.per_step_labels:
         data = D.synthetic_per_step(cfg.synthetic, cfg.seq_len, cfg.in_features, cfg.num_classes, seed=cfg.seed,
                                     variable_length=cfg.variable_length)
         x, y = data[0], data[1]
@@ -437,13 +468,14 @@ def evaluate_job(cfg: Config, standalone: bool = False) -> Dict:
     variables = dict(variables)
     eng.model.check_directions(variables, f"model {src}")
     eng.model.check_pooling(variables, pooling, f"model {src}")
+    eng.model.check_vocab(variables, vocab, f"model {src}")       # before the row averaging below, which must never touch the table
     for k, v in list(variables.items()):
         want = shapes.get(k)
-        if want is not None and tuple(v.shape) != want and v.dim() == 2 and len(want) == 2 and v.shape[1] == want[1]:
+        if k != "Embedding/weights" and want is not None and tuple(v.shape) != want and v.dim() == 2 and len(want) == 2 and v.shape[1] == want[1]:
             variables[k] = v.float().mean(0, keepdim=True).expand(want).contiguous()
     eng.model.load_reference_state_dict(variables, strict=False)
     eng.flat.refresh_shadow()
-    xs = torch.as_tensor(x).to(device=device, dtype=torch.float32)
+    xs = torch.as_tensor(x).to(device=device, dtype=_input_dtype(cfg))
     ys = torch.as_tensor(y).to(device)
     ls = None if lengths is None else torch.as_tensor(lengths).to(device=device, dtype=torch.int32)
     sl = lambda a, b: None if ls is None else ls[a:b]
@@ -527,7 +559,8 @@ def run_job(cfg: Config, standalone: bool = False) -> Dict:
         ckpt.save_averaged_model(cfg.output_path, res0["records"], res0["variables"],
                                  {"world_size": world_size, "sync_mode": cfg.sync_mode, "average_scope": cfg.average_scope,
                                   "hidden_units": cfg.hidden_units, "pooling": cfg.pooling,
-                                  "attention_units": cfg.attention_units, "seconds": total})
+                                  "attention_units": cfg.attention_units, "vocab_size": cfg.vocab_size,
+                                  "seconds": total})
     if not cfg.quiet:
         print("RNN-LSTM - Total Processing Time {}s".format(total))
     return {"results": results, "seconds": total, "world_size": world_size, "partitions": n_shards}
