@@ -139,6 +139,13 @@ def process_batch_ragged(train_xy: Sequence[Sequence[str]], seq_len: int, in_fea
         xs.append([float(v) for v in row[:-1]])
         ys.append(int(float(row[-1])))
         ls.append(width // in_features)
+    x = _pad_steps(xs, ls, seq_len, in_features, normalize)
+    return x, np.asarray(ys, dtype=np.int64), np.asarray(ls, dtype=np.int32)
+
+
+def _pad_steps(xs, ls, seq_len: int, in_features: int, normalize: bool) -> np.ndarray:
+    """Rows of ``ls[i] * in_features`` values -> ``x float32 [N, seq_len, in_features]``, zero-padded on the right.
+    ``normalize``: global min-max over the real values only (padding excluded)."""
     if not xs:
         raise ValueError("empty partition: no parsable rows")
     if normalize:
@@ -148,7 +155,7 @@ def process_batch_ragged(train_xy: Sequence[Sequence[str]], seq_len: int, in_fea
     x = np.zeros((len(xs), seq_len, in_features), dtype=np.float32)
     for i, r in enumerate(xs):
         x[i, :ls[i]] = np.asarray(r, dtype=np.float32).reshape(ls[i], in_features)
-    return x, np.asarray(ys, dtype=np.int64), np.asarray(ls, dtype=np.int32)
+    return x
 
 
 def process_batch_per_step(train_xy: Sequence[Sequence[str]], seq_len: int, in_features: int, num_classes: int,
@@ -178,17 +185,10 @@ def process_batch_per_step(train_xy: Sequence[Sequence[str]], seq_len: int, in_f
         xs.append([float(v) for v in row[:k * in_features]])
         ys.append(lab)
         ls.append(k)
-    if not xs:
-        raise ValueError("empty partition: no parsable rows")
-    if normalize:
-        flat = min_max_normalizer(np.concatenate([np.asarray(r, dtype=np.float64) for r in xs]))
-        off = np.cumsum([0] + [len(r) for r in xs])
-        xs = [flat[off[i]:off[i + 1]] for i in range(len(xs))]
-    x = np.zeros((len(xs), seq_len, in_features), dtype=np.float32)
+    x = _pad_steps(xs, ls, seq_len, in_features, normalize)
     y = np.zeros((len(xs), seq_len), dtype=np.int64)
-    for i, r in enumerate(xs):
-        x[i, :ls[i]] = np.asarray(r, dtype=np.float32).reshape(ls[i], in_features)
-        y[i, :ls[i]] = ys[i]
+    for i, lab in enumerate(ys):
+        y[i, :ls[i]] = lab
     if variable_length:
         return x, y, np.asarray(ls, dtype=np.int32)
     return x, y
@@ -248,6 +248,27 @@ def process_tokens(train_xy: Sequence[Sequence[str]], seq_len: int, vocab_size: 
     if variable_length:
         return x, y, np.asarray(ls, dtype=np.int32)
     return x, y
+
+
+def parse_rows(rows: Sequence[Sequence[str]], cfg):
+    """Rows -> ``(x, y, lengths)`` by the parser the flags of ``cfg`` select (``--vocab_size``, ``--per_step_labels``,
+    ``--variable_length``); ``lengths`` is None unless ``cfg.variable_length``."""
+    if cfg.vocab_size > 0:
+        x, y, *lengths = process_tokens(rows, cfg.seq_len, cfg.vocab_size, cfg.num_classes,
+                                        variable_length=cfg.variable_length, per_step_labels=cfg.per_step_labels)
+    elif cfg.per_step_labels:
+        x, y, *lengths = process_batch_per_step(rows, cfg.seq_len, cfg.in_features, cfg.num_classes,
+                                                variable_length=cfg.variable_length, normalize=cfg.normalize)
+    elif cfg.variable_length:
+        x, y, *lengths = process_batch_ragged(rows, cfg.seq_len, cfg.in_features, normalize=cfg.normalize)
+    else:
+        x, y, *lengths = process_batch(rows, normalize=cfg.normalize, seq_len=cfg.seq_len, in_features=cfg.in_features)
+    return x, y, (lengths[0] if lengths else None)
+
+
+def input_dtype(cfg) -> torch.dtype:
+    """The dtype ``x`` goes to the device in: token ids stay int32 (4 B per position on the host -> device copy)."""
+    return torch.int32 if cfg.vocab_size > 0 else torch.float32
 
 
 def resolve_batch_size(batch_size: int, shard_rows: int) -> int:
@@ -367,6 +388,21 @@ def synthetic_lengths(n: int, seq_len: int, seed: int = 0) -> np.ndarray:
     """Per-sample lengths, uniform in ``[max(1, seq_len // 4), seq_len]``, int32, from a generator seeded apart from the data's."""
     rng = np.random.default_rng([seed, 0x6C656E])
     return rng.integers(max(1, seq_len // 4), seq_len + 1, size=n).astype(np.int32)
+
+
+def synthetic(cfg, n: int, seed: int):
+    """``n`` synthetic samples of the task the flags of ``cfg`` select -> ``(x, y, lengths)``; ``lengths`` is None unless
+    ``cfg.variable_length``."""
+    if cfg.vocab_size > 0:
+        x, y, *lengths = synthetic_tokens(n, cfg.seq_len, cfg.vocab_size, cfg.num_classes, seed=seed,
+                                          variable_length=cfg.variable_length, per_step_labels=cfg.per_step_labels)
+    elif cfg.per_step_labels:
+        x, y, *lengths = synthetic_per_step(n, cfg.seq_len, cfg.in_features, cfg.num_classes, seed=seed,
+                                            variable_length=cfg.variable_length)
+    else:
+        x, y, *lengths = synthetic_sequences(n, cfg.seq_len, cfg.in_features, cfg.num_classes, seed=seed,
+                                             variable_length=cfg.variable_length)
+    return x, y, (lengths[0] if lengths else None)
 
 
 # ------------------------------------------------------------------------------------------------

@@ -297,12 +297,7 @@ class TrainEngine:
         was_training = self.model.training
         self.model.eval()
         try:
-            if self.model.per_step:
-                loss, correct, n = self.model.score_per_step(x, y, lengths)
-                return loss, correct.float() / n.float()
-            h = self.model.features(x, lengths)
-            logits = self.model.head(h)
+            loss, correct, count = self.model.score(x, y, lengths)
         finally:
             self.model.train(was_training)
-        from .ops import reference as ref
-        return ref.softmax_xent(logits, y), ref.accuracy(logits, y)
+        return loss, correct.float() / count.float()

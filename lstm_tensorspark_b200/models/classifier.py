@@ -175,14 +175,25 @@ class SequenceClassifier(nn.Module):
         logits, loss, correct = F.head_xent(h, self.head.weights, self.head.bias, labels)
         return loss, logits, correct
 
-    def score_per_step(self, x: torch.Tensor, labels: torch.Tensor, lengths: Optional[torch.Tensor] = None):
-        """Per-step evaluation without gradients (call in eval mode): -> (mean loss, correct count, N) over the counted
-        positions, device tensors (no host sync)."""
+    @torch.no_grad()
+    def score(self, x: torch.Tensor, labels: torch.Tensor, lengths: Optional[torch.Tensor] = None, first: int = 0):
+        """Evaluation without gradients (call in eval mode): -> (mean loss, correct count, count) over rows ``first:`` of the
+        batch, device tensors (no host sync).  The count is of the counted positions with ``--per_step_labels``, of the rows
+        otherwise.  The whole batch runs through the stack, so a tail can be scored in a batch of the usual static shape."""
+        from ..ops import reference as ref
         self.check_labels(labels)
-        with torch.no_grad():
+        labels = labels[first:]
+        if self.per_step:
             h_seq = self.sequence_features(x, lengths)
-            _logits, loss, correct, n = F.head_xent_per_step(h_seq, self.head.weights, self.head.bias, labels, lengths)
-        return loss, correct, n
+            if first == 0:
+                _logits, loss, correct, n = F.head_xent_per_step(h_seq, self.head.weights, self.head.bias, labels, lengths)
+                return loss, correct, n
+            h_seq = h_seq[:, first:]
+            logits = self.head(h_seq.reshape(-1, h_seq.shape[2])).float().view(h_seq.shape[0], h_seq.shape[1], -1)
+            return ref.softmax_xent_per_step(logits.transpose(0, 1), labels, None if lengths is None else lengths[first:])
+        logits = self.head(self.features(x, lengths))[first:].float()
+        count = torch.full((), labels.shape[0], dtype=torch.int64, device=logits.device)
+        return ref.softmax_xent(logits, labels), (logits.argmax(1) == labels).sum(), count
 
     # ---- reference variable naming ------------------------------------------------
     def named_reference_variables(self) -> List[Tuple[str, torch.Tensor]]:
@@ -198,6 +209,14 @@ class SequenceClassifier(nn.Module):
         if self.embedding is not None:
             out.append(("Embedding/weights", self.embedding.weights))
         return out
+
+    def check_compatible(self, variables: Dict[str, torch.Tensor], settings: Dict, what: str = "checkpoint") -> None:
+        """Raise unless ``variables`` and the flags ``settings`` recorded beside them (``utils.checkpoint.recorded_settings``)
+        were written by a model this one can load: the same directions, ``--pooling`` and ``--vocab_size``, checked in that
+        order."""
+        self.check_directions(variables, what)
+        self.check_pooling(variables, settings.get("pooling"), what)
+        self.check_vocab(variables, settings.get("vocab_size"), what)
 
     def check_vocab(self, variables: Dict[str, torch.Tensor], recorded: Optional[int] = None, what: str = "checkpoint") -> None:
         """Raise unless ``variables`` (and the vocabulary ``recorded`` beside them; nothing recorded: the table's row count, or 0

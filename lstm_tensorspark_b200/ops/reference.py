@@ -244,11 +244,11 @@ def head_xent_per_step(h_seq, weights, bias, labels, lengths=None):
 
 
 def softmax_xent_per_step(logits, labels, lengths=None):
-    """``logits [B,T,C]``, ``labels [B,T]`` -> (mean NLL over counted positions, accuracy over them, N)."""
+    """``logits [B,T,C]``, ``labels [B,T]`` -> (mean NLL over counted positions, correct count among them, N)."""
     keep = step_mask(lengths, logits.shape[0], logits.shape[1], device=logits.device)
     lg, lab = logits[keep].float(), labels.to(logits.device)[keep].long()
     n = keep.sum()
-    return (torch.nn.functional.cross_entropy(lg, lab, reduction="sum") / n, (lg.argmax(1) == lab).float().sum() / n, n)
+    return torch.nn.functional.cross_entropy(lg, lab, reduction="sum") / n, (lg.argmax(1) == lab).sum(), n
 
 
 POOLING_MODES = ("last", "mean", "max", "attention")

@@ -26,7 +26,7 @@ from .config import Config
 from .models.classifier import SequenceClassifier
 from .models.recurrent.lstm import clear_weight_decay_collection
 from .ops import functional as F
-from .ops.loss import compute_accuracy, compute_loss, report_accuracy, report_loss
+from .ops.loss import report_accuracy, report_loss
 from .ops.optim import FlatOptimizer
 from .parallel.comm import Communicator, make_communicator
 from .utils import checkpoint as ckpt
@@ -104,24 +104,11 @@ def train_rnn(partition, cfg: Config, rank: int = 0, world_size: int = 1, comm: 
     dtype = resolve_dtype(cfg, device)
     F.set_backend(cfg.backend if cfg.backend != "auto" else "auto")
 
-    train_lengths = None
     if isinstance(rows, tuple):
         train_x, train_y = rows[0], rows[1]
         train_lengths = rows[2] if len(rows) > 2 else None
-    elif cfg.vocab_size > 0:
-        parsed = _parse_tokens(cfg, rows)
-        train_x, train_y = parsed[0], parsed[1]
-        train_lengths = parsed[2] if cfg.variable_length else None
-    elif cfg.per_step_labels:
-        parsed = D.process_batch_per_step(rows, cfg.seq_len, cfg.in_features, cfg.num_classes,
-                                          variable_length=cfg.variable_length, normalize=cfg.normalize)
-        train_x, train_y = parsed[0], parsed[1]
-        train_lengths = parsed[2] if cfg.variable_length else None
-    elif cfg.variable_length:
-        train_x, train_y, train_lengths = D.process_batch_ragged(rows, cfg.seq_len, cfg.in_features, normalize=cfg.normalize)
     else:
-        train_x, train_y = D.process_batch(rows, normalize=cfg.normalize, seq_len=cfg.seq_len,
-                                           in_features=cfg.in_features)
+        train_x, train_y, train_lengths = D.parse_rows(rows, cfg)
     batch_size = D.resolve_batch_size(cfg.batch_size, train_x.shape[0])
 
     # ---- model + optimizer + sync = one TrainEngine (the same object bench.py drives) ----------------------
@@ -139,7 +126,7 @@ def train_rnn(partition, cfg: Config, rank: int = 0, world_size: int = 1, comm: 
     sink = M.SummarySink(os.path.join(model_save_dir, "train"))
     jlog = M.JsonLog(cfg.json_log)
 
-    x_dtype = _input_dtype(cfg)                      # token ids stay int32 (4 B per position on the host -> device copy)
+    x_dtype = D.input_dtype(cfg)
     if cfg.data_residency == "host":
         # the reference's feed (src/rnn.py:264-267: every batch travels host -> device), as an asynchronous DMA pipeline
         loader = D.PinnedHostLoader(train_x, train_y, batch_size, device, dtype=x_dtype, shuffle=True,
@@ -156,9 +143,7 @@ def train_rnn(partition, cfg: Config, rank: int = 0, world_size: int = 1, comm: 
             src = ckpt.latest_checkpoint(src)
         if src:
             variables, meta, opt_state = ckpt.load(src)
-            model.check_directions(variables, f"checkpoint {src}")
-            model.check_pooling(variables, (meta.get("config") or {}).get("pooling"), f"checkpoint {src}")
-            model.check_vocab(variables, (meta.get("config") or {}).get("vocab_size"), f"checkpoint {src}")
+            model.check_compatible(variables, ckpt.recorded_settings(meta), f"checkpoint {src}")
             model.load_reference_state_dict(variables, strict=False)
             eng.flat.refresh_shadow()
             if opt_state is not None:
@@ -244,15 +229,10 @@ def train_rnn(partition, cfg: Config, rank: int = 0, world_size: int = 1, comm: 
                            opt_state={"optimizer": comm.optimizer_state(optimizer), "loader": loader.state_dict()})
                 model.eval()                                         # no dropout while scoring
                 with torch.no_grad(), M.capture(sink):
-                    if model.per_step:                               # over the counted positions of the batch
-                        xent, ok, n = model.score_per_step(train_input, train_labels, batch_lengths)
-                        e_loss = report_loss(xent)
-                        e_acc = report_accuracy(ok.float() / n.float())
-                    else:
-                        h = model.features(train_input, batch_lengths)   # same batch, from the initial state (src/rnn.py:276-279)
-                        logits = model.head(h)
-                        e_loss = compute_loss(labels=train_labels, logits=logits)
-                        e_acc = compute_accuracy(labels=train_labels, logits=logits)
+                    # same batch, from the initial state (src/rnn.py:276-279)
+                    xent, ok, n = model.score(train_input, train_labels, batch_lengths)
+                    e_loss = report_loss(xent)
+                    e_acc = report_accuracy(ok.float() / n.float())
                 model.train()
                 t_loss, t_acc = float(e_loss.item()), float(e_acc.item())
                 extra = {}
@@ -362,35 +342,9 @@ def resolve_workers(cfg: Config, standalone: bool) -> int:
     return max(1, min(cfg.partitions, cap))
 
 
-def _input_dtype(cfg: Config) -> torch.dtype:
-    return torch.int32 if cfg.vocab_size > 0 else torch.float32
-
-
-def _parse_tokens(cfg: Config, rows):
-    return D.process_tokens(rows, cfg.seq_len, cfg.vocab_size, cfg.num_classes, variable_length=cfg.variable_length,
-                            per_step_labels=cfg.per_step_labels)
-
-
-def _synthetic_tokens(cfg: Config, n: int, seed: int):
-    return D.synthetic_tokens(n, cfg.seq_len, cfg.vocab_size, cfg.num_classes, seed=seed, variable_length=cfg.variable_length,
-                              per_step_labels=cfg.per_step_labels)
-
-
 def load_shards(cfg: Config, world_size: int, standalone: bool):
     if cfg.synthetic:
-        n_per = cfg.synthetic // world_size
-        shards = []
-        for r in range(world_size):
-            if cfg.vocab_size > 0:
-                shards.append((r, _synthetic_tokens(cfg, n_per, cfg.seed + r)))
-                continue
-            if cfg.per_step_labels:
-                shards.append((r, D.synthetic_per_step(n_per, cfg.seq_len, cfg.in_features, cfg.num_classes, seed=cfg.seed + r,
-                                                       variable_length=cfg.variable_length)))
-                continue
-            shards.append((r, D.synthetic_sequences(n_per, cfg.seq_len, cfg.in_features, cfg.num_classes, seed=cfg.seed + r,
-                                                    variable_length=cfg.variable_length)))
-        return shards
+        return [(r, D.synthetic(cfg, cfg.synthetic // world_size, cfg.seed + r)) for r in range(world_size)]
     if standalone:
         return [(0, D.read_dataset_from_path(cfg.training_path))]
     return D.text_to_partitions(cfg.training_path, world_size, shuffle=True, seed=cfg.seed, remainder=cfg.remainder)
@@ -398,8 +352,8 @@ def load_shards(cfg: Config, world_size: int, standalone: bool):
 
 def _find_trained_model(cfg: Config, standalone: bool):
     """--resume <file | dir>, else <output_path>/averaged_model.pt (distributed job), else the latest checkpoint under
-    --checkpoint_path.  -> (variables in the reference's names, description, the --pooling and the --vocab_size the file
-    records, each or None)."""
+    --checkpoint_path.  -> (variables in the reference's names, description, the flags the file records
+    (``utils.checkpoint.recorded_settings``))."""
     src = cfg.resume
     if not src and not standalone and cfg.output_path and os.path.isfile(os.path.join(cfg.output_path, "averaged_model.pt")):
         src = os.path.join(cfg.output_path, "averaged_model.pt")
@@ -409,16 +363,14 @@ def _find_trained_model(cfg: Config, standalone: bool):
         src = os.path.join(src, "averaged_model.pt")
     if src and os.path.isfile(src) and src.endswith(".pt"):
         blob = torch.load(src, map_location="cpu", weights_only=False)
-        meta = blob.get("meta") or {}
-        return blob["variables"], src, meta.get("pooling"), meta.get("vocab_size")
+        return blob["variables"], src, ckpt.recorded_settings(blob.get("meta") or {})
     if src and os.path.isdir(src):
         if ckpt.latest_checkpoint(src) is None and os.path.isdir(os.path.join(src, "0")):
             src = os.path.join(src, "0")
         last = ckpt.latest_checkpoint(src)
         if last:
             variables, meta, _ = ckpt.load(last)
-            recorded = meta.get("config") or {}
-            return variables, last, recorded.get("pooling"), recorded.get("vocab_size")
+            return variables, last, ckpt.recorded_settings(meta)
     raise FileNotFoundError("--mode eval: no trained model found (give --resume <averaged_model.pt | checkpoint dir>)")
 
 
@@ -427,34 +379,9 @@ def evaluate_job(cfg: Config, standalone: bool = False) -> Dict:
     file in batches of ``--batch_size``, forward kernels only, one device.  Not in the reference (its ``--mode`` flag knows
     only ``train`` and the averaged model is thrown away, src/rnn.py:371,407-408); it closes the train -> average -> use loop."""
     from .engine import TrainEngine
-    variables, src, pooling, vocab = _find_trained_model(cfg, standalone)
-    lengths = None
-    if cfg.vocab_size > 0:
-        data = _synthetic_tokens(cfg, cfg.synthetic, cfg.seed) if cfg.synthetic else \
-            _parse_tokens(cfg, D.read_dataset_from_path(cfg.training_path))
-        x, y = data[0], data[1]
-        lengths = data[2] if cfg.variable_length else None
-    elif cfg.synthetic and cfg.per_step_labels:
-        data = D.synthetic_per_step(cfg.synthetic, cfg.seq_len, cfg.in_features, cfg.num_classes, seed=cfg.seed,
-                                    variable_length=cfg.variable_length)
-        x, y = data[0], data[1]
-        lengths = data[2] if cfg.variable_length else None
-    elif cfg.per_step_labels:
-        data = D.process_batch_per_step(D.read_dataset_from_path(cfg.training_path), cfg.seq_len, cfg.in_features,
-                                        cfg.num_classes, variable_length=cfg.variable_length, normalize=cfg.normalize)
-        x, y = data[0], data[1]
-        lengths = data[2] if cfg.variable_length else None
-    elif cfg.synthetic:
-        data = D.synthetic_sequences(cfg.synthetic, cfg.seq_len, cfg.in_features, cfg.num_classes, seed=cfg.seed,
-                                     variable_length=cfg.variable_length)
-        x, y = data[0], data[1]
-        lengths = data[2] if cfg.variable_length else None
-    elif cfg.variable_length:
-        x, y, lengths = D.process_batch_ragged(D.read_dataset_from_path(cfg.training_path), cfg.seq_len, cfg.in_features,
-                                               normalize=cfg.normalize)
-    else:
-        rows = D.read_dataset_from_path(cfg.training_path)
-        x, y = D.process_batch(rows, normalize=cfg.normalize, seq_len=cfg.seq_len, in_features=cfg.in_features)
+    variables, src, settings = _find_trained_model(cfg, standalone)
+    x, y, lengths = D.synthetic(cfg, cfg.synthetic, cfg.seed) if cfg.synthetic else \
+        D.parse_rows(D.read_dataset_from_path(cfg.training_path), cfg)
     device = resolve_device(cfg, 0)
     dtype = resolve_dtype(cfg, device)
     F.set_backend(cfg.backend if cfg.backend != "auto" else "auto")
@@ -466,68 +393,32 @@ def evaluate_job(cfg: Config, standalone: bool = False) -> Dict:
     # scoring with another batch size uses the mean learned row for every sample
     shapes = {k: tuple(v.shape) for k, v in eng.model.named_reference_variables()}
     variables = dict(variables)
-    eng.model.check_directions(variables, f"model {src}")
-    eng.model.check_pooling(variables, pooling, f"model {src}")
-    eng.model.check_vocab(variables, vocab, f"model {src}")       # before the row averaging below, which must never touch the table
+    eng.model.check_compatible(variables, settings, f"model {src}")   # before the row averaging below, which must never touch the table
     for k, v in list(variables.items()):
         want = shapes.get(k)
         if k != "Embedding/weights" and want is not None and tuple(v.shape) != want and v.dim() == 2 and len(want) == 2 and v.shape[1] == want[1]:
             variables[k] = v.float().mean(0, keepdim=True).expand(want).contiguous()
     eng.model.load_reference_state_dict(variables, strict=False)
     eng.flat.refresh_shadow()
-    xs = torch.as_tensor(x).to(device=device, dtype=_input_dtype(cfg))
+    xs = torch.as_tensor(x).to(device=device, dtype=D.input_dtype(cfg))
     ys = torch.as_tensor(y).to(device)
     ls = None if lengths is None else torch.as_tensor(lengths).to(device=device, dtype=torch.int32)
-    sl = lambda a, b: None if ls is None else ls[a:b]
+    # full batches (static shapes for the kernels), then the tail as the last `bs` rows, counting only the ones not seen yet;
+    # --per_step_labels weighs each batch by its number of counted positions
+    windows = [(lo, 0) for lo in range(0, n - bs + 1, bs)] + ([(n - bs, bs - n % bs)] if n % bs else [])
+    loss_sum, correct, count = 0.0, 0, 0
+    start = time.time()
+    for lo, first in windows:
+        loss, ok, cnt = eng.model.score(xs[lo:lo + bs], ys[lo:lo + bs], None if ls is None else ls[lo:lo + bs], first)
+        loss_sum += float(loss) * int(cnt); correct += int(ok); count += int(cnt)
+    out = {"mode": "eval", "model": src, "samples": n}
     if eng.model.per_step:
-        return _evaluate_per_step(cfg, eng, src, xs, ys, ls, bs)
-    loss_sum, correct, seen = 0.0, 0.0, 0
-    start = time.time()
-    for lo in range(0, n - bs + 1, bs):                 # full batches (static shapes for the kernels); the tail is scored below
-        l, a = eng.evaluate(xs[lo:lo + bs], ys[lo:lo + bs], sl(lo, lo + bs))
-        loss_sum += float(l) * bs; correct += float(a) * bs; seen += bs
-    if seen < n:                                        # remainder: the last `bs` rows, counting only the ones not seen yet
-        from .ops import reference as ref
-        with torch.no_grad():
-            logits = eng.model.head(eng.model.features(xs[n - bs:], sl(n - bs, n)))[bs - (n - seen):]
-        tail_y = ys[seen:]
-        loss_sum += float(ref.softmax_xent(logits.float(), tail_y)) * (n - seen)
-        correct += float(ref.accuracy(logits.float(), tail_y)) * (n - seen)
-        seen = n
-    out = {"mode": "eval", "model": src, "samples": seen, "loss": loss_sum / seen, "accuracy": correct / seen,
-           "seconds": time.time() - start}
+        out["positions"] = count
+    out.update(loss=loss_sum / count, accuracy=correct / count, seconds=time.time() - start)
     if not cfg.quiet:
-        print("RNN-LSTM - eval: model {model}, {samples} samples, loss {loss:.6f}, accuracy {accuracy:.4f}".format(**out))
-    if cfg.json_log:
-        jl = M.JsonLog(cfg.json_log); jl.write(**out); jl.close()
-    return out
-
-
-def _evaluate_per_step(cfg: Config, eng, src: str, xs, ys, ls, bs: int) -> Dict:
-    """``--mode eval`` with ``--per_step_labels``: loss and accuracy over every counted position of the file, each batch weighted
-    by its number of positions.  The tail runs as the last ``bs`` rows (static shapes for the kernels), of which only the rows
-    not seen yet are scored."""
-    n = xs.shape[0]
-    sl = lambda a, b: None if ls is None else ls[a:b]
-    loss_sum, correct, positions = 0.0, 0.0, 0
-    start = time.time()
-    seen = 0
-    for lo in range(0, n - bs + 1, bs):
-        loss, ok, cnt = eng.model.score_per_step(xs[lo:lo + bs], ys[lo:lo + bs], sl(lo, lo + bs))
-        loss_sum += float(loss) * int(cnt); correct += float(ok); positions += int(cnt); seen += bs
-    if seen < n:                                        # remainder: score the tail rows alone, in one smaller batch
-        from .ops import reference as ref
-        with torch.no_grad():
-            h_seq = eng.model.sequence_features(xs[n - bs:], sl(n - bs, n))[:, bs - (n - seen):]
-            logits = eng.model.head(h_seq.reshape(-1, h_seq.shape[2])).float().view(h_seq.shape[0], n - seen, -1)
-        loss, acc, cnt = ref.softmax_xent_per_step(logits.transpose(0, 1), ys[seen:], sl(seen, n))
-        loss_sum += float(loss) * int(cnt); correct += float(acc) * int(cnt); positions += int(cnt)
-        seen = n
-    out = {"mode": "eval", "model": src, "samples": seen, "positions": positions, "loss": loss_sum / positions,
-           "accuracy": correct / positions, "seconds": time.time() - start}
-    if not cfg.quiet:
-        print("RNN-LSTM - eval: model {model}, {samples} samples, {positions} positions, loss {loss:.6f}, "
-              "accuracy {accuracy:.4f}".format(**out))
+        positions = "{positions} positions, " if eng.model.per_step else ""
+        print(("RNN-LSTM - eval: model {model}, {samples} samples, " + positions +
+               "loss {loss:.6f}, accuracy {accuracy:.4f}").format(**out))
     if cfg.json_log:
         jl = M.JsonLog(cfg.json_log); jl.write(**out); jl.close()
     return out

@@ -115,6 +115,12 @@ def load(prefix_path: str) -> Tuple[Dict[str, torch.Tensor], dict, Optional[dict
     return variables, meta, opt
 
 
+def recorded_settings(meta: dict) -> dict:
+    """The flags a model file recorded: a training checkpoint keeps them under ``meta["config"]``, ``averaged_model.pt`` keeps
+    the ones it records (``pooling``, ``vocab_size``, ...) at the top level of its meta."""
+    return meta.get("config") or meta
+
+
 def save_averaged_model(output_path: str, records, variables: Dict[str, torch.Tensor], meta: dict):
     """Write the cross-replica average to ``--output_path`` (the reference computes it and throws it away,
     src/rnn.py:407-408, Q12).  ``records`` = the 8 keyed ``map_data_by_key`` entries."""
