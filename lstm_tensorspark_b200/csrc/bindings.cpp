@@ -52,7 +52,7 @@ int ts_head_step_bwd(const void*, const float*, const float*, const float*, void
 int ts_gemm_generic(const void*, const void*, void*, const float*, int, int, int, long long, long long, long long, long long, long long,
                     int, int, int, float, cudaStream_t);
 int ts_gemm2(const void*, const void*, void*, const float*, int, int, int, int, int, int, int, int, int, int, int, int, int,
-             const unsigned int*, const int*, unsigned int*, int*, int, int, int, int, cudaStream_t);
+             const unsigned int*, const int*, unsigned int*, int*, int, int, int, int, float*, int, cudaStream_t);
 int ts_lstm_seq_fwd(const void*, const void*, const float*, const void*, const float*, void*, const float*, void*, void*, int,
                     int, int, unsigned int*, int, cudaStream_t, const void*, const unsigned int*, int, int, int, const int*, int,
                     void*, const int*, const unsigned int*);
@@ -568,10 +568,12 @@ void fused_allreduce(const Tensor& ptrs, int64_t mc_in, int64_t mc_param, int64_
 // ---- general wgmma GEMM (csrc/gemm2_wgmma.cu): C[M,N] (=|+=) op(A)·op(B) (+bias) ------------------------------------
 // a_mn = false: A is [M,K] (K contiguous); true: A is [K,M] (M contiguous).  b_mn = false: B is [N,K]; true: B is [K,N].
 // out: optional preallocated C (fp32 for accumulate = C += A·B, or any mode); out_fp32 selects the dtype of a fresh C.
+// rowsum: optional fp32 [M] that also receives the row sums of op(A) over K (overwritten, or accumulated with rowsum_acc).
 Tensor gemm2(const Tensor& A, const Tensor& B, const std::optional<Tensor>& bias, std::optional<Tensor> out, bool a_mn, bool b_mn,
              bool out_fp32, bool accumulate, int64_t ctas, int64_t bn, int64_t max_ctas, const std::optional<Tensor>& gate,
              const std::vector<int64_t>& gate_cfg, const std::optional<Tensor>& done, const std::optional<Tensor>& gate_err,
-             int64_t stream_handle, bool pdl, int64_t a_fold, int64_t b_fold, int64_t fold_cols) {
+             int64_t stream_handle, bool pdl, int64_t a_fold, int64_t b_fold, int64_t fold_cols, const std::optional<Tensor>& rowsum,
+             bool rowsum_acc) {
   // a_fold / b_fold: the operand is the 2-D storage view [fold, T * fold_cols] of a batch-major [fold, T, fold_cols] array that
   // is read as the time-major matrix [T * fold, fold_cols] (A: K-major, K = fold_cols;  B: MN-major, N = fold_cols)
   TORCH_CHECK(A.is_cuda() && B.is_cuda(), "gemm2: CUDA tensors");
@@ -603,12 +605,18 @@ Tensor gemm2(const Tensor& A, const Tensor& B, const std::optional<Tensor>& bias
     gp = (const unsigned int*)gate->data_ptr<int>();
     for (int i = 0; i < 7; ++i) gcfg[i] = (int)gate_cfg[i];
   }
+  float* rp = nullptr;
+  if (rowsum.has_value()) {
+    TORCH_CHECK(rowsum->is_cuda() && rowsum->scalar_type() == torch::kFloat32 && rowsum->is_contiguous() && rowsum->numel() == M &&
+                C.scalar_type() == torch::kFloat32, "gemm2: rowsum must be a contiguous fp32 [M] next to an fp32 output");
+    rp = rowsum->data_ptr<float>();
+  }
   unsigned int* dp = nullptr;
   if (done.has_value()) { TORCH_CHECK(done->is_cuda() && done->scalar_type() == torch::kInt32, "gemm2: done int32 cuda"); dp = (unsigned int*)done->data_ptr<int>(); }
   check(ts_gemm2(A.data_ptr(), B.data_ptr(), C.data_ptr(), fptr(bias), M, N, K, (int)A.stride(0), (int)B.stride(0), (int)C.stride(0),
                  a_mn ? 1 : 0, b_mn ? 1 : 0, out_mode, (int)ctas, (int)bn, A.device().index(), (int)max_ctas, gp, gcfg, dp,
                  gate_err.has_value() ? gate_err->data_ptr<int>() : nullptr, pdl ? 1 : 0, (int)a_fold, (int)b_fold, (int)fold_cols,
-                 stream_handle ? (cudaStream_t)stream_handle : stream()), "gemm2");
+                 rp, rowsum_acc ? 1 : 0, stream_handle ? (cudaStream_t)stream_handle : stream()), "gemm2");
   return C;
 }
 
@@ -823,7 +831,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("b_mn") = false, py::arg("out_fp32") = false, py::arg("accumulate") = false, py::arg("ctas") = 2, py::arg("bn") = 256,
         py::arg("max_ctas") = 0, py::arg("gate") = py::none(), py::arg("gate_cfg") = std::vector<int64_t>{}, py::arg("done") = py::none(),
         py::arg("gate_err") = py::none(), py::arg("stream") = 0, py::arg("pdl") = false, py::arg("a_fold") = 0, py::arg("b_fold") = 0,
-        py::arg("fold_cols") = 0);
+        py::arg("fold_cols") = 0, py::arg("rowsum") = py::none(), py::arg("rowsum_acc") = false);
   m.def("lstm_seq_fwd", &lstm_seq_fwd, py::arg("gx"), py::arg("w_h"), py::arg("bias"), py::arg("h0"), py::arg("c0"),
         py::arg("sync_ws"), py::arg("variant") = 0, py::arg("dbg") = py::none(), py::arg("in_gate") = py::none(),
         py::arg("in_gate_tiles_n") = 0, py::arg("extra_signal") = false, py::arg("lengths") = py::none(), py::arg("reverse") = false,

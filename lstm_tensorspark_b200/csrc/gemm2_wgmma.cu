@@ -12,6 +12,9 @@
 //   * fp32 output can ACCUMULATE into C (beta = 1): weight gradients go straight into the flat gradient buffer.
 //   * Optional dataflow gate: tile rows are only loaded once the arrival counters of their time step have reached their
 //     target (the producer of A is a concurrently running persistent kernel - the layer wavefront).
+//   * Optional row sums of op(A) (fp32 output): the CTAs of the first column of tiles also multiply their A stages by an
+//     all-ones 64 x 8 B block (one extra m64n8k16 per k16, 1/32 of the tile's MMAs), so dW = dG^T · X brings the bias
+//     gradient db = dG^T · 1 with it, summed over K in the same order - no separate column-sum pass over dG.
 //
 //   warp 0 : TMA producer     warps 1..3 : idle     warps 4..11 : two consumer warpgroups (wgmma + epilogue)
 // Persistent, static round-robin tile schedule over min(#tiles, #SMs / kCtas) clusters.
@@ -39,7 +42,8 @@ template <int kCtas, int BN> struct Cfg2 {
   static constexpr int kBBytes = BN * BK * 2;                    // the whole B tile lands in every CTA
   static constexpr int kStageBytes = kABytes + kBBytes;
   static constexpr int kStages = (200 * 1024) / kStageBytes > 8 ? 8 : (200 * 1024) / kStageBytes;
-  static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align*/ + 256 /*barriers*/;
+  static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align*/ + 1024 /*barriers, padded to 1 KB*/
+                                     + 1024 /*all-ones B block*/;
 };
 
 TC_DEVICE uint32_t cluster_ctarank2() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
@@ -75,6 +79,9 @@ struct Gemm2Params {
   // tensor map describes the storage as [fold = Bsz rows][T * F columns]; logical row r lives at storage row r % fold, columns
   // (r / fold) * fold_cols + [0, F).  a_fold: the K-major A operand (rows = M);  b_fold: the MN-major B operand (rows = K).
   int a_fold, b_fold, fold_cols;
+  // Row sums of op(A) (see the top of the file): rowsum[m] (=|+=, rowsum_acc) sum_k op(A)[m, k]; null = none.
+  float* rowsum;
+  int rowsum_acc;
 };
 
 template <int kCtas, int BN, bool kAMN, bool kBMN, int kOut>
@@ -88,6 +95,7 @@ gemm2_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::kStages * C::kStageBytes);
   uint64_t* full = bars;
   uint64_t* empty = bars + C::kStages;
+  uint8_t* smem_ones = smem + C::kStages * C::kStageBytes + 1024;      // 1024-aligned: one 8 x 64 bf16 swizzle atom of 1.0
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -205,9 +213,17 @@ gemm2_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__
     };
     uint32_t stage = 0, phase = 0;
     const int N = p.N, M = p.M;
+    if (p.rowsum != nullptr) {                            // the all-ones B block (every byte pattern is 1.0: no swizzle to mind)
+      reinterpret_cast<uint32_t*>(smem_ones)[threadIdx.x - kConsWarp0 * 32] = 0x3F803F80u;
+      tc::fence_proxy_async();                            // generic-proxy stores -> wgmma (async-proxy) reads
+      asm volatile("bar.sync 1, 256;" ::: "memory");
+    }
+    const uint64_t dones = tc::desc_kmajor_sw128(tc::smem_u32(smem_ones));
     for (int tile = cluster_id; tile < num_tiles; tile += num_clusters) {
       const int m0 = tile_m_of(tile) * TM + (int)crank * BM, n0 = (tile % tiles_n) * BN;
+      const bool rs = p.rowsum != nullptr && n0 == 0;     // this tile also sums its A rows
       float acc[BN / 2];
+      float rsum[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
       uint32_t prev = 0;
@@ -220,15 +236,30 @@ gemm2_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__
 #pragma unroll
         for (int k = 0; k < BK / 16; ++k)
           tc::Wgmma<BN, kAMN ? 1 : 0, kBMN ? 1 : 0>::mma(acc, da + k * kAStep, db + k * kBStep, (kb > 0 || k > 0) ? 1u : 0u);
+        if (rs) {
+          tc::fence_regs(rsum);
+#pragma unroll
+          for (int k = 0; k < BK / 16; ++k)
+            tc::Wgmma<8, kAMN ? 1 : 0, 0>::mma(rsum, da + k * kAStep, dones + k * (32 >> 4), (kb > 0 || k > 0) ? 1u : 0u);
+        }
         tc::wgmma_commit();
         tc::fence_regs(acc);
+        tc::fence_regs(rsum);
         if (kb > 0) { tc::wgmma_wait<1>(); release(prev); }     // the previous stage's MMAs have retired
         prev = stage;
         if (++stage == C::kStages) { stage = 0; phase ^= 1; }
       }
       tc::wgmma_wait<0>();
       tc::fence_regs(acc);
+      tc::fence_regs(rsum);
       release(prev);
+      if (rs && (lane & 3) == 0) {                        // every column of the n8 fragment holds the row sum: column 0
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int row = m0 + 64 * wg + tc::acc_row(2 * h, wq, lane);
+          if (row < M) p.rowsum[row] = rsum[2 * h] + (p.rowsum_acc ? p.rowsum[row] : 0.f);
+        }
+      }
       // epilogue straight from the accumulator fragments: a lane quad covers 8 consecutive columns of one row
 #pragma unroll
       for (int i = 0; i < BN / 2; i += 2) {
@@ -327,10 +358,11 @@ int launch_major(const void* A, const void* B, const Gemm2Params& p, int lda, in
 // A: K-major [M, K] (lda = row pitch) or MN-major [K, M];  B: K-major [N, K] or MN-major [K, N];  C [M, N] row pitch ldc.
 // out_mode: 0 bf16, 1 fp32, 2 fp32 accumulate (C += A·B).  ctas: 1 or 2 (cluster sharing the B tile).  bn: 128 or 256.
 // gate_cfg[7] = {count, stride (u32 words), base, per_step, rows_per_step, use_last, reverse_m} (see Gemm2Params); max_ctas > 0 caps the grid.
+// rowsum (fp32 [M], or null): also rowsum[m] (=|+= with rowsum_acc) the sum over K of op(A)[m, :] (fp32 output only).
 extern "C" int ts_gemm2(const void* A, const void* B, void* C, const float* bias, int M, int N, int K, int lda, int ldb, int ldc,
                         int a_mn, int b_mn, int out_mode, int ctas, int bn, int dev, int max_ctas, const unsigned int* gate,
                         const int* gate_cfg, unsigned int* done, int* gate_err, int pdl, int a_fold, int b_fold, int fold_cols,
-                        cudaStream_t st) {
+                        float* rowsum, int rowsum_acc, cudaStream_t st) {
   if (K % 8 != 0 || lda % 8 != 0 || ldb % 8 != 0) { ts::set_last_error("gemm2: K and the operand pitches must be multiples of 8"); return -2; }
   if ((a_mn && M % 8 != 0) || (b_mn && N % 8 != 0) || N % 8 != 0) { ts::set_last_error("gemm2: M (MN-major A) / N must be multiples of 8"); return -2; }
   if (out_mode != OUT_BF16 && ldc % 2 != 0) { ts::set_last_error("gemm2: fp32 output needs an even row pitch"); return -2; }
@@ -341,7 +373,9 @@ extern "C" int ts_gemm2(const void* A, const void* B, void* C, const float* bias
   if (b_fold && (!b_mn || b_fold % 64 != 0 || K % b_fold != 0 || N % bn != 0 || fold_cols < N)) {
     ts::set_last_error("gemm2: folded B needs an MN-major operand, fold % 64 == 0, K % fold == 0, N % bn == 0"); return -2;
   }
+  if (rowsum != nullptr && out_mode == OUT_BF16) { ts::set_last_error("gemm2: row sums of A need an fp32 output"); return -2; }
   Gemm2Params p{};
+  p.rowsum = rowsum; p.rowsum_acc = rowsum_acc;
   p.C = C; p.bias = bias; p.M = M; p.N = N; p.K = K; p.ldc = ldc;
   p.a_fold = a_fold; p.b_fold = b_fold; p.fold_cols = fold_cols;
   p.gate = gate; p.gate_err = gate_err; p.done = done; p.pdl = pdl;

@@ -107,6 +107,15 @@ TC_DEVICE int acc_col(int i, int l) { return 8 * (i >> 2) + 2 * (l & 3) + (i & 1
 
 // D (+)= A[smem] * B[smem], m64 x N x k16, bf16 in, fp32 accumulate.  TA / TB: 0 = K-major operand, 1 = MN-major.
 template <int N, int TA, int TB> struct Wgmma;
+template <int TA, int TB> struct Wgmma<8, TA, TB> {
+  TC_DEVICE static void mma(float (&d)[4], uint64_t da, uint64_t db, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %6, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n8k16.f32.bf16.bf16 {%0,%1,%2,%3}, %4, %5, p, 1, 1, %7, %8;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+        : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB));
+  }
+};
 template <int TA, int TB> struct Wgmma<16, TA, TB> {
   TC_DEVICE static void mma(float (&d)[8], uint64_t da, uint64_t db, uint32_t scale_d) {
     asm volatile(

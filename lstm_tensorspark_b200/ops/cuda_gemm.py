@@ -53,7 +53,7 @@ def folded_ok(x_bm: torch.Tensor) -> bool:
 def matmul(a: Optional[torch.Tensor], b_t: Optional[torch.Tensor], out: Optional[torch.Tensor] = None, accumulate: bool = False,
            out_dtype: Optional[torch.dtype] = None, bias: Optional[torch.Tensor] = None, max_ctas: int = 0,
            a_folded: Optional[torch.Tensor] = None, b_folded: Optional[torch.Tensor] = None, pdl: bool = False,
-           ctas: int = 0) -> torch.Tensor:
+           ctas: int = 0, rowsum: Optional[tuple] = None) -> torch.Tensor:
     """``a [M,K] @ b_t[N,K]^T`` (+ bias[N]); either operand may be a transposed view (then it is MN-major and is read in
     place).  ``out`` fp32 + ``accumulate`` -> ``out += a @ b_t^T``.
 
@@ -61,10 +61,15 @@ def matmul(a: Optional[torch.Tensor], b_t: Optional[torch.Tensor], out: Optional
     time-major matrix ``X = [T*B, F]``: ``a = X`` resp. ``b_t = X^T``.
 
     ``pdl``: programmatic dependent launch of the tensor-core GEMM (it starts once every CTA of the previous kernel is resident
-    and waits for that kernel before it exits).  ``ctas``: CTAs per tile cluster, 1 or 2 (0 = ``LSTM_TS_GEMM_CTAS``)."""
+    and waits for that kernel before it exits).  ``ctas``: CTAs per tile cluster, 1 or 2 (0 = ``LSTM_TS_GEMM_CTAS``).
+
+    ``rowsum`` = (fp32 [M] tensor, accumulate flag): the same launch also writes (or adds) the row sums of ``a`` over K into it
+    (tensor-core path with fp32 output only: a bias gradient next to its weight gradient)."""
     E = ext()
     ctas = ctas or GEMM_CTAS
+    rs = dict(rowsum=rowsum[0], rowsum_acc=rowsum[1]) if rowsum is not None else {}
     if a_folded is not None or b_folded is not None:
+        assert rowsum is None or a_folded is None, "row sums of a folded A are not supported"
         xb = a_folded if a_folded is not None else b_folded
         Bsz, T, F = xb.shape
         store = xb.view(Bsz, T * F)
@@ -78,7 +83,7 @@ def matmul(a: Optional[torch.Tensor], b_t: Optional[torch.Tensor], out: Optional
                            accumulate=accumulate, ctas=ctas, bn=GEMM_BN if b_t.shape[0] > 128 else 128, max_ctas=max_ctas, pdl=pdl,
                            a_fold=Bsz, fold_cols=F)
         return E.gemm2(other[1], store, bias=bias, out=out, a_mn=other[0], b_mn=True, out_fp32=out_dtype == torch.float32,
-                       accumulate=accumulate, ctas=ctas, bn=GEMM_BN, max_ctas=max_ctas, pdl=pdl, b_fold=Bsz, fold_cols=F)
+                       accumulate=accumulate, ctas=ctas, bn=GEMM_BN, max_ctas=max_ctas, pdl=pdl, b_fold=Bsz, fold_cols=F, **rs)
     M, K = a.shape
     N = b_t.shape[0]
     assert b_t.shape[1] == K, (a.shape, b_t.shape)
@@ -90,8 +95,9 @@ def matmul(a: Optional[torch.Tensor], b_t: Optional[torch.Tensor], out: Optional
             and (out is None or (out.stride(1) == 1 and out.stride(0) % 4 == 0 and out.data_ptr() % 16 == 0)):
         STATS["tc"] += 1
         return E.gemm2(ma[1], mb[1], bias=bias, out=out, a_mn=ma[0], b_mn=mb[0], out_fp32=out_dtype == torch.float32,
-                       accumulate=accumulate, ctas=ctas, bn=GEMM_BN if N > 128 else 128, max_ctas=max_ctas, pdl=pdl)
+                       accumulate=accumulate, ctas=ctas, bn=GEMM_BN if N > 128 else 128, max_ctas=max_ctas, pdl=pdl, **rs)
     assert a_folded is None and b_folded is None, "folded operands need the tensor-core path (check folded_ok first)"
+    assert rowsum is None, "row sums need the tensor-core path"
     STATS["generic"] += 1
     a_g = a if a.dtype in (torch.float32, torch.bfloat16) else a.float()
     b_g = b_t if b_t.dtype in (torch.float32, torch.bfloat16) else b_t.float()

@@ -7,7 +7,7 @@ recurrences co-resident, the upper layer's x-projection / dX as a dataflow-gated
 shape / fp32): our CUDA-core GEMM per step (csrc/gemm_generic.cu) + the fused pointwise cell kernels (csrc/lstm_pointwise.cu).
 Weight gradients are wgmma GEMMs over all T at once (``[4H, T·B] x [T·B, D | H]``, both operands MN-major and read in
 place), fp32, written straight into the flat gradient buffer; bias gradients are deterministic column sums running next to
-them.  Nothing in here reaches cuBLAS / cuDNN.  Math parity: original src/models/recurrent/lstm.py:88-122.
+them, or, for the lower layer of the pipelined pair, row sums of dG^T computed by its dW_h GEMM itself.  Nothing in here reaches cuBLAS / cuDNN.  Math parity: original src/models/recurrent/lstm.py:88-122.
 """
 from __future__ import annotations
 
@@ -106,15 +106,18 @@ def grad_sink(w_addr: int):
 
 
 def _accumulate_grad(w_addr: int, a_t: torch.Tensor, b: torch.Tensor, b_folded: bool = False, pdl: bool = False,
-                     max_ctas: int = 0):
+                     max_ctas: int = 0, ctas: int = 0, rowsum=None):
     """dW = a_t @ b in fp32 (``a_t`` = dG^T as a transposed view, ``b`` = the layer input: both operands MN-major, read in
     place by the wgmma GEMM; ``b_folded``: ``b`` is the batch-major [B,T,D] array standing for the time-major [T*B, D]
     matrix).  When the parameter lives in a FlatParams buffer the product lands straight in its grad
     view (overwrite on the first write of a step, accumulate afterwards) and None is returned to autograd.
     ``pdl``: launch as a programmatic dependent of the previous kernel (single-CTA tiles on at most ``max_ctas`` SMs, next to a
     recurrence that is still running).  Such a GEMM is no "big launch" for the gradient buckets: what precedes it in the stream
-    may still be running when it starts, so no bucket's allreduce is launched under it."""
-    ops = dict(a=a_t, b_t=None, b_folded=b) if b_folded else dict(a=a_t, b_t=b.t())
+    may still be running when it starts, so no bucket's allreduce is launched under it.  ``ctas``: CTAs per tile cluster of
+    an ordinary launch (0 = ``cuda_gemm.GEMM_CTAS``).  ``rowsum``: see ``cuda_gemm.matmul`` (the bias gradient, summed by the
+    same launch)."""
+    ops = dict(a=a_t, b_t=None, b_folded=b, ctas=ctas) if b_folded else dict(a=a_t, b_t=b.t(), ctas=ctas)
+    ops["rowsum"] = rowsum
     if pdl:
         ops.update(pdl=True, ctas=1, max_ctas=max_ctas)
     sink = grad_sink(w_addr)
@@ -493,8 +496,9 @@ def lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths=None, reverse=Fal
 # The reference stacks layers strictly one after the other (original src/models/recurrent/rnn.py:38-42); here layer l+1
 # trails layer l by a couple of time steps and the next layer's input projection leaves the critical path altogether.
 # Where both recurrences do not fit side by side (an H100 at H = 1024: 64 + 64 + 8 > 132 SMs), the pair is PIPELINED instead:
-# the recurrences run one after the other and the GEMMs that do not feed the running recurrence move onto the SMs it leaves idle
-#     forward :  L_a  || gx_b (gated)                    ->  L_b
+# the recurrences run one after the other and the GEMMs move onto the SMs the running recurrence leaves idle (L_a's own input
+# projection gx_a too: L_a waits for it block by block)
+#     forward :  L_a  || gx_a, gx_b (gated)              ->  L_b
 #     backward:  L_b  || dx_b (gated)                    ->  L_a  || dW_xb, dW_hb, db_b
 # =====================================================================================================================
 FOLDED_FEED = os.environ.get("LSTM_TS_FOLDED_FEED", "1") != "0"   # batch-major input read in place by the first layer's GEMMs
@@ -516,7 +520,8 @@ _WARM = set()
 def _warm_wavefront_kernels(device):
     """CUDA loads kernels lazily, and loading one may wait for every running kernel to finish.  The wavefront's kernels WAIT
     FOR EACH OTHER on the device, so a kernel that is loaded for the first time while its producers are already spinning would
-    deadlock (until the bounded spins time out).  Load the gated GEMM instantiations once, before the first concurrent use."""
+    deadlock (until the bounded spins time out).  Load the gated GEMM instantiations and the pipelined pair's ungated
+    ``done``-publishing x-projection (the same instantiation, contiguous or folded input) once, before the first concurrent use."""
     if device.index in _WARM:
         return
     a = torch.zeros(256, 64, dtype=torch.bfloat16, device=device)
@@ -543,8 +548,8 @@ def pair_schedule(T: int, B: int, D: int, h_a: int, h_b: int, sms: int, coreside
     clusters of 4 (``_coresident_ctas``).  Every recurrence runs two batch tiles per CTA, H/16 CTAs.  Both schedules need
     B = 256 (one GEMM tile row per time step), resident weights (H <= 1024) and 256-aligned widths.
       "wavefront": both recurrences co-resident, the gated GEMM on the SMs they leave free (H_a/16 + H_b/16 + 8 SMs).
-      "pipelined": the recurrences run one after the other; next to each runs a GEMM that does not feed it (forward: L_a with
-                   gx_b; backward: L_b with dx_b, then L_a with dW_xb, dW_hb and db_b).  Needs max(H)/16 + 8 SMs.
+      "pipelined": the recurrences run one after the other, GEMMs next to them (forward: L_a with its own gx_a and with gx_b;
+                   backward: L_b with dx_b, then L_a with dW_xb, dW_hb and db_b).  Needs max(H)/16 + 8 SMs.
       None: two separate layers."""
     if B != 256 or T < 2 or D % 8 != 0 or any(h % 256 != 0 or h > 1024 for h in (h_a, h_b)):
         return None
@@ -554,6 +559,18 @@ def pair_schedule(T: int, B: int, D: int, h_a: int, h_b: int, sms: int, coreside
     if max(h_a, h_b) // 16 <= coresident and max(h_a, h_b) // 16 + 8 <= sms:
         return "pipelined"
     return None
+
+
+def pipelined_fwd_split(sms: int, d: int, h_a: int, h_b: int) -> tuple:
+    """SMs of the pipelined pair's forward side GEMMs -> (gx_a CTAs, gx_b CTAs).  Both run next to L_a on the ``sms - h_a / 16``
+    SMs its CTAs leave free, one single-CTA 128 x 256 tile per SM, and both must keep pace with it: L_a waits for gx_a(t) at its
+    step t, and L_b (after L_a) for the last gx_b rows.  Their work per step is 2·B·4h_a·d and 2·B·4h_b·h_a FLOP, so the free
+    SMs are split in the ratio d : h_b: 34 + 34 at the headline 2 x 1024 on a 132-SM H100, where a step of L_a takes about
+    20 us and 34 SMs compute a step's 2.1 GFLOP of either GEMM in about 12 us (5.2 TFLOP/s per SM with single-CTA tiles,
+    bench/side_gemms.py on an H100 80GB HBM3 at 700 W)."""
+    free = max(2, sms - h_a // 16)
+    n_a = min(free - 1, max(1, round(free * d / (d + h_b)))) if d > 0 else 0     # d = 0: gx_a computed before L_a
+    return n_a, free - n_a
 
 
 def _pair_schedule_of(x_seq: torch.Tensor, h_a: int, h_b: int) -> Optional[str]:
@@ -624,12 +641,15 @@ class _LSTMPairFn(torch.autograd.Function):
         h0a_c, h0b_c = h0a.detach().to(cd).contiguous(), h0b.detach().to(cd).contiguous()
         c0a_f, c0b_f = c0a.detach().float().contiguous(), c0b.detach().float().contiguous()
         _warm_wavefront_kernels(dev)
-        if x_bm is None:
+        opt = dict(dtype=cd, device=dev)
+        side_a = pipelined and D >= 64                                   # gx_a next to L_a (the tensor-core GEMM needs K >= 64)
+        if side_a:
+            gx_a = torch.empty(T, B, 4 * Ha, **opt)                      # written next to L_a (see below)
+        elif x_bm is None:
             gx_a = _gemm_tn(x2d, wxa).view(T, B, 4 * Ha)
         else:
             STATS["tc_gemm"] += 1; STATS["kernels"] += 1; STATS["folded_feed"] = STATS.get("folded_feed", 0) + 1
             gx_a = G.matmul(None, wxa, out_dtype=cd, a_folded=x_bm).view(T, B, 4 * Ha)
-        opt = dict(dtype=cd, device=dev)
         h_seq_a = torch.empty(T + 1, B, Ha, **opt); c_seq_a = torch.empty(T + 1, B, Ha, dtype=torch.float32, device=dev)
         act_a = torch.empty(T, B, 4 * Ha, **opt); til_a = torch.empty((T + 1) * 2 * 128 * Ha, **opt)
         h_seq_b = torch.empty(T + 1, B, Hb, **opt); c_seq_b = torch.empty(T + 1, B, Hb, dtype=torch.float32, device=dev)
@@ -640,25 +660,36 @@ class _LSTMPairFn(torch.autograd.Function):
         h_drop_a = torch.empty(T, B, Ha, **opt) if dra else None
         h_drop_b = torch.empty(T, B, Hb, **opt) if drb else None
         hin_b = h_seq_a[1:] if h_drop_a is None else h_drop_a            # layer b's input sequence
-        tn = 4 * Hb // 256
-        ws_a, ws_b, done = _pair_ws(dev, "fwd", T * tn * 2)
+        tn, tn_a = 4 * Hb // 256, 4 * Ha // 256
+        ws_a, ws_b, done = _pair_ws(dev, "fwd", T * 2 * (tn + (tn_a if side_a else 0)))
         done.zero_()                                                     # (the prologue kernels zero ws_a / ws_b)
+        done, done_a = done[:T * 2 * tn], done[T * 2 * tn:]
         var = _pair_variant(schedule)                                    # two batch tiles per CTA: 64 CTAs per layer at H = 1024
         # ONE stream, a programmatic-dependent-launch chain: L_a -> L_b (starts once every CTA of L_a is resident) -> gated GEMM
         # (starts once every CTA of L_b is resident, on the SMs that are left).  The order in which the three grids take their
         # SMs is thereby fixed (a kernel that is still queueing could otherwise starve the chain head of co-resident SMs).
         # Everything the later kernels need up front (prologues, zeroed counters) is enqueued before the chain head.
-        # Pipelined: L_a -> gated GEMM (programmatic dependent, on the SMs L_a leaves free) -> L_b, an ordinary launch that
-        # starts once both are complete (the GEMM waits for L_a before it exits).
+        # Pipelined: L_a -> gx_a GEMM -> gated gx_b GEMM (programmatic dependents, on the SMs L_a leaves free) -> L_b, an ordinary
+        # launch that starts once all three are complete (each GEMM waits for its predecessor before it exits).  L_a waits for
+        # gx_a's 128 x 256 blocks as the wavefront's L_b does for gx_b's; the gx_a GEMM is ungated, so nothing it waits for
+        # depends on L_a, and its capped grid walks the M tiles (time steps) in order.
         E.lstm_seq_prologue(h0a_c, c0a_f, h_seq_a, c_seq_a, til_a, ws_a)
         E.lstm_seq_prologue(h0b_c, c0b_f, h_seq_b, c_seq_b, til_b, ws_b)
-        E.lstm_seq_fwd_into(gx_a, wha, ba_f, h0a_c, c0a_f, h_seq_a, c_seq_a, act_a, til_a, ws_a, var, None, 0, True, 0, 1, lengths,
-                            h_drop=h_drop_a, **dra)
+        E.lstm_seq_fwd_into(gx_a, wha, ba_f, h0a_c, c0a_f, h_seq_a, c_seq_a, act_a, til_a, ws_a, var, done_a if side_a else None,
+                            tn_a if side_a else 0, True, 0, 1, lengths, h_drop=h_drop_a, **dra)
+        if pipelined:
+            ctas_a, free_ctas = pipelined_fwd_split(_sms(dev), D if side_a else 0, Ha, Hb)
+        if side_a:
+            a_op = dict(A=x2d, a_fold=0) if x_bm is None else dict(A=x_bm.reshape(B, T * D), a_fold=B, fold_cols=D)
+            E.gemm2(B=wxa, out=gx_a.view(T * B, 4 * Ha), ctas=1, bn=256, max_ctas=ctas_a, done=done_a, pdl=True, **a_op)
+            STATS["tc_gemm"] += 1; STATS["kernels"] += 1; STATS["pipelined_side_gemms"] = STATS.get("pipelined_side_gemms", 0) + 1
+            if x_bm is not None:
+                STATS["folded_feed"] = STATS.get("folded_feed", 0) + 1
         if not pipelined:
             E.lstm_seq_fwd_into(gx_b, whb, bb_f, h0b_c, c0b_f, h_seq_b, c_seq_b, act_b, til_b, ws_b, var, done, tn, False, 0, 3, lengths,
                                 h_drop=h_drop_b, **drb)
-        # single-CTA tiles: the recurrences' CTAs are spread one per TPC, the SMs they leave free rarely form CTA pairs
-        free_ctas = max(1, _sms(dev) - Ha // 16 - (0 if pipelined else Hb // 16))
+            # single-CTA tiles: the recurrences' CTAs are spread one per TPC, the SMs they leave free rarely form CTA pairs
+            free_ctas = max(1, _sms(dev) - Ha // 16 - Hb // 16)
         E.gemm2(hin_b.view(T * B, Ha), wxb, out=gx_b.view(T * B, 4 * Hb), ctas=1, bn=256, max_ctas=free_ctas,
                 gate=ws_a[_gate_off(var):], gate_cfg=_gate_cfg(var, 2, Ha // 64, 4, 4 * Ha // 64, 2, 1, B, False), done=done,
                 gate_err=ws_a[SYNC_WORDS - 1:], pdl=True)
@@ -742,10 +773,26 @@ class _LSTMPairFn(torch.autograd.Function):
             dw_hb = _accumulate_grad(a[4], dg_b.t(), h_seq_b[:T].reshape(T * B, Hb))
             db_b = _bias_grad(a[5], dg_b, under_gemm=dw_hb is None, part=1)
         dg_a = dpre_a.view(T * B, 4 * Ha)
-        dw_xa = _accumulate_grad(a[0], dg_a.t(), x2d, b_folded=ctx.x_folded)
-        _bias_grad(a[2], dg_a, under_gemm=dw_xa is None, part=0)
-        dw_ha = _accumulate_grad(a[1], dg_a.t(), h_seq_a[:T].reshape(T * B, Ha))
-        db_a = _bias_grad(a[2], dg_a, under_gemm=dw_ha is None, part=1)
+        if pipelined:
+            # 2 x 1024 on a 132-SM H100: single-CTA 128 x 256 tiles put the 128 tiles of each of these GEMMs on 128 SMs in one
+            # wave, at the per-SM rate of the capped side GEMMs; 2-CTA clusters ran them at about half that rate per SM
+            # (bench/side_gemms.py).  The tile's K order, and with it every bit of dW, is the same either way.  db_a comes out of
+            # the dW_ha launch as the row sums of dG_a^T (csrc/gemm2_wgmma.cu): the column-sum kernels beside these GEMMs only
+            # found the 4 SMs the GEMMs leave free and ran on after them.
+            dw_xa = _accumulate_grad(a[0], dg_a.t(), x2d, b_folded=ctx.x_folded, ctas=1)
+            bsink = grad_sink(a[2])
+            db_a = bsink[0] if bsink is not None else torch.empty(4 * Ha, **f32)
+            dw_ha = _accumulate_grad(a[1], dg_a.t(), h_seq_a[:T].reshape(T * B, Ha), ctas=1,
+                                     rowsum=(db_a, bsink is not None and bsink[1]))
+            STATS["fused_bias_grads"] = STATS.get("fused_bias_grads", 0) + 1
+            if bsink is not None:
+                db_a = None
+                _grads_written()
+        else:
+            dw_xa = _accumulate_grad(a[0], dg_a.t(), x2d, b_folded=ctx.x_folded)
+            _bias_grad(a[2], dg_a, under_gemm=dw_xa is None, part=0)
+            dw_ha = _accumulate_grad(a[1], dg_a.t(), h_seq_a[:T].reshape(T * B, Ha))
+            db_a = _bias_grad(a[2], dg_a, under_gemm=dw_ha is None, part=1)
         dx = None
         if ctx.needs_input_grad[0]:                                       # (never with a folded input: lstm_pair_sequence)
             dx = G.matmul(dg_a, wxa.t(), out_dtype=cd).view(T, B, D)
