@@ -23,6 +23,7 @@ FUSED_CLIP_ERROR = ("--clip_grad_norm with --sync_mode grad_allreduce needs the 
 
 
 ATTENTION_UNITS_DEFAULT = 128
+NUM_CLASSES_DEFAULT = 3
 
 
 @dataclass
@@ -34,7 +35,7 @@ class Config:
     epochs: int = 1
     hidden_units: str = "128,256"
     batch_size: int = 10                # 0 => whole shard in one batch (reference intent, Q3)
-    num_classes: int = 3
+    num_classes: int = NUM_CLASSES_DEFAULT
     in_features: int = 4
     learning_rate: float = 1e-3
     evaluate_every: int = 10
@@ -63,6 +64,8 @@ class Config:
     vocab_size: int = 0                 # V > 0: the input is int token ids [B,T] (one step: [B]) and the first layer reads
                                         # x_t = Embedding[tok_t], a learned [V, in_features] table (nn.Embedding); a CSV row is k ids
                                         # followed by the label (--per_step_labels: by k labels).  0 = float features
+    next_token: bool = False            # language modelling (needs --vocab_size V): the label of step t is the token of step t + 1.
+                                        # Turns on --per_step_labels and sets --num_classes to V; a CSV row is seq_len + 1 ids
     dtype: str = "auto"                 # auto: bf16 on cuda, fp32 on cpu
     device: str = "auto"                # auto | cpu | cuda
     backend: str = "auto"               # auto | cuda_ext (hand-written sm_90a kernels) | torch
@@ -99,6 +102,13 @@ class Config:
     fault_inject: str = ""              # "rank:step" => that rank exits abnormally at that step (test hook)
     timeout_s: float = 600.0
     quiet: bool = False
+
+    def __post_init__(self):
+        # --next_token implies the label layout and the class count (validate() reports the combinations it refuses)
+        if self.next_token and self.vocab_size > 0:
+            self.per_step_labels = True
+            if self.num_classes == NUM_CLASSES_DEFAULT:
+                self.num_classes = self.vocab_size
 
     # ------------------------------------------------------------------------------------------
     def hidden_list(self) -> List[int]:
@@ -144,6 +154,22 @@ class Config:
             raise ValueError("--batch_size must be >= 0 (0 = whole shard)")
         if self.seq_len < 1:
             raise ValueError("--seq_len must be >= 1")
+        if self.next_token:
+            if self.vocab_size <= 0:
+                raise ValueError("--next_token needs --vocab_size V > 0: it predicts the next token id out of the V of the vocabulary")
+            if self.seq_len < 2:
+                raise ValueError("--next_token needs --seq_len >= 2 (a row is seq_len + 1 token ids: seq_len inputs, each labelled "
+                                 "with the id that follows it)")
+            if self.num_classes != self.vocab_size:
+                raise ValueError(f"--next_token sets --num_classes to --vocab_size ({self.vocab_size}), got --num_classes "
+                                 f"{self.num_classes}: drop --num_classes")
+            if self.pooling != "last":
+                raise ValueError(f"--next_token does not combine with --pooling {self.pooling}: every step's output is scored, "
+                                 "there is nothing to pool")
+            if self.bidirectional:
+                raise ValueError("--next_token does not combine with --bidirectional: a reverse layer sees the token it is asked to "
+                                 "predict")
+            self.per_step_labels = True
         if self.variable_length and self.seq_len < 2:
             raise ValueError("--variable_length needs --seq_len >= 2 (the longest sample's number of steps)")
         if self.bidirectional and self.seq_len < 2:
@@ -230,6 +256,9 @@ _HELP = {
     "vocab_size": "Read token ids through a learned embedding table of V rows and --in_features columns (nn.Embedding in front "
                   "of the first layer); a CSV row is k ids followed by the label (or by k labels with --per_step_labels). "
                   "0 = float features",
+    "next_token": "Train a next-token language model on --vocab_size V token ids: the label of step t is the id of step t + 1 "
+                  "(turns on --per_step_labels, sets --num_classes to V); a CSV row is seq_len + 1 ids, or 2..seq_len + 1 with "
+                  "--variable_length; evaluations also report perplexity = exp(loss)",
     "per_step_labels": "Label every time step (sequence labelling): labels [B,T], loss and accuracy over the real positions; "
                        "a CSV row is k*in_features values followed by k labels",
 }

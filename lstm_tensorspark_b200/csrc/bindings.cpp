@@ -49,6 +49,13 @@ long long ts_head_step_bwd_scratch(int, int, int);
 int ts_head_step_bwd_tickets(int);
 int ts_head_step_bwd(const void*, const float*, const float*, const float*, void*, float*, float*, float*, unsigned int*, int, int, int,
                      int, int, cudaStream_t);
+int ts_vocab_head_parts(int);
+int ts_vocab_head_blocks(int);
+int ts_vocab_head_fwd(const void*, const void*, const float*, const long long*, const int*, void*, float*, float*, int*, unsigned int*,
+                      float*, int*, int*, int, int, int, int, int, cudaStream_t);
+int ts_vocab_head_dlogits(const void*, const void*, const float*, const long long*, const int*, const float*, const float*, const int*,
+                          void*, int, int, int, int, int, int, int, cudaStream_t);
+int ts_vocab_head_colsum(const void*, float*, int, int, int, cudaStream_t);
 int ts_gemm_generic(const void*, const void*, void*, const float*, int, int, int, long long, long long, long long, long long, long long,
                     int, int, int, float, cudaStream_t);
 int ts_gemm2(const void*, const void*, void*, const float*, int, int, int, int, int, int, int, int, int, int, int, int, int,
@@ -361,6 +368,67 @@ Tensor head_step_bwd(const Tensor& h, const Tensor& W, const Tensor& dlogits, co
                          db.data_ptr<float>(), scratch.data_ptr<float>(), (unsigned int*)tickets.data_ptr<int>(), R, H, C, is_bf16(h),
                          accumulate ? 1 : 0, stream()), "head_step_bwd");
   return dh;
+}
+
+// ---- large-vocabulary per-step head (csrc/head_vocab.cu) ------------------------------------------------------------
+// h bf16 [T·B, H] packed time-major rows, Wb bf16 [H, C], bias fp32 [C], labels int64 [B,T], optional lengths int32 [B] (0 allowed),
+// part: fp32 scratch of at least T·B * vocab_head_parts(C) * 4 elements -> lse [T·B], loss, correct, N.  No logits are stored and
+// nothing is read back to the host.
+void vocab_head_check(const Tensor& h, const Tensor& Wb, const Tensor& bias, const Tensor& labels, int64_t T) {
+  chk_cuda(h, "h"); chk_cuda(Wb, "Wb"); chk_cuda(bias, "bias"); chk_cuda(labels, "labels");
+  TORCH_CHECK(h.dim() == 2 && Wb.dim() == 2 && h.scalar_type() == torch::kBFloat16 && Wb.scalar_type() == torch::kBFloat16 &&
+              Wb.size(0) == h.size(1), "vocab head: h bf16 [T*B,H], Wb bf16 [H,C]");
+  const int64_t R = h.size(0), H = h.size(1), C = Wb.size(1);
+  TORCH_CHECK(H % 64 == 0 && C % 8 == 0 && C >= 8, "vocab head: H % 64 == 0 and C % 8 == 0");
+  TORCH_CHECK(T >= 1 && R % T == 0 && R * std::max(C, H) < (int64_t(1) << 40) && R < (int64_t(1) << 31), "vocab head: rows must be T*B");
+  TORCH_CHECK(bias.scalar_type() == torch::kFloat32 && bias.numel() == C && ((uintptr_t)bias.data_ptr() % 8) == 0, "vocab head: bias fp32 [C]");
+  TORCH_CHECK(labels.scalar_type() == torch::kInt64 && labels.dim() == 2 && labels.size(0) == R / T && labels.size(1) == T, "labels int64 [B,T]");
+}
+
+std::vector<Tensor> vocab_head_fwd(const Tensor& h, const Tensor& Wb, const Tensor& bias, const Tensor& labels,
+                                   const std::optional<Tensor>& lengths, int64_t T, Tensor part) {
+  vocab_head_check(h, Wb, bias, labels, T);
+  c10::cuda::CUDAGuard g(h.device());
+  const int R = h.size(0), H = h.size(1), C = Wb.size(1), B = R / (int)T;
+  chk_cuda(part, "part");
+  TORCH_CHECK(part.scalar_type() == torch::kFloat32 && part.numel() >= (int64_t)R * ts_vocab_head_parts(C) * 4 &&
+              ((uintptr_t)part.data_ptr() % 16) == 0, "vocab head: part scratch");
+  auto fo = torch::TensorOptions().device(h.device()).dtype(torch::kFloat32);
+  const int blocks = ts_vocab_head_blocks(R);
+  auto lse = torch::empty({R}, fo), part_loss = torch::empty({blocks}, fo), loss = torch::empty({1}, fo);
+  auto ints = torch::zeros({blocks + 4}, fo.dtype(torch::kInt32));          // [blocks] per-block counts, ticket, correct, N
+  int* ip = ints.data_ptr<int>();
+  check(ts_vocab_head_fwd(h.data_ptr(), Wb.data_ptr(), bias.data_ptr<float>(), (const long long*)labels.data_ptr<int64_t>(),
+                          lengths_ptr(lengths, B, h), part.data_ptr(), lse.data_ptr<float>(), part_loss.data_ptr<float>(), ip,
+                          (unsigned int*)(ip + blocks), loss.data_ptr<float>(), ip + blocks + 1, ip + blocks + 2, (int)T, B, H, C,
+                          h.get_device(), stream()), "vocab_head_fwd");
+  return {lse, loss, ints.narrow(0, blocks + 1, 1), ints.narrow(0, blocks + 2, 1)};
+}
+
+// dl [rows, C] bf16 <- (softmax - onehot) * dloss / N of rows [row0, row0 + rows) of h (0 at uncounted rows); lse, count: the forward's.
+void vocab_head_dlogits(const Tensor& h, const Tensor& Wb, const Tensor& bias, const Tensor& labels, const std::optional<Tensor>& lengths,
+                        int64_t T, const Tensor& lse, const Tensor& count, const Tensor& dloss, int64_t row0, int64_t rows, Tensor dl) {
+  vocab_head_check(h, Wb, bias, labels, T);
+  c10::cuda::CUDAGuard g(h.device());
+  const int R = h.size(0), H = h.size(1), C = Wb.size(1), B = R / (int)T;
+  chk_cuda(lse, "lse"); chk_cuda(count, "count"); chk_cuda(dloss, "dloss"); chk_cuda(dl, "dl");
+  TORCH_CHECK(lse.scalar_type() == torch::kFloat32 && lse.numel() == R && count.scalar_type() == torch::kInt32 && count.numel() == 1 &&
+              dloss.scalar_type() == torch::kFloat32 && dloss.numel() == 1, "vocab head: lse fp32 [R], count int32 [1], dloss fp32 [1]");
+  TORCH_CHECK(rows >= 1 && row0 >= 0 && row0 + rows <= R && dl.scalar_type() == torch::kBFloat16 && dl.numel() >= rows * C,
+              "vocab head: dl bf16 [rows, C]");
+  check(ts_vocab_head_dlogits(h.data_ptr(), Wb.data_ptr(), bias.data_ptr<float>(), (const long long*)labels.data_ptr<int64_t>(),
+                              lengths_ptr(lengths, B, h), lse.data_ptr<float>(), dloss.data_ptr<float>(), count.data_ptr<int>(),
+                              dl.data_ptr(), (int)T, B, H, C, (int)row0, (int)rows, h.get_device(), stream()), "vocab_head_dlogits");
+}
+
+// db [C] (+)= column sums of dl [rows, C] (bf16), summed in a fixed order.
+void vocab_head_colsum(const Tensor& dl, Tensor db, bool accumulate) {
+  chk_cuda(dl, "dl"); chk_cuda(db, "db");
+  c10::cuda::CUDAGuard g(dl.device());
+  TORCH_CHECK(dl.dim() == 2 && dl.scalar_type() == torch::kBFloat16 && dl.size(1) % 2 == 0 && db.scalar_type() == torch::kFloat32 &&
+              db.numel() == dl.size(1), "vocab head: dl bf16 [rows, C], db fp32 [C]");
+  check(ts_vocab_head_colsum(dl.data_ptr(), db.data_ptr<float>(), (int)dl.size(0), (int)dl.size(1), accumulate ? 1 : 0, stream()),
+        "vocab_head_colsum");
 }
 
 // ---- pooling over time (csrc/seq_pool.cu) ---------------------------------------------------------------------
@@ -801,6 +869,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("head_step_fwd", &head_step_fwd, py::arg("h"), py::arg("W"), py::arg("bias"), py::arg("labels"), py::arg("lengths"), py::arg("T"));
   m.def("head_step_bwd", &head_step_bwd, py::arg("h"), py::arg("W"), py::arg("dlogits"), py::arg("dloss"), py::arg("dW"), py::arg("db"),
         py::arg("accumulate"));
+  m.def("vocab_head_parts", [](int64_t C) { return ts_vocab_head_parts((int)C); });
+  m.def("vocab_head_fwd", &vocab_head_fwd, py::arg("h"), py::arg("Wb"), py::arg("bias"), py::arg("labels"), py::arg("lengths"),
+        py::arg("T"), py::arg("part"));
+  m.def("vocab_head_dlogits", &vocab_head_dlogits, py::arg("h"), py::arg("Wb"), py::arg("bias"), py::arg("labels"), py::arg("lengths"),
+        py::arg("T"), py::arg("lse"), py::arg("count"), py::arg("dloss"), py::arg("row0"), py::arg("rows"), py::arg("dl"));
+  m.def("vocab_head_colsum", &vocab_head_colsum, py::arg("dl"), py::arg("db"), py::arg("accumulate"));
   m.def("head_bwd", &head_bwd, py::arg("h"), py::arg("W"), py::arg("dlogits"), py::arg("dloss"), py::arg("dW"), py::arg("db"),
         py::arg("accumulate") = false);
   m.def("flat_adam", &flat_adam, py::arg("p"), py::arg("g"), py::arg("m"), py::arg("v"), py::arg("shadow"), py::arg("lr_t"),

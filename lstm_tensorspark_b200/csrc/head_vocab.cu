@@ -1,0 +1,457 @@
+// Large-vocabulary per-step head (next-token language modelling): softmax cross-entropy over C >= 512 classes at every row of
+// h [R = T·B, H] without ever storing the logits [R, C] or an fp32 dlogits [R, C].
+//
+//   logits = h [R,H] (bf16, K-major) · W [H,C] (bf16, read in place as an MN-major operand) + bias (fp32), fp32 accumulators.
+//
+//   * vocab_head_gemm_kernel<kFwd>: TMA + wgmma over 128-row x 256-class tiles (a cluster of two CTAs computes 256 rows and
+//     shares the W tile by multicast, as gemm2_wgmma.cu).  The epilogue never writes the tile: per row it reduces the tile's
+//     max, sum exp(l - max), arg-max and the label's logit from the accumulator fragments into part[R, C/256] (16 B each).
+//   * vocab_head_combine_kernel: merges a row's partials in a fixed order -> lse[R]; loss, correct and N through per-block
+//     partials summed by the last block (ticket): two calls on the same inputs give the same bits.
+//   * vocab_head_gemm_kernel<kDlogits>: the same main loop over one chunk of rows recomputes the logits; the epilogue writes
+//     dlogits = (exp(l - lse) - onehot) · dloss / N at counted rows, 0 elsewhere, as bf16 into a scratch [chunk rows, C] that
+//     the caller feeds to the general GEMM (dh = dlogits · W^T, dW += h^T · dlogits).
+//   * vocab_head_colsum_kernel: db (+)= column sums of the bf16 dlogits chunk, summed in a fixed order.
+//
+// Tiles are walked in bands of 16 cluster tiles (4096 rows): inside a band the class tile is the outer index, so the band's rows
+// of h stay in L2 and W streams from HBM once per band.  Row r = t·B + b counts iff t < lengths[b]; lengths may be 0.
+//
+//   warp 0 : TMA producer     warps 1..3 : idle     warps 4..11 : two consumer warpgroups (wgmma + epilogue)
+#include <cuda.h>
+#include <cuda_bf16.h>
+#include <cuda_runtime.h>
+
+#include "hopper.cuh"
+#include "tmap.h"
+
+namespace {
+
+constexpr int BM = 128;                     // rows per CTA (two m64 warpgroups)
+constexpr int BN = 256;                     // classes per tile
+constexpr int BK = 64;                      // 64 bf16 = 128 B = one swizzle atom
+constexpr int kCtas = 2;                    // CTAs per cluster: 256 rows share one W tile
+constexpr int TM = BM * kCtas;
+constexpr int kBandTiles = 16;              // cluster tiles per band
+constexpr int kThreads = 384;
+constexpr int kConsWarp0 = 4;
+constexpr int kABytes = BM * BK * 2;        // 16 KB
+constexpr int kBBytes = BN * BK * 2;        // 32 KB: the whole W tile lands in both CTAs
+constexpr int kStageBytes = kABytes + kBBytes;
+constexpr int kStages = 4;
+constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align*/ + 1024 /*barriers*/;
+
+enum Mode { kFwd = 0, kDlogits = 1 };
+
+struct VocabParams {
+  const float* bias;           // [C]
+  const long long* labels;     // [B, T]
+  const int* lengths;          // [B] or null
+  float4* part;                // kFwd: [R, tiles_n] {max, sum exp, arg-max (int bits), label logit or 0}
+  const float* lse;            // kDlogits: [R]
+  const float* dloss;          // kDlogits: [1]
+  const int* count;            // kDlogits: [1] N
+  __nv_bfloat16* dl;           // kDlogits: [rows, C]
+  int R, H, C, T, B;
+  int row0, rows;              // this launch covers rows [row0, row0 + rows) of h
+};
+
+TC_DEVICE uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
+TC_DEVICE void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
+  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+TC_DEVICE uint32_t mapa(uint32_t local_smem_addr, uint32_t cta) {
+  uint32_t r;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_smem_addr), "r"(cta));
+  return r;
+}
+TC_DEVICE void mbar_arrive_cluster(uint32_t cluster_bar_addr) {
+  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_bar_addr) : "memory");
+}
+
+// tile -> (cluster tile row, class tile): bands of kBandTiles cluster tiles, class tile outer inside a band
+TC_DEVICE void tile_coords(int tile, int tiles_m, int tiles_n, int& tm, int& tn) {
+  const int per_band = kBandTiles * tiles_n;
+  const int band = tile / per_band, rem = tile - band * per_band;
+  const int gm = min(kBandTiles, tiles_m - band * kBandTiles);
+  tn = rem / gm;
+  tm = band * kBandTiles + rem - tn * gm;
+}
+
+template <int kMode>
+__global__ void __launch_bounds__(kThreads, 1)
+vocab_head_gemm_kernel(const __grid_constant__ CUtensorMap tmap_h, const __grid_constant__ CUtensorMap tmap_w, const VocabParams p) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* smem_a = smem;
+  uint8_t* smem_b = smem + kStages * kABytes;
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + kStages * kStageBytes);
+  uint64_t* empty = full + kStages;
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const uint32_t crank = cluster_ctarank();
+  const int tiles_n = (p.C + BN - 1) / BN;
+  const int tiles_m = (p.rows + TM - 1) / TM;
+  const int num_tiles = tiles_m * tiles_n;
+  const int num_kb = p.H / BK;
+  const int cluster_id = blockIdx.x / kCtas, num_clusters = gridDim.x / kCtas;
+
+  if (warp == 0 && lane == 0) {
+    tc::prefetch_tmap(&tmap_h);
+    tc::prefetch_tmap(&tmap_w);
+  }
+  if (warp == 1 && lane == 0) {
+    // empty: every consumer warp of both CTAs (the W half this CTA loads lands in both)
+    for (int s = 0; s < kStages; ++s) { tc::mbar_init(&full[s], 1); tc::mbar_init(&empty[s], 8 * kCtas); }
+    tc::fence_barrier_init();
+  }
+  __syncthreads();
+  cluster_sync();                                // the peer's barriers are initialised before anything arrives on them
+
+  // The consumers hold 128 accumulator registers per thread and the epilogue works on all of them: setmaxnreg moves registers
+  // from warpgroup 0 (producer and idle warps) to them, (168 - 56) * 128 = (224 - 168) * 256.  All four warps of a warpgroup
+  // execute it at the top of the warpgroup's branch.
+  if (warp < kConsWarp0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 56;" ::: "memory");
+    if (warp == 0) {
+      // ===================================================================== TMA producer
+      const uint32_t full0 = tc::smem_u32(full), empty0 = tc::smem_u32(empty);
+      const uint32_t sa0 = tc::smem_u32(smem_a), sb0 = tc::smem_u32(smem_b);
+      uint32_t stage = 0, phase = 0;
+      for (int tile = cluster_id; tile < num_tiles; tile += num_clusters) {
+        int tm, tn;
+        tile_coords(tile, tiles_m, tiles_n, tm, tn);
+        const int m0 = p.row0 + tm * TM + (int)crank * BM;
+        const int n0 = tn * BN + (int)crank * (BN / kCtas);
+        for (int kb = 0, k0 = 0; kb < num_kb; ++kb, k0 += BK) {
+          const uint32_t eb = empty0 + 8 * stage, fb = full0 + 8 * stage;
+          while (!tc::mbar_try_wait_u32(eb, phase ^ 1)) {}
+          if (tc::elect_one()) {
+            tc::mbar_expect_tx_u32(fb, kStageBytes);
+            tc::tma_load_2d_u32(sa0 + stage * kABytes, &tmap_h, fb, k0, m0);
+            const uint32_t sb = sb0 + stage * kBBytes + crank * (kBBytes / kCtas);     // this CTA's half of the W tile
+#pragma unroll
+            for (int j = 0; j < BN / kCtas / 64; ++j) tc::tma_load_2d_mc(sb + j * 8192, &tmap_w, fb, n0 + 64 * j, k0, 3);
+          }
+          __syncwarp();
+          if (++stage == kStages) { stage = 0; phase ^= 1; }
+        }
+      }
+    }
+  } else {
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 224;" ::: "memory");
+    // ===================================================================== consumers: wgmma main loop + epilogue
+    const int wg = (warp - kConsWarp0) >> 2;             // rows [64 wg, +64) of the CTA's 128
+    const int wq = warp & 3;
+    const uint32_t full0 = tc::smem_u32(full), empty0 = tc::smem_u32(empty);
+    const uint32_t empty0_peer = mapa(empty0, crank ^ 1u);
+    const uint64_t da0 = tc::desc_kmajor_sw128(tc::smem_u32(smem_a) + wg * 8192);
+    const uint64_t db0 = tc::desc_mnmajor_sw128(tc::smem_u32(smem_b));
+    auto release = [&](uint32_t st) {                     // this warp has finished reading stage st (in both CTAs)
+      if (lane == 0) {
+        tc::mbar_arrive_u32(empty0 + 8 * st);
+        mbar_arrive_cluster(empty0_peer + 8 * st);
+      }
+    };
+    float scale = 0.f;
+    if (kMode == kDlogits) scale = *p.dloss / (float)*p.count;
+    uint32_t stage = 0, phase = 0;
+    for (int tile = cluster_id; tile < num_tiles; tile += num_clusters) {
+      int tm, tn;
+      tile_coords(tile, tiles_m, tiles_n, tm, tn);
+      const int m0 = p.row0 + tm * TM + (int)crank * BM, n0 = tn * BN;
+      float acc[BN / 2];
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      uint32_t prev = 0;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        while (!tc::mbar_try_wait_u32(full0 + 8 * stage, phase)) {}
+        const uint64_t da = da0 + (uint64_t)(stage * (kABytes >> 4));
+        const uint64_t db = db0 + (uint64_t)(stage * (kBBytes >> 4));
+        tc::fence_regs(acc);
+        tc::wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / 16; ++k)
+          tc::Wgmma<BN, 0, 1>::mma(acc, da + k * (32 >> 4), db + k * (2048 >> 4), (kb > 0 || k > 0) ? 1u : 0u);
+        tc::wgmma_commit();
+        tc::fence_regs(acc);
+        if (kb > 0) { tc::wgmma_wait<1>(); release(prev); }     // the previous stage's MMAs have retired
+        prev = stage;
+        if (++stage == kStages) { stage = 0; phase ^= 1; }
+      }
+      tc::wgmma_wait<0>();
+      tc::fence_regs(acc);
+      release(prev);                                            // the ring moves on to the next tile during this epilogue
+
+      const int cq = n0 + 2 * (lane & 3);
+      int y[2];
+      bool valid[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int row = m0 + 64 * wg + 16 * wq + (lane >> 2) + 8 * h;
+        valid[h] = row < p.row0 + p.rows;
+        const int t = row / p.B, b = row - t * p.B;
+        const bool counted = valid[h] && (p.lengths == nullptr || t < p.lengths[b]);
+        y[h] = counted ? (int)p.labels[(size_t)b * p.T + t] : -1;      // -1: an uncounted row
+      }
+      const int row_lo = m0 + 64 * wg + 16 * wq + (lane >> 2);
+      if (kMode == kFwd) {
+        // l = acc + bias; classes beyond C (C % 8 == 0: whole 8-column groups) become -inf, so the passes below skip them
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          const int col = cq + 8 * j;
+          if (col < p.C) {
+            const float2 b = *reinterpret_cast<const float2*>(p.bias + col);
+            acc[4 * j] += b.x; acc[4 * j + 1] += b.y; acc[4 * j + 2] += b.x; acc[4 * j + 3] += b.y;
+          } else {
+            acc[4 * j] = acc[4 * j + 1] = acc[4 * j + 2] = acc[4 * j + 3] = -INFINITY;
+          }
+        }
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float mx = -INFINITY, ly = 0.f;
+          int arg = 0x7fffffff;
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const float l = acc[4 * j + 2 * h + e];
+              const int col = cq + 8 * j + e;
+              if (l > mx) { mx = l; arg = col; }                // ascending columns: the smallest index wins a tie
+              if (col == y[h]) ly = l;
+            }
+#pragma unroll
+          for (int o = 1; o < 4; o <<= 1) {
+            const float m2 = __shfl_xor_sync(0xffffffffu, mx, o);
+            const int a2 = __shfl_xor_sync(0xffffffffu, arg, o);
+            if (m2 > mx || (m2 == mx && a2 < arg)) { mx = m2; arg = a2; }
+            ly += __shfl_xor_sync(0xffffffffu, ly, o);
+          }
+          float se = 0.f;
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j) se += __expf(acc[4 * j + 2 * h] - mx) + __expf(acc[4 * j + 2 * h + 1] - mx);
+#pragma unroll
+          for (int o = 1; o < 4; o <<= 1) se += __shfl_xor_sync(0xffffffffu, se, o);
+          if (valid[h] && (lane & 3) == 0)
+            p.part[(size_t)(row_lo + 8 * h) * tiles_n + tn] = make_float4(mx, se, __int_as_float(arg), ly);
+        }
+      } else {
+        float lse[2];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) lse[h] = valid[h] ? p.lse[row_lo + 8 * h] : 0.f;
+        __nv_bfloat16* drow = p.dl + (size_t)(row_lo - p.row0) * p.C;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          const int col = cq + 8 * j;
+          if (col < p.C) {
+            const float2 b = *reinterpret_cast<const float2*>(p.bias + col);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              if (valid[h]) {
+                float d0 = 0.f, d1 = 0.f;
+                if (y[h] >= 0) {
+                  d0 = (__expf(acc[4 * j + 2 * h] + b.x - lse[h]) - (col == y[h] ? 1.f : 0.f)) * scale;
+                  d1 = (__expf(acc[4 * j + 2 * h + 1] + b.y - lse[h]) - (col + 1 == y[h] ? 1.f : 0.f)) * scale;
+                }
+                *reinterpret_cast<__nv_bfloat162*>(drow + (size_t)(8 * h) * p.C + col) = __floats2bfloat162_rn(d0, d1);
+              }
+            }
+          }
+        }
+      }
+    }
+  }
+
+  __syncthreads();
+  cluster_sync();                                // nobody leaves while the peer may still multicast into / arrive on its smem
+}
+
+// ---- combine ----------------------------------------------------------------------------------------------------------------
+constexpr int kCombWarps = 16;                   // rows per block
+
+struct CombineParams {
+  const float4* part;          // [R, nt]
+  const long long* labels;
+  const int* lengths;
+  float* lse;                  // [R]
+  float* part_loss;            // [gridDim.x]
+  int* part_ok;                // [gridDim.x]
+  unsigned int* ticket;        // [1]: 0 on entry, left 0
+  float* loss;
+  int* correct;
+  int* count;
+  int R, T, B, nt;
+};
+
+// One warp per row: lane i merges class tiles i, i + 32, ... in ascending order, then the lanes merge in a fixed tree.
+__global__ void __launch_bounds__(kCombWarps * 32) vocab_head_combine_kernel(const CombineParams p) {
+  __shared__ float red_f[kCombWarps];
+  __shared__ int red_i[kCombWarps];
+  __shared__ int n_s, last_s;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  // N = sum of lengths (T·B without): every block sums the B ints itself (exact, so the order does not matter)
+  int N = p.T * p.B;
+  if (p.lengths != nullptr) {
+    if (threadIdx.x == 0) n_s = 0;
+    __syncthreads();
+    int s = 0;
+    for (int b = threadIdx.x; b < p.B; b += blockDim.x) s += p.lengths[b];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if (lane == 0 && s) atomicAdd(&n_s, s);
+    __syncthreads();
+    N = n_s;
+  }
+  const int row = blockIdx.x * kCombWarps + warp;
+  float nll = 0.f;
+  int ok = 0;
+  if (row < p.R) {
+    float mx = -INFINITY, se = 0.f, ly = 0.f;
+    int arg = 0x7fffffff;
+    for (int i = lane; i < p.nt; i += 32) {
+      const float4 v = p.part[(size_t)row * p.nt + i];
+      const int a = __float_as_int(v.z);
+      if (v.x > mx) { se = se * __expf(mx - v.x) + v.y; mx = v.x; arg = a; }
+      else se += v.y * __expf(v.x - mx);
+      ly += v.w;
+    }
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const float m2 = __shfl_xor_sync(0xffffffffu, mx, o), s2 = __shfl_xor_sync(0xffffffffu, se, o);
+      const int a2 = __shfl_xor_sync(0xffffffffu, arg, o);
+      ly += __shfl_xor_sync(0xffffffffu, ly, o);
+      const float m = fmaxf(mx, m2);
+      if (m != -INFINITY) se = se * __expf(mx - m) + s2 * __expf(m2 - m);
+      if (m2 > mx || (m2 == mx && a2 < arg)) arg = a2;
+      mx = m;
+    }
+    const float lse = mx + __logf(se);
+    if (lane == 0) {
+      p.lse[row] = lse;
+      const int t = row / p.B, b = row - t * p.B;
+      if (p.lengths == nullptr || t < p.lengths[b]) {
+        nll = lse - ly;
+        ok = arg == (int)p.labels[(size_t)b * p.T + t] ? 1 : 0;
+      }
+    }
+  }
+  if (lane == 0) { red_f[warp] = nll; red_i[warp] = ok; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float s = 0.f;
+    int k = 0;
+    for (int w = 0; w < kCombWarps; ++w) { s += red_f[w]; k += red_i[w]; }
+    p.part_loss[blockIdx.x] = s;
+    p.part_ok[blockIdx.x] = k;
+    __threadfence();
+    last_s = atomicAdd(p.ticket, 1u) == gridDim.x - 1;
+  }
+  __syncthreads();
+  if (last_s && warp == 0) {                     // the last block sums every block's partial: lane-strided, then a fixed tree
+    __threadfence();
+    const volatile float* pl = p.part_loss;
+    const volatile int* po = p.part_ok;
+    float s = 0.f;
+    int k = 0;
+    for (int i = lane; i < (int)gridDim.x; i += 32) { s += pl[i]; k += po[i]; }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) { s += __shfl_xor_sync(0xffffffffu, s, o); k += __shfl_xor_sync(0xffffffffu, k, o); }
+    if (lane == 0) {
+      *p.loss = s / (float)N;
+      *p.correct = k;
+      *p.count = N;
+      *p.ticket = 0u;
+    }
+  }
+}
+
+// ---- db ---------------------------------------------------------------------------------------------------------------------
+// Block (32, 8): 64 columns; thread (x, y) sums rows y, y + 8, ... of its column pair, then y = 0 adds the 8 sums in order.
+__global__ void __launch_bounds__(256) vocab_head_colsum_kernel(const __nv_bfloat16* __restrict__ dl, float* __restrict__ db, int rows,
+                                                                int C, int accumulate) {
+  __shared__ float2 red[8][32];
+  const int col = (blockIdx.x * 32 + threadIdx.x) * 2;
+  float2 s = make_float2(0.f, 0.f);
+  if (col < C) {
+#pragma unroll 4
+    for (int r = threadIdx.y; r < rows; r += 8) {
+      const float2 v = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(dl + (size_t)r * C + col));
+      s.x += v.x; s.y += v.y;
+    }
+  }
+  red[threadIdx.y][threadIdx.x] = s;
+  __syncthreads();
+  if (threadIdx.y == 0 && col < C) {
+    for (int y = 1; y < 8; ++y) { s.x += red[y][threadIdx.x].x; s.y += red[y][threadIdx.x].y; }
+    if (accumulate) { s.x += db[col]; s.y += db[col + 1]; }
+    db[col] = s.x; db[col + 1] = s.y;
+  }
+}
+
+template <int kMode>
+int launch_gemm(const void* h, const void* Wb, const VocabParams& p, int dev, cudaStream_t st) {
+  if (p.H % BK != 0 || p.C % 8 != 0 || p.C < 8 || p.rows < 1) { ts::set_last_error("vocab head: needs H % 64 == 0 and C % 8 == 0"); return -2; }
+  CUtensorMap th, tw;
+  if (int rc = ts::make_tmap_2d_bf16(&th, h, (uint64_t)p.R, (uint64_t)p.H, (uint64_t)p.H, BK, BM)) return rc;
+  if (int rc = ts::make_tmap_2d_bf16(&tw, Wb, (uint64_t)p.H, (uint64_t)p.C, (uint64_t)p.C, 64, BK)) return rc;
+  auto kern = vocab_head_gemm_kernel<kMode>;
+  static bool attr_set = false;
+  if (!attr_set) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);
+    if (e != cudaSuccess) return (int)e;
+    attr_set = true;
+  }
+  const int tiles = ((p.rows + TM - 1) / TM) * ((p.C + BN - 1) / BN);
+  int clusters = ts::sm_count(dev) / kCtas;
+  if (clusters < 1) clusters = 1;
+  if (tiles < clusters) clusters = tiles;
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3(clusters * kCtas); cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = kSmemBytes; cfg.stream = st;
+  cudaLaunchAttribute at[1];
+  at[0].id = cudaLaunchAttributeClusterDimension;
+  at[0].val.clusterDim.x = kCtas; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
+  cfg.attrs = at; cfg.numAttrs = 1;
+  return (int)cudaLaunchKernelEx(&cfg, kern, th, tw, p);
+}
+
+}  // namespace
+
+// Scratch of the forward: part = float4 [R, ts_vocab_head_parts(C)]; part_loss / part_ok = [ts_vocab_head_blocks(R)]; 1 zeroed
+// ticket word (left zeroed).
+extern "C" int ts_vocab_head_parts(int C) { return (C + BN - 1) / BN; }
+extern "C" int ts_vocab_head_blocks(int R) { return (R + kCombWarps - 1) / kCombWarps; }
+
+// h: bf16 [R = T·B, H] packed time-major rows, Wb: bf16 [H, C] packed, labels int64 [B, T], lengths int32 [B] or null.
+// -> lse [R], loss (mean NLL over the counted rows), correct, count (N) [1] each.
+extern "C" int ts_vocab_head_fwd(const void* h, const void* Wb, const float* bias, const long long* labels, const int* lengths,
+                                 void* part, float* lse, float* part_loss, int* part_ok, unsigned int* ticket, float* loss,
+                                 int* correct, int* count, int T, int B, int H, int C, int dev, cudaStream_t st) {
+  const int R = T * B;
+  VocabParams p{};
+  p.bias = bias; p.labels = labels; p.lengths = lengths; p.part = reinterpret_cast<float4*>(part);
+  p.R = R; p.H = H; p.C = C; p.T = T; p.B = B; p.row0 = 0; p.rows = R;
+  if (int rc = launch_gemm<kFwd>(h, Wb, p, dev, st)) return rc;
+  CombineParams c{reinterpret_cast<const float4*>(part), labels, lengths, lse, part_loss, part_ok, ticket, loss, correct, count,
+                  R, T, B, ts_vocab_head_parts(C)};
+  vocab_head_combine_kernel<<<ts_vocab_head_blocks(R), kCombWarps * 32, 0, st>>>(c);
+  return (int)cudaGetLastError();
+}
+
+// dl [rows, C] bf16 = dlogits of rows [row0, row0 + rows) of h (see the top of the file); lse / count from the forward.
+extern "C" int ts_vocab_head_dlogits(const void* h, const void* Wb, const float* bias, const long long* labels, const int* lengths,
+                                     const float* lse, const float* dloss, const int* count, void* dl, int T, int B, int H, int C,
+                                     int row0, int rows, int dev, cudaStream_t st) {
+  VocabParams p{};
+  p.bias = bias; p.labels = labels; p.lengths = lengths; p.lse = lse; p.dloss = dloss; p.count = count;
+  p.dl = reinterpret_cast<__nv_bfloat16*>(dl);
+  p.R = T * B; p.H = H; p.C = C; p.T = T; p.B = B; p.row0 = row0; p.rows = rows;
+  if (row0 < 0 || row0 % BM != 0 || row0 + rows > p.R) { ts::set_last_error("vocab head: a chunk starts at a multiple of 128 rows inside h"); return -2; }
+  return launch_gemm<kDlogits>(h, Wb, p, dev, st);
+}
+
+// db [C] (+)= column sums of dl [rows, C] (bf16), C even.
+extern "C" int ts_vocab_head_colsum(const void* dl, float* db, int rows, int C, int accumulate, cudaStream_t st) {
+  vocab_head_colsum_kernel<<<(C + 63) / 64, dim3(32, 8), 0, st>>>(reinterpret_cast<const __nv_bfloat16*>(dl), db, rows, C, accumulate);
+  return (int)cudaGetLastError();
+}

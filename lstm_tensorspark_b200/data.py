@@ -195,9 +195,12 @@ def process_batch_per_step(train_xy: Sequence[Sequence[str]], seq_len: int, in_f
 
 
 def process_tokens(train_xy: Sequence[Sequence[str]], seq_len: int, vocab_size: int, num_classes: int = 0,
-                   variable_length: bool = False, per_step_labels: bool = False):
+                   variable_length: bool = False, per_step_labels: bool = False, next_token: bool = False):
     """Rows of token ids (``--vocab_size``) -> ``(x int32 [N, seq_len] ([N] when seq_len == 1), y int64 [N] or [N, seq_len])``,
     plus ``lengths`` int32 [N] with ``variable_length``.
+
+    ``next_token`` (``--next_token``): a row is ``k`` ids and nothing else, ``k = seq_len + 1``, or ``2 <= k <= seq_len + 1`` with
+    ``variable_length``; the input is ids ``0..k-2``, the label of step t is id ``t + 1`` and the length is ``k - 1``.
 
     A row is ``k`` ids followed by the label, or with ``per_step_labels`` by ``k`` labels; ``k = seq_len``, or
     ``1 <= k <= seq_len`` with ``variable_length`` (then padded on the right with id 0, label 0, never read).  A non-integer id,
@@ -206,19 +209,29 @@ def process_tokens(train_xy: Sequence[Sequence[str]], seq_len: int, vocab_size: 
     if seq_len < 1 or vocab_size < 1:
         raise ValueError("token rows need seq_len >= 1 and vocab_size >= 1")
     want = f"1..{seq_len}" if variable_length else f"{seq_len}"
+    if next_token:
+        if seq_len < 2:
+            raise ValueError("next-token rows need seq_len >= 2")
+        per_step_labels = True
+        want = f"2..{seq_len + 1}" if variable_length else f"{seq_len + 1}"
     xs, ys, ls = [], [], []
     for n, row in enumerate(train_xy):
-        if len(row) <= 1:
+        if len(row) <= 1 and not next_token:
             continue
-        if per_step_labels:
+        if next_token:
+            k, rem = len(row) - 1, 0                   # k steps: the last id is a label only
+        elif per_step_labels:
             k, rem = divmod(len(row), 2)
         else:
             k, rem = len(row) - 1, 0
         if rem or not (k == seq_len or (variable_length and 1 <= k <= seq_len)):
+            if next_token:
+                raise ValueError(f"row {n}: {len(row)} fields is not {want} token ids (--next_token: every id but the last is "
+                                 "an input, every id but the first a label)")
             raise ValueError(f"row {n}: {len(row)} fields is not {want} token ids followed by "
                              f"{'one label per step' if per_step_labels else 'the label'}")
         ids = []
-        for v in row[:k]:
+        for v in row[:k + 1 if next_token else k]:
             s = str(v).strip()
             try:
                 i = int(s)
@@ -227,8 +240,11 @@ def process_tokens(train_xy: Sequence[Sequence[str]], seq_len: int, vocab_size: 
             if not 0 <= i < vocab_size:
                 raise ValueError(f"row {n}: token id {i} outside [0, {vocab_size}) (--vocab_size {vocab_size})")
             ids.append(i)
-        lab = [int(float(v)) for v in row[k:]]
-        if per_step_labels:
+        if next_token:
+            ids, lab = ids[:-1], ids[1:]
+        else:
+            lab = [int(float(v)) for v in row[k:]]
+        if per_step_labels and not next_token:
             bad = [v for v in lab if not 0 <= v < num_classes]
             if bad:
                 raise ValueError(f"row {n}: label {bad[0]} outside [0, {num_classes})")
@@ -255,7 +271,8 @@ def parse_rows(rows: Sequence[Sequence[str]], cfg):
     ``--variable_length``); ``lengths`` is None unless ``cfg.variable_length``."""
     if cfg.vocab_size > 0:
         x, y, *lengths = process_tokens(rows, cfg.seq_len, cfg.vocab_size, cfg.num_classes,
-                                        variable_length=cfg.variable_length, per_step_labels=cfg.per_step_labels)
+                                        variable_length=cfg.variable_length, per_step_labels=cfg.per_step_labels,
+                                        next_token=getattr(cfg, "next_token", False))
     elif cfg.per_step_labels:
         x, y, *lengths = process_batch_per_step(rows, cfg.seq_len, cfg.in_features, cfg.num_classes,
                                                 variable_length=cfg.variable_length, normalize=cfg.normalize)
@@ -384,6 +401,47 @@ def synthetic_tokens(n: int, seq_len: int, vocab_size: int, num_classes: int, se
     return (x, y) if lengths is None else (x, y, lengths)
 
 
+NEXT_TOKEN_PROBS = (0.6, 0.2, 0.1, 0.1)
+# entropy of a step of the chain below in nats: the loss a perfect model reaches (perplexity exp(1.0889) = 2.97)
+NEXT_TOKEN_ENTROPY = -sum(p * float(np.log(p)) for p in NEXT_TOKEN_PROBS)
+
+
+def next_token_chain(vocab_size: int, seed: int = 0) -> np.ndarray:
+    """The successor table ``[V, 4]`` of the synthetic language (``synthetic_next_token``): id i is followed by
+    ``succ[i, j]`` with probability ``NEXT_TOKEN_PROBS[j]``; the four successors of an id are distinct."""
+    if vocab_size < 4:
+        raise ValueError("the synthetic next-token chain needs vocab_size >= 4")
+    rng = np.random.default_rng([seed, 0x6E7874])
+    base = rng.integers(0, vocab_size, size=vocab_size)
+    step = rng.integers(1, max(1, (vocab_size - 1) // 3) + 1, size=vocab_size)
+    return ((base[:, None] + np.arange(4)[None, :] * step[:, None]) % vocab_size).astype(np.int64)
+
+
+def synthetic_next_token(n: int, seq_len: int, vocab_size: int, seed: int = 0, variable_length: bool = False):
+    """A learnable language (``--next_token``): a fixed sparse first-order Markov chain over the ids (``next_token_chain``), so
+    the achievable loss is known in closed form (``NEXT_TOKEN_ENTROPY``).  ``n`` walks of ``seq_len + 1`` ids from a uniform
+    start -> ``(x int32 [n, T] = ids 0..T-1, y int64 [n, T] = ids 1..T)``, plus ``lengths`` with ``variable_length`` (those of
+    ``synthetic_lengths``; padded steps hold id 0 and label 0).  Drawn by a generator of its own: the draws of the other
+    synthetic tasks are untouched."""
+    if seq_len < 2:
+        raise ValueError("next-token sequences need seq_len >= 2")
+    succ = next_token_chain(vocab_size, seed)
+    rng = np.random.default_rng([seed, 0x6E7874, 1])
+    tok = np.empty((n, seq_len + 1), dtype=np.int64)
+    tok[:, 0] = rng.integers(0, vocab_size, size=n)
+    pick = rng.choice(4, size=(n, seq_len), p=NEXT_TOKEN_PROBS)
+    for t in range(seq_len):
+        tok[:, t + 1] = succ[tok[:, t], pick[:, t]]
+    x, y = tok[:, :-1].astype(np.int32), tok[:, 1:].copy()
+    if not variable_length:
+        return x, y
+    lengths = synthetic_lengths(n, seq_len, seed)
+    pad = np.arange(seq_len)[None, :] >= lengths[:, None]
+    x[pad] = 0
+    y[pad] = 0
+    return x, y, lengths
+
+
 def synthetic_lengths(n: int, seq_len: int, seed: int = 0) -> np.ndarray:
     """Per-sample lengths, uniform in ``[max(1, seq_len // 4), seq_len]``, int32, from a generator seeded apart from the data's."""
     rng = np.random.default_rng([seed, 0x6C656E])
@@ -393,7 +451,9 @@ def synthetic_lengths(n: int, seq_len: int, seed: int = 0) -> np.ndarray:
 def synthetic(cfg, n: int, seed: int):
     """``n`` synthetic samples of the task the flags of ``cfg`` select -> ``(x, y, lengths)``; ``lengths`` is None unless
     ``cfg.variable_length``."""
-    if cfg.vocab_size > 0:
+    if getattr(cfg, "next_token", False):
+        x, y, *lengths = synthetic_next_token(n, cfg.seq_len, cfg.vocab_size, seed=seed, variable_length=cfg.variable_length)
+    elif cfg.vocab_size > 0:
         x, y, *lengths = synthetic_tokens(n, cfg.seq_len, cfg.vocab_size, cfg.num_classes, seed=seed,
                                           variable_length=cfg.variable_length, per_step_labels=cfg.per_step_labels)
     elif cfg.per_step_labels:

@@ -165,10 +165,14 @@ class SequenceClassifier(nn.Module):
 
     def forward(self, x: torch.Tensor, labels: torch.Tensor, lengths: Optional[torch.Tensor] = None):
         """-> (loss, logits, correct_count); with ``--per_step_labels`` logits are ``[B,T,C]`` and the loss and the count run over
-        the counted positions (``ops.reference.head_xent_per_step``)."""
+        the counted positions (``ops.reference.head_xent_per_step``).  Where the large-vocabulary head runs
+        (``ops.functional.vocab_head_supported``: bf16 on the GPU, 512 classes or more) no logits exist and the slot holds None."""
         self.check_labels(labels)
         if self.per_step:
             h_seq = self.sequence_features(x, lengths)
+            if F.vocab_head_supported(h_seq, self.cfg.num_classes):
+                loss, correct, _n = F.vocab_xent_per_step(h_seq, self.head.weights, self.head.bias, labels, lengths)
+                return loss, None, correct
             logits, loss, correct, _n = F.head_xent_per_step(h_seq, self.head.weights, self.head.bias, labels, lengths)
             return loss, logits, correct
         h = self.features(x, lengths)
@@ -182,15 +186,23 @@ class SequenceClassifier(nn.Module):
         otherwise.  The whole batch runs through the stack, so a tail can be scored in a batch of the usual static shape."""
         from ..ops import reference as ref
         self.check_labels(labels)
-        labels = labels[first:]
         if self.per_step:
             h_seq = self.sequence_features(x, lengths)
+            if F.vocab_head_supported(h_seq, self.cfg.num_classes):
+                # the tail is a mask, not a slice: rows before `first` get length 0, and no [rows, C] array is ever built
+                if first > 0:
+                    B, T = labels.shape
+                    full = torch.full((B,), T, dtype=torch.int32, device=h_seq.device) if lengths is None else lengths
+                    lengths = torch.where(torch.arange(B, device=h_seq.device) < first, torch.zeros_like(full), full)
+                return F.vocab_xent_per_step(h_seq, self.head.weights, self.head.bias, labels, lengths)
+            labels = labels[first:]
             if first == 0:
                 _logits, loss, correct, n = F.head_xent_per_step(h_seq, self.head.weights, self.head.bias, labels, lengths)
                 return loss, correct, n
             h_seq = h_seq[:, first:]
             logits = self.head(h_seq.reshape(-1, h_seq.shape[2])).float().view(h_seq.shape[0], h_seq.shape[1], -1)
             return ref.softmax_xent_per_step(logits.transpose(0, 1), labels, None if lengths is None else lengths[first:])
+        labels = labels[first:]
         logits = self.head(self.features(x, lengths))[first:].float()
         count = torch.full((), labels.shape[0], dtype=torch.int64, device=logits.device)
         return ref.softmax_xent(logits, labels), (logits.argmax(1) == labels).sum(), count
@@ -212,11 +224,20 @@ class SequenceClassifier(nn.Module):
 
     def check_compatible(self, variables: Dict[str, torch.Tensor], settings: Dict, what: str = "checkpoint") -> None:
         """Raise unless ``variables`` and the flags ``settings`` recorded beside them (``utils.checkpoint.recorded_settings``)
-        were written by a model this one can load: the same directions, ``--pooling`` and ``--vocab_size``, checked in that
-        order."""
+        were written by a model this one can load: the same directions, ``--pooling``, ``--vocab_size`` and ``--next_token``,
+        checked in that order."""
         self.check_directions(variables, what)
         self.check_pooling(variables, settings.get("pooling"), what)
         self.check_vocab(variables, settings.get("vocab_size"), what)
+        self.check_next_token(settings.get("next_token"), what)
+
+    def check_next_token(self, recorded: Optional[bool] = None, what: str = "checkpoint") -> None:
+        """Raise unless the file was written with this run's ``--next_token`` (nothing recorded counts as off): the variables
+        have the same shapes either way, but a head trained on given labels does not predict the next token."""
+        saved, mine = bool(recorded), bool(getattr(self.cfg, "next_token", False))
+        if saved != mine:
+            raise ValueError(f"{what} was written {'with' if saved else 'without'} --next_token, this run is "
+                             f"{'with' if mine else 'without'} it: {'add' if saved else 'drop'} --next_token")
 
     def check_vocab(self, variables: Dict[str, torch.Tensor], recorded: Optional[int] = None, what: str = "checkpoint") -> None:
         """Raise unless ``variables`` (and the vocabulary ``recorded`` beside them; nothing recorded: the table's row count, or 0

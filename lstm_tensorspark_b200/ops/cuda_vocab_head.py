@@ -1,0 +1,83 @@
+"""CUDA op of the large-vocabulary per-step head (csrc/head_vocab.cu): softmax cross-entropy over ``C >= 512`` classes at every
+time step without storing the logits ``[B,T,C]`` or an fp32 dlogits ``[T·B,C]``.
+
+Forward: one fused TMA + wgmma launch reduces every 128 x 256 logit tile to four numbers per row in its epilogue, a second small
+launch merges them into ``lse [T·B]``, the loss, the correct count and N.  Backward, in chunks of ``ROW_CHUNK`` rows, in index
+order on one stream: the logits of the chunk are recomputed and turned into bf16 dlogits in a reused scratch ``[ROW_CHUNK, C]``,
+then ``dh = dlogits W^T``, ``dW += h^T dlogits`` (straight into the flat gradient buffer) and ``db += column sums`` - every sum in
+a fixed order, so two calls on the same inputs give the same bits.  N, lse and the masks stay on the device: a captured CUDA
+graph holds across batches with other lengths.
+"""
+from __future__ import annotations
+
+import torch
+
+from . import cuda_gemm as G
+from .cuda_ext import ext
+
+ROW_CHUNK = 4096          # rows of h per backward chunk: the schedule depends on the shapes only
+MIN_CLASSES = 512
+
+
+def supported(h_seq: torch.Tensor, num_classes: int) -> bool:
+    """Does this op take the head (bf16 activations on the GPU, ``H % 64 == 0``, ``C % 8 == 0``, ``C >= 512``)?  Everything
+    else stays with ``cuda_head.head_xent_per_step``."""
+    return (h_seq.is_cuda and h_seq.dtype == torch.bfloat16 and h_seq.dim() == 3 and h_seq.shape[2] % 64 == 0
+            and num_classes % 8 == 0 and num_classes >= MIN_CLASSES)
+
+
+class _VocabXentFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, h_seq, weights, bias, labels, lengths):
+        from .cuda_lstm import STATS, _lowp
+        E = ext()
+        T, B, H = h_seq.shape
+        hc = h_seq.detach()
+        h2 = hc.reshape(T * B, H) if hc.is_contiguous() else hc.contiguous().view(T * B, H)
+        wb = _lowp(weights, torch.bfloat16)                   # the maintained bf16 shadow, or one rounding of the fp32 weights
+        b = bias.detach().float().contiguous()
+        lab = labels.long().contiguous()
+        ln = None if lengths is None else lengths.contiguous()
+        part = torch.empty(T * B * E.vocab_head_parts(wb.shape[1]) * 4, dtype=torch.float32, device=h2.device)
+        lse, loss, correct, count = E.vocab_head_fwd(h2, wb, b, lab, ln, T, part)
+        STATS["vocab_head_fwd"] = STATS.get("vocab_head_fwd", 0) + 1
+        ctx.save_for_backward(h2, wb, b, lab, ln, lse, count)
+        ctx.shape = (T, B, H)
+        ctx.addrs = (weights.data_ptr(), bias.data_ptr())
+        ctx.mark_non_differentiable(correct, count)
+        return loss.squeeze(0), correct.squeeze(0), count.squeeze(0)
+
+    @staticmethod
+    def backward(ctx, dloss, _dcorrect_unused, _dcount_unused):
+        from .cuda_lstm import STATS, grad_sink
+        E = ext()
+        h2, wb, b, lab, ln, lse, count = ctx.saved_tensors
+        T = ctx.shape[0]
+        R, H = h2.shape
+        C = wb.shape[1]
+        sw, sb = grad_sink(ctx.addrs[0]), grad_sink(ctx.addrs[1])
+        scale = dloss.detach().float().reshape(1).contiguous()
+        if sw is not None and sb is not None:
+            (dw, acc_w), (db, acc_b) = sw, sb
+            ret = (None, None)
+        else:
+            dw = torch.empty(H, C, dtype=torch.float32, device=h2.device)
+            db = torch.empty(C, dtype=torch.float32, device=h2.device)
+            acc_w = acc_b = False
+            ret = (dw, db)
+        dh = torch.empty_like(h2)
+        dl = torch.empty(min(ROW_CHUNK, R), C, dtype=torch.bfloat16, device=h2.device)
+        for r0 in range(0, R, ROW_CHUNK):
+            rows = min(ROW_CHUNK, R - r0)
+            d = dl[:rows]
+            E.vocab_head_dlogits(h2, wb, b, lab, ln, T, lse, count, scale, r0, rows, d)
+            G.matmul(d, wb, out=dh[r0:r0 + rows])                                              # dh = dlogits W^T
+            G.matmul(h2[r0:r0 + rows].t(), d.t(), out=dw, accumulate=bool(acc_w or r0 > 0))    # dW (+)= h^T dlogits
+            E.vocab_head_colsum(d, db.view(-1), bool(acc_b or r0 > 0))
+        STATS["vocab_head_bwd"] = STATS.get("vocab_head_bwd", 0) + 1
+        return dh.view(ctx.shape), ret[0], ret[1], None, None
+
+
+def vocab_xent_per_step(h_seq, weights, bias, labels, lengths=None):
+    """-> (mean loss over the counted positions, correct count, N); see ``ops.functional.vocab_xent_per_step``."""
+    return _VocabXentFn.apply(h_seq, weights, bias, labels, lengths)

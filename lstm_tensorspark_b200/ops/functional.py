@@ -77,6 +77,29 @@ def head_xent_per_step(h_seq, weights, bias, labels, lengths=None):
     return ref.head_xent_per_step(h_seq, weights, bias, labels, lengths)
 
 
+def vocab_head_supported(h_seq, num_classes: int) -> bool:
+    """Does ``vocab_xent_per_step`` run its own GPU kernels on this input (bf16 on the CUDA backend, ``H % 64 == 0``,
+    ``C % 8 == 0``, ``C >= 512``)?  Otherwise it is the composition through ``head_xent_per_step``."""
+    if not _use_ext(h_seq):
+        return False
+    from . import cuda_vocab_head
+    return cuda_vocab_head.supported(h_seq, num_classes)
+
+
+def vocab_xent_per_step(h_seq, weights, bias, labels, lengths=None):
+    """The per-step head for many classes (a next-token language model's softmax): the loss, the correct count and N of
+    ``head_xent_per_step`` - the same mask, normalisation and gradients - without the logits, which are neither returned nor
+    stored.  ``lengths`` may hold zeros here (a row that does not count at all).  On the GPU bf16 ``h_seq`` with
+    ``H % 64 == 0``, ``C % 8 == 0`` and ``C >= 512`` runs on the tensor cores (csrc/head_vocab.cu); every other input goes
+    through ``head_xent_per_step``."""
+    if vocab_head_supported(h_seq, weights.shape[1]):
+        from . import cuda_vocab_head
+        return cuda_vocab_head.vocab_xent_per_step(h_seq, weights, bias, labels, lengths)
+    if _use_ext(h_seq):
+        return head_xent_per_step(h_seq, weights, bias, labels, lengths)[1:]
+    return ref.vocab_xent_per_step(h_seq, weights, bias, labels, lengths)
+
+
 def pool_sequence(h_seq, lengths=None, mode: str = "mean", attention=None):
     """Pool ``h_seq [T,B,H]`` over each row's counted steps -> ``s [B,H]`` fp32 (``reference.pool_sequence``); ``mode`` mean,
     max or attention (``attention = (W_a, b_a, v)``)."""

@@ -243,6 +243,11 @@ def head_xent_per_step(h_seq, weights, bias, labels, lengths=None):
     return logits, loss, correct, keep.sum()
 
 
+def vocab_xent_per_step(h_seq, weights, bias, labels, lengths=None):
+    """``head_xent_per_step`` without the logits -> (loss, correct, N): the reference of the large-vocabulary head."""
+    return head_xent_per_step(h_seq, weights, bias, labels, lengths)[1:]
+
+
 def softmax_xent_per_step(logits, labels, lengths=None):
     """``logits [B,T,C]``, ``labels [B,T]`` -> (mean NLL over counted positions, correct count among them, N)."""
     keep = step_mask(lengths, logits.shape[0], logits.shape[1], device=logits.device)

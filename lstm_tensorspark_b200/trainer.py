@@ -13,6 +13,7 @@ shared by all ranks; a real resume path exists (Q4); replicas start from identic
 from __future__ import annotations
 
 import json
+import math
 import os
 import sys
 import time
@@ -239,10 +240,14 @@ def train_rnn(partition, cfg: Config, rank: int = 0, world_size: int = 1, comm: 
                 if g_norm is not None:                               # the pre-clip norm of this step's gradient
                     sink.add("grad_norm", g_norm)
                     extra["grad_norm"] = g_norm
+                if cfg.next_token:
+                    extra["perplexity"] = math.exp(t_loss)
+                    sink.add("perplexity", extra["perplexity"])
                 sink.flush(step)
                 jlog.write(step=step, loss=t_loss, acc=t_acc, rank=rank, **extra)
             if use_bar:
-                total_steps.set_description("Loss: {:.4f} - t_acc {:.3f}".format(t_loss, t_acc))
+                ppl = " - ppl {:.2f}".format(extra["perplexity"]) if cfg.next_token else ""
+                total_steps.set_description("Loss: {:.4f} - t_acc {:.3f}".format(t_loss, t_acc) + ppl)
 
     # ---- the cross-replica average (src/rnn.py:393-407) ------------------------------------------------
     with M.nvtx_range("final_param_avg", cfg.nvtx):
@@ -415,10 +420,12 @@ def evaluate_job(cfg: Config, standalone: bool = False) -> Dict:
     if eng.model.per_step:
         out["positions"] = count
     out.update(loss=loss_sum / count, accuracy=correct / count, seconds=time.time() - start)
+    if cfg.next_token:
+        out["perplexity"] = math.exp(out["loss"])
     if not cfg.quiet:
         positions = "{positions} positions, " if eng.model.per_step else ""
         print(("RNN-LSTM - eval: model {model}, {samples} samples, " + positions +
-               "loss {loss:.6f}, accuracy {accuracy:.4f}").format(**out))
+               "loss {loss:.6f}, accuracy {accuracy:.4f}" + (", perplexity {perplexity:.4f}" if cfg.next_token else "")).format(**out))
     if cfg.json_log:
         jl = M.JsonLog(cfg.json_log); jl.write(**out); jl.close()
     return out
@@ -451,7 +458,7 @@ def run_job(cfg: Config, standalone: bool = False) -> Dict:
                                  {"world_size": world_size, "sync_mode": cfg.sync_mode, "average_scope": cfg.average_scope,
                                   "hidden_units": cfg.hidden_units, "pooling": cfg.pooling,
                                   "attention_units": cfg.attention_units, "vocab_size": cfg.vocab_size,
-                                  "seconds": total})
+                                  "next_token": cfg.next_token, "seconds": total})
     if not cfg.quiet:
         print("RNN-LSTM - Total Processing Time {}s".format(total))
     return {"results": results, "seconds": total, "world_size": world_size, "partitions": n_shards}

@@ -117,7 +117,7 @@ def load(prefix_path: str) -> Tuple[Dict[str, torch.Tensor], dict, Optional[dict
 
 def recorded_settings(meta: dict) -> dict:
     """The flags a model file recorded: a training checkpoint keeps them under ``meta["config"]``, ``averaged_model.pt`` keeps
-    the ones it records (``pooling``, ``vocab_size``, ...) at the top level of its meta."""
+    the ones it records (``pooling``, ``vocab_size``, ``next_token``, ...) at the top level of its meta."""
     return meta.get("config") or meta
 
 
