@@ -24,6 +24,8 @@ FUSED_CLIP_ERROR = ("--clip_grad_norm with --sync_mode grad_allreduce needs the 
 
 ATTENTION_UNITS_DEFAULT = 128
 NUM_CLASSES_DEFAULT = 3
+MAX_NEW_TOKENS_DEFAULT = 32
+TEMPERATURE_DEFAULT = 1.0
 
 
 @dataclass
@@ -66,6 +68,8 @@ class Config:
                                         # followed by the label (--per_step_labels: by k labels).  0 = float features
     next_token: bool = False            # language modelling (needs --vocab_size V): the label of step t is the token of step t + 1.
                                         # Turns on --per_step_labels and sets --num_classes to V; a CSV row is seq_len + 1 ids
+    max_new_tokens: int = MAX_NEW_TOKENS_DEFAULT  # --mode generate: tokens sampled after each prompt
+    temperature: float = TEMPERATURE_DEFAULT      # --mode generate: sample from softmax(logits / temperature); 0 = greedy
     dtype: str = "auto"                 # auto: bf16 on cuda, fp32 on cpu
     device: str = "auto"                # auto | cpu | cuda
     backend: str = "auto"               # auto | cuda_ext (hand-written sm_90a kernels) | torch
@@ -214,9 +218,20 @@ class Config:
             raise ValueError(f"unknown --data_residency {self.data_residency}")
         if self.remainder not in ("drop", "spread"):
             raise ValueError(f"unknown --remainder {self.remainder}")
-        if self.mode not in ("train", "eval"):
-            raise ValueError("--mode is train (the only one the reference implements, src/rnn.py:371) or eval (score a trained "
-                             "model: --resume <averaged_model.pt | checkpoint dir>, default = what the last training run left)")
+        if self.mode not in ("train", "eval", "generate"):
+            raise ValueError("--mode is train (the only one the reference implements, src/rnn.py:371), eval (score a trained "
+                             "model: --resume <averaged_model.pt | checkpoint dir>, default = what the last training run left) or "
+                             "generate (continue prompts with a --next_token model, found the same way)")
+        if self.max_new_tokens < 1:
+            raise ValueError(f"--max_new_tokens must be >= 1, got {self.max_new_tokens}")
+        if not (math.isfinite(self.temperature) and self.temperature >= 0):
+            raise ValueError(f"--temperature must be a finite number >= 0 (0 = greedy), got {self.temperature}")
+        if self.mode == "generate" and not self.next_token:
+            raise ValueError("--mode generate needs --next_token (and the --vocab_size the model was trained with): it continues "
+                             "token sequences with a next-token language model")
+        for flag, default in (("max_new_tokens", MAX_NEW_TOKENS_DEFAULT), ("temperature", TEMPERATURE_DEFAULT)):
+            if getattr(self, flag) != default and self.mode != "generate":
+                warnings.warn(f"--{flag} {getattr(self, flag)} has no effect without --mode generate")
         return self
 
 
@@ -245,7 +260,11 @@ _HELP = {
     "training_path": "Path to training set",
     "labels_path": "Path to training_labels",
     "output_path": "Path for store network state",
-    "mode": "Execution mode",
+    "mode": "Execution mode: train, eval (score a trained model) or generate (continue the prompts of --training_path, or of "
+            "--synthetic walks, with a --next_token model; writes <output_path>/generated.csv)",
+    "max_new_tokens": "--mode generate: tokens to sample after each prompt (>= 1)",
+    "temperature": "--mode generate: sample from softmax(logits / temperature) by Gumbel-max with noise seeded by --seed; 0 = "
+                   "greedy (the arg-max)",
     "checkpoint_path": "Directory where to save network model and logs",
     "clip_grad_norm": "Clip the gradient by its global L2 norm to this value before the update, as "
                       "torch.nn.utils.clip_grad_norm_ (0 = off); the norm includes the --weight_decay term and, with "

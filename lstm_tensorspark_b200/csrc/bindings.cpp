@@ -8,6 +8,7 @@
 #include <c10/cuda/CUDAException.h>
 #include <cuda_runtime.h>
 
+#include <cmath>
 #include <optional>
 #include <string>
 #include <vector>
@@ -56,6 +57,10 @@ int ts_vocab_head_fwd(const void*, const void*, const float*, const long long*, 
 int ts_vocab_head_dlogits(const void*, const void*, const float*, const long long*, const int*, const float*, const float*, const int*,
                           void*, int, int, int, int, int, int, int, cudaStream_t);
 int ts_vocab_head_colsum(const void*, float*, int, int, int, cudaStream_t);
+int ts_vocab_sample(const void*, const void*, const float*, float, unsigned int, int*, const int*, void*, int*, unsigned int*, int*,
+                    float*, int*, float*, int, int, int, int, int, int, cudaStream_t);
+int ts_vocab_sample_logits(const float*, float, unsigned int, int*, const int*, void*, int*, unsigned int*, int*, float*, int*, float*,
+                           int, int, int, int, cudaStream_t);
 int ts_gemm_generic(const void*, const void*, void*, const float*, int, int, int, long long, long long, long long, long long, long long,
                     int, int, int, float, cudaStream_t);
 int ts_gemm2(const void*, const void*, void*, const float*, int, int, int, int, int, int, int, int, int, int, int, int, int,
@@ -429,6 +434,75 @@ void vocab_head_colsum(const Tensor& dl, Tensor db, bool accumulate) {
               db.numel() == dl.size(1), "vocab head: dl bf16 [rows, C], db fp32 [C]");
   check(ts_vocab_head_colsum(dl.data_ptr(), db.data_ptr<float>(), (int)dl.size(0), (int)dl.size(1), accumulate ? 1 : 0, stream()),
         "vocab_head_colsum");
+}
+
+// ---- sampling the next token (csrc/head_vocab.cu) -------------------------------------------------------------------
+// tokens int32 [B] (written), step int32 [1] (read, advanced by one), row0 int32 [1] (the noise counter's row word of row 0),
+// optional rec_tok int32 / rec_lp fp32 [B, N] (column
+// step - s0 written) -> logprob fp32 [B].  Scratch is allocated here; nothing is read back to the host.
+struct SampleOut {
+  int* rec_tok = nullptr;
+  float* rec_lp = nullptr;
+  int N = 0;
+};
+SampleOut sample_check(int64_t B, const Tensor& like, const Tensor& step, const Tensor& row0, const Tensor& tokens,
+                       const std::optional<Tensor>& rec_tok, const std::optional<Tensor>& rec_lp, double temperature) {
+  chk_cuda(step, "step"); chk_cuda(row0, "row0"); chk_cuda(tokens, "tokens");
+  TORCH_CHECK(row0.scalar_type() == torch::kInt32 && row0.numel() == 1 && row0.device() == like.device(), "vocab sample: row0 int32 [1]");
+  TORCH_CHECK(std::isfinite(temperature) && temperature >= 0, "vocab sample: temperature must be finite and >= 0");
+  TORCH_CHECK(step.scalar_type() == torch::kInt32 && step.numel() == 1 && step.device() == like.device(), "vocab sample: step int32 [1]");
+  TORCH_CHECK(tokens.scalar_type() == torch::kInt32 && tokens.numel() == B && tokens.device() == like.device(), "vocab sample: tokens int32 [B]");
+  SampleOut o;
+  TORCH_CHECK(rec_tok.has_value() == rec_lp.has_value(), "vocab sample: rec_tok and rec_lp go together");
+  if (rec_tok.has_value()) {
+    chk_cuda(*rec_tok, "rec_tok"); chk_cuda(*rec_lp, "rec_lp");
+    TORCH_CHECK(rec_tok->scalar_type() == torch::kInt32 && rec_tok->dim() == 2 && rec_tok->size(0) == B &&
+                rec_lp->scalar_type() == torch::kFloat32 && rec_lp->sizes() == rec_tok->sizes() &&
+                rec_tok->device() == like.device() && rec_lp->device() == like.device(), "vocab sample: records int32 / fp32 [B, N]");
+    o.rec_tok = rec_tok->data_ptr<int>(); o.rec_lp = rec_lp->data_ptr<float>(); o.N = (int)rec_tok->size(1);
+  }
+  return o;
+}
+
+Tensor vocab_sample(const Tensor& h, const Tensor& Wb, const Tensor& bias, double temperature, int64_t seed, Tensor step, const Tensor& row0,
+                    Tensor tokens, const std::optional<Tensor>& rec_tok, const std::optional<Tensor>& rec_lp, int64_t s0) {
+  chk_cuda(h, "h"); chk_cuda(Wb, "Wb"); chk_cuda(bias, "bias");
+  TORCH_CHECK(h.dim() == 2 && Wb.dim() == 2 && h.scalar_type() == torch::kBFloat16 && Wb.scalar_type() == torch::kBFloat16 &&
+              Wb.size(0) == h.size(1) && h.size(0) >= 1 && h.size(0) < (int64_t(1) << 24), "vocab sample: h bf16 [B,H], Wb bf16 [H,C]");
+  TORCH_CHECK(h.size(1) % 64 == 0 && Wb.size(1) % 8 == 0 && Wb.size(1) >= 8, "vocab sample: H % 64 == 0 and C % 8 == 0");
+  TORCH_CHECK(bias.scalar_type() == torch::kFloat32 && bias.numel() == Wb.size(1) && ((uintptr_t)bias.data_ptr() % 8) == 0,
+              "vocab sample: bias fp32 [C]");
+  c10::cuda::CUDAGuard g(h.device());
+  const int B = h.size(0), H = h.size(1), C = Wb.size(1);
+  const SampleOut o = sample_check(B, h, step, row0, tokens, rec_tok, rec_lp, temperature);
+  const int nt = ts_vocab_head_parts(C);
+  auto fo = torch::TensorOptions().device(h.device()).dtype(torch::kFloat32);
+  auto part = torch::empty({(int64_t)B * nt * 4}, fo), logprob = torch::empty({B}, fo);
+  auto part_arg = torch::empty({(int64_t)B * nt}, fo.dtype(torch::kInt32)), ticket = torch::zeros({1}, fo.dtype(torch::kInt32));
+  check(ts_vocab_sample(h.data_ptr(), Wb.data_ptr(), bias.data_ptr<float>(), (float)temperature, (unsigned int)(seed & 0xffffffff),
+                        step.data_ptr<int>(), row0.data_ptr<int>(), part.data_ptr(), part_arg.data_ptr<int>(), (unsigned int*)ticket.data_ptr<int>(),
+                        tokens.data_ptr<int>(), logprob.data_ptr<float>(), o.rec_tok, o.rec_lp, o.N, (int)s0, B, H, C, h.get_device(),
+                        stream()), "vocab_sample");
+  return logprob;
+}
+
+// The same from fp32 logits [B, C] (bias included).
+Tensor vocab_sample_logits(const Tensor& logits, double temperature, int64_t seed, Tensor step, const Tensor& row0, Tensor tokens,
+                           const std::optional<Tensor>& rec_tok, const std::optional<Tensor>& rec_lp, int64_t s0) {
+  chk_cuda(logits, "logits");
+  TORCH_CHECK(logits.dim() == 2 && logits.scalar_type() == torch::kFloat32 && logits.size(1) >= 1 &&
+              logits.numel() < (int64_t(1) << 40), "vocab sample: logits fp32 [B, C]");
+  c10::cuda::CUDAGuard g(logits.device());
+  const int B = logits.size(0), C = logits.size(1);
+  const SampleOut o = sample_check(B, logits, step, row0, tokens, rec_tok, rec_lp, temperature);
+  const int nt = ts_vocab_head_parts(C);
+  auto fo = torch::TensorOptions().device(logits.device()).dtype(torch::kFloat32);
+  auto part = torch::empty({(int64_t)B * nt * 4}, fo), logprob = torch::empty({B}, fo);
+  auto part_arg = torch::empty({(int64_t)B * nt}, fo.dtype(torch::kInt32)), ticket = torch::zeros({1}, fo.dtype(torch::kInt32));
+  check(ts_vocab_sample_logits(logits.data_ptr<float>(), (float)temperature, (unsigned int)(seed & 0xffffffff), step.data_ptr<int>(),
+                               row0.data_ptr<int>(), part.data_ptr(), part_arg.data_ptr<int>(), (unsigned int*)ticket.data_ptr<int>(), tokens.data_ptr<int>(),
+                               logprob.data_ptr<float>(), o.rec_tok, o.rec_lp, o.N, (int)s0, B, C, stream()), "vocab_sample_logits");
+  return logprob;
 }
 
 // ---- pooling over time (csrc/seq_pool.cu) ---------------------------------------------------------------------
@@ -875,6 +949,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("vocab_head_dlogits", &vocab_head_dlogits, py::arg("h"), py::arg("Wb"), py::arg("bias"), py::arg("labels"), py::arg("lengths"),
         py::arg("T"), py::arg("lse"), py::arg("count"), py::arg("dloss"), py::arg("row0"), py::arg("rows"), py::arg("dl"));
   m.def("vocab_head_colsum", &vocab_head_colsum, py::arg("dl"), py::arg("db"), py::arg("accumulate"));
+  m.def("vocab_sample", &vocab_sample, py::arg("h"), py::arg("Wb"), py::arg("bias"), py::arg("temperature"), py::arg("seed"),
+        py::arg("step"), py::arg("row0"), py::arg("tokens"), py::arg("rec_tok"), py::arg("rec_lp"), py::arg("s0"));
+  m.def("vocab_sample_logits", &vocab_sample_logits, py::arg("logits"), py::arg("temperature"), py::arg("seed"), py::arg("step"),
+        py::arg("row0"), py::arg("tokens"), py::arg("rec_tok"), py::arg("rec_lp"), py::arg("s0"));
   m.def("head_bwd", &head_bwd, py::arg("h"), py::arg("W"), py::arg("dlogits"), py::arg("dloss"), py::arg("dW"), py::arg("db"),
         py::arg("accumulate") = false);
   m.def("flat_adam", &flat_adam, py::arg("p"), py::arg("g"), py::arg("m"), py::arg("v"), py::arg("shadow"), py::arg("lr_t"),

@@ -12,6 +12,11 @@
 //     dlogits = (exp(l - lse) - onehot) · dloss / N at counted rows, 0 elsewhere, as bf16 into a scratch [chunk rows, C] that
 //     the caller feeds to the general GEMM (dh = dlogits · W^T, dW += h^T · dlogits).
 //   * vocab_head_colsum_kernel: db (+)= column sums of the bf16 dlogits chunk, summed in a fixed order.
+//   * vocab_head_gemm_kernel<kSample> (text generation, R = B rows of one step): the same main loop; the epilogue reduces each
+//     row of a tile to the max and sum exp(l - max) of the logits and the max of the perturbed score (sample_score below), its
+//     class and the logit there; vocab_sample_combine_kernel merges the tiles of a row in a fixed order into the sampled token
+//     and its log-probability.  vocab_sample_logits_kernel makes the same partials from stored fp32 logits (the inputs this
+//     GEMM does not take).
 //
 // Tiles are walked in bands of 16 cluster tiles (4096 rows): inside a band the class tile is the outer index, so the band's rows
 // of h stay in L2 and W streams from HBM once per band.  Row r = t·B + b counts iff t < lengths[b]; lengths may be 0.
@@ -23,6 +28,7 @@
 
 #include "hopper.cuh"
 #include "tmap.h"
+#include "ts_common.cuh"
 
 namespace {
 
@@ -40,7 +46,7 @@ constexpr int kStageBytes = kABytes + kBBytes;
 constexpr int kStages = 4;
 constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align*/ + 1024 /*barriers*/;
 
-enum Mode { kFwd = 0, kDlogits = 1 };
+enum Mode { kFwd = 0, kDlogits = 1, kSample = 2 };
 
 struct VocabParams {
   const float* bias;           // [C]
@@ -53,7 +59,43 @@ struct VocabParams {
   __nv_bfloat16* dl;           // kDlogits: [rows, C]
   int R, H, C, T, B;
   int row0, rows;              // this launch covers rows [row0, row0 + rows) of h
+  // kSample (T = 1): part {max, sum exp, best perturbed score, logit at it}, part_arg [R, tiles_n] the class of the best score
+  int* part_arg;
+  const int* step;             // decode step s (device-resident: a captured graph reads its current value)
+  uint32_t seed;
+  float inv_tau;               // 1 / temperature in fp32; -1 at temperature 0 (greedy: the score is the logit, no noise is drawn)
+  const int* row_base;         // row word of local row 0 in the noise counter (device-resident, as step)
 };
+
+// ---- sampling -----------------------------------------------------------------------------------------------------------------
+// The sampling definition, shared with ops/reference.py (sample_noise_words / sample_scores / sample_logits): change both or
+// neither.  For row b at decode step s, with logits l = h W + bias:
+//   temperature 0 (greedy): token = argmax_c l_c, the smallest index on a tie; no noise is drawn.
+//   temperature t > 0: Gumbel-max, token = argmax_c (l_c / t + g_c), an exact draw from softmax(l / t), with
+//     g_c = -log(-log u_c), u_c = ((word >> 8) + 0.5) * 2^-24 (strictly inside (0, 1), so no score is infinite), where word is word c & 3
+//     of Philox4x32-10 at key (seed & 0xffffffff, 0x53414D50) and counter (c >> 2, row0 + b, s, 0).  row0 places the batch in a
+//     larger set of prompts (generation in batches: the prompt's index), so no two prompts share a stream.  The second key word
+//     keeps these streams apart from the dropout masks (key (seed, partition)).
+//   The op also returns log p(token) = l_token - logsumexp(l), under the model's own softmax(l) whatever the temperature.
+// Rounding: l is fp32 (bf16 h x bf16 W accumulated in fp32, plus the fp32 bias, or the fp32 logits of the fallback); the score
+// is fmaf(l, 1/t, g) in fp32.  u has 25 significant bits at u >= 1/2, where fp32 would round 1 - 2^-25 to 1 and -log u to 0:
+// below 1/2 u is exact in fp32 and -log u = -log(u); above it 1 - u is exact and -log u = -log1p(-(1 - u)) > 0.
+constexpr uint32_t kSampleKey1 = 0x53414D50u;      // "SAMP"
+
+TC_DEVICE uint4 sample_words(uint32_t seed, uint32_t row, uint32_t s, int c) {
+  return ts::philox4x32_10(make_uint4((uint32_t)c >> 2, row, s, 0u), make_uint2(seed, kSampleKey1));
+}
+TC_DEVICE float sample_gumbel(uint32_t w) {
+  const uint32_t k = w >> 8;
+  const float u = ((float)k + 0.5f) * 0x1p-24f;
+  const float e = k < (1u << 23) ? -__logf(u) : -log1pf(-(((float)((1u << 24) - 1u - k) + 0.5f) * 0x1p-24f));
+  return -__logf(e);
+}
+TC_DEVICE float sample_score(float l, float inv_tau, uint32_t w) { return fmaf(l, inv_tau, sample_gumbel(w)); }
+// best-score merge: the larger score, the smaller class on a tie
+TC_DEVICE void sample_take(float& best, int& arg, float& lbest, float b2, int a2, float l2) {
+  if (b2 > best || (b2 == best && a2 < arg)) { best = b2; arg = a2; lbest = l2; }
+}
 
 TC_DEVICE uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
 TC_DEVICE void cluster_sync() {
@@ -191,12 +233,14 @@ vocab_head_gemm_kernel(const __grid_constant__ CUtensorMap tmap_h, const __grid_
       for (int h = 0; h < 2; ++h) {
         const int row = m0 + 64 * wg + 16 * wq + (lane >> 2) + 8 * h;
         valid[h] = row < p.row0 + p.rows;
-        const int t = row / p.B, b = row - t * p.B;
-        const bool counted = valid[h] && (p.lengths == nullptr || t < p.lengths[b]);
-        y[h] = counted ? (int)p.labels[(size_t)b * p.T + t] : -1;      // -1: an uncounted row
+        if (kMode != kSample) {
+          const int t = row / p.B, b = row - t * p.B;
+          const bool counted = valid[h] && (p.lengths == nullptr || t < p.lengths[b]);
+          y[h] = counted ? (int)p.labels[(size_t)b * p.T + t] : -1;      // -1: an uncounted row
+        }
       }
       const int row_lo = m0 + 64 * wg + 16 * wq + (lane >> 2);
-      if (kMode == kFwd) {
+      if (kMode == kFwd || kMode == kSample) {
         // l = acc + bias; classes beyond C (C % 8 == 0: whole 8-column groups) become -inf, so the passes below skip them
 #pragma unroll
         for (int j = 0; j < BN / 8; ++j) {
@@ -208,33 +252,76 @@ vocab_head_gemm_kernel(const __grid_constant__ CUtensorMap tmap_h, const __grid_
             acc[4 * j] = acc[4 * j + 1] = acc[4 * j + 2] = acc[4 * j + 3] = -INFINITY;
           }
         }
+        if (kMode == kSample) {
+          const bool greedy = p.inv_tau < 0.f;
+          const uint32_t s = greedy ? 0u : (uint32_t)*p.step;
+          const uint32_t r0 = greedy ? 0u : (uint32_t)*p.row_base;
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          float mx = -INFINITY, ly = 0.f;
-          int arg = 0x7fffffff;
+          for (int h = 0; h < 2; ++h) {
+            const int b = row_lo + 8 * h;                        // T = 1: row = batch row
+            const bool noise = !greedy && valid[h];            // rows past B draw nothing
+            float mx = -INFINITY, best = -INFINITY, lbest = 0.f;
+            int arg = 0x7fffffff;
 #pragma unroll
-          for (int j = 0; j < BN / 8; ++j)
-#pragma unroll
-            for (int e = 0; e < 2; ++e) {
-              const float l = acc[4 * j + 2 * h + e];
-              const int col = cq + 8 * j + e;
-              if (l > mx) { mx = l; arg = col; }                // ascending columns: the smallest index wins a tie
-              if (col == y[h]) ly = l;
+            for (int j = 0; j < BN / 8; ++j) {
+              const int col = cq + 8 * j;
+              const float l0 = acc[4 * j + 2 * h], l1 = acc[4 * j + 2 * h + 1];
+              float s0 = l0, s1 = l1;
+              if (noise && col < p.C) {
+                const uint4 w = sample_words(p.seed, r0 + (uint32_t)b, s, col);   // col even: words (col & 3, col & 3 + 1)
+                s0 = sample_score(l0, p.inv_tau, (col & 2) ? w.z : w.x);
+                s1 = sample_score(l1, p.inv_tau, (col & 2) ? w.w : w.y);
+              }
+              mx = fmaxf(mx, fmaxf(l0, l1));
+              if (s0 > best) { best = s0; arg = col; lbest = l0; }       // ascending columns: the smallest index wins a tie
+              if (s1 > best) { best = s1; arg = col + 1; lbest = l1; }
             }
 #pragma unroll
-          for (int o = 1; o < 4; o <<= 1) {
-            const float m2 = __shfl_xor_sync(0xffffffffu, mx, o);
-            const int a2 = __shfl_xor_sync(0xffffffffu, arg, o);
-            if (m2 > mx || (m2 == mx && a2 < arg)) { mx = m2; arg = a2; }
-            ly += __shfl_xor_sync(0xffffffffu, ly, o);
+            for (int o = 1; o < 4; o <<= 1) {
+              mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+              const float b2 = __shfl_xor_sync(0xffffffffu, best, o), l2 = __shfl_xor_sync(0xffffffffu, lbest, o);
+              const int a2 = __shfl_xor_sync(0xffffffffu, arg, o);
+              sample_take(best, arg, lbest, b2, a2, l2);
+            }
+            float se = 0.f;
+#pragma unroll
+            for (int j = 0; j < BN / 8; ++j) se += __expf(acc[4 * j + 2 * h] - mx) + __expf(acc[4 * j + 2 * h + 1] - mx);
+#pragma unroll
+            for (int o = 1; o < 4; o <<= 1) se += __shfl_xor_sync(0xffffffffu, se, o);
+            if (valid[h] && (lane & 3) == 0) {
+              p.part[(size_t)b * tiles_n + tn] = make_float4(mx, se, best, lbest);
+              p.part_arg[(size_t)b * tiles_n + tn] = arg;
+            }
           }
-          float se = 0.f;
+        } else {
 #pragma unroll
-          for (int j = 0; j < BN / 8; ++j) se += __expf(acc[4 * j + 2 * h] - mx) + __expf(acc[4 * j + 2 * h + 1] - mx);
+          for (int h = 0; h < 2; ++h) {
+            float mx = -INFINITY, ly = 0.f;
+            int arg = 0x7fffffff;
 #pragma unroll
-          for (int o = 1; o < 4; o <<= 1) se += __shfl_xor_sync(0xffffffffu, se, o);
-          if (valid[h] && (lane & 3) == 0)
-            p.part[(size_t)(row_lo + 8 * h) * tiles_n + tn] = make_float4(mx, se, __int_as_float(arg), ly);
+            for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                const float l = acc[4 * j + 2 * h + e];
+                const int col = cq + 8 * j + e;
+                if (l > mx) { mx = l; arg = col; }                // ascending columns: the smallest index wins a tie
+                if (col == y[h]) ly = l;
+              }
+#pragma unroll
+            for (int o = 1; o < 4; o <<= 1) {
+              const float m2 = __shfl_xor_sync(0xffffffffu, mx, o);
+              const int a2 = __shfl_xor_sync(0xffffffffu, arg, o);
+              if (m2 > mx || (m2 == mx && a2 < arg)) { mx = m2; arg = a2; }
+              ly += __shfl_xor_sync(0xffffffffu, ly, o);
+            }
+            float se = 0.f;
+#pragma unroll
+            for (int j = 0; j < BN / 8; ++j) se += __expf(acc[4 * j + 2 * h] - mx) + __expf(acc[4 * j + 2 * h + 1] - mx);
+#pragma unroll
+            for (int o = 1; o < 4; o <<= 1) se += __shfl_xor_sync(0xffffffffu, se, o);
+            if (valid[h] && (lane & 3) == 0)
+              p.part[(size_t)(row_lo + 8 * h) * tiles_n + tn] = make_float4(mx, se, __int_as_float(arg), ly);
+          }
         }
       } else {
         float lse[2];
@@ -389,6 +476,137 @@ __global__ void __launch_bounds__(256) vocab_head_colsum_kernel(const __nv_bfloa
   }
 }
 
+// ---- sampling: partials from stored logits, and the combine -------------------------------------------------------------
+constexpr int kSampleWarps = 8;
+
+// One warp per (row, class tile of BN): the partials of vocab_head_gemm_kernel<kSample> from fp32 logits [B, C] (bias included).
+// Lane i takes the four classes 4 i + 128 k + [0, 4) of the tile, k = 0, 1: one Philox call each.
+__global__ void __launch_bounds__(kSampleWarps * 32)
+vocab_sample_logits_kernel(const float* __restrict__ logits, VocabParams p) {
+  const int lane = threadIdx.x & 31;
+  const int tiles_n = (p.C + BN - 1) / BN;
+  const int gw = blockIdx.x * kSampleWarps + (threadIdx.x >> 5);
+  if (gw >= p.B * tiles_n) return;
+  const int b = gw / tiles_n, tn = gw - b * tiles_n;
+  const bool greedy = p.inv_tau < 0.f;
+  const uint32_t s = greedy ? 0u : (uint32_t)*p.step;
+  const uint32_t r0 = greedy ? 0u : (uint32_t)*p.row_base;
+  float l[8], sc[8];
+#pragma unroll
+  for (int k = 0; k < 2; ++k) {
+    const int c0 = tn * BN + 128 * k + 4 * lane;
+    uint4 w = make_uint4(0u, 0u, 0u, 0u);
+    if (!greedy && c0 < p.C) w = sample_words(p.seed, r0 + (uint32_t)b, s, c0);
+    const uint32_t ws[4] = {w.x, w.y, w.z, w.w};
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int c = c0 + i;
+      l[4 * k + i] = c < p.C ? logits[(size_t)b * p.C + c] : -INFINITY;
+      sc[4 * k + i] = (greedy || c >= p.C) ? l[4 * k + i] : sample_score(l[4 * k + i], p.inv_tau, ws[i]);
+    }
+  }
+  float mx = -INFINITY, best = -INFINITY, lbest = 0.f;
+  int arg = 0x7fffffff;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    mx = fmaxf(mx, l[i]);
+    if (sc[i] > best) { best = sc[i]; arg = tn * BN + 128 * (i >> 2) + 4 * lane + (i & 3); lbest = l[i]; }
+  }
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    const float b2 = __shfl_xor_sync(0xffffffffu, best, o), l2 = __shfl_xor_sync(0xffffffffu, lbest, o);
+    const int a2 = __shfl_xor_sync(0xffffffffu, arg, o);
+    sample_take(best, arg, lbest, b2, a2, l2);
+  }
+  float se = 0.f;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) se += __expf(l[i] - mx);
+  se = ts::warp_sum(se);
+  if (lane == 0) {
+    p.part[(size_t)b * tiles_n + tn] = make_float4(mx, se, best, lbest);
+    p.part_arg[(size_t)b * tiles_n + tn] = arg;
+  }
+}
+
+struct SampleCombineParams {
+  const float4* part;          // [B, nt] {max, sum exp, best score, logit at it}
+  const int* part_arg;         // [B, nt]
+  int* step;                   // [1]: read by every block, advanced by the last one
+  unsigned int* ticket;        // [1]: 0 on entry, left 0
+  int* tokens;                 // [B]
+  float* logprob;              // [B]
+  int* rec_tok;                // [B, N] or null: column step - s0 gets the token
+  float* rec_lp;               // [B, N] or null
+  int N, s0, B, nt;
+};
+
+// One warp per row: lane i merges class tiles i, i + 32, ... in ascending order, then the lanes merge in a fixed tree (the
+// smaller class wins a tie of the best score).  Two calls on the same partials give the same bits.
+__global__ void __launch_bounds__(kCombWarps * 32) vocab_sample_combine_kernel(const SampleCombineParams p) {
+  __shared__ int last_s;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int s = *(volatile const int*)p.step;
+  const int row = blockIdx.x * kCombWarps + warp;
+  if (row < p.B) {
+    float mx = -INFINITY, se = 0.f, best = -INFINITY, lbest = 0.f;
+    int arg = 0x7fffffff;
+    for (int i = lane; i < p.nt; i += 32) {
+      const float4 v = p.part[(size_t)row * p.nt + i];
+      if (v.x > mx) { se = se * __expf(mx - v.x) + v.y; mx = v.x; }
+      else se += v.y * __expf(v.x - mx);
+      if (v.z > best) { best = v.z; arg = p.part_arg[(size_t)row * p.nt + i]; lbest = v.w; }
+    }
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const float m2 = __shfl_xor_sync(0xffffffffu, mx, o), s2 = __shfl_xor_sync(0xffffffffu, se, o);
+      const float m = fmaxf(mx, m2);
+      if (m != -INFINITY) se = se * __expf(mx - m) + s2 * __expf(m2 - m);
+      mx = m;
+      const float b2 = __shfl_xor_sync(0xffffffffu, best, o), l2 = __shfl_xor_sync(0xffffffffu, lbest, o);
+      const int a2 = __shfl_xor_sync(0xffffffffu, arg, o);
+      sample_take(best, arg, lbest, b2, a2, l2);
+    }
+    if (lane == 0) {
+      const float lp = lbest - (mx + __logf(se));
+      p.tokens[row] = arg;
+      p.logprob[row] = lp;
+      const int col = s - p.s0;
+      if (p.rec_tok != nullptr && col >= 0 && col < p.N) {
+        p.rec_tok[(size_t)row * p.N + col] = arg;
+        p.rec_lp[(size_t)row * p.N + col] = lp;
+      }
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    __threadfence();
+    last_s = atomicAdd(p.ticket, 1u) == gridDim.x - 1;         // every block has read the step before the last one advances it
+  }
+  __syncthreads();
+  if (last_s && threadIdx.x == 0) {
+    *p.step = s + 1;
+    *p.ticket = 0u;
+  }
+}
+
+int launch_sample_combine(const VocabParams& v, unsigned int* ticket, int* tokens, float* logprob, int* rec_tok, float* rec_lp,
+                          int N, int s0, cudaStream_t st) {
+  SampleCombineParams c{v.part, v.part_arg, const_cast<int*>(v.step), ticket, tokens, logprob, rec_tok, rec_lp, N, s0, v.B,
+                        (v.C + BN - 1) / BN};
+  vocab_sample_combine_kernel<<<(v.B + kCombWarps - 1) / kCombWarps, kCombWarps * 32, 0, st>>>(c);
+  return (int)cudaGetLastError();
+}
+
+VocabParams sample_params(const float* bias, void* part, int* part_arg, int* step, const int* row_base, unsigned int seed,
+                          float temperature, int B, int H, int C) {
+  VocabParams p{};
+  p.bias = bias; p.part = reinterpret_cast<float4*>(part); p.part_arg = part_arg; p.step = step; p.row_base = row_base;
+  p.seed = seed; p.inv_tau = temperature > 0.f ? 1.0f / temperature : -1.f;
+  p.R = B; p.H = H; p.C = C; p.T = 1; p.B = B; p.row0 = 0; p.rows = B;
+  return p;
+}
+
 template <int kMode>
 int launch_gemm(const void* h, const void* Wb, const VocabParams& p, int dev, cudaStream_t st) {
   if (p.H % BK != 0 || p.C % 8 != 0 || p.C < 8 || p.rows < 1) { ts::set_last_error("vocab head: needs H % 64 == 0 and C % 8 == 0"); return -2; }
@@ -454,4 +672,28 @@ extern "C" int ts_vocab_head_dlogits(const void* h, const void* Wb, const float*
 extern "C" int ts_vocab_head_colsum(const void* dl, float* db, int rows, int C, int accumulate, cudaStream_t st) {
   vocab_head_colsum_kernel<<<(C + 63) / 64, dim3(32, 8), 0, st>>>(reinterpret_cast<const __nv_bfloat16*>(dl), db, rows, C, accumulate);
   return (int)cudaGetLastError();
+}
+
+// Sampling (see sample_score above): h bf16 [B, H], Wb bf16 [H, C], bias fp32 [C]; part float4 [B, ts_vocab_head_parts(C)],
+// part_arg int [B, ts_vocab_head_parts(C)], 1 zeroed ticket word (left zeroed); step int [1], advanced by one; row_base int [1],
+// the noise counter's row word of row 0.
+// -> tokens [B], logprob [B], and with rec_tok / rec_lp [B, N] column step - s0 of each.
+extern "C" int ts_vocab_sample(const void* h, const void* Wb, const float* bias, float temperature, unsigned int seed, int* step,
+                               const int* row_base, void* part, int* part_arg, unsigned int* ticket, int* tokens, float* logprob, int* rec_tok,
+                               float* rec_lp, int N, int s0, int B, int H, int C, int dev, cudaStream_t st) {
+  const VocabParams p = sample_params(bias, part, part_arg, step, row_base, seed, temperature, B, H, C);
+  if (int rc = launch_gemm<kSample>(h, Wb, p, dev, st)) return rc;
+  return launch_sample_combine(p, ticket, tokens, logprob, rec_tok, rec_lp, N, s0, st);
+}
+
+// The same from stored fp32 logits [B, C] (bias included): the inputs vocab_head_gemm_kernel does not take.
+extern "C" int ts_vocab_sample_logits(const float* logits, float temperature, unsigned int seed, int* step, const int* row_base,
+                                      void* part, int* part_arg,
+                                      unsigned int* ticket, int* tokens, float* logprob, int* rec_tok, float* rec_lp, int N, int s0,
+                                      int B, int C, cudaStream_t st) {
+  const VocabParams p = sample_params(nullptr, part, part_arg, step, row_base, seed, temperature, B, 0, C);
+  const int warps = B * ts_vocab_head_parts(C);
+  vocab_sample_logits_kernel<<<(warps + kSampleWarps - 1) / kSampleWarps, kSampleWarps * 32, 0, st>>>(logits, p);
+  if (cudaError_t e = cudaGetLastError()) return (int)e;
+  return launch_sample_combine(p, ticket, tokens, logprob, rec_tok, rec_lp, N, s0, st);
 }

@@ -442,6 +442,51 @@ def synthetic_next_token(n: int, seq_len: int, vocab_size: int, seed: int = 0, v
     return x, y, lengths
 
 
+def process_prompts(rows: Sequence[Sequence[str]], seq_len: int, vocab_size: int):
+    """Prompts of ``--mode generate``: a row is ``k`` token ids, ``1 <= k <= seq_len`` -> ``(x int32 [N, seq_len]`` right-padded
+    with id 0, ``lengths int32 [N])``.  A non-integer id, an id outside ``[0, vocab_size)`` or a row that is empty or longer than
+    ``seq_len`` is an error naming the row."""
+    xs = []
+    for n, row in enumerate(rows):
+        fields = [str(v).strip() for v in row]
+        if not any(fields):
+            raise ValueError(f"row {n}: an empty prompt (a prompt is 1..{seq_len} token ids)")
+        if len(fields) > seq_len:
+            raise ValueError(f"row {n}: a prompt of {len(fields)} token ids is longer than --seq_len {seq_len}")
+        ids = []
+        for s in fields:
+            try:
+                i = int(s)
+            except ValueError:
+                raise ValueError(f"row {n}: token id {s!r} is not an integer") from None
+            if not 0 <= i < vocab_size:
+                raise ValueError(f"row {n}: token id {i} outside [0, {vocab_size}) (--vocab_size {vocab_size})")
+            ids.append(i)
+        xs.append(ids)
+    if not xs:
+        raise ValueError("no prompts: the file has no rows")
+    x = np.zeros((len(xs), seq_len), dtype=np.int32)
+    for i, r in enumerate(xs):
+        x[i, :len(r)] = r
+    return x, np.asarray([len(r) for r in xs], dtype=np.int32)
+
+
+def synthetic_prompts(n: int, seq_len: int, vocab_size: int, seed: int = 0):
+    """``n`` prompts from the synthetic language: the first ``max(1, seq_len // 4)`` ids of the walks of
+    ``synthetic_next_token`` -> ``(x int32 [n, k], lengths int32 [n])``."""
+    k = max(1, seq_len // 4)
+    x = synthetic_next_token(n, seq_len, vocab_size, seed=seed)[0][:, :k].copy()
+    return x, np.full(n, k, dtype=np.int32)
+
+
+def legal_fraction(prompts: np.ndarray, lengths: np.ndarray, generated: np.ndarray, succ: np.ndarray) -> float:
+    """The share of the generated transitions - each prompt's last id to the first generated id, then generated id to generated
+    id - that the chain ``succ [V, 4]`` (``next_token_chain``) allows."""
+    prev = np.concatenate([prompts[np.arange(len(lengths)), lengths - 1][:, None], generated[:, :-1]], 1).astype(np.int64)
+    ok = (succ[prev] == generated.astype(np.int64)[:, :, None]).any(2)
+    return float(ok.mean())
+
+
 def synthetic_lengths(n: int, seq_len: int, seed: int = 0) -> np.ndarray:
     """Per-sample lengths, uniform in ``[max(1, seq_len // 4), seq_len]``, int32, from a generator seeded apart from the data's."""
     rng = np.random.default_rng([seed, 0x6C656E])

@@ -96,6 +96,7 @@ class SequenceClassifier(nn.Module):
             self.embedding = Embedding(self.vocab_size, cfg.in_features, init_std=cfg.init_std, device=device, generator=generator)
         self.flat: Optional[FlatParams] = None
         self._allocator = allocator
+        self._decoders: Dict[tuple, "_Decoder"] = {}       # generate(): static buffers (and CUDA graph), one per batch shape
         self.compute_dtype = torch.float32
 
     def build_flat(self, allocator: Optional[Callable] = None) -> FlatParams:
@@ -207,6 +208,58 @@ class SequenceClassifier(nn.Module):
         count = torch.full((), labels.shape[0], dtype=torch.int64, device=logits.device)
         return ref.softmax_xent(logits, labels), (logits.argmax(1) == labels).sum(), count
 
+    # ---- text generation -----------------------------------------------------------
+    @torch.no_grad()
+    def generate(self, prompt: torch.Tensor, lengths: Optional[torch.Tensor], max_new_tokens: int, temperature: float = 1.0,
+                 seed: int = 0, graph: Optional[bool] = None, row0: int = 0):
+        """Continue each prompt (``--next_token`` models): ``prompt`` int ``[B,T]`` right-padded token ids, ``lengths`` int32 ``[B]``
+        (None: every row is T long) -> (tokens int32 ``[B,N]``, log p(token) fp32 ``[B,N]`` under the model's softmax),
+        ``N = max_new_tokens``, sampled at ``temperature`` with the noise of ``seed`` (``ops.functional.vocab_sample``; step s
+        draws token s).  ``row0``: the index of row 0 among all the prompts when they run in batches; row b draws the noise of
+        prompt ``row0 + b``, so no two prompts of one generation share it.
+
+        The prompt runs through the whole-sequence path; token 0 is sampled from the top layer's state after each row's own last
+        prompt token.  Every later token embeds the previous one and takes one step of each layer from the carried state (the
+        one-step path ``RNN.fit_layers`` in eval mode), then samples.  The state lives in static buffers; on the GPU the decode
+        step is captured once per batch shape as a CUDA graph (``graph=False``: eager) and replayed; ``row0`` and the step counter
+        live on the device, so one graph serves every batch, and another temperature or seed replaces it (one graph per shape is
+        kept).  The graph runs the eager loop's kernels; with the deterministic recurrences (``--deterministic``) both give the
+        same bits.  Nothing waits for the device until the caller reads the result."""
+        if not getattr(self.cfg, "next_token", False):
+            raise ValueError("generate needs a language model trained with --next_token (this one predicts given labels)")
+        N = int(max_new_tokens)
+        if N < 1:
+            raise ValueError(f"max_new_tokens must be >= 1, got {max_new_tokens}")
+        if prompt.dim() != 2:
+            raise ValueError(f"generate needs prompts [B,T] of token ids, got {tuple(prompt.shape)}")
+        B, dev = prompt.shape[0], prompt.device
+        use_graph = dev.type == "cuda" if graph is None else bool(graph)
+        was_training = self.training
+        self.eval()
+        try:
+            self.sequence_features(prompt, lengths)
+            key = (B, N, str(dev), use_graph)
+            noise = (float(temperature), int(seed) & 0xFFFFFFFF)
+            dec = self._decoders.get(key)
+            if dec is None or (dec.temperature, dec.seed) != noise:
+                dec = self._decoders[key] = _Decoder(self, B, N, *noise, dev)
+            for layer, (h, c) in zip(self.rnn.layers, dec.state):
+                h.copy_(layer.ht)
+                c.copy_(layer.Ct)
+            dec.step.zero_()
+            dec.row0.fill_(int(row0))
+            dec.sample(self.rnn.layers[-1].ht)
+            for s in range(1, N):
+                if dec.graph is not None:
+                    dec.graph.replay()
+                    continue
+                dec.run()
+                if use_graph and s + 1 < N:
+                    dec.capture()
+        finally:
+            self.train(was_training)
+        return dec.tokens_out.clone(), dec.logprob_out.clone()
+
     # ---- reference variable naming ------------------------------------------------
     def named_reference_variables(self) -> List[Tuple[str, torch.Tensor]]:
         out = []
@@ -288,3 +341,42 @@ class SequenceClassifier(nn.Module):
                     raise KeyError(f"checkpoint is missing variable {k}")
         if self.flat is not None:
             self.flat.refresh_shadow()
+
+
+class _Decoder:
+    """The static buffers of ``SequenceClassifier.generate`` at one batch shape: the carried state of every layer, the previous
+    token, the device-resident step counter and row offset and the ``[B,N]`` results, and once captured the CUDA graph of one decode step."""
+
+    def __init__(self, model: SequenceClassifier, B: int, N: int, temperature: float, seed: int, device):
+        self.model, self.temperature, self.seed = model, temperature, seed
+        self.state = [(layer.ht.detach().clone(), layer.Ct.detach().clone()) for layer in model.rnn.layers]
+        self.tokens = torch.zeros(B, dtype=torch.int32, device=device)
+        self.step = torch.zeros(1, dtype=torch.int32, device=device)
+        self.row0 = torch.zeros(1, dtype=torch.int32, device=device)
+        self.tokens_out = torch.zeros(B, N, dtype=torch.int32, device=device)
+        self.logprob_out = torch.zeros(B, N, dtype=torch.float32, device=device)
+        self.graph = None
+
+    def sample(self, h: torch.Tensor) -> None:
+        head = self.model.head
+        F.vocab_sample(h, head.weights, head.bias, self.temperature, self.seed, self.step, tokens=self.tokens,
+                       record=(self.tokens_out, self.logprob_out, 0), row0=self.row0)
+
+    def run(self) -> None:
+        """One decode step: embed the previous token, one step of every layer from the buffers (which get the new state), sample."""
+        layers = self.model.rnn.layers
+        for layer, (h, c) in zip(layers, self.state):
+            layer._set_state(h, c)
+            layer.state = []                        # nothing to roll back to: the buffers are the state
+        top = self.model.rnn.fit_layers(self.model._input(self.tokens), train=False)
+        for layer, (h, c) in zip(layers, self.state):
+            h.copy_(layer.ht)
+            c.copy_(layer.Ct)
+        self.sample(top)
+
+    def capture(self) -> None:
+        """Capture ``run`` (after it ran eagerly once at this shape, so every kernel is loaded and every workspace exists)."""
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g):
+            self.run()
+        self.graph = g

@@ -81,3 +81,36 @@ class _VocabXentFn(torch.autograd.Function):
 def vocab_xent_per_step(h_seq, weights, bias, labels, lengths=None):
     """-> (mean loss over the counted positions, correct count, N); see ``ops.functional.vocab_xent_per_step``."""
     return _VocabXentFn.apply(h_seq, weights, bias, labels, lengths)
+
+
+def _device_int(v, device):
+    return v if isinstance(v, torch.Tensor) else torch.full((1,), int(v), dtype=torch.int32, device=device)
+
+
+def _sample_args(step, row0, tokens, record, B, device):
+    tok = torch.empty(B, dtype=torch.int32, device=device) if tokens is None else tokens
+    rec_tok, rec_lp, s0 = (None, None, 0) if record is None else record
+    return _device_int(step, device), _device_int(row0, device), tok, rec_tok, rec_lp, s0
+
+
+def vocab_sample(h, weights, bias, temperature: float, seed: int, step, tokens=None, record=None, row0=0):
+    """Sample the next token from ``h [B,H]`` bf16 through the head's tensor-core kernel (``kSample``), without storing the
+    logits; see ``ops.functional.vocab_sample``."""
+    from .cuda_lstm import STATS, _lowp
+    B = h.shape[0]
+    step_t, row_t, tok, rec_tok, rec_lp, s0 = _sample_args(step, row0, tokens, record, B, h.device)
+    wb = _lowp(weights, torch.bfloat16)
+    lp = ext().vocab_sample(h.detach().contiguous(), wb, bias.detach().float().contiguous(), float(temperature), int(seed), step_t,
+                            row_t, tok, rec_tok, rec_lp, int(s0))
+    STATS["vocab_sample"] = STATS.get("vocab_sample", 0) + 1
+    return tok, lp
+
+
+def vocab_sample_logits(logits, temperature: float, seed: int, step, tokens=None, record=None, row0=0):
+    """The same sampling from stored fp32 logits ``[B,C]`` (bias included): the inputs the tensor-core kernel does not take."""
+    from .cuda_lstm import STATS
+    step_t, row_t, tok, rec_tok, rec_lp, s0 = _sample_args(step, row0, tokens, record, logits.shape[0], logits.device)
+    lp = ext().vocab_sample_logits(logits.float().contiguous(), float(temperature), int(seed), step_t, row_t, tok, rec_tok, rec_lp,
+                                   int(s0))
+    STATS["vocab_sample"] = STATS.get("vocab_sample", 0) + 1
+    return tok, lp

@@ -6,6 +6,8 @@ mandatory: a missing/unbuilt extension raises instead of silently falling back t
 """
 from __future__ import annotations
 
+import math
+
 import torch
 
 from . import reference as ref
@@ -98,6 +100,41 @@ def vocab_xent_per_step(h_seq, weights, bias, labels, lengths=None):
     if _use_ext(h_seq):
         return head_xent_per_step(h_seq, weights, bias, labels, lengths)[1:]
     return ref.vocab_xent_per_step(h_seq, weights, bias, labels, lengths)
+
+
+def vocab_sample(h, weights, bias, temperature: float, seed: int, step, tokens=None, record=None, row0=0):
+    """Sample the next token of every row from the head's logits ``l = h W + bias`` (``h [B,H]``, ``W [H,C]``) without a host
+    round trip -> (tokens int32 ``[B]``, log p(token) under ``softmax(l)`` fp32 ``[B]``).  Temperature 0 is the arg-max; above 0
+    Gumbel-max with counter-based noise (``reference.sample_logits`` holds the definition).  ``step``: the decode step, an int
+    or an int32 ``[1]`` device tensor that this call advances by one (a captured graph then draws new noise on each replay).
+    ``tokens``: an int32 ``[B]`` buffer to write the tokens into; ``record = (tok [B,N], logprob [B,N], s0)``: column
+    ``step - s0`` of each also gets them.  ``row0`` (an int or an int32 ``[1]`` device tensor): the noise counter's row word of
+    row 0, the index of the batch's first prompt when prompts run in batches, so every prompt draws its own noise.  On the GPU bf16 ``h`` with ``H % 64 == 0``, ``C % 8 == 0`` and ``C >= 512`` runs in
+    the head's tensor-core kernel (csrc/head_vocab.cu); every other input computes the fp32 logits with the head GEMM and
+    samples them with one more kernel.  Two calls on the same inputs give the same bits."""
+    temperature = float(temperature)
+    if not (math.isfinite(temperature) and temperature >= 0):
+        raise ValueError(f"temperature must be finite and >= 0, got {temperature}")
+    if vocab_head_supported(h.unsqueeze(0), weights.shape[1]):
+        from . import cuda_vocab_head
+        return cuda_vocab_head.vocab_sample(h, weights, bias, temperature, seed, step, tokens, record, row0)
+    if _use_ext(h):
+        from . import cuda_gemm, cuda_vocab_head
+        logits = cuda_gemm.matmul(h.reshape(h.shape[0], -1), weights.detach().t(), bias=bias.detach().float(), out_dtype=torch.float32)
+        return cuda_vocab_head.vocab_sample_logits(logits, temperature, seed, step, tokens, record, row0)
+    s = int(step)
+    tok, logp = ref.vocab_sample(h, weights, bias, temperature, seed, s, int(row0))
+    logp = logp.float()
+    if isinstance(step, torch.Tensor):
+        step.add_(1)
+    if tokens is not None:
+        tok = tokens.copy_(tok)
+    if record is not None:
+        rec_tok, rec_lp, s0 = record
+        if 0 <= s - s0 < rec_tok.shape[1]:
+            rec_tok[:, s - s0] = tok
+            rec_lp[:, s - s0] = logp
+    return tok, logp
 
 
 def pool_sequence(h_seq, lengths=None, mode: str = "mean", attention=None):

@@ -12,6 +12,7 @@ contiguous slice of rows therefore owns complete (i,f,g,o) quadruples of a hidde
 from __future__ import annotations
 
 import dataclasses
+import math
 from typing import Optional, Tuple, Union
 
 import torch
@@ -246,6 +247,58 @@ def head_xent_per_step(h_seq, weights, bias, labels, lengths=None):
 def vocab_xent_per_step(h_seq, weights, bias, labels, lengths=None):
     """``head_xent_per_step`` without the logits -> (loss, correct, N): the reference of the large-vocabulary head."""
     return head_xent_per_step(h_seq, weights, bias, labels, lengths)[1:]
+
+
+# ---- sampling the next token ------------------------------------------------------------------------------------------
+# The definition is shared with the CUDA kernels (csrc/head_vocab.cu sample_score): change both or neither.
+SAMPLE_KEY1 = 0x53414D50
+
+
+def sample_noise_words(B: int, C: int, seed: int, step: int, device=None, row0: int = 0) -> torch.Tensor:
+    """``[B, C]`` int64 u32 words: class ``c`` of row ``b`` at decode step ``step`` takes word ``c & 3`` of Philox4x32-10 at key
+    ``(seed & 0xffffffff, SAMPLE_KEY1)`` and counter ``(c >> 2, row0 + b, step, 0)``.  ``row0`` places the batch in a larger set
+    of prompts (the index of its first prompt), so that no two prompts of a generation share a noise stream."""
+    G = (C + 3) // 4
+    g = torch.arange(G, dtype=torch.int64, device=device).view(1, G).expand(B, G)
+    b = ((torch.arange(B, dtype=torch.int64, device=device) + int(row0)) & _U32).view(B, 1).expand(B, G)
+    ctr = torch.stack([g, b, torch.full_like(g, int(step) & _U32), torch.zeros_like(g)], -1)
+    return philox4x32_10(ctr, int(seed) & _U32, SAMPLE_KEY1).reshape(B, 4 * G)[:, :C]
+
+
+def sample_uniform(words: torch.Tensor) -> torch.Tensor:
+    """u = ((word >> 8) + 0.5) * 2^-24, exact in fp64 and strictly inside (0, 1), so no score is infinite.  (In fp32 u is exact
+    below 1/2 and 1 - u above it: the kernels take -log u from whichever is exact.)"""
+    return ((words >> 8).double() + 0.5) * 2.0 ** -24
+
+
+def sample_scores(logits: torch.Tensor, temperature: float, seed: int, step: int, row0: int = 0) -> torch.Tensor:
+    """Perturbed scores ``[B, C]`` in fp64: the logits at temperature 0, else ``l / t + g`` with the Gumbel noise
+    ``g = -log(-log u)`` of ``sample_noise_words``."""
+    l = logits.double()
+    if temperature == 0:
+        return l
+    u = sample_uniform(sample_noise_words(l.shape[0], l.shape[1], seed, step, device=l.device, row0=row0))
+    return l / temperature - torch.log(-torch.log(u))
+
+
+def sample_logits(logits: torch.Tensor, temperature: float, seed: int, step: int, row0: int = 0):
+    """Sample one token per row of ``logits [B, C]`` -> (tokens int32 [B], log p(token) under softmax(logits), fp64 [B]).
+
+    Temperature 0: the arg-max, the smallest index on a tie, and no noise.  Temperature t > 0: Gumbel-max,
+    ``argmax_c (l_c / t + g_c)``, an exact draw from ``softmax(l / t)``; the noise is counter-based (``sample_noise_words``), so
+    row b at step s gets the draw of counter row ``row0 + b`` whatever else is in the batch.  The log-probability is under the model's own
+    ``softmax(l)`` at every temperature."""
+    if not (math.isfinite(temperature) and temperature >= 0):
+        raise ValueError(f"temperature must be finite and >= 0, got {temperature}")
+    l = logits.double()
+    tok = sample_scores(l, temperature, seed, step, row0).argmax(1)
+    logp = torch.log_softmax(l, 1).gather(1, tok.view(-1, 1)).squeeze(1)
+    return tok.to(torch.int32), logp
+
+
+def vocab_sample(h, weights, bias, temperature: float, seed: int, step, row0: int = 0):
+    """``sample_logits`` of ``l = h W + bias`` (``h [B,H]``, ``W [H,C]``) computed in fp64: the reference of the sampling op."""
+    return sample_logits(dense_head(h.double(), weights.double(), bias.double()), temperature, seed, int(step), int(row0))
 
 
 def softmax_xent_per_step(logits, labels, lengths=None):

@@ -376,26 +376,17 @@ def _find_trained_model(cfg: Config, standalone: bool):
         if last:
             variables, meta, _ = ckpt.load(last)
             return variables, last, ckpt.recorded_settings(meta)
-    raise FileNotFoundError("--mode eval: no trained model found (give --resume <averaged_model.pt | checkpoint dir>)")
+    raise FileNotFoundError(f"--mode {cfg.mode}: no trained model found (give --resume <averaged_model.pt | checkpoint dir>)")
 
 
-def evaluate_job(cfg: Config, standalone: bool = False) -> Dict:
-    """``--mode eval``: score a trained model on ``--training_path`` (or ``--synthetic``) - loss and accuracy over the whole
-    file in batches of ``--batch_size``, forward kernels only, one device.  Not in the reference (its ``--mode`` flag knows
-    only ``train`` and the averaged model is thrown away, src/rnn.py:371,407-408); it closes the train -> average -> use loop."""
+def _load_trained_model(cfg: Config, found, batch_size: int, device: torch.device, dtype: torch.dtype):
+    """A TrainEngine in eval mode holding the model ``_find_trained_model`` found (``found``), after the compatibility checks
+    (``SequenceClassifier.check_compatible``).  The reference's trainable initial state is one row PER BATCH ROW
+    ([batch_size, H], src/models/recurrent/lstm.py:24-33): at another batch size every row starts from the mean learned row."""
     from .engine import TrainEngine
-    variables, src, settings = _find_trained_model(cfg, standalone)
-    x, y, lengths = D.synthetic(cfg, cfg.synthetic, cfg.seed) if cfg.synthetic else \
-        D.parse_rows(D.read_dataset_from_path(cfg.training_path), cfg)
-    device = resolve_device(cfg, 0)
-    dtype = resolve_dtype(cfg, device)
-    F.set_backend(cfg.backend if cfg.backend != "auto" else "auto")
-    n = x.shape[0]
-    bs = D.resolve_batch_size(cfg.batch_size if cfg.batch_size and cfg.batch_size <= n else 0, n)
-    eng = TrainEngine(cfg, 0, 1, Communicator(0, 1), batch_size=bs, device=device, dtype=dtype)
-    eng.model.eval()                                    # scoring: no dropout
-    # the reference's trainable initial state is one row PER BATCH ROW ([batch_size, H], src/models/recurrent/lstm.py:24-33):
-    # scoring with another batch size uses the mean learned row for every sample
+    variables, src, settings = found
+    eng = TrainEngine(cfg, 0, 1, Communicator(0, 1), batch_size=batch_size, device=device, dtype=dtype)
+    eng.model.eval()                                    # no dropout
     shapes = {k: tuple(v.shape) for k, v in eng.model.named_reference_variables()}
     variables = dict(variables)
     eng.model.check_compatible(variables, settings, f"model {src}")   # before the row averaging below, which must never touch the table
@@ -405,6 +396,23 @@ def evaluate_job(cfg: Config, standalone: bool = False) -> Dict:
             variables[k] = v.float().mean(0, keepdim=True).expand(want).contiguous()
     eng.model.load_reference_state_dict(variables, strict=False)
     eng.flat.refresh_shadow()
+    return eng
+
+
+def evaluate_job(cfg: Config, standalone: bool = False) -> Dict:
+    """``--mode eval``: score a trained model on ``--training_path`` (or ``--synthetic``) - loss and accuracy over the whole
+    file in batches of ``--batch_size``, forward kernels only, one device.  Not in the reference (its ``--mode`` flag knows
+    only ``train`` and the averaged model is thrown away, src/rnn.py:371,407-408); it closes the train -> average -> use loop."""
+    found = _find_trained_model(cfg, standalone)
+    src = found[1]
+    x, y, lengths = D.synthetic(cfg, cfg.synthetic, cfg.seed) if cfg.synthetic else \
+        D.parse_rows(D.read_dataset_from_path(cfg.training_path), cfg)
+    device = resolve_device(cfg, 0)
+    dtype = resolve_dtype(cfg, device)
+    F.set_backend(cfg.backend if cfg.backend != "auto" else "auto")
+    n = x.shape[0]
+    bs = D.resolve_batch_size(cfg.batch_size if cfg.batch_size and cfg.batch_size <= n else 0, n)
+    eng = _load_trained_model(cfg, found, bs, device, dtype)
     xs = torch.as_tensor(x).to(device=device, dtype=D.input_dtype(cfg))
     ys = torch.as_tensor(y).to(device)
     ls = None if lengths is None else torch.as_tensor(lengths).to(device=device, dtype=torch.int32)
@@ -431,10 +439,66 @@ def evaluate_job(cfg: Config, standalone: bool = False) -> Dict:
     return out
 
 
+def generate_job(cfg: Config, standalone: bool = False) -> Dict:
+    """``--mode generate``: continue prompts with a trained ``--next_token`` model, found as ``--mode eval`` finds it, on one
+    device in batches of ``--batch_size`` (a short last batch is filled with copies of its first prompt, whose output is dropped,
+    so every batch has the shape the decode graph was captured at).  Prompts are the rows of ``--training_path`` (1..seq_len ids
+    each) or, with ``--synthetic n``, the starts of n walks of the synthetic chain; ``--max_new_tokens`` ids are drawn per prompt
+    at ``--temperature`` with noise seeded by ``--seed``; prompt i draws the noise of counter row i, so a prompt's continuation
+    does not depend on ``--batch_size`` and a prompt repeated k times gives k independent samples.  Writes ``<output_path>/generated.csv`` (one line of ids per prompt, in
+    prompt order) and reports tokens/s, the mean log-probability per token and, with ``--synthetic``, the share of generated
+    transitions the chain allows."""
+    found = _find_trained_model(cfg, standalone)
+    src = found[1]
+    if cfg.synthetic:
+        prompts, lengths = D.synthetic_prompts(cfg.synthetic, cfg.seq_len, cfg.vocab_size, cfg.seed)
+    else:
+        prompts, lengths = D.process_prompts(D.read_dataset_from_path(cfg.training_path), cfg.seq_len, cfg.vocab_size)
+    device = resolve_device(cfg, 0)
+    dtype = resolve_dtype(cfg, device)
+    F.set_backend(cfg.backend if cfg.backend != "auto" else "auto")
+    n, N = prompts.shape[0], cfg.max_new_tokens
+    bs = min(cfg.batch_size, n) if cfg.batch_size else n
+    eng = _load_trained_model(cfg, found, bs, device, dtype)
+    outs, lps = [], []
+    start = time.time()
+    for lo in range(0, n, bs):
+        rows = min(bs, n - lo)
+        idx = np.concatenate([np.arange(lo, lo + rows), np.full(bs - rows, lo)])     # the short tail: masked copies of row lo
+        width = int(lengths[idx].max())
+        x = torch.as_tensor(prompts[idx, :width]).to(device=device, dtype=torch.int32)
+        ls = torch.as_tensor(lengths[idx]).to(device=device, dtype=torch.int32)
+        tok, lp = eng.model.generate(x, ls, N, cfg.temperature, cfg.seed, row0=lo)       # prompt lo + b: its own noise
+        outs.append(tok[:rows])
+        lps.append(lp[:rows])
+    tokens = torch.cat(outs).cpu().numpy()                 # the one wait for the device
+    logprob = torch.cat(lps).double().cpu().numpy()
+    seconds = time.time() - start
+    _check_device_errors(device, None)
+    os.makedirs(cfg.output_path or ".", exist_ok=True)
+    path = os.path.join(cfg.output_path or ".", "generated.csv")
+    with open(path, "w") as f:
+        f.writelines(",".join(str(int(v)) for v in row) + "\n" for row in tokens)
+    out = {"mode": "generate", "model": src, "prompts": n, "tokens": int(tokens.size), "seconds": seconds,
+           "tokens_per_s": tokens.size / max(seconds, 1e-9), "mean_logprob": float(logprob.mean()), "temperature": cfg.temperature,
+           "output": path}
+    if cfg.synthetic:
+        out["legal_fraction"] = D.legal_fraction(prompts, lengths, tokens, D.next_token_chain(cfg.vocab_size, cfg.seed))
+    if not cfg.quiet:
+        print(("RNN-LSTM - generate: model {model}, {prompts} prompts, {tokens} tokens in {seconds:.3f}s ({tokens_per_s:.1f} "
+               "tokens/s), mean log-probability {mean_logprob:.4f} per token" +
+               (", legal_fraction {legal_fraction:.4f}" if cfg.synthetic else "") + ", wrote {output}").format(**out))
+    if cfg.json_log:
+        jl = M.JsonLog(cfg.json_log); jl.write(**out); jl.close()
+    return out
+
+
 def run_job(cfg: Config, standalone: bool = False) -> Dict:
     """``main`` of both entry points: shard -> N replicas -> average -> output."""
     if cfg.mode == "eval":
         return evaluate_job(cfg, standalone)
+    if cfg.mode == "generate":
+        return generate_job(cfg, standalone)
     from .parallel.launch import launch, in_torchrun
     world_size = resolve_workers(cfg, standalone)
     if in_torchrun():
