@@ -68,6 +68,9 @@ class Config:
                                         # followed by the label (--per_step_labels: by k labels).  0 = float features
     next_token: bool = False            # language modelling (needs --vocab_size V): the label of step t is the token of step t + 1.
                                         # Turns on --per_step_labels and sets --num_classes to V; a CSV row is seq_len + 1 ids
+    stateful: bool = False              # --next_token on one token stream cut into --batch_size parallel streams: consecutive
+                                        # batches continue each stream and start from the state the previous batch ended in,
+                                        # detached (truncated backpropagation through time); --mode eval scores the whole stream
     max_new_tokens: int = MAX_NEW_TOKENS_DEFAULT  # --mode generate: tokens sampled after each prompt
     temperature: float = TEMPERATURE_DEFAULT      # --mode generate: sample from softmax(logits / temperature); 0 = greedy
     dtype: str = "auto"                 # auto: bf16 on cuda, fp32 on cpu
@@ -158,6 +161,20 @@ class Config:
             raise ValueError("--batch_size must be >= 0 (0 = whole shard)")
         if self.seq_len < 1:
             raise ValueError("--seq_len must be >= 1")
+        if self.stateful:
+            if not self.next_token:
+                raise ValueError("--stateful needs --next_token: it carries the state along one token stream, whose labels are "
+                                 "the ids that follow")
+            if self.variable_length:
+                raise ValueError("--stateful does not combine with --variable_length: the stream is cut into segments of "
+                                 "exactly --seq_len positions and has no padding")
+            if self.learn_initial_state:
+                raise ValueError("--stateful does not combine with --learn_initial_state true: a pass starts from the zero state "
+                                 "and every later segment from the state the previous one ended in")
+            if self.pooling != "last":
+                raise ValueError(f"--stateful does not combine with --pooling {self.pooling}: every step's output is scored")
+            if self.batch_size < 1:
+                raise ValueError("--stateful needs --batch_size B >= 1: the stream is cut into B parallel streams")
         if self.next_token:
             if self.vocab_size <= 0:
                 raise ValueError("--next_token needs --vocab_size V > 0: it predicts the next token id out of the V of the vocabulary")
@@ -278,6 +295,10 @@ _HELP = {
     "next_token": "Train a next-token language model on --vocab_size V token ids: the label of step t is the id of step t + 1 "
                   "(turns on --per_step_labels, sets --num_classes to V); a CSV row is seq_len + 1 ids, or 2..seq_len + 1 with "
                   "--variable_length; evaluations also report perplexity = exp(loss)",
+    "stateful": "With --next_token: read --training_path (or --synthetic) as one token stream cut into --batch_size parallel "
+                "streams; each batch continues every stream by --seq_len positions from the state the previous batch ended in, "
+                "with gradients stopped there (truncated backpropagation through time); --mode eval reports the perplexity of the "
+                "whole stream",
     "per_step_labels": "Label every time step (sequence labelling): labels [B,T], loss and accuracy over the real positions; "
                        "a CSV row is k*in_features values followed by k labels",
 }

@@ -487,6 +487,90 @@ def legal_fraction(prompts: np.ndarray, lengths: np.ndarray, generated: np.ndarr
     return float(ok.mean())
 
 
+# ------------------------------------------------------------------------------------------------
+# one token stream (--stateful)
+# ------------------------------------------------------------------------------------------------
+def token_stream(rows: Sequence[Sequence[str]], vocab_size: int) -> np.ndarray:
+    """``--stateful``: the ids of every row concatenated in file order -> int64 ``[n]``.  A row holds any number of ids, at least
+    one.  A non-integer id or an id outside ``[0, vocab_size)`` is an error naming the row."""
+    ids = []
+    for n, row in enumerate(rows):
+        fields = [str(v).strip() for v in row]
+        if not any(fields):
+            raise ValueError(f"row {n}: no token ids (--stateful: a row is one or more ids of the stream)")
+        for s in fields:
+            try:
+                i = int(s)
+            except ValueError:
+                raise ValueError(f"row {n}: token id {s!r} is not an integer") from None
+            if not 0 <= i < vocab_size:
+                raise ValueError(f"row {n}: token id {i} outside [0, {vocab_size}) (--vocab_size {vocab_size})")
+            ids.append(i)
+    if not ids:
+        raise ValueError("empty stream: the file has no token ids")
+    return np.asarray(ids, dtype=np.int64)
+
+
+def synthetic_stream(n: int, seq_len: int, vocab_size: int, seed: int = 0) -> np.ndarray:
+    """``--stateful --synthetic n``: one walk of ``n * seq_len + 1`` ids of the chain of ``synthetic_next_token``
+    (``next_token_chain``) from a uniform start -> int64.  Drawn by a generator of its own: the other synthetic tasks are
+    untouched."""
+    succ = next_token_chain(vocab_size, seed)
+    m = n * seq_len + 1
+    rng = np.random.default_rng([seed, 0x6E7874, 2])
+    tok = np.empty(m, dtype=np.int64)
+    tok[0] = rng.integers(0, vocab_size)
+    pick = rng.choice(4, size=m - 1, p=NEXT_TOKEN_PROBS)
+    for t in range(m - 1):
+        tok[t + 1] = succ[tok[t], pick[t]]
+    return tok
+
+
+def split_stream(stream: np.ndarray, parts: int) -> List[np.ndarray]:
+    """``--partitions N`` of one stream: ``N`` contiguous pieces of ``(n - 1) // N`` transitions each; consecutive pieces share
+    one id (the last id of piece r is the first of piece r + 1), so no transition is lost.  The fewer than ``N`` transitions
+    left at the end are dropped."""
+    per = (len(stream) - 1) // parts
+    if per < 1:
+        raise ValueError(f"a stream of {len(stream)} ids cannot be split into {parts} partitions")
+    return [stream[r * per:(r + 1) * per + 1] for r in range(parts)]
+
+
+def stream_layout(stream: np.ndarray, batch_size: int, seq_len: int, tail: bool = False):
+    """One shard's stream of ``n`` ids as ``B = batch_size`` parallel streams of ``L = (n - 1) // B`` positions: stream ``b`` has
+    the inputs ``s[b L + p]`` and the labels ``s[b L + p + 1]``, ``0 <= p < L``.  Segment ``k`` is positions
+    ``k T .. k T + T - 1`` of every stream (``T = seq_len``); there are ``K = L // T`` of them.  -> ``(x int32 [K B, T],
+    y int64 [K B, T], tail_len)``, rows in (segment, stream) order, so batch ``k`` is rows ``k B .. k B + B - 1``.
+
+    Training drops the ``L - K T < T`` positions left at the end of each stream (``tail_len = 0``).  ``tail``: they become one
+    more segment, right-padded with id 0 and label 0, and ``tail_len = L - K T`` is its length in every row (0: none)."""
+    n, B, T = len(stream), int(batch_size), int(seq_len)
+    L = (n - 1) // B
+    K = L // T
+    if K == 0 and not (tail and L > 0):
+        raise ValueError(f"a shard of {n} ids holds no segment of --batch_size {B} streams x --seq_len {T} positions: it needs "
+                         f"at least {B * T + 1} ids")
+    inp = stream[:B * L].reshape(B, L)
+    lab = stream[1:B * L + 1].reshape(B, L)
+    rest = L - K * T if tail else 0
+    segs = K + (1 if rest else 0)
+    x = np.zeros((B, segs * T), dtype=np.int32)
+    y = np.zeros((B, segs * T), dtype=np.int64)
+    x[:, :K * T + rest] = inp[:, :K * T + rest]
+    y[:, :K * T + rest] = lab[:, :K * T + rest]
+    x = x.reshape(B, segs, T).transpose(1, 0, 2).reshape(segs * B, T)
+    y = y.reshape(B, segs, T).transpose(1, 0, 2).reshape(segs * B, T)
+    return np.ascontiguousarray(x), np.ascontiguousarray(y), rest
+
+
+def load_stream(cfg, n_synthetic: int = 0) -> np.ndarray:
+    """The token stream of ``--stateful``: ``--synthetic n`` walks ``synthetic_stream``, otherwise the ids of ``--training_path``
+    (``token_stream``)."""
+    if cfg.synthetic:
+        return synthetic_stream(n_synthetic or cfg.synthetic, cfg.seq_len, cfg.vocab_size, cfg.seed)
+    return token_stream(read_dataset_from_path(cfg.training_path), cfg.vocab_size)
+
+
 def synthetic_lengths(n: int, seq_len: int, seed: int = 0) -> np.ndarray:
     """Per-sample lengths, uniform in ``[max(1, seq_len // 4), seq_len]``, int32, from a generator seeded apart from the data's."""
     rng = np.random.default_rng([seed, 0x6C656E])
@@ -560,6 +644,10 @@ class DeviceShard:
         if self.lengths is None:
             return self.x.index_select(0, idx), self.y.index_select(0, idx)
         return self.x.index_select(0, idx), self.y.index_select(0, idx), self.lengths.index_select(0, idx)
+
+    def opened_pass(self) -> bool:
+        """Was the batch ``next()`` handed out last the first of a pass over the shard?"""
+        return self._i == 1
 
     def state_dict(self):
         return {"gen": self.gen.get_state(), "i": self._i,
@@ -652,6 +740,10 @@ class PinnedHostLoader:
         lo = self._i * self.batch_size
         self._i += 1
         return lo
+
+    def opened_pass(self) -> bool:
+        """Was the batch ``next()`` handed out last the first of a pass over the shard?"""
+        return self._consumed[1] == 1
 
     def state_dict(self):
         """Position of the NEXT batch to be handed out (prefetched-but-unconsumed batches are not counted), exact across a

@@ -6,6 +6,7 @@ This is what ``bench.py``, ``__graft_entry__.smoke`` and the per-replica trainer
     loss = eng.step(x, y)            # forward, backward, (fused allreduce +) optimizer update
     loss = eng.step(x, y, lengths)   # variable-length batch: int32 [B] per-sample lengths, x right-padded
     norm = eng.grad_norm()           # --clip_grad_norm: the last step's gradient norm before clipping (None without)
+    loss = eng.step(x, y, reset=k == 0)  # --stateful: batch k of a pass continues every stream from the state batch k-1 ended in
 
 One step replaces the reference's ``sess.run([train_op, loss], feed_dict=...)`` (original src/rnn.py:264-267):
 H2D feed, forward, backward, 14·L+2 ApplyAdam launches, D2H loss.  With ``cuda_graph=True`` the whole step is
@@ -87,6 +88,14 @@ class TrainEngine:
         self._dropout_on = rnn.dropout > 0 and len(rnn.layers) > 1
         rnn.dropout_key = (cfg.seed & 0xFFFFFFFF, rank if partition_key is None else int(partition_key))
         rnn.dropout_step = torch.zeros(1, dtype=torch.int32, device=device) if device.type == "cuda" else 0
+        # --stateful: static buffers per layer (h in the compute dtype, as the kernels store it; c fp32).  `state` is what the next
+        # step starts from, `state_prev` what the last step started from; a captured graph reads and writes these same buffers
+        self.stateful = bool(getattr(cfg, "stateful", False))
+        self.state = self.state_prev = None
+        if self.stateful:
+            bs = cfg.batch_size if batch_size is None else batch_size
+            self.state = rnn.zero_state(bs, dtype, device)
+            self.state_prev = rnn.zero_state(bs, dtype, device)
 
     # ---------------------------------------------------------------------------------------------------
     def _make_bucket_plan(self):
@@ -153,8 +162,13 @@ class TrainEngine:
             comm.launch_bucket(b["lo"], b["hi"])
 
     def _step_eager(self, x: torch.Tensor, y: torch.Tensor, lengths: Optional[torch.Tensor] = None) -> torch.Tensor:
+        if self.stateful:
+            with torch.no_grad():
+                for (h, c), (hp, cp) in zip(self.state, self.state_prev):
+                    hp.copy_(h)
+                    cp.copy_(c)
         self.flat.zero_grad()
-        loss, _logits, _correct = self.model(x, y, lengths)
+        loss, _logits, _correct = self.model(x, y, lengths, state=self.state_prev)
         if self._wd_autograd:
             loss = loss + torch.stack([fn(v) * wd for (v, fn, wd) in self._wd_autograd]).sum()
         l2 = None
@@ -174,6 +188,11 @@ class TrainEngine:
             loss = loss.detach() + l2
         if self._dropout_on:
             self._bump_dropout_step()
+        if self.stateful:
+            with torch.no_grad():
+                for (h, c), (hT, cT) in zip(self.state, self.model.rnn.final_state()):
+                    h.copy_(hT)
+                    c.copy_(cT)
         return loss.detach()
 
     def _bump_dropout_step(self):
@@ -192,10 +211,19 @@ class TrainEngine:
         else:
             rnn.dropout_step = int(n)
 
-    def step(self, x: torch.Tensor, y: torch.Tensor, lengths: Optional[torch.Tensor] = None) -> torch.Tensor:
+    def step(self, x: torch.Tensor, y: torch.Tensor, lengths: Optional[torch.Tensor] = None, reset: bool = False) -> torch.Tensor:
         """One full training step on this replica; returns the (detached, device) loss.  ``lengths``: optional int32 ``[B]``
-        per-sample sequence lengths of a right-padded ``x`` (a captured graph must have been captured with lengths too)."""
+        per-sample sequence lengths of a right-padded ``x`` (a captured graph must have been captured with lengths too).
+
+        ``--stateful``: the step copies ``state`` into ``state_prev``, runs forward and backward from ``state_prev`` (a constant:
+        no gradient crosses the segment boundary) and after the update writes the final states into ``state``.  ``reset``: the
+        batch opens a new pass over the streams; ``state`` is zeroed first (one ``zero_()`` outside any graph, so a captured
+        step stays valid across passes)."""
         self.steps_done += 1
+        if reset and self.stateful:
+            for h, c in self.state:
+                h.zero_()
+                c.zero_()
         if self._graph is None:
             return self._step_eager(x, y, lengths)
         if (lengths is None) != (self._static[2] is None):
@@ -222,6 +250,17 @@ class TrainEngine:
         if self.optimizer.clip_norm <= 0:
             return None
         return self.optimizer.clip_out[0].clone()
+
+    def carried_state(self):
+        """``--stateful``: ``[(h [B,H], c [B,H]) per layer]``, the buffers the next step starts from (None without the flag)."""
+        return self.state
+
+    def load_carried_state(self, state) -> None:
+        """Put a saved carried state (``carried_state()`` of an earlier run, on any device) into the buffers."""
+        with torch.no_grad():
+            for (h, c), (h1, c1) in zip(self.state, state):
+                h.copy_(h1)
+                c.copy_(c1)
 
     def graph_inputs(self):
         """(x, y, lengths) input buffers of the captured graph (lengths None when captured without), or None: a loader that
@@ -258,7 +297,8 @@ class TrainEngine:
         snap = {"data": self.flat.data.clone(), "step_count": opt.step_count,
                 "m": None if opt.m is None else opt.m.clone(), "v": None if opt.v is None else opt.v.clone(),
                 "step_dev": None if opt.step_dev is None else opt.step_dev.clone(),
-                "dropout_step": self.model.rnn.dropout_step.clone()}
+                "dropout_step": self.model.rnn.dropout_step.clone(),
+                "state": None if not self.stateful else [(h.clone(), c.clone()) for h, c in self.state + self.state_prev]}
         s = torch.cuda.Stream()
         s.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(s):
@@ -286,6 +326,10 @@ class TrainEngine:
             if snap["step_dev"] is not None:
                 opt.step_dev.copy_(snap["step_dev"])
             self.model.rnn.dropout_step.copy_(snap["dropout_step"])
+            if snap["state"] is not None:                   # capturing does not advance the carry
+                for (h, c), (h1, c1) in zip(self.state + self.state_prev, snap["state"]):
+                    h.copy_(h1)
+                    c.copy_(c1)
             opt.step_count = snap["step_count"]
         self._graph, self._static, self._bound = g, (sx, sy, sl, sloss), bound
         return g
@@ -293,11 +337,11 @@ class TrainEngine:
     @torch.no_grad()
     def evaluate(self, x: torch.Tensor, y: torch.Tensor, lengths: Optional[torch.Tensor] = None):
         """Loss and accuracy of a batch with the model in eval mode (no dropout); ``--per_step_labels``: over the counted
-        positions of ``y [B,T]``."""
+        positions of ``y [B,T]``.  ``--stateful``: from ``state_prev``, the state the last step's batch was trained from."""
         was_training = self.model.training
         self.model.eval()
         try:
-            loss, correct, count = self.model.score(x, y, lengths)
+            loss, correct, count = self.model.score(x, y, lengths, state=self.state_prev)
         finally:
             self.model.train(was_training)
         return loss, correct.float() / count.float()

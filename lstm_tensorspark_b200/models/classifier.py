@@ -132,6 +132,17 @@ class SequenceClassifier(nn.Module):
         e = self.embedding(x, lengths if x.dim() == 2 else None, self.compute_dtype)
         return e[0] if x.dim() == 1 else e.transpose(0, 1)
 
+    def _start(self, batch_size: int, state) -> None:
+        self.rnn.reset_state(batch_size)
+        if state is not None:
+            self.rnn.start_state(state)
+
+    @staticmethod
+    def _whole_sequences_only(state) -> None:
+        if state is not None:
+            raise ValueError("a carried state needs a label at every step (--next_token --stateful): a classifier of whole "
+                             "sequences starts each one from the initial state")
+
     def features(self, x: torch.Tensor, lengths: Optional[torch.Tensor] = None) -> torch.Tensor:
         """``lengths``: optional int32 ``[B]`` per-sample sequence lengths (right-padded ``x``).  The top layer's last state, or
         with ``--pooling mean | max | attention`` its outputs pooled over each sample's steps (``ops.reference.pool_sequence``),
@@ -156,39 +167,43 @@ class SequenceClassifier(nn.Module):
     def per_step(self) -> bool:
         return bool(getattr(self.cfg, "per_step_labels", False))
 
-    def sequence_features(self, x: torch.Tensor, lengths: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """The top layer's whole output ``[T,B,H_last]`` (bidirectional ``[T,B,2 H_last]``) of ``x [B,T,D]``."""
+    def sequence_features(self, x: torch.Tensor, lengths: Optional[torch.Tensor] = None, state=None) -> torch.Tensor:
+        """The top layer's whole output ``[T,B,H_last]`` (bidirectional ``[T,B,2 H_last]``) of ``x [B,T,D]``.  ``state``: optional
+        ``[(h, c) per layer]`` to start from instead of the initial state (``RNN.start_state``); the state the pass ends in is
+        ``self.rnn.final_state()``."""
         if not self._is_sequence(x):
             flag = "--per_step_labels" if self.per_step else f"--pooling {self.pooling}"
             raise ValueError(f"{flag} needs sequences [B,T,D] (token ids: [B,T]), got {tuple(x.shape)}")
-        self.rnn.reset_state(x.shape[0])
+        self._start(x.shape[0], state)
         return self.rnn.fit_sequence_all(self._input(x, lengths), lengths=lengths)
 
-    def forward(self, x: torch.Tensor, labels: torch.Tensor, lengths: Optional[torch.Tensor] = None):
-        """-> (loss, logits, correct_count); with ``--per_step_labels`` logits are ``[B,T,C]`` and the loss and the count run over
+    def forward(self, x: torch.Tensor, labels: torch.Tensor, lengths: Optional[torch.Tensor] = None, state=None):
+        """``state``: optional ``[(h, c) per layer]`` to start from (``sequence_features``), a constant to autograd.
+        -> (loss, logits, correct_count); with ``--per_step_labels`` logits are ``[B,T,C]`` and the loss and the count run over
         the counted positions (``ops.reference.head_xent_per_step``).  Where the large-vocabulary head runs
         (``ops.functional.vocab_head_supported``: bf16 on the GPU, 512 classes or more) no logits exist and the slot holds None."""
         self.check_labels(labels)
         if self.per_step:
-            h_seq = self.sequence_features(x, lengths)
+            h_seq = self.sequence_features(x, lengths, state)
             if F.vocab_head_supported(h_seq, self.cfg.num_classes):
                 loss, correct, _n = F.vocab_xent_per_step(h_seq, self.head.weights, self.head.bias, labels, lengths)
                 return loss, None, correct
             logits, loss, correct, _n = F.head_xent_per_step(h_seq, self.head.weights, self.head.bias, labels, lengths)
             return loss, logits, correct
+        self._whole_sequences_only(state)
         h = self.features(x, lengths)
         logits, loss, correct = F.head_xent(h, self.head.weights, self.head.bias, labels)
         return loss, logits, correct
 
     @torch.no_grad()
-    def score(self, x: torch.Tensor, labels: torch.Tensor, lengths: Optional[torch.Tensor] = None, first: int = 0):
+    def score(self, x: torch.Tensor, labels: torch.Tensor, lengths: Optional[torch.Tensor] = None, first: int = 0, state=None):
         """Evaluation without gradients (call in eval mode): -> (mean loss, correct count, count) over rows ``first:`` of the
-        batch, device tensors (no host sync).  The count is of the counted positions with ``--per_step_labels``, of the rows
+        batch, device tensors (no host sync); ``state`` as in ``forward``.  The count is of the counted positions with ``--per_step_labels``, of the rows
         otherwise.  The whole batch runs through the stack, so a tail can be scored in a batch of the usual static shape."""
         from ..ops import reference as ref
         self.check_labels(labels)
         if self.per_step:
-            h_seq = self.sequence_features(x, lengths)
+            h_seq = self.sequence_features(x, lengths, state)
             if F.vocab_head_supported(h_seq, self.cfg.num_classes):
                 # the tail is a mask, not a slice: rows before `first` get length 0, and no [rows, C] array is ever built
                 if first > 0:
@@ -204,6 +219,7 @@ class SequenceClassifier(nn.Module):
             logits = self.head(h_seq.reshape(-1, h_seq.shape[2])).float().view(h_seq.shape[0], h_seq.shape[1], -1)
             return ref.softmax_xent_per_step(logits.transpose(0, 1), labels, None if lengths is None else lengths[first:])
         labels = labels[first:]
+        self._whole_sequences_only(state)
         logits = self.head(self.features(x, lengths))[first:].float()
         count = torch.full((), labels.shape[0], dtype=torch.int64, device=logits.device)
         return ref.softmax_xent(logits, labels), (logits.argmax(1) == labels).sum(), count

@@ -84,6 +84,28 @@ class RNN(nn.Module):
         for layer in self.directions():
             layer.reset_state(batch_size)
 
+    def start_state(self, state: List[tuple]):
+        """Start the next pass from ``state = [(h [B,H], c [B,H]) per layer]`` instead of the initial state variables (a carried
+        stream state, ``--stateful``).  It is a constant to autograd: no gradient flows into it."""
+        if self.bidirectional:
+            raise ValueError("a carried state needs a unidirectional stack: the reverse direction has no state to carry forward")
+        if len(state) != len(self.layers):
+            raise ValueError(f"a carried state needs one (h, c) per layer: {len(self.layers)} layers, got {len(state)}")
+        for layer, (h, c) in zip(self.layers, state):
+            layer._set_state(h.detach(), c.detach())
+            layer.state = []
+
+    def final_state(self) -> List[tuple]:
+        """``[(h_T, c_T) per layer]``: the state the last pass ended in (with ``lengths``: each row's state after its own last
+        step).  ``h_T`` is in the compute dtype, as the kernels store it."""
+        return [(layer.ht, layer.Ct) for layer in self.layers]
+
+    def zero_state(self, batch_size: int, dtype: torch.dtype, device) -> List[tuple]:
+        """The state a stream starts from: ``[(h [B,H] zeros in dtype, c [B,H] zeros in fp32 (fp64 for an fp64 model))]``."""
+        c_dtype = torch.promote_types(dtype, torch.float32)
+        return [(torch.zeros(batch_size, l.num_hidden, dtype=dtype, device=device),
+                 torch.zeros(batch_size, l.num_hidden, dtype=c_dtype, device=device)) for l in self.layers]
+
     def fit_layers(self, input_data: torch.Tensor, train: bool = True, lengths: Optional[torch.Tensor] = None) -> torch.Tensor:
         """``[B,D]``: one step per layer (reference semantics, rnn.py:38-42; ``lengths`` is ignored; not bidirectional).
         ``[B,T,D]``: full unroll; returns the last layer's h at the last step, ``[B,H_last]`` - with ``lengths`` (int32 ``[B]``,

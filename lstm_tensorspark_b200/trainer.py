@@ -105,7 +105,12 @@ def train_rnn(partition, cfg: Config, rank: int = 0, world_size: int = 1, comm: 
     dtype = resolve_dtype(cfg, device)
     F.set_backend(cfg.backend if cfg.backend != "auto" else "auto")
 
-    if isinstance(rows, tuple):
+    if cfg.stateful:
+        # one token stream (a piece of it with --partitions) as --batch_size parallel streams, in (segment, stream) order
+        stream = rows if isinstance(rows, np.ndarray) else D.token_stream(rows, cfg.vocab_size)
+        train_x, train_y, _ = D.stream_layout(stream, cfg.batch_size, cfg.seq_len)
+        train_lengths = None
+    elif isinstance(rows, tuple):
         train_x, train_y = rows[0], rows[1]
         train_lengths = rows[2] if len(rows) > 2 else None
     else:
@@ -128,12 +133,13 @@ def train_rnn(partition, cfg: Config, rank: int = 0, world_size: int = 1, comm: 
     jlog = M.JsonLog(cfg.json_log)
 
     x_dtype = D.input_dtype(cfg)
+    shuffle = not cfg.stateful                 # the stream layout is served in order: batch k continues the streams of batch k-1
     if cfg.data_residency == "host":
         # the reference's feed (src/rnn.py:264-267: every batch travels host -> device), as an asynchronous DMA pipeline
-        loader = D.PinnedHostLoader(train_x, train_y, batch_size, device, dtype=x_dtype, shuffle=True,
+        loader = D.PinnedHostLoader(train_x, train_y, batch_size, device, dtype=x_dtype, shuffle=shuffle,
                                     seed=cfg.seed + 17 * (rank + 1), depth=3, lengths=train_lengths)
     else:
-        loader = D.DeviceShard(train_x, train_y, batch_size, device, dtype=x_dtype, shuffle=True,
+        loader = D.DeviceShard(train_x, train_y, batch_size, device, dtype=x_dtype, shuffle=shuffle,
                                seed=cfg.seed + 17 * (rank + 1), lengths=train_lengths)
     start_step = 0
     if cfg.resume or cfg.use_pretrained_model:
@@ -145,6 +151,7 @@ def train_rnn(partition, cfg: Config, rank: int = 0, world_size: int = 1, comm: 
         if src:
             variables, meta, opt_state = ckpt.load(src)
             model.check_compatible(variables, ckpt.recorded_settings(meta), f"checkpoint {src}")
+            check_stateful(opt_state, meta, cfg, f"checkpoint {src}")
             model.load_reference_state_dict(variables, strict=False)
             eng.flat.refresh_shadow()
             if opt_state is not None:
@@ -154,6 +161,8 @@ def train_rnn(partition, cfg: Config, rank: int = 0, world_size: int = 1, comm: 
                     st = opt_state["loader"]
                     if bool(st.get("pinned")) == isinstance(loader, D.PinnedHostLoader):
                         loader.load_state_dict(st)                   # continue the data order, do not replay it
+                        if cfg.stateful and opt_state.get("state") is not None:
+                            eng.load_carried_state(opt_state["state"])   # ... and every stream from where it stopped
                     else:
                         sys.stderr.write(f"{tag} - checkpoint was written with another --data_residency: data order starts over\n")
             start_step = int(meta.get("global_step", -1)) + 1
@@ -206,7 +215,7 @@ def train_rnn(partition, cfg: Config, rank: int = 0, world_size: int = 1, comm: 
                 # static shapes: replay the captured step from here on (host feed: one graph per staging slot, no extra copy)
                 eng.capture(train_input, train_labels, bind=list(loader.dev) if isinstance(loader, D.PinnedHostLoader) else (),
                             lengths=batch_lengths)
-            loss = eng.step(train_input, train_labels, batch_lengths)
+            loss = eng.step(train_input, train_labels, batch_lengths, reset=cfg.stateful and loader.opened_pass())
         samples += batch_size
 
         with M.nvtx_range("param_avg", cfg.nvtx):
@@ -227,11 +236,14 @@ def train_rnn(partition, cfg: Config, rank: int = 0, world_size: int = 1, comm: 
                 saver.save(model.reference_state_dict(), global_step=step,
                            extra={"rank": rank, "world_size": world_size, "partition_key": partition_key,
                                   "loss": t_loss, "config": cfg.__dict__},
-                           opt_state={"optimizer": comm.optimizer_state(optimizer), "loader": loader.state_dict()})
+                           opt_state={"optimizer": comm.optimizer_state(optimizer), "loader": loader.state_dict(),
+                                      "stateful": cfg.stateful,
+                                      "state": None if not cfg.stateful else
+                                      [(h.detach().cpu().clone(), c.detach().cpu().clone()) for h, c in eng.carried_state()]})
                 model.eval()                                         # no dropout while scoring
                 with torch.no_grad(), M.capture(sink):
-                    # same batch, from the initial state (src/rnn.py:276-279)
-                    xent, ok, n = model.score(train_input, train_labels, batch_lengths)
+                    # same batch, from the initial state (src/rnn.py:276-279); --stateful: from the state it was trained from
+                    xent, ok, n = model.score(train_input, train_labels, batch_lengths, state=eng.state_prev)
                     e_loss = report_loss(xent)
                     e_acc = report_accuracy(ok.float() / n.float())
                 model.train()
@@ -347,7 +359,23 @@ def resolve_workers(cfg: Config, standalone: bool) -> int:
     return max(1, min(cfg.partitions, cap))
 
 
+def check_stateful(opt_state: Optional[dict], meta: dict, cfg: Config, what: str) -> None:
+    """Resuming training: raise unless the checkpoint was written with this run's ``--stateful`` (recorded in its optimizer-state
+    file, else in its flags; nothing recorded counts as off).  The variables are the same either way, but the data order and
+    the carried state are not."""
+    saved = bool(opt_state.get("stateful")) if opt_state is not None and "stateful" in opt_state else \
+        bool(ckpt.recorded_settings(meta).get("stateful"))
+    if saved != bool(cfg.stateful):
+        raise ValueError(f"{what} was written {'with' if saved else 'without'} --stateful, this run is "
+                         f"{'with' if cfg.stateful else 'without'} it: {'add' if saved else 'drop'} --stateful to resume it "
+                         "(--mode eval scores it either way)")
+
+
 def load_shards(cfg: Config, world_size: int, standalone: bool):
+    if cfg.stateful:
+        # one stream; --partitions: contiguous pieces of it, consecutive pieces sharing one id
+        stream = D.load_stream(cfg)
+        return [(0, stream)] if standalone else list(enumerate(D.split_stream(stream, world_size)))
     if cfg.synthetic:
         return [(r, D.synthetic(cfg, cfg.synthetic // world_size, cfg.seed + r)) for r in range(world_size)]
     if standalone:
@@ -405,6 +433,8 @@ def evaluate_job(cfg: Config, standalone: bool = False) -> Dict:
     only ``train`` and the averaged model is thrown away, src/rnn.py:371,407-408); it closes the train -> average -> use loop."""
     found = _find_trained_model(cfg, standalone)
     src = found[1]
+    if cfg.stateful:
+        return _evaluate_stream(cfg, found)
     x, y, lengths = D.synthetic(cfg, cfg.synthetic, cfg.seed) if cfg.synthetic else \
         D.parse_rows(D.read_dataset_from_path(cfg.training_path), cfg)
     device = resolve_device(cfg, 0)
@@ -434,6 +464,42 @@ def evaluate_job(cfg: Config, standalone: bool = False) -> Dict:
         positions = "{positions} positions, " if eng.model.per_step else ""
         print(("RNN-LSTM - eval: model {model}, {samples} samples, " + positions +
                "loss {loss:.6f}, accuracy {accuracy:.4f}" + (", perplexity {perplexity:.4f}" if cfg.next_token else "")).format(**out))
+    if cfg.json_log:
+        jl = M.JsonLog(cfg.json_log); jl.write(**out); jl.close()
+    return out
+
+
+def _evaluate_stream(cfg: Config, found) -> Dict:
+    """``--mode eval --stateful``: the perplexity of the whole stream (``--training_path`` or ``--synthetic``) cut into
+    ``--batch_size`` streams (``data.stream_layout``), the state carried from segment to segment from zero.  The positions left
+    after the last full segment run as one more segment with that length in every row, so every position is scored."""
+    src = found[1]
+    stream = D.load_stream(cfg)
+    B, T = cfg.batch_size, cfg.seq_len
+    x, y, tail = D.stream_layout(stream, B, T, tail=True)
+    device = resolve_device(cfg, 0)
+    dtype = resolve_dtype(cfg, device)
+    F.set_backend(cfg.backend if cfg.backend != "auto" else "auto")
+    eng = _load_trained_model(cfg, found, B, device, dtype)
+    model = eng.model
+    xs = torch.as_tensor(x).to(device=device, dtype=D.input_dtype(cfg))
+    ys = torch.as_tensor(y).to(device)
+    segs = x.shape[0] // B
+    tail_lengths = torch.full((B,), tail, dtype=torch.int32, device=device) if tail else None
+    state = model.rnn.zero_state(B, eng.dtype, device)
+    loss_sum, correct, count = 0.0, 0, 0
+    start = time.time()
+    for k in range(segs):
+        lengths = tail_lengths if (tail and k == segs - 1) else None
+        loss, ok, cnt = model.score(xs[k * B:(k + 1) * B], ys[k * B:(k + 1) * B], lengths, state=state)
+        state = model.rnn.final_state()
+        loss_sum += float(loss) * int(cnt); correct += int(ok); count += int(cnt)
+    out = {"mode": "eval", "model": src, "stream": int(len(stream)), "streams": B, "positions": count,
+           "loss": loss_sum / count, "accuracy": correct / count, "seconds": time.time() - start}
+    out["perplexity"] = math.exp(out["loss"])
+    if not cfg.quiet:
+        print(("RNN-LSTM - eval: model {model}, a stream of {stream} ids in {streams} streams, {positions} positions, "
+               "loss {loss:.6f}, accuracy {accuracy:.4f}, perplexity {perplexity:.4f}").format(**out))
     if cfg.json_log:
         jl = M.JsonLog(cfg.json_log); jl.write(**out); jl.close()
     return out
@@ -522,7 +588,7 @@ def run_job(cfg: Config, standalone: bool = False) -> Dict:
                                  {"world_size": world_size, "sync_mode": cfg.sync_mode, "average_scope": cfg.average_scope,
                                   "hidden_units": cfg.hidden_units, "pooling": cfg.pooling,
                                   "attention_units": cfg.attention_units, "vocab_size": cfg.vocab_size,
-                                  "next_token": cfg.next_token, "seconds": total})
+                                  "next_token": cfg.next_token, "stateful": cfg.stateful, "seconds": total})
     if not cfg.quiet:
         print("RNN-LSTM - Total Processing Time {}s".format(total))
     return {"results": results, "seconds": total, "world_size": world_size, "partitions": n_shards}
