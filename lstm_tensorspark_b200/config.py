@@ -71,6 +71,8 @@ class Config:
     stateful: bool = False              # --next_token on one token stream cut into --batch_size parallel streams: consecutive
                                         # batches continue each stream and start from the state the previous batch ended in,
                                         # detached (truncated backpropagation through time); --mode eval scores the whole stream
+    tie_embeddings: bool = False        # --next_token with --in_features == the last --hidden_units: the softmax reads the embedding
+                                        # table as its weights, logits = h Embedding^T + bias (Press & Wolf 2017), no Dense1/weights
     max_new_tokens: int = MAX_NEW_TOKENS_DEFAULT  # --mode generate: tokens sampled after each prompt
     temperature: float = TEMPERATURE_DEFAULT      # --mode generate: sample from softmax(logits / temperature); 0 = greedy
     dtype: str = "auto"                 # auto: bf16 on cuda, fp32 on cpu
@@ -175,6 +177,13 @@ class Config:
                 raise ValueError(f"--stateful does not combine with --pooling {self.pooling}: every step's output is scored")
             if self.batch_size < 1:
                 raise ValueError("--stateful needs --batch_size B >= 1: the stream is cut into B parallel streams")
+        if self.tie_embeddings:
+            if not self.next_token:
+                raise ValueError("--tie_embeddings needs --next_token: the softmax can share the embedding table only when its "
+                                 "classes are the vocabulary")
+            if self.in_features != self.hidden_list()[-1]:
+                raise ValueError(f"--tie_embeddings needs --in_features (the embedding width, {self.in_features}) equal to the last "
+                                 f"--hidden_units ({self.hidden_list()[-1]}): the softmax reads the table's rows as its weights")
         if self.next_token:
             if self.vocab_size <= 0:
                 raise ValueError("--next_token needs --vocab_size V > 0: it predicts the next token id out of the V of the vocabulary")
@@ -299,6 +308,9 @@ _HELP = {
                 "streams; each batch continues every stream by --seq_len positions from the state the previous batch ended in, "
                 "with gradients stopped there (truncated backpropagation through time); --mode eval reports the perplexity of the "
                 "whole stream",
+    "tie_embeddings": "With --next_token and --in_features equal to the last --hidden_units: the softmax reuses the embedding "
+                      "table as its weights (logits = h Embedding^T + Dense1/bias; weight tying, Press & Wolf 2017), so the model "
+                      "has no Dense1/weights and the table's gradient is the sum of both uses",
     "per_step_labels": "Label every time step (sequence labelling): labels [B,T], loss and accuracy over the real positions; "
                        "a CSV row is k*in_features values followed by k labels",
 }

@@ -52,12 +52,12 @@ int ts_head_step_bwd(const void*, const float*, const float*, const float*, void
                      int, int, cudaStream_t);
 int ts_vocab_head_parts(int);
 int ts_vocab_head_blocks(int);
-int ts_vocab_head_fwd(const void*, const void*, const float*, const long long*, const int*, void*, float*, float*, int*, unsigned int*,
+int ts_vocab_head_fwd(const void*, const void*, int, const float*, const long long*, const int*, void*, float*, float*, int*, unsigned int*,
                       float*, int*, int*, int, int, int, int, int, cudaStream_t);
-int ts_vocab_head_dlogits(const void*, const void*, const float*, const long long*, const int*, const float*, const float*, const int*,
+int ts_vocab_head_dlogits(const void*, const void*, int, const float*, const long long*, const int*, const float*, const float*, const int*,
                           void*, int, int, int, int, int, int, int, cudaStream_t);
 int ts_vocab_head_colsum(const void*, float*, int, int, int, cudaStream_t);
-int ts_vocab_sample(const void*, const void*, const float*, float, unsigned int, int*, const int*, void*, int*, unsigned int*, int*,
+int ts_vocab_sample(const void*, const void*, int, const float*, float, unsigned int, int*, const int*, void*, int*, unsigned int*, int*,
                     float*, int*, float*, int, int, int, int, int, int, cudaStream_t);
 int ts_vocab_sample_logits(const float*, float, unsigned int, int*, const int*, void*, int*, unsigned int*, int*, float*, int*, float*,
                            int, int, int, int, cudaStream_t);
@@ -376,25 +376,32 @@ Tensor head_step_bwd(const Tensor& h, const Tensor& W, const Tensor& dlogits, co
 }
 
 // ---- large-vocabulary per-step head (csrc/head_vocab.cu) ------------------------------------------------------------
-// h bf16 [T·B, H] packed time-major rows, Wb bf16 [H, C], bias fp32 [C], labels int64 [B,T], optional lengths int32 [B] (0 allowed),
-// part: fp32 scratch of at least T·B * vocab_head_parts(C) * 4 elements -> lse [T·B], loss, correct, N.  No logits are stored and
-// nothing is read back to the host.
-void vocab_head_check(const Tensor& h, const Tensor& Wb, const Tensor& bias, const Tensor& labels, int64_t T) {
-  chk_cuda(h, "h"); chk_cuda(Wb, "Wb"); chk_cuda(bias, "bias"); chk_cuda(labels, "labels");
+// h bf16 [T·B, H] packed time-major rows, Wb bf16 [H, C] (w_kmajor: the tied embedding table [C, H], read in place as a K-major
+// operand; the flag is explicit because H == C would make the shapes ambiguous), bias fp32 [C], labels int64 [B,T], optional
+// lengths int32 [B] (0 allowed), part: fp32 scratch of at least T·B * vocab_head_parts(C) * 4 elements -> lse [T·B], loss,
+// correct, N.  No logits are stored and nothing is read back to the host.
+int64_t vocab_classes(const Tensor& h, const Tensor& Wb, bool w_kmajor, const char* what) {
   TORCH_CHECK(h.dim() == 2 && Wb.dim() == 2 && h.scalar_type() == torch::kBFloat16 && Wb.scalar_type() == torch::kBFloat16 &&
-              Wb.size(0) == h.size(1), "vocab head: h bf16 [T*B,H], Wb bf16 [H,C]");
-  const int64_t R = h.size(0), H = h.size(1), C = Wb.size(1);
+              Wb.size(w_kmajor ? 1 : 0) == h.size(1), what, ": h bf16 [rows,H], Wb bf16 ", w_kmajor ? "[C,H]" : "[H,C]");
+  TORCH_CHECK(!w_kmajor || (Wb.is_contiguous() && (uintptr_t)Wb.data_ptr() % 16 == 0), what, ": the table [C,H] must be packed and "
+              "16-byte aligned (TMA)");
+  return Wb.size(w_kmajor ? 0 : 1);
+}
+
+void vocab_head_check(const Tensor& h, const Tensor& Wb, bool w_kmajor, const Tensor& bias, const Tensor& labels, int64_t T) {
+  chk_cuda(h, "h"); chk_cuda(Wb, "Wb"); chk_cuda(bias, "bias"); chk_cuda(labels, "labels");
+  const int64_t R = h.size(0), H = h.size(1), C = vocab_classes(h, Wb, w_kmajor, "vocab head");
   TORCH_CHECK(H % 64 == 0 && C % 8 == 0 && C >= 8, "vocab head: H % 64 == 0 and C % 8 == 0");
   TORCH_CHECK(T >= 1 && R % T == 0 && R * std::max(C, H) < (int64_t(1) << 40) && R < (int64_t(1) << 31), "vocab head: rows must be T*B");
   TORCH_CHECK(bias.scalar_type() == torch::kFloat32 && bias.numel() == C && ((uintptr_t)bias.data_ptr() % 8) == 0, "vocab head: bias fp32 [C]");
   TORCH_CHECK(labels.scalar_type() == torch::kInt64 && labels.dim() == 2 && labels.size(0) == R / T && labels.size(1) == T, "labels int64 [B,T]");
 }
 
-std::vector<Tensor> vocab_head_fwd(const Tensor& h, const Tensor& Wb, const Tensor& bias, const Tensor& labels,
+std::vector<Tensor> vocab_head_fwd(const Tensor& h, const Tensor& Wb, bool w_kmajor, const Tensor& bias, const Tensor& labels,
                                    const std::optional<Tensor>& lengths, int64_t T, Tensor part) {
-  vocab_head_check(h, Wb, bias, labels, T);
+  vocab_head_check(h, Wb, w_kmajor, bias, labels, T);
   c10::cuda::CUDAGuard g(h.device());
-  const int R = h.size(0), H = h.size(1), C = Wb.size(1), B = R / (int)T;
+  const int R = h.size(0), H = h.size(1), C = Wb.size(w_kmajor ? 0 : 1), B = R / (int)T;
   chk_cuda(part, "part");
   TORCH_CHECK(part.scalar_type() == torch::kFloat32 && part.numel() >= (int64_t)R * ts_vocab_head_parts(C) * 4 &&
               ((uintptr_t)part.data_ptr() % 16) == 0, "vocab head: part scratch");
@@ -403,7 +410,7 @@ std::vector<Tensor> vocab_head_fwd(const Tensor& h, const Tensor& Wb, const Tens
   auto lse = torch::empty({R}, fo), part_loss = torch::empty({blocks}, fo), loss = torch::empty({1}, fo);
   auto ints = torch::zeros({blocks + 4}, fo.dtype(torch::kInt32));          // [blocks] per-block counts, ticket, correct, N
   int* ip = ints.data_ptr<int>();
-  check(ts_vocab_head_fwd(h.data_ptr(), Wb.data_ptr(), bias.data_ptr<float>(), (const long long*)labels.data_ptr<int64_t>(),
+  check(ts_vocab_head_fwd(h.data_ptr(), Wb.data_ptr(), w_kmajor ? 1 : 0, bias.data_ptr<float>(), (const long long*)labels.data_ptr<int64_t>(),
                           lengths_ptr(lengths, B, h), part.data_ptr(), lse.data_ptr<float>(), part_loss.data_ptr<float>(), ip,
                           (unsigned int*)(ip + blocks), loss.data_ptr<float>(), ip + blocks + 1, ip + blocks + 2, (int)T, B, H, C,
                           h.get_device(), stream()), "vocab_head_fwd");
@@ -411,17 +418,18 @@ std::vector<Tensor> vocab_head_fwd(const Tensor& h, const Tensor& Wb, const Tens
 }
 
 // dl [rows, C] bf16 <- (softmax - onehot) * dloss / N of rows [row0, row0 + rows) of h (0 at uncounted rows); lse, count: the forward's.
-void vocab_head_dlogits(const Tensor& h, const Tensor& Wb, const Tensor& bias, const Tensor& labels, const std::optional<Tensor>& lengths,
-                        int64_t T, const Tensor& lse, const Tensor& count, const Tensor& dloss, int64_t row0, int64_t rows, Tensor dl) {
-  vocab_head_check(h, Wb, bias, labels, T);
+void vocab_head_dlogits(const Tensor& h, const Tensor& Wb, bool w_kmajor, const Tensor& bias, const Tensor& labels,
+                        const std::optional<Tensor>& lengths, int64_t T, const Tensor& lse, const Tensor& count, const Tensor& dloss,
+                        int64_t row0, int64_t rows, Tensor dl) {
+  vocab_head_check(h, Wb, w_kmajor, bias, labels, T);
   c10::cuda::CUDAGuard g(h.device());
-  const int R = h.size(0), H = h.size(1), C = Wb.size(1), B = R / (int)T;
+  const int R = h.size(0), H = h.size(1), C = Wb.size(w_kmajor ? 0 : 1), B = R / (int)T;
   chk_cuda(lse, "lse"); chk_cuda(count, "count"); chk_cuda(dloss, "dloss"); chk_cuda(dl, "dl");
   TORCH_CHECK(lse.scalar_type() == torch::kFloat32 && lse.numel() == R && count.scalar_type() == torch::kInt32 && count.numel() == 1 &&
               dloss.scalar_type() == torch::kFloat32 && dloss.numel() == 1, "vocab head: lse fp32 [R], count int32 [1], dloss fp32 [1]");
   TORCH_CHECK(rows >= 1 && row0 >= 0 && row0 + rows <= R && dl.scalar_type() == torch::kBFloat16 && dl.numel() >= rows * C,
               "vocab head: dl bf16 [rows, C]");
-  check(ts_vocab_head_dlogits(h.data_ptr(), Wb.data_ptr(), bias.data_ptr<float>(), (const long long*)labels.data_ptr<int64_t>(),
+  check(ts_vocab_head_dlogits(h.data_ptr(), Wb.data_ptr(), w_kmajor ? 1 : 0, bias.data_ptr<float>(), (const long long*)labels.data_ptr<int64_t>(),
                               lengths_ptr(lengths, B, h), lse.data_ptr<float>(), dloss.data_ptr<float>(), count.data_ptr<int>(),
                               dl.data_ptr(), (int)T, B, H, C, (int)row0, (int)rows, h.get_device(), stream()), "vocab_head_dlogits");
 }
@@ -464,22 +472,23 @@ SampleOut sample_check(int64_t B, const Tensor& like, const Tensor& step, const 
   return o;
 }
 
-Tensor vocab_sample(const Tensor& h, const Tensor& Wb, const Tensor& bias, double temperature, int64_t seed, Tensor step, const Tensor& row0,
-                    Tensor tokens, const std::optional<Tensor>& rec_tok, const std::optional<Tensor>& rec_lp, int64_t s0) {
+Tensor vocab_sample(const Tensor& h, const Tensor& Wb, bool w_kmajor, const Tensor& bias, double temperature, int64_t seed, Tensor step,
+                    const Tensor& row0, Tensor tokens, const std::optional<Tensor>& rec_tok, const std::optional<Tensor>& rec_lp,
+                    int64_t s0) {
   chk_cuda(h, "h"); chk_cuda(Wb, "Wb"); chk_cuda(bias, "bias");
-  TORCH_CHECK(h.dim() == 2 && Wb.dim() == 2 && h.scalar_type() == torch::kBFloat16 && Wb.scalar_type() == torch::kBFloat16 &&
-              Wb.size(0) == h.size(1) && h.size(0) >= 1 && h.size(0) < (int64_t(1) << 24), "vocab sample: h bf16 [B,H], Wb bf16 [H,C]");
-  TORCH_CHECK(h.size(1) % 64 == 0 && Wb.size(1) % 8 == 0 && Wb.size(1) >= 8, "vocab sample: H % 64 == 0 and C % 8 == 0");
-  TORCH_CHECK(bias.scalar_type() == torch::kFloat32 && bias.numel() == Wb.size(1) && ((uintptr_t)bias.data_ptr() % 8) == 0,
+  const int64_t Cw = vocab_classes(h, Wb, w_kmajor, "vocab sample");
+  TORCH_CHECK(h.size(0) >= 1 && h.size(0) < (int64_t(1) << 24), "vocab sample: h bf16 [B,H] with 1 <= B < 2^24");
+  TORCH_CHECK(h.size(1) % 64 == 0 && Cw % 8 == 0 && Cw >= 8, "vocab sample: H % 64 == 0 and C % 8 == 0");
+  TORCH_CHECK(bias.scalar_type() == torch::kFloat32 && bias.numel() == Cw && ((uintptr_t)bias.data_ptr() % 8) == 0,
               "vocab sample: bias fp32 [C]");
   c10::cuda::CUDAGuard g(h.device());
-  const int B = h.size(0), H = h.size(1), C = Wb.size(1);
+  const int B = h.size(0), H = h.size(1), C = (int)Cw;
   const SampleOut o = sample_check(B, h, step, row0, tokens, rec_tok, rec_lp, temperature);
   const int nt = ts_vocab_head_parts(C);
   auto fo = torch::TensorOptions().device(h.device()).dtype(torch::kFloat32);
   auto part = torch::empty({(int64_t)B * nt * 4}, fo), logprob = torch::empty({B}, fo);
   auto part_arg = torch::empty({(int64_t)B * nt}, fo.dtype(torch::kInt32)), ticket = torch::zeros({1}, fo.dtype(torch::kInt32));
-  check(ts_vocab_sample(h.data_ptr(), Wb.data_ptr(), bias.data_ptr<float>(), (float)temperature, (unsigned int)(seed & 0xffffffff),
+  check(ts_vocab_sample(h.data_ptr(), Wb.data_ptr(), w_kmajor ? 1 : 0, bias.data_ptr<float>(), (float)temperature, (unsigned int)(seed & 0xffffffff),
                         step.data_ptr<int>(), row0.data_ptr<int>(), part.data_ptr(), part_arg.data_ptr<int>(), (unsigned int*)ticket.data_ptr<int>(),
                         tokens.data_ptr<int>(), logprob.data_ptr<float>(), o.rec_tok, o.rec_lp, o.N, (int)s0, B, H, C, h.get_device(),
                         stream()), "vocab_sample");
@@ -944,12 +953,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("head_step_bwd", &head_step_bwd, py::arg("h"), py::arg("W"), py::arg("dlogits"), py::arg("dloss"), py::arg("dW"), py::arg("db"),
         py::arg("accumulate"));
   m.def("vocab_head_parts", [](int64_t C) { return ts_vocab_head_parts((int)C); });
-  m.def("vocab_head_fwd", &vocab_head_fwd, py::arg("h"), py::arg("Wb"), py::arg("bias"), py::arg("labels"), py::arg("lengths"),
+  m.def("vocab_head_fwd", &vocab_head_fwd, py::arg("h"), py::arg("Wb"), py::arg("w_kmajor"), py::arg("bias"), py::arg("labels"), py::arg("lengths"),
         py::arg("T"), py::arg("part"));
-  m.def("vocab_head_dlogits", &vocab_head_dlogits, py::arg("h"), py::arg("Wb"), py::arg("bias"), py::arg("labels"), py::arg("lengths"),
+  m.def("vocab_head_dlogits", &vocab_head_dlogits, py::arg("h"), py::arg("Wb"), py::arg("w_kmajor"), py::arg("bias"), py::arg("labels"), py::arg("lengths"),
         py::arg("T"), py::arg("lse"), py::arg("count"), py::arg("dloss"), py::arg("row0"), py::arg("rows"), py::arg("dl"));
   m.def("vocab_head_colsum", &vocab_head_colsum, py::arg("dl"), py::arg("db"), py::arg("accumulate"));
-  m.def("vocab_sample", &vocab_sample, py::arg("h"), py::arg("Wb"), py::arg("bias"), py::arg("temperature"), py::arg("seed"),
+  m.def("vocab_sample", &vocab_sample, py::arg("h"), py::arg("Wb"), py::arg("w_kmajor"), py::arg("bias"), py::arg("temperature"), py::arg("seed"),
         py::arg("step"), py::arg("row0"), py::arg("tokens"), py::arg("rec_tok"), py::arg("rec_lp"), py::arg("s0"));
   m.def("vocab_sample_logits", &vocab_sample_logits, py::arg("logits"), py::arg("temperature"), py::arg("seed"), py::arg("step"),
         py::arg("row0"), py::arg("tokens"), py::arg("rec_tok"), py::arg("rec_lp"), py::arg("s0"));

@@ -2,6 +2,8 @@
 // h [R = T·B, H] without ever storing the logits [R, C] or an fp32 dlogits [R, C].
 //
 //   logits = h [R,H] (bf16, K-major) · W [H,C] (bf16, read in place as an MN-major operand) + bias (fp32), fp32 accumulators.
+//   With tied embeddings the weights are the embedding table [C,H] = W^T, read in place as a K-major operand (kBK = true
+//   below): the same products in the same k order, only the shared-memory layout of the B tile differs.
 //
 //   * vocab_head_gemm_kernel<kFwd>: TMA + wgmma over 128-row x 256-class tiles (a cluster of two CTAs computes 256 rows and
 //     shares the W tile by multicast, as gemm2_wgmma.cu).  The epilogue never writes the tile: per row it reduces the tile's
@@ -120,7 +122,9 @@ TC_DEVICE void tile_coords(int tile, int tiles_m, int tiles_n, int& tm, int& tn)
   tm = band * kBandTiles + rem - tn * gm;
 }
 
-template <int kMode>
+// kBK: the B operand is a K-major table [C, H] (tied embeddings), else the MN-major W [H, C].  K-major: each CTA's half of the
+// 256-class tile is one TMA box of 64 k (128 B, one swizzle atom) x 128 class rows, multicast to both CTAs like the W boxes.
+template <int kMode, bool kBK>
 __global__ void __launch_bounds__(kThreads, 1)
 vocab_head_gemm_kernel(const __grid_constant__ CUtensorMap tmap_h, const __grid_constant__ CUtensorMap tmap_w, const VocabParams p) {
   extern __shared__ uint8_t smem_raw[];
@@ -173,8 +177,12 @@ vocab_head_gemm_kernel(const __grid_constant__ CUtensorMap tmap_h, const __grid_
             tc::mbar_expect_tx_u32(fb, kStageBytes);
             tc::tma_load_2d_u32(sa0 + stage * kABytes, &tmap_h, fb, k0, m0);
             const uint32_t sb = sb0 + stage * kBBytes + crank * (kBBytes / kCtas);     // this CTA's half of the W tile
+            if (kBK) {
+              tc::tma_load_2d_mc(sb, &tmap_w, fb, k0, n0, 3);                              // class rows [n0, n0 + 128)
+            } else {
 #pragma unroll
-            for (int j = 0; j < BN / kCtas / 64; ++j) tc::tma_load_2d_mc(sb + j * 8192, &tmap_w, fb, n0 + 64 * j, k0, 3);
+              for (int j = 0; j < BN / kCtas / 64; ++j) tc::tma_load_2d_mc(sb + j * 8192, &tmap_w, fb, n0 + 64 * j, k0, 3);
+            }
           }
           __syncwarp();
           if (++stage == kStages) { stage = 0; phase ^= 1; }
@@ -189,7 +197,8 @@ vocab_head_gemm_kernel(const __grid_constant__ CUtensorMap tmap_h, const __grid_
     const uint32_t full0 = tc::smem_u32(full), empty0 = tc::smem_u32(empty);
     const uint32_t empty0_peer = mapa(empty0, crank ^ 1u);
     const uint64_t da0 = tc::desc_kmajor_sw128(tc::smem_u32(smem_a) + wg * 8192);
-    const uint64_t db0 = tc::desc_mnmajor_sw128(tc::smem_u32(smem_b));
+    const uint64_t db0 = kBK ? tc::desc_kmajor_sw128(tc::smem_u32(smem_b)) : tc::desc_mnmajor_sw128(tc::smem_u32(smem_b));
+    constexpr uint32_t kBStep = kBK ? (32 >> 4) : (2048 >> 4);   // per k16: 32 B along a K-major row, 16 rows of the MN-major tile
     auto release = [&](uint32_t st) {                     // this warp has finished reading stage st (in both CTAs)
       if (lane == 0) {
         tc::mbar_arrive_u32(empty0 + 8 * st);
@@ -215,7 +224,7 @@ vocab_head_gemm_kernel(const __grid_constant__ CUtensorMap tmap_h, const __grid_
         tc::wgmma_fence();
 #pragma unroll
         for (int k = 0; k < BK / 16; ++k)
-          tc::Wgmma<BN, 0, 1>::mma(acc, da + k * (32 >> 4), db + k * (2048 >> 4), (kb > 0 || k > 0) ? 1u : 0u);
+          tc::Wgmma<BN, 0, kBK ? 0 : 1>::mma(acc, da + k * (32 >> 4), db + k * kBStep, (kb > 0 || k > 0) ? 1u : 0u);
         tc::wgmma_commit();
         tc::fence_regs(acc);
         if (kb > 0) { tc::wgmma_wait<1>(); release(prev); }     // the previous stage's MMAs have retired
@@ -607,13 +616,15 @@ VocabParams sample_params(const float* bias, void* part, int* part_arg, int* ste
   return p;
 }
 
-template <int kMode>
-int launch_gemm(const void* h, const void* Wb, const VocabParams& p, int dev, cudaStream_t st) {
+template <int kMode, bool kBK>
+int launch_gemm_b(const void* h, const void* Wb, const VocabParams& p, int dev, cudaStream_t st) {
   if (p.H % BK != 0 || p.C % 8 != 0 || p.C < 8 || p.rows < 1) { ts::set_last_error("vocab head: needs H % 64 == 0 and C % 8 == 0"); return -2; }
+  if (kBK && reinterpret_cast<uintptr_t>(Wb) % 16 != 0) { ts::set_last_error("vocab head: the K-major table must be 16-byte aligned"); return -2; }
   CUtensorMap th, tw;
   if (int rc = ts::make_tmap_2d_bf16(&th, h, (uint64_t)p.R, (uint64_t)p.H, (uint64_t)p.H, BK, BM)) return rc;
-  if (int rc = ts::make_tmap_2d_bf16(&tw, Wb, (uint64_t)p.H, (uint64_t)p.C, (uint64_t)p.C, 64, BK)) return rc;
-  auto kern = vocab_head_gemm_kernel<kMode>;
+  if (kBK) { if (int rc = ts::make_tmap_2d_bf16(&tw, Wb, (uint64_t)p.C, (uint64_t)p.H, (uint64_t)p.H, BK, BN / kCtas)) return rc; }
+  else     { if (int rc = ts::make_tmap_2d_bf16(&tw, Wb, (uint64_t)p.H, (uint64_t)p.C, (uint64_t)p.C, 64, BK)) return rc; }
+  auto kern = vocab_head_gemm_kernel<kMode, kBK>;
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);
@@ -633,6 +644,12 @@ int launch_gemm(const void* h, const void* Wb, const VocabParams& p, int dev, cu
   return (int)cudaLaunchKernelEx(&cfg, kern, th, tw, p);
 }
 
+// w_kmajor: Wb is the table [C, H] (tied embeddings), else W [H, C]
+template <int kMode>
+int launch_gemm(const void* h, const void* Wb, int w_kmajor, const VocabParams& p, int dev, cudaStream_t st) {
+  return w_kmajor ? launch_gemm_b<kMode, true>(h, Wb, p, dev, st) : launch_gemm_b<kMode, false>(h, Wb, p, dev, st);
+}
+
 }  // namespace
 
 // Scratch of the forward: part = float4 [R, ts_vocab_head_parts(C)]; part_loss / part_ok = [ts_vocab_head_blocks(R)]; 1 zeroed
@@ -640,16 +657,17 @@ int launch_gemm(const void* h, const void* Wb, const VocabParams& p, int dev, cu
 extern "C" int ts_vocab_head_parts(int C) { return (C + BN - 1) / BN; }
 extern "C" int ts_vocab_head_blocks(int R) { return (R + kCombWarps - 1) / kCombWarps; }
 
-// h: bf16 [R = T·B, H] packed time-major rows, Wb: bf16 [H, C] packed, labels int64 [B, T], lengths int32 [B] or null.
+// h: bf16 [R = T·B, H] packed time-major rows, Wb: bf16 [H, C] packed (w_kmajor: the table [C, H] packed, 16-byte aligned),
+// labels int64 [B, T], lengths int32 [B] or null.
 // -> lse [R], loss (mean NLL over the counted rows), correct, count (N) [1] each.
-extern "C" int ts_vocab_head_fwd(const void* h, const void* Wb, const float* bias, const long long* labels, const int* lengths,
+extern "C" int ts_vocab_head_fwd(const void* h, const void* Wb, int w_kmajor, const float* bias, const long long* labels, const int* lengths,
                                  void* part, float* lse, float* part_loss, int* part_ok, unsigned int* ticket, float* loss,
                                  int* correct, int* count, int T, int B, int H, int C, int dev, cudaStream_t st) {
   const int R = T * B;
   VocabParams p{};
   p.bias = bias; p.labels = labels; p.lengths = lengths; p.part = reinterpret_cast<float4*>(part);
   p.R = R; p.H = H; p.C = C; p.T = T; p.B = B; p.row0 = 0; p.rows = R;
-  if (int rc = launch_gemm<kFwd>(h, Wb, p, dev, st)) return rc;
+  if (int rc = launch_gemm<kFwd>(h, Wb, w_kmajor, p, dev, st)) return rc;
   CombineParams c{reinterpret_cast<const float4*>(part), labels, lengths, lse, part_loss, part_ok, ticket, loss, correct, count,
                   R, T, B, ts_vocab_head_parts(C)};
   vocab_head_combine_kernel<<<ts_vocab_head_blocks(R), kCombWarps * 32, 0, st>>>(c);
@@ -657,7 +675,7 @@ extern "C" int ts_vocab_head_fwd(const void* h, const void* Wb, const float* bia
 }
 
 // dl [rows, C] bf16 = dlogits of rows [row0, row0 + rows) of h (see the top of the file); lse / count from the forward.
-extern "C" int ts_vocab_head_dlogits(const void* h, const void* Wb, const float* bias, const long long* labels, const int* lengths,
+extern "C" int ts_vocab_head_dlogits(const void* h, const void* Wb, int w_kmajor, const float* bias, const long long* labels, const int* lengths,
                                      const float* lse, const float* dloss, const int* count, void* dl, int T, int B, int H, int C,
                                      int row0, int rows, int dev, cudaStream_t st) {
   VocabParams p{};
@@ -665,7 +683,7 @@ extern "C" int ts_vocab_head_dlogits(const void* h, const void* Wb, const float*
   p.dl = reinterpret_cast<__nv_bfloat16*>(dl);
   p.R = T * B; p.H = H; p.C = C; p.T = T; p.B = B; p.row0 = row0; p.rows = rows;
   if (row0 < 0 || row0 % BM != 0 || row0 + rows > p.R) { ts::set_last_error("vocab head: a chunk starts at a multiple of 128 rows inside h"); return -2; }
-  return launch_gemm<kDlogits>(h, Wb, p, dev, st);
+  return launch_gemm<kDlogits>(h, Wb, w_kmajor, p, dev, st);
 }
 
 // db [C] (+)= column sums of dl [rows, C] (bf16), C even.
@@ -674,15 +692,15 @@ extern "C" int ts_vocab_head_colsum(const void* dl, float* db, int rows, int C, 
   return (int)cudaGetLastError();
 }
 
-// Sampling (see sample_score above): h bf16 [B, H], Wb bf16 [H, C], bias fp32 [C]; part float4 [B, ts_vocab_head_parts(C)],
+// Sampling (see sample_score above): h bf16 [B, H], Wb bf16 [H, C] (w_kmajor: [C, H]), bias fp32 [C]; part float4 [B, ts_vocab_head_parts(C)],
 // part_arg int [B, ts_vocab_head_parts(C)], 1 zeroed ticket word (left zeroed); step int [1], advanced by one; row_base int [1],
 // the noise counter's row word of row 0.
 // -> tokens [B], logprob [B], and with rec_tok / rec_lp [B, N] column step - s0 of each.
-extern "C" int ts_vocab_sample(const void* h, const void* Wb, const float* bias, float temperature, unsigned int seed, int* step,
+extern "C" int ts_vocab_sample(const void* h, const void* Wb, int w_kmajor, const float* bias, float temperature, unsigned int seed, int* step,
                                const int* row_base, void* part, int* part_arg, unsigned int* ticket, int* tokens, float* logprob, int* rec_tok,
                                float* rec_lp, int N, int s0, int B, int H, int C, int dev, cudaStream_t st) {
   const VocabParams p = sample_params(bias, part, part_arg, step, row_base, seed, temperature, B, H, C);
-  if (int rc = launch_gemm<kSample>(h, Wb, p, dev, st)) return rc;
+  if (int rc = launch_gemm<kSample>(h, Wb, w_kmajor, p, dev, st)) return rc;
   return launch_sample_combine(p, ticket, tokens, logprob, rec_tok, rec_lp, N, s0, st);
 }
 

@@ -16,21 +16,29 @@ from .recurrent.rnn import RNN
 
 
 class DenseHead(nn.Module):
-    """``Dense1``: weights ``[H_last, C]`` (bidirectional: ``[2 H_last, C]``), bias ``[C]`` (truncated normal, src/rnn.py:214-221)."""
+    """``Dense1``: weights ``[H_last, C]`` (bidirectional: ``[2 H_last, C]``), bias ``[C]`` (truncated normal, src/rnn.py:214-221).
+    ``tied`` (``--tie_embeddings``): the weights are drawn as usual, so the bias and every later parameter get the draws of the
+    untied model, and then discarded (``weights`` is None): the softmax reads the embedding table instead."""
 
-    def __init__(self, in_features: int, num_classes: int, init_std: float = 1.0, device=None, generator=None):
+    def __init__(self, in_features: int, num_classes: int, init_std: float = 1.0, device=None, generator=None, tied: bool = False):
         super().__init__()
         init = lambda t, generator=None: truncated_normal_(t, init_std, generator)
         self.weights = create_variable("weights", (in_features, num_classes), initializer=init, device=device,
                                        generator=generator)
         self.bias = create_variable("bias", (num_classes,), initializer=init, device=device, generator=generator)
+        if tied:
+            self.weights = None
 
-    def forward(self, h: torch.Tensor) -> torch.Tensor:
+    def forward(self, h: torch.Tensor, weights: Optional[torch.Tensor] = None, class_major: bool = False) -> torch.Tensor:
+        """Evaluation logits ``h W + bias``; ``weights``: the matrix to read instead of ``self.weights`` (``class_major``: it is
+        ``[C,H] = W^T``, the tied embedding table)."""
+        w = self.weights if weights is None else weights
         h2 = h.reshape(h.shape[0], -1)
         if h2.is_cuda and F.get_backend() != "torch":
             from ..ops import cuda_gemm             # evaluation logits: our own GEMM kernels, no library call on the CUDA path
-            return cuda_gemm.matmul(h2, self.weights.detach().t(), bias=self.bias.detach().float(), out_dtype=torch.float32)
-        return h2.float() @ self.weights + self.bias
+            w_t = w.detach() if class_major else w.detach().t()
+            return cuda_gemm.matmul(h2, w_t, bias=self.bias.detach().float(), out_dtype=torch.float32)
+        return h2.float() @ (w.t() if class_major else w) + self.bias
 
 
 class Attention(nn.Module):
@@ -79,7 +87,9 @@ class SequenceClassifier(nn.Module):
         head_std = cfg.init_std if cfg.init != "scaled" else cfg.init_std / (head_in ** 0.5)
         self.rnn = RNN(settings, dropout=cfg.dropout, learn_initial_state=cfg.resolved_learn_initial_state(), init_std=cfg.init_std,
                        init=cfg.init, weight_decay=(cfg.weight_decay or None), device=device, generator=generator)
-        self.head = DenseHead(head_in, cfg.num_classes, init_std=head_std, device=device, generator=generator)
+        # --tie_embeddings: the softmax reads the embedding table (head_weights); Dense1/weights is drawn and discarded
+        self.tied = bool(getattr(cfg, "tie_embeddings", False))
+        self.head = DenseHead(head_in, cfg.num_classes, init_std=head_std, device=device, generator=generator, tied=self.tied)
         if cfg.bidirectional:
             # drawn after every parameter of the unidirectional model, which therefore keeps its initial weights
             self.rnn.add_reverse_layers()
@@ -94,6 +104,9 @@ class SequenceClassifier(nn.Module):
         if self.vocab_size > 0:
             # drawn last (after the reverse layers and the attention weights): every run without it keeps its initial weights
             self.embedding = Embedding(self.vocab_size, cfg.in_features, init_std=cfg.init_std, device=device, generator=generator)
+        if self.tied and (self.embedding is None or tuple(self.embedding.weights.shape) != (cfg.num_classes, head_in)):
+            raise ValueError("--tie_embeddings needs --next_token with --in_features equal to the last --hidden_units: the softmax "
+                             "reads the [V, E] embedding table as its [E, V] weights")
         self.flat: Optional[FlatParams] = None
         self._allocator = allocator
         self._decoders: Dict[tuple, "_Decoder"] = {}       # generate(): static buffers (and CUDA graph), one per batch shape
@@ -114,9 +127,30 @@ class SequenceClassifier(nn.Module):
             if self.flat.data.is_cuda and F.get_backend() != "torch":
                 # the CUDA ops write these gradients straight into the flat buffer (first write of a step overwrites):
                 # zero_grad() then has nothing to memset
-                self.flat.enable_direct_grads(self.rnn.averaged_parameters() + [self.head.weights, self.head.bias] +
+                self.flat.enable_direct_grads(self.rnn.averaged_parameters() +
+                                              [p for p in (self.head.weights, self.head.bias) if p is not None] +
                                               ([] if self.attention is None else list(self.attention.params())) +
                                               ([] if self.embedding is None else [self.embedding.weights]))
+
+    def head_weights(self) -> Tuple[torch.Tensor, bool]:
+        """-> (the matrix the softmax reads, class_major): ``Dense1/weights [H_last, C]``, or with ``--tie_embeddings`` the
+        embedding table ``[V, E]`` itself (``W = table^T``: logits_c = h . table[c] + bias_c).  The table is handed over as it is,
+        never as a transposed view: the ops find its bf16 shadow and its gradient sink by its address and shape.  Every use of
+        the head (training, scoring, evaluation logits, sampling) reads the weights through here."""
+        if self.tied:
+            return self.embedding.weights, True
+        return self.head.weights, False
+
+    def _dense_weights(self) -> torch.Tensor:
+        """The head's ``W [H_last, C]`` for the ops that take no class-major operand (the per-step head of fewer than 512
+        classes, fp32, the torch backend): with ``--tie_embeddings`` the table's transpose through autograd, so its gradient
+        reaches the table in the table's layout."""
+        w, class_major = self.head_weights()
+        return w.t().contiguous() if class_major else w
+
+    def head_logits(self, h: torch.Tensor) -> torch.Tensor:
+        """Evaluation logits ``[rows, C]`` fp32 of ``h [rows, H_last]``."""
+        return self.head(h, *self.head_weights())
 
     def _is_sequence(self, x: torch.Tensor) -> bool:
         """Whole sequences: ``[B,T,D]`` features, or ``[B,T]`` token ids with ``--vocab_size``."""
@@ -186,9 +220,10 @@ class SequenceClassifier(nn.Module):
         if self.per_step:
             h_seq = self.sequence_features(x, lengths, state)
             if F.vocab_head_supported(h_seq, self.cfg.num_classes):
-                loss, correct, _n = F.vocab_xent_per_step(h_seq, self.head.weights, self.head.bias, labels, lengths)
+                w, class_major = self.head_weights()
+                loss, correct, _n = F.vocab_xent_per_step(h_seq, w, self.head.bias, labels, lengths, class_major=class_major)
                 return loss, None, correct
-            logits, loss, correct, _n = F.head_xent_per_step(h_seq, self.head.weights, self.head.bias, labels, lengths)
+            logits, loss, correct, _n = F.head_xent_per_step(h_seq, self._dense_weights(), self.head.bias, labels, lengths)
             return loss, logits, correct
         self._whole_sequences_only(state)
         h = self.features(x, lengths)
@@ -210,17 +245,18 @@ class SequenceClassifier(nn.Module):
                     B, T = labels.shape
                     full = torch.full((B,), T, dtype=torch.int32, device=h_seq.device) if lengths is None else lengths
                     lengths = torch.where(torch.arange(B, device=h_seq.device) < first, torch.zeros_like(full), full)
-                return F.vocab_xent_per_step(h_seq, self.head.weights, self.head.bias, labels, lengths)
+                w, class_major = self.head_weights()
+                return F.vocab_xent_per_step(h_seq, w, self.head.bias, labels, lengths, class_major=class_major)
             labels = labels[first:]
             if first == 0:
-                _logits, loss, correct, n = F.head_xent_per_step(h_seq, self.head.weights, self.head.bias, labels, lengths)
+                _logits, loss, correct, n = F.head_xent_per_step(h_seq, self._dense_weights(), self.head.bias, labels, lengths)
                 return loss, correct, n
             h_seq = h_seq[:, first:]
-            logits = self.head(h_seq.reshape(-1, h_seq.shape[2])).float().view(h_seq.shape[0], h_seq.shape[1], -1)
+            logits = self.head_logits(h_seq.reshape(-1, h_seq.shape[2])).float().view(h_seq.shape[0], h_seq.shape[1], -1)
             return ref.softmax_xent_per_step(logits.transpose(0, 1), labels, None if lengths is None else lengths[first:])
         labels = labels[first:]
         self._whole_sequences_only(state)
-        logits = self.head(self.features(x, lengths))[first:].float()
+        logits = self.head_logits(self.features(x, lengths))[first:].float()
         count = torch.full((), labels.shape[0], dtype=torch.int64, device=logits.device)
         return ref.softmax_xent(logits, labels), (logits.argmax(1) == labels).sum(), count
 
@@ -281,7 +317,8 @@ class SequenceClassifier(nn.Module):
         out = []
         for layer in self.rnn.directions():
             out += layer.named_reference_variables()
-        out.append(("Dense1/weights", self.head.weights))
+        if not self.tied:                           # --tie_embeddings: the softmax reads Embedding/weights
+            out.append(("Dense1/weights", self.head.weights))
         out.append(("Dense1/bias", self.head.bias))
         if self.attention is not None:
             out.append(("Attention/weights", self.attention.weights))
@@ -294,11 +331,27 @@ class SequenceClassifier(nn.Module):
     def check_compatible(self, variables: Dict[str, torch.Tensor], settings: Dict, what: str = "checkpoint") -> None:
         """Raise unless ``variables`` and the flags ``settings`` recorded beside them (``utils.checkpoint.recorded_settings``)
         were written by a model this one can load: the same directions, ``--pooling``, ``--vocab_size`` and ``--next_token``,
-        checked in that order."""
+        checked in that order, then ``--tie_embeddings``."""
         self.check_directions(variables, what)
         self.check_pooling(variables, settings.get("pooling"), what)
         self.check_vocab(variables, settings.get("vocab_size"), what)
         self.check_next_token(settings.get("next_token"), what)
+        self.check_tied(variables, settings.get("tie_embeddings"), what)
+
+    def check_tied(self, variables: Dict[str, torch.Tensor], recorded: Optional[bool] = None, what: str = "checkpoint") -> None:
+        """Raise unless ``variables`` (and the flag ``recorded`` beside them; nothing recorded counts as untied) were written
+        under this model's ``--tie_embeddings``: a checkpoint loads with ``strict=False`` and would otherwise leave an untied
+        model's Dense1/weights at their initial values, or silently drop a trained softmax matrix."""
+        saved, has_w = bool(recorded), "Dense1/weights" in variables
+        if saved == self.tied and has_w == (not self.tied):
+            return
+        desc = "with" if saved else "without"
+        if saved == has_w:
+            desc += f" --tie_embeddings but {'with' if has_w else 'without'} a Dense1/weights matrix"
+        else:
+            desc += " --tie_embeddings"
+        raise ValueError(f"{what} was written {desc}, this run is {'with' if self.tied else 'without'} it: "
+                         f"{'drop' if self.tied else 'add'} --tie_embeddings")
 
     def check_next_token(self, recorded: Optional[bool] = None, what: str = "checkpoint") -> None:
         """Raise unless the file was written with this run's ``--next_token`` (nothing recorded counts as off): the variables
@@ -374,9 +427,9 @@ class _Decoder:
         self.graph = None
 
     def sample(self, h: torch.Tensor) -> None:
-        head = self.model.head
-        F.vocab_sample(h, head.weights, head.bias, self.temperature, self.seed, self.step, tokens=self.tokens,
-                       record=(self.tokens_out, self.logprob_out, 0), row0=self.row0)
+        w, class_major = self.model.head_weights()
+        F.vocab_sample(h, w, self.model.head.bias, self.temperature, self.seed, self.step, tokens=self.tokens,
+                       record=(self.tokens_out, self.logprob_out, 0), row0=self.row0, class_major=class_major)
 
     def run(self) -> None:
         """One decode step: embed the previous token, one step of every layer from the buffers (which get the new state), sample."""

@@ -94,6 +94,18 @@ class _HeadXentStepFn(torch.autograd.Function):
         sw, sb = grad_sink(ctx.addrs[0]), grad_sink(ctx.addrs[1])
         dl = dloss.detach().float().reshape(1).contiguous()
         dw = db = None
+        if (sw is None) != (sb is None):
+            # one of the two has a sink: a tied head (--tie_embeddings) reads the table's transpose, a tensor of its own, next to
+            # the registered bias.  That sink is taken by now, so it gets its gradient here; the other goes back to autograd
+            dw = torch.empty_like(w)
+            db = torch.empty(w.shape[1], dtype=torch.float32, device=w.device)
+            dh = E.head_step_bwd(h2, w, dlogits, dl, dw, db, False)
+            for sink, g in ((sw, dw), (sb, db)):
+                if sink is not None and sink[1]:
+                    sink[0].add_(g)
+                elif sink is not None:
+                    sink[0].copy_(g)
+            return dh.view(ctx.shape).to(ctx.h_dtype), None if sw is not None else dw, None if sb is not None else db, None, None
         if sw is not None and sb is not None:
             if sw[1] != sb[1]:                             # one of the two already holds a gradient: bring both to "accumulate"
                 if not sw[1]:

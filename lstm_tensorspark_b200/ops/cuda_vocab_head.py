@@ -7,6 +7,10 @@ order on one stream: the logits of the chunk are recomputed and turned into bf16
 then ``dh = dlogits W^T``, ``dW += h^T dlogits`` (straight into the flat gradient buffer) and ``db += column sums`` - every sum in
 a fixed order, so two calls on the same inputs give the same bits.  N, lse and the masks stay on the device: a captured CUDA
 graph holds across batches with other lengths.
+
+``class_major=True`` (tied embeddings): ``weights`` is the embedding table ``[C,H] = W^T`` itself, which the head kernels read in
+place as a K-major operand.  Backward then computes ``dh = dlogits · table`` and ``dTable (+)= dlogits^T h`` into the table's
+gradient sink, where the embedding's scatter-add later in the same backward pass adds its own part.
 """
 from __future__ import annotations
 
@@ -26,23 +30,38 @@ def supported(h_seq: torch.Tensor, num_classes: int) -> bool:
             and num_classes % 8 == 0 and num_classes >= MIN_CLASSES)
 
 
+def _weights_lowp(weights: torch.Tensor, class_major: bool) -> torch.Tensor:
+    """The bf16 operand of the head kernels: the maintained shadow, or one rounding of the fp32 weights.  ``class_major``: the
+    table ``[C,H]`` itself (never a transposed view: the shadow and the gradient sink are found by the parameter's address and
+    shape), read by TMA in place, which needs a 16-byte aligned base (FlatParams places every parameter at a multiple of 64
+    elements, so a shadow view always is) and ``H % 8 == 0`` (implied by ``H % 64 == 0``)."""
+    from .cuda_lstm import _lowp
+    wb = _lowp(weights, torch.bfloat16)
+    if class_major:
+        assert wb.is_contiguous() and wb.data_ptr() % 16 == 0, "the tied table's bf16 operand must be packed and 16-byte aligned"
+    return wb
+
+
 class _VocabXentFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, h_seq, weights, bias, labels, lengths):
-        from .cuda_lstm import STATS, _lowp
+    def forward(ctx, h_seq, weights, bias, labels, lengths, class_major=False):
+        from .cuda_lstm import STATS
         E = ext()
         T, B, H = h_seq.shape
         hc = h_seq.detach()
         h2 = hc.reshape(T * B, H) if hc.is_contiguous() else hc.contiguous().view(T * B, H)
-        wb = _lowp(weights, torch.bfloat16)                   # the maintained bf16 shadow, or one rounding of the fp32 weights
+        wb = _weights_lowp(weights, class_major)
         b = bias.detach().float().contiguous()
         lab = labels.long().contiguous()
         ln = None if lengths is None else lengths.contiguous()
-        part = torch.empty(T * B * E.vocab_head_parts(wb.shape[1]) * 4, dtype=torch.float32, device=h2.device)
-        lse, loss, correct, count = E.vocab_head_fwd(h2, wb, b, lab, ln, T, part)
+        C = wb.shape[0 if class_major else 1]
+        part = torch.empty(T * B * E.vocab_head_parts(C) * 4, dtype=torch.float32, device=h2.device)
+        lse, loss, correct, count = E.vocab_head_fwd(h2, wb, bool(class_major), b, lab, ln, T, part)
         STATS["vocab_head_fwd"] = STATS.get("vocab_head_fwd", 0) + 1
+        if class_major:
+            STATS["vocab_head_fwd_tied"] = STATS.get("vocab_head_fwd_tied", 0) + 1
         ctx.save_for_backward(h2, wb, b, lab, ln, lse, count)
-        ctx.shape = (T, B, H)
+        ctx.shape, ctx.class_major = (T, B, H), bool(class_major)
         ctx.addrs = (weights.data_ptr(), bias.data_ptr())
         ctx.mark_non_differentiable(correct, count)
         return loss.squeeze(0), correct.squeeze(0), count.squeeze(0)
@@ -52,16 +71,16 @@ class _VocabXentFn(torch.autograd.Function):
         from .cuda_lstm import STATS, grad_sink
         E = ext()
         h2, wb, b, lab, ln, lse, count = ctx.saved_tensors
-        T = ctx.shape[0]
+        T, cm = ctx.shape[0], ctx.class_major
         R, H = h2.shape
-        C = wb.shape[1]
+        C = wb.shape[0 if cm else 1]
         sw, sb = grad_sink(ctx.addrs[0]), grad_sink(ctx.addrs[1])
         scale = dloss.detach().float().reshape(1).contiguous()
         if sw is not None and sb is not None:
             (dw, acc_w), (db, acc_b) = sw, sb
             ret = (None, None)
         else:
-            dw = torch.empty(H, C, dtype=torch.float32, device=h2.device)
+            dw = torch.empty(*((C, H) if cm else (H, C)), dtype=torch.float32, device=h2.device)
             db = torch.empty(C, dtype=torch.float32, device=h2.device)
             acc_w = acc_b = False
             ret = (dw, db)
@@ -70,17 +89,22 @@ class _VocabXentFn(torch.autograd.Function):
         for r0 in range(0, R, ROW_CHUNK):
             rows = min(ROW_CHUNK, R - r0)
             d = dl[:rows]
-            E.vocab_head_dlogits(h2, wb, b, lab, ln, T, lse, count, scale, r0, rows, d)
-            G.matmul(d, wb, out=dh[r0:r0 + rows])                                              # dh = dlogits W^T
-            G.matmul(h2[r0:r0 + rows].t(), d.t(), out=dw, accumulate=bool(acc_w or r0 > 0))    # dW (+)= h^T dlogits
+            E.vocab_head_dlogits(h2, wb, cm, b, lab, ln, T, lse, count, scale, r0, rows, d)
+            acc = bool(acc_w or r0 > 0)
+            if cm:
+                G.matmul(d, wb.t(), out=dh[r0:r0 + rows])                                      # dh = dlogits table
+                G.matmul(d.t(), h2[r0:r0 + rows].t(), out=dw, accumulate=acc)                   # dTable (+)= dlogits^T h
+            else:
+                G.matmul(d, wb, out=dh[r0:r0 + rows])                                          # dh = dlogits W^T
+                G.matmul(h2[r0:r0 + rows].t(), d.t(), out=dw, accumulate=acc)                   # dW (+)= h^T dlogits
             E.vocab_head_colsum(d, db.view(-1), bool(acc_b or r0 > 0))
         STATS["vocab_head_bwd"] = STATS.get("vocab_head_bwd", 0) + 1
-        return dh.view(ctx.shape), ret[0], ret[1], None, None
+        return dh.view(ctx.shape), ret[0], ret[1], None, None, None
 
 
-def vocab_xent_per_step(h_seq, weights, bias, labels, lengths=None):
+def vocab_xent_per_step(h_seq, weights, bias, labels, lengths=None, class_major=False):
     """-> (mean loss over the counted positions, correct count, N); see ``ops.functional.vocab_xent_per_step``."""
-    return _VocabXentFn.apply(h_seq, weights, bias, labels, lengths)
+    return _VocabXentFn.apply(h_seq, weights, bias, labels, lengths, bool(class_major))
 
 
 def _device_int(v, device):
@@ -93,16 +117,18 @@ def _sample_args(step, row0, tokens, record, B, device):
     return _device_int(step, device), _device_int(row0, device), tok, rec_tok, rec_lp, s0
 
 
-def vocab_sample(h, weights, bias, temperature: float, seed: int, step, tokens=None, record=None, row0=0):
+def vocab_sample(h, weights, bias, temperature: float, seed: int, step, tokens=None, record=None, row0=0, class_major=False):
     """Sample the next token from ``h [B,H]`` bf16 through the head's tensor-core kernel (``kSample``), without storing the
     logits; see ``ops.functional.vocab_sample``."""
-    from .cuda_lstm import STATS, _lowp
+    from .cuda_lstm import STATS
     B = h.shape[0]
     step_t, row_t, tok, rec_tok, rec_lp, s0 = _sample_args(step, row0, tokens, record, B, h.device)
-    wb = _lowp(weights, torch.bfloat16)
-    lp = ext().vocab_sample(h.detach().contiguous(), wb, bias.detach().float().contiguous(), float(temperature), int(seed), step_t,
+    wb = _weights_lowp(weights, class_major)
+    lp = ext().vocab_sample(h.detach().contiguous(), wb, bool(class_major), bias.detach().float().contiguous(), float(temperature), int(seed), step_t,
                             row_t, tok, rec_tok, rec_lp, int(s0))
     STATS["vocab_sample"] = STATS.get("vocab_sample", 0) + 1
+    if class_major:
+        STATS["vocab_sample_tied"] = STATS.get("vocab_sample_tied", 0) + 1
     return tok, lp
 
 

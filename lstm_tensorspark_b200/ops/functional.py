@@ -88,21 +88,25 @@ def vocab_head_supported(h_seq, num_classes: int) -> bool:
     return cuda_vocab_head.supported(h_seq, num_classes)
 
 
-def vocab_xent_per_step(h_seq, weights, bias, labels, lengths=None):
+def vocab_xent_per_step(h_seq, weights, bias, labels, lengths=None, class_major: bool = False):
     """The per-step head for many classes (a next-token language model's softmax): the loss, the correct count and N of
     ``head_xent_per_step`` - the same mask, normalisation and gradients - without the logits, which are neither returned nor
     stored.  ``lengths`` may hold zeros here (a row that does not count at all).  On the GPU bf16 ``h_seq`` with
     ``H % 64 == 0``, ``C % 8 == 0`` and ``C >= 512`` runs on the tensor cores (csrc/head_vocab.cu); every other input goes
-    through ``head_xent_per_step``."""
-    if vocab_head_supported(h_seq, weights.shape[1]):
+    through ``head_xent_per_step``.  ``class_major``: ``weights`` is ``[C,H]`` (a tied embedding table, ``W^T``), read in place
+    by the tensor-core kernels; the other paths read ``weights.t().contiguous()`` through autograd, so the gradient reaches
+    ``weights`` in its own layout."""
+    C = weights.shape[0 if class_major else 1]
+    if vocab_head_supported(h_seq, C):
         from . import cuda_vocab_head
-        return cuda_vocab_head.vocab_xent_per_step(h_seq, weights, bias, labels, lengths)
+        return cuda_vocab_head.vocab_xent_per_step(h_seq, weights, bias, labels, lengths, class_major)
+    w = weights.t().contiguous() if class_major else weights
     if _use_ext(h_seq):
-        return head_xent_per_step(h_seq, weights, bias, labels, lengths)[1:]
-    return ref.vocab_xent_per_step(h_seq, weights, bias, labels, lengths)
+        return head_xent_per_step(h_seq, w, bias, labels, lengths)[1:]
+    return ref.vocab_xent_per_step(h_seq, w, bias, labels, lengths)
 
 
-def vocab_sample(h, weights, bias, temperature: float, seed: int, step, tokens=None, record=None, row0=0):
+def vocab_sample(h, weights, bias, temperature: float, seed: int, step, tokens=None, record=None, row0=0, class_major: bool = False):
     """Sample the next token of every row from the head's logits ``l = h W + bias`` (``h [B,H]``, ``W [H,C]``) without a host
     round trip -> (tokens int32 ``[B]``, log p(token) under ``softmax(l)`` fp32 ``[B]``).  Temperature 0 is the arg-max; above 0
     Gumbel-max with counter-based noise (``reference.sample_logits`` holds the definition).  ``step``: the decode step, an int
@@ -111,19 +115,21 @@ def vocab_sample(h, weights, bias, temperature: float, seed: int, step, tokens=N
     ``step - s0`` of each also gets them.  ``row0`` (an int or an int32 ``[1]`` device tensor): the noise counter's row word of
     row 0, the index of the batch's first prompt when prompts run in batches, so every prompt draws its own noise.  On the GPU bf16 ``h`` with ``H % 64 == 0``, ``C % 8 == 0`` and ``C >= 512`` runs in
     the head's tensor-core kernel (csrc/head_vocab.cu); every other input computes the fp32 logits with the head GEMM and
-    samples them with one more kernel.  Two calls on the same inputs give the same bits."""
+    samples them with one more kernel.  Two calls on the same inputs give the same bits.  ``class_major``: ``weights`` is
+    ``[C,H]`` (a tied embedding table, ``W^T``), read in place."""
     temperature = float(temperature)
     if not (math.isfinite(temperature) and temperature >= 0):
         raise ValueError(f"temperature must be finite and >= 0, got {temperature}")
-    if vocab_head_supported(h.unsqueeze(0), weights.shape[1]):
+    if vocab_head_supported(h.unsqueeze(0), weights.shape[0 if class_major else 1]):
         from . import cuda_vocab_head
-        return cuda_vocab_head.vocab_sample(h, weights, bias, temperature, seed, step, tokens, record, row0)
+        return cuda_vocab_head.vocab_sample(h, weights, bias, temperature, seed, step, tokens, record, row0, class_major)
     if _use_ext(h):
         from . import cuda_gemm, cuda_vocab_head
-        logits = cuda_gemm.matmul(h.reshape(h.shape[0], -1), weights.detach().t(), bias=bias.detach().float(), out_dtype=torch.float32)
+        w_t = weights.detach() if class_major else weights.detach().t()          # the GEMM's b_t operand: [C,H]
+        logits = cuda_gemm.matmul(h.reshape(h.shape[0], -1), w_t, bias=bias.detach().float(), out_dtype=torch.float32)
         return cuda_vocab_head.vocab_sample_logits(logits, temperature, seed, step, tokens, record, row0)
     s = int(step)
-    tok, logp = ref.vocab_sample(h, weights, bias, temperature, seed, s, int(row0))
+    tok, logp = ref.vocab_sample(h, weights, bias, temperature, seed, s, int(row0), class_major=class_major)
     logp = logp.float()
     if isinstance(step, torch.Tensor):
         step.add_(1)

@@ -244,9 +244,10 @@ def head_xent_per_step(h_seq, weights, bias, labels, lengths=None):
     return logits, loss, correct, keep.sum()
 
 
-def vocab_xent_per_step(h_seq, weights, bias, labels, lengths=None):
-    """``head_xent_per_step`` without the logits -> (loss, correct, N): the reference of the large-vocabulary head."""
-    return head_xent_per_step(h_seq, weights, bias, labels, lengths)[1:]
+def vocab_xent_per_step(h_seq, weights, bias, labels, lengths=None, class_major: bool = False):
+    """``head_xent_per_step`` without the logits -> (loss, correct, N): the reference of the large-vocabulary head.
+    ``class_major``: ``weights`` is ``[C,H]`` = ``W^T`` (a tied embedding table)."""
+    return head_xent_per_step(h_seq, weights.t() if class_major else weights, bias, labels, lengths)[1:]
 
 
 # ---- sampling the next token ------------------------------------------------------------------------------------------
@@ -296,9 +297,11 @@ def sample_logits(logits: torch.Tensor, temperature: float, seed: int, step: int
     return tok.to(torch.int32), logp
 
 
-def vocab_sample(h, weights, bias, temperature: float, seed: int, step, row0: int = 0):
-    """``sample_logits`` of ``l = h W + bias`` (``h [B,H]``, ``W [H,C]``) computed in fp64: the reference of the sampling op."""
-    return sample_logits(dense_head(h.double(), weights.double(), bias.double()), temperature, seed, int(step), int(row0))
+def vocab_sample(h, weights, bias, temperature: float, seed: int, step, row0: int = 0, class_major: bool = False):
+    """``sample_logits`` of ``l = h W + bias`` (``h [B,H]``, ``W [H,C]``; ``class_major``: ``weights`` is ``[C,H]`` = ``W^T``)
+    computed in fp64: the reference of the sampling op."""
+    w = weights.t() if class_major else weights
+    return sample_logits(dense_head(h.double(), w.double(), bias.double()), temperature, seed, int(step), int(row0))
 
 
 def softmax_xent_per_step(logits, labels, lengths=None):

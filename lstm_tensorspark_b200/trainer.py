@@ -588,7 +588,8 @@ def run_job(cfg: Config, standalone: bool = False) -> Dict:
                                  {"world_size": world_size, "sync_mode": cfg.sync_mode, "average_scope": cfg.average_scope,
                                   "hidden_units": cfg.hidden_units, "pooling": cfg.pooling,
                                   "attention_units": cfg.attention_units, "vocab_size": cfg.vocab_size,
-                                  "next_token": cfg.next_token, "stateful": cfg.stateful, "seconds": total})
+                                  "next_token": cfg.next_token, "stateful": cfg.stateful,
+                                  "tie_embeddings": cfg.tie_embeddings, "seconds": total})
     if not cfg.quiet:
         print("RNN-LSTM - Total Processing Time {}s".format(total))
     return {"results": results, "seconds": total, "world_size": world_size, "partitions": n_shards}
