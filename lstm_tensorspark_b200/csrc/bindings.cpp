@@ -762,8 +762,16 @@ Tensor gemm2(const Tensor& A, const Tensor& B, const std::optional<Tensor>& bias
                 C.scalar_type() == torch::kFloat32, "gemm2: rowsum must be a contiguous fp32 [M] next to an fp32 output");
     rp = rowsum->data_ptr<float>();
   }
+  TORCH_CHECK((ctas == 1 || ctas == 2) && (bn == 128 || bn == 256), "gemm2: ctas must be 1 or 2 and bn 128 or 256 (got ", ctas, ", ", bn, ")");
   unsigned int* dp = nullptr;
-  if (done.has_value()) { TORCH_CHECK(done->is_cuda() && done->scalar_type() == torch::kInt32, "gemm2: done int32 cuda"); dp = (unsigned int*)done->data_ptr<int>(); }
+  if (done.has_value()) {
+    TORCH_CHECK(done->is_cuda() && done->scalar_type() == torch::kInt32 && done->is_contiguous(), "gemm2: done must be a contiguous int32 cuda tensor");
+    // one counter per 128-row block and bn-column tile; a 2-CTA cluster's peer counts its block even where all its rows lie past M
+    const int64_t blocks = (M + 128 * ctas - 1) / (128 * ctas) * ctas * ((N + bn - 1) / bn);
+    TORCH_CHECK(done->numel() >= blocks, "gemm2: done needs ceil(M / (128 * ctas)) * ctas * ceil(N / bn) = ", blocks,
+                " counters, got ", done->numel());
+    dp = (unsigned int*)done->data_ptr<int>();
+  }
   check(ts_gemm2(A.data_ptr(), B.data_ptr(), C.data_ptr(), fptr(bias), M, N, K, (int)A.stride(0), (int)B.stride(0), (int)C.stride(0),
                  a_mn ? 1 : 0, b_mn ? 1 : 0, out_mode, (int)ctas, (int)bn, A.device().index(), (int)max_ctas, gp, gcfg, dp,
                  gate_err.has_value() ? gate_err->data_ptr<int>() : nullptr, pdl ? 1 : 0, (int)a_fold, (int)b_fold, (int)fold_cols,

@@ -363,6 +363,7 @@ extern "C" int ts_gemm2(const void* A, const void* B, void* C, const float* bias
                         int a_mn, int b_mn, int out_mode, int ctas, int bn, int dev, int max_ctas, const unsigned int* gate,
                         const int* gate_cfg, unsigned int* done, int* gate_err, int pdl, int a_fold, int b_fold, int fold_cols,
                         float* rowsum, int rowsum_acc, cudaStream_t st) {
+  if (M < 1 || N < 1 || K < 1) { ts::set_last_error("gemm2: M, N and K must be positive"); return -2; }
   if (K % 8 != 0 || lda % 8 != 0 || ldb % 8 != 0) { ts::set_last_error("gemm2: K and the operand pitches must be multiples of 8"); return -2; }
   if ((a_mn && M % 8 != 0) || (b_mn && N % 8 != 0) || N % 8 != 0) { ts::set_last_error("gemm2: M (MN-major A) / N must be multiples of 8"); return -2; }
   if (out_mode != OUT_BF16 && ldc % 2 != 0) { ts::set_last_error("gemm2: fp32 output needs an even row pitch"); return -2; }

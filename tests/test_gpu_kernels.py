@@ -217,28 +217,6 @@ def test_flat_update_kernels_against_fp64(E, dev, n, kind, t0, wd, gscale):
     print(f"\nflat {kind} n={n} t0={t0} wd={wd}: worst update ratio {worst:.3f}")
 
 
-@pytest.mark.parametrize("ctas,bn", [(1, 128), (1, 256), (2, 128), (2, 256)])
-@pytest.mark.parametrize("a_mn,b_mn", [(False, False), (False, True), (True, False), (True, True)])
-def test_tcgen05_gemm2(E, dev, ctas, bn, a_mn, b_mn):
-    """General wgmma GEMM: K-major / MN-major operands, 1-CTA tiles and 2-CTA clusters sharing B, bf16 / fp32 / accumulating output, ragged shapes."""
-    torch.manual_seed(0)
-    for (M, N, K) in [(128, 128, 64), (512, 512, 256), (1000, 520, 264), (4096, 1024, 2048)]:
-        A = (torch.randn(K, M, device=dev) * 0.5).bfloat16() if a_mn else (torch.randn(M, K, device=dev) * 0.5).bfloat16()
-        Bm = (torch.randn(K, N, device=dev) * 0.5).bfloat16() if b_mn else (torch.randn(N, K, device=dev) * 0.5).bfloat16()
-        bias = torch.randn(N, device=dev)
-        R = (A.float().t() if a_mn else A.float()) @ (Bm.float() if b_mn else Bm.float().t())
-        scale = float(R.abs().max())
-        C32 = E.gemm2(A, Bm, bias=bias, a_mn=a_mn, b_mn=b_mn, out_fp32=True, ctas=ctas, bn=bn)
-        assert (C32 - R - bias).abs().max() / scale < 2e-3
-        C16 = E.gemm2(A, Bm, a_mn=a_mn, b_mn=b_mn, ctas=ctas, bn=bn)
-        assert (C16.float() - R).abs().max() / scale < 1.6e-2
-        acc = torch.full((M, N), 3.0, device=dev)
-        E.gemm2(A, Bm, out=acc, a_mn=a_mn, b_mn=b_mn, accumulate=True, ctas=ctas, bn=bn)
-        assert (acc - 3.0 - R).abs().max() / scale < 2e-3
-        E.gemm2(A, Bm, out=acc, a_mn=a_mn, b_mn=b_mn, out_fp32=True, ctas=ctas, bn=bn)          # overwrite: no trace of the old content
-        assert (acc - R).abs().max() / scale < 2e-3
-
-
 @pytest.mark.parametrize("ctas,bn", [(1, 128), (2, 256)])
 @pytest.mark.parametrize("Bsz,T,F", [(128, 3, 128), (256, 5, 256), (384, 2, 512)])
 def test_tcgen05_gemm2_folded_batch_major_operand(E, dev, ctas, bn, Bsz, T, F):
