@@ -75,6 +75,8 @@ class Config:
                                         # table as its weights, logits = h Embedding^T + bias (Press & Wolf 2017), no Dense1/weights
     max_new_tokens: int = MAX_NEW_TOKENS_DEFAULT  # --mode generate: tokens sampled after each prompt
     temperature: float = TEMPERATURE_DEFAULT      # --mode generate: sample from softmax(logits / temperature); 0 = greedy
+    top_k: int = 0                      # --mode generate: sample from the k most likely classes only (ties at the k-th kept); 0 = off
+    top_p: float = 1.0                  # --mode generate: then from the smallest top set of tempered mass >= P (nucleus); 1 = off
     dtype: str = "auto"                 # auto: bf16 on cuda, fp32 on cpu
     device: str = "auto"                # auto | cpu | cuda
     backend: str = "auto"               # auto | cuda_ext (hand-written sm_90a kernels) | torch
@@ -252,12 +254,22 @@ class Config:
             raise ValueError(f"--max_new_tokens must be >= 1, got {self.max_new_tokens}")
         if not (math.isfinite(self.temperature) and self.temperature >= 0):
             raise ValueError(f"--temperature must be a finite number >= 0 (0 = greedy), got {self.temperature}")
+        if self.top_k < 0:
+            raise ValueError(f"--top_k must be an integer >= 0 (0 = off), got {self.top_k}")
+        if not (math.isfinite(self.top_p) and 0 < self.top_p <= 1):
+            raise ValueError(f"--top_p must be a number in (0, 1] (1 = off), got {self.top_p}")
         if self.mode == "generate" and not self.next_token:
             raise ValueError("--mode generate needs --next_token (and the --vocab_size the model was trained with): it continues "
                              "token sequences with a next-token language model")
-        for flag, default in (("max_new_tokens", MAX_NEW_TOKENS_DEFAULT), ("temperature", TEMPERATURE_DEFAULT)):
+        for flag, default in (("max_new_tokens", MAX_NEW_TOKENS_DEFAULT), ("temperature", TEMPERATURE_DEFAULT), ("top_k", 0),
+                              ("top_p", 1.0)):
             if getattr(self, flag) != default and self.mode != "generate":
                 warnings.warn(f"--{flag} {getattr(self, flag)} has no effect without --mode generate")
+        if self.mode == "generate" and self.temperature == 0:
+            for flag, default in (("top_k", 0), ("top_p", 1.0)):
+                if getattr(self, flag) != default:
+                    warnings.warn(f"--{flag} {getattr(self, flag)} has no effect with --temperature 0: greedy decoding takes the "
+                                  "arg-max, which every filter keeps")
         return self
 
 
@@ -291,6 +303,11 @@ _HELP = {
     "max_new_tokens": "--mode generate: tokens to sample after each prompt (>= 1)",
     "temperature": "--mode generate: sample from softmax(logits / temperature) by Gumbel-max with noise seeded by --seed; 0 = "
                    "greedy (the arg-max)",
+    "top_k": "--mode generate: sample only from the K classes with the largest logits (every class tied with the K-th is kept); "
+             "0 = off.  No effect at --temperature 0",
+    "top_p": "--mode generate: nucleus sampling, after --top_k: sample only from the classes with the largest logits whose "
+             "share of softmax(logits / temperature) first reaches P (ties at the cut are kept); 1 = off.  The reported "
+             "log-probabilities stay under the full softmax",
     "checkpoint_path": "Directory where to save network model and logs",
     "clip_grad_norm": "Clip the gradient by its global L2 norm to this value before the update, as "
                       "torch.nn.utils.clip_grad_norm_ (0 = off); the norm includes the --weight_decay term and, with "

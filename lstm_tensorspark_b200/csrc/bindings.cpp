@@ -59,8 +59,10 @@ int ts_vocab_head_dlogits(const void*, const void*, int, const float*, const lon
 int ts_vocab_head_colsum(const void*, float*, int, int, int, cudaStream_t);
 int ts_vocab_sample(const void*, const void*, int, const float*, float, unsigned int, int*, const int*, void*, int*, unsigned int*, int*,
                     float*, int*, float*, int, int, int, int, int, int, cudaStream_t);
-int ts_vocab_sample_logits(const float*, float, unsigned int, int*, const int*, void*, int*, unsigned int*, int*, float*, int*, float*,
-                           int, int, int, int, cudaStream_t);
+int ts_vocab_sample_logits(const float*, const float*, float, unsigned int, int*, const int*, void*, int*, unsigned int*, int*, float*, int*,
+                           float*, int, int, int, int, cudaStream_t);
+int ts_vocab_head_logits(const void*, const void*, int, const float*, float*, int, int, int, int, cudaStream_t);
+int ts_vocab_threshold(const float*, int, int, int, double, float, float*, cudaStream_t);
 int ts_gemm_generic(const void*, const void*, void*, const float*, int, int, int, long long, long long, long long, long long, long long,
                     int, int, int, float, cudaStream_t);
 int ts_gemm2(const void*, const void*, void*, const float*, int, int, int, int, int, int, int, int, int, int, int, int, int,
@@ -495,23 +497,68 @@ Tensor vocab_sample(const Tensor& h, const Tensor& Wb, bool w_kmajor, const Tens
   return logprob;
 }
 
-// The same from fp32 logits [B, C] (bias included).
-Tensor vocab_sample_logits(const Tensor& logits, double temperature, int64_t seed, Tensor step, const Tensor& row0, Tensor tokens,
-                           const std::optional<Tensor>& rec_tok, const std::optional<Tensor>& rec_lp, int64_t s0) {
+void chk_logits(const Tensor& logits) {
   chk_cuda(logits, "logits");
-  TORCH_CHECK(logits.dim() == 2 && logits.scalar_type() == torch::kFloat32 && logits.size(1) >= 1 &&
-              logits.numel() < (int64_t(1) << 40), "vocab sample: logits fp32 [B, C]");
+  TORCH_CHECK(logits.dim() == 2 && logits.scalar_type() == torch::kFloat32 && logits.is_contiguous() && logits.size(0) >= 1 &&
+              logits.size(1) >= 1 && logits.size(1) < (int64_t(1) << 31) && logits.numel() < (int64_t(1) << 40),
+              "vocab sample: logits fp32 [B, C], packed");
+}
+
+// The same from fp32 logits [B, C] (bias included).  tau fp32 [B] (top-k / top-p, temperature > 0): only the classes with
+// l >= tau[b] are candidates.
+Tensor vocab_sample_logits(const Tensor& logits, double temperature, int64_t seed, Tensor step, const Tensor& row0, Tensor tokens,
+                           const std::optional<Tensor>& rec_tok, const std::optional<Tensor>& rec_lp, int64_t s0,
+                           const std::optional<Tensor>& tau) {
+  chk_logits(logits);
   c10::cuda::CUDAGuard g(logits.device());
   const int B = logits.size(0), C = logits.size(1);
   const SampleOut o = sample_check(B, logits, step, row0, tokens, rec_tok, rec_lp, temperature);
+  if (tau.has_value()) {
+    chk_cuda(*tau, "tau");
+    TORCH_CHECK(tau->scalar_type() == torch::kFloat32 && tau->numel() == B && tau->is_contiguous() && tau->device() == logits.device(),
+                "vocab sample: tau fp32 [B]");
+    TORCH_CHECK(temperature > 0, "vocab sample: a threshold needs temperature > 0 (greedy keeps the arg-max, which no filter drops)");
+  }
   const int nt = ts_vocab_head_parts(C);
   auto fo = torch::TensorOptions().device(logits.device()).dtype(torch::kFloat32);
   auto part = torch::empty({(int64_t)B * nt * 4}, fo), logprob = torch::empty({B}, fo);
   auto part_arg = torch::empty({(int64_t)B * nt}, fo.dtype(torch::kInt32)), ticket = torch::zeros({1}, fo.dtype(torch::kInt32));
-  check(ts_vocab_sample_logits(logits.data_ptr<float>(), (float)temperature, (unsigned int)(seed & 0xffffffff), step.data_ptr<int>(),
+  check(ts_vocab_sample_logits(logits.data_ptr<float>(), tau.has_value() ? tau->data_ptr<float>() : nullptr, (float)temperature,
+                               (unsigned int)(seed & 0xffffffff), step.data_ptr<int>(),
                                row0.data_ptr<int>(), part.data_ptr(), part_arg.data_ptr<int>(), (unsigned int*)ticket.data_ptr<int>(), tokens.data_ptr<int>(),
                                logprob.data_ptr<float>(), o.rec_tok, o.rec_lp, o.N, (int)s0, B, C, stream()), "vocab_sample_logits");
   return logprob;
+}
+
+// logits fp32 [B, C] = h W + bias from the sampling kernel's main loop: the values vocab_sample scores, stored (top-k / top-p).
+Tensor vocab_head_logits(const Tensor& h, const Tensor& Wb, bool w_kmajor, const Tensor& bias) {
+  chk_cuda(h, "h"); chk_cuda(Wb, "Wb"); chk_cuda(bias, "bias");
+  const int64_t Cw = vocab_classes(h, Wb, w_kmajor, "vocab logits");
+  TORCH_CHECK(h.is_contiguous() && h.size(0) >= 1 && h.size(0) < (int64_t(1) << 24), "vocab logits: h bf16 [B,H] packed, 1 <= B < 2^24");
+  TORCH_CHECK(h.size(1) % 64 == 0 && Cw % 8 == 0 && Cw >= 8, "vocab logits: H % 64 == 0 and C % 8 == 0");
+  TORCH_CHECK(bias.scalar_type() == torch::kFloat32 && bias.numel() == Cw && ((uintptr_t)bias.data_ptr() % 8) == 0,
+              "vocab logits: bias fp32 [C]");
+  c10::cuda::CUDAGuard g(h.device());
+  const int B = h.size(0), H = h.size(1), C = (int)Cw;
+  auto logits = torch::empty({B, C}, torch::TensorOptions().device(h.device()).dtype(torch::kFloat32));
+  check(ts_vocab_head_logits(h.data_ptr(), Wb.data_ptr(), w_kmajor ? 1 : 0, bias.data_ptr<float>(), logits.data_ptr<float>(), B, H, C,
+                             h.get_device(), stream()), "vocab_head_logits");
+  return logits;
+}
+
+// tau fp32 [B]: the top-k / top-p threshold of each row of logits fp32 [B, C] (csrc/head_vocab.cu, vocab_threshold_kernel);
+// top_k 0 and top_p 1 are off.  No host sync: the filters are kernel arguments.
+Tensor vocab_threshold(const Tensor& logits, int64_t top_k, double top_p, double temperature) {
+  chk_logits(logits);
+  TORCH_CHECK(top_k >= 0, "vocab threshold: top_k must be >= 0 (0 = off), got ", top_k);
+  TORCH_CHECK(std::isfinite(top_p) && top_p > 0 && top_p <= 1, "vocab threshold: top_p must be in (0, 1] (1 = off), got ", top_p);
+  TORCH_CHECK(std::isfinite(temperature) && temperature > 0, "vocab threshold: temperature must be finite and > 0, got ", temperature);
+  c10::cuda::CUDAGuard g(logits.device());
+  const int B = logits.size(0), C = logits.size(1);
+  auto tau = torch::empty({B}, torch::TensorOptions().device(logits.device()).dtype(torch::kFloat32));
+  check(ts_vocab_threshold(logits.data_ptr<float>(), B, C, (int)std::min<int64_t>(top_k, C), top_p, (float)temperature,
+                           tau.data_ptr<float>(), stream()), "vocab_threshold");
+  return tau;
 }
 
 // ---- pooling over time (csrc/seq_pool.cu) ---------------------------------------------------------------------
@@ -969,7 +1016,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("vocab_sample", &vocab_sample, py::arg("h"), py::arg("Wb"), py::arg("w_kmajor"), py::arg("bias"), py::arg("temperature"), py::arg("seed"),
         py::arg("step"), py::arg("row0"), py::arg("tokens"), py::arg("rec_tok"), py::arg("rec_lp"), py::arg("s0"));
   m.def("vocab_sample_logits", &vocab_sample_logits, py::arg("logits"), py::arg("temperature"), py::arg("seed"), py::arg("step"),
-        py::arg("row0"), py::arg("tokens"), py::arg("rec_tok"), py::arg("rec_lp"), py::arg("s0"));
+        py::arg("row0"), py::arg("tokens"), py::arg("rec_tok"), py::arg("rec_lp"), py::arg("s0"), py::arg("tau") = py::none());
+  m.def("vocab_head_logits", &vocab_head_logits, py::arg("h"), py::arg("Wb"), py::arg("w_kmajor"), py::arg("bias"));
+  m.def("vocab_threshold", &vocab_threshold, py::arg("logits"), py::arg("top_k"), py::arg("top_p"), py::arg("temperature"));
   m.def("head_bwd", &head_bwd, py::arg("h"), py::arg("W"), py::arg("dlogits"), py::arg("dloss"), py::arg("dW"), py::arg("db"),
         py::arg("accumulate") = false);
   m.def("flat_adam", &flat_adam, py::arg("p"), py::arg("g"), py::arg("m"), py::arg("v"), py::arg("shadow"), py::arg("lr_t"),

@@ -19,6 +19,9 @@
 //     class and the logit there; vocab_sample_combine_kernel merges the tiles of a row in a fixed order into the sampled token
 //     and its log-probability.  vocab_sample_logits_kernel makes the same partials from stored fp32 logits (the inputs this
 //     GEMM does not take).
+//   * Top-k / top-p sampling needs the whole row, so it stores it: vocab_head_gemm_kernel<kLogits> (the same main loop; the
+//     epilogue writes acc + bias as fp32 logits [B, C]), vocab_threshold_kernel (the row's threshold tau, a radix select),
+//     vocab_sample_logits_kernel<true> (the partials over the classes with l >= tau) and the same combine.
 //
 // Tiles are walked in bands of 16 cluster tiles (4096 rows): inside a band the class tile is the outer index, so the band's rows
 // of h stay in L2 and W streams from HBM once per band.  Row r = t·B + b counts iff t < lengths[b]; lengths may be 0.
@@ -48,14 +51,21 @@ constexpr int kStageBytes = kABytes + kBBytes;
 constexpr int kStages = 4;
 constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align*/ + 1024 /*barriers*/;
 
-enum Mode { kFwd = 0, kDlogits = 1, kSample = 2 };
+enum Mode { kFwd = 0, kDlogits = 1, kSample = 2, kLogits = 3 };
 
 struct VocabParams {
   const float* bias;           // [C]
   const long long* labels;     // [B, T]
   const int* lengths;          // [B] or null
-  float4* part;                // kFwd: [R, tiles_n] {max, sum exp, arg-max (int bits), label logit or 0}
-  const float* lse;            // kDlogits: [R]
+  // The unions overlay pointers no mode reads together, so the layout (and the code of every other mode) stays as it was.
+  union {
+    float4* part;              // kFwd: [R, tiles_n] {max, sum exp, arg-max (int bits), label logit or 0}
+    float* logits;             // kLogits: [B, C] fp32, acc + bias
+  };
+  union {
+    const float* lse;          // kDlogits: [R]
+    const float* tau;          // vocab_sample_logits_kernel<true>: [B] the kept set's threshold, l >= tau
+  };
   const float* dloss;          // kDlogits: [1]
   const int* count;            // kDlogits: [1] N
   __nv_bfloat16* dl;           // kDlogits: [rows, C]
@@ -82,6 +92,21 @@ struct VocabParams {
 // Rounding: l is fp32 (bf16 h x bf16 W accumulated in fp32, plus the fp32 bias, or the fp32 logits of the fallback); the score
 // is fmaf(l, 1/t, g) in fp32.  u has 25 significant bits at u >= 1/2, where fp32 would round 1 - 2^-25 to 1 and -log u to 0:
 // below 1/2 u is exact in fp32 and -log u = -log(u); above it 1 - u is exact and -log u = -log1p(-(1 - u)) > 0.
+//
+// Top-k / top-p (nucleus) filtering, shared with ops/reference.py (sample_threshold / sample_logits): at temperature t > 0 the
+// token is argmax over c in K of (l_c / t + g_c), with the same noise g, an exact draw from softmax(l / t) restricted to K and
+// renormalised.  K = {c : l_c >= tau}:
+//   top-k (0 < k < C): tau_k = the k-th largest logit counted with multiplicity; every class tied at it is kept.
+//   top-p (0 < p < 1): q = softmax(l / t) over {l >= tau_k} (all classes without top-k); tau = the largest logit value v with
+//     q-mass of {l >= v} at least p (ties at v are kept).  Both: top-k first, then top-p on what is left.
+//   Off (k = 0 or k >= C, p = 1) or t = 0: no filter, the kernels above.  log p(token) stays under the full softmax(l).
+// Coupling: the filtered path's logits are the same fp32 values kSample scores (acc + bias from the same main loop, or the same
+// GEMM's logits on the fallback) and its scores are the same sample_score, so the filtered token equals the unfiltered one
+// whenever that token is in K.
+// Rounding of the threshold: ties and the k-th value are decided on the fp32 logits exactly.  Top-p masses are
+// exp((l - max) / t) in fp32 (__expf((l - max) * (1/t))), rounded to fixed point in units of 2^-32 of the row max's mass and
+// summed as u64 integers (so the sums do not depend on the order or the grid); the cut is the first value, from the top, where
+// the running sum reaches ceil(p · Z) (fp64 product, Z the total).  A class below 2^-33 of the max's mass counts as 0.
 constexpr uint32_t kSampleKey1 = 0x53414D50u;      // "SAMP"
 
 TC_DEVICE uint4 sample_words(uint32_t seed, uint32_t row, uint32_t s, int c) {
@@ -242,14 +267,14 @@ vocab_head_gemm_kernel(const __grid_constant__ CUtensorMap tmap_h, const __grid_
       for (int h = 0; h < 2; ++h) {
         const int row = m0 + 64 * wg + 16 * wq + (lane >> 2) + 8 * h;
         valid[h] = row < p.row0 + p.rows;
-        if (kMode != kSample) {
+        if (kMode == kFwd || kMode == kDlogits) {
           const int t = row / p.B, b = row - t * p.B;
           const bool counted = valid[h] && (p.lengths == nullptr || t < p.lengths[b]);
           y[h] = counted ? (int)p.labels[(size_t)b * p.T + t] : -1;      // -1: an uncounted row
         }
       }
       const int row_lo = m0 + 64 * wg + 16 * wq + (lane >> 2);
-      if (kMode == kFwd || kMode == kSample) {
+      if (kMode == kFwd || kMode == kSample || kMode == kLogits) {
         // l = acc + bias; classes beyond C (C % 8 == 0: whole 8-column groups) become -inf, so the passes below skip them
 #pragma unroll
         for (int j = 0; j < BN / 8; ++j) {
@@ -261,7 +286,19 @@ vocab_head_gemm_kernel(const __grid_constant__ CUtensorMap tmap_h, const __grid_
             acc[4 * j] = acc[4 * j + 1] = acc[4 * j + 2] = acc[4 * j + 3] = -INFINITY;
           }
         }
-        if (kMode == kSample) {
+        if (kMode == kLogits) {
+          // the fp32 values kSample scores, stored (T = 1: row = batch row; rows past B are not written)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            if (!valid[h]) continue;
+            float* lrow = p.logits + (size_t)(row_lo + 8 * h) * p.C;
+#pragma unroll
+            for (int j = 0; j < BN / 8; ++j) {
+              const int col = cq + 8 * j;
+              if (col < p.C) *reinterpret_cast<float2*>(lrow + col) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+            }
+          }
+        } else if (kMode == kSample) {
           const bool greedy = p.inv_tau < 0.f;
           const uint32_t s = greedy ? 0u : (uint32_t)*p.step;
           const uint32_t r0 = greedy ? 0u : (uint32_t)*p.row_base;
@@ -490,6 +527,9 @@ constexpr int kSampleWarps = 8;
 
 // One warp per (row, class tile of BN): the partials of vocab_head_gemm_kernel<kSample> from fp32 logits [B, C] (bias included).
 // Lane i takes the four classes 4 i + 128 k + [0, 4) of the tile, k = 0, 1: one Philox call each.
+// kFilter (temperature > 0): only the classes with l >= tau[b] are scored, the others score -inf; a group of four classes with
+// none kept draws no noise.  Max and sum exp still run over every class (the log-probability is under the full softmax).
+template <bool kFilter>
 __global__ void __launch_bounds__(kSampleWarps * 32)
 vocab_sample_logits_kernel(const float* __restrict__ logits, VocabParams p) {
   const int lane = threadIdx.x & 31;
@@ -501,17 +541,37 @@ vocab_sample_logits_kernel(const float* __restrict__ logits, VocabParams p) {
   const uint32_t s = greedy ? 0u : (uint32_t)*p.step;
   const uint32_t r0 = greedy ? 0u : (uint32_t)*p.row_base;
   float l[8], sc[8];
+  if (kFilter) {
+    const float tau = p.tau[b];
 #pragma unroll
-  for (int k = 0; k < 2; ++k) {
-    const int c0 = tn * BN + 128 * k + 4 * lane;
-    uint4 w = make_uint4(0u, 0u, 0u, 0u);
-    if (!greedy && c0 < p.C) w = sample_words(p.seed, r0 + (uint32_t)b, s, c0);
-    const uint32_t ws[4] = {w.x, w.y, w.z, w.w};
+    for (int k = 0; k < 2; ++k) {
+      const int c0 = tn * BN + 128 * k + 4 * lane;
+      bool any = false;
 #pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const int c = c0 + i;
-      l[4 * k + i] = c < p.C ? logits[(size_t)b * p.C + c] : -INFINITY;
-      sc[4 * k + i] = (greedy || c >= p.C) ? l[4 * k + i] : sample_score(l[4 * k + i], p.inv_tau, ws[i]);
+      for (int i = 0; i < 4; ++i) {
+        l[4 * k + i] = c0 + i < p.C ? logits[(size_t)b * p.C + c0 + i] : -INFINITY;
+        any |= l[4 * k + i] >= tau;
+      }
+      uint4 w = make_uint4(0u, 0u, 0u, 0u);
+      if (any) w = sample_words(p.seed, r0 + (uint32_t)b, s, c0);
+      const uint32_t ws[4] = {w.x, w.y, w.z, w.w};
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+        sc[4 * k + i] = (c0 + i < p.C && l[4 * k + i] >= tau) ? sample_score(l[4 * k + i], p.inv_tau, ws[i]) : -INFINITY;
+    }
+  } else {
+#pragma unroll
+    for (int k = 0; k < 2; ++k) {
+      const int c0 = tn * BN + 128 * k + 4 * lane;
+      uint4 w = make_uint4(0u, 0u, 0u, 0u);
+      if (!greedy && c0 < p.C) w = sample_words(p.seed, r0 + (uint32_t)b, s, c0);
+      const uint32_t ws[4] = {w.x, w.y, w.z, w.w};
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const int c = c0 + i;
+        l[4 * k + i] = c < p.C ? logits[(size_t)b * p.C + c] : -INFINITY;
+        sc[4 * k + i] = (greedy || c >= p.C) ? l[4 * k + i] : sample_score(l[4 * k + i], p.inv_tau, ws[i]);
+      }
     }
   }
   float mx = -INFINITY, best = -INFINITY, lbest = 0.f;
@@ -536,6 +596,119 @@ vocab_sample_logits_kernel(const float* __restrict__ logits, VocabParams p) {
     p.part[(size_t)b * tiles_n + tn] = make_float4(mx, se, best, lbest);
     p.part_arg[(size_t)b * tiles_n + tn] = arg;
   }
+}
+
+// ---- the top-k / top-p threshold (definition above sample_words) --------------------------------------------------------------
+// One CTA per row.  A radix select over the order-preserving u32 image of the fp32 logits, in four 8-bit passes from the top
+// byte: each pass bins the candidates (the classes whose key agrees with the prefix fixed so far) by their next byte, per warp in
+// shared memory with u64 integer atomics, and one warp finds the bin where the running total from the top reaches the target.
+// Top-k counts classes (target k); top-p sums fixed-point masses (target ceil(p · Z), Z from the first pass) over the classes at
+// or above the top-k threshold.  Integer sums: the result does not depend on the order of the atomics, the grid or the SM count.
+constexpr int kSelThreads = 512;
+constexpr int kSelWarps = kSelThreads / 32;
+
+TC_DEVICE uint32_t order_key(float f) {                    // a < b <=> key(a) < key(b) for non-NaN a, b; -0 and +0 share one key
+  const uint32_t u = __float_as_uint(f == 0.f ? 0.f : f);
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+TC_DEVICE float key_value(uint32_t k) { return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k); }
+TC_DEVICE unsigned long long mass_fixed(float l, float mx, float inv_tau) {   // exp((l - max) / t) in units of 2^-32
+  return __float2ull_rn(__expf((l - mx) * inv_tau) * 0x1p32f);
+}
+
+struct SelectShared {
+  unsigned long long hist[kSelWarps][256];
+  unsigned long long bins[256];
+  unsigned long long above, target;
+  uint32_t bin, none;
+};
+
+// -> the largest key v such that the total over the candidates with key >= v (and key >= lo) reaches the target: the k-th
+// largest key (mass = false, target k) or the nucleus cut (mass = true, target ceil(p · Z)).  0 if the target is out of reach.
+TC_DEVICE uint32_t radix_select(const float* __restrict__ row, int C, uint32_t lo, bool mass, float mx, float inv_tau,
+                                unsigned long long k, double top_p, SelectShared& sh) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  uint32_t prefix = 0;
+  unsigned long long above = 0, target = k;
+  for (int shift = 24; shift >= 0; shift -= 8) {
+    for (int i = threadIdx.x; i < kSelWarps * 256; i += kSelThreads) (&sh.hist[0][0])[i] = 0ull;
+    __syncthreads();
+    const uint32_t hi = shift == 24 ? 0u : ~0u << (shift + 8);             // the bytes fixed by earlier passes
+    for (int c = threadIdx.x; c < C; c += kSelThreads) {
+      const float l = row[c];
+      const uint32_t key = order_key(l);
+      if (l == l && key >= lo && (key & hi) == prefix)
+        atomicAdd(&sh.hist[warp][(key >> shift) & 255u], mass ? mass_fixed(l, mx, inv_tau) : 1ull);
+    }
+    __syncthreads();
+    if (threadIdx.x < 256) {
+      unsigned long long v = 0;
+      for (int w = 0; w < kSelWarps; ++w) v += sh.hist[w][threadIdx.x];
+      sh.bins[threadIdx.x] = v;
+    }
+    __syncthreads();
+    if (warp == 0) {
+      unsigned long long v[8], own = 0;                                    // lane i owns bins 8 i .. 8 i + 7
+#pragma unroll
+      for (int i = 0; i < 8; ++i) { v[i] = sh.bins[8 * lane + i]; own += v[i]; }
+      unsigned long long suffix = own;                                     // the total of this lane's bins and every higher one
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const unsigned long long t = __shfl_down_sync(0xffffffffu, suffix, o);
+        if (lane + o < 32) suffix += t;
+      }
+      if (mass && shift == 24) {                                          // Z: the first pass sees every candidate
+        const double z = (double)__shfl_sync(0xffffffffu, suffix, 0);
+        target = (unsigned long long)ceil(top_p * z);
+        if (target < 1) target = 1;
+      }
+      const bool mine = above + (suffix - own) < target && target <= above + suffix;
+      const unsigned who = __ballot_sync(0xffffffffu, mine);
+      if (who == 0u) {                                                     // out of reach (NaNs among the k): no threshold
+        if (lane == 0) sh.none = 1;
+      } else if (mine) {
+        unsigned long long run = above + (suffix - own);
+        int bin = 8 * lane;
+        for (int i = 7; i >= 0; --i) {
+          if (run + v[i] >= target) { bin = 8 * lane + i; break; }
+          run += v[i];
+        }
+        sh.bin = (uint32_t)bin; sh.above = run; sh.none = 0;
+      }
+      if (lane == 0) sh.target = target;
+    }
+    __syncthreads();
+    if (sh.none) return 0u;
+    prefix |= sh.bin << shift;
+    above = sh.above;
+    target = sh.target;
+  }
+  return prefix;
+}
+
+// tau [B]: the kept set of row b is {c : l_c >= tau[b]} (-inf: every class).  top_k 0 or >= C and top_p >= 1 are off.
+__global__ void __launch_bounds__(kSelThreads)
+vocab_threshold_kernel(const float* __restrict__ logits, int C, int top_k, double top_p, float inv_tau, float* __restrict__ tau) {
+  __shared__ SelectShared sh;
+  __shared__ uint32_t red[kSelWarps];
+  const float* row = logits + (size_t)blockIdx.x * C;
+  uint32_t lo = 0;
+  if (top_k > 0 && top_k < C) lo = radix_select(row, C, 0u, false, 0.f, 0.f, (unsigned long long)top_k, 1.0, sh);
+  if (top_p < 1.0) {
+    uint32_t m = 0;                                                       // the row's largest (non-NaN) key
+    for (int c = threadIdx.x; c < C; c += kSelThreads) {
+      const float l = row[c];
+      if (l == l) m = max(m, order_key(l));
+    }
+    m = __reduce_max_sync(0xffffffffu, m);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = m;
+    __syncthreads();
+    m = 0;
+    for (int w = 0; w < kSelWarps; ++w) m = max(m, red[w]);
+    const float mx = key_value(m);
+    if (isfinite(mx)) lo = radix_select(row, C, lo, true, mx, inv_tau, 0ull, top_p, sh);
+  }
+  if (threadIdx.x == 0) tau[blockIdx.x] = lo <= order_key(-INFINITY) ? -INFINITY : key_value(lo);
 }
 
 struct SampleCombineParams {
@@ -704,14 +877,34 @@ extern "C" int ts_vocab_sample(const void* h, const void* Wb, int w_kmajor, cons
   return launch_sample_combine(p, ticket, tokens, logprob, rec_tok, rec_lp, N, s0, st);
 }
 
-// The same from stored fp32 logits [B, C] (bias included): the inputs vocab_head_gemm_kernel does not take.
-extern "C" int ts_vocab_sample_logits(const float* logits, float temperature, unsigned int seed, int* step, const int* row_base,
-                                      void* part, int* part_arg,
+// The same from stored fp32 logits [B, C] (bias included): the inputs vocab_head_gemm_kernel does not take, and top-k / top-p.
+// tau [B] or null: with tau (temperature > 0) only the classes with l >= tau[b] are candidates.
+extern "C" int ts_vocab_sample_logits(const float* logits, const float* tau, float temperature, unsigned int seed, int* step,
+                                      const int* row_base, void* part, int* part_arg,
                                       unsigned int* ticket, int* tokens, float* logprob, int* rec_tok, float* rec_lp, int N, int s0,
                                       int B, int C, cudaStream_t st) {
-  const VocabParams p = sample_params(nullptr, part, part_arg, step, row_base, seed, temperature, B, 0, C);
+  VocabParams p = sample_params(nullptr, part, part_arg, step, row_base, seed, temperature, B, 0, C);
+  p.tau = tau;
   const int warps = B * ts_vocab_head_parts(C);
-  vocab_sample_logits_kernel<<<(warps + kSampleWarps - 1) / kSampleWarps, kSampleWarps * 32, 0, st>>>(logits, p);
+  const dim3 grid((warps + kSampleWarps - 1) / kSampleWarps);
+  if (tau != nullptr) vocab_sample_logits_kernel<true><<<grid, kSampleWarps * 32, 0, st>>>(logits, p);
+  else vocab_sample_logits_kernel<false><<<grid, kSampleWarps * 32, 0, st>>>(logits, p);
   if (cudaError_t e = cudaGetLastError()) return (int)e;
   return launch_sample_combine(p, ticket, tokens, logprob, rec_tok, rec_lp, N, s0, st);
+}
+
+// logits fp32 [B, C] = h [B, H] · W + bias through the sampling kernel's main loop (vocab_head_gemm_kernel<kLogits>): the same
+// fp32 values ts_vocab_sample scores.  Same operand conditions as ts_vocab_sample.
+extern "C" int ts_vocab_head_logits(const void* h, const void* Wb, int w_kmajor, const float* bias, float* logits, int B, int H, int C,
+                                    int dev, cudaStream_t st) {
+  VocabParams p = sample_params(bias, nullptr, nullptr, nullptr, nullptr, 0u, 0.f, B, H, C);
+  p.logits = logits;
+  return launch_gemm<kLogits>(h, Wb, w_kmajor, p, dev, st);
+}
+
+// tau [B] of the top-k / top-p filter (definition above sample_words) from fp32 logits [B, C] at temperature > 0.
+extern "C" int ts_vocab_threshold(const float* logits, int B, int C, int top_k, double top_p, float temperature, float* tau,
+                                  cudaStream_t st) {
+  vocab_threshold_kernel<<<B, kSelThreads, 0, st>>>(logits, C, top_k, top_p, 1.0f / temperature, tau);
+  return (int)cudaGetLastError();
 }

@@ -263,19 +263,21 @@ class SequenceClassifier(nn.Module):
     # ---- text generation -----------------------------------------------------------
     @torch.no_grad()
     def generate(self, prompt: torch.Tensor, lengths: Optional[torch.Tensor], max_new_tokens: int, temperature: float = 1.0,
-                 seed: int = 0, graph: Optional[bool] = None, row0: int = 0):
+                 seed: int = 0, graph: Optional[bool] = None, row0: int = 0, top_k: int = 0, top_p: float = 1.0):
         """Continue each prompt (``--next_token`` models): ``prompt`` int ``[B,T]`` right-padded token ids, ``lengths`` int32 ``[B]``
         (None: every row is T long) -> (tokens int32 ``[B,N]``, log p(token) fp32 ``[B,N]`` under the model's softmax),
         ``N = max_new_tokens``, sampled at ``temperature`` with the noise of ``seed`` (``ops.functional.vocab_sample``; step s
         draws token s).  ``row0``: the index of row 0 among all the prompts when they run in batches; row b draws the noise of
-        prompt ``row0 + b``, so no two prompts of one generation share it.
+        prompt ``row0 + b``, so no two prompts of one generation share it.  ``top_k`` / ``top_p``: draw from the top-k classes
+        and then from the nucleus of q-mass ``top_p`` only (0 and 1: off; no effect at temperature 0); the log-probabilities stay
+        under the full softmax.
 
         The prompt runs through the whole-sequence path; token 0 is sampled from the top layer's state after each row's own last
         prompt token.  Every later token embeds the previous one and takes one step of each layer from the carried state (the
         one-step path ``RNN.fit_layers`` in eval mode), then samples.  The state lives in static buffers; on the GPU the decode
         step is captured once per batch shape as a CUDA graph (``graph=False``: eager) and replayed; ``row0`` and the step counter
-        live on the device, so one graph serves every batch, and another temperature or seed replaces it (one graph per shape is
-        kept).  The graph runs the eager loop's kernels; with the deterministic recurrences (``--deterministic``) both give the
+        live on the device, so one graph serves every batch, and another temperature, seed or filter replaces it (one graph per
+        shape is kept).  The graph runs the eager loop's kernels; with the deterministic recurrences (``--deterministic``) both give the
         same bits.  Nothing waits for the device until the caller reads the result."""
         if not getattr(self.cfg, "next_token", False):
             raise ValueError("generate needs a language model trained with --next_token (this one predicts given labels)")
@@ -284,6 +286,8 @@ class SequenceClassifier(nn.Module):
             raise ValueError(f"max_new_tokens must be >= 1, got {max_new_tokens}")
         if prompt.dim() != 2:
             raise ValueError(f"generate needs prompts [B,T] of token ids, got {tuple(prompt.shape)}")
+        from ..ops import reference as ref
+        ref.check_sample_filters(top_k, top_p)
         B, dev = prompt.shape[0], prompt.device
         use_graph = dev.type == "cuda" if graph is None else bool(graph)
         was_training = self.training
@@ -291,9 +295,9 @@ class SequenceClassifier(nn.Module):
         try:
             self.sequence_features(prompt, lengths)
             key = (B, N, str(dev), use_graph)
-            noise = (float(temperature), int(seed) & 0xFFFFFFFF)
+            noise = (float(temperature), int(seed) & 0xFFFFFFFF, int(top_k), float(top_p))
             dec = self._decoders.get(key)
-            if dec is None or (dec.temperature, dec.seed) != noise:
+            if dec is None or (dec.temperature, dec.seed, dec.top_k, dec.top_p) != noise:
                 dec = self._decoders[key] = _Decoder(self, B, N, *noise, dev)
             for layer, (h, c) in zip(self.rnn.layers, dec.state):
                 h.copy_(layer.ht)
@@ -416,8 +420,8 @@ class _Decoder:
     """The static buffers of ``SequenceClassifier.generate`` at one batch shape: the carried state of every layer, the previous
     token, the device-resident step counter and row offset and the ``[B,N]`` results, and once captured the CUDA graph of one decode step."""
 
-    def __init__(self, model: SequenceClassifier, B: int, N: int, temperature: float, seed: int, device):
-        self.model, self.temperature, self.seed = model, temperature, seed
+    def __init__(self, model: SequenceClassifier, B: int, N: int, temperature: float, seed: int, top_k: int, top_p: float, device):
+        self.model, self.temperature, self.seed, self.top_k, self.top_p = model, temperature, seed, top_k, top_p
         self.state = [(layer.ht.detach().clone(), layer.Ct.detach().clone()) for layer in model.rnn.layers]
         self.tokens = torch.zeros(B, dtype=torch.int32, device=device)
         self.step = torch.zeros(1, dtype=torch.int32, device=device)
@@ -429,7 +433,8 @@ class _Decoder:
     def sample(self, h: torch.Tensor) -> None:
         w, class_major = self.model.head_weights()
         F.vocab_sample(h, w, self.model.head.bias, self.temperature, self.seed, self.step, tokens=self.tokens,
-                       record=(self.tokens_out, self.logprob_out, 0), row0=self.row0, class_major=class_major)
+                       record=(self.tokens_out, self.logprob_out, 0), row0=self.row0, class_major=class_major, top_k=self.top_k,
+                       top_p=self.top_p)
 
     def run(self) -> None:
         """One decode step: embed the previous token, one step of every layer from the buffers (which get the new state), sample."""

@@ -117,26 +117,37 @@ def _sample_args(step, row0, tokens, record, B, device):
     return _device_int(step, device), _device_int(row0, device), tok, rec_tok, rec_lp, s0
 
 
-def vocab_sample(h, weights, bias, temperature: float, seed: int, step, tokens=None, record=None, row0=0, class_major=False):
+def vocab_sample(h, weights, bias, temperature: float, seed: int, step, tokens=None, record=None, row0=0, class_major=False,
+                 top_k: int = 0, top_p: float = 1.0):
     """Sample the next token from ``h [B,H]`` bf16 through the head's tensor-core kernel (``kSample``), without storing the
-    logits; see ``ops.functional.vocab_sample``."""
+    logits; see ``ops.functional.vocab_sample``.  With a filter on (the caller passes ``top_k = 0`` and ``top_p = 1`` when it is
+    off) the same main loop stores the fp32 logits (``kLogits``) and ``vocab_sample_logits`` samples them."""
     from .cuda_lstm import STATS
-    B = h.shape[0]
-    step_t, row_t, tok, rec_tok, rec_lp, s0 = _sample_args(step, row0, tokens, record, B, h.device)
     wb = _weights_lowp(weights, class_major)
-    lp = ext().vocab_sample(h.detach().contiguous(), wb, bool(class_major), bias.detach().float().contiguous(), float(temperature), int(seed), step_t,
-                            row_t, tok, rec_tok, rec_lp, int(s0))
-    STATS["vocab_sample"] = STATS.get("vocab_sample", 0) + 1
+    hc, bc = h.detach().contiguous(), bias.detach().float().contiguous()
     if class_major:
         STATS["vocab_sample_tied"] = STATS.get("vocab_sample_tied", 0) + 1
+    if top_k > 0 or top_p < 1:
+        logits = ext().vocab_head_logits(hc, wb, bool(class_major), bc)
+        return vocab_sample_logits(logits, temperature, seed, step, tokens, record, row0, top_k, top_p)
+    step_t, row_t, tok, rec_tok, rec_lp, s0 = _sample_args(step, row0, tokens, record, h.shape[0], h.device)
+    lp = ext().vocab_sample(hc, wb, bool(class_major), bc, float(temperature), int(seed), step_t, row_t, tok, rec_tok, rec_lp, int(s0))
+    STATS["vocab_sample"] = STATS.get("vocab_sample", 0) + 1
     return tok, lp
 
 
-def vocab_sample_logits(logits, temperature: float, seed: int, step, tokens=None, record=None, row0=0):
-    """The same sampling from stored fp32 logits ``[B,C]`` (bias included): the inputs the tensor-core kernel does not take."""
+def vocab_sample_logits(logits, temperature: float, seed: int, step, tokens=None, record=None, row0=0, top_k: int = 0,
+                        top_p: float = 1.0):
+    """The same sampling from stored fp32 logits ``[B,C]`` (bias included): the inputs the tensor-core kernel does not take, and
+    top-k / top-p (on: ``top_k > 0`` or ``top_p < 1``, at temperature > 0), where ``vocab_threshold`` computes each row's
+    threshold first and the sampling kernel scores only the classes at or above it."""
     from .cuda_lstm import STATS
     step_t, row_t, tok, rec_tok, rec_lp, s0 = _sample_args(step, row0, tokens, record, logits.shape[0], logits.device)
-    lp = ext().vocab_sample_logits(logits.float().contiguous(), float(temperature), int(seed), step_t, row_t, tok, rec_tok, rec_lp,
-                                   int(s0))
+    lg = logits.float().contiguous()
+    tau = None
+    if top_k > 0 or top_p < 1:
+        tau = ext().vocab_threshold(lg, int(top_k), float(top_p), float(temperature))
+        STATS["vocab_sample_filtered"] = STATS.get("vocab_sample_filtered", 0) + 1
+    lp = ext().vocab_sample_logits(lg, float(temperature), int(seed), step_t, row_t, tok, rec_tok, rec_lp, int(s0), tau)
     STATS["vocab_sample"] = STATS.get("vocab_sample", 0) + 1
     return tok, lp

@@ -106,7 +106,8 @@ def vocab_xent_per_step(h_seq, weights, bias, labels, lengths=None, class_major:
     return ref.vocab_xent_per_step(h_seq, w, bias, labels, lengths)
 
 
-def vocab_sample(h, weights, bias, temperature: float, seed: int, step, tokens=None, record=None, row0=0, class_major: bool = False):
+def vocab_sample(h, weights, bias, temperature: float, seed: int, step, tokens=None, record=None, row0=0, class_major: bool = False,
+                 top_k: int = 0, top_p: float = 1.0):
     """Sample the next token of every row from the head's logits ``l = h W + bias`` (``h [B,H]``, ``W [H,C]``) without a host
     round trip -> (tokens int32 ``[B]``, log p(token) under ``softmax(l)`` fp32 ``[B]``).  Temperature 0 is the arg-max; above 0
     Gumbel-max with counter-based noise (``reference.sample_logits`` holds the definition).  ``step``: the decode step, an int
@@ -116,20 +117,34 @@ def vocab_sample(h, weights, bias, temperature: float, seed: int, step, tokens=N
     row 0, the index of the batch's first prompt when prompts run in batches, so every prompt draws its own noise.  On the GPU bf16 ``h`` with ``H % 64 == 0``, ``C % 8 == 0`` and ``C >= 512`` runs in
     the head's tensor-core kernel (csrc/head_vocab.cu); every other input computes the fp32 logits with the head GEMM and
     samples them with one more kernel.  Two calls on the same inputs give the same bits.  ``class_major``: ``weights`` is
-    ``[C,H]`` (a tied embedding table, ``W^T``), read in place."""
+    ``[C,H]`` (a tied embedding table, ``W^T``), read in place.
+
+    ``top_k`` (int >= 0, 0 = off) and ``top_p`` (in (0, 1], 1 = off): at temperature > 0 the draw is restricted to the row's
+    top-k classes, then to its nucleus of q-mass ``top_p`` (``reference.sample_threshold`` holds the definition), with the same
+    noise: the token is the unfiltered one whenever that one is kept.  The log-probability stays under the full ``softmax(l)``.
+    On the GPU a filter stores the row's fp32 logits (the tensor-core kernel's own values, or the fallback's), computes each
+    row's threshold on the device and samples the classes at or above it; with the filters off or at temperature 0 the
+    unfiltered kernels run."""
     temperature = float(temperature)
     if not (math.isfinite(temperature) and temperature >= 0):
         raise ValueError(f"temperature must be finite and >= 0, got {temperature}")
-    if vocab_head_supported(h.unsqueeze(0), weights.shape[0 if class_major else 1]):
+    ref.check_sample_filters(top_k, top_p)
+    top_k, top_p = int(top_k), float(top_p)
+    C = weights.shape[0 if class_major else 1]
+    if not ref.sample_filters_active(C, temperature, top_k, top_p):
+        top_k, top_p = 0, 1.0
+    if vocab_head_supported(h.unsqueeze(0), C):
         from . import cuda_vocab_head
-        return cuda_vocab_head.vocab_sample(h, weights, bias, temperature, seed, step, tokens, record, row0, class_major)
+        return cuda_vocab_head.vocab_sample(h, weights, bias, temperature, seed, step, tokens, record, row0, class_major,
+                                            top_k, top_p)
     if _use_ext(h):
         from . import cuda_gemm, cuda_vocab_head
         w_t = weights.detach() if class_major else weights.detach().t()          # the GEMM's b_t operand: [C,H]
         logits = cuda_gemm.matmul(h.reshape(h.shape[0], -1), w_t, bias=bias.detach().float(), out_dtype=torch.float32)
-        return cuda_vocab_head.vocab_sample_logits(logits, temperature, seed, step, tokens, record, row0)
+        return cuda_vocab_head.vocab_sample_logits(logits, temperature, seed, step, tokens, record, row0, top_k, top_p)
     s = int(step)
-    tok, logp = ref.vocab_sample(h, weights, bias, temperature, seed, s, int(row0), class_major=class_major)
+    tok, logp = ref.vocab_sample(h, weights, bias, temperature, seed, s, int(row0), class_major=class_major, top_k=top_k,
+                                 top_p=top_p)
     logp = logp.float()
     if isinstance(step, torch.Tensor):
         step.add_(1)

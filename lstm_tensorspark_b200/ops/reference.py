@@ -282,26 +282,76 @@ def sample_scores(logits: torch.Tensor, temperature: float, seed: int, step: int
     return l / temperature - torch.log(-torch.log(u))
 
 
-def sample_logits(logits: torch.Tensor, temperature: float, seed: int, step: int, row0: int = 0):
+def check_sample_filters(top_k, top_p) -> None:
+    """Raise unless ``top_k`` is an int >= 0 (0 = off) and ``top_p`` a finite number in (0, 1] (1 = off)."""
+    if isinstance(top_k, bool) or int(top_k) != top_k or top_k < 0:
+        raise ValueError(f"top_k must be an integer >= 0 (0 = off), got {top_k}")
+    if not (math.isfinite(top_p) and 0 < top_p <= 1):
+        raise ValueError(f"top_p must be a finite number in (0, 1] (1 = off), got {top_p}")
+
+
+def sample_filters_active(num_classes: int, temperature: float, top_k: int = 0, top_p: float = 1.0) -> bool:
+    """Does a filter change the draw: temperature > 0 and ``0 < top_k < C`` or ``top_p < 1``?  (Greedy always keeps the arg-max.)"""
+    return temperature > 0 and (0 < top_k < num_classes or top_p < 1)
+
+
+def sample_threshold(logits: torch.Tensor, temperature: float, top_k: int = 0, top_p: float = 1.0) -> torch.Tensor:
+    """The kept set's threshold ``tau [B]`` (fp64) of top-k / top-p sampling: row b keeps ``{c : l_c >= tau_b}`` (-inf: every
+    class).  In fp64, with the definition of csrc/head_vocab.cu:
+
+    * top-k (``0 < k < C``): ``tau_k`` = the k-th largest logit counted with multiplicity (every class tied at it is kept);
+    * top-p (``0 < p < 1``): ``q = softmax(l / t)`` over ``{l >= tau_k}`` (every class without top-k); ``tau`` = the largest
+      logit value v whose set ``{l >= v}`` holds q-mass >= p (ties at v are kept).  Top-k first, then top-p: the order of
+      Hugging Face's samplers.
+    Temperature 0 or both filters off: -inf."""
+    check_sample_filters(top_k, top_p)
+    l = logits.double()
+    B, C = l.shape
+    tau = torch.full((B,), float("-inf"), dtype=torch.float64, device=l.device)
+    if not sample_filters_active(C, temperature, top_k, top_p):
+        return tau
+    if 0 < top_k < C:
+        tau = l.topk(int(top_k), 1).values[:, -1]
+    if top_p < 1:
+        keep = l >= tau.unsqueeze(1)
+        mx = l.max(1, keepdim=True).values
+        e = torch.where(keep, torch.exp((l - mx) / temperature), torch.zeros((), dtype=torch.float64, device=l.device))
+        vals, order = l.sort(1, descending=True)
+        cum = e.gather(1, order).cumsum(1)
+        first = (cum >= top_p * e.sum(1, keepdim=True)).int().argmax(1)      # the first position from the top where it holds
+        tau = vals.gather(1, first.view(-1, 1)).squeeze(1)
+    return tau
+
+
+def sample_logits(logits: torch.Tensor, temperature: float, seed: int, step: int, row0: int = 0, top_k: int = 0,
+                  top_p: float = 1.0):
     """Sample one token per row of ``logits [B, C]`` -> (tokens int32 [B], log p(token) under softmax(logits), fp64 [B]).
 
     Temperature 0: the arg-max, the smallest index on a tie, and no noise.  Temperature t > 0: Gumbel-max,
     ``argmax_c (l_c / t + g_c)``, an exact draw from ``softmax(l / t)``; the noise is counter-based (``sample_noise_words``), so
-    row b at step s gets the draw of counter row ``row0 + b`` whatever else is in the batch.  The log-probability is under the model's own
-    ``softmax(l)`` at every temperature."""
+    row b at step s gets the draw of counter row ``row0 + b`` whatever else is in the batch.  ``top_k`` / ``top_p``
+    (``sample_threshold``): the argmax runs over the kept classes only, with the same noise, an exact draw from ``softmax(l / t)``
+    restricted to them and renormalised; the token is the unfiltered one whenever that one is kept.  The log-probability is under
+    the model's own full ``softmax(l)`` at every temperature and filter."""
     if not (math.isfinite(temperature) and temperature >= 0):
         raise ValueError(f"temperature must be finite and >= 0, got {temperature}")
+    check_sample_filters(top_k, top_p)
     l = logits.double()
-    tok = sample_scores(l, temperature, seed, step, row0).argmax(1)
+    s = sample_scores(l, temperature, seed, step, row0)
+    if sample_filters_active(l.shape[1], temperature, top_k, top_p):
+        keep = l >= sample_threshold(l, temperature, top_k, top_p).unsqueeze(1)
+        s = torch.where(keep, s, torch.full((), float("-inf"), dtype=torch.float64, device=l.device))
+    tok = s.argmax(1)
     logp = torch.log_softmax(l, 1).gather(1, tok.view(-1, 1)).squeeze(1)
     return tok.to(torch.int32), logp
 
 
-def vocab_sample(h, weights, bias, temperature: float, seed: int, step, row0: int = 0, class_major: bool = False):
+def vocab_sample(h, weights, bias, temperature: float, seed: int, step, row0: int = 0, class_major: bool = False, top_k: int = 0,
+                 top_p: float = 1.0):
     """``sample_logits`` of ``l = h W + bias`` (``h [B,H]``, ``W [H,C]``; ``class_major``: ``weights`` is ``[C,H]`` = ``W^T``)
     computed in fp64: the reference of the sampling op."""
     w = weights.t() if class_major else weights
-    return sample_logits(dense_head(h.double(), w.double(), bias.double()), temperature, seed, int(step), int(row0))
+    return sample_logits(dense_head(h.double(), w.double(), bias.double()), temperature, seed, int(step), int(row0), top_k, top_p)
 
 
 def softmax_xent_per_step(logits, labels, lengths=None):

@@ -510,7 +510,7 @@ def generate_job(cfg: Config, standalone: bool = False) -> Dict:
     device in batches of ``--batch_size`` (a short last batch is filled with copies of its first prompt, whose output is dropped,
     so every batch has the shape the decode graph was captured at).  Prompts are the rows of ``--training_path`` (1..seq_len ids
     each) or, with ``--synthetic n``, the starts of n walks of the synthetic chain; ``--max_new_tokens`` ids are drawn per prompt
-    at ``--temperature`` with noise seeded by ``--seed``; prompt i draws the noise of counter row i, so a prompt's continuation
+    at ``--temperature`` (filtered by ``--top_k`` / ``--top_p``) with noise seeded by ``--seed``; prompt i draws the noise of counter row i, so a prompt's continuation
     does not depend on ``--batch_size`` and a prompt repeated k times gives k independent samples.  Writes ``<output_path>/generated.csv`` (one line of ids per prompt, in
     prompt order) and reports tokens/s, the mean log-probability per token and, with ``--synthetic``, the share of generated
     transitions the chain allows."""
@@ -534,7 +534,8 @@ def generate_job(cfg: Config, standalone: bool = False) -> Dict:
         width = int(lengths[idx].max())
         x = torch.as_tensor(prompts[idx, :width]).to(device=device, dtype=torch.int32)
         ls = torch.as_tensor(lengths[idx]).to(device=device, dtype=torch.int32)
-        tok, lp = eng.model.generate(x, ls, N, cfg.temperature, cfg.seed, row0=lo)       # prompt lo + b: its own noise
+        tok, lp = eng.model.generate(x, ls, N, cfg.temperature, cfg.seed, row0=lo,        # prompt lo + b: its own noise
+                                     top_k=cfg.top_k, top_p=cfg.top_p)
         outs.append(tok[:rows])
         lps.append(lp[:rows])
     tokens = torch.cat(outs).cpu().numpy()                 # the one wait for the device
@@ -547,12 +548,13 @@ def generate_job(cfg: Config, standalone: bool = False) -> Dict:
         f.writelines(",".join(str(int(v)) for v in row) + "\n" for row in tokens)
     out = {"mode": "generate", "model": src, "prompts": n, "tokens": int(tokens.size), "seconds": seconds,
            "tokens_per_s": tokens.size / max(seconds, 1e-9), "mean_logprob": float(logprob.mean()), "temperature": cfg.temperature,
-           "output": path}
+           "top_k": cfg.top_k, "top_p": cfg.top_p, "output": path}
     if cfg.synthetic:
         out["legal_fraction"] = D.legal_fraction(prompts, lengths, tokens, D.next_token_chain(cfg.vocab_size, cfg.seed))
     if not cfg.quiet:
         print(("RNN-LSTM - generate: model {model}, {prompts} prompts, {tokens} tokens in {seconds:.3f}s ({tokens_per_s:.1f} "
-               "tokens/s), mean log-probability {mean_logprob:.4f} per token" +
+               "tokens/s) at temperature {temperature:g}, top_k {top_k}, top_p {top_p:g}, mean log-probability {mean_logprob:.4f} "
+               "per token" +
                (", legal_fraction {legal_fraction:.4f}" if cfg.synthetic else "") + ", wrote {output}").format(**out))
     if cfg.json_log:
         jl = M.JsonLog(cfg.json_log); jl.write(**out); jl.close()
