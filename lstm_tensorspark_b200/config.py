@@ -57,6 +57,8 @@ class Config:
                                         # [forward | reverse] (2 H wide), as nn.LSTM(bidirectional=True) on a packed sequence
     dropout: float = 0.0                # nn.LSTM(dropout=P): in training, the output sequence of every layer but the last is
                                         # multiplied by a Bernoulli(1-P) mask / (1-P) before the next layer reads it
+    weight_drop: float = 0.0            # AWD-LSTM weight drop: in training, every layer direction's recurrent weights W_h are
+                                        # multiplied by a Bernoulli(1-P) mask / (1-P) drawn once per step (DropConnect)
     per_step_labels: bool = False       # sequence labelling: a label at every time step ([B,T]), the head scores the top layer's
                                         # output at each step (nn.LSTM -> nn.Linear -> cross_entropy over the real positions); a CSV
                                         # row is k*in_features values followed by k labels
@@ -230,6 +232,8 @@ class Config:
         if self.dropout > 0 and len(self.hidden_list()) == 1:
             warnings.warn(f"--dropout {self.dropout} has no effect with one layer: dropout applies between stacked layers "
                           "(it drops the output of every layer but the last)")
+        if not 0.0 <= self.weight_drop < 1.0:
+            raise ValueError(f"--weight_drop must satisfy 0 <= P < 1, got {self.weight_drop}")
         if self.sync_mode not in ("param_avg", "grad_allreduce", "none"):
             raise ValueError(f"unknown --sync_mode {self.sync_mode}")
         if not (math.isfinite(self.clip_grad_norm) and self.clip_grad_norm >= 0):
@@ -328,6 +332,10 @@ _HELP = {
     "tie_embeddings": "With --next_token and --in_features equal to the last --hidden_units: the softmax reuses the embedding "
                       "table as its weights (logits = h Embedding^T + Dense1/bias; weight tying, Press & Wolf 2017), so the model "
                       "has no Dense1/weights and the table's gradient is the sum of both uses",
+    "weight_drop": "Weight drop (DropConnect on the recurrent weights, AWD-LSTM): in training, every layer's hidden-to-hidden "
+                   "matrix W_h (both directions, one-layer models too) is multiplied by a Bernoulli(1 - P) mask scaled by "
+                   "1 / (1 - P), one mask per training step shared by every time step and batch row; evaluation and generation "
+                   "use the raw weights.  0 = off",
     "per_step_labels": "Label every time step (sequence labelling): labels [B,T], loss and accuracy over the real positions; "
                        "a CSV row is k*in_features values followed by k labels",
 }

@@ -74,6 +74,7 @@ int ts_lstm_seq_bwd(const void*, const void*, const void*, const float*, const v
                     int, int, unsigned int*, int, cudaStream_t, const unsigned int*, int, int, int, const int*, int,
                     const int*, const unsigned int*);
 int ts_dropout(const void*, void*, int, int, int, int, int, const int*, const unsigned int*, cudaStream_t);
+int ts_weight_drop_grad(const float*, float*, int, int, int, const int*, const unsigned int*, cudaStream_t);
 int ts_lstm_seq_prologue(const void*, const float*, void*, float*, void*, unsigned int*, int, int, cudaStream_t);
 int ts_seq_pool_fwd(const void*, int, const int*, const float*, int, int, int, int, float*, int*, cudaStream_t);
 int ts_seq_pool_attn_scores(float*, const float*, const float*, const int*, int, int, int, float*, cudaStream_t);
@@ -252,6 +253,21 @@ Tensor dropout(const Tensor& x, const Tensor& step, const std::vector<int64_t>& 
   auto y = torch::empty_like(x);
   check(ts_dropout(x.data_ptr(), y.data_ptr(), (int)steps, (int)B, (int)H, (int)t0, is_bf16(x), ds, dd, stream()), "dropout");
   return y;
+}
+
+// Weight drop's gradient: dst (+)= src * mask * scale over fp32 [R, H] (R = 4H rows of W_h), the mask of `desc` at time 0, as
+// `dropout` draws it for the [1, R, H] weight image.  src may be dst when accumulate is false (in place).
+void weight_drop_grad(const Tensor& src, Tensor dst, const Tensor& step, const std::vector<int64_t>& desc, bool accumulate) {
+  chk_cuda(src, "src"); chk_cuda(dst, "dst");
+  TORCH_CHECK(src.scalar_type() == torch::kFloat32 && dst.scalar_type() == torch::kFloat32 && src.dim() == 2 && src.sizes() == dst.sizes(),
+              "weight_drop_grad: src and dst must be fp32 [R, H] of the same shape");
+  TORCH_CHECK(!accumulate || src.data_ptr() != dst.data_ptr(), "weight_drop_grad: in place only in overwrite mode");
+  c10::cuda::CUDAGuard g(src.device());
+  unsigned int dd[5];
+  const int* ds = drop_args(step, desc, src, dd);
+  TORCH_CHECK(dd[4] == 0, "weight_drop_grad: the weight mask has no row offset (row0 = 0)");
+  check(ts_weight_drop_grad(src.data_ptr<float>(), dst.data_ptr<float>(), (int)src.size(0), (int)src.size(1), accumulate ? 1 : 0, ds, dd,
+                            stream()), "weight_drop_grad");
 }
 
 // ---- head ---------------------------------------------------------------------------------------------------
@@ -1071,4 +1087,6 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("in_gate_tiles_n") = 0, py::arg("extra_signal") = false, py::arg("lengths") = py::none(), py::arg("reverse") = false,
         py::arg("drop_step") = py::none(), py::arg("drop_desc") = std::vector<int64_t>{});
   m.def("dropout", &dropout, py::arg("x"), py::arg("step"), py::arg("desc"), py::arg("t0") = 0);
+  m.def("weight_drop_grad", &weight_drop_grad, py::arg("src"), py::arg("dst"), py::arg("step"), py::arg("desc"),
+        py::arg("accumulate") = false);
 }

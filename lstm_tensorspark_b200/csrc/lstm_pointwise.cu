@@ -171,6 +171,60 @@ extern "C" int ts_dropout(const void* x, void* y, int steps, int B, int H, int t
 }
 
 
+// Weight drop (DropConnect on the recurrent weights): the gradient of W_h' = W_h * M * s reaching W_h, dst (+)= src * M * s over
+// one fp32 [R, H] matrix (R = 4H stored rows).  M is the mask of ts::dropout_keep8 with the matrix taken as ONE time step of R
+// rows (t = 0; the weight stream's c2 comes with the descriptor), the same mask ts_dropout applies to the [1, R, H] image in the
+// forward pass.  One thread per Philox group (8 units of a row): one Philox call, 16 B loads and stores when H % 8 == 0.  src may
+// be dst (overwrite, in place): every element is read by the thread that writes it.
+namespace {
+__global__ void weight_drop_grad_kernel(const float* src, float* dst, int R, int H, int accumulate, ts::DropSpec d) {
+  const int groups = (H + 7) / 8;
+  const long long total = (long long)R * groups;
+  const uint32_t step = (uint32_t)__ldg(d.step);
+  const bool vec = (H & 7) == 0;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int g = (int)(i % groups), r = (int)(i / groups);
+    const uint32_t keep = ts::dropout_keep8(d, step, r, 8 * g, 0, H);
+    const size_t base = (size_t)r * H + 8 * g;
+    if (vec) {
+      float4 v[2] = {*reinterpret_cast<const float4*>(src + base), *reinterpret_cast<const float4*>(src + base + 4)};
+      float4 o[2] = {make_float4(0.f, 0.f, 0.f, 0.f), make_float4(0.f, 0.f, 0.f, 0.f)};
+      if (accumulate) { o[0] = *reinterpret_cast<const float4*>(dst + base); o[1] = *reinterpret_cast<const float4*>(dst + base + 4); }
+      float* vf = reinterpret_cast<float*>(v);
+      float* of = reinterpret_cast<float*>(o);
+#pragma unroll
+      for (int u = 0; u < 8; ++u) {
+        const float m = ((keep >> u) & 1u) ? __fmul_rn(vf[u], d.scale) : 0.f;
+        of[u] = accumulate ? __fadd_rn(of[u], m) : m;
+      }
+      *reinterpret_cast<float4*>(dst + base) = o[0];
+      *reinterpret_cast<float4*>(dst + base + 4) = o[1];
+    } else {
+#pragma unroll
+      for (int u = 0; u < 8; ++u) {
+        if (8 * g + u >= H) break;
+        const float m = ((keep >> u) & 1u) ? __fmul_rn(src[base + u], d.scale) : 0.f;
+        dst[base + u] = accumulate ? __fadd_rn(dst[base + u], m) : m;
+      }
+    }
+  }
+}
+}  // namespace
+
+extern "C" int ts_weight_drop_grad(const float* src, float* dst, int R, int H, int accumulate, const int* drop_step,
+                                   const unsigned int* drop_desc, cudaStream_t st) {
+  if (drop_step == nullptr) return -2;
+  if ((H & 7) == 0 && (((uintptr_t)src | (uintptr_t)dst) & 15) != 0) return -3;      // the 16 B path needs aligned rows
+  const ts::DropSpec d = ts::make_drop_spec(drop_step, drop_desc);
+  const long long total = (long long)R * ((H + 7) / 8);
+  int blocks = (int)((total + 255) / 256);
+  if (blocks > 132 * 8) blocks = 132 * 8;
+  if (blocks < 1) return 0;
+  weight_drop_grad_kernel<<<blocks, 256, 0, st>>>(src, dst, R, H, accumulate, d);
+  return (int)cudaGetLastError();
+}
+
+
 // [B,T,D] -> [T,B,D] for a row-contiguous tensor (row = D elements, row_bytes % 16 == 0): a pure row permutation, so it
 // runs at copy speed with 16 B vectors (the framework's generic strided copy of the transposed view takes 3.5x longer).
 // Replaces the batch-major -> time-major feed conversion in front of the first layer's x-projection GEMM.

@@ -140,17 +140,17 @@ class LSTMLayer(nn.Module):
             self._set_state(self.h0, self.c0)
         self.state = []
 
-    def train_layer(self, input_data: torch.Tensor):
-        h, c = F.lstm_cell_step(input_data, self.ht, self.Ct, self.w_x, self.w_h, self.bias)
+    def train_layer(self, input_data: torch.Tensor, weight_drop=None):
+        h, c = F.lstm_cell_step(input_data, self.ht, self.Ct, self.w_x, self.w_h, self.bias, weight_drop=weight_drop)
         self._set_state(h, c)
 
     def restore_state(self):
         self._set_state(self.state[-1][0], self.state[-1][1])
 
-    def fit_next(self, data: torch.Tensor, train: bool = True, dropout=None) -> torch.Tensor:
+    def fit_next(self, data: torch.Tensor, train: bool = True, dropout=None, weight_drop=None) -> torch.Tensor:
         """One step.  ``dropout``: optional ``ops.reference.DropoutSpec`` of the returned output (time 0); the carried state
-        is not dropped."""
-        self.train_layer(data)
+        is not dropped.  ``weight_drop``: optional weight-drop ``DropoutSpec``: the step reads ``W_h * M * s``."""
+        self.train_layer(data, weight_drop)
         out = F.dropout(self.ht, dropout)
         if train:
             self.state.append((self.ht, self.Ct))
@@ -160,17 +160,19 @@ class LSTMLayer(nn.Module):
         return out
 
     # ---- whole-sequence path (the thing the persistent kernel implements) ----------------------
-    def fit_sequence(self, x_seq: torch.Tensor, lengths: Optional[torch.Tensor] = None, dropout=None) -> torch.Tensor:
+    def fit_sequence(self, x_seq: torch.Tensor, lengths: Optional[torch.Tensor] = None, dropout=None,
+                     weight_drop=None) -> torch.Tensor:
         """``x_seq [T,B,D]`` -> ``h_seq [T,B,H]``; final (ht, Ct) stored on the layer.  ``lengths`` (int32 ``[B]``, right
         padding): the final state is each row's state after its own last step; padded positions of ``h_seq`` carry it.
         A reverse layer runs from the last step to the first: its final state is the one after step 0, and its padded
         positions hold the initial state.  ``dropout``: optional ``ops.reference.DropoutSpec``; the returned sequence is then
-        the dropped one (the final state is not dropped)."""
+        the dropped one (the final state is not dropped).  ``weight_drop``: optional weight-drop ``DropoutSpec``: every step reads
+        ``W_h * M * s`` (``ops.reference.weight_drop``) and ``w_h`` gets the masked gradient."""
         B = x_seq.shape[1]
         if B != self.ht.shape[0]:
             self.reset_state(B)
         h_seq, h_T, c_T = F.lstm_layer_sequence(x_seq, self.ht, self.Ct, self.w_x, self.w_h, self.bias, lengths=lengths,
-                                                reverse=self.reverse, dropout=dropout)
+                                                reverse=self.reverse, dropout=dropout, weight_drop=weight_drop)
         self._set_state(h_T, c_T)
         self.state.append((h_T, c_T))
         return h_seq

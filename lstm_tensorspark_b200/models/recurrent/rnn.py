@@ -6,7 +6,8 @@ Public surface mirrors original src/models/recurrent/rnn.py:5-53: ``RNN(settings
 ``num_hidden``, ``batch_size``).  New: ``fit_layers`` also accepts a sequence ``[B,T,D]`` and unrolls it
 through time on the fused per-layer sequence op (the reference only ever takes one step), and
 ``add_reverse_layers()`` makes the stack bidirectional, and ``dropout`` drops the output of every layer but the last while
-the module is in training mode (``nn.LSTM(dropout=...)``).
+the module is in training mode (``nn.LSTM(dropout=...)``).  ``weight_drop`` drops connections of every layer direction's
+recurrent weights ``W_h`` in training mode, one mask per training step (AWD-LSTM's ``WeightDrop``, Merity et al. 2017).
 """
 from __future__ import annotations
 
@@ -22,14 +23,17 @@ EXPORT_KEYS = ("wf", "wi", "wo", "wc", "bf", "bi", "bc", "bo")
 
 
 class RNN(nn.Module):
-    def __init__(self, settings: Iterable[dict], dropout: float = 0.0, **layer_kw):
+    def __init__(self, settings: Iterable[dict], dropout: float = 0.0, weight_drop: float = 0.0, **layer_kw):
         super().__init__()
         if not 0.0 <= dropout < 1.0:
             raise ValueError(f"dropout must satisfy 0 <= P < 1, got {dropout}")
+        if not 0.0 <= weight_drop < 1.0:
+            raise ValueError(f"weight_drop must satisfy 0 <= P < 1, got {weight_drop}")
         self.layers = nn.ModuleList()
         self.reverse_layers = nn.ModuleList()      # empty, or one reverse-time layer per entry of ``layers``
         self._layer_kw = layer_kw
         self.dropout = float(dropout)
+        self.weight_drop = float(weight_drop)
         # the mask's key (seed, partition) and step counter (training steps completed: an int32 [1] device tensor on the GPU,
         # an int on the CPU); a TrainEngine sets and advances them
         self.dropout_key = (0, 0)
@@ -41,6 +45,13 @@ class RNN(nn.Module):
         if not self.training or self.dropout == 0 or layer >= len(self.layers) - 1:
             return None
         return DropoutSpec(self.dropout, self.dropout_key, layer, reverse, self.dropout_step)
+
+    def weight_drop_spec(self, layer: int, reverse: bool = False) -> Optional[DropoutSpec]:
+        """The weight drop of layer ``layer``'s ``W_h`` (direction ``reverse``) in this forward pass: every layer, the top one
+        included; None with P = 0 and in eval mode.  Same key and step counter as ``dropout_spec``, its own counter stream."""
+        if not self.training or self.weight_drop == 0:
+            return None
+        return DropoutSpec(self.weight_drop, self.dropout_key, layer, reverse, self.dropout_step, weight=True)
 
     def _make(self, setting: dict, reverse: bool = False) -> LSTMLayer:
         name = setting["layer_name"] + ("_reverse" if reverse else "")
@@ -116,7 +127,7 @@ class RNN(nn.Module):
                 raise ValueError("a bidirectional stack needs whole sequences [B,T,D]: the one-step [B,D] path runs forward only")
             state = input_data
             for i, layer in enumerate(self.layers):
-                state = layer.fit_next(state, train=train, dropout=self.dropout_spec(i))
+                state = layer.fit_next(state, train=train, dropout=self.dropout_spec(i), weight_drop=self.weight_drop_spec(i))
             return state
         if input_data.dim() != 3:
             raise ValueError(f"expected [B,D] or [B,T,D], got {tuple(input_data.shape)}")
@@ -139,8 +150,8 @@ class RNN(nn.Module):
         from ...ops import functional as F
         if self.bidirectional:
             for i, (la, lr) in enumerate(zip(self.layers, self.reverse_layers)):
-                seq = torch.cat([la.fit_sequence(seq, lengths, self.dropout_spec(i)),
-                                 lr.fit_sequence(seq, lengths, self.dropout_spec(i, True))], 2)
+                seq = torch.cat([la.fit_sequence(seq, lengths, self.dropout_spec(i), self.weight_drop_spec(i)),
+                                 lr.fit_sequence(seq, lengths, self.dropout_spec(i, True), self.weight_drop_spec(i, True))], 2)
             return seq
         i, n = 0, len(self.layers)
         while i < n:
@@ -153,12 +164,14 @@ class RNN(nn.Module):
                         l.reset_state(B)
                 seq, hT_a, cT_a, hT_b, cT_b = F.lstm_pair_sequence(seq, (la.ht, la.Ct, la.w_x, la.w_h, la.bias),
                                                                      (lb.ht, lb.Ct, lb.w_x, lb.w_h, lb.bias), lengths=lengths,
-                                                                     dropouts=(self.dropout_spec(i), self.dropout_spec(i + 1)))
+                                                                     dropouts=(self.dropout_spec(i), self.dropout_spec(i + 1)),
+                                                                     weight_drops=(self.weight_drop_spec(i),
+                                                                                   self.weight_drop_spec(i + 1)))
                 la._set_state(hT_a, cT_a); la.state.append((hT_a, cT_a))
                 lb._set_state(hT_b, cT_b); lb.state.append((hT_b, cT_b))
                 i += 2
             else:
-                seq = la.fit_sequence(seq, lengths, self.dropout_spec(i))
+                seq = la.fit_sequence(seq, lengths, self.dropout_spec(i), self.weight_drop_spec(i))
                 i += 1
         return seq
 

@@ -28,7 +28,8 @@ FORCE_GENERIC = os.environ.get("LSTM_TS_FORCE_GENERIC", "0") == "1"
 #   6 no L2 prefetch, 7 cluster-scope acquire on the exchange barriers), [16:18) sync mode (0 per-k-block dataflow counters,
 #   1 one counter per batch tile = grid barrier, 2 per-CTA flags), bit 18 acquire polls, bit 19 no forward K-split.
 SEQ_VARIANT = int(os.environ.get("LSTM_TS_SEQ_VARIANT", "0"))
-STATS = {"fast_fwd": 0, "fast_bwd": 0, "generic_fwd": 0, "generic_bwd": 0, "tc_gemm": 0, "kernels": 0}
+STATS = {"fast_fwd": 0, "fast_bwd": 0, "generic_fwd": 0, "generic_bwd": 0, "tc_gemm": 0, "kernels": 0, "weight_drop": 0,
+         "weight_drop_grad": 0}
 
 
 # Gradient-bucket overlap (engine.TrainEngine + parallel/fused_comm.py): HOOKS["grads_written"] is called after every weight /
@@ -58,9 +59,12 @@ def _after_big_launch(flush: bool = False):
         AFTER_SEQ_BWD.pop(0)[1]()
 
 
+_HOLD = {"on": False}        # True while a written gradient still waits for its weight-drop mask (see _LSTMPairFn.backward)
+
+
 def _grads_written():
     h = HOOKS["grads_written"]
-    if h is not None and not _CHUNKING["on"]:
+    if h is not None and not _CHUNKING["on"] and not _HOLD["on"]:
         h()
 
 _PARAMS = {}          # fp32 param address -> (bf16 shadow view, fp32 grad view), maintained by models.flat.FlatParams
@@ -106,7 +110,7 @@ def grad_sink(w_addr: int):
 
 
 def _accumulate_grad(w_addr: int, a_t: torch.Tensor, b: torch.Tensor, b_folded: bool = False, pdl: bool = False,
-                     max_ctas: int = 0, ctas: int = 0, rowsum=None):
+                     max_ctas: int = 0, ctas: int = 0, rowsum=None, wdrop=None, defer: bool = False):
     """dW = a_t @ b in fp32 (``a_t`` = dG^T as a transposed view, ``b`` = the layer input: both operands MN-major, read in
     place by the wgmma GEMM; ``b_folded``: ``b`` is the batch-major [B,T,D] array standing for the time-major [T*B, D]
     matrix).  When the parameter lives in a FlatParams buffer the product lands straight in its grad
@@ -115,21 +119,39 @@ def _accumulate_grad(w_addr: int, a_t: torch.Tensor, b: torch.Tensor, b_folded: 
     recurrence that is still running).  Such a GEMM is no "big launch" for the gradient buckets: what precedes it in the stream
     may still be running when it starts, so no bucket's allreduce is launched under it.  ``ctas``: CTAs per tile cluster of
     an ordinary launch (0 = ``cuda_gemm.GEMM_CTAS``).  ``rowsum``: see ``cuda_gemm.matmul`` (the bias gradient, summed by the
-    same launch)."""
+    same launch).
+
+    ``wdrop``: the kernel arguments of a weight-drop spec (``_drop_args``): the product is the gradient of the masked matrix and
+    ``weight_drop_grad`` masks it into the sink - in place on a first write, from an fp32 scratch when the sink accumulates - or
+    into the tensor returned to autograd.  The gradient counts as written only once the mask is enqueued.  ``defer``: return a
+    callable that launches the mask (and reports the gradient written) and returns what autograd gets, for a caller that has
+    programmatic dependents to launch right behind the GEMM first."""
     ops = dict(a=a_t, b_t=None, b_folded=b, ctas=ctas) if b_folded else dict(a=a_t, b_t=b.t(), ctas=ctas)
     ops["rowsum"] = rowsum
     if pdl:
         ops.update(pdl=True, ctas=1, max_ctas=max_ctas)
     sink = grad_sink(w_addr)
     if sink is not None:
+        scratch = bool(wdrop) and sink[1]
         if not pdl:
             _big_launch_begin()
-        G.matmul(out=sink[0], accumulate=sink[1], **ops)
+        part = G.matmul(out_dtype=torch.float32, **ops) if scratch else G.matmul(out=sink[0], accumulate=sink[1], **ops)
         if not pdl:
             _after_big_launch()              # finished buckets of earlier gradients: allreduce them under this GEMM
-        _grads_written()
-        return None
-    return G.matmul(out_dtype=torch.float32, **ops)
+
+        def finish():
+            if wdrop:
+                _weight_drop_grad(part if scratch else sink[0], sink[0], wdrop, scratch)
+            _grads_written()
+            return None
+    else:
+        dw = G.matmul(out_dtype=torch.float32, **ops)
+
+        def finish():
+            if wdrop:
+                _weight_drop_grad(dw, dw, wdrop, False)
+            return dw
+    return finish if defer else finish()
 
 
 _BIAS_SPLIT = {}
@@ -315,6 +337,24 @@ def _drop_args(spec, device) -> dict:
     return {"drop_step": step, "drop_desc": spec.desc()}
 
 
+def _weight_image(w_h_c: torch.Tensor, spec) -> torch.Tensor:
+    """Weight drop: ``W_h' = W_h * M * s`` of a weight-drop spec (``reference.weight_drop``), computed from the compute-dtype copy
+    (the bf16 shadow, or fp32) by the dropout kernel over its ``[1, 4H, H]`` view; ``w_h_c`` itself for None / P = 0."""
+    d = _drop_args(spec, w_h_c.device)
+    if not d:
+        return w_h_c
+    STATS["weight_drop"] += 1
+    STATS["kernels"] += 1
+    return ext().dropout(w_h_c.unsqueeze(0), d["drop_step"], d["drop_desc"], 0)[0]
+
+
+def _weight_drop_grad(src: torch.Tensor, dst: torch.Tensor, wdrop: dict, accumulate: bool) -> None:
+    """``dst (+)= src * M * s``: the gradient of the masked matrix -> the gradient of ``W_h`` (csrc/lstm_pointwise.cu)."""
+    STATS["weight_drop_grad"] += 1
+    STATS["kernels"] += 1
+    ext().weight_drop_grad(src, dst, wdrop["drop_step"], wdrop["drop_desc"], accumulate)
+
+
 class _DropoutFn(torch.autograd.Function):
     """Standalone dropout (csrc/lstm_pointwise.cu ts_dropout), forward and backward with the same mask: the one-step path and
     the shapes the persistent kernels do not fuse it into.  ``x [..., B, H]``, leading dims = times t0, t0 + 1, ..."""
@@ -341,14 +381,15 @@ def dropout(x: torch.Tensor, spec, t0: int = 0) -> torch.Tensor:
 
 class _LSTMSeqFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x_seq, h0, c0, w_x, w_h, bias, lengths=None, reverse=False, dropout=None):
+    def forward(ctx, x_seq, h0, c0, w_x, w_h, bias, lengths=None, reverse=False, dropout=None, weight_drop=None):
         E = ext()
         T, B, D = x_seq.shape
         H = w_h.shape[1]
         cd = x_seq.dtype
         x2d = x_seq.reshape(T * B, D).contiguous()
         w_x_c = _lowp(w_x, cd)
-        w_h_c = _lowp(w_h, cd)
+        ctx.wdrop = _drop_args(weight_drop, x_seq.device)
+        w_h_c = _weight_image(_lowp(w_h, cd), weight_drop)             # every step reads the masked image (weight drop)
         bias_f = bias.detach().float().contiguous()
         gx = _gemm_tn(x2d, w_x_c).view(T, B, 4 * H)
         fast = fast_path_supported(B, H, cd, x_seq.device)
@@ -447,22 +488,24 @@ class _LSTMSeqFn(torch.autograd.Function):
         dg_t = dg2d.t()
         dw_x = _accumulate_grad(ctx.w_addrs[0], dg_t, x2d)
         h_prev = h_seq[1:] if ctx.reverse else h_seq[:T]          # the h each step's dG pairs with
-        dw_h = _accumulate_grad(ctx.w_addrs[1], dg_t, h_prev.reshape(T * B, H))
+        dw_h = _accumulate_grad(ctx.w_addrs[1], dg_t, h_prev.reshape(T * B, H), wdrop=ctx.wdrop)
         db = _bias_grad(ctx.w_addrs[2], dg2d)
         dx = None
         if ctx.needs_input_grad[0]:
             dx = G.matmul(dg2d, w_x_c.t(), out_dtype=cd).view(T, B, D)        # dG · W_x: W_x read in place as an MN-major operand
             STATS["kernels"] += 1
         h0_dt, c0_dt = ctx.in_dtypes
-        return dx, dh0.to(h0_dt), dc0.to(c0_dt), dw_x, dw_h, db, None, None, None
+        return dx, dh0.to(h0_dt), dc0.to(c0_dt), dw_x, dw_h, db, None, None, None, None
 
 
-def lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths=None, reverse=False, dropout=None):
+def lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths=None, reverse=False, dropout=None, weight_drop=None):
     """``x_seq [T,B,D]`` (bf16 or fp32) -> ``(h_seq [T,B,H], h_T, c_T)``.  ``lengths``: optional int32 ``[B]`` on the batch's
     device, right padding (``ops/reference.py``); the persistent kernels then run their masked instantiations.  ``reverse``:
     the reverse-time direction (time T-1 down to 0; ``h_T`` / ``c_T`` are then the state after time 0).  ``dropout``: a
     ``reference.DropoutSpec``; the first output is then the dropped sequence (the persistent kernels store it next to h_seq
-    and mask the incoming gradient as they load it; other shapes run the standalone dropout kernel)."""
+    and mask the incoming gradient as they load it; other shapes run the standalone dropout kernel).  ``weight_drop``: a weight-drop
+    ``reference.DropoutSpec``: the kernels read the masked image ``W_h * M * s`` in place of ``W_h`` and the weight gradient is
+    masked on its way into the sink (one mask for every batch chunk)."""
     if (not x_seq.is_contiguous() and not x_seq.requires_grad and x_seq.transpose(0, 1).is_contiguous()
             and (x_seq.shape[2] * x_seq.element_size()) % 16 == 0):
         x_seq = ext().transpose01(x_seq.transpose(0, 1))     # batch-major feed -> time-major, a row permutation at copy speed
@@ -478,14 +521,14 @@ def lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths=None, reverse=Fal
         try:
             outs = [_LSTMSeqFn.apply(x_seq[:, b0:b0 + chunk].contiguous(), h0[b0:b0 + chunk], c0[b0:b0 + chunk], w_x, w_h, bias,
                                      None if lengths is None else lengths[b0:b0 + chunk], reverse,
-                                     None if dropout is None else dropout.at_rows(b0))
+                                     None if dropout is None else dropout.at_rows(b0), weight_drop)
                     for b0 in range(0, B, chunk)]
         finally:
             _CHUNKING["on"] = False
         STATS["batch_chunks"] = STATS.get("batch_chunks", 0) + len(outs)
         return (torch.cat([o[0] for o in outs], dim=1), torch.cat([o[1] for o in outs], dim=0),
                 torch.cat([o[2] for o in outs], dim=0))
-    return _LSTMSeqFn.apply(x_seq.contiguous(), h0, c0, w_x, w_h, bias, lengths, reverse, dropout)
+    return _LSTMSeqFn.apply(x_seq.contiguous(), h0, c0, w_x, w_h, bias, lengths, reverse, dropout, weight_drop)
 
 
 # =====================================================================================================================
@@ -625,7 +668,7 @@ def _gate_cfg(var: int, tiles_m: int, nkb: int, per_kb_step: int, ctas_per_tile:
 class _LSTMPairFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x_seq, h0a, c0a, w_xa, w_ha, b_a, h0b, c0b, w_xb, w_hb, b_b, lengths=None, schedule="wavefront", drop_a=None,
-                drop_b=None):
+                drop_b=None, wdrop_a=None, wdrop_b=None):
         E = ext()
         pipelined = schedule == "pipelined"
         dev = x_seq.device
@@ -637,6 +680,8 @@ class _LSTMPairFn(torch.autograd.Function):
         x_bm = x_seq.transpose(0, 1) if not x_seq.is_contiguous() else None
         x2d = x_seq.reshape(T * B, D) if x_bm is None else x_bm
         wxa, wha, wxb, whb = _lowp(w_xa, cd), _lowp(w_ha, cd), _lowp(w_xb, cd), _lowp(w_hb, cd)
+        wha, whb = _weight_image(wha, wdrop_a), _weight_image(whb, wdrop_b)          # weight drop: the masked images
+        ctx.wdrop = (_drop_args(wdrop_a, dev), _drop_args(wdrop_b, dev))
         ba_f, bb_f = b_a.detach().float().contiguous(), b_b.detach().float().contiguous()
         h0a_c, h0b_c = h0a.detach().to(cd).contiguous(), h0b.detach().to(cd).contiguous()
         c0a_f, c0b_f = c0a.detach().float().contiguous(), c0b.detach().float().contiguous()
@@ -715,6 +760,7 @@ class _LSTMPairFn(torch.autograd.Function):
         E = ext()
         x2d, h_seq_a, c_seq_a, act_a, h_seq_b, c_seq_b, act_b, wxa, wha, wxb, whb, hin_b = ctx.saved_tensors
         dra, drb = ctx.drop
+        wda, wdb = ctx.wdrop
         if dh_seq_b is None:
             drb = {}
         T, B, D, Ha, Hb = ctx.dims
@@ -760,18 +806,30 @@ class _LSTMPairFn(torch.autograd.Function):
             # concurrent column-sum launches would share the slab scratch).  Gradient buckets are launched under the next
             # ordinary launch (dW_xa), not under these: a programmatic dependent may start before the kernels ahead of it in
             # the stream are complete.
+            # Weight drop: dW_hb's mask is an ordinary launch behind the column sums (it runs after L_a, before dW_xa), and the
+            # gradient counts as written only from then on.
             side = max(1, (_sms(dev) - Ha // 16 - _COLSUM_SMS) // 2)
             dw_xb = _accumulate_grad(a[3], dg_b.t(), hin_b.reshape(T * B, Ha), pdl=True, max_ctas=side)
-            dw_hb = _accumulate_grad(a[4], dg_b.t(), h_seq_b[:T].reshape(T * B, Hb), pdl=True, max_ctas=side)
-            db_b = _bias_grad(a[5], dg_b, under_gemm=True, max_ctas=4 * _COLSUM_SMS)
+            if wdb:
+                _HOLD["on"] = True
+                try:
+                    finish_hb = _accumulate_grad(a[4], dg_b.t(), h_seq_b[:T].reshape(T * B, Hb), pdl=True, max_ctas=side,
+                                                 wdrop=wdb, defer=True)
+                    db_b = _bias_grad(a[5], dg_b, under_gemm=True, max_ctas=4 * _COLSUM_SMS)
+                finally:
+                    _HOLD["on"] = False
+                dw_hb = finish_hb()
+            else:
+                dw_hb = _accumulate_grad(a[4], dg_b.t(), h_seq_b[:T].reshape(T * B, Hb), pdl=True, max_ctas=side)
+                db_b = _bias_grad(a[5], dg_b, under_gemm=True, max_ctas=4 * _COLSUM_SMS)
         else:
             # the bias column sums run NEXT TO the first weight-gradient GEMM of their layer (same dG, idle SMs), not after it
             # (each GEMM is followed by: finished gradient buckets [programmatic dependents of the GEMM], then half of the layer's
             # bias column sums [programmatic dependent of whatever was launched last] - all three run side by side)
             dw_xb = _accumulate_grad(a[3], dg_b.t(), hin_b.reshape(T * B, Ha))
             _bias_grad(a[5], dg_b, under_gemm=dw_xb is None, part=0)
-            dw_hb = _accumulate_grad(a[4], dg_b.t(), h_seq_b[:T].reshape(T * B, Hb))
-            db_b = _bias_grad(a[5], dg_b, under_gemm=dw_hb is None, part=1)
+            dw_hb = _accumulate_grad(a[4], dg_b.t(), h_seq_b[:T].reshape(T * B, Hb), wdrop=wdb)
+            db_b = _bias_grad(a[5], dg_b, under_gemm=dw_hb is None and not wdb, part=1)
         dg_a = dpre_a.view(T * B, 4 * Ha)
         if pipelined:
             # 2 x 1024 on a 132-SM H100: single-CTA 128 x 256 tiles put the 128 tiles of each of these GEMMs on 128 SMs in one
@@ -783,7 +841,7 @@ class _LSTMPairFn(torch.autograd.Function):
             bsink = grad_sink(a[2])
             db_a = bsink[0] if bsink is not None else torch.empty(4 * Ha, **f32)
             dw_ha = _accumulate_grad(a[1], dg_a.t(), h_seq_a[:T].reshape(T * B, Ha), ctas=1,
-                                     rowsum=(db_a, bsink is not None and bsink[1]))
+                                     rowsum=(db_a, bsink is not None and bsink[1]), wdrop=wda)
             STATS["fused_bias_grads"] = STATS.get("fused_bias_grads", 0) + 1
             if bsink is not None:
                 db_a = None
@@ -791,23 +849,24 @@ class _LSTMPairFn(torch.autograd.Function):
         else:
             dw_xa = _accumulate_grad(a[0], dg_a.t(), x2d, b_folded=ctx.x_folded)
             _bias_grad(a[2], dg_a, under_gemm=dw_xa is None, part=0)
-            dw_ha = _accumulate_grad(a[1], dg_a.t(), h_seq_a[:T].reshape(T * B, Ha))
-            db_a = _bias_grad(a[2], dg_a, under_gemm=dw_ha is None, part=1)
+            dw_ha = _accumulate_grad(a[1], dg_a.t(), h_seq_a[:T].reshape(T * B, Ha), wdrop=wda)
+            db_a = _bias_grad(a[2], dg_a, under_gemm=dw_ha is None and not wda, part=1)
         dx = None
         if ctx.needs_input_grad[0]:                                       # (never with a folded input: lstm_pair_sequence)
             dx = G.matmul(dg_a, wxa.t(), out_dtype=cd).view(T, B, D)
             STATS["kernels"] += 1
         t = ctx.in_dtypes
         return (dx, dh0a.to(t[0]), dc0a.to(t[1]), dw_xa, dw_ha, db_a, dh0b.to(t[2]), dc0b.to(t[3]), dw_xb, dw_hb, db_b, None, None,
-                None, None)
+                None, None, None, None)
 
 
-def lstm_pair_sequence(x_seq, la, lb, lengths=None, schedule=None, dropouts=(None, None)):
+def lstm_pair_sequence(x_seq, la, lb, lengths=None, schedule=None, dropouts=(None, None), weight_drops=(None, None)):
     """Two stacked layers as one op.  ``la`` / ``lb`` = (h0, c0, w_x, w_h, bias).  -> (h_seq_b, hT_a, cT_a, hT_b, cT_b).
     ``lengths``: optional int32 ``[B]`` per-row lengths (both layers run their masked kernels; the gated GEMM is unchanged).
     ``schedule``: "wavefront" or "pipelined" (see ``pair_schedule``); None = the one ``pair_schedule`` picks for the device.
     ``dropouts``: ``reference.DropoutSpec`` (or None) of layer a's output (the input of layer b) and of layer b's output (the
-    first result)."""
+    first result).  ``weight_drops``: weight-drop ``reference.DropoutSpec`` (or None) of layer a's and layer b's ``W_h``: the
+    recurrences read the masked images, and each ``dW_h`` is masked on its way into the sink."""
     _check_lengths_arg(lengths, x_seq.shape[1], x_seq.device)
     if schedule is None:
         schedule = _pair_schedule_of(x_seq, la[3].shape[1], lb[3].shape[1])
@@ -817,7 +876,7 @@ def lstm_pair_sequence(x_seq, la, lb, lengths=None, schedule=None, dropouts=(Non
     if (not x_seq.is_contiguous() and not x_seq.requires_grad and x_seq.transpose(0, 1).is_contiguous()
             and (x_seq.shape[2] * x_seq.element_size()) % 16 == 0):
         if FOLDED_FEED and G.folded_ok(x_seq.transpose(0, 1)):
-            return _LSTMPairFn.apply(x_seq, *la, *lb, lengths, schedule, *dropouts)  # read in place (see forward)
+            return _LSTMPairFn.apply(x_seq, *la, *lb, lengths, schedule, *dropouts, *weight_drops)  # read in place (see forward)
         x_seq = ext().transpose01(x_seq.transpose(0, 1))
         STATS["kernels"] += 1
-    return _LSTMPairFn.apply(x_seq.contiguous(), *la, *lb, lengths, schedule, *dropouts)
+    return _LSTMPairFn.apply(x_seq.contiguous(), *la, *lb, lengths, schedule, *dropouts, *weight_drops)

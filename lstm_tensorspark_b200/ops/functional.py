@@ -36,22 +36,27 @@ def _use_ext(t: torch.Tensor) -> bool:
     return False
 
 
-def lstm_cell_step(x, h, c, w_x, w_h, bias):
+def lstm_cell_step(x, h, c, w_x, w_h, bias, weight_drop=None):
+    """One step.  ``weight_drop``: optional weight-drop ``reference.DropoutSpec``: the step reads ``W_h * M * s``
+    (``reference.weight_drop``)."""
     if _use_ext(x):
         from . import cuda_lstm
-        h_seq, h_T, c_T = cuda_lstm.lstm_layer_sequence(x.unsqueeze(0), h, c, w_x, w_h, bias)
+        h_seq, h_T, c_T = cuda_lstm.lstm_layer_sequence(x.unsqueeze(0), h, c, w_x, w_h, bias, weight_drop=weight_drop)
         return h_T, c_T
-    return ref.lstm_cell_step(x, h, c, w_x, w_h, bias)
+    return ref.lstm_cell_step(x, h, c, w_x, ref.weight_drop(w_h, weight_drop), bias)
 
 
-def lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths=None, reverse=False, dropout=None):
+def lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths=None, reverse=False, dropout=None, weight_drop=None):
     """``lengths``: optional int32 ``[B]`` per-row sequence lengths (right padding, see ``reference.lstm_layer_sequence``).
     ``reverse``: the reverse-time direction of a bidirectional layer (same reference).  ``dropout``: optional
-    ``reference.DropoutSpec``: the first output is then the dropped sequence."""
+    ``reference.DropoutSpec``: the first output is then the dropped sequence.  ``weight_drop``: optional weight-drop
+    ``reference.DropoutSpec``: every step reads ``W_h * M * s`` and ``W_h`` gets the masked gradient."""
     if _use_ext(x_seq):
         from . import cuda_lstm
-        return cuda_lstm.lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths=lengths, reverse=reverse, dropout=dropout)
-    return ref.lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths=lengths, reverse=reverse, dropout=dropout)
+        return cuda_lstm.lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths=lengths, reverse=reverse, dropout=dropout,
+                                             weight_drop=weight_drop)
+    return ref.lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths=lengths, reverse=reverse, dropout=dropout,
+                                   weight_drop=weight_drop)
 
 
 def dropout(x, spec, t0: int = 0):
@@ -185,6 +190,6 @@ def lstm_pair_supported(x_seq, h_a: int, h_b: int) -> bool:
     return cuda_lstm.wavefront_supported(x_seq, h_a, h_b)
 
 
-def lstm_pair_sequence(x_seq, la, lb, lengths=None, dropouts=(None, None)):
+def lstm_pair_sequence(x_seq, la, lb, lengths=None, dropouts=(None, None), weight_drops=(None, None)):
     from . import cuda_lstm
-    return cuda_lstm.lstm_pair_sequence(x_seq, la, lb, lengths=lengths, dropouts=dropouts)
+    return cuda_lstm.lstm_pair_sequence(x_seq, la, lb, lengths=lengths, dropouts=dropouts, weight_drops=weight_drops)

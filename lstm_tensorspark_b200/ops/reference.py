@@ -81,6 +81,9 @@ def philox4x32_10(ctr: torch.Tensor, key0, key1) -> torch.Tensor:
     return torch.stack(c, -1)
 
 
+WEIGHT_DROP_C2 = 0x80000000      # high bit of c2: the weight-drop masks (DropoutSpec.weight)
+
+
 def dropout_threshold(p: float) -> int:
     """A unit is kept iff its 16-bit value is >= this: P quantised to 1/65536."""
     return min(int(round(p * 65536)), 65535)
@@ -97,13 +100,17 @@ class DropoutSpec:
 
     ``key``: (seed, partition) - replicas draw different masks.  ``layer`` / ``reverse``: counter word c2 = 2 layer + reverse.
     ``step``: training steps completed (counter word c3) - an int32 ``[1]`` device tensor on the CUDA path (a captured graph
-    reads its current value), an int on the CPU.  ``row0``: batch row of local row 0 (batch chunks)."""
+    reads its current value), an int on the CPU.  ``row0``: batch row of local row 0 (batch chunks).
+
+    ``weight``: the weight-drop stream instead (DropConnect on the layer direction's ``W_h [4H, H]``, ``weight_drop``): the
+    matrix is one time step of 4H rows and c2 = 0x80000000 | (2 layer + reverse), apart from every output stream's c2 < 2^31."""
     p: float
     key: Tuple[int, int]
     layer: int
     reverse: bool
     step: Union[int, torch.Tensor]
     row0: int = 0
+    weight: bool = False
 
     @property
     def thr(self) -> int:
@@ -111,7 +118,7 @@ class DropoutSpec:
 
     @property
     def c2(self) -> int:
-        return 2 * self.layer + int(self.reverse)
+        return (WEIGHT_DROP_C2 if self.weight else 0) | (2 * self.layer + int(self.reverse))
 
     def desc(self):
         """{key0, key1, thr, c2, row0} as the kernels take it."""
@@ -150,8 +157,23 @@ def dropout(x: torch.Tensor, spec: Optional[DropoutSpec], t0: int = 0) -> torch.
     return torch.where(keep, y, torch.zeros((), dtype=x.dtype, device=x.device))
 
 
+def weight_drop_mask(spec: DropoutSpec, rows: int, H: int, device=None) -> torch.Tensor:
+    """Keep mask ``[rows, H]`` (bool) of a weight-drop ``spec``: ``dropout_mask`` of one time step (t = 0) of ``rows`` rows, so row
+    r, unit k takes counter (r ceil(H/8) + k/8, 0, c2, step).  Row r is the stored (gate-interleaved) row of ``W_h``."""
+    return dropout_mask(spec, 1, rows, H, device=device)[0]
+
+
+def weight_drop(w_h: torch.Tensor, spec: Optional[DropoutSpec]) -> torch.Tensor:
+    """Weight drop (DropConnect on the recurrent weights, AWD-LSTM's ``WeightDrop``): ``W_h * M * s`` of a ``weight`` spec, rounded
+    to ``W_h``'s dtype once; the gradient reaching ``W_h`` is ``M * s`` times the gradient of the masked matrix.  ``spec`` None or
+    P = 0: ``w_h`` itself."""
+    if spec is None or spec.p == 0:
+        return w_h
+    return dropout(w_h.unsqueeze(0), spec)[0]
+
+
 def lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths: Optional[torch.Tensor] = None, reverse: bool = False,
-                        dropout: Optional[DropoutSpec] = None):
+                        dropout: Optional[DropoutSpec] = None, weight_drop: Optional[DropoutSpec] = None):
     """Unrolled layer: ``x_seq [T,B,D]`` -> ``(h_seq [T,B,H], h_T, c_T)``.
 
     ``lengths`` (int32 ``[B]``, right padding): at a step ``t >= lengths[b]`` row ``b`` holds its state (``h_t = h_{t-1}``,
@@ -164,8 +186,12 @@ def lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths: Optional[torch.T
     ``nn.LSTM(bidirectional=True)`` on a packed sequence.
 
     ``dropout``: the first output is the dropped sequence (``dropout`` below) - the input of the next layer; the final state is
-    not dropped."""
+    not dropped.
+
+    ``weight_drop``: a ``weight`` ``DropoutSpec``; every step and row reads ``weight_drop(w_h, spec)`` in place of ``w_h``, built
+    inside autograd, so ``w_h`` gets the masked gradient."""
     T = x_seq.shape[0]
+    w_h = _weight_drop(w_h, weight_drop)
     keep = None
     if lengths is not None:
         check_lengths(lengths, x_seq.shape[1], T)
@@ -190,7 +216,8 @@ def lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths: Optional[torch.T
     return _dropout(torch.stack(outs, 0), dropout), h, c
 
 
-_dropout = dropout          # (lstm_layer_sequence's argument shadows the function)
+_dropout = dropout          # (lstm_layer_sequence's arguments shadow these functions)
+_weight_drop = weight_drop
 
 
 def dense_head(h, weights, bias):
