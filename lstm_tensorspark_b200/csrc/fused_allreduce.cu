@@ -265,7 +265,8 @@ extern "C" int ts_fused_allreduce(const unsigned long long* ptrs, unsigned long 
                                   long long n, int rank, int world, int mode, int two_shot, int multicast, int blocks,
                                   float lr, float b1, float b2, float eps, float wd, double timeout_s,
                                   cudaStream_t st, int* step_dev, long long wd_n, int bump_step, int pdl) {
-  if (world > kMaxRanks || world < 1 || n % 4 != 0) return -2;
+  // the decay is chosen per float4: a cut inside one would decay a different range than [0, wd_n)
+  if (world > kMaxRanks || world < 1 || n % 4 != 0 || (wd_n >= 0 && wd_n % 4 != 0)) return -2;
   if (blocks > kMaxBlocks) blocks = kMaxBlocks;
   if (blocks < 1) blocks = 1;
   ARArgs a;

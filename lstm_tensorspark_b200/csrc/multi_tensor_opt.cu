@@ -163,7 +163,7 @@ __global__ void __launch_bounds__(256) flat_grad_norm_kernel(const float4* __res
 extern "C" int ts_flat_adam(float* p, const float* g, float* m, float* v, void* shadow, long long n, float lr_t,
                             float b1, float b2, float eps, float wd, float gscale, cudaStream_t st, int* step_dev, long long wd_n,
                             const float* clip) {
-  if (n % 4) return -2;
+  if (n % 4 || (wd_n >= 0 && wd_n % 4)) return -2;       // the decay is chosen per float4: [0, wd_n) must end on one
   size_t n4 = (size_t)n / 4;
   if (step_dev) inc_step_kernel<<<1, 1, 0, st>>>(step_dev);
   auto kern = clip ? flat_adam_kernel<true> : flat_adam_kernel<false>;
@@ -174,7 +174,7 @@ extern "C" int ts_flat_adam(float* p, const float* g, float* m, float* v, void* 
 
 extern "C" int ts_flat_sgd(float* p, const float* g, void* shadow, long long n, float lr, float wd, float gscale,
                            cudaStream_t st, long long wd_n, const float* clip) {
-  if (n % 4) return -2;
+  if (n % 4 || (wd_n >= 0 && wd_n % 4)) return -2;
   size_t n4 = (size_t)n / 4;
   auto kern = clip ? flat_sgd_kernel<true> : flat_sgd_kernel<false>;
   kern<<<grid_for(n4), 256, 0, st>>>((float4*)p, (const float4*)g, (uint2*)shadow, n4, lr, wd, gscale,
@@ -189,7 +189,7 @@ extern "C" long long ts_flat_grad_norm_scratch(long long n) { return grid_for((s
 // out: fp32 [2] = {norm, coef}; p is read only when wd != 0.
 extern "C" int ts_flat_grad_norm(const float* g, const float* p, long long n, float wd, float gscale, long long wd_n, float max_norm,
                                  double* scratch, float* out, cudaStream_t st) {
-  if (n % 4) return -2;
+  if (n % 4 || (wd_n >= 0 && wd_n % 4)) return -2;
   size_t n4 = (size_t)n / 4;
   const int grid = grid_for(n4);
   flat_grad_norm_kernel<<<grid, 256, 0, st>>>((const float4*)g, (const float4*)p, n4, wd, gscale,

@@ -41,6 +41,19 @@ class FlatOptimizer:
             raise ValueError(f"unknown optimizer {kind!r}")
 
     @property
+    def wd_numel(self) -> int:
+        """Weight decay covers flat elements ``[0, wd_numel)``; -1 = all.  The update kernels choose the decay per float4, so
+        the cut is a multiple of 4 (``FlatParams.lstm_numel`` is one of ``ALIGN``)."""
+        return self._wd_numel
+
+    @wd_numel.setter
+    def wd_numel(self, value: int):
+        value = int(value)
+        if value < -1 or (value >= 0 and value % 4):
+            raise ValueError(f"wd_numel must be -1 or a non-negative multiple of 4, got {value}")
+        self._wd_numel = value
+
+    @property
     def clip_norm(self) -> float:
         """Clip the gradient by its global norm to this value before the update (0 = off).  The norm is that of the gradient
         the update uses - ``g * grad_scale`` plus the weight-decay term over ``[0, wd_numel)`` - and the update uses

@@ -128,6 +128,8 @@ class FusedComm(TorchDistComm):
         """One launch over elements [elem_off, elem_off + n) of the symmetric buffers (a gradient bucket or the whole message)."""
         E = ext()
         A = self.arena
+        # the kernel moves float4s: a bucket starts on one, and its clipped weight-decay cut below stays a multiple of 4
+        assert elem_off % 4 == 0, f"bucket offset {elem_off} is not a multiple of 4 elements"
         two_shot = (4 * n >= TWO_SHOT_BYTES) if force is None else (force == "two_shot")
         # NVLS (in-switch reduction) pays from 3 ranks up; with 2 ranks the peer-pointer kernel is faster stand-alone (measured:
         # measured) - but it needs 122 registers, so a bucket that has to squeeze onto the SMs a

@@ -2,6 +2,7 @@
 two-shot allreduce, the wavefront GEMM's gate configuration, the generation-gated bucket queue."""
 import types
 
+import pytest
 import torch
 
 from lstm_tensorspark_b200.models.flat import FlatParams
@@ -51,6 +52,23 @@ def test_owned_ranges_of_bucketed_two_shot_adam():
                 assert lo % 4 == 0 and hi % 4 == 0
                 covered[lo:hi] += 1
         assert bool((covered == 1).all())              # every Adam slot has exactly one owner (one-shot bucket: rank 0)
+
+
+def test_weight_decay_cut_is_whole_float4s():
+    """The update kernels choose the weight decay per float4, so ``FlatOptimizer.wd_numel`` is -1 or a multiple of 4; the
+    cut the engine sets (``FlatParams.lstm_numel``) is a multiple of ``ALIGN``."""
+    from lstm_tensorspark_b200.models.flat import ALIGN, FlatParams
+    from lstm_tensorspark_b200.ops.optim import FlatOptimizer
+    flat = FlatParams([torch.nn.Parameter(torch.zeros(10, 3))], [torch.nn.Parameter(torch.zeros(5))])
+    assert flat.lstm_numel % ALIGN == 0 and ALIGN % 4 == 0
+    opt = FlatOptimizer(flat, 0.1, "sgd", weight_decay=0.1)
+    for ok in (-1, 0, 4, flat.lstm_numel):
+        opt.wd_numel = ok
+        assert opt.wd_numel == ok
+    for bad in (-2, 2, 30):
+        with pytest.raises(ValueError, match="wd_numel"):
+            opt.wd_numel = bad
+    assert opt.wd_numel == flat.lstm_numel
 
 
 def test_wavefront_gate_configuration():
