@@ -77,7 +77,7 @@ int ts_dropout(const void*, void*, int, int, int, int, int, const int*, const un
 int ts_weight_drop_grad(const float*, float*, int, int, int, const int*, const unsigned int*, cudaStream_t);
 int ts_lstm_seq_prologue(const void*, const float*, void*, float*, void*, unsigned int*, int, int, cudaStream_t);
 int ts_seq_pool_fwd(const void*, int, const int*, const float*, int, int, int, int, float*, int*, cudaStream_t);
-int ts_seq_pool_attn_scores(float*, const float*, const float*, const int*, int, int, int, float*, cudaStream_t);
+int ts_seq_pool_attn_scores(float*, const float*, const float*, const int*, int, int, int, float*, int, cudaStream_t);
 int ts_seq_pool_attn_bwd(const void*, int, const float*, const float*, const float*, const float*, const int*, int, int, int, int,
                          float*, void*, float*, unsigned int*, float*, float*, int, int, cudaStream_t);
 int ts_seq_pool_bwd(const float*, const int*, const int*, const float*, const float*, int, int, int, int, void*, int, cudaStream_t);
@@ -605,7 +605,8 @@ std::vector<Tensor> seq_pool_fwd(const Tensor& h, const std::optional<Tensor>& l
 }
 
 // u fp32 [T·B, A]: h W_a in, tanh(h W_a + b_a) out (0 at uncounted steps) -> alpha fp32 [T,B], the softmax over counted steps.
-Tensor seq_pool_attn_scores(Tensor u, const Tensor& ba, const Tensor& v, const std::optional<Tensor>& lengths, int64_t T) {
+// exact: tanh in fp64 rounded once (fp32 h), else tanh.approx (bf16 h).
+Tensor seq_pool_attn_scores(Tensor u, const Tensor& ba, const Tensor& v, const std::optional<Tensor>& lengths, int64_t T, bool exact) {
   chk_cuda(u, "u");
   TORCH_CHECK(u.dim() == 2 && u.scalar_type() == torch::kFloat32 && T >= 1 && u.size(0) % T == 0, "seq_pool_attn_scores: u fp32 [T·B, A]");
   c10::cuda::CUDAGuard g(u.device());
@@ -613,7 +614,7 @@ Tensor seq_pool_attn_scores(Tensor u, const Tensor& ba, const Tensor& v, const s
   chk_f32(ba, A, "b_a"); chk_f32(v, A, "v");
   auto alpha = torch::empty({T, B}, u.options());
   check(ts_seq_pool_attn_scores(u.data_ptr<float>(), ba.data_ptr<float>(), v.data_ptr<float>(), lengths_ptr(lengths, B, u), (int)T, B, A,
-                                alpha.data_ptr<float>(), stream()), "seq_pool_attn_scores");
+                                alpha.data_ptr<float>(), (int)exact, stream()), "seq_pool_attn_scores");
   return alpha;
 }
 
@@ -1012,7 +1013,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("xent_rows", &xent_rows);
   m.def("head_fwd", &head_fwd);
   m.def("seq_pool_fwd", &seq_pool_fwd, py::arg("h"), py::arg("lengths"), py::arg("T"), py::arg("mode"), py::arg("alpha"));
-  m.def("seq_pool_attn_scores", &seq_pool_attn_scores, py::arg("u"), py::arg("b_a"), py::arg("v"), py::arg("lengths"), py::arg("T"));
+  m.def("seq_pool_attn_scores", &seq_pool_attn_scores, py::arg("u"), py::arg("b_a"), py::arg("v"), py::arg("lengths"), py::arg("T"),
+        py::arg("exact") = false);
   m.def("seq_pool_attn_bwd", &seq_pool_attn_bwd, py::arg("h"), py::arg("ds"), py::arg("alpha"), py::arg("u"), py::arg("v"),
         py::arg("lengths"), py::arg("T"), py::arg("dv"), py::arg("dba"), py::arg("acc_dv"), py::arg("acc_dba"));
   m.def("seq_pool_bwd", &seq_pool_bwd, py::arg("ds"), py::arg("lengths"), py::arg("T"), py::arg("mode"), py::arg("argmax"),

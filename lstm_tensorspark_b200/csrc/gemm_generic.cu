@@ -10,6 +10,7 @@ namespace {
 
 constexpr int GT = 32;     // output tile
 constexpr int GK = 16;     // k tile
+constexpr int GCHUNK = 64; // k tiles per partial sum
 
 template <typename TA, typename TB, typename TC>
 __global__ void __launch_bounds__(256) gemm_generic_kernel(const TA* __restrict__ A, const TB* __restrict__ B, TC* __restrict__ C,
@@ -18,8 +19,12 @@ __global__ void __launch_bounds__(256) gemm_generic_kernel(const TA* __restrict_
   __shared__ float sa[GK][GT + 1];
   __shared__ float sb[GK][GT + 1];
   const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;          // 16 x 16 threads, 2 x 2 outputs each
-  const int m0 = blockIdx.y * GT, n0 = blockIdx.x * GT;
-  float acc[2][2] = {{0.f, 0.f}, {0.f, 0.f}};
+  const int m0 = blockIdx.x * GT, n0 = blockIdx.y * GT;          // M on grid x (up to 2^31 - 1 blocks): M = T·B rows
+  // Long contractions (the weight gradients, K = T·B rows) are summed in three levels - GK products per k tile, GCHUNK k tiles
+  // per chunk, the chunks - so that the fp32 rounding error grows with about GK + GCHUNK + K / (GK·GCHUNK) terms instead of K.
+  // With K <= GK it is the plain fma chain.
+  float acc[2][2] = {{0.f, 0.f}, {0.f, 0.f}}, chunk[2][2] = {{0.f, 0.f}, {0.f, 0.f}};
+  int tiles = 0;
   for (int k0 = 0; k0 < K; k0 += GK) {
     for (int i = threadIdx.x; i < GK * GT; i += 256) {
       const int kk = i / GT, mm = i % GT;
@@ -29,14 +34,30 @@ __global__ void __launch_bounds__(256) gemm_generic_kernel(const TA* __restrict_
       sb[kk][mm] = (n < N && k < K) ? ts::Cvt<TB>::to_f(B[(long long)k * b_rs + (long long)n * b_cs]) : 0.f;
     }
     __syncthreads();
+    float part[2][2] = {{0.f, 0.f}, {0.f, 0.f}};
 #pragma unroll
     for (int kk = 0; kk < GK; ++kk) {
       const float a0 = sa[kk][ty], a1 = sa[kk][ty + 16], b0 = sb[kk][tx], b1 = sb[kk][tx + 16];
-      acc[0][0] = fmaf(a0, b0, acc[0][0]); acc[0][1] = fmaf(a0, b1, acc[0][1]);
-      acc[1][0] = fmaf(a1, b0, acc[1][0]); acc[1][1] = fmaf(a1, b1, acc[1][1]);
+      part[0][0] = fmaf(a0, b0, part[0][0]); part[0][1] = fmaf(a0, b1, part[0][1]);
+      part[1][0] = fmaf(a1, b0, part[1][0]); part[1][1] = fmaf(a1, b1, part[1][1]);
     }
     __syncthreads();
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+#pragma unroll
+      for (int j = 0; j < 2; ++j) chunk[i][j] += part[i][j];
+    if (++tiles == GCHUNK) {
+#pragma unroll
+      for (int i = 0; i < 2; ++i)
+#pragma unroll
+        for (int j = 0; j < 2; ++j) { acc[i][j] += chunk[i][j]; chunk[i][j] = 0.f; }
+      tiles = 0;
+    }
   }
+#pragma unroll
+  for (int i = 0; i < 2; ++i)
+#pragma unroll
+    for (int j = 0; j < 2; ++j) acc[i][j] += chunk[i][j];
 #pragma unroll
   for (int i = 0; i < 2; ++i)
 #pragma unroll
@@ -54,7 +75,7 @@ __global__ void __launch_bounds__(256) gemm_generic_kernel(const TA* __restrict_
 template <typename TA, typename TB, typename TC>
 int launch_g(const void* A, const void* B, void* C, const float* bias, int M, int N, int K, long long a_rs, long long a_cs, long long b_rs,
              long long b_cs, long long c_rs, float beta, cudaStream_t st) {
-  dim3 grid((N + GT - 1) / GT, (M + GT - 1) / GT);
+  dim3 grid((M + GT - 1) / GT, (N + GT - 1) / GT);
   gemm_generic_kernel<TA, TB, TC><<<grid, 256, 0, st>>>((const TA*)A, (const TB*)B, (TC*)C, bias, M, N, K, a_rs, a_cs, b_rs, b_cs, c_rs, beta);
   return (int)cudaGetLastError();
 }

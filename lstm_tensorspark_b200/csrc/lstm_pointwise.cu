@@ -4,6 +4,8 @@
 // The 4-gate GEMM that feeds them is a library GEMM on this path; shapes that fit the tensor-core tiling
 // take the persistent wgmma kernel in lstm_seq_wgmma.cu instead.
 //
+// kFast (bf16): tanh.approx activations, within the bf16 storage's error; fp32 (kFast = false) computes them in fp64 and rounds
+// once (ts::tanhf_acc / sigmoidf_acc), so the fp32 path is as accurate as fp32 storage.
 // Layout: pre/act/dpre are [B, 4H] with column n = 4*j + g, g: 0=i 1=f 2=g(candidate) 3=o. c is fp32.
 // kMasked (per-row lengths, right padding): at step t >= lengths[b] row b holds its state - forward h_t = h_{t-1}, c_t = c_{t-1};
 // backward dpre = 0, dc passes through and the total dh is handed on (dh_out) instead of going through W_h.
@@ -36,10 +38,10 @@ __global__ void lstm_pointwise_fwd_kernel(const T* __restrict__ pre, const float
   if (kFast) {
     i = ts::sigmoidf_fast(pi); f = ts::sigmoidf_fast(pf); g = ts::tanhf_fast(pg); o = ts::sigmoidf_fast(po);
   } else {
-    i = ts::sigmoidf_acc(pi); f = ts::sigmoidf_acc(pf); g = tanhf(pg); o = ts::sigmoidf_acc(po);
+    i = ts::sigmoidf_acc(pi); f = ts::sigmoidf_acc(pf); g = ts::tanhf_acc(pg); o = ts::sigmoidf_acc(po);
   }
   float c = f * c_prev[idx] + i * g;
-  float h = o * (kFast ? ts::tanhf_fast(c) : tanhf(c));
+  float h = o * (kFast ? ts::tanhf_fast(c) : ts::tanhf_acc(c));
   c_out[idx] = c;
   h_out[idx] = ts::Cvt<T>::from_f(h);
   T* a = act + (size_t)idx * 4;
@@ -74,7 +76,7 @@ __global__ void lstm_pointwise_bwd_kernel(const T* __restrict__ dh_a, const floa
   const T* a = act + (size_t)idx * 4;
   float i = ts::Cvt<T>::to_f(a[0]), f = ts::Cvt<T>::to_f(a[1]);
   float g = ts::Cvt<T>::to_f(a[2]), o = ts::Cvt<T>::to_f(a[3]);
-  float tc = kFast ? ts::tanhf_fast(c_new[idx]) : tanhf(c_new[idx]);
+  float tc = kFast ? ts::tanhf_fast(c_new[idx]) : ts::tanhf_acc(c_new[idx]);
   float dc = (dc_in ? dc_in[idx] : 0.f) + dh * o * (1.f - tc * tc);
   float d_o = dh * tc;
   float d_i = dc * g, d_f = dc * c_prev[idx], d_g = dc * i;

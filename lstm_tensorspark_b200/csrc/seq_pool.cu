@@ -71,7 +71,9 @@ __global__ void __launch_bounds__(kThreads) seq_pool_fwd_kernel(const TIn* __res
 }
 
 // Attention scores, one CTA per batch row b.  u [T·B, A]: in h W_a (fp32), out tanh(h W_a + b_a) at counted steps, 0 at the
-// others.  alpha [T,B]: first e_t, then the softmax weights (0 at uncounted steps).
+// others.  alpha [T,B]: first e_t, then the softmax weights (0 at uncounted steps).  kExact (fp32 h): tanh in fp64, rounded once
+// (ts::tanhf_acc); otherwise tanh.approx, within the bf16 path's error.
+template <bool kExact>
 __global__ void __launch_bounds__(kThreads) attn_scores_kernel(float* __restrict__ u, const float* __restrict__ ba,
                                                                const float* __restrict__ v, const int* __restrict__ lengths,
                                                                int T, int B, int A, float* __restrict__ alpha) {
@@ -87,7 +89,7 @@ __global__ void __launch_bounds__(kThreads) attn_scores_kernel(float* __restrict
     }
     float e = 0.f;
     for (int k = lane; k < A; k += 32) {
-      const float x = tanhf(row[k] + ba[k]);
+      const float x = kExact ? ts::tanhf_acc(row[k] + ba[k]) : ts::tanhf_fast(row[k] + ba[k]);
       row[k] = x;
       e = fmaf(x, v[k], e);
     }
@@ -232,9 +234,12 @@ extern "C" int ts_seq_pool_fwd(const void* h, int h_bf16, const int* lengths, co
 }
 
 extern "C" int ts_seq_pool_attn_scores(float* u, const float* ba, const float* v, const int* lengths, int T, int B, int A,
-                                       float* alpha, cudaStream_t st) {
+                                       float* alpha, int exact, cudaStream_t st) {
   if (T < 1 || B < 1 || A < 1) return -2;
-  attn_scores_kernel<<<B, kThreads, 0, st>>>(u, ba, v, lengths, T, B, A, alpha);
+  if (exact)
+    attn_scores_kernel<true><<<B, kThreads, 0, st>>>(u, ba, v, lengths, T, B, A, alpha);
+  else
+    attn_scores_kernel<false><<<B, kThreads, 0, st>>>(u, ba, v, lengths, T, B, A, alpha);
   return (int)cudaGetLastError();
 }
 

@@ -15,8 +15,11 @@ TS_DEVICE float tanhf_fast(float x) {
 }
 // sigmoid(x) = 0.5*tanh(0.5x)+0.5 : ONE MUFU op (tanh.approx) instead of ex2 + rcp
 TS_DEVICE float sigmoidf_fast(float x) { return fmaf(0.5f, tanhf_fast(0.5f * x), 0.5f); }
-// accurate variants for the fp32 parity path
-TS_DEVICE float sigmoidf_acc(float x) { return 1.0f / (1.0f + expf(-x)); }
+// Accurate variants for the fp32 path: computed in fp64 and rounded once.  build.py compiles with --use_fast_math, which turns
+// the fp32 tanhf / expf / division into tanh.approx / ex2.approx / rcp.approx (relative error up to about 2^-11, no better than
+// bf16); it leaves fp64 math alone.
+TS_DEVICE float tanhf_acc(float x) { return (float)tanh((double)x); }
+TS_DEVICE float sigmoidf_acc(float x) { return (float)(1.0 / (1.0 + exp(-(double)x))); }
 
 template <typename T> struct Cvt;
 template <> struct Cvt<float> {

@@ -40,7 +40,7 @@ class _PoolFn(torch.autograd.Function):
             wa = _lowp(w_a, torch.bfloat16) if h2.dtype == torch.bfloat16 else w_a.detach().float().contiguous()
             ba, vv = b_a.detach().float().contiguous(), v.detach().float().contiguous()
             u = cuda_gemm.matmul(h2, wa.t(), out_dtype=torch.float32)          # h W_a [T·B, A]; tanh(. + b_a) in place below
-            alpha = E.seq_pool_attn_scores(u, ba, vv, ln, T)
+            alpha = E.seq_pool_attn_scores(u, ba, vv, ln, T, exact=h2.dtype == torch.float32)
             s, _ = E.seq_pool_fwd(h2, ln, T, m, alpha)
             _count("pool_attention_fwd")
             ctx.save_for_backward(h2, alpha, u, wa, vv)

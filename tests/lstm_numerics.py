@@ -4,10 +4,15 @@
 T = 512, B = 64, H = 2048 a single fp64 [T, B, 4H] tensor is 2.1 GB, and the rounding points sit inside the backward):
   * ``rounding=None``: fp64 - the exact result of the operation on the inputs the kernels get;
   * ``rounding=Bf16(...)``: fp32 with every bf16 rounding of the fast path in its place - what an ideal kernel with those
-    rounding points computes.  Its distance from fp64 is the error the bf16 storage alone explains.
-``check_budget`` then holds a kernel's error against fp64 to ALPHA x the emulation's error (plus a small floor), per time step
-for the sequences, so that a defect confined to one step of hundreds cannot hide in a global norm.  ``model`` composes the
-layers into the whole classifier (stacked, bidirectional, dropout, head) with the same two arms.
+    rounding points computes.  Its distance from fp64 is the error the bf16 storage alone explains;
+  * ``rounding=Generic()``: the same for the bf16 generic path (H % 64 != 0 and other shapes the persistent kernels do not
+    take: a CUDA-core GEMM per time step and the fused cell kernels of csrc/lstm_pointwise.cu);
+  * ``rounding=Fp32()``: the fp32 generic path (``--dtype fp32``) - every operation in fp32, nothing rounded to bf16, exact
+    activations.
+``check_budget`` then holds a kernel's error against fp64 to ALPHA x the emulation's error (plus a small floor: FLOOR for the
+bf16 arms, FLOOR_F32 for the fp32 one), per time step for the sequences, so that a defect confined to one step of hundreds
+cannot hide in a global norm.  ``model`` composes the layers into the whole classifier (stacked, bidirectional, dropout, head)
+with the same arms.
 
 Rounding points of the fast path (ops/cuda_lstm.py, csrc/lstm_seq_wgmma.cu), all round-to-nearest-even:
   forward   gx = x W_x^T is stored bf16 (_gemm_tn); with the forward K-split (cluster of 2) a member adds the PEER's half of the
@@ -18,6 +23,16 @@ Rounding points of the fast path (ops/cuda_lstm.py, csrc/lstm_seq_wgmma.cu), all
             fp32; the cell backward reads the bf16 activations and fp32 c, and stores dG as bf16; dW_x / dW_h are fp32 products
             of bf16 operands, db the fp32 column sum of the bf16 dG, dx = dG W_x is stored bf16.
   pair      h_seq of layer a (bf16) is layer b's input; dx of layer b (bf16) is layer a's dh_seq (ops/cuda_lstm._LSTMPairFn).
+
+Rounding points of the bf16 generic path (ops/cuda_lstm._LSTMSeqFn with ``fast_path_supported`` false), where they differ:
+  forward   pre = bf16(gx + h W_h^T): the GEMM adds the fp32 product to the bf16 gx in fp32 and stores the bf16 pre buffer,
+            the fp32 bias is added to it afterwards by the cell kernel; no forward K-split;
+  backward  the recurrent product dG W_h is fp32 and never rounded (the fp32 output of the GEMM, or accumulated into the fp32
+            dh handed to the step before); gx, the activations, h, dG and dx are bf16 and c fp32 as on the fast path;
+  dropout   the standalone dropout kernel masks the output (bf16(h x scale), as the fast path) and the incoming gradient,
+            which it stores as bf16(dh x scale) before the cell kernel reads it.
+The fp32 generic path has no rounding point besides fp32 arithmetic: its GEMMs accumulate in fp32 into fp32 outputs, and its
+cell kernels compute the activations in fp64 and round them once (csrc/ts_common.cuh tanhf_acc / sigmoidf_acc).
 
 The optimizer update (csrc/multi_tensor_opt.cu, TF-1.0 Adam with "epsilon-hat" or SGD over the flat fp32 master buffer) has no
 bf16 rounding point and no emulation arm: ``adam_update`` / ``sgd_update`` compute it in fp64 from the kernel's own fp32
@@ -56,6 +71,10 @@ ALPHA = 2.0
 # <= 2^-11; sigmoid(x) = 0.5 tanh(x / 2) + 0.5).  One step's h = o * tanh(c) carries two such approximations, so a kernel
 # that is exact up to them may sit 2 x 2^-11 away from the emulation where the emulation itself happens to be exact.
 FLOOR = 2.0 * 2.0 ** -11
+# The fp32 path's floor: its activations are correctly rounded up to a last-bit error, so the floor only has to absorb fp32
+# rounding of a different order than the emulation's where the emulation happens to be close to fp64 - a few ulp.  A kernel
+# whose tanh were off by 2^-15 (let alone tanh.approx's 2^-11) exceeds it.
+FLOOR_F32 = 2.0 ** -20
 
 
 @dataclasses.dataclass(frozen=True)
@@ -74,6 +93,21 @@ class Bf16:
         fwd = ext().lstm_seq_config(False, H, B, variant)
         bwd = ext().lstm_seq_config(True, H, B, variant)
         return cls(fwd_split=2 if fwd[3] else 1, bwd_split=2 if bwd[2] else 4)
+
+
+@dataclasses.dataclass(frozen=True)
+class Generic:
+    """The bf16 generic path's rounding (module docstring).  ``approx``: as ``Bf16.approx``."""
+    approx: float = 0.0
+
+
+@dataclasses.dataclass(frozen=True)
+class Fp32:
+    """The fp32 generic path: fp32 arithmetic, no bf16 rounding, exact sigmoid and tanh.  ``split``: the recurrent products
+    as the fp32 sum of that many K parts (another order of the same fp32 sums); ``approx``: as ``Bf16.approx`` - both only for
+    stand-ins of a kernel in tests of this module."""
+    split: int = 1
+    approx: float = 0.0
 
 
 @dataclasses.dataclass(frozen=True)
@@ -103,19 +137,27 @@ class LayerOut(NamedTuple):
     db: torch.Tensor
 
 
-def _round(r: Optional[Bf16], x: torch.Tensor) -> torch.Tensor:
-    return x if r is None else x.to(torch.bfloat16).to(x.dtype)
+def _round(r, x: torch.Tensor) -> torch.Tensor:
+    return x if r is None or isinstance(r, Fp32) else x.to(torch.bfloat16).to(x.dtype)
 
 
-def _tanh(r: Optional[Bf16], x: torch.Tensor) -> torch.Tensor:
+def _tanh(r, x: torch.Tensor) -> torch.Tensor:
     y = torch.tanh(x)
     if r is not None and r.approx:
         y = y * (1.0 + r.approx * torch.sin(x * 4099.0))
     return y
 
 
-def _sigmoid(r: Optional[Bf16], x: torch.Tensor) -> torch.Tensor:
-    return torch.sigmoid(x) if r is None else 0.5 * _tanh(r, 0.5 * x) + 0.5
+def _sigmoid(r, x: torch.Tensor) -> torch.Tensor:
+    if r is None or (isinstance(r, Fp32) and not r.approx):
+        return torch.sigmoid(x)
+    return 0.5 * _tanh(r, 0.5 * x) + 0.5
+
+
+def _split_mm(a, b, parts):
+    """a @ b as the fp32 sum of ``parts`` products over K slices (Fp32.split)."""
+    q = -(-a.shape[1] // parts)
+    return sum(a[:, s:s + q] @ b[s:s + q] for s in range(0, a.shape[1], q))
 
 
 def _keep(lengths, T, B, device):
@@ -127,7 +169,9 @@ def _keep(lengths, T, B, device):
 def _rec_fwd(r, h, w_h):
     """h_{t-1} W_h^T.  Forward K-split: gate column n belongs to cluster member m = (n % 128) // 64, which contracts K half m
     itself (fp32) and receives the other half from its peer as bf16."""
-    if r is None or r.fwd_split == 1:
+    if isinstance(r, Fp32) and r.split > 1:
+        return _split_mm(h, w_h.t(), r.split)
+    if r is None or not isinstance(r, Bf16) or r.fwd_split == 1:
         return h @ w_h.t()
     hk = h.shape[1] // 2
     p0 = h[:, :hk] @ w_h[:, :hk].t()
@@ -137,8 +181,11 @@ def _rec_fwd(r, h, w_h):
 
 
 def _rec_bwd(r, dg, w_h):
-    """dG W_h: ``bwd_split`` fp32 partial sums over K quarters / halves, each rounded to bf16, summed in fp32."""
-    if r is None:
+    """dG W_h: ``bwd_split`` fp32 partial sums over K quarters / halves, each rounded to bf16, summed in fp32 (the fast path);
+    one fp32 product, not rounded (the generic paths)."""
+    if isinstance(r, Fp32) and r.split > 1:
+        return _split_mm(dg, w_h, r.split)
+    if r is None or not isinstance(r, Bf16):
         return dg @ w_h
     q = dg.shape[1] // r.bwd_split
     out = None
@@ -171,7 +218,10 @@ def _forward(x, h0, c0, w_x, w_h, bias, keep, reverse, r, defect):
             else:
                 rows = slice(ROWS * defect.index, ROWS * (defect.index + 1))
                 hin[rows] = h_before[rows]
-        pre = (_rec_fwd(r, hin, w_h) + gx[t] + bias).view(B, H, 4)
+        rec = _rec_fwd(r, hin, w_h) + gx[t]
+        if isinstance(r, Generic):
+            rec = _round(r, rec)                      # the GEMM's bf16 output buffer, before the cell kernel adds the bias
+        pre = (rec + bias).view(B, H, 4)
         i, f = _sigmoid(r, pre[..., 0]), _sigmoid(r, pre[..., 1])
         g, o = _tanh(r, pre[..., 2]), _sigmoid(r, pre[..., 3])
         c_new = f * c + i * g
@@ -204,6 +254,8 @@ def _backward(fw, x, w_x, w_h, dh_seq, dh_T, dc_T, keep, reverse, r, defect, dh_
             dht = dh
         elif dh_scale is None:
             dht = dh + _round(r, dh_seq[t].to(dt))
+        elif isinstance(r, Generic):                  # the standalone dropout kernel stores bf16(dh_seq x mask x scale)
+            dht = dh + _round(r, _round(r, dh_seq[t].to(dt)) * dh_scale[t])
         else:
             dht = dh + _round(r, dh_seq[t].to(dt)) * dh_scale[t]
         i, f, g, o = acts[t].unbind(-1)
@@ -399,7 +451,7 @@ def check_budget(name: str, got: torch.Tensor, fp64: torch.Tensor, emulated: tor
     if not worst <= 1.0:
         where = f" at step {s}" if per_step else ""
         raise AssertionError(
-            f"{name}{where}: error vs fp64 {float(ek[s]):.3e} exceeds {alpha} x the bf16 emulation's {float(ee[s]):.3e} + "
+            f"{name}{where}: error vs fp64 {float(ek[s]):.3e} exceeds {alpha} x the emulation's {float(ee[s]):.3e} + "
             f"{floor:.2e} x |fp64| {float(sc[s]):.3e} (ratio {worst:.2f}; kernel / emulation error "
             f"{float(ek[s]) / max(float(ee[s]), 1e-300):.2f})")
     return worst

@@ -35,15 +35,18 @@ def _stats():
     return {k: cuda_lstm.STATS.get(k, 0) for k in KEYS}
 
 
-def _engine(**kw):
+def _engine(dtype=torch.bfloat16, **kw):
+    """A one-rank engine computing in ``dtype``: bf16 (weights made bf16-representable, so that learning rate 0 keeps the
+    shadow exact) or fp32 (``--dtype fp32``: the kernels read the fp32 master itself; the weights are left as initialised)."""
     from lstm_tensorspark_b200.config import Config
     from lstm_tensorspark_b200.engine import TrainEngine
     cfg = Config(partitions=1, sync_mode="none", init="scaled", device="cuda", quiet=True, backend="auto",
                  **{"learning_rate": 0.0, **kw})
-    eng = TrainEngine(cfg, 0, 1, None, batch_size=cfg.batch_size, device=DEV, dtype=torch.bfloat16)
-    with torch.no_grad():
-        eng.flat.data.copy_(eng.flat.data.bfloat16().float())         # bf16-representable initial weights
-        eng.flat.refresh_shadow()
+    eng = TrainEngine(cfg, 0, 1, None, batch_size=cfg.batch_size, device=DEV, dtype=dtype)
+    if dtype == torch.bfloat16:
+        with torch.no_grad():
+            eng.flat.data.copy_(eng.flat.data.bfloat16().float())     # bf16-representable initial weights
+            eng.flat.refresh_shadow()
     return eng
 
 
@@ -91,9 +94,10 @@ def _segments(eng, names):
     return {names[id(p)]: (o, p.shape) for p, o in zip(eng.flat.params, eng.flat.offsets)}
 
 
-def _reference_params(eng, seg, data, dt):
+def _reference_params(eng, seg, data, dt, bf16_weights=True):
     """The weights a step reads, from ``data`` (a snapshot of the fp32 master buffer): W_x / W_h rounded to bf16 here (the
-    kernels read them from the shadow), the rest fp32.  Initial states that are not learned are the layers' zero buffers."""
+    kernels read them from the shadow; ``bf16_weights=False``: an fp32 engine, which reads the master), the rest fp32.  Initial
+    states that are not learned are the layers' zero buffers."""
     rnn = eng.model.rnn
 
     def get(name, k, lay):
@@ -101,7 +105,7 @@ def _reference_params(eng, seg, data, dt):
             return getattr(lay, k).detach().to(dt)
         o, shape = seg[f"{name}/{k}"]
         t = data[o:o + shape.numel()].view(shape)
-        return (t.bfloat16() if k in ("w_x", "w_h") else t).to(dt)
+        return (t.bfloat16() if bf16_weights and k in ("w_x", "w_h") else t).to(dt)
 
     def one(l, lay):
         name = f"LSTMLayer{l}" + ("_reverse" if lay.reverse else "")
@@ -135,7 +139,7 @@ def _load_resumed_state(eng, step, seed):
 
 def _model_case(case, hidden, T, B, D, per_step, steps=STEPS, lengths_seed=None, bidirectional=False, dropout=0.0,
                 learn_initial_state=False, free_engine=False, learning_rate=0.0, optimizer="adam", weight_decay=0.0,
-                graph=False, resume_at=None, stale_shadow=False):
+                graph=False, resume_at=None, stale_shadow=False, dtype=torch.bfloat16, rounding=None, weight_drop=0.0):
     """One training step after the other, each checked against the weights it read:
       * before the step: the bf16 shadow is the master rounded to nearest even, bit for bit;
       * the loss, h_T (eval mode, computed before the step) and every gradient of the flat buffer within the budget of the fp64
@@ -146,19 +150,25 @@ def _model_case(case, hidden, T, B, D, per_step, steps=STEPS, lengths_seed=None,
     ``per_step``: the STATS deltas one training step must show (the path the case targets).  ``graph``: the step is captured
     once (on the first batch; STATS count only there) and replayed on every batch.  ``resume_at``: the run starts from a state
     loaded as a resumed run would at that step.  ``stale_shadow``: the shadow of the weights before step 1 is put back after
-    it, standing in for a missing refresh (the shadow assertion is off): step 2's check must raise."""
+    it, standing in for a missing refresh (the shadow assertion is off): step 2's check must raise.
+    ``dtype``: the engine's compute dtype; fp32 checks against the ``lstm_numerics.Fp32`` arm with the fp32 floor, and reads
+    unrounded weights.  ``rounding``: the emulation arm's rounding in place of the fast path's (the bf16 generic path).
+    ``weight_drop``: P of --weight_drop; both arms read the masked W_h of the step and mask its gradient."""
     from lstm_tensorspark_b200 import data as Dm
     from lstm_tensorspark_b200.models.flat import ALIGN
     from lstm_tensorspark_b200.ops import cuda_lstm
     hs = [int(h) for h in hidden.split(",")]
-    eng = _engine(hidden_units=hidden, in_features=D, seq_len=T, batch_size=B, num_classes=C, bidirectional=bidirectional,
+    from lstm_tensorspark_b200.ops import reference as ops_ref
+    from test_gpu_weight_drop import _masked_grad
+    bf16 = dtype == torch.bfloat16
+    eng = _engine(dtype, hidden_units=hidden, in_features=D, seq_len=T, batch_size=B, num_classes=C, bidirectional=bidirectional,
                   dropout=dropout, learn_initial_state=learn_initial_state, variable_length=lengths_seed is not None,
-                  learning_rate=learning_rate, optimizer=optimizer, weight_decay=weight_decay)
+                  learning_rate=learning_rate, optimizer=optimizer, weight_decay=weight_decay, weight_drop=weight_drop)
     flat, opt = eng.flat, eng.optimizer
     if resume_at is not None:
         _load_resumed_state(eng, resume_at, seed=3)
     xs, ys = Dm.synthetic_sequences(steps * B, T, D, C, seed=5)
-    xs, ys = torch.as_tensor(xs).to(DEV).bfloat16(), torch.as_tensor(ys).to(DEV)
+    xs, ys = torch.as_tensor(xs).to(DEV).to(dtype), torch.as_tensor(ys).to(DEV)
     names = _names(eng)
     assert len(names) == len(flat.params)
     seg = _segments(eng, names)
@@ -170,7 +180,9 @@ def _model_case(case, hidden, T, B, D, per_step, steps=STEPS, lengths_seed=None,
     for o, shape in seg.values():
         real[o:o + shape.numel()] = True
     adam = optimizer == "adam"
-    rounding = _roundings(hs, T, B, D, bidirectional)
+    if rounding is None:
+        rounding = _roundings(hs, T, B, D, bidirectional) if bf16 else N.Fp32()
+    floor = N.FLOOR if bf16 else N.FLOOR_F32
     t0 = opt.step_count
     drop0 = int(eng.model.rnn.dropout_step)
     worst, worst_update = {}, 0.0
@@ -178,10 +190,11 @@ def _model_case(case, hidden, T, B, D, per_step, steps=STEPS, lengths_seed=None,
         x, y = xs[s * B:(s + 1) * B], ys[s * B:(s + 1) * B]
         lengths = None if lengths_seed is None else _lengths(T, B, lengths_seed + s)
         before = {"p": flat.data.clone(), "m": opt.m.clone() if adam else None, "v": opt.v.clone() if adam else None,
-                  "shadow": flat.shadow.clone(), "t": int(opt.step_dev), "drop": int(eng.model.rnn.dropout_step)}
-        if not stale_shadow:
+                  "shadow": None if flat.shadow is None else flat.shadow.clone(), "t": int(opt.step_dev),
+                  "drop": int(eng.model.rnn.dropout_step)}
+        if not stale_shadow and bf16:
             N.check_shadow(f"{case} before step {s}", flat.shadow, flat.data)
-        assert before["drop"] == drop0 + (s if dropout > 0 else 0), (case, s, before["drop"])
+        assert before["drop"] == drop0 + (s if dropout > 0 or weight_drop > 0 else 0), (case, s, before["drop"])
         assert not adam or before["t"] == t0 + s, (case, s, before["t"])
         eng.model.eval()
         with torch.no_grad():
@@ -229,14 +242,27 @@ def _model_case(case, hidden, T, B, D, per_step, steps=STEPS, lengths_seed=None,
             del loss, h_T
             torch.cuda.empty_cache()
         drop = N.Dropout(dropout, eng.model.rnn.dropout_key, before["drop"]) if dropout > 0 else None
+        wspecs = {}
+        if weight_drop > 0:
+            for l in range(len(hs)):
+                for rev in ((False, True) if bidirectional else (False,)):
+                    wspecs[f"LSTMLayer{l}" + ("_reverse" if rev else "")] = ops_ref.DropoutSpec(
+                        weight_drop, eng.model.rnn.dropout_key, l, rev, before["drop"], weight=True)
         with torch.no_grad():
             arms = {}
             for arm, dt, r in (("fp64", torch.float64, None), ("emu", torch.float32, rounding)):
-                layers, head = _reference_params(eng, seg, before["p"], dt)
+                layers, head = _reference_params(eng, seg, before["p"], dt, bf16_weights=bf16)
+                raw = layers                                        # eval mode: no dropout, no weight drop
+                if wspecs:                                          # W_h * M * s of the step, from the weights the kernels read
+                    mask = lambda p, n: (*p[:3], ops_ref.weight_drop(p[3].to(dtype), wspecs[n]).to(dt), p[4])
+                    layers = [(mask(p[0], f"LSTMLayer{l}"), mask(p[1], f"LSTMLayer{l}_reverse")) if bidirectional
+                              else mask(p, f"LSTMLayer{l}") for l, p in enumerate(layers)]
                 kw = dict(lengths=lengths, bidirectional=bidirectional, rounding=r)
                 full = N.model(x.to(dt), layers, head, y, dropout=drop, **kw)
-                h_eval = full.h_T if drop is None else N.model(x.to(dt), layers, head, y, backward=False, **kw).h_T
+                h_eval = full.h_T if drop is None and not wspecs else N.model(x.to(dt), raw, head, y, backward=False, **kw).h_T
                 arms[arm] = {"loss": full.loss, "h_T": h_eval, **full.grads}
+                for n, sp in wspecs.items():
+                    arms[arm][f"{n}/w_h"] = _masked_grad(arms[arm][f"{n}/w_h"], sp)
                 for k in decayed:                                       # the L2 term of create_variable
                     o, shape = seg[k]
                     if k.split("/")[1] in ("h0", "c0"):                 # ... through autograd: in the gradient
@@ -245,14 +271,14 @@ def _model_case(case, hidden, T, B, D, per_step, steps=STEPS, lengths_seed=None,
             l2 = sum(N.f32(weight_decay) * 0.5 * float((before["p"][o:o + sh.numel()].double() ** 2).sum())
                      for o, sh in (seg[k] for k in decayed))
             got["loss"] = got["loss"].double() - l2                     # the reported loss includes the L2 value
-            ratios = {k: N.check_budget(f"{case} step {s} {k}", g, arms["fp64"][k], arms["emu"][k], per_step=k == "h_T")
-                      for k, g in got.items()}
+            ratios = {k: N.check_budget(f"{case} step {s} {k}", g, arms["fp64"][k], arms["emu"][k], per_step=k == "h_T",
+                                        floor=floor) for k, g in got.items()}
             del arms
         for k, v in ratios.items():
             worst[k] = max(worst.get(k, 0.0), v)
     top = sorted(worst.items(), key=lambda kv: -kv[1])[:4]
     print(f"\n{case}: worst budget ratio {top[0][1]:.3f} over {steps} steps (" + ", ".join(f"{k} {v:.3f}" for k, v in top) +
-          f"); alpha {N.ALPHA}, floor {N.FLOOR:.2e}; worst update ratio {worst_update:.3f}")
+          f"); alpha {N.ALPHA}, floor {floor:.2e}; worst update ratio {worst_update:.3f}")
 
 
 def _sched(T, B, D, ha, hb):

@@ -250,8 +250,9 @@ def test_head_op_against_fp64(T, B, H, Cn, ragged, dtype):
         arms[arm] = {"logits": lg, "loss": l_, "dh": N._round(rr, dh_ * 0.37) if rr is not None else dh_ * 0.37,
                      "dW": dW_ * 0.37, "db": db_ * 0.37}
     got = {"logits": logits, "loss": loss, "dh": dh, "dW": dW, "db": db}
+    floor = N.FLOOR if dtype == torch.bfloat16 else N.FLOOR_F32
     for k, v in got.items():
-        N.check_budget(f"head T={T} B={B} C={Cn} {k}", v, arms["fp64"][k], arms["emu"][k], per_step=k == "logits")
+        N.check_budget(f"head T={T} B={B} C={Cn} {k}", v, arms["fp64"][k], arms["emu"][k], per_step=k == "logits", floor=floor)
     pred = logits.argmax(2)
     assert int(correct) == int(((pred == labels) & keep).sum())
     if lengths is not None:

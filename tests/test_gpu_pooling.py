@@ -163,20 +163,22 @@ def _pool_names(eng):
 
 
 def _case(case, mode, hidden, T, B, D, path, steps=2, lengths_seed=None, bidirectional=False, dropout=0.0, learning_rate=0.0,
-          graph=False, negative=False, A=128):
+          graph=False, negative=False, A=128, dtype=torch.bfloat16):
     """Training steps, each checked (loss and every gradient of the flat buffer) against the fp64 reference at the weights it
     read.  ``path``: a STATS key one step must bump (besides the pooling launches).  ``graph``: captured on the first batch and
     replayed on every batch, each with lengths of its own.  ``negative``: the reference (both arms) takes the mean over T - the
-    check must fail."""
+    check must fail.  ``dtype``: the engine's compute dtype (fp32: the lstm_numerics.Fp32 arm and floor)."""
     from lstm_tensorspark_b200 import data as Dm
-    eng = _engine(hidden_units=hidden, in_features=D, seq_len=T, batch_size=B, num_classes=C, bidirectional=bidirectional,
+    bf16 = dtype == torch.bfloat16
+    eng = _engine(dtype, hidden_units=hidden, in_features=D, seq_len=T, batch_size=B, num_classes=C, bidirectional=bidirectional,
                   dropout=dropout, variable_length=lengths_seed is not None, learning_rate=learning_rate, pooling=mode,
                   attention_units=A)
     flat = eng.flat
     xs, ys = Dm.synthetic_sequences(steps * B, T, D, C, seed=5)
-    xs, ys = torch.as_tensor(xs).to(DEV).bfloat16(), torch.as_tensor(ys).to(DEV)
+    xs, ys = torch.as_tensor(xs).to(DEV).to(dtype), torch.as_tensor(ys).to(DEV)
     seg = _segments(eng, _pool_names(eng))
-    rounding = _roundings([int(h) for h in hidden.split(",")], T, B, D, bidirectional)
+    rounding = _roundings([int(h) for h in hidden.split(",")], T, B, D, bidirectional) if bf16 else N.Fp32()
+    floor = N.FLOOR if bf16 else N.FLOOR_F32
     worst = {}
     for s in range(steps):
         x, y = xs[s * B:(s + 1) * B], ys[s * B:(s + 1) * B]
@@ -198,7 +200,7 @@ def _case(case, mode, hidden, T, B, D, path, steps=2, lengths_seed=None, bidirec
         with torch.no_grad():
             arms = {}
             for arm, dt, r in (("fp64", torch.float64, None), ("emu", torch.float32, rounding)):
-                layers, head = _reference_params(eng, seg, before["p"], dt)
+                layers, head = _reference_params(eng, seg, before["p"], dt, bf16_weights=bf16)
                 att = None
                 if mode == "attention":
                     att = tuple(before["p"][o:o + sh.numel()].view(sh).to(dt)
@@ -212,7 +214,8 @@ def _case(case, mode, hidden, T, B, D, path, steps=2, lengths_seed=None, bidirec
                 return
             assert set(got) <= set(arms["fp64"]) and (mode != "attention" or "Attention/context" in got), sorted(got)
             for k, g in got.items():
-                worst[k] = max(worst.get(k, 0.0), N.check_budget(f"{case} step {s} {k}", g, arms["fp64"][k], arms["emu"][k]))
+                worst[k] = max(worst.get(k, 0.0), N.check_budget(f"{case} step {s} {k}", g, arms["fp64"][k], arms["emu"][k],
+                                                                 floor=floor))
             del arms
     top = sorted(worst.items(), key=lambda kv: -kv[1])[:3]
     print(f"\n{case}: worst budget ratio " + ", ".join(f"{k} {v:.3f}" for k, v in top))
@@ -335,8 +338,9 @@ def test_pool_op_against_fp64(mode, T, B, H, A, ragged, dtype):
         dh, g = pool_backward(ds.to(dt), h.to(dt), keep, mode, a, saved, rr)
         arms[arm] = {"s": s, "dh": dh, **g}
     assert set(got) == set(arms["fp64"])
+    floor = N.FLOOR if dtype == torch.bfloat16 else N.FLOOR_F32            # fp32 h: exact tanh, the fp32 floor
     for k, v in got.items():
-        N.check_budget(f"{mode} T={T} B={B} H={H} A={A} {k}", v, arms["fp64"][k], arms["emu"][k])
+        N.check_budget(f"{mode} T={T} B={B} H={H} A={A} {k}", v, arms["fp64"][k], arms["emu"][k], floor=floor)
     if lengths is not None:
         assert float(got["dh"].float().transpose(0, 1)[~keep.t()].abs().max()) == 0.0     # no gradient into uncounted steps
     if mode == "max" and dtype == torch.bfloat16:

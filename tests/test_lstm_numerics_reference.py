@@ -128,6 +128,61 @@ def test_a_defect_at_one_step_breaks_the_budget(long_case, defect, tensor):
         assert _rel(got.dx[t], fp64.dx[t]) > 0.1
 
 
+# --- the generic path's arms: bf16 (Generic) and fp32 (Fp32) --------------------------------------------------------------
+G_T, G_B, G_H, G_D = 128, 64, 96, 40           # H % 64 != 0: a bf16 layer of this shape runs on the generic path
+G_LENGTHS = _lengths(G_T, G_B, 8)
+
+
+@pytest.fixture(scope="module")
+def generic_case():
+    """fp64 and both generic arms of one masked reverse layer: (fp64, {arm: emulation}, fp32 inputs)."""
+    params64, grads64 = _inputs(G_T, G_B, G_H, G_D, seed=9)
+    args32 = [p.float() for p in params64] + [g.float() for g in grads64]
+    kw = dict(lengths=G_LENGTHS, reverse=True)
+    fp64 = N.layer(*params64, *grads64, **kw)
+    emu = {"generic": N.layer(*args32, rounding=N.Generic(), **kw), "fp32": N.layer(*args32, rounding=N.Fp32(), **kw)}
+    return fp64, emu, lambda rounding, defect=None: N.layer(*args32, rounding=rounding, defect=defect, **kw)
+
+
+def _budget_floor(got, fp64, emu, floor):
+    return {name: N.check_budget(name, g, f, e, per_step=name in ("h_seq", "dx"), floor=floor)
+            for name, g, f, e in zip(N.LayerOut._fields, got, fp64, emu)}
+
+
+@pytest.mark.parametrize("arm,standin,floor", [
+    ("generic", N.Generic(approx=2.0 ** -11), N.FLOOR),            # tanh.approx-sized activations, as the bf16 cell kernels
+    ("fp32", N.Fp32(split=2, approx=2.0 ** -24), N.FLOOR_F32),      # other fp32 sums, activations off by an ulp
+])
+def test_generic_arms_sit_inside_the_budget_of_a_second_realisation(generic_case, arm, standin, floor):
+    fp64, emu, run = generic_case
+    ratios = _budget_floor(run(standin), fp64, emu[arm], floor)
+    assert max(ratios.values()) <= 1.0, ratios
+    lo, hi = (1e-4, 2e-2) if arm == "generic" else (1e-8, 1e-5)     # bf16-sized / fp32-sized distances from fp64
+    assert lo < _rel(emu[arm].h_seq, fp64.h_seq) < hi and lo < _rel(emu[arm].dw_h, fp64.dw_h) < hi
+
+
+def test_generic_arm_differs_from_the_fast_path_emulation(generic_case):
+    """The generic arm rounds pre before the bias and never the recurrent gradient product: not the fast path's numbers."""
+    fp64, emu, run = generic_case
+    fast = run(Bf16(fwd_split=1, bwd_split=4))
+    assert not torch.equal(fast.h_seq, emu["generic"].h_seq) and not torch.equal(fast.dx, emu["generic"].dx)
+
+
+def test_fp32_budget_rejects_a_tanh_off_by_2_to_the_minus_15(generic_case):
+    """A 128-step fp32 layer whose every tanh (and sigmoid) carries a relative error of 2^-15 - sixteen times smaller than
+    tanh.approx's - is over the fp32 budget."""
+    fp64, emu, run = generic_case
+    with pytest.raises(AssertionError, match=r"error vs fp64 .*ratio"):
+        _budget_floor(run(N.Fp32(approx=2.0 ** -15)), fp64, emu["fp32"], N.FLOOR_F32)
+
+
+def test_a_defect_at_one_step_breaks_the_generic_budget(generic_case):
+    """One k-block of h dropped from the recurrent product at one step, on the bf16 generic arm."""
+    fp64, emu, run = generic_case
+    with pytest.raises(AssertionError, match=r"h_seq at step \d+: .*ratio"):
+        _budget_floor(run(N.Generic(approx=2.0 ** -11), Defect("drop_kblock", STEP, 0)), fp64, emu["generic"], N.FLOOR)
+
+
 # --- the whole model ----------------------------------------------------------------------------------------------------
 def _model_inputs(hidden, T, B, D, C, seed, bidirectional=False, initial_state=False, dtype=torch.float64):
     """x [B,T,D], per-layer (direction) (h0, c0, w_x, w_h, bias), head (W, b), labels: bf16-representable where the kernels
