@@ -134,7 +134,7 @@ def head_kernels(args, dev, reps=200):
     dloss = torch.ones(1, device=dev)
     fwd = lambda: E.head_step_fwd(h, W, b, y, lengths, T)
     dlogits = fwd()[1]
-    bwd = lambda: E.head_step_bwd(h, W, dlogits, dloss, dW, db, False)
+    bwd = lambda: E.head_step_bwd(h, W, dlogits, dloss, dW, db, False, False)
     return {"rows": T * B, "H": H, "C": C, "fwd_us": _timed(fwd, reps, 10) * 1e3, "bwd_us": _timed(bwd, reps, 10) * 1e3}
 
 

@@ -42,14 +42,14 @@ int ts_ar_flag_words();
 int ts_ar_slots();
 int ts_head_fwd_tc(const void*, int, const float*, const float*, const long long*, float*, float*, float*, int*, int, int, int, cudaStream_t);
 int ts_head_logits_generic(const void*, const float*, const float*, float*, int, int, int, int, cudaStream_t);
-int ts_head_bwd(const void*, const float*, const float*, const float*, void*, float*, float*, int, int, int, int, int, cudaStream_t);
+int ts_head_bwd(const void*, const float*, const float*, const float*, void*, float*, float*, int, int, int, int, int, int, cudaStream_t);
 int ts_head_step_fwd_generic_parts(int);
 int ts_head_step_fwd(const void*, int, int, const float*, const float*, const long long*, const int*, float*, float*, float*, int*,
                      unsigned int*, float*, int*, int*, int, int, int, int, int*, cudaStream_t);
 long long ts_head_step_bwd_scratch(int, int, int);
 int ts_head_step_bwd_tickets(int);
 int ts_head_step_bwd(const void*, const float*, const float*, const float*, void*, float*, float*, float*, unsigned int*, int, int, int,
-                     int, int, cudaStream_t);
+                     int, int, int, cudaStream_t);
 int ts_vocab_head_parts(int);
 int ts_vocab_head_blocks(int);
 int ts_vocab_head_fwd(const void*, const void*, int, const float*, const long long*, const int*, void*, float*, float*, int*, unsigned int*,
@@ -315,8 +315,9 @@ std::vector<Tensor> head_fwd(const Tensor& h, const Tensor& W, const Tensor& bia
 }
 
 // dh = (dloss * dlogits) W^T [B,H] (dtype of h), dW (+)= h^T (dloss * dlogits) [H,C], db (+)= column sums: one launch.
+// acc_w / acc_b: add into dW / db instead of overwriting them.
 Tensor head_bwd(const Tensor& h, const Tensor& W, const Tensor& dlogits, const std::optional<Tensor>& dloss, Tensor dW, Tensor db,
-                bool accumulate) {
+                bool acc_w, bool acc_b) {
   chk_cuda(h, "h"); chk_cuda(W, "W"); chk_cuda(dlogits, "dlogits"); chk_cuda(dW, "dW"); chk_cuda(db, "db");
   c10::cuda::CUDAGuard g(h.device());
   const int B = h.size(0), H = h.size(1), C = W.size(1);
@@ -324,7 +325,7 @@ Tensor head_bwd(const Tensor& h, const Tensor& W, const Tensor& dlogits, const s
   TORCH_CHECK(dlogits.scalar_type() == torch::kFloat32 && dlogits.numel() == (int64_t)B * C, "head_bwd: dlogits fp32 [B,C]");
   auto dh = torch::empty_like(h);
   check(ts_head_bwd(h.data_ptr(), W.data_ptr<float>(), dlogits.data_ptr<float>(), fptr(dloss), dh.data_ptr(), dW.data_ptr<float>(),
-                    db.data_ptr<float>(), B, H, C, is_bf16(h), accumulate ? 1 : 0, stream()), "head_bwd");
+                    db.data_ptr<float>(), B, H, C, is_bf16(h), acc_w ? 1 : 0, acc_b ? 1 : 0, stream()), "head_bwd");
   return dh;
 }
 
@@ -375,9 +376,9 @@ std::vector<Tensor> head_step_fwd(const Tensor& h, const Tensor& W, const Tensor
 }
 
 // dh = (dloss * dlogits) W^T [T·B,H] (dtype of h), dW (+)= h^T (dloss * dlogits), db (+)= column sums: one launch, reduced in a
-// fixed order (bitwise reproducible).
+// fixed order (bitwise reproducible).  acc_w / acc_b: add into dW / db instead of overwriting them.
 Tensor head_step_bwd(const Tensor& h, const Tensor& W, const Tensor& dlogits, const std::optional<Tensor>& dloss, Tensor dW, Tensor db,
-                     bool accumulate) {
+                     bool acc_w, bool acc_b) {
   chk_cuda(h, "h"); chk_cuda(W, "W"); chk_cuda(dlogits, "dlogits"); chk_cuda(dW, "dW"); chk_cuda(db, "db");
   c10::cuda::CUDAGuard g(h.device());
   const int R = h.size(0), H = h.size(1), C = W.size(1);
@@ -389,7 +390,7 @@ Tensor head_step_bwd(const Tensor& h, const Tensor& W, const Tensor& dlogits, co
   auto tickets = torch::zeros({ts_head_step_bwd_tickets(H)}, fo.dtype(torch::kInt32));
   check(ts_head_step_bwd(h.data_ptr(), W.data_ptr<float>(), dlogits.data_ptr<float>(), fptr(dloss), dh.data_ptr(), dW.data_ptr<float>(),
                          db.data_ptr<float>(), scratch.data_ptr<float>(), (unsigned int*)tickets.data_ptr<int>(), R, H, C, is_bf16(h),
-                         accumulate ? 1 : 0, stream()), "head_step_bwd");
+                         acc_w ? 1 : 0, acc_b ? 1 : 0, stream()), "head_step_bwd");
   return dh;
 }
 
@@ -1024,7 +1025,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.attr("EMBED_BWD_LAUNCHES") = ts_embed_bwd_launches();
   m.def("head_step_fwd", &head_step_fwd, py::arg("h"), py::arg("W"), py::arg("bias"), py::arg("labels"), py::arg("lengths"), py::arg("T"));
   m.def("head_step_bwd", &head_step_bwd, py::arg("h"), py::arg("W"), py::arg("dlogits"), py::arg("dloss"), py::arg("dW"), py::arg("db"),
-        py::arg("accumulate"));
+        py::arg("acc_w"), py::arg("acc_b"));
   m.def("vocab_head_parts", [](int64_t C) { return ts_vocab_head_parts((int)C); });
   m.def("vocab_head_fwd", &vocab_head_fwd, py::arg("h"), py::arg("Wb"), py::arg("w_kmajor"), py::arg("bias"), py::arg("labels"), py::arg("lengths"),
         py::arg("T"), py::arg("part"));
@@ -1038,7 +1039,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("vocab_head_logits", &vocab_head_logits, py::arg("h"), py::arg("Wb"), py::arg("w_kmajor"), py::arg("bias"));
   m.def("vocab_threshold", &vocab_threshold, py::arg("logits"), py::arg("top_k"), py::arg("top_p"), py::arg("temperature"));
   m.def("head_bwd", &head_bwd, py::arg("h"), py::arg("W"), py::arg("dlogits"), py::arg("dloss"), py::arg("dW"), py::arg("db"),
-        py::arg("accumulate") = false);
+        py::arg("acc_w") = false, py::arg("acc_b") = false);
   m.def("flat_adam", &flat_adam, py::arg("p"), py::arg("g"), py::arg("m"), py::arg("v"), py::arg("shadow"), py::arg("lr_t"),
         py::arg("b1"), py::arg("b2"), py::arg("eps"), py::arg("wd"), py::arg("gscale"), py::arg("step_dev") = py::none(),
         py::arg("wd_numel") = -1, py::arg("clip") = py::none());

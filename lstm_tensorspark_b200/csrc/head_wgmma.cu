@@ -202,7 +202,8 @@ head_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmap_h, const HeadParams 
 template <typename T, int CP, typename TDH>
 __global__ void __launch_bounds__(128) head_bwd_kernel(const T* __restrict__ h, const float* __restrict__ W, const float* __restrict__ dlogits,
                                                        const float* __restrict__ dloss, TDH* __restrict__ dh, float* __restrict__ dW,
-                                                       float* __restrict__ db, int B, int H, int C, int rows_per_block, int accumulate) {
+                                                       float* __restrict__ db, int B, int H, int C, int rows_per_block, int acc_w,
+                                                       int acc_b) {
   // thread = (hidden column j, row group q of 4): lanes 0..31 of a warp = 32 consecutive j (coalesced h / dh accesses), warp = q.
   // Row b of the slab is handled by group b % 4; the four partial dW rows are added in fixed order through shared memory.
   extern __shared__ float ds[];                         // [rows_per_block][CP] dlogits slab, then [4][kHBwdJ][CP] partials
@@ -252,20 +253,20 @@ __global__ void __launch_bounds__(128) head_bwd_kernel(const T* __restrict__ h, 
 #pragma unroll
   for (int c = 0; c < CP; ++c) part[(q * kHBwdJ + jl) * CP + c] = acc[c];
   __syncthreads();
-  const bool atomic = gridDim.y > 1 || accumulate;
+  const bool atomic_w = gridDim.y > 1 || acc_w, atomic_b = gridDim.y > 1 || acc_b;
   for (int i = threadIdx.x; i < kHBwdJ * CP; i += 128) {            // fixed-order sum of the four row groups
     const int jj = i / CP, c = i % CP;
     const int jg = blockIdx.x * kHBwdJ + jj;
     if (jg < H && c < C) {
       const float t = ((part[(0 * kHBwdJ + jj) * CP + c] + part[(1 * kHBwdJ + jj) * CP + c]) + part[(2 * kHBwdJ + jj) * CP + c]) +
                       part[(3 * kHBwdJ + jj) * CP + c];
-      if (atomic) atomicAdd(dW + (size_t)jg * C + c, t); else dW[(size_t)jg * C + c] = t;
+      if (atomic_w) atomicAdd(dW + (size_t)jg * C + c, t); else dW[(size_t)jg * C + c] = t;
     }
   }
   if (blockIdx.x == 0 && threadIdx.x < C) {
     float s = 0.f;
     for (int b = 0; b < nb; ++b) s += ds[b * CP + threadIdx.x];
-    if (atomic) atomicAdd(db + threadIdx.x, s); else db[threadIdx.x] = s;
+    if (atomic_b) atomicAdd(db + threadIdx.x, s); else db[threadIdx.x] = s;
   }
 }
 
@@ -283,19 +284,19 @@ __global__ void head_bwd_dh_generic(const float* __restrict__ W, const float* __
 }
 template <typename T>
 __global__ void head_bwd_dw_generic(const T* __restrict__ h, const float* __restrict__ dlogits, const float* __restrict__ dloss,
-                                    float* __restrict__ dW, float* __restrict__ db, int B, int H, int C, int accumulate) {
+                                    float* __restrict__ dW, float* __restrict__ db, int B, int H, int C, int acc_w, int acc_b) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   const float scale = dloss ? *dloss : 1.f;
   if (i < (long long)H * C) {
     const int j = (int)(i / C), c = (int)(i % C);
     float s = 0.f;
     for (int b = 0; b < B; ++b) s = fmaf(ts::Cvt<T>::to_f(h[(size_t)b * H + j]), dlogits[(size_t)b * C + c], s);
-    dW[i] = (accumulate ? dW[i] : 0.f) + s * scale;
+    dW[i] = (acc_w ? dW[i] : 0.f) + s * scale;
   } else if (i < (long long)H * C + C) {
     const int c = (int)(i - (long long)H * C);
     float s = 0.f;
     for (int b = 0; b < B; ++b) s += dlogits[(size_t)b * C + c];
-    db[c] = (accumulate ? db[c] : 0.f) + s * scale;
+    db[c] = (acc_b ? db[c] : 0.f) + s * scale;
   }
 }
 // logits for heads the tensor-core kernel does not take (fp32 activations, very wide heads): one thread per output
@@ -312,22 +313,20 @@ __global__ void head_logits_generic(const T* __restrict__ h, const float* __rest
 
 template <typename T, typename TDH>
 int launch_bwd(const void* h, const float* W, const float* dlogits, const float* dloss, void* dh, float* dW, float* db, int B, int H, int C,
-               int accumulate, cudaStream_t st) {
+               int acc_w, int acc_b, cudaStream_t st) {
   if (C > 32) {
     const long long n1 = (long long)B * H, n2 = (long long)H * C + C;
     head_bwd_dh_generic<T, TDH><<<(unsigned)((n1 + 255) / 256), 256, 0, st>>>(W, dlogits, dloss, (TDH*)dh, B, H, C);
-    head_bwd_dw_generic<T><<<(unsigned)((n2 + 255) / 256), 256, 0, st>>>((const T*)h, dlogits, dloss, dW, db, B, H, C, accumulate);
+    head_bwd_dw_generic<T><<<(unsigned)((n2 + 255) / 256), 256, 0, st>>>((const T*)h, dlogits, dloss, dW, db, B, H, C, acc_w, acc_b);
     return (int)cudaGetLastError();
   }
   // one slab (no atomics: deterministic) while the dlogits slab fits in shared memory, 32-row slabs + fp32 atomics beyond
   const int cp = C <= 8 ? 8 : (C <= 16 ? 16 : 32);
   const int rows = (size_t)(B + 4 * kHBwdJ) * cp * sizeof(float) <= 48 * 1024 ? B : 32;
   dim3 grid((H + kHBwdJ - 1) / kHBwdJ, (B + rows - 1) / rows);
-  if (grid.y > 1 && !accumulate) {
-    cudaMemsetAsync(dW, 0, sizeof(float) * (size_t)H * C, st);
-    cudaMemsetAsync(db, 0, sizeof(float) * (size_t)C, st);
-  }
-#define HEAD_BWD(CP) head_bwd_kernel<T, CP, TDH><<<grid, 128, (rows + 4 * kHBwdJ) * CP * sizeof(float), st>>>((const T*)h, W, dlogits, dloss, (TDH*)dh, dW, db, B, H, C, rows, accumulate)
+  if (grid.y > 1 && !acc_w) cudaMemsetAsync(dW, 0, sizeof(float) * (size_t)H * C, st);
+  if (grid.y > 1 && !acc_b) cudaMemsetAsync(db, 0, sizeof(float) * (size_t)C, st);
+#define HEAD_BWD(CP) head_bwd_kernel<T, CP, TDH><<<grid, 128, (rows + 4 * kHBwdJ) * CP * sizeof(float), st>>>((const T*)h, W, dlogits, dloss, (TDH*)dh, dW, db, B, H, C, rows, acc_w, acc_b)
   if (C <= 8) HEAD_BWD(8); else if (C <= 16) HEAD_BWD(16); else HEAD_BWD(32);
 #undef HEAD_BWD
   return (int)cudaGetLastError();
@@ -637,7 +636,8 @@ __global__ void __launch_bounds__(128) head_step_bwd_kernel(const T* __restrict_
                                                             const float* __restrict__ dlogits, const float* __restrict__ dloss,
                                                             TDH* __restrict__ dh, float* __restrict__ dW, float* __restrict__ db,
                                                             float* __restrict__ pdw, float* __restrict__ pdb,
-                                                            unsigned int* __restrict__ tickets, int R, int H, int C, int accumulate) {
+                                                            unsigned int* __restrict__ tickets, int R, int H, int C, int acc_w,
+                                                            int acc_b) {
   constexpr int RPB = step_bwd_rows<CP>();
   extern __shared__ float ds[];                         // [RPB][CP] dlogits slab, then [4][kHBwdJ][CP] partials
   float* part = ds + (size_t)RPB * CP;
@@ -712,29 +712,29 @@ __global__ void __launch_bounds__(128) head_step_bwd_kernel(const T* __restrict_
       const volatile float* src = pdw + (size_t)jg * C + c;
       float s = 0.f;
       for (int k = 0; k < ns; ++k) s += src[(size_t)k * H * C];
-      dW[(size_t)jg * C + c] = (accumulate ? dW[(size_t)jg * C + c] : 0.f) + s;
+      dW[(size_t)jg * C + c] = (acc_w ? dW[(size_t)jg * C + c] : 0.f) + s;
     }
   }
   if (blockIdx.x == 0 && threadIdx.x < C) {
     const volatile float* src = pdb + threadIdx.x;
     float s = 0.f;
     for (int k = 0; k < ns; ++k) s += src[(size_t)k * C];
-    db[threadIdx.x] = (accumulate ? db[threadIdx.x] : 0.f) + s;
+    db[threadIdx.x] = (acc_b ? db[threadIdx.x] : 0.f) + s;
   }
   if (threadIdx.x == 0) tickets[blockIdx.x] = 0u;
 }
 
 template <typename T, typename TDH>
 int launch_step_bwd(const void* h, const float* W, const float* dlogits, const float* dloss, void* dh, float* dW, float* db,
-                    float* scratch, unsigned int* tickets, int R, int H, int C, int accumulate, cudaStream_t st) {
-  if (C > 32) return launch_bwd<T, TDH>(h, W, dlogits, dloss, dh, dW, db, R, H, C, accumulate, st);   // per-output kernels: no atomics
+                    float* scratch, unsigned int* tickets, int R, int H, int C, int acc_w, int acc_b, cudaStream_t st) {
+  if (C > 32) return launch_bwd<T, TDH>(h, W, dlogits, dloss, dh, dW, db, R, H, C, acc_w, acc_b, st);   // per-output kernels: no atomics
 #define STEP_BWD(CP)                                                                                                      \
   do {                                                                                                                    \
     constexpr int rows = step_bwd_rows<CP>();                                                                             \
     const int ns = (R + rows - 1) / rows;                                                                                 \
     dim3 grid((H + kHBwdJ - 1) / kHBwdJ, ns);                                                                             \
     head_step_bwd_kernel<T, CP, TDH><<<grid, 128, (rows + 4 * kHBwdJ) * CP * sizeof(float), st>>>(                         \
-        (const T*)h, W, dlogits, dloss, (TDH*)dh, dW, db, scratch, scratch + (size_t)ns * H * C, tickets, R, H, C, accumulate); \
+        (const T*)h, W, dlogits, dloss, (TDH*)dh, dW, db, scratch, scratch + (size_t)ns * H * C, tickets, R, H, C, acc_w, acc_b); \
   } while (0)
   if (C <= 8) STEP_BWD(8); else if (C <= 16) STEP_BWD(16); else STEP_BWD(32);
 #undef STEP_BWD
@@ -781,11 +781,11 @@ extern "C" int ts_head_logits_generic(const void* h, const float* W, const float
   return (int)cudaGetLastError();
 }
 
-// dh dtype follows h (bf16 -> bf16, fp32 -> fp32); dW [H, C] / db [C] fp32, accumulate = add into them.
+// dh dtype follows h (bf16 -> bf16, fp32 -> fp32); dW [H, C] / db [C] fp32, acc_w / acc_b = add into dW / db.
 extern "C" int ts_head_bwd(const void* h, const float* W, const float* dlogits, const float* dloss, void* dh, float* dW, float* db,
-                           int B, int H, int C, int is_bf16, int accumulate, cudaStream_t st) {
-  if (is_bf16) return launch_bwd<__nv_bfloat16, __nv_bfloat16>(h, W, dlogits, dloss, dh, dW, db, B, H, C, accumulate, st);
-  return launch_bwd<float, float>(h, W, dlogits, dloss, dh, dW, db, B, H, C, accumulate, st);
+                           int B, int H, int C, int is_bf16, int acc_w, int acc_b, cudaStream_t st) {
+  if (is_bf16) return launch_bwd<__nv_bfloat16, __nv_bfloat16>(h, W, dlogits, dloss, dh, dW, db, B, H, C, acc_w, acc_b, st);
+  return launch_bwd<float, float>(h, W, dlogits, dloss, dh, dW, db, B, H, C, acc_w, acc_b, st);
 }
 
 // ---- per-step head ------------------------------------------------------------------------------------------------------
@@ -849,8 +849,9 @@ extern "C" int ts_head_step_bwd_tickets(int H) { return (H + kHBwdJ - 1) / kHBwd
 
 // h [R, H] (packed), dlogits [R, C] in row order -> dh [R, H] (dtype of h), dW [H, C] / db [C] (+)= (dloss-scaled) sums.
 extern "C" int ts_head_step_bwd(const void* h, const float* W, const float* dlogits, const float* dloss, void* dh, float* dW, float* db,
-                                float* scratch, unsigned int* tickets, int R, int H, int C, int is_bf16, int accumulate, cudaStream_t st) {
+                                float* scratch, unsigned int* tickets, int R, int H, int C, int is_bf16, int acc_w, int acc_b,
+                                cudaStream_t st) {
   if (is_bf16)
-    return launch_step_bwd<__nv_bfloat16, __nv_bfloat16>(h, W, dlogits, dloss, dh, dW, db, scratch, tickets, R, H, C, accumulate, st);
-  return launch_step_bwd<float, float>(h, W, dlogits, dloss, dh, dW, db, scratch, tickets, R, H, C, accumulate, st);
+    return launch_step_bwd<__nv_bfloat16, __nv_bfloat16>(h, W, dlogits, dloss, dh, dW, db, scratch, tickets, R, H, C, acc_w, acc_b, st);
+  return launch_step_bwd<float, float>(h, W, dlogits, dloss, dh, dW, db, scratch, tickets, R, H, C, acc_w, acc_b, st);
 }

@@ -84,10 +84,10 @@ class FlatParams:
         re-casting the weights every step; also the fp32 grad view so weight-gradient GEMMs accumulate in place."""
         if self.shadow is None or not self.data.is_cuda:
             return
-        from ..ops import cuda_lstm
+        from ..ops.params import register_param
         for p, o in zip(self.params, self.offsets):
-            cuda_lstm.register_param(p.data_ptr(), self.shadow[o:o + p.numel()].view(p.shape),
-                                     self.grad[o:o + p.numel()].view(p.shape), owner=self)
+            register_param(p.data_ptr(), self.shadow[o:o + p.numel()].view(p.shape), self.grad[o:o + p.numel()].view(p.shape),
+                           owner=self)
 
     def refresh_shadow(self):
         if self.shadow is not None:

@@ -11,12 +11,8 @@ from __future__ import annotations
 
 import torch
 
-from .cuda_ext import LAUNCHES, ext
-
-
-def _count(key: str) -> None:
-    from .cuda_lstm import STATS
-    STATS[key] = STATS.get(key, 0) + 1
+from .cuda_ext import LAUNCHES, count, ext
+from .params import grad_out, lowp
 
 
 def _tokens(tokens: torch.Tensor) -> torch.Tensor:
@@ -27,31 +23,28 @@ def _tokens(tokens: torch.Tensor) -> torch.Tensor:
 class _EmbedFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, tokens, table, lengths, dtype):
-        from .cuda_lstm import _lowp
         tok = _tokens(tokens)
         if tok.device != table.device:
             raise ValueError(f"tokens on {tok.device}, the embedding table on {table.device}")
-        tab = _lowp(table, torch.bfloat16) if dtype == torch.bfloat16 else table.detach().float().contiguous()
+        tab = lowp(table, torch.bfloat16) if dtype == torch.bfloat16 else table.detach().float().contiguous()
         ln = None if lengths is None else lengths.contiguous()
         x = ext().embed_fwd(tab, tok, ln)
-        _count("embed_fwd")
+        count("embed_fwd")
         ctx.tok, ctx.ln, ctx.addr, ctx.shape = tok, ln, table.data_ptr(), tuple(table.shape)
         return x if x.dtype == dtype else x.to(dtype)
 
     @staticmethod
     def backward(ctx, dx):
-        from .cuda_lstm import grad_sink
         E = ext()
         d = dx.detach()
         if d.dtype not in (torch.bfloat16, torch.float32):
             d = d.float()
         d = d.contiguous()
-        sink = grad_sink(ctx.addr)
-        out = sink[0] if sink is not None else torch.empty(ctx.shape, dtype=torch.float32, device=d.device)
-        E.embed_bwd(d, ctx.tok, ctx.ln, out, sink is not None and sink[1])
+        out, acc, ret = grad_out(ctx.addr, ctx.shape, d.device)
+        E.embed_bwd(d, ctx.tok, ctx.ln, out, acc)
         LAUNCHES["n"] += E.EMBED_BWD_LAUNCHES - 1
-        _count("embed_bwd")
-        return None, (None if sink is not None else out), None, None
+        count("embed_bwd")
+        return None, ret, None, None
 
 
 def embedding(tokens, table, lengths=None, dtype=None):

@@ -10,7 +10,14 @@ import os
 _EXT = None
 _ERR = None
 LAUNCHES = {"n": 0}          # number of OUR kernels launched through the extension (bench.py "gpu_launches")
+# which paths the ops took (also read as ``cuda_lstm.STATS``): fixed keys are incremented in place, the others through ``count``
+STATS = {"fast_fwd": 0, "fast_bwd": 0, "generic_fwd": 0, "generic_bwd": 0, "tc_gemm": 0, "kernels": 0, "weight_drop": 0,
+         "weight_drop_grad": 0}
 _NO_KERNEL = {"ar_max_blocks", "ar_flag_words", "ar_slots"}
+
+
+def count(key: str, n: int = 1) -> None:
+    STATS[key] = STATS.get(key, 0) + n
 
 
 class _Counting:

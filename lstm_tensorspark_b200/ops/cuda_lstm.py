@@ -16,7 +16,8 @@ from typing import Optional
 
 import torch
 
-from .cuda_ext import ext
+from .cuda_ext import STATS, count, ext
+from .params import grad_out, lowp
 from . import cuda_gemm as G
 
 _SYNC_WS = {}
@@ -28,8 +29,6 @@ FORCE_GENERIC = os.environ.get("LSTM_TS_FORCE_GENERIC", "0") == "1"
 #   6 no L2 prefetch, 7 cluster-scope acquire on the exchange barriers), [16:18) sync mode (0 per-k-block dataflow counters,
 #   1 one counter per batch tile = grid barrier, 2 per-CTA flags), bit 18 acquire polls, bit 19 no forward K-split.
 SEQ_VARIANT = int(os.environ.get("LSTM_TS_SEQ_VARIANT", "0"))
-STATS = {"fast_fwd": 0, "fast_bwd": 0, "generic_fwd": 0, "generic_bwd": 0, "tc_gemm": 0, "kernels": 0, "weight_drop": 0,
-         "weight_drop_grad": 0}
 
 
 # Gradient-bucket overlap (engine.TrainEngine + parallel/fused_comm.py): HOOKS["grads_written"] is called after every weight /
@@ -67,47 +66,6 @@ def _grads_written():
     if h is not None and not _CHUNKING["on"] and not _HOLD["on"]:
         h()
 
-_PARAMS = {}          # fp32 param address -> (bf16 shadow view, fp32 grad view), maintained by models.flat.FlatParams
-DIRECT_GRADS = os.environ.get("LSTM_TS_DIRECT_GRADS", "1") == "1"
-
-
-def register_param(addr: int, shadow: torch.Tensor, grad: torch.Tensor, owner=None) -> None:
-    import weakref
-    _PARAMS[addr] = (shadow, grad, weakref.ref(owner) if owner is not None else None)
-
-
-def _lookup(addr: int):
-    ent = _PARAMS.get(addr)
-    if ent is None:
-        return None
-    if ent[2] is not None and ent[2]() is None:       # the FlatParams buffer died: its address may have been reused
-        del _PARAMS[addr]
-        return None
-    return ent
-
-
-def _lowp(w: torch.Tensor, cd: torch.dtype) -> torch.Tensor:
-    """bf16 copy of a weight: the optimizer-maintained shadow when there is one, a cast otherwise."""
-    if cd == torch.bfloat16:
-        ent = _lookup(w.data_ptr())
-        if ent is not None and ent[0].shape == w.shape:
-            return ent[0]
-    return w.detach().to(cd).contiguous()
-
-
-def grad_sink(w_addr: int):
-    """-> (fp32 grad view inside the flat buffer, accumulate flag) for a registered parameter, or None.
-    accumulate False = first write of this step: the kernel overwrites (no zero-filled buffer needed)."""
-    ent = _lookup(w_addr) if DIRECT_GRADS else None
-    if ent is None:
-        return None
-    owner = ent[2]() if ent[2] is not None else None
-    if owner is None or w_addr not in owner._direct:
-        if owner is not None:
-            owner.ensure_zeroed(w_addr)
-        return ent[1], True
-    return ent[1], owner.take_sink(w_addr)
-
 
 def _accumulate_grad(w_addr: int, a_t: torch.Tensor, b: torch.Tensor, b_folded: bool = False, pdl: bool = False,
                      max_ctas: int = 0, ctas: int = 0, rowsum=None, wdrop=None, defer: bool = False):
@@ -130,27 +88,21 @@ def _accumulate_grad(w_addr: int, a_t: torch.Tensor, b: torch.Tensor, b_folded: 
     ops["rowsum"] = rowsum
     if pdl:
         ops.update(pdl=True, ctas=1, max_ctas=max_ctas)
-    sink = grad_sink(w_addr)
-    if sink is not None:
-        scratch = bool(wdrop) and sink[1]
-        if not pdl:
-            _big_launch_begin()
-        part = G.matmul(out_dtype=torch.float32, **ops) if scratch else G.matmul(out=sink[0], accumulate=sink[1], **ops)
-        if not pdl:
-            _after_big_launch()              # finished buckets of earlier gradients: allreduce them under this GEMM
+    out, acc, ret = grad_out(w_addr, (a_t.shape[0], b.shape[-1]), a_t.device)
+    scratch = bool(wdrop) and acc
+    big = ret is None and not pdl
+    if big:
+        _big_launch_begin()
+    part = G.matmul(out_dtype=torch.float32, **ops) if scratch else G.matmul(out=out, accumulate=acc, **ops)
+    if big:
+        _after_big_launch()              # finished buckets of earlier gradients: allreduce them under this GEMM
 
-        def finish():
-            if wdrop:
-                _weight_drop_grad(part if scratch else sink[0], sink[0], wdrop, scratch)
+    def finish():
+        if wdrop:
+            _weight_drop_grad(part if scratch else out, out, wdrop, scratch)
+        if ret is None:
             _grads_written()
-            return None
-    else:
-        dw = G.matmul(out_dtype=torch.float32, **ops)
-
-        def finish():
-            if wdrop:
-                _weight_drop_grad(dw, dw, wdrop, False)
-            return dw
+        return ret
     return finish if defer else finish()
 
 
@@ -163,42 +115,30 @@ def _bias_grad(b_addr: int, dg2d: torch.Tensor, under_gemm: bool = False, part: 
     ``part`` 0 / 1: only the first / second half of the columns (one half under each of the layer's two weight-gradient GEMMs:
     on the ~20 idle SMs a half takes about as long as the GEMM it hides under); the value for autograd comes from part 1.
     ``max_ctas`` (whole-column launches): at most that many CTAs, each walking several slabs (the same sums)."""
-    fast = dg2d.is_cuda and dg2d.dtype == torch.bfloat16 and dg2d.shape[1] % 512 == 0 and dg2d.is_contiguous()
+    n = dg2d.shape[1]
+    fast = dg2d.is_cuda and dg2d.dtype == torch.bfloat16 and n % 512 == 0 and dg2d.is_contiguous()
     if part == 0:
         if not fast:
             return None                                   # everything happens with the part-1 call
-        sink = grad_sink(b_addr)
-        _BIAS_SPLIT[b_addr] = sink
-        if sink is None:
-            return None
-        half = dg2d.shape[1] // 2
+        out, acc, _ = _BIAS_SPLIT[b_addr] = grad_out(b_addr, (n,), dg2d.device)
         STATS["kernels"] += 1
-        ext().colsum_bf16_into(dg2d, sink[0], not sink[1], under_gemm, 0, half)
+        ext().colsum_bf16_into(dg2d, out, not acc, under_gemm, 0, n // 2)
         return None
     if part == 1 and fast and b_addr in _BIAS_SPLIT:
-        sink = _BIAS_SPLIT.pop(b_addr)
-        if sink is not None:
-            half = dg2d.shape[1] // 2
-            STATS["kernels"] += 1
-            ext().colsum_bf16_into(dg2d, sink[0], not sink[1], under_gemm, half, half)
-            _grads_written()
-            return None
-        return ext().colsum_bf16(dg2d)
-    fast = dg2d.is_cuda and dg2d.dtype == torch.bfloat16 and dg2d.shape[1] % 256 == 0 and dg2d.is_contiguous()
-    sink = grad_sink(b_addr)
-    if fast:
+        out, acc, ret = _BIAS_SPLIT.pop(b_addr)
         STATS["kernels"] += 1
-        if sink is not None:
-            ext().colsum_bf16_into(dg2d, sink[0], not sink[1], under_gemm and part < 0, max_ctas=max_ctas)
-            _grads_written()
-            return None
-        return ext().colsum_bf16(dg2d)
-    ones = torch.ones(1, dg2d.shape[0], dtype=dg2d.dtype, device=dg2d.device)
-    if sink is not None:
-        G.matmul(ones, dg2d.t(), out=sink[0].view(1, -1), accumulate=sink[1])
+        ext().colsum_bf16_into(dg2d, out, not acc, under_gemm, n // 2, n // 2)
+    else:
+        out, acc, ret = grad_out(b_addr, (n,), dg2d.device)
+        if dg2d.is_cuda and dg2d.dtype == torch.bfloat16 and n % 256 == 0 and dg2d.is_contiguous():
+            STATS["kernels"] += 1
+            ext().colsum_bf16_into(dg2d, out, not acc, under_gemm and part < 0, max_ctas=max_ctas)
+        else:
+            ones = torch.ones(1, dg2d.shape[0], dtype=dg2d.dtype, device=dg2d.device)
+            G.matmul(ones, dg2d.t(), out=out.view(1, -1), accumulate=acc)
+    if ret is None:
         _grads_written()
-        return None
-    return G.matmul(ones, dg2d.t(), out_dtype=torch.float32).view(-1)
+    return ret
 
 
 SYNC_WORDS = 8192        # csrc/lstm_seq_wgmma.cu kSyncWords; the last word is the sticky error flag
@@ -387,9 +327,9 @@ class _LSTMSeqFn(torch.autograd.Function):
         H = w_h.shape[1]
         cd = x_seq.dtype
         x2d = x_seq.reshape(T * B, D).contiguous()
-        w_x_c = _lowp(w_x, cd)
+        w_x_c = lowp(w_x, cd)
         ctx.wdrop = _drop_args(weight_drop, x_seq.device)
-        w_h_c = _weight_image(_lowp(w_h, cd), weight_drop)             # every step reads the masked image (weight drop)
+        w_h_c = _weight_image(lowp(w_h, cd), weight_drop)             # every step reads the masked image (weight drop)
         bias_f = bias.detach().float().contiguous()
         gx = _gemm_tn(x2d, w_x_c).view(T, B, 4 * H)
         fast = fast_path_supported(B, H, cd, x_seq.device)
@@ -525,7 +465,7 @@ def lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths=None, reverse=Fal
                     for b0 in range(0, B, chunk)]
         finally:
             _CHUNKING["on"] = False
-        STATS["batch_chunks"] = STATS.get("batch_chunks", 0) + len(outs)
+        count("batch_chunks", len(outs))
         return (torch.cat([o[0] for o in outs], dim=1), torch.cat([o[1] for o in outs], dim=0),
                 torch.cat([o[2] for o in outs], dim=0))
     return _LSTMSeqFn.apply(x_seq.contiguous(), h0, c0, w_x, w_h, bias, lengths, reverse, dropout, weight_drop)
@@ -679,7 +619,7 @@ class _LSTMPairFn(torch.autograd.Function):
         # weight-gradient GEMM of the first layer (folded tensor map, csrc/gemm2_wgmma.cu): no transpose pass
         x_bm = x_seq.transpose(0, 1) if not x_seq.is_contiguous() else None
         x2d = x_seq.reshape(T * B, D) if x_bm is None else x_bm
-        wxa, wha, wxb, whb = _lowp(w_xa, cd), _lowp(w_ha, cd), _lowp(w_xb, cd), _lowp(w_hb, cd)
+        wxa, wha, wxb, whb = lowp(w_xa, cd), lowp(w_ha, cd), lowp(w_xb, cd), lowp(w_hb, cd)
         wha, whb = _weight_image(wha, wdrop_a), _weight_image(whb, wdrop_b)          # weight drop: the masked images
         ctx.wdrop = (_drop_args(wdrop_a, dev), _drop_args(wdrop_b, dev))
         ba_f, bb_f = b_a.detach().float().contiguous(), b_b.detach().float().contiguous()
@@ -693,7 +633,7 @@ class _LSTMPairFn(torch.autograd.Function):
         elif x_bm is None:
             gx_a = _gemm_tn(x2d, wxa).view(T, B, 4 * Ha)
         else:
-            STATS["tc_gemm"] += 1; STATS["kernels"] += 1; STATS["folded_feed"] = STATS.get("folded_feed", 0) + 1
+            STATS["tc_gemm"] += 1; STATS["kernels"] += 1; count("folded_feed")
             gx_a = G.matmul(None, wxa, out_dtype=cd, a_folded=x_bm).view(T, B, 4 * Ha)
         h_seq_a = torch.empty(T + 1, B, Ha, **opt); c_seq_a = torch.empty(T + 1, B, Ha, dtype=torch.float32, device=dev)
         act_a = torch.empty(T, B, 4 * Ha, **opt); til_a = torch.empty((T + 1) * 2 * 128 * Ha, **opt)
@@ -727,9 +667,9 @@ class _LSTMPairFn(torch.autograd.Function):
         if side_a:
             a_op = dict(A=x2d, a_fold=0) if x_bm is None else dict(A=x_bm.reshape(B, T * D), a_fold=B, fold_cols=D)
             E.gemm2(B=wxa, out=gx_a.view(T * B, 4 * Ha), ctas=1, bn=256, max_ctas=ctas_a, done=done_a, pdl=True, **a_op)
-            STATS["tc_gemm"] += 1; STATS["kernels"] += 1; STATS["pipelined_side_gemms"] = STATS.get("pipelined_side_gemms", 0) + 1
+            STATS["tc_gemm"] += 1; STATS["kernels"] += 1; count("pipelined_side_gemms")
             if x_bm is not None:
-                STATS["folded_feed"] = STATS.get("folded_feed", 0) + 1
+                count("folded_feed")
         if not pipelined:
             E.lstm_seq_fwd_into(gx_b, whb, bb_f, h0b_c, c0b_f, h_seq_b, c_seq_b, act_b, til_b, ws_b, var, done, tn, False, 0, 3, lengths,
                                 h_drop=h_drop_b, **drb)
@@ -743,7 +683,7 @@ class _LSTMPairFn(torch.autograd.Function):
                                 h_drop=h_drop_b, **drb)
         STATS["fast_fwd"] += 2
         STATS["kernels"] += 3
-        STATS[schedule + "_fwd"] = STATS.get(schedule + "_fwd", 0) + 1
+        count(schedule + "_fwd")
         ctx.save_for_backward(x2d, h_seq_a, c_seq_a, act_a, h_seq_b, c_seq_b, act_b, wxa, wha, wxb, whb, hin_b)
         ctx.set_materialize_grads(False)
         ctx.drop = (dra, drb)
@@ -838,13 +778,10 @@ class _LSTMPairFn(torch.autograd.Function):
             # the dW_ha launch as the row sums of dG_a^T (csrc/gemm2_wgmma.cu): the column-sum kernels beside these GEMMs only
             # found the 4 SMs the GEMMs leave free and ran on after them.
             dw_xa = _accumulate_grad(a[0], dg_a.t(), x2d, b_folded=ctx.x_folded, ctas=1)
-            bsink = grad_sink(a[2])
-            db_a = bsink[0] if bsink is not None else torch.empty(4 * Ha, **f32)
-            dw_ha = _accumulate_grad(a[1], dg_a.t(), h_seq_a[:T].reshape(T * B, Ha), ctas=1,
-                                     rowsum=(db_a, bsink is not None and bsink[1]), wdrop=wda)
-            STATS["fused_bias_grads"] = STATS.get("fused_bias_grads", 0) + 1
-            if bsink is not None:
-                db_a = None
+            db_out, db_acc, db_a = grad_out(a[2], (4 * Ha,), dev)
+            dw_ha = _accumulate_grad(a[1], dg_a.t(), h_seq_a[:T].reshape(T * B, Ha), ctas=1, rowsum=(db_out, db_acc), wdrop=wda)
+            count("fused_bias_grads")
+            if db_a is None:
                 _grads_written()
         else:
             dw_xa = _accumulate_grad(a[0], dg_a.t(), x2d, b_folded=ctx.x_folded)

@@ -12,21 +12,16 @@ from __future__ import annotations
 
 import torch
 
-from .cuda_ext import ext
+from .cuda_ext import count, ext
+from .params import grad_out, lowp
 
 MODES = {"mean": 0, "max": 1, "attention": 2}
-
-
-def _count(key: str) -> None:
-    from .cuda_lstm import STATS
-    STATS[key] = STATS.get(key, 0) + 1
 
 
 class _PoolFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, h_seq, lengths, mode, w_a, b_a, v):
         from . import cuda_gemm
-        from .cuda_lstm import _lowp
         E = ext()
         T, B, H = h_seq.shape
         hc = h_seq.detach()
@@ -37,18 +32,18 @@ class _PoolFn(torch.autograd.Function):
         m = MODES[mode]
         ctx.mode, ctx.T, ctx.h_dtype, ctx.ln = m, T, h_seq.dtype, ln
         if m == 2:
-            wa = _lowp(w_a, torch.bfloat16) if h2.dtype == torch.bfloat16 else w_a.detach().float().contiguous()
+            wa = lowp(w_a, torch.bfloat16) if h2.dtype == torch.bfloat16 else w_a.detach().float().contiguous()
             ba, vv = b_a.detach().float().contiguous(), v.detach().float().contiguous()
             u = cuda_gemm.matmul(h2, wa.t(), out_dtype=torch.float32)          # h W_a [T·B, A]; tanh(. + b_a) in place below
             alpha = E.seq_pool_attn_scores(u, ba, vv, ln, T, exact=h2.dtype == torch.float32)
             s, _ = E.seq_pool_fwd(h2, ln, T, m, alpha)
-            _count("pool_attention_fwd")
+            count("pool_attention_fwd")
             ctx.save_for_backward(h2, alpha, u, wa, vv)
             ctx.addrs = (w_a.data_ptr(), b_a.data_ptr(), v.data_ptr())
         else:
             s, am = E.seq_pool_fwd(h2, ln, T, m, None)
             ctx.save_for_backward(am if m == 1 else None)
-        _count("pool_fwd")
+        count("pool_fwd")
         return s
 
     @staticmethod
@@ -58,30 +53,23 @@ class _PoolFn(torch.autograd.Function):
         dsf = ds.detach().float().contiguous()
         B, H = dsf.shape
         out_bf16 = ctx.h_dtype == torch.bfloat16
-        _count("pool_bwd")
+        count("pool_bwd")
         if m != 2:
             (am,) = ctx.saved_tensors
             dh = E.seq_pool_bwd(dsf, ln, T, m, am, None, None, out_bf16)
             return dh.view(T, B, H).to(ctx.h_dtype), None, None, None, None, None
         from . import cuda_gemm
-        from .cuda_lstm import grad_sink
         h2, alpha, u, wa, vv = ctx.saved_tensors
         A = u.shape[1]
-        sinks = [grad_sink(a) for a in ctx.addrs]
-        dv = sinks[2][0] if sinks[2] is not None else torch.empty(A, dtype=torch.float32, device=dsf.device)
-        dba = sinks[1][0] if sinks[1] is not None else torch.empty(A, dtype=torch.float32, device=dsf.device)
-        acc_dv, acc_dba = sinks[2] is not None and sinks[2][1], sinks[1] is not None and sinks[1][1]
+        dwa, acc_dwa, ret_dwa = grad_out(ctx.addrs[0], wa.shape, dsf.device)
+        dba, acc_dba, ret_dba = grad_out(ctx.addrs[1], (A,), dsf.device)
+        dv, acc_dv, ret_dv = grad_out(ctx.addrs[2], (A,), dsf.device)
         dU = E.seq_pool_attn_bwd(h2, dsf, alpha, u, vv, ln, T, dv, dba, acc_dv, acc_dba)       # dtype of h
         G = cuda_gemm.matmul(dU, wa, out_dtype=torch.float32)                                 # dU W_a^T [T·B, H]
-        if sinks[0] is not None:
-            cuda_gemm.matmul(h2.t(), dU.t(), out=sinks[0][0], accumulate=sinks[0][1])         # dW_a = h^T dU
-            dwa = None
-        else:
-            dwa = cuda_gemm.matmul(h2.t(), dU.t(), out_dtype=torch.float32)
+        cuda_gemm.matmul(h2.t(), dU.t(), out=dwa, accumulate=acc_dwa)                         # dW_a = h^T dU
         dh = E.seq_pool_bwd(dsf, ln, T, m, None, alpha, G, out_bf16)
-        _count("pool_attention_bwd")
-        return (dh.view(T, B, H).to(ctx.h_dtype), None, None, dwa,
-                None if sinks[1] is not None else dba, None if sinks[2] is not None else dv)
+        count("pool_attention_bwd")
+        return dh.view(T, B, H).to(ctx.h_dtype), None, None, ret_dwa, ret_dba, ret_dv
 
 
 def pool_sequence(h_seq, lengths=None, mode: str = "mean", attention=None):

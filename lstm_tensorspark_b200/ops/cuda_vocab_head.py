@@ -17,7 +17,8 @@ from __future__ import annotations
 import torch
 
 from . import cuda_gemm as G
-from .cuda_ext import ext
+from .cuda_ext import count, ext
+from .params import grad_out, lowp
 
 ROW_CHUNK = 4096          # rows of h per backward chunk: the schedule depends on the shapes only
 MIN_CLASSES = 512
@@ -35,8 +36,7 @@ def _weights_lowp(weights: torch.Tensor, class_major: bool) -> torch.Tensor:
     table ``[C,H]`` itself (never a transposed view: the shadow and the gradient sink are found by the parameter's address and
     shape), read by TMA in place, which needs a 16-byte aligned base (FlatParams places every parameter at a multiple of 64
     elements, so a shadow view always is) and ``H % 8 == 0`` (implied by ``H % 64 == 0``)."""
-    from .cuda_lstm import _lowp
-    wb = _lowp(weights, torch.bfloat16)
+    wb = lowp(weights, torch.bfloat16)
     if class_major:
         assert wb.is_contiguous() and wb.data_ptr() % 16 == 0, "the tied table's bf16 operand must be packed and 16-byte aligned"
     return wb
@@ -45,7 +45,6 @@ def _weights_lowp(weights: torch.Tensor, class_major: bool) -> torch.Tensor:
 class _VocabXentFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, h_seq, weights, bias, labels, lengths, class_major=False):
-        from .cuda_lstm import STATS
         E = ext()
         T, B, H = h_seq.shape
         hc = h_seq.detach()
@@ -56,40 +55,32 @@ class _VocabXentFn(torch.autograd.Function):
         ln = None if lengths is None else lengths.contiguous()
         C = wb.shape[0 if class_major else 1]
         part = torch.empty(T * B * E.vocab_head_parts(C) * 4, dtype=torch.float32, device=h2.device)
-        lse, loss, correct, count = E.vocab_head_fwd(h2, wb, bool(class_major), b, lab, ln, T, part)
-        STATS["vocab_head_fwd"] = STATS.get("vocab_head_fwd", 0) + 1
+        lse, loss, correct, n = E.vocab_head_fwd(h2, wb, bool(class_major), b, lab, ln, T, part)
+        count("vocab_head_fwd")
         if class_major:
-            STATS["vocab_head_fwd_tied"] = STATS.get("vocab_head_fwd_tied", 0) + 1
-        ctx.save_for_backward(h2, wb, b, lab, ln, lse, count)
+            count("vocab_head_fwd_tied")
+        ctx.save_for_backward(h2, wb, b, lab, ln, lse, n)
         ctx.shape, ctx.class_major = (T, B, H), bool(class_major)
         ctx.addrs = (weights.data_ptr(), bias.data_ptr())
-        ctx.mark_non_differentiable(correct, count)
-        return loss.squeeze(0), correct.squeeze(0), count.squeeze(0)
+        ctx.mark_non_differentiable(correct, n)
+        return loss.squeeze(0), correct.squeeze(0), n.squeeze(0)
 
     @staticmethod
     def backward(ctx, dloss, _dcorrect_unused, _dcount_unused):
-        from .cuda_lstm import STATS, grad_sink
         E = ext()
-        h2, wb, b, lab, ln, lse, count = ctx.saved_tensors
+        h2, wb, b, lab, ln, lse, n = ctx.saved_tensors
         T, cm = ctx.shape[0], ctx.class_major
         R, H = h2.shape
         C = wb.shape[0 if cm else 1]
-        sw, sb = grad_sink(ctx.addrs[0]), grad_sink(ctx.addrs[1])
+        dw, acc_w, ret_w = grad_out(ctx.addrs[0], (C, H) if cm else (H, C), h2.device)
+        db, acc_b, ret_b = grad_out(ctx.addrs[1], (C,), h2.device)
         scale = dloss.detach().float().reshape(1).contiguous()
-        if sw is not None and sb is not None:
-            (dw, acc_w), (db, acc_b) = sw, sb
-            ret = (None, None)
-        else:
-            dw = torch.empty(*((C, H) if cm else (H, C)), dtype=torch.float32, device=h2.device)
-            db = torch.empty(C, dtype=torch.float32, device=h2.device)
-            acc_w = acc_b = False
-            ret = (dw, db)
         dh = torch.empty_like(h2)
         dl = torch.empty(min(ROW_CHUNK, R), C, dtype=torch.bfloat16, device=h2.device)
         for r0 in range(0, R, ROW_CHUNK):
             rows = min(ROW_CHUNK, R - r0)
             d = dl[:rows]
-            E.vocab_head_dlogits(h2, wb, cm, b, lab, ln, T, lse, count, scale, r0, rows, d)
+            E.vocab_head_dlogits(h2, wb, cm, b, lab, ln, T, lse, n, scale, r0, rows, d)
             acc = bool(acc_w or r0 > 0)
             if cm:
                 G.matmul(d, wb.t(), out=dh[r0:r0 + rows])                                      # dh = dlogits table
@@ -98,8 +89,8 @@ class _VocabXentFn(torch.autograd.Function):
                 G.matmul(d, wb, out=dh[r0:r0 + rows])                                          # dh = dlogits W^T
                 G.matmul(h2[r0:r0 + rows].t(), d.t(), out=dw, accumulate=acc)                   # dW (+)= h^T dlogits
             E.vocab_head_colsum(d, db.view(-1), bool(acc_b or r0 > 0))
-        STATS["vocab_head_bwd"] = STATS.get("vocab_head_bwd", 0) + 1
-        return dh.view(ctx.shape), ret[0], ret[1], None, None, None
+        count("vocab_head_bwd")
+        return dh.view(ctx.shape), ret_w, ret_b, None, None, None
 
 
 def vocab_xent_per_step(h_seq, weights, bias, labels, lengths=None, class_major=False):
@@ -122,17 +113,16 @@ def vocab_sample(h, weights, bias, temperature: float, seed: int, step, tokens=N
     """Sample the next token from ``h [B,H]`` bf16 through the head's tensor-core kernel (``kSample``), without storing the
     logits; see ``ops.functional.vocab_sample``.  With a filter on (the caller passes ``top_k = 0`` and ``top_p = 1`` when it is
     off) the same main loop stores the fp32 logits (``kLogits``) and ``vocab_sample_logits`` samples them."""
-    from .cuda_lstm import STATS
     wb = _weights_lowp(weights, class_major)
     hc, bc = h.detach().contiguous(), bias.detach().float().contiguous()
     if class_major:
-        STATS["vocab_sample_tied"] = STATS.get("vocab_sample_tied", 0) + 1
+        count("vocab_sample_tied")
     if top_k > 0 or top_p < 1:
         logits = ext().vocab_head_logits(hc, wb, bool(class_major), bc)
         return vocab_sample_logits(logits, temperature, seed, step, tokens, record, row0, top_k, top_p)
     step_t, row_t, tok, rec_tok, rec_lp, s0 = _sample_args(step, row0, tokens, record, h.shape[0], h.device)
     lp = ext().vocab_sample(hc, wb, bool(class_major), bc, float(temperature), int(seed), step_t, row_t, tok, rec_tok, rec_lp, int(s0))
-    STATS["vocab_sample"] = STATS.get("vocab_sample", 0) + 1
+    count("vocab_sample")
     return tok, lp
 
 
@@ -141,13 +131,12 @@ def vocab_sample_logits(logits, temperature: float, seed: int, step, tokens=None
     """The same sampling from stored fp32 logits ``[B,C]`` (bias included): the inputs the tensor-core kernel does not take, and
     top-k / top-p (on: ``top_k > 0`` or ``top_p < 1``, at temperature > 0), where ``vocab_threshold`` computes each row's
     threshold first and the sampling kernel scores only the classes at or above it."""
-    from .cuda_lstm import STATS
     step_t, row_t, tok, rec_tok, rec_lp, s0 = _sample_args(step, row0, tokens, record, logits.shape[0], logits.device)
     lg = logits.float().contiguous()
     tau = None
     if top_k > 0 or top_p < 1:
         tau = ext().vocab_threshold(lg, int(top_k), float(top_p), float(temperature))
-        STATS["vocab_sample_filtered"] = STATS.get("vocab_sample_filtered", 0) + 1
+        count("vocab_sample_filtered")
     lp = ext().vocab_sample_logits(lg, float(temperature), int(seed), step_t, row_t, tok, rec_tok, rec_lp, int(s0), tau)
-    STATS["vocab_sample"] = STATS.get("vocab_sample", 0) + 1
+    count("vocab_sample")
     return tok, lp

@@ -53,10 +53,10 @@ def test_pointwise_cell_fwd_bwd(E, dev, dtype, tol):
                                          (150, 128, 65, torch.bfloat16), (150, 128, 129, torch.bfloat16),
                                          # bf16 h the tensor-core kernel does not take (C > 256, H % 8 != 0): logits on CUDA cores
                                          (130, 64, 300, torch.bfloat16), (128, 100, 10, torch.bfloat16)])
-def test_head_forward_and_backward(E, dev, B, H, C, dtype):
+def test_head_forward_and_backward_per_output_flags(E, dev, B, H, C, dtype):
     """Tensor-core head (bf16 h: TMA + wgmma, epilogue from the accumulator registers) / generic head (fp32 h, or shapes the
     tensor-core kernel does not take) vs the fp32 reference, and the fused backward kernel (dh, dW, db in one launch, overwrite and
-    accumulate)."""
+    accumulate).  Both backward kernels take one flag per output: dW overwritten while db accumulates, and the reverse."""
     ref = _ref()
     torch.manual_seed(0)
     h = (torch.randn(B, H, device=dev) * 0.5).to(dtype)
@@ -81,15 +81,22 @@ def test_head_forward_and_backward(E, dev, B, H, C, dtype):
     dW = torch.full((H, C), 7.0, device=dev)
     db = torch.full((C,), 7.0, device=dev)
     one = torch.ones(1, device=dev)
-    dh = E.head_bwd(h.contiguous(), W, dlog, one, dW, db, False)             # overwrite: the 7s must be gone
+    dh = E.head_bwd(h.contiguous(), W, dlog, one, dW, db, False, False)      # overwrite: the 7s must be gone
     tol = 2e-2 if dtype == torch.bfloat16 else 1e-4
     assert (dW - h.float().t() @ dlog).abs().max() <= 1e-4 * max(1.0, float(dW.abs().max()))
     assert (db - dlog.sum(0)).abs().max() < 1e-5
     dh_ref = dlog @ W.t()
     assert (dh.float() - dh_ref).abs().max() <= tol * float(dh_ref.abs().max()) + 1e-7
     dW2, db2 = dW.clone(), db.clone()
-    E.head_bwd(h.contiguous(), W, dlog, one, dW2, db2, True)                 # accumulate
+    E.head_bwd(h.contiguous(), W, dlog, one, dW2, db2, True, True)           # accumulate
     assert (dW2 - 2 * dW).abs().max() <= 1e-4 * max(1.0, float(dW.abs().max())) and (db2 - 2 * db).abs().max() < 1e-5
+    for bwd in (E.head_bwd, E.head_step_bwd):                                 # one flag per output: each overwrites or adds alone
+        for acc_w, acc_b in ((False, True), (True, False)):
+            dW3 = dW.clone() if acc_w else torch.full_like(dW, 7.0)
+            db3 = db.clone() if acc_b else torch.full_like(db, 7.0)
+            bwd(h.contiguous(), W, dlog, one, dW3, db3, acc_w, acc_b)
+            assert (dW3 - (1 + acc_w) * dW).abs().max() <= 1e-4 * max(1.0, float(dW.abs().max())), (bwd, acc_w, acc_b)
+            assert (db3 - (1 + acc_b) * db).abs().max() < 1e-5, (bwd, acc_w, acc_b)
 
 
 @pytest.mark.parametrize("C", [10, 300])                  # the tensor-core head, and the CUDA-core logits + xent_rows
@@ -127,7 +134,7 @@ def test_head_edges_against_fp64(E, dev, C):
     dloss = 0.37
     dW = torch.full((H, C), 7.0, device=dev)
     db = torch.full((C,), 7.0, device=dev)
-    dh = E.head_bwd(hd, Wd, dlog, torch.tensor([dloss], device=dev), dW, db, False)
+    dh = E.head_bwd(hd, Wd, dlog, torch.tensor([dloss], device=dev), dW, db, False, False)
     # the backward against fp64 products of the dlogits it is given: where the classes tie at logits near 160, fp32's
     # lse = max + log(sum) carries an absolute error of up to half an ulp of 160, so dlogits (checked above) sit up to
     # ~1e-5 relative from fp64, and dW[0, 3] = 0.37 x 40 x sum over 100 rows cancels to 0 in fp64 but not in that error

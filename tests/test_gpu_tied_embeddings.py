@@ -108,26 +108,25 @@ def test_class_major_needs_a_packed_aligned_table():
         E.vocab_head_fwd(h.reshape(T * B, H), off, True, b, labels, None, T, part)
 
 
-def test_op_with_direct_gradients_off(monkeypatch):
-    """``LSTM_TS_DIRECT_GRADS=0``: the table's gradient leaves the op through autograd in the table's layout."""
+def test_op_gradients_with_and_without_a_flat_buffer():
+    """A table and bias outside any flat buffer: their gradients leave the op through autograd in the table's layout, with the
+    same bits as the ones written straight into the flat buffer's sinks."""
     from lstm_tensorspark_b200.models.flat import FlatParams
-    from lstm_tensorspark_b200.ops import cuda_lstm
     from lstm_tensorspark_b200.ops import functional as F
     T, B, H, Cn = 6, 50, 128, 1024
     h, W, b, labels, lengths = _inputs(T, B, H, Cn, True, seed=4)
     table = torch.nn.Parameter(W.t().contiguous().bfloat16().float())
     bias = torch.nn.Parameter(b.clone())
+    plain = (torch.nn.Parameter(table.detach().clone()), torch.nn.Parameter(bias.detach().clone()))
     flat = FlatParams([], [table, bias])
     flat.ensure_shadow()
     flat.enable_direct_grads([table, bias])
+    flat.zero_grad()
     want = _run_tied(h, table.detach(), bias.detach(), labels, lengths, dloss=1.0)
-    for direct in (True, False):
-        monkeypatch.setattr(cuda_lstm, "DIRECT_GRADS", direct)
-        flat.grad.zero_()
-        flat.zero_grad()
+    for direct, (tp, bp) in ((True, (table, bias)), (False, plain)):
         hp = h.clone().requires_grad_(True)
-        F.vocab_xent_per_step(hp, table, bias, labels, lengths, class_major=True)[0].backward()
-        assert torch.equal(table.grad, want[4]) and torch.equal(bias.grad, want[5]) and torch.equal(hp.grad, want[3]), direct
+        F.vocab_xent_per_step(hp, tp, bp, labels, lengths, class_major=True)[0].backward()
+        assert torch.equal(tp.grad, want[4]) and torch.equal(bp.grad, want[5]) and torch.equal(hp.grad, want[3]), direct
 
 
 # ---- whole training steps ------------------------------------------------------------------------------------------------------
@@ -211,7 +210,9 @@ def test_eager_and_graph_steps_give_the_same_bits():
 def test_fallback_heads_sum_both_gradients(V, dtype):
     """Inputs the tensor-core head does not take (C < 512; fp32) run the per-step head on ``table.t().contiguous()``: the
     tied engine's table gradient is the untied engine's embedding gradient plus its Dense1 gradient transposed, with the
-    untied Dense1/weights set to the table's transpose.  bf16 runs with the direct gradient sinks on."""
+    untied Dense1/weights set to the table's transpose.  bf16 runs with the direct gradient sinks on.  Both engines run the
+    recurrences with the in-order operand stream (``deterministic``): the two are compared element by element, and the default
+    stream does not give the same bits from run to run."""
     from lstm_tensorspark_b200.config import Config
     from lstm_tensorspark_b200.engine import TrainEngine
     hidden, T, B, E = "128,128", 16, 64, 128
@@ -219,7 +220,7 @@ def test_fallback_heads_sum_both_gradients(V, dtype):
     for tied in (True, False):
         cfg = Config(partitions=1, sync_mode="none", init="scaled", device="cuda", quiet=True, hidden_units=hidden, in_features=E,
                      seq_len=T, batch_size=B, vocab_size=V, next_token=True, tie_embeddings=tied, learning_rate=0.0,
-                     variable_length=True)
+                     variable_length=True, deterministic=True)
         eng = TrainEngine(cfg, 0, 1, None, batch_size=B, device=DEV, dtype=dtype)
         assert bool(eng.flat._direct) == (dtype == torch.bfloat16)
         engines.append(eng)
