@@ -59,6 +59,11 @@ class Config:
                                         # multiplied by a Bernoulli(1-P) mask / (1-P) before the next layer reads it
     weight_drop: float = 0.0            # AWD-LSTM weight drop: in training, every layer direction's recurrent weights W_h are
                                         # multiplied by a Bernoulli(1-P) mask / (1-P) drawn once per step (DropConnect)
+    output_dropout: float = 0.0         # in training, the top layer's output sequence is dropped before the head / pooling reads it
+    input_dropout: float = 0.0          # in training, the embedding output x_t is dropped before the first layer (--vocab_size)
+    embedding_dropout: float = 0.0      # in training, whole rows of the embedding table are dropped for the lookup, one mask per step
+    locked_dropout: bool = False        # --dropout / --output_dropout / --input_dropout draw one mask per sequence and training step,
+                                        # shared by every time step (AWD-LSTM's LockedDropout), not a new mask per step
     per_step_labels: bool = False       # sequence labelling: a label at every time step ([B,T]), the head scores the top layer's
                                         # output at each step (nn.LSTM -> nn.Linear -> cross_entropy over the real positions); a CSV
                                         # row is k*in_features values followed by k labels
@@ -234,6 +239,19 @@ class Config:
                           "(it drops the output of every layer but the last)")
         if not 0.0 <= self.weight_drop < 1.0:
             raise ValueError(f"--weight_drop must satisfy 0 <= P < 1, got {self.weight_drop}")
+        for flag in ("output_dropout", "input_dropout", "embedding_dropout"):
+            p = getattr(self, flag)
+            if not 0.0 <= p < 1.0:
+                raise ValueError(f"--{flag} must satisfy 0 <= P < 1, got {p}")
+            if p > 0 and flag != "output_dropout" and self.vocab_size <= 0:
+                raise ValueError(f"--{flag} needs --vocab_size > 0: it drops the token embedding, and float features have none")
+        if self.output_dropout > 0 and self.pooling == "last" and not self.per_step_labels:
+            raise ValueError("--output_dropout needs a head that reads the top layer's output sequence (--per_step_labels, "
+                             "--next_token or --pooling mean | max | attention): with --pooling last the head reads only the "
+                             "final state, and there is no sequence to drop")
+        if self.locked_dropout and not (self.dropout > 0 or self.output_dropout > 0 or self.input_dropout > 0):
+            warnings.warn("--locked_dropout has no effect without --dropout, --output_dropout or --input_dropout > 0: it shares "
+                          "their masks across time steps")
         if self.sync_mode not in ("param_avg", "grad_allreduce", "none"):
             raise ValueError(f"unknown --sync_mode {self.sync_mode}")
         if not (math.isfinite(self.clip_grad_norm) and self.clip_grad_norm >= 0):
@@ -336,6 +354,17 @@ _HELP = {
                    "matrix W_h (both directions, one-layer models too) is multiplied by a Bernoulli(1 - P) mask scaled by "
                    "1 / (1 - P), one mask per training step shared by every time step and batch row; evaluation and generation "
                    "use the raw weights.  0 = off",
+    "output_dropout": "In training, drop the top layer's output sequence (both directions) with probability P before the head "
+                      "or the pooling reads it (AWD-LSTM's dropout); needs --per_step_labels, --next_token or --pooling mean | "
+                      "max | attention.  0 = off",
+    "input_dropout": "In training, drop the embedding output x_t = Embedding[tok_t] with probability P before the first layer "
+                     "reads it (AWD-LSTM's dropouti); needs --vocab_size > 0.  0 = off",
+    "embedding_dropout": "In training, drop whole rows of the embedding table with probability P for the lookup, one mask over "
+                         "the V ids per training step, kept rows scaled by 1 / (1 - P) (AWD-LSTM's dropoute); needs --vocab_size "
+                         "> 0.  With --tie_embeddings the softmax still reads the raw table.  0 = off",
+    "locked_dropout": "Locked (variational) dropout: --dropout, --output_dropout and --input_dropout draw one mask per sequence "
+                      "and training step, shared by every time step (AWD-LSTM's LockedDropout; Gal & Ghahramani 2016), instead "
+                      "of a new mask at every step",
     "per_step_labels": "Label every time step (sequence labelling): labels [B,T], loss and accuracy over the real positions; "
                        "a CSV row is k*in_features values followed by k labels",
 }

@@ -82,8 +82,10 @@ int ts_seq_pool_attn_bwd(const void*, int, const float*, const float*, const flo
                          float*, void*, float*, unsigned int*, float*, float*, int, int, cudaStream_t);
 int ts_seq_pool_bwd(const float*, const int*, const int*, const float*, const float*, int, int, int, int, void*, int, cudaStream_t);
 void ts_embed_scratch_numel(long long, long long, long long, long long*);
-int ts_embed_fwd(const void*, int, const int*, const int*, int, int, int, int, void*, cudaStream_t);
-int ts_embed_bwd(const void*, int, const int*, const int*, int, int, int, int, float*, int, int*, int*, float*, cudaStream_t);
+int ts_embed_fwd(const void*, int, const int*, const int*, int, int, int, int, void*, const int*, const unsigned int*, const int*,
+                 const unsigned int*, cudaStream_t);
+int ts_embed_bwd(const void*, int, const int*, const int*, int, int, int, int, float*, int, int*, int*, float*, const int*,
+                 const unsigned int*, const int*, const unsigned int*, cudaStream_t);
 int ts_embed_bwd_launches();
 const char* ts_last_error();
 }
@@ -670,16 +672,22 @@ void chk_tokens(const Tensor& tok, const Tensor& like) {
               "tokens must be int32 [B,T] on the table's device");
 }
 
-// table [V,E] (bf16 or fp32), tokens int32 [B,T] -> x [T,B,E] of the table's dtype, time-major
-Tensor embed_fwd(const Tensor& table, const Tensor& tokens, const std::optional<Tensor>& lengths) {
+// table [V,E] (bf16 or fp32), tokens int32 [B,T] -> x [T,B,E] of the table's dtype, time-major.  in_step / in_desc: input
+// dropout over each position's E units, row_step / row_desc: embedding dropout over the V rows (drop_args; None = off).
+Tensor embed_fwd(const Tensor& table, const Tensor& tokens, const std::optional<Tensor>& lengths,
+                 const std::optional<Tensor>& in_step, const std::vector<int64_t>& in_desc,
+                 const std::optional<Tensor>& row_step, const std::vector<int64_t>& row_desc) {
   chk_cuda(table, "table");
   TORCH_CHECK(table.dim() == 2, "embed_fwd: table [V,E]");
   chk_tokens(tokens, table);
   c10::cuda::CUDAGuard g(table.device());
   const int B = tokens.size(0), T = tokens.size(1), V = table.size(0), E = table.size(1);
   auto x = torch::empty({T, B, E}, table.options());
+  unsigned int di[5], de[5];
+  const int* is = drop_args(in_step, in_desc, table, di);
+  const int* rs = drop_args(row_step, row_desc, table, de);
   check(ts_embed_fwd(table.data_ptr(), is_bf16(table), tokens.data_ptr<int>(), lengths_ptr(lengths, B, table), T, B, E, V,
-                     x.data_ptr(), stream()), "embed_fwd");
+                     x.data_ptr(), is, di, rs, de, stream()), "embed_fwd");
   return x;
 }
 
@@ -702,8 +710,11 @@ EmbedScratch embed_scratch(const Tensor& like, int64_t N, int64_t V, int64_t E) 
   return {b[0].data_ptr<int>(), b[1].data_ptr<int>(), b[2].data_ptr<float>()};
 }
 
-// dx [T·B, E] (bf16 or fp32) -> dW fp32 [V,E]: every row written (accumulate false) or added to the rows of ids present
-void embed_bwd(const Tensor& dx, const Tensor& tokens, const std::optional<Tensor>& lengths, Tensor dW, bool accumulate) {
+// dx [T·B, E] (bf16 or fp32) -> dW fp32 [V,E]: every row written (accumulate false) or added to the rows of ids present; the
+// dropout arguments are the forward's (embed_fwd)
+void embed_bwd(const Tensor& dx, const Tensor& tokens, const std::optional<Tensor>& lengths, Tensor dW, bool accumulate,
+               const std::optional<Tensor>& in_step, const std::vector<int64_t>& in_desc,
+               const std::optional<Tensor>& row_step, const std::vector<int64_t>& row_desc) {
   chk_cuda(dx, "dx"); chk_cuda(dW, "dW");
   chk_tokens(tokens, dx);
   const int B = tokens.size(0), T = tokens.size(1);
@@ -711,9 +722,12 @@ void embed_bwd(const Tensor& dx, const Tensor& tokens, const std::optional<Tenso
   const int V = dW.size(0), E = dW.size(1);
   TORCH_CHECK(dx.numel() == (int64_t)T * B * E, "embed_bwd: dx [T·B, E]");
   c10::cuda::CUDAGuard g(dx.device());
+  unsigned int di[5], de[5];
+  const int* is = drop_args(in_step, in_desc, dx, di);
+  const int* rs = drop_args(row_step, row_desc, dx, de);
   auto s = embed_scratch(dx, (int64_t)T * B, V, E);
   check(ts_embed_bwd(dx.data_ptr(), is_bf16(dx), tokens.data_ptr<int>(), lengths_ptr(lengths, B, dx), T, B, E, V,
-                     dW.data_ptr<float>(), accumulate ? 1 : 0, s.zeroed, s.ints, s.floats, stream()), "embed_bwd");
+                     dW.data_ptr<float>(), accumulate ? 1 : 0, s.zeroed, s.ints, s.floats, is, di, rs, de, stream()), "embed_bwd");
 }
 
 // ---- optimizer ----------------------------------------------------------------------------------------------
@@ -1020,8 +1034,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("lengths"), py::arg("T"), py::arg("dv"), py::arg("dba"), py::arg("acc_dv"), py::arg("acc_dba"));
   m.def("seq_pool_bwd", &seq_pool_bwd, py::arg("ds"), py::arg("lengths"), py::arg("T"), py::arg("mode"), py::arg("argmax"),
         py::arg("alpha"), py::arg("G"), py::arg("out_bf16"));
-  m.def("embed_fwd", &embed_fwd, py::arg("table"), py::arg("tokens"), py::arg("lengths"));
-  m.def("embed_bwd", &embed_bwd, py::arg("dx"), py::arg("tokens"), py::arg("lengths"), py::arg("dW"), py::arg("accumulate"));
+  m.def("embed_fwd", &embed_fwd, py::arg("table"), py::arg("tokens"), py::arg("lengths"), py::arg("in_step") = py::none(),
+        py::arg("in_desc") = std::vector<int64_t>{}, py::arg("row_step") = py::none(), py::arg("row_desc") = std::vector<int64_t>{});
+  m.def("embed_bwd", &embed_bwd, py::arg("dx"), py::arg("tokens"), py::arg("lengths"), py::arg("dW"), py::arg("accumulate"),
+        py::arg("in_step") = py::none(), py::arg("in_desc") = std::vector<int64_t>{}, py::arg("row_step") = py::none(),
+        py::arg("row_desc") = std::vector<int64_t>{});
   m.attr("EMBED_BWD_LAUNCHES") = ts_embed_bwd_launches();
   m.def("head_step_fwd", &head_step_fwd, py::arg("h"), py::arg("W"), py::arg("bias"), py::arg("labels"), py::arg("lengths"), py::arg("T"));
   m.def("head_step_bwd", &head_step_bwd, py::arg("h"), py::arg("W"), py::arg("dlogits"), py::arg("dloss"), py::arg("dW"), py::arg("db"),

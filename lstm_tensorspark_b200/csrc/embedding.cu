@@ -55,10 +55,24 @@ TS_DEVICE int block_excl_scan(int v, int* wt, int& total) {
   return base + x - v;
 }
 
-template <typename TT>
+// Keep bit of table row v under the row mask (embedding dropout): unit v % 8 of counter (v / 8, 0, c2, step).
+TS_DEVICE bool row_kept(const ts::DropSpec& d, int v, int V) {
+  return (ts::dropout_keep8(d, (uint32_t)__ldg(d.step), 0, v & ~7, 0, V) >> (v & 7)) & 1u;
+}
+
+// The factor of a kept unit: the scale of whichever mask is on, or their fp32 product with both.
+TS_DEVICE float drop_factor(const ts::DropSpec& di, const ts::DropSpec& de) {
+  if (di.step && de.step) return __fmul_rn(de.scale, di.scale);
+  return di.step ? di.scale : de.scale;
+}
+
+// kMask: the gather under input dropout (di, over the E units of row (t, b)) and / or embedding dropout (de, whole table rows);
+// either spec may be null (step == nullptr).  Dropped units and rows write +0; a dropped row is not read.
+template <typename TT, bool kMask>
 __global__ void __launch_bounds__(kFwdThreads) embed_fwd_kernel(const TT* __restrict__ table, const int* __restrict__ tok,
                                                                 const int* __restrict__ lengths, int T, int B, int E, int V,
-                                                                long long N, int vec, TT* __restrict__ x) {
+                                                                long long N, int vec, TT* __restrict__ x, ts::DropSpec di,
+                                                                ts::DropSpec de) {
   const long long r = (long long)blockIdx.x * (kFwdThreads / 32) + (threadIdx.x >> 5);
   if (r >= N) return;
   const int lane = threadIdx.x & 31;
@@ -70,6 +84,29 @@ __global__ void __launch_bounds__(kFwdThreads) embed_fwd_kernel(const TT* __rest
     if (v >= 0 && v < V) id = v;
   }
   TT* dst = x + r * E;
+  if constexpr (kMask) {
+    if (id >= 0 && de.step && !row_kept(de, id, V)) id = -1;
+    const float f = drop_factor(di, de);
+    const uint32_t step_i = di.step ? (uint32_t)__ldg(di.step) : 0u;
+    const TT* src = table + (size_t)(id < 0 ? 0 : id) * E;
+    if (vec && sizeof(TT) == 2) {                              // a 16 B chunk = 8 units = one Philox group
+      const int nv = E / 8;
+      uint4* d4 = reinterpret_cast<uint4*>(dst);
+      const uint4* s4 = reinterpret_cast<const uint4*>(src);
+      for (int k = lane; k < nv; k += 32) {
+        if (id < 0) { d4[k] = make_uint4(0u, 0u, 0u, 0u); continue; }
+        const uint32_t keep = di.step ? ts::dropout_keep8(di, step_i, b, 8 * k, t, E) : 0xffu;
+        d4[k] = keep ? ts::dropout_bf16x8(__ldg(s4 + k), keep, f) : make_uint4(0u, 0u, 0u, 0u);
+      }
+      return;
+    }
+    for (int k = lane; k < E; k += 32) {
+      bool kept = id >= 0;
+      if (kept && di.step) kept = (ts::dropout_keep8(di, step_i, b, k & ~7, t, E) >> (k & 7)) & 1u;
+      dst[k] = kept ? ts::Cvt<TT>::from_f(__fmul_rn(ts::Cvt<TT>::to_f(src[k]), f)) : ts::Cvt<TT>::from_f(0.f);
+    }
+    return;
+  }
   if (vec) {
     const int nv = (int)(E * sizeof(TT) / 16);
     uint4* d4 = reinterpret_cast<uint4*>(dst);
@@ -182,12 +219,15 @@ __global__ void __launch_bounds__(kChunk) embed_plan_kernel(int V, int N, int nc
   }
 }
 
-template <typename TD>
+// kMask: the table gradient under the gather's masks.  Row r = t·B + b adds float(dx) * s_i where input-kept and 0 where dropped
+// (plain float(dx) without input dropout), in the same row and piece order; the id's sum is multiplied once by s_e.  A dropped
+// id writes 0 (overwrite) or nothing (accumulate) and reads no dx.
+template <typename TD, bool kMask>
 __global__ void __launch_bounds__(kSumThreads) embed_sum_kernel(const TD* __restrict__ dx, int E, int V, const int* __restrict__ offs,
                                                                 const int* __restrict__ xoff, const int* __restrict__ poff,
                                                                 const int* __restrict__ sorted, float* __restrict__ partial,
                                                                 unsigned int* __restrict__ tickets, float* __restrict__ dW,
-                                                                int accumulate) {
+                                                                int accumulate, int B, ts::DropSpec di, ts::DropSpec de) {
   __shared__ int rows[kSeg];
   __shared__ bool last_s;
   int v, j;
@@ -207,8 +247,10 @@ __global__ void __launch_bounds__(kSumThreads) embed_sum_kernel(const TD* __rest
   }
   const int beg = offs[v], c = offs[v + 1] - beg;
   float* out = dW + (size_t)v * E;
-  if (c == 0) {
-    if (!accumulate)
+  bool dropped = false;
+  if constexpr (kMask) dropped = de.step && !row_kept(de, v, V);
+  if (c == 0 || dropped) {
+    if (!accumulate && (!kMask || j == 0))
       for (int col = threadIdx.x; col < E; col += kSumThreads) out[col] = 0.f;
     return;
   }
@@ -217,12 +259,46 @@ __global__ void __launch_bounds__(kSumThreads) embed_sum_kernel(const TD* __rest
   if ((int)threadIdx.x < nr) rows[threadIdx.x] = sorted[beg + r0 + threadIdx.x];
   __syncthreads();
   float* dst = pieces == 1 ? nullptr : partial + (size_t)(poff[v] + j) * E;
-  for (int col = threadIdx.x; col < E; col += kSumThreads) {
-    float acc = 0.f;
+  const float se = kMask && de.step ? de.scale : 1.f;
+  if constexpr (kMask) {
+    // one thread per group of 8 columns: one Philox call per (row, group)
+    const uint32_t step_i = di.step ? (uint32_t)__ldg(di.step) : 0u;
+    for (int g0 = 8 * threadIdx.x; g0 < E; g0 += 8 * kSumThreads) {
+      const int ng = min(8, E - g0);
+      float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+      for (int q = 0; q < nr; ++q) {
+        const int r = rows[q], t = r / B, b = r - t * B;
+        const TD* src = dx + (size_t)r * E + g0;
+        if (di.step) {
+          const uint32_t keep = ts::dropout_keep8(di, step_i, b, g0, t, E);
+#pragma unroll
+          for (int i = 0; i < 8; ++i)
+            if (i < ng) acc[i] += ((keep >> i) & 1u) ? __fmul_rn(ts::Cvt<TD>::to_f(src[i]), di.scale) : 0.f;
+        } else {
+#pragma unroll
+          for (int i = 0; i < 8; ++i)
+            if (i < ng) acc[i] += ts::Cvt<TD>::to_f(src[i]);
+        }
+      }
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        if (i >= ng) break;
+        if (pieces == 1) {
+          const float a = __fmul_rn(acc[i], se);
+          out[g0 + i] = accumulate ? out[g0 + i] + a : a;
+        } else {
+          dst[g0 + i] = acc[i];
+        }
+      }
+    }
+  } else {
+    for (int col = threadIdx.x; col < E; col += kSumThreads) {
+      float acc = 0.f;
 #pragma unroll 4
-    for (int q = 0; q < nr; ++q) acc += ts::Cvt<TD>::to_f(dx[(size_t)rows[q] * E + col]);
-    if (pieces == 1) out[col] = accumulate ? out[col] + acc : acc;
-    else dst[col] = acc;
+      for (int q = 0; q < nr; ++q) acc += ts::Cvt<TD>::to_f(dx[(size_t)rows[q] * E + col]);
+      if (pieces == 1) out[col] = accumulate ? out[col] + acc : acc;
+      else dst[col] = acc;
+    }
   }
   if (pieces == 1) return;
   __threadfence();
@@ -235,6 +311,7 @@ __global__ void __launch_bounds__(kSumThreads) embed_sum_kernel(const TD* __rest
   for (int col = threadIdx.x; col < E; col += kSumThreads) {
     float acc = 0.f;
     for (int q = 0; q < pieces; ++q) acc += __ldcg(p + (size_t)q * E + col);
+    if constexpr (kMask) acc = __fmul_rn(acc, se);
     out[col] = accumulate ? out[col] + acc : acc;
   }
   if (threadIdx.x == 0) tickets[v] = 0u;
@@ -274,25 +351,34 @@ extern "C" void ts_embed_scratch_numel(long long N, long long V, long long E, lo
   ints[1] = (2 * (N / kSeg) + 2) * E;        // pieces of multi-piece ids: sum ceil(c / kSeg) over c > kSeg <= 2 N / kSeg
 }
 
-// table [V, E] (bf16 iff bf16), tok int32 [B, T], lengths int32 [B] or null -> x [T·B, E] of the table's type.
+// table [V, E] (bf16 iff bf16), tok int32 [B, T], lengths int32 [B] or null -> x [T·B, E] of the table's type.  Dropout
+// (ts::make_drop_spec): in_step / in_desc = input dropout over the E units of each position, row_step / row_desc = embedding
+// dropout over the V rows; null steps = off, and with both off the unmasked kernel runs.
 extern "C" int ts_embed_fwd(const void* table, int bf16, const int* tok, const int* lengths, int T, int B, int E, int V, void* x,
+                            const int* in_step, const unsigned int* in_desc, const int* row_step, const unsigned int* row_desc,
                             cudaStream_t st) {
   if (T < 1 || B < 1 || E < 1 || V < 1) return -2;
   const long long N = (long long)T * B;
   const size_t elt = bf16 ? 2 : 4;
   const int vec = ((size_t)E * elt) % 16 == 0 && ((uintptr_t)table % 16) == 0 && ((uintptr_t)x % 16) == 0;
   const unsigned grid = (unsigned)((N + kFwdThreads / 32 - 1) / (kFwdThreads / 32));
-  if (bf16)
-    embed_fwd_kernel<__nv_bfloat16><<<grid, kFwdThreads, 0, st>>>((const __nv_bfloat16*)table, tok, lengths, T, B, E, V, N, vec,
-                                                                  (__nv_bfloat16*)x);
-  else
-    embed_fwd_kernel<float><<<grid, kFwdThreads, 0, st>>>((const float*)table, tok, lengths, T, B, E, V, N, vec, (float*)x);
+  const ts::DropSpec di = ts::make_drop_spec(in_step, in_desc), de = ts::make_drop_spec(row_step, row_desc);
+  const bool mask = in_step || row_step;
+  if (bf16) {
+    auto k = mask ? embed_fwd_kernel<__nv_bfloat16, true> : embed_fwd_kernel<__nv_bfloat16, false>;
+    k<<<grid, kFwdThreads, 0, st>>>((const __nv_bfloat16*)table, tok, lengths, T, B, E, V, N, vec, (__nv_bfloat16*)x, di, de);
+  } else {
+    auto k = mask ? embed_fwd_kernel<float, true> : embed_fwd_kernel<float, false>;
+    k<<<grid, kFwdThreads, 0, st>>>((const float*)table, tok, lengths, T, B, E, V, N, vec, (float*)x, di, de);
+  }
   return (int)cudaGetLastError();
 }
 
-// dx [T·B, E] (bf16 iff dx_bf16) -> dW fp32 [V, E]: overwrite every row (accumulate = 0) or add to the rows of ids present.
+// dx [T·B, E] (bf16 iff dx_bf16) -> dW fp32 [V, E]: overwrite every row (accumulate = 0) or add to the rows of ids present.  The
+// dropout arguments are the forward's: the sum kernel then applies the same masks (ts_embed_fwd).
 extern "C" int ts_embed_bwd(const void* dx, int dx_bf16, const int* tok, const int* lengths, int T, int B, int E, int V, float* dW,
-                            int accumulate, int* zeroed, int* scratch, float* partial, cudaStream_t st) {
+                            int accumulate, int* zeroed, int* scratch, float* partial, const int* in_step,
+                            const unsigned int* in_desc, const int* row_step, const unsigned int* row_desc, cudaStream_t st) {
   if (T < 1 || B < 1 || E < 1 || V < 1) return -2;
   const long long N64 = (long long)T * B;
   if (N64 > (1LL << 30) || (long long)V > (1LL << 30)) return -3;
@@ -306,12 +392,17 @@ extern "C" int ts_embed_bwd(const void* dx, int dx_bf16, const int* tok, const i
   embed_plan_kernel<<<1, kChunk, 0, st>>>(V, N, nchunks, counts, s.offs, s.xoff, s.poff, s.cursor, s.elem_run, s.elem_rank,
                                           s.run_id, s.run_cnt, s.run_base, s.nruns, s.sorted);
   const unsigned grid = (unsigned)(V + N / kSeg + 1);          // one CTA per id + at most N / kSeg further pieces
-  if (dx_bf16)
-    embed_sum_kernel<__nv_bfloat16><<<grid, kSumThreads, 0, st>>>((const __nv_bfloat16*)dx, E, V, s.offs, s.xoff, s.poff, s.sorted,
-                                                                  partial, tickets, dW, accumulate);
-  else
-    embed_sum_kernel<float><<<grid, kSumThreads, 0, st>>>((const float*)dx, E, V, s.offs, s.xoff, s.poff, s.sorted, partial,
-                                                          tickets, dW, accumulate);
+  const ts::DropSpec di = ts::make_drop_spec(in_step, in_desc), de = ts::make_drop_spec(row_step, row_desc);
+  const bool mask = in_step || row_step;
+  if (dx_bf16) {
+    auto k = mask ? embed_sum_kernel<__nv_bfloat16, true> : embed_sum_kernel<__nv_bfloat16, false>;
+    k<<<grid, kSumThreads, 0, st>>>((const __nv_bfloat16*)dx, E, V, s.offs, s.xoff, s.poff, s.sorted, partial, tickets, dW,
+                                    accumulate, B, di, de);
+  } else {
+    auto k = mask ? embed_sum_kernel<float, true> : embed_sum_kernel<float, false>;
+    k<<<grid, kSumThreads, 0, st>>>((const float*)dx, E, V, s.offs, s.xoff, s.poff, s.sorted, partial, tickets, dW, accumulate,
+                                    B, di, de);
+  }
   return (int)cudaGetLastError();
 }
 

@@ -59,6 +59,11 @@ TS_DEVICE uint4 philox4x32_10(uint4 c, uint2 k) {
 //   key (key0, key1) = (seed, partition); counter = (b * ceil(H/8) + j/8, t, c2 = 2 * layer + reverse, step).
 //   The 4 words give eight 16-bit values: unit 8g + i uses word i/2, low half for even i.  Kept iff value >= thr.
 //   A kept value is multiplied by scale = 65536 / (65536 - thr) in fp32 (exact expectation for the quantised P).
+// c2 also tells the other mask sites apart (bits above the layer index): weight drop, the embedding's input and row masks.
+// kDropLocked in c2 makes the mask locked (AWD-LSTM's LockedDropout): the time word is 0, so every step shares one mask.
+constexpr uint32_t kDropLocked = 0x20000000u;
+constexpr uint32_t kDropInput = 0x40000000u;     // the embedding output x_t (counter over its E units)
+constexpr uint32_t kDropRows = 0x10000000u;      // whole rows of the embedding table (one time step, one row of V units)
 struct DropSpec {
   const int* step;        // device-resident step counter (c3): a captured CUDA graph reads the current value
   uint32_t key0, key1;
@@ -81,7 +86,8 @@ inline DropSpec make_drop_spec(const int* step, const unsigned int* desc) {
 // Keep bits of the 8 hidden units [j, j + 8) (j % 8 == 0) of local batch row b at time t: bit i = unit j + i.
 TS_DEVICE uint32_t dropout_keep8(const DropSpec& d, uint32_t step, int b, int j, int t, int H) {
   const uint32_t c0 = (uint32_t)(b + d.row0) * (uint32_t)((H + 7) / 8) + (uint32_t)(j >> 3);
-  const uint4 r = philox4x32_10(make_uint4(c0, (uint32_t)t, d.c2, step), make_uint2(d.key0, d.key1));
+  const uint32_t tw = (d.c2 & kDropLocked) ? 0u : (uint32_t)t;
+  const uint4 r = philox4x32_10(make_uint4(c0, tw, d.c2, step), make_uint2(d.key0, d.key1));
   const uint32_t w[4] = {r.x, r.y, r.z, r.w};
   uint32_t keep = 0;
 #pragma unroll

@@ -81,11 +81,12 @@ class TrainEngine:
         self._bound = {}                        # (x ptr, y ptr, lengths ptr, shape) -> (graph captured on those buffers, its loss)
         self._bound_keepalive = []
         self.steps_done = 0
-        # dropout between layers and weight drop: the masks are keyed on (seed, partition) and on the number of training steps
-        # this engine has completed - a counter of its own, device-resident on the GPU (a captured graph advances it; the
-        # optimizer's step_dev is bumped before backward by the fused allreduce and never by SGD), a host int on the CPU
+        # every dropout (between layers, output, input, embedding rows, weight drop): the masks are keyed on (seed, partition)
+        # and on the number of training steps this engine has completed - a counter of its own, device-resident on the GPU (a
+        # captured graph advances it; the optimizer's step_dev is bumped before backward by the fused allreduce and never by
+        # SGD), a host int on the CPU
         rnn = self.model.rnn
-        self._dropout_on = (rnn.dropout > 0 and len(rnn.layers) > 1) or rnn.weight_drop > 0
+        self._dropout_on = rnn.draws_masks
         rnn.dropout_key = (cfg.seed & 0xFFFFFFFF, rank if partition_key is None else int(partition_key))
         rnn.dropout_step = torch.zeros(1, dtype=torch.int32, device=device) if device.type == "cuda" else 0
         # --stateful: static buffers per layer (h in the compute dtype, as the kernels store it; c fp32).  `state` is what the next

@@ -71,8 +71,9 @@ class Embedding(nn.Module):
         self.weights = create_variable("weights", (vocab_size, dim), device=device, generator=generator,
                                        initializer=lambda t, generator=None: truncated_normal_(t, init_std, generator))
 
-    def forward(self, tokens: torch.Tensor, lengths: Optional[torch.Tensor] = None, dtype=None) -> torch.Tensor:
-        return F.embedding(tokens, self.weights, lengths, dtype)
+    def forward(self, tokens: torch.Tensor, lengths: Optional[torch.Tensor] = None, dtype=None, input_dropout=None,
+                embedding_dropout=None) -> torch.Tensor:
+        return F.embedding(tokens, self.weights, lengths, dtype, input_dropout, embedding_dropout)
 
 
 class SequenceClassifier(nn.Module):
@@ -85,7 +86,10 @@ class SequenceClassifier(nn.Module):
         settings = cfg.net_settings(bs)
         head_in = settings[-1]["num_hidden"] * (2 if cfg.bidirectional else 1)
         head_std = cfg.init_std if cfg.init != "scaled" else cfg.init_std / (head_in ** 0.5)
-        self.rnn = RNN(settings, dropout=cfg.dropout, weight_drop=getattr(cfg, "weight_drop", 0.0), learn_initial_state=cfg.resolved_learn_initial_state(), init_std=cfg.init_std,
+        self.rnn = RNN(settings, dropout=cfg.dropout, weight_drop=getattr(cfg, "weight_drop", 0.0),
+                       output_dropout=getattr(cfg, "output_dropout", 0.0), input_dropout=getattr(cfg, "input_dropout", 0.0),
+                       embedding_dropout=getattr(cfg, "embedding_dropout", 0.0),
+                       locked=getattr(cfg, "locked_dropout", False), learn_initial_state=cfg.resolved_learn_initial_state(), init_std=cfg.init_std,
                        init=cfg.init, weight_decay=(cfg.weight_decay or None), device=device, generator=generator)
         # --tie_embeddings: the softmax reads the embedding table (head_weights); Dense1/weights is drawn and discarded
         self.tied = bool(getattr(cfg, "tie_embeddings", False))
@@ -163,7 +167,8 @@ class SequenceClassifier(nn.Module):
             return x.to(self.compute_dtype) if x.is_floating_point() else x
         if x.is_floating_point() or x.dim() not in (1, 2):
             raise ValueError(f"--vocab_size needs integer token ids [B,T] (one step: [B]), got {x.dtype} {tuple(x.shape)}")
-        e = self.embedding(x, lengths if x.dim() == 2 else None, self.compute_dtype)
+        e = self.embedding(x, lengths if x.dim() == 2 else None, self.compute_dtype, self.rnn.input_dropout_spec(),
+                           self.rnn.embedding_dropout_spec())
         return e[0] if x.dim() == 1 else e.transpose(0, 1)
 
     def _start(self, batch_size: int, state) -> None:

@@ -8,6 +8,10 @@ through time on the fused per-layer sequence op (the reference only ever takes o
 ``add_reverse_layers()`` makes the stack bidirectional, and ``dropout`` drops the output of every layer but the last while
 the module is in training mode (``nn.LSTM(dropout=...)``).  ``weight_drop`` drops connections of every layer direction's
 recurrent weights ``W_h`` in training mode, one mask per training step (AWD-LSTM's ``WeightDrop``, Merity et al. 2017).
+``output_dropout`` drops the top layer's output sequence, ``input_dropout`` the embedding output and ``embedding_dropout``
+whole rows of the embedding table (the model's embedding reads ``input_dropout_spec`` / ``embedding_dropout_spec``);
+``locked`` shares one mask of ``dropout``, ``output_dropout`` and ``input_dropout`` across every time step (AWD-LSTM's
+``LockedDropout``).
 """
 from __future__ import annotations
 
@@ -23,17 +27,22 @@ EXPORT_KEYS = ("wf", "wi", "wo", "wc", "bf", "bi", "bc", "bo")
 
 
 class RNN(nn.Module):
-    def __init__(self, settings: Iterable[dict], dropout: float = 0.0, weight_drop: float = 0.0, **layer_kw):
+    def __init__(self, settings: Iterable[dict], dropout: float = 0.0, weight_drop: float = 0.0, output_dropout: float = 0.0,
+                 input_dropout: float = 0.0, embedding_dropout: float = 0.0, locked: bool = False, **layer_kw):
         super().__init__()
-        if not 0.0 <= dropout < 1.0:
-            raise ValueError(f"dropout must satisfy 0 <= P < 1, got {dropout}")
-        if not 0.0 <= weight_drop < 1.0:
-            raise ValueError(f"weight_drop must satisfy 0 <= P < 1, got {weight_drop}")
+        for name, p in (("dropout", dropout), ("weight_drop", weight_drop), ("output_dropout", output_dropout),
+                        ("input_dropout", input_dropout), ("embedding_dropout", embedding_dropout)):
+            if not 0.0 <= p < 1.0:
+                raise ValueError(f"{name} must satisfy 0 <= P < 1, got {p}")
         self.layers = nn.ModuleList()
         self.reverse_layers = nn.ModuleList()      # empty, or one reverse-time layer per entry of ``layers``
         self._layer_kw = layer_kw
         self.dropout = float(dropout)
         self.weight_drop = float(weight_drop)
+        self.output_dropout = float(output_dropout)
+        self.input_dropout = float(input_dropout)
+        self.embedding_dropout = float(embedding_dropout)
+        self.locked = bool(locked)
         # the mask's key (seed, partition) and step counter (training steps completed: an int32 [1] device tensor on the GPU,
         # an int on the CPU); a TrainEngine sets and advances them
         self.dropout_key = (0, 0)
@@ -41,10 +50,32 @@ class RNN(nn.Module):
         self.add_layers(settings)
 
     def dropout_spec(self, layer: int, reverse: bool = False) -> Optional[DropoutSpec]:
-        """The dropout of layer ``layer``'s output in this forward pass: None for the top layer, with P = 0 and in eval mode."""
-        if not self.training or self.dropout == 0 or layer >= len(self.layers) - 1:
+        """The dropout of layer ``layer``'s output in this forward pass: ``dropout`` below the top layer, ``output_dropout`` for
+        the top layer; None with P = 0 and in eval mode."""
+        p = self.output_dropout if layer >= len(self.layers) - 1 else self.dropout
+        if not self.training or p == 0:
             return None
-        return DropoutSpec(self.dropout, self.dropout_key, layer, reverse, self.dropout_step)
+        return DropoutSpec(p, self.dropout_key, layer, reverse, self.dropout_step, locked=self.locked)
+
+    def input_dropout_spec(self) -> Optional[DropoutSpec]:
+        """The dropout of the embedding output ``x_t`` (``"input"`` site) in this forward pass; None with P = 0 and in eval
+        mode."""
+        if not self.training or self.input_dropout == 0:
+            return None
+        return DropoutSpec(self.input_dropout, self.dropout_key, 0, False, self.dropout_step, site="input", locked=self.locked)
+
+    def embedding_dropout_spec(self) -> Optional[DropoutSpec]:
+        """The dropout of whole embedding-table rows (``"rows"`` site, one mask per training step); None with P = 0 and in eval
+        mode."""
+        if not self.training or self.embedding_dropout == 0:
+            return None
+        return DropoutSpec(self.embedding_dropout, self.dropout_key, 0, False, self.dropout_step, site="rows")
+
+    @property
+    def draws_masks(self) -> bool:
+        """Does a training step draw any mask (the step counter must then advance)?"""
+        return ((self.dropout > 0 and len(self.layers) > 1) or self.weight_drop > 0 or self.output_dropout > 0
+                or self.input_dropout > 0 or self.embedding_dropout > 0)
 
     def weight_drop_spec(self, layer: int, reverse: bool = False) -> Optional[DropoutSpec]:
         """The weight drop of layer ``layer``'s ``W_h`` (direction ``reverse``) in this forward pass: every layer, the top one

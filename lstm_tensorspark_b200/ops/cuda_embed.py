@@ -6,12 +6,14 @@ lengths are read there too (no host sync: a captured graph holds across token ba
   backward  the first layer's ``dx`` (its wgmma dX GEMM) -> ``dEmbedding`` straight into the table's flat gradient sink, in three
             launches (rank, plan, sum): a stable counting sort of the counted positions by id and a fixed-order fp32 sum per id,
             so the result is bitwise reproducible and independent of the grid.
+Dropout (``input_dropout`` over each position's E units, ``embedding_dropout`` over whole table rows): the gather and the sum
+launch their masked instantiations, which draw the masks in place (``reference.embedding``); the launch count is unchanged.
 Semantics: ``reference.embedding``."""
 from __future__ import annotations
 
 import torch
 
-from .cuda_ext import LAUNCHES, count, ext
+from .cuda_ext import LAUNCHES, count, drop_args, ext
 from .params import grad_out, lowp
 
 
@@ -22,15 +24,20 @@ def _tokens(tokens: torch.Tensor) -> torch.Tensor:
 
 class _EmbedFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, tokens, table, lengths, dtype):
+    def forward(ctx, tokens, table, lengths, dtype, input_dropout, embedding_dropout):
         tok = _tokens(tokens)
         if tok.device != table.device:
             raise ValueError(f"tokens on {tok.device}, the embedding table on {table.device}")
         tab = lowp(table, torch.bfloat16) if dtype == torch.bfloat16 else table.detach().float().contiguous()
         ln = None if lengths is None else lengths.contiguous()
-        x = ext().embed_fwd(tab, tok, ln)
+        di, de = drop_args(input_dropout, tab.device), drop_args(embedding_dropout, tab.device)
+        drop = {"in_step": di.get("drop_step"), "in_desc": di.get("drop_desc", []),
+                "row_step": de.get("drop_step"), "row_desc": de.get("drop_desc", [])}
+        x = ext().embed_fwd(tab, tok, ln, **drop)
         count("embed_fwd")
-        ctx.tok, ctx.ln, ctx.addr, ctx.shape = tok, ln, table.data_ptr(), tuple(table.shape)
+        if di or de:
+            count("embed_fwd_dropout")
+        ctx.tok, ctx.ln, ctx.addr, ctx.shape, ctx.drop = tok, ln, table.data_ptr(), tuple(table.shape), drop
         return x if x.dtype == dtype else x.to(dtype)
 
     @staticmethod
@@ -41,13 +48,15 @@ class _EmbedFn(torch.autograd.Function):
             d = d.float()
         d = d.contiguous()
         out, acc, ret = grad_out(ctx.addr, ctx.shape, d.device)
-        E.embed_bwd(d, ctx.tok, ctx.ln, out, acc)
+        E.embed_bwd(d, ctx.tok, ctx.ln, out, acc, **ctx.drop)
         LAUNCHES["n"] += E.EMBED_BWD_LAUNCHES - 1
         count("embed_bwd")
-        return None, ret, None, None
+        if ctx.drop["in_step"] is not None or ctx.drop["row_step"] is not None:
+            count("embed_bwd_dropout")
+        return None, ret, None, None, None, None
 
 
-def embedding(tokens, table, lengths=None, dtype=None):
+def embedding(tokens, table, lengths=None, dtype=None, input_dropout=None, embedding_dropout=None):
     if tokens.is_floating_point():
         raise ValueError(f"--vocab_size needs integer token ids, got {tokens.dtype}")
-    return _EmbedFn.apply(tokens, table, lengths, table.dtype if dtype is None else dtype)
+    return _EmbedFn.apply(tokens, table, lengths, table.dtype if dtype is None else dtype, input_dropout, embedding_dropout)

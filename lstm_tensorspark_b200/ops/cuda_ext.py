@@ -7,12 +7,14 @@ from __future__ import annotations
 import importlib
 import os
 
+import torch
+
 _EXT = None
 _ERR = None
 LAUNCHES = {"n": 0}          # number of OUR kernels launched through the extension (bench.py "gpu_launches")
 # which paths the ops took (also read as ``cuda_lstm.STATS``): fixed keys are incremented in place, the others through ``count``
 STATS = {"fast_fwd": 0, "fast_bwd": 0, "generic_fwd": 0, "generic_bwd": 0, "tc_gemm": 0, "kernels": 0, "weight_drop": 0,
-         "weight_drop_grad": 0}
+         "weight_drop_grad": 0, "embed_fwd_dropout": 0, "embed_bwd_dropout": 0}
 _NO_KERNEL = {"ar_max_blocks", "ar_flag_words", "ar_slots"}
 
 
@@ -37,6 +39,15 @@ class _Counting:
         object.__setattr__(self, name, call)
         return call
 
+def drop_args(spec, device) -> dict:
+    """Keyword arguments of the kernels for a ``reference.DropoutSpec`` (none for None / P = 0): the device-resident step
+    counter and the descriptor {key0, key1, thr, c2, row0}."""
+    if spec is None or spec.p == 0:
+        return {}
+    step = spec.step
+    if not isinstance(step, torch.Tensor):                       # (a caller without an engine: no graph capture to honour)
+        step = torch.tensor([int(step)], dtype=torch.int32, device=device)
+    return {"drop_step": step, "drop_desc": spec.desc()}
 
 
 def ext():

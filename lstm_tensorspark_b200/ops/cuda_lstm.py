@@ -17,6 +17,7 @@ from typing import Optional
 import torch
 
 from .cuda_ext import STATS, count, ext
+from .cuda_ext import drop_args as _drop_args
 from .params import grad_out, lowp
 from . import cuda_gemm as G
 
@@ -264,17 +265,6 @@ def _check_lengths_arg(lengths: Optional[torch.Tensor], B: int, device) -> None:
                                 or not lengths.is_contiguous()):
         raise ValueError(f"lengths must be a contiguous int32 [{B}] tensor on {device}, got {lengths.dtype} "
                          f"{tuple(lengths.shape)} on {lengths.device}")
-
-
-def _drop_args(spec, device) -> dict:
-    """Keyword arguments of the kernels for a ``reference.DropoutSpec`` (none for None / P = 0): the device-resident step
-    counter and the descriptor {key0, key1, thr, c2, row0}."""
-    if spec is None or spec.p == 0:
-        return {}
-    step = spec.step
-    if not isinstance(step, torch.Tensor):                       # (a caller without an engine: no graph capture to honour)
-        step = torch.tensor([int(step)], dtype=torch.int32, device=device)
-    return {"drop_step": step, "drop_desc": spec.desc()}
 
 
 def _weight_image(w_h_c: torch.Tensor, spec) -> torch.Tensor:

@@ -172,14 +172,15 @@ def pool_sequence(h_seq, lengths=None, mode: str = "mean", attention=None):
     return ref.pool_sequence(h_seq, lengths, mode, attention)
 
 
-def embedding(tokens, table, lengths=None, dtype=None):
+def embedding(tokens, table, lengths=None, dtype=None, input_dropout=None, embedding_dropout=None):
     """``tokens`` int ``[B,T]`` (int64 is cast to int32) or ``[B]`` -> ``x [T,B,E]``, time-major, in ``dtype`` (the compute dtype;
-    default the table's) (``reference.embedding``).  On the GPU the bf16 path reads the table's maintained bf16 shadow."""
+    default the table's) (``reference.embedding``).  On the GPU the bf16 path reads the table's maintained bf16 shadow.
+    ``input_dropout`` / ``embedding_dropout``: optional ``reference.DropoutSpec`` of the ``"input"`` and ``"rows"`` sites."""
     dtype = table.dtype if dtype is None else dtype
     if _use_ext(table):
         from . import cuda_embed
-        return cuda_embed.embedding(tokens, table, lengths, dtype)
-    return ref.embedding(tokens, table, lengths).to(dtype)
+        return cuda_embed.embedding(tokens, table, lengths, dtype, input_dropout, embedding_dropout)
+    return ref.embedding(tokens, table, lengths, input_dropout, embedding_dropout).to(dtype)
 
 
 def lstm_pair_supported(x_seq, h_a: int, h_b: int) -> bool:

@@ -82,6 +82,10 @@ def philox4x32_10(ctr: torch.Tensor, key0, key1) -> torch.Tensor:
 
 
 WEIGHT_DROP_C2 = 0x80000000      # high bit of c2: the weight-drop masks (DropoutSpec.weight)
+INPUT_DROP_C2 = 0x40000000       # the embedding output x_t, over its E units (DropoutSpec.site "input")
+LOCKED_C2 = 0x20000000           # a locked mask: the counter's time word is 0, one mask for every step (DropoutSpec.locked)
+ROW_DROP_C2 = 0x10000000         # whole rows of the embedding table (DropoutSpec.site "rows")
+DROPOUT_SITES = ("layer", "input", "rows")
 
 
 def dropout_threshold(p: float) -> int:
@@ -103,7 +107,12 @@ class DropoutSpec:
     reads its current value), an int on the CPU.  ``row0``: batch row of local row 0 (batch chunks).
 
     ``weight``: the weight-drop stream instead (DropConnect on the layer direction's ``W_h [4H, H]``, ``weight_drop``): the
-    matrix is one time step of 4H rows and c2 = 0x80000000 | (2 layer + reverse), apart from every output stream's c2 < 2^31."""
+    matrix is one time step of 4H rows and c2 = 0x80000000 | (2 layer + reverse), apart from every output stream's c2 < 2^31.
+
+    ``site``: ``"layer"`` (a layer's output: between layers, and the top layer's with ``--output_dropout``), ``"input"`` (the
+    embedding output ``x_t [B, E]``, c2 = 0x40000000; ``layer`` / ``reverse`` unused) or ``"rows"`` (whole rows of the ``[V, E]``
+    embedding table: one step of one row of V units, c2 = 0x10000000).  ``locked``: one mask per sequence and step, shared by
+    every time step (AWD-LSTM's ``LockedDropout``): c2 gains 0x20000000 and the counter's time word is 0 (layer and input sites)."""
     p: float
     key: Tuple[int, int]
     layer: int
@@ -111,6 +120,14 @@ class DropoutSpec:
     step: Union[int, torch.Tensor]
     row0: int = 0
     weight: bool = False
+    site: str = "layer"
+    locked: bool = False
+
+    def __post_init__(self):
+        if self.site not in DROPOUT_SITES:
+            raise ValueError(f"dropout site must be one of {', '.join(DROPOUT_SITES)}, got {self.site!r}")
+        if self.locked and (self.weight or self.site == "rows"):
+            raise ValueError("only the layer and input masks can be locked: weight drop and row masks have no time axis")
 
     @property
     def thr(self) -> int:
@@ -118,7 +135,12 @@ class DropoutSpec:
 
     @property
     def c2(self) -> int:
-        return (WEIGHT_DROP_C2 if self.weight else 0) | (2 * self.layer + int(self.reverse))
+        if self.weight:
+            return WEIGHT_DROP_C2 | (2 * self.layer + int(self.reverse))
+        if self.site == "rows":
+            return ROW_DROP_C2
+        base = INPUT_DROP_C2 if self.site == "input" else 2 * self.layer + int(self.reverse)
+        return (LOCKED_C2 if self.locked else 0) | base
 
     def desc(self):
         """{key0, key1, thr, c2, row0} as the kernels take it."""
@@ -130,10 +152,13 @@ class DropoutSpec:
 
 def dropout_mask(spec: DropoutSpec, T: int, B: int, H: int, t0: int = 0, device=None) -> torch.Tensor:
     """Keep mask ``[T,B,H]`` (bool) of ``spec`` at times ``t0 .. t0 + T - 1``: counter (b * ceil(H/8) + j/8, t, c2, step),
-    unit 8g + i takes 16-bit half (i & 1) of word i/2 and is kept iff that value >= thr."""
+    unit 8g + i takes 16-bit half (i & 1) of word i/2 and is kept iff that value >= thr.  A locked spec's counter has time word
+    0 at every t."""
     step = int(spec.step) & _U32
     g = (H + 7) // 8
     t = torch.arange(t0, t0 + T, dtype=torch.int64, device=device).view(T, 1, 1).expand(T, B, g)
+    if spec.c2 & LOCKED_C2:
+        t = torch.zeros_like(t)
     b = torch.arange(B, dtype=torch.int64, device=device).view(1, B, 1) + spec.row0
     c0 = (b * g + torch.arange(g, dtype=torch.int64, device=device).view(1, 1, g)).expand(T, B, g)
     ctr = torch.stack([c0, t, torch.full_like(c0, spec.c2), torch.full_like(c0, step)], -1)
@@ -422,22 +447,60 @@ def pool_sequence(h_seq, lengths=None, mode: str = "mean", attention=None):
     raise ValueError(f"unknown pooling {mode!r}: one of {', '.join(POOLING_MODES)}")
 
 
-def embedding(tokens, table, lengths=None):
+def embedding_row_mask(spec: DropoutSpec, V: int, device=None) -> torch.Tensor:
+    """Keep mask ``[V]`` (bool) of a ``"rows"`` spec (embedding dropout): ``dropout_mask`` of one step of one row of V units, so id
+    v takes unit v % 8 of counter (v / 8, 0, c2, step)."""
+    return dropout_mask(spec, 1, 1, V, device=device)[0, 0]
+
+
+def dropout_factor(*specs: Optional[DropoutSpec]) -> torch.Tensor:
+    """fp32 factor of a unit kept by every active spec: the scale of the one spec on, or the fp32 product of the scales."""
+    on = [s for s in specs if s is not None and s.p > 0]
+    f = dropout_scale(on[0].p)
+    for s in on[1:]:
+        f = dropout_scale(s.p) * f
+    return f
+
+
+def embedding(tokens, table, lengths=None, input_dropout: Optional[DropoutSpec] = None,
+              embedding_dropout: Optional[DropoutSpec] = None):
     """Token embedding in front of the first layer (``--vocab_size``): ``nn.Embedding`` read time-major.  ``tokens`` int ``[B,T]``
     (or ``[B]``, one step), ``table [V,E]``, ``lengths`` optional int ``[B]`` -> ``x [T,B,E]`` of the table's dtype with
     ``x[t,b] = table[tokens[b,t]]`` at counted positions (``t < lengths[b]``, id in ``[0, V)``) and 0 elsewhere.  Uncounted
-    positions give the table no gradient; a counted one adds its ``dx`` to its id's row."""
+    positions give the table no gradient; a counted one adds its ``dx`` to its id's row.
+
+    ``input_dropout``: an ``"input"`` spec; unit e of position (t, b) is kept where ``dropout_mask(spec, T, B, E)`` is.
+    ``embedding_dropout``: a ``"rows"`` spec; a position reads 0 where its id's row is dropped (``embedding_row_mask``).  A
+    kept unit is ``w * f`` (``dropout_factor``), rounded once to the table's dtype (bf16: from float(w); fp64: ``w`` times each
+    scale); the gradient follows through autograd."""
     tok = tokens.long()
     if tok.dim() == 1:
         tok = tok.unsqueeze(1)
     tok = tok.t()                                                    # [T,B]
     T, B = tok.shape
-    V = table.shape[0]
+    V, E = table.shape
     keep = (tok >= 0) & (tok < V)
     if lengths is not None:
         keep = keep & (torch.arange(T, device=tok.device).unsqueeze(1) < lengths.to(tok.device).long().unsqueeze(0))
-    rows = table[torch.where(keep, tok, torch.zeros_like(tok))]       # [T,B,E]
-    return rows * keep.unsqueeze(2).to(table.dtype)
+    safe = torch.where(keep, tok, torch.zeros_like(tok))
+    rows = table[safe]                                               # [T,B,E]
+    specs = [s for s in (input_dropout, embedding_dropout) if s is not None and s.p > 0]
+    if not specs:
+        return rows * keep.unsqueeze(2).to(table.dtype)
+    if embedding_dropout is not None and embedding_dropout.p > 0:
+        keep = keep & embedding_row_mask(embedding_dropout, V, device=tok.device)[safe]
+    keep = keep.unsqueeze(2).expand(T, B, E)
+    if input_dropout is not None and input_dropout.p > 0:
+        keep = keep & dropout_mask(input_dropout, T, B, E, device=tok.device)
+    if rows.dtype == torch.float64:                                   # (fp64: one product per scale, no fp32 rounding)
+        y = rows
+        for s in specs:
+            y = y * dropout_scale(s.p).double()
+    elif rows.dtype == torch.float32:
+        y = rows * dropout_factor(*specs)
+    else:
+        y = (rows.float() * dropout_factor(*specs)).to(rows.dtype)
+    return torch.where(keep, y, torch.zeros((), dtype=table.dtype, device=table.device))
 
 
 def clip_coefficient(g_total_segments, max_norm: float):
