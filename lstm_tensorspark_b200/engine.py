@@ -22,6 +22,7 @@ from .config import FUSED_CLIP_ERROR, Config
 from .models.classifier import SequenceClassifier
 from .models.recurrent.lstm import clear_weight_decay_collection, weight_decay_collection
 from .ops import functional as F
+from .ops import params
 from .ops.optim import FlatOptimizer
 from .parallel.comm import Communicator
 
@@ -101,7 +102,7 @@ class TrainEngine:
     # ---------------------------------------------------------------------------------------------------
     def _make_bucket_plan(self):
         """Gradient buckets in the order backward finishes them: [top layer (+ head)], ..., [layer 0].  A bucket = a
-        contiguous element range of the flat buffer + the parameters that must have been written before it may be synced.
+        contiguous element range of the flat buffer + the parameters that must have been released before it may be synced.
         (Reference counterpart: the one-shot reduceByKey over all weights, original src/rnn.py:393-407 - here the sync
         of the upper layers hides under the backward recurrence of the layers below.)  Bidirectional: every direction of a layer
         is a layer here (flat order: forward, reverse per depth; backward finishes the reverse direction first)."""
@@ -120,8 +121,8 @@ class TrainEngine:
         plan = []
         for li in reversed(range(len(layers))):
             l = layers[li]
-            # [w_h, bias] finishes with the layer's bias gradient, [w_x] already with its weight-gradient GEMM: two buckets per
-            # layer, each launched under the GEMM / recurrence kernel that follows it in backward
+            # [w_h, bias] is released with the layer's bias gradient, [w_x] already with its weight-gradient GEMM (or with the dX
+            # GEMM when there is one): two buckets per layer, each launched under the GEMM / recurrence kernel that follows it
             lo_x, lo_h, hi = off[id(l.w_x)], off[id(l.w_h)], end[li]
             need_h = [l.w_h, l.bias]
             if li == len(layers) - 1 and others_direct:
@@ -137,28 +138,24 @@ class TrainEngine:
         return plan
 
     def _backward_with_buckets(self, loss: torch.Tensor):
-        from .ops import cuda_lstm
         flat, comm, plan = self.flat, self.comm, self._bucket_plan
         comm.begin_grad_step(flat, self.optimizer)
         state = {"next": 0}
 
-        def ready():
-            # queue every leading bucket whose parameters have all been written; it is launched (PDL) right after the next big
+        def ready(released):
+            # queue every leading bucket whose parameters have all been released; it is launched (PDL) right after the next big
             # backward kernel (weight-gradient GEMM / lower layer's recurrence), i.e. it runs next to that kernel
             while state["next"] < len(plan) - 1:
                 b = plan[state["next"]]
-                if b["need"] is None or (b["need"] & flat._stale):
+                if b["need"] is None or not b["need"] <= released:
                     break
-                cuda_lstm.queue_after_big_launch(lambda b=b: comm.launch_bucket(b["lo"], b["hi"], pdl=_BUCKET_PDL, blocks=self.cfg.grad_bucket_blocks))
+                params.queue_after_big_launch(lambda b=b: comm.launch_bucket(b["lo"], b["hi"], pdl=_BUCKET_PDL, blocks=self.cfg.grad_bucket_blocks))
                 state["next"] += 1
 
-        cuda_lstm.HOOKS["grads_written"] = ready
-        try:
+        with params.releases_to(ready):
             loss.backward()
-        finally:
-            cuda_lstm.HOOKS["grads_written"] = None
         flat.finalize_grads()
-        cuda_lstm._after_big_launch(flush=True)             # queued, but no big kernel followed (generic path / last layer)
+        params.after_big_launch(flush=True)                 # queued, but no big kernel followed (generic path / last layer)
         for b in plan[state["next"]:]:
             comm.launch_bucket(b["lo"], b["hi"])
 

@@ -14,7 +14,7 @@ from __future__ import annotations
 import torch
 
 from .cuda_ext import LAUNCHES, count, drop_args, ext
-from .params import grad_out, lowp
+from .params import grad_out, lowp, release
 
 
 def _tokens(tokens: torch.Tensor) -> torch.Tensor:
@@ -50,6 +50,7 @@ class _EmbedFn(torch.autograd.Function):
         out, acc, ret = grad_out(ctx.addr, ctx.shape, d.device)
         E.embed_bwd(d, ctx.tok, ctx.ln, out, acc, **ctx.drop)
         LAUNCHES["n"] += E.EMBED_BWD_LAUNCHES - 1
+        release(ctx.addr)
         count("embed_bwd")
         if ctx.drop["in_step"] is not None or ctx.drop["row_step"] is not None:
             count("embed_bwd_dropout")

@@ -7,7 +7,7 @@ from __future__ import annotations
 import torch
 
 from .cuda_ext import count, ext
-from .params import grad_out
+from .params import grad_out, release
 
 
 class _HeadXentFn(torch.autograd.Function):
@@ -39,6 +39,7 @@ class _HeadXentFn(torch.autograd.Function):
         db, acc_b, ret_b = grad_out(ctx.addrs[1], (w.shape[1],), w.device)
         dl = dloss.detach().float().reshape(1).contiguous()
         dh = ext().head_bwd(hcc, w, dlogits, dl, dw, db, acc_w, acc_b)
+        release(*ctx.addrs)
         return dh.to(ctx.h_dtype), ret_w, ret_b, None
 
 
@@ -80,6 +81,7 @@ class _HeadXentStepFn(torch.autograd.Function):
         db, acc_b, ret_b = grad_out(ctx.addrs[1], (w.shape[1],), w.device)
         dl = dloss.detach().float().reshape(1).contiguous()
         dh = ext().head_step_bwd(h2, w, dlogits, dl, dw, db, acc_w, acc_b)
+        release(*ctx.addrs)
         return dh.view(ctx.shape).to(ctx.h_dtype), ret_w, ret_b, None, None
 
 

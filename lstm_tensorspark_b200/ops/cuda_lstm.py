@@ -18,7 +18,7 @@ import torch
 
 from .cuda_ext import STATS, count, ext
 from .cuda_ext import drop_args as _drop_args
-from .params import grad_out, lowp
+from .params import Countdown, after_big_launch, big_launch_begin, grad_out, lowp, release
 from . import cuda_gemm as G
 
 _SYNC_WS = {}
@@ -32,44 +32,8 @@ FORCE_GENERIC = os.environ.get("LSTM_TS_FORCE_GENERIC", "0") == "1"
 SEQ_VARIANT = int(os.environ.get("LSTM_TS_SEQ_VARIANT", "0"))
 
 
-# Gradient-bucket overlap (engine.TrainEngine + parallel/fused_comm.py): HOOKS["grads_written"] is called after every weight /
-# bias gradient has been written; callables queued in AFTER_SEQ_BWD are run right after the NEXT big backward kernel has been
-# launched (a persistent recurrence kernel or a weight-gradient GEMM: both execute griddepcontrol.launch_dependents).  They
-# launch a finished bucket's fused allreduce + update as a programmatic dependent, so it runs NEXT TO that kernel (on the SMs
-# the recurrence leaves idle / co-resident with the GEMM's CTAs) instead of after it.
-HOOKS = {"grads_written": None}
-AFTER_SEQ_BWD = []          # [(generation when queued, closure)]
-_GEN = {"n": 0}
-
-
-def queue_after_big_launch(fn):
-    AFTER_SEQ_BWD.append((_GEN["n"], fn))
-
-
-def _big_launch_begin():
-    """A big backward kernel (recurrence / weight-gradient GEMM) is about to be launched as an ORDINARY launch: everything
-    enqueued before it is complete when it starts."""
-    _GEN["n"] += 1
-
-
-def _after_big_launch(flush: bool = False):
-    """Launch the queued bucket closures as programmatic dependents of the kernel just launched - but only those queued
-    BEFORE that kernel was launched: a dependent may start while its primary runs, so its inputs must not come from it."""
-    while AFTER_SEQ_BWD and (flush or AFTER_SEQ_BWD[0][0] < _GEN["n"]):
-        AFTER_SEQ_BWD.pop(0)[1]()
-
-
-_HOLD = {"on": False}        # True while a written gradient still waits for its weight-drop mask (see _LSTMPairFn.backward)
-
-
-def _grads_written():
-    h = HOOKS["grads_written"]
-    if h is not None and not _CHUNKING["on"] and not _HOLD["on"]:
-        h()
-
-
-def _accumulate_grad(w_addr: int, a_t: torch.Tensor, b: torch.Tensor, b_folded: bool = False, pdl: bool = False,
-                     max_ctas: int = 0, ctas: int = 0, rowsum=None, wdrop=None, defer: bool = False):
+def _grad_gemm(w_addr: int, a_t: torch.Tensor, b: torch.Tensor, b_folded: bool = False, pdl: bool = False, max_ctas: int = 0,
+               ctas: int = 0, rowsum=None, masked: bool = False) -> tuple:
     """dW = a_t @ b in fp32 (``a_t`` = dG^T as a transposed view, ``b`` = the layer input: both operands MN-major, read in
     place by the wgmma GEMM; ``b_folded``: ``b`` is the batch-major [B,T,D] array standing for the time-major [T*B, D]
     matrix).  When the parameter lives in a FlatParams buffer the product lands straight in its grad
@@ -78,67 +42,53 @@ def _accumulate_grad(w_addr: int, a_t: torch.Tensor, b: torch.Tensor, b_folded: 
     recurrence that is still running).  Such a GEMM is no "big launch" for the gradient buckets: what precedes it in the stream
     may still be running when it starts, so no bucket's allreduce is launched under it.  ``ctas``: CTAs per tile cluster of
     an ordinary launch (0 = ``cuda_gemm.GEMM_CTAS``).  ``rowsum``: see ``cuda_gemm.matmul`` (the bias gradient, summed by the
-    same launch).
-
-    ``wdrop``: the kernel arguments of a weight-drop spec (``_drop_args``): the product is the gradient of the masked matrix and
-    ``weight_drop_grad`` masks it into the sink - in place on a first write, from an fp32 scratch when the sink accumulates - or
-    into the tensor returned to autograd.  The gradient counts as written only once the mask is enqueued.  ``defer``: return a
-    callable that launches the mask (and reports the gradient written) and returns what autograd gets, for a caller that has
-    programmatic dependents to launch right behind the GEMM first."""
+    same launch).  ``masked``: an accumulating sink gets the product in an fp32 scratch, for ``_weight_drop_grad`` to add in.
+    -> ``(product, sink, what autograd gets)``, where ``product is sink`` unless it is that scratch."""
     ops = dict(a=a_t, b_t=None, b_folded=b, ctas=ctas) if b_folded else dict(a=a_t, b_t=b.t(), ctas=ctas)
     ops["rowsum"] = rowsum
     if pdl:
         ops.update(pdl=True, ctas=1, max_ctas=max_ctas)
     out, acc, ret = grad_out(w_addr, (a_t.shape[0], b.shape[-1]), a_t.device)
-    scratch = bool(wdrop) and acc
+    scratch = masked and acc
     big = ret is None and not pdl
     if big:
-        _big_launch_begin()
+        big_launch_begin()
     part = G.matmul(out_dtype=torch.float32, **ops) if scratch else G.matmul(out=out, accumulate=acc, **ops)
     if big:
-        _after_big_launch()              # finished buckets of earlier gradients: allreduce them under this GEMM
-
-    def finish():
-        if wdrop:
-            _weight_drop_grad(part if scratch else out, out, wdrop, scratch)
-        if ret is None:
-            _grads_written()
-        return ret
-    return finish if defer else finish()
+        after_big_launch()               # finished buckets of earlier gradients: allreduce them under this GEMM
+    return (part if scratch else out), out, ret
 
 
-_BIAS_SPLIT = {}
+def _accumulate_grad(w_addr: int, a_t: torch.Tensor, b: torch.Tensor, wdrop=None, **gemm):
+    """``_grad_gemm``, then with ``wdrop`` (``_drop_args`` of a weight-drop spec) ``_weight_drop_grad`` -> what autograd gets."""
+    part, out, ret = _grad_gemm(w_addr, a_t, b, masked=bool(wdrop), **gemm)
+    if wdrop:
+        _weight_drop_grad(part, out, wdrop, part is not out)
+    return ret
 
 
-def _bias_grad(b_addr: int, dg2d: torch.Tensor, under_gemm: bool = False, part: int = -1, max_ctas: int = 0):
+def _bias_grad(b_addr: int, dg2d: torch.Tensor, under_gemm: bool = False, part: int = -1, max_ctas: int = 0, sink=None):
     """db = column sums of dG; straight into the flat grad view when there is one.  ``under_gemm``: the previous launch of the
     stream is a weight-gradient GEMM over the same dG that leaves SMs idle - run next to it (programmatic dependent launch).
     ``part`` 0 / 1: only the first / second half of the columns (one half under each of the layer's two weight-gradient GEMMs:
-    on the ~20 idle SMs a half takes about as long as the GEMM it hides under); the value for autograd comes from part 1.
+    on the ~20 idle SMs a half takes about as long as the GEMM it hides under).  Part 0 returns its ``sink`` (None when the columns
+    do not split), which the caller passes to part 1; otherwise -> what autograd gets.
     ``max_ctas`` (whole-column launches): at most that many CTAs, each walking several slabs (the same sums)."""
     n = dg2d.shape[1]
-    fast = dg2d.is_cuda and dg2d.dtype == torch.bfloat16 and n % 512 == 0 and dg2d.is_contiguous()
+    if part >= 0 and dg2d.is_cuda and dg2d.dtype == torch.bfloat16 and n % 512 == 0 and dg2d.is_contiguous():
+        out, acc, ret = sink = sink or grad_out(b_addr, (n,), dg2d.device)
+        STATS["kernels"] += 1
+        ext().colsum_bf16_into(dg2d, out, not acc, under_gemm, part * (n // 2), n // 2)
+        return sink if part == 0 else ret
     if part == 0:
-        if not fast:
-            return None                                   # everything happens with the part-1 call
-        out, acc, _ = _BIAS_SPLIT[b_addr] = grad_out(b_addr, (n,), dg2d.device)
+        return None                                   # everything happens with the part-1 call
+    out, acc, ret = grad_out(b_addr, (n,), dg2d.device)
+    if dg2d.is_cuda and dg2d.dtype == torch.bfloat16 and n % 256 == 0 and dg2d.is_contiguous():
         STATS["kernels"] += 1
-        ext().colsum_bf16_into(dg2d, out, not acc, under_gemm, 0, n // 2)
-        return None
-    if part == 1 and fast and b_addr in _BIAS_SPLIT:
-        out, acc, ret = _BIAS_SPLIT.pop(b_addr)
-        STATS["kernels"] += 1
-        ext().colsum_bf16_into(dg2d, out, not acc, under_gemm, n // 2, n // 2)
+        ext().colsum_bf16_into(dg2d, out, not acc, under_gemm and part < 0, max_ctas=max_ctas)
     else:
-        out, acc, ret = grad_out(b_addr, (n,), dg2d.device)
-        if dg2d.is_cuda and dg2d.dtype == torch.bfloat16 and n % 256 == 0 and dg2d.is_contiguous():
-            STATS["kernels"] += 1
-            ext().colsum_bf16_into(dg2d, out, not acc, under_gemm and part < 0, max_ctas=max_ctas)
-        else:
-            ones = torch.ones(1, dg2d.shape[0], dtype=dg2d.dtype, device=dg2d.device)
-            G.matmul(ones, dg2d.t(), out=out.view(1, -1), accumulate=acc)
-    if ret is None:
-        _grads_written()
+        ones = torch.ones(1, dg2d.shape[0], dtype=dg2d.dtype, device=dg2d.device)
+        G.matmul(ones, dg2d.t(), out=out.view(1, -1), accumulate=acc)
     return ret
 
 
@@ -256,9 +206,6 @@ def _gemm_tn(a: torch.Tensor, w: torch.Tensor) -> torch.Tensor:
     return G.matmul(a, w, out_dtype=a.dtype)
 
 
-_CHUNKING = {"on": False}      # True while lstm_layer_sequence feeds batch chunks (weight gradients then accumulate over calls)
-
-
 def _check_lengths_arg(lengths: Optional[torch.Tensor], B: int, device) -> None:
     """Shape / dtype / device of per-row lengths; the values are not read (that would synchronise with the device)."""
     if lengths is not None and (lengths.dtype != torch.int32 or lengths.shape != (B,) or lengths.device != device
@@ -311,7 +258,7 @@ def dropout(x: torch.Tensor, spec, t0: int = 0) -> torch.Tensor:
 
 class _LSTMSeqFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x_seq, h0, c0, w_x, w_h, bias, lengths=None, reverse=False, dropout=None, weight_drop=None):
+    def forward(ctx, x_seq, h0, c0, w_x, w_h, bias, lengths=None, reverse=False, dropout=None, weight_drop=None, chunks=None):
         E = ext()
         T, B, D = x_seq.shape
         H = w_h.shape[1]
@@ -362,7 +309,7 @@ class _LSTMSeqFn(torch.autograd.Function):
         ctx.fast = fast
         ctx.lengths = lengths
         ctx.reverse = reverse
-        ctx.whole_batch = not _CHUNKING["on"]
+        ctx.chunks = chunks                    # a params.Countdown shared by the batch chunks of one layer, or None
         ctx.dims = (T, B, D, H)
         ctx.w_addrs = (w_x.data_ptr(), w_h.data_ptr(), bias.data_ptr())
         ctx.in_dtypes = (h0.dtype, c0.dtype)
@@ -391,12 +338,12 @@ class _LSTMSeqFn(torch.autograd.Function):
         dhT = (dh_T.float().contiguous() if dh_T is not None else torch.zeros(B, H, dtype=torch.float32, device=dev))
         if ctx.fast:
             w_hT = _transposed(w_h_c)
-            _big_launch_begin()
+            big_launch_begin()
             dpre, dh0, dc0 = E.lstm_seq_bwd(dh_seq, w_hT, act, c_seq, dhT, dcT, _sync_ws(dev), _seq_variant(B, H, dev),
                                             lengths=ctx.lengths, reverse=ctx.reverse, **drop)
             STATS["fast_bwd"] += 1
             STATS["kernels"] += 1
-            _after_big_launch()                  # finished gradient buckets of the layers above: sync them under this recurrence
+            after_big_launch()                   # finished gradient buckets of the layers above: sync them under this recurrence
         else:
             dpre = torch.empty_like(act)
             dh_rec: Optional[torch.Tensor] = dhT if dh_T is not None else None
@@ -416,16 +363,21 @@ class _LSTMSeqFn(torch.autograd.Function):
             STATS["kernels"] += T
         dg2d = dpre.view(T * B, 4 * H)
         dg_t = dg2d.t()
-        dw_x = _accumulate_grad(ctx.w_addrs[0], dg_t, x2d)
+        a, rel = ctx.w_addrs, (release if ctx.chunks is None else ctx.chunks.releaser())
+        dw_x = _accumulate_grad(a[0], dg_t, x2d)
+        if not ctx.needs_input_grad[0]:
+            rel(a[0])                                              # (else W_x is released after the dX GEMM reads it)
         h_prev = h_seq[1:] if ctx.reverse else h_seq[:T]          # the h each step's dG pairs with
-        dw_h = _accumulate_grad(ctx.w_addrs[1], dg_t, h_prev.reshape(T * B, H), wdrop=ctx.wdrop)
-        db = _bias_grad(ctx.w_addrs[2], dg2d)
+        dw_h = _accumulate_grad(a[1], dg_t, h_prev.reshape(T * B, H), wdrop=ctx.wdrop)
+        db = _bias_grad(a[2], dg2d)
+        rel(a[1], a[2])
         dx = None
         if ctx.needs_input_grad[0]:
             dx = G.matmul(dg2d, w_x_c.t(), out_dtype=cd).view(T, B, D)        # dG · W_x: W_x read in place as an MN-major operand
             STATS["kernels"] += 1
+            rel(a[0])
         h0_dt, c0_dt = ctx.in_dtypes
-        return dx, dh0.to(h0_dt), dc0.to(c0_dt), dw_x, dw_h, db, None, None, None, None
+        return dx, dh0.to(h0_dt), dc0.to(c0_dt), dw_x, dw_h, db, None, None, None, None, None
 
 
 def lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths=None, reverse=False, dropout=None, weight_drop=None):
@@ -446,15 +398,13 @@ def lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths=None, reverse=Fal
     chunk = _batch_chunk(B, H, x_seq.dtype, x_seq.device)
     if chunk is not None:
         # more batch tiles than the persistent kernels can keep co-resident: the sequences are independent, so run the fast
-        # path per batch chunk (weight-gradient contributions accumulate across chunks) instead of the per-step generic path
-        _CHUNKING["on"] = True
-        try:
-            outs = [_LSTMSeqFn.apply(x_seq[:, b0:b0 + chunk].contiguous(), h0[b0:b0 + chunk], c0[b0:b0 + chunk], w_x, w_h, bias,
-                                     None if lengths is None else lengths[b0:b0 + chunk], reverse,
-                                     None if dropout is None else dropout.at_rows(b0), weight_drop)
-                    for b0 in range(0, B, chunk)]
-        finally:
-            _CHUNKING["on"] = False
+        # path per batch chunk (weight-gradient contributions accumulate across chunks) instead of the per-step generic path;
+        # the chunk whose backward runs last releases the parameters
+        chunks = Countdown((B + chunk - 1) // chunk)
+        outs = [_LSTMSeqFn.apply(x_seq[:, b0:b0 + chunk].contiguous(), h0[b0:b0 + chunk], c0[b0:b0 + chunk], w_x, w_h, bias,
+                                 None if lengths is None else lengths[b0:b0 + chunk], reverse,
+                                 None if dropout is None else dropout.at_rows(b0), weight_drop, chunks)
+                for b0 in range(0, B, chunk)]
         count("batch_chunks", len(outs))
         return (torch.cat([o[0] for o in outs], dim=1), torch.cat([o[1] for o in outs], dim=0),
                 torch.cat([o[2] for o in outs], dim=0))
@@ -476,15 +426,7 @@ def lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths=None, reverse=Fal
 # =====================================================================================================================
 FOLDED_FEED = os.environ.get("LSTM_TS_FOLDED_FEED", "1") != "0"   # batch-major input read in place by the first layer's GEMMs
 WAVEFRONT = os.environ.get("LSTM_TS_WAVEFRONT", "1") == "1"
-_SIDE_STREAMS = {}
 _WS_PAIR = {}
-
-
-def _side_streams(device):
-    key = device.index
-    if key not in _SIDE_STREAMS:
-        _SIDE_STREAMS[key] = (torch.cuda.Stream(device=device), torch.cuda.Stream(device=device))
-    return _SIDE_STREAMS[key]
 
 
 _WARM = set()
@@ -736,52 +678,48 @@ class _LSTMPairFn(torch.autograd.Function):
             # concurrent column-sum launches would share the slab scratch).  Gradient buckets are launched under the next
             # ordinary launch (dW_xa), not under these: a programmatic dependent may start before the kernels ahead of it in
             # the stream are complete.
-            # Weight drop: dW_hb's mask is an ordinary launch behind the column sums (it runs after L_a, before dW_xa), and the
-            # gradient counts as written only from then on.
+            # Weight drop: dW_hb's mask is an ordinary launch behind the column sums (it runs after L_a, before dW_xa), and W_hb is
+            # released only from then on.
             side = max(1, (_sms(dev) - Ha // 16 - _COLSUM_SMS) // 2)
             dw_xb = _accumulate_grad(a[3], dg_b.t(), hin_b.reshape(T * B, Ha), pdl=True, max_ctas=side)
+            release(a[3])
+            part, out, dw_hb = _grad_gemm(a[4], dg_b.t(), h_seq_b[:T].reshape(T * B, Hb), pdl=True, max_ctas=side, masked=bool(wdb))
+            db_b = _bias_grad(a[5], dg_b, under_gemm=True, max_ctas=4 * _COLSUM_SMS)
             if wdb:
-                _HOLD["on"] = True
-                try:
-                    finish_hb = _accumulate_grad(a[4], dg_b.t(), h_seq_b[:T].reshape(T * B, Hb), pdl=True, max_ctas=side,
-                                                 wdrop=wdb, defer=True)
-                    db_b = _bias_grad(a[5], dg_b, under_gemm=True, max_ctas=4 * _COLSUM_SMS)
-                finally:
-                    _HOLD["on"] = False
-                dw_hb = finish_hb()
-            else:
-                dw_hb = _accumulate_grad(a[4], dg_b.t(), h_seq_b[:T].reshape(T * B, Hb), pdl=True, max_ctas=side)
-                db_b = _bias_grad(a[5], dg_b, under_gemm=True, max_ctas=4 * _COLSUM_SMS)
+                _weight_drop_grad(part, out, wdb, part is not out)
         else:
             # the bias column sums run NEXT TO the first weight-gradient GEMM of their layer (same dG, idle SMs), not after it
             # (each GEMM is followed by: finished gradient buckets [programmatic dependents of the GEMM], then half of the layer's
             # bias column sums [programmatic dependent of whatever was launched last] - all three run side by side)
             dw_xb = _accumulate_grad(a[3], dg_b.t(), hin_b.reshape(T * B, Ha))
-            _bias_grad(a[5], dg_b, under_gemm=dw_xb is None, part=0)
+            release(a[3])
+            sink = _bias_grad(a[5], dg_b, under_gemm=dw_xb is None, part=0)
             dw_hb = _accumulate_grad(a[4], dg_b.t(), h_seq_b[:T].reshape(T * B, Hb), wdrop=wdb)
-            db_b = _bias_grad(a[5], dg_b, under_gemm=dw_hb is None and not wdb, part=1)
+            db_b = _bias_grad(a[5], dg_b, under_gemm=dw_hb is None and not wdb, part=1, sink=sink)
+        release(a[4], a[5])
         dg_a = dpre_a.view(T * B, 4 * Ha)
+        # pipelined, 2 x 1024 on a 132-SM H100: single-CTA 128 x 256 tiles put the 128 tiles of each of layer a's weight-gradient
+        # GEMMs on 128 SMs in one wave, at the per-SM rate of the capped side GEMMs; 2-CTA clusters ran them at about half that
+        # rate per SM (bench/side_gemms.py).  The tile's K order, and with it every bit of dW, is the same either way.  db_a comes
+        # out of the dW_ha launch as the row sums of dG_a^T (csrc/gemm2_wgmma.cu): the column-sum kernels beside these GEMMs only
+        # found the 4 SMs the GEMMs leave free and ran on after them.
+        dw_xa = _accumulate_grad(a[0], dg_a.t(), x2d, b_folded=ctx.x_folded, ctas=1 if pipelined else 0)
+        if not ctx.needs_input_grad[0]:
+            release(a[0])                                                 # (else W_xa is released after the dX GEMM reads it)
         if pipelined:
-            # 2 x 1024 on a 132-SM H100: single-CTA 128 x 256 tiles put the 128 tiles of each of these GEMMs on 128 SMs in one
-            # wave, at the per-SM rate of the capped side GEMMs; 2-CTA clusters ran them at about half that rate per SM
-            # (bench/side_gemms.py).  The tile's K order, and with it every bit of dW, is the same either way.  db_a comes out of
-            # the dW_ha launch as the row sums of dG_a^T (csrc/gemm2_wgmma.cu): the column-sum kernels beside these GEMMs only
-            # found the 4 SMs the GEMMs leave free and ran on after them.
-            dw_xa = _accumulate_grad(a[0], dg_a.t(), x2d, b_folded=ctx.x_folded, ctas=1)
             db_out, db_acc, db_a = grad_out(a[2], (4 * Ha,), dev)
             dw_ha = _accumulate_grad(a[1], dg_a.t(), h_seq_a[:T].reshape(T * B, Ha), ctas=1, rowsum=(db_out, db_acc), wdrop=wda)
             count("fused_bias_grads")
-            if db_a is None:
-                _grads_written()
         else:
-            dw_xa = _accumulate_grad(a[0], dg_a.t(), x2d, b_folded=ctx.x_folded)
-            _bias_grad(a[2], dg_a, under_gemm=dw_xa is None, part=0)
+            sink = _bias_grad(a[2], dg_a, under_gemm=dw_xa is None, part=0)
             dw_ha = _accumulate_grad(a[1], dg_a.t(), h_seq_a[:T].reshape(T * B, Ha), wdrop=wda)
-            db_a = _bias_grad(a[2], dg_a, under_gemm=dw_ha is None and not wda, part=1)
+            db_a = _bias_grad(a[2], dg_a, under_gemm=dw_ha is None and not wda, part=1, sink=sink)
+        release(a[1], a[2])
         dx = None
         if ctx.needs_input_grad[0]:                                       # (never with a folded input: lstm_pair_sequence)
             dx = G.matmul(dg_a, wxa.t(), out_dtype=cd).view(T, B, D)
             STATS["kernels"] += 1
+            release(a[0])
         t = ctx.in_dtypes
         return (dx, dh0a.to(t[0]), dc0a.to(t[1]), dw_xa, dw_ha, db_a, dh0b.to(t[2]), dc0b.to(t[3]), dw_xb, dw_hb, db_b, None, None,
                 None, None, None, None)

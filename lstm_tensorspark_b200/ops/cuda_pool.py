@@ -13,7 +13,7 @@ from __future__ import annotations
 import torch
 
 from .cuda_ext import count, ext
-from .params import grad_out, lowp
+from .params import grad_out, lowp, release
 
 MODES = {"mean": 0, "max": 1, "attention": 2}
 
@@ -69,6 +69,7 @@ class _PoolFn(torch.autograd.Function):
         cuda_gemm.matmul(h2.t(), dU.t(), out=dwa, accumulate=acc_dwa)                         # dW_a = h^T dU
         dh = E.seq_pool_bwd(dsf, ln, T, m, None, alpha, G, out_bf16)
         count("pool_attention_bwd")
+        release(*ctx.addrs)
         return dh.view(T, B, H).to(ctx.h_dtype), None, None, ret_dwa, ret_dba, ret_dv
 
 

@@ -18,7 +18,7 @@ import torch
 
 from . import cuda_gemm as G
 from .cuda_ext import count, ext
-from .params import grad_out, lowp
+from .params import grad_out, lowp, release
 
 ROW_CHUNK = 4096          # rows of h per backward chunk: the schedule depends on the shapes only
 MIN_CLASSES = 512
@@ -90,6 +90,7 @@ class _VocabXentFn(torch.autograd.Function):
                 G.matmul(h2[r0:r0 + rows].t(), d.t(), out=dw, accumulate=acc)                   # dW (+)= h^T dlogits
             E.vocab_head_colsum(d, db.view(-1), bool(acc_b or r0 > 0))
         count("vocab_head_bwd")
+        release(*(ctx.addrs[1:] if cm else ctx.addrs))    # (a tied table's gradient is finished by the embedding's backward)
         return dh.view(ctx.shape), ret_w, ret_b, None, None, None
 
 

@@ -273,29 +273,26 @@ def test_graph_replays_draw_a_new_mask_each(monkeypatch):
 
 
 @pytest.mark.parametrize("hidden", ["1024,1024", "1024"])
-def test_the_bucket_hook_sees_only_masked_gradients(hidden):
-    """A single-replica stand-in for the gradient buckets: whenever the hook that launches them fires, it snapshots (in stream
-    order, where a bucket launched then would read) every W_h gradient already marked written.  Each snapshot must be the final,
-    masked gradient: zero wherever the mask dropped.  The stand-in needs one GPU; the buckets' allreduce itself needs two."""
-    from lstm_tensorspark_b200.ops import cuda_lstm
+def test_every_released_w_h_gradient_is_masked(hidden):
+    """A single-replica stand-in for the gradient buckets: whenever a parameter is released to them, a listener snapshots (in
+    stream order, where a bucket launched then would read) every W_h gradient already released.  Each snapshot must be the
+    final, masked gradient: zero wherever the mask dropped.  The stand-in needs one GPU; the buckets' allreduce itself needs two."""
+    from lstm_tensorspark_b200.ops import params
     x, y = _headline_batch()
     eng = _headline_engine(weight_drop=0.5, hidden_units=hidden)
     flat, rnn = eng.flat, eng.model.rnn
     snaps = {}
 
-    def hook():
+    def hook(released):
         for l, layer in enumerate(rnn.layers):
-            if l not in snaps and layer.w_h.data_ptr() in flat._direct and layer.w_h.data_ptr() not in flat._stale:
+            if l not in snaps and layer.w_h.data_ptr() in flat._direct and layer.w_h.data_ptr() in released:
                 snaps[l] = layer.w_h.grad.clone()
 
     flat.zero_grad()
-    assert cuda_lstm.HOOKS["grads_written"] is None
-    cuda_lstm.HOOKS["grads_written"] = hook
-    try:
-        n0 = _stats()
+    assert params._LISTENER is None
+    n0 = _stats()
+    with params.releases_to(hook):
         eng.step(x, y)
-    finally:
-        cuda_lstm.HOOKS["grads_written"] = None
     torch.cuda.synchronize()
     assert _delta(n0)["weight_drop_grad"] == len(rnn.layers)
     assert sorted(snaps) == list(range(len(rnn.layers)))

@@ -1,5 +1,6 @@
 """Host-side logic of the GPU path that does not need a GPU: lazy gradient zeroing, ownership of Adam slots under bucketed
-two-shot allreduce, the wavefront GEMM's gate configuration, the generation-gated bucket queue."""
+two-shot allreduce, the wavefront GEMM's gate configuration, the generation-gated bucket queue and the release of parameters
+to the gradient buckets."""
 import types
 
 import pytest
@@ -84,20 +85,78 @@ def test_wavefront_gate_configuration():
     assert CL._gate_cfg(v1, 2, 4 * H // 64, 1, 4 * H // 64, T + 1, -1, B, True) == [2, 1, 64 * (T + 1), -64, B, 0, 1]
 
 
-def test_bucket_queue_never_releases_a_dependent_of_its_own_producer():
-    from lstm_tensorspark_b200.ops import cuda_lstm as CL
-    CL.AFTER_SEQ_BWD.clear()
+def test_big_launch_queue_never_releases_a_dependent_of_its_own_producer():
+    from lstm_tensorspark_b200.ops import params as P
+    P._QUEUE.clear()
     fired = []
-    CL._big_launch_begin()                              # GEMM 1 is launched ...
-    CL.queue_after_big_launch(lambda: fired.append("bucket of GEMM 1"))     # ... and its bucket becomes ready
-    CL._after_big_launch()
+    P.big_launch_begin()                                # GEMM 1 is launched ...
+    P.queue_after_big_launch(lambda: fired.append("bucket of GEMM 1"))      # ... and its bucket becomes ready
+    P.after_big_launch()
     assert fired == []                                  # not under GEMM 1 itself (a dependent may start while its primary runs)
-    CL._big_launch_begin()                              # GEMM 2
-    CL._after_big_launch()
+    P.big_launch_begin()                                # GEMM 2
+    P.after_big_launch()
     assert fired == ["bucket of GEMM 1"]                # under the NEXT big kernel
-    CL.queue_after_big_launch(lambda: fired.append("last"))
-    CL._after_big_launch(flush=True)                    # end of backward: whatever is left goes in stream order
-    assert fired[-1] == "last" and not CL.AFTER_SEQ_BWD
+    P.queue_after_big_launch(lambda: fired.append("last"))
+    P.after_big_launch(flush=True)                      # end of backward: whatever is left goes in stream order
+    assert fired[-1] == "last" and not P._QUEUE
+
+
+def test_buckets_are_ready_once_released_and_in_plan_order():
+    """``TrainEngine._backward_with_buckets`` over a scripted backward pass: a bucket is queued only once every parameter it
+    needs is released - a sink taken (the gradient being written) is not enough - and only after the buckets ahead of it in
+    the plan; the last bucket goes after backward."""
+    from lstm_tensorspark_b200.engine import TrainEngine
+    from lstm_tensorspark_b200.ops import params as P
+    P._QUEUE.clear()
+    flat, ps, other = _flat()
+    flat.enable_direct_grads(ps + other)
+    for p, o in zip(flat.params, flat.offsets):
+        P.register_param(p.data_ptr(), p.detach().bfloat16(), flat.grad[o:o + p.numel()].view(p.shape), owner=flat)
+    w_x, w_h, b = (p.data_ptr() for p in ps)
+    head = other[0].data_ptr()
+    plan = [{"lo": 0, "hi": 1, "need": {w_x}}, {"lo": 1, "hi": 2, "need": {w_h, b, head}}, {"lo": 2, "hi": 3, "need": {w_x}}]
+    launched = []
+    comm = types.SimpleNamespace(begin_grad_step=lambda flat, opt: None,
+                                 launch_bucket=lambda lo, hi, **kw: launched.append(lo))
+
+    def big_launch():
+        P.big_launch_begin()
+        P.after_big_launch()
+
+    def backward():
+        P.release(head)
+        for addr in (w_h, b):
+            P.grad_out(addr, (1,), "cpu")
+        P.release(w_h, b)                               # bucket 1 is complete, but bucket 0 comes first
+        big_launch()
+        P.grad_out(w_x, (1,), "cpu")                    # bucket 0's gradient is being written: not released yet
+        big_launch()
+        assert launched == []
+        P.release(w_x)                                  # buckets 0 and 1 queued, in plan order ...
+        assert launched == []
+        big_launch()                                    # ... behind the next big launch
+        assert launched == [0, 1]
+
+    eng = types.SimpleNamespace(flat=flat, comm=comm, _bucket_plan=plan, optimizer=None,
+                                cfg=types.SimpleNamespace(grad_bucket_blocks=0))
+    flat.zero_grad()
+    TrainEngine._backward_with_buckets(eng, types.SimpleNamespace(backward=backward))
+    assert launched == [0, 1, 2]
+    assert P._LISTENER is None
+    P.release(w_x)                                      # outside a backward pass: nobody listens
+    assert launched == [0, 1, 2]
+
+
+def test_a_countdown_releases_once_from_the_last_op():
+    from lstm_tensorspark_b200.ops import params as P
+    seen = []
+    chunks = P.Countdown(3)
+    with P.releases_to(lambda released: seen.append(sorted(released))):
+        rels = [chunks.releaser() for _ in range(3)]    # the backward passes of three batch chunks, in autograd's order
+        for rel in rels:
+            rel(11)
+            rel(12, 13)
+    assert seen == [[11], [11, 12, 13]]
 
 
 def test_device_shard_gathers_into_given_buffers():
