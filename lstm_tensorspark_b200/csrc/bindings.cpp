@@ -26,7 +26,7 @@ int ts_colsum_bf16(const void*, float*, void*, int, int, int, int, int, int, cud
 long long ts_colsum_scratch_bytes(int, int);
 int ts_lstm_pointwise_bwd(const void*, const float*, const float*, const void*, const float*, const float*, void*,
                           float*, int, int, int, cudaStream_t, const int*, int, float*);
-int ts_xent_rows(const float*, const long long*, float*, float*, int*, int, int, cudaStream_t);
+int ts_xent_rows(const float*, const long long*, float*, float*, float*, int*, int, int, int, cudaStream_t);
 int ts_flat_adam(float*, const float*, float*, float*, void*, long long, float, float, float, float, float, float,
                  cudaStream_t, int*, long long, const float*);
 int ts_flat_sgd(float*, const float*, void*, long long, float, float, float, cudaStream_t, long long, const float*);
@@ -281,8 +281,9 @@ std::vector<Tensor> xent_rows(const Tensor& logits, const Tensor& labels) {
   auto dlogits = torch::empty_like(logits);
   auto loss = torch::zeros({1}, logits.options());
   auto correct = torch::zeros({1}, logits.options().dtype(torch::kInt32));
+  auto nll = torch::empty({B}, logits.options());
   check(ts_xent_rows(logits.data_ptr<float>(), (const long long*)labels.data_ptr<int64_t>(), dlogits.data_ptr<float>(),
-                     loss.data_ptr<float>(), correct.data_ptr<int>(), B, C, stream()), "xent_rows");
+                     nll.data_ptr<float>(), loss.data_ptr<float>(), correct.data_ptr<int>(), B, C, 0, stream()), "xent_rows");
   return {dlogits, loss, correct};
 }
 
@@ -308,8 +309,10 @@ std::vector<Tensor> head_fwd(const Tensor& h, const Tensor& W, const Tensor& bia
     auto hc = h.contiguous();
     check(ts_head_logits_generic(hc.data_ptr(), W.data_ptr<float>(), bias.data_ptr<float>(), logits.data_ptr<float>(), B, H, C, is_bf16(hc), stream()),
           "head_logits_generic");
+    auto nll = torch::empty({B}, fo);
     check(ts_xent_rows(logits.data_ptr<float>(), (const long long*)labels.data_ptr<int64_t>(), dlogits.data_ptr<float>(),
-                       loss.data_ptr<float>(), correct.data_ptr<int>(), B, C, stream()), "xent_rows");
+                       nll.data_ptr<float>(), loss.data_ptr<float>(), correct.data_ptr<int>(), B, C, is_bf16(hc) ? 0 : 1, stream()),
+          "xent_rows");
   } else {
     check(rc, "head_fwd_tc");
   }

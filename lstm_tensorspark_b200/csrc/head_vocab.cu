@@ -750,7 +750,10 @@ __global__ void __launch_bounds__(kCombWarps * 32) vocab_sample_combine_kernel(c
       sample_take(best, arg, lbest, b2, a2, l2);
     }
     if (lane == 0) {
-      const float lp = lbest - (mx + __logf(se));
+      // (l - max) - log(sum), the log in fp64 (one per row): lbest - (max + __logf(sum)) rounded at the magnitude of the max and
+      // lost every log-probability below half an ulp of it, and __logf's absolute error near sum = 1 is ten times the rest
+      // (tests/test_gpu_head_edges.py::test_sample, spread regime: log p = -1.1e-7 at max 2008 came out as 0)
+      const float lp = (lbest - mx) - ts::logf_acc(se);
       p.tokens[row] = arg;
       p.logprob[row] = lp;
       const int col = s - p.s0;

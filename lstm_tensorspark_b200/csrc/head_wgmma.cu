@@ -199,6 +199,22 @@ head_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmap_h, const HeadParams 
 // its dW[j, 0:C) partial in registers; per batch row: dh[b, j] = sum_c d[b,c] W[j,c] (written once), dW[j,c] += h[b,j] d[b,c].
 // The dlogits slab sits in shared memory (broadcast reads).  One slab (the common case) is deterministic: no atomics.
 // ---------------------------------------------------------------------------------------------------------------------
+// db of a dlogits slab ds [nb][CP] in shared memory: its column sums as a pairwise tree over the rows, in place (ds is not read
+// again) -> ds[c].  A single fp32 chain over up to 1024 rows was 3.5x the fp32 budget of a db that cancels
+// (tests/test_gpu_head_edges.py::test_per_step_row_edges, the fp32 case of 1023 rows); the tree's error grows with log2(rows).
+// Called by every thread of the block.
+template <int CP>
+__device__ __forceinline__ void slab_colsum_tree(float* ds, int nb) {
+  for (int w = 1; w < nb; w <<= 1) {
+    const int pairs = (nb + 2 * w - 1) / (2 * w);
+    for (int i = threadIdx.x; i < pairs * CP; i += blockDim.x) {
+      const int b = (i / CP) * 2 * w, c = i % CP;
+      if (b + w < nb) ds[b * CP + c] += ds[(b + w) * CP + c];
+    }
+    __syncthreads();
+  }
+}
+
 template <typename T, int CP, typename TDH>
 __global__ void __launch_bounds__(128) head_bwd_kernel(const T* __restrict__ h, const float* __restrict__ W, const float* __restrict__ dlogits,
                                                        const float* __restrict__ dloss, TDH* __restrict__ dh, float* __restrict__ dW,
@@ -263,10 +279,12 @@ __global__ void __launch_bounds__(128) head_bwd_kernel(const T* __restrict__ h, 
       if (atomic_w) atomicAdd(dW + (size_t)jg * C + c, t); else dW[(size_t)jg * C + c] = t;
     }
   }
-  if (blockIdx.x == 0 && threadIdx.x < C) {
-    float s = 0.f;
-    for (int b = 0; b < nb; ++b) s += ds[b * CP + threadIdx.x];
-    if (atomic_b) atomicAdd(db + threadIdx.x, s); else db[threadIdx.x] = s;
+  if (blockIdx.x == 0) {                                            // (uniform in the block: the tree synchronises it)
+    slab_colsum_tree<CP>(ds, nb);
+    if (threadIdx.x < C) {
+      const float s = ds[threadIdx.x];
+      if (atomic_b) atomicAdd(db + threadIdx.x, s); else db[threadIdx.x] = s;
+    }
   }
 }
 
@@ -578,6 +596,10 @@ __global__ void head_step_logits_generic(const T* __restrict__ h, const float* _
 
 constexpr int kXentWarps = 8;                                      // rows per block of xent_steps_kernel
 
+// kExact (fp32 activations): the accurate softmax of xent_rows_kernel<true> (head_xent.cu), for the same reasons
+// (tests/test_gpu_head_edges.py::test_per_step_head, fp32 rows of the negative regime: dh up to 15x its budget before); the bf16
+// instantiation keeps the fast intrinsics.
+template <bool kExact>
 __global__ void __launch_bounds__(kXentWarps * 32) xent_steps_kernel(const HeadStepParams p) {
   __shared__ int misc[2];
   __shared__ float red_f[kXentWarps];
@@ -605,12 +627,14 @@ __global__ void __launch_bounds__(kXentWarps * 32) xent_steps_kernel(const HeadS
         if (om > mx || (om == mx && oa < arg)) { mx = om; arg = oa; }
       }
       float se = 0.f;
-      for (int c = lane; c < p.C; c += 32) se += expf(l[c] - mx);
+      for (int c = lane; c < p.C; c += 32) se += kExact ? ts::expf_acc(l[c] - mx) : expf(l[c] - mx);
       se = ts::warp_sum(se);
-      const float lse = mx + logf(se);
+      const float ls = kExact ? ts::logf_acc(se) : logf(se);
+      const float lse = mx + ls;
       const int y = (int)p.labels[(size_t)b * p.T + t];
-      for (int c = lane; c < p.C; c += 32) d[c] = (expf(l[c] - lse) - (c == y ? 1.f : 0.f)) * invN;
-      if (lane == 0) { nll = lse - l[y]; ok = arg == y ? 1 : 0; }
+      for (int c = lane; c < p.C; c += 32)
+        d[c] = ((kExact ? ts::expf_acc((l[c] - mx) - ls) : expf(l[c] - lse)) - (c == y ? 1.f : 0.f)) * invN;
+      if (lane == 0) { nll = kExact ? (mx - l[y]) + ls : lse - l[y]; ok = arg == y ? 1 : 0; }
     }
   }
   if (lane == 0) { red_f[warp] = nll; red_i[warp] = ok; }
@@ -694,10 +718,9 @@ __global__ void __launch_bounds__(128) head_step_bwd_kernel(const T* __restrict_
       pdw[((size_t)blockIdx.y * H + jg) * C + c] = ((part[(0 * kHBwdJ + jj) * CP + c] + part[(1 * kHBwdJ + jj) * CP + c]) +
                                                     part[(2 * kHBwdJ + jj) * CP + c]) + part[(3 * kHBwdJ + jj) * CP + c];
   }
-  if (blockIdx.x == 0 && threadIdx.x < C) {
-    float s = 0.f;
-    for (int b = 0; b < nb; ++b) s += ds[b * CP + threadIdx.x];
-    pdb[(size_t)blockIdx.y * C + threadIdx.x] = s;
+  if (blockIdx.x == 0) {                                            // (uniform in the block: the tree synchronises it)
+    slab_colsum_tree<CP>(ds, nb);
+    if (threadIdx.x < C) pdb[(size_t)blockIdx.y * C + threadIdx.x] = ds[threadIdx.x];
   }
   __threadfence();
   __syncthreads();
@@ -833,7 +856,8 @@ extern "C" int ts_head_step_fwd(const void* h, int ldh, int is_bf16, const float
   if (is_bf16) head_step_logits_generic<__nv_bfloat16><<<(unsigned)((n + 255) / 256), 256, 0, st>>>((const __nv_bfloat16*)h, W, bias, logits, T, B, H, C);
   else head_step_logits_generic<float><<<(unsigned)((n + 255) / 256), 256, 0, st>>>((const float*)h, W, bias, logits, T, B, H, C);
   p.num_tiles = (R + kXentWarps - 1) / kXentWarps;
-  xent_steps_kernel<<<p.num_tiles, kXentWarps * 32, 0, st>>>(p);
+  if (is_bf16) xent_steps_kernel<false><<<p.num_tiles, kXentWarps * 32, 0, st>>>(p);
+  else xent_steps_kernel<true><<<p.num_tiles, kXentWarps * 32, 0, st>>>(p);
   return (int)cudaGetLastError();
 }
 extern "C" int ts_head_step_fwd_generic_parts(int R) { return (R + kXentWarps - 1) / kXentWarps; }

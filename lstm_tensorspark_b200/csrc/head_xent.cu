@@ -6,8 +6,13 @@
 
 namespace {
 
+// kExact (fp32 activations): exp / log in fp64 rounded once, and log-probabilities as (l - max) - log(sum) so that no fp32
+// rounding at the magnitude of the logits enters them (tests/test_gpu_head_edges.py::test_last_state_head, fp32 rows of the
+// negative regime, where l - (max + log(sum)) at l ~ -990 was off by up to half an ulp of 990 in every probability).  The bf16
+// instantiation keeps the fast intrinsics and l - (max + log(sum)).  Each row's NLL goes to nll[row]; sum_rows_kernel adds them.
+template <bool kExact>
 __global__ void xent_rows_kernel(const float* __restrict__ logits, const long long* __restrict__ labels,
-                                 float* __restrict__ dlogits, float* __restrict__ loss_sum, int* __restrict__ correct,
+                                 float* __restrict__ dlogits, float* __restrict__ nll, int* __restrict__ correct,
                                  int B, int C) {
   int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   int lane = threadIdx.x & 31;
@@ -23,24 +28,45 @@ __global__ void xent_rows_kernel(const float* __restrict__ logits, const long lo
     if (om > mx || (om == mx && oa < arg)) { mx = om; arg = oa; }
   }
   float se = 0.f;
-  for (int c = lane; c < C; c += 32) se += expf(r[c] - mx);
+  for (int c = lane; c < C; c += 32) se += kExact ? ts::expf_acc(r[c] - mx) : expf(r[c] - mx);
   se = ts::warp_sum(se);
-  float lse = mx + logf(se);
+  const float ls = kExact ? ts::logf_acc(se) : logf(se);
+  float lse = mx + ls;
   int y = (int)labels[warp];
   float invB = 1.0f / (float)B;
   for (int c = lane; c < C; c += 32)
-    dlogits[(size_t)warp * C + c] = (expf(r[c] - lse) - (c == y ? 1.f : 0.f)) * invB;
+    dlogits[(size_t)warp * C + c] = ((kExact ? ts::expf_acc((r[c] - mx) - ls) : expf(r[c] - lse)) - (c == y ? 1.f : 0.f)) * invB;
   if (lane == 0) {
-    atomicAdd(loss_sum, lse - r[y]);
+    nll[warp] = kExact ? (mx - r[y]) + ls : lse - r[y];
     if (arg == y) atomicAdd(correct, 1);
   }
 }
 
+// loss_sum = the sum of nll [B] in a fixed order: thread t adds rows t, t + 256, ..., then a tree over the threads.  (One fp32
+// atomicAdd per row summed in whatever order the warps arrived: not reproducible, and up to 2x the fp32 budget of the loss over
+// 200 rows, tests/test_gpu_head_edges.py::test_last_state_head, fp32 rows.)
+constexpr int kSumThreads = 256;
+__global__ void __launch_bounds__(kSumThreads) sum_rows_kernel(const float* __restrict__ nll, float* __restrict__ loss_sum, int B) {
+  __shared__ float red[kSumThreads];
+  float s = 0.f;
+  for (int i = threadIdx.x; i < B; i += kSumThreads) s += nll[i];
+  red[threadIdx.x] = s;
+  __syncthreads();
+  for (int w = kSumThreads / 2; w > 0; w >>= 1) {
+    if (threadIdx.x < w) red[threadIdx.x] += red[threadIdx.x + w];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) *loss_sum = red[0];
+}
+
 }  // namespace
 
-extern "C" int ts_xent_rows(const float* logits, const long long* labels, float* dlogits, float* loss_sum, int* correct,
-                            int B, int C, cudaStream_t st) {
+// exact: the fp32 path's accurate softmax (xent_rows_kernel<true>).  nll: scratch [B].  loss_sum is overwritten.
+extern "C" int ts_xent_rows(const float* logits, const long long* labels, float* dlogits, float* nll, float* loss_sum, int* correct,
+                            int B, int C, int exact, cudaStream_t st) {
   int thr = 128, blk = (B * 32 + thr - 1) / thr;
-  xent_rows_kernel<<<blk, thr, 0, st>>>(logits, labels, dlogits, loss_sum, correct, B, C);
+  if (exact) xent_rows_kernel<true><<<blk, thr, 0, st>>>(logits, labels, dlogits, nll, correct, B, C);
+  else xent_rows_kernel<false><<<blk, thr, 0, st>>>(logits, labels, dlogits, nll, correct, B, C);
+  sum_rows_kernel<<<1, kSumThreads, 0, st>>>(nll, loss_sum, B);
   return (int)cudaGetLastError();
 }

@@ -20,6 +20,8 @@ TS_DEVICE float sigmoidf_fast(float x) { return fmaf(0.5f, tanhf_fast(0.5f * x),
 // bf16); it leaves fp64 math alone.
 TS_DEVICE float tanhf_acc(float x) { return (float)tanh((double)x); }
 TS_DEVICE float sigmoidf_acc(float x) { return (float)(1.0 / (1.0 + exp(-(double)x))); }
+TS_DEVICE float expf_acc(float x) { return (float)exp((double)x); }
+TS_DEVICE float logf_acc(float x) { return (float)log((double)x); }
 
 template <typename T> struct Cvt;
 template <> struct Cvt<float> {

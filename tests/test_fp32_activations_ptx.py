@@ -1,8 +1,8 @@
-"""The fp32 instantiations of the cell kernels (csrc/lstm_pointwise.cu) and of the attention scores (csrc/seq_pool.cu) must not
-use the approximate activations.  build.py compiles with --use_fast_math, under which tanhf becomes tanh.approx.f32 and
-expf / division ex2.approx / rcp.approx (relative error up to about 2^-11): the fp32 path would then be no more accurate than
-the bf16 one, which keeps them on purpose.  This compiles both files to PTX with the build's own flags and reads every kernel
-entry; it needs nvcc, not a GPU."""
+"""The fp32 instantiations of the cell kernels (csrc/lstm_pointwise.cu), of the attention scores (csrc/seq_pool.cu) and of the
+heads' generic softmax (csrc/head_xent.cu, csrc/head_wgmma.cu) must not use the approximate activations.  build.py compiles
+with --use_fast_math, under which tanhf becomes tanh.approx.f32 and expf / logf / division ex2.approx / lg2.approx / rcp.approx
+(relative error up to about 2^-11): the fp32 path would then be no more accurate than the bf16 one, which keeps them on
+purpose.  This compiles the files to PTX with the build's own flags and reads every kernel entry; it needs nvcc, not a GPU."""
 import os
 import re
 import shutil
@@ -57,3 +57,16 @@ def test_fp32_attention_scores_use_no_approximate_tanh(tmp_path):
     assert len(exact) == 1 and len(fast) == 1, sorted(scores)
     assert "tanh.approx" not in scores[exact[0]]
     assert "tanh.approx.f32" in scores[fast[0]]
+
+
+@pytest.mark.skipif(_nvcc() is None, reason="needs nvcc")
+@pytest.mark.parametrize("src,kernel", [("head_xent.cu", "xent_rows_kernel"), ("head_wgmma.cu", "xent_steps_kernel")])
+def test_fp32_softmax_heads_use_no_approximate_exp_or_log(tmp_path, src, kernel):
+    """The generic softmax of the last-state and per-step heads: the fp32 instantiation (kExact) takes exp and log in fp64, the
+    bf16 one keeps ex2.approx / lg2.approx (the control of the parser)."""
+    ents = _entries(src, tmp_path)
+    exact = [b for n, b in ents.items() if f"{kernel}ILb1E" in n]
+    fast = [b for n, b in ents.items() if f"{kernel}ILb0E" in n]
+    assert len(exact) == 1 and len(fast) == 1, sorted(ents)
+    assert not re.findall(r"\b(?:ex2|lg2)\.approx(?:\.ftz)?\.f32", exact[0])
+    assert re.search(r"\bex2\.approx(?:\.ftz)?\.f32", fast[0]) and re.search(r"\blg2\.approx(?:\.ftz)?\.f32", fast[0])

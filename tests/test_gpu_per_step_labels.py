@@ -112,33 +112,38 @@ def _per_step_labels(n, T, seed):
 
 
 def _case(case, hidden, T, B, D, path, steps=2, lengths_seed=None, bidirectional=False, dropout=0.0, learning_rate=0.0,
-          graph=False, negative=False):
+          graph=False, negative=False, dtype=torch.bfloat16):
     """Training steps, each checked (loss and every gradient of the flat buffer) against the fp64 reference at the weights it
-    read.  ``path``: a STATS key one step must bump (besides the per-step head on the tensor cores).  ``graph``: captured on the
-    first batch and replayed on every batch, each with lengths of its own.  ``negative``: the reference (both arms) normalises by
-    T·B - the loss check must fail."""
+    read.  ``path``: a STATS key one step must bump (besides the per-step head: on the tensor cores in bf16, on the generic
+    kernels in fp32).  ``graph``: captured on the first batch and replayed on every batch, each with lengths of its own.
+    ``negative``: the reference (both arms) normalises by T·B - the loss check must fail.  ``dtype``: the engine's compute
+    dtype (fp32: the lstm_numerics.Fp32 arm and floor, and the reference reads the fp32 master)."""
     from lstm_tensorspark_b200 import data as Dm
-    eng = _engine(hidden_units=hidden, in_features=D, seq_len=T, batch_size=B, num_classes=C, bidirectional=bidirectional,
+    bf16 = dtype == torch.bfloat16
+    head_key = "head_per_step_tc" if bf16 else "head_per_step"
+    eng = _engine(dtype, hidden_units=hidden, in_features=D, seq_len=T, batch_size=B, num_classes=C, bidirectional=bidirectional,
                   dropout=dropout, variable_length=lengths_seed is not None, learning_rate=learning_rate, per_step_labels=True)
     flat = eng.flat
     xs, _ = Dm.synthetic_sequences(steps * B, T, D, C, seed=5)
-    xs, ys = torch.as_tensor(xs).to(DEV).bfloat16(), _per_step_labels(steps * B, T, 7)
+    xs, ys = torch.as_tensor(xs).to(DEV).to(dtype), _per_step_labels(steps * B, T, 7)
     seg = _segments(eng, _names(eng))
-    rounding = _roundings([int(h) for h in hidden.split(",")], T, B, D, bidirectional)
+    rounding = _roundings([int(h) for h in hidden.split(",")], T, B, D, bidirectional) if bf16 else N.Fp32()
+    floor = N.FLOOR if bf16 else N.FLOOR_F32
     worst = {}
     for s in range(steps):
         x, y = xs[s * B:(s + 1) * B], ys[s * B:(s + 1) * B]
         lengths = None if lengths_seed is None else _lengths(T, B, lengths_seed + s)
         before = {"p": flat.data.clone(), "drop": int(eng.model.rnn.dropout_step)}
-        n_tc, n_path = _stat("head_per_step_tc"), _stat(path)
+        n_tc, n_path, n_tc_any = _stat(head_key), _stat(path), _stat("head_per_step_tc")
         if graph and s == 0:
             eng.capture(x, y, lengths=lengths)
-            assert _stat("head_per_step_tc") > n_tc and _stat(path) > n_path, case
-            n_tc, n_path = _stat("head_per_step_tc"), _stat(path)
+            assert _stat(head_key) > n_tc and _stat(path) > n_path, case
+            n_tc, n_path = _stat(head_key), _stat(path)
         loss = eng.step(x, y, lengths)
         torch.cuda.synchronize()
         if not graph:
-            assert _stat("head_per_step_tc") == n_tc + 1 and _stat(path) > n_path, (case, s)
+            assert _stat(head_key) == n_tc + 1 and _stat(path) > n_path, (case, s)
+            assert bf16 or _stat("head_per_step_tc") == n_tc_any, (case, s)           # fp32: the generic kernels
         got = {"loss": loss.float()}
         for k, (o, shape) in seg.items():
             got[k] = flat.grad[o:o + shape.numel()].view(shape).clone()
@@ -146,7 +151,7 @@ def _case(case, hidden, T, B, D, path, steps=2, lengths_seed=None, bidirectional
         with torch.no_grad():
             arms = {}
             for arm, dt, r in (("fp64", torch.float64, None), ("emu", torch.float32, rounding)):
-                layers, head = _reference_params(eng, seg, before["p"], dt)
+                layers, head = _reference_params(eng, seg, before["p"], dt, bf16_weights=bf16)
                 l_, g_ = model_per_step(x.to(dt), layers, head, y, lengths, bidirectional, drop, r,
                                         norm_all=negative)
                 arms[arm] = {"loss": l_, **g_}
@@ -155,7 +160,8 @@ def _case(case, hidden, T, B, D, path, steps=2, lengths_seed=None, bidirectional
                     N.check_budget(f"{case} loss", got["loss"], arms["fp64"]["loss"], arms["emu"]["loss"])
                 return
             for k, g in got.items():
-                worst[k] = max(worst.get(k, 0.0), N.check_budget(f"{case} step {s} {k}", g, arms["fp64"][k], arms["emu"][k]))
+                worst[k] = max(worst.get(k, 0.0), N.check_budget(f"{case} step {s} {k}", g, arms["fp64"][k], arms["emu"][k],
+                                                                 floor=floor))
             del arms
     top = sorted(worst.items(), key=lambda kv: -kv[1])[:3]
     print(f"\n{case}: worst budget ratio " + ", ".join(f"{k} {v:.3f}" for k, v in top))
@@ -196,6 +202,13 @@ def test_adam_graph_replays_with_changing_lengths():
     """Captured once, replayed on 3 batches with lengths of their own: N is computed on the device at every replay."""
     _case("per-step adam graph", "1024,1024", 128, 256, 1024, "pipelined_fwd", steps=3, lengths_seed=51, learning_rate=1e-3,
           graph=True)
+
+
+def test_fp32_ragged_adam():
+    """``--dtype fp32`` with lengths, two Adam steps: the layers and the per-step head on the generic kernels (the head's
+    softmax in xent_steps_kernel, its backward on the CUDA cores), against the Fp32 arm with the fp32 floor."""
+    _case("per-step fp32 ragged adam", "48,48", 32, 20, 12, "generic_fwd", lengths_seed=71, learning_rate=1e-3,
+          dtype=torch.float32)
 
 
 def test_negative_control_normalised_by_all_positions():
