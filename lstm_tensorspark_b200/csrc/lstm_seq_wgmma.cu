@@ -15,7 +15,7 @@
 //     the whole cell with one thread per batch row (the cell state never leaves its registers).  With one batch tile per
 //     CTA the two warpgroups split its rows; with two (kTiles = 2) they PING-PONG: each warpgroup owns one tile for the whole
 //     launch, so one tile's cell epilogue, exchange and dataflow signal run while the other tile's MMAs do.  At H = 1024
-//     with two batch tiles per CTA the ring holds 6 stages forward, 4 backward.
+//     with two batch tiles per CTA the ring holds 6 stages forward, 4 backward; with one, 4 forward (pick_stages).
 //   * The forward pass can split K across a cluster of 2 CTAs and the backward pass does across 4 (one gate-column quarter
 //     each); the partial accumulators are reduce-scattered through DISTRIBUTED SHARED MEMORY with st.async (bytes are
 //     counted on the receiver's mbarrier: no release/acquire fences).  Every member then owns 16 hidden units.
@@ -1247,6 +1247,10 @@ int dispatch_dir(const CUtensorMap& tw, const SeqParams& p, int grid, int stages
 }
 
 int pick_stages(int H, bool bwd, int tiles) {
+  // One tile per CTA forward with H >= 1024 (>= 16 k-blocks per step, the resident slice takes >= 128 KB): 4 stages, not the
+  // deepest ring that fits.  At B = 256, H = 1024 on an H100 80GB HBM3 (700 W) a step took 10.9-11.5 us with 4 stages against
+  // 11.3-12.1 us with 6 (11.3-11.8 with 5, 12.1-12.4 with 3), eight runs each; 4 was the fastest within every set of runs.
+  if (!bwd && tiles == 1 && H / BK >= 16 && smem_bytes(H, false, 4, 1) <= 227 * 1024) return 4;
   for (int s = 6; s >= 2; --s)
     if (smem_bytes(H, bwd, s, tiles) <= 227 * 1024) return s;
   return 0;

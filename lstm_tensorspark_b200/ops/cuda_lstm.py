@@ -145,26 +145,58 @@ def _bwd_cluster(H: int) -> int:
     return 4 if H <= 1024 else 2
 
 
-def _tiles_per_cta(B: int, H: int, device) -> Optional[int]:
+def tiles_per_cta(B: int, H: int, coresident: int) -> Optional[int]:
     """Batch tiles per CTA of the persistent kernels (1, or 2 when one tile per CTA needs more CTAs than can be co-resident),
-    None when neither fits.  H / 16 CTAs per batch tile (pair); all of them must be co-resident (dataflow sync between CTAs),
-    in clusters for the backward pass.  Two tiles per CTA need the resident weight slice (H <= 1024); larger H streams it through
-    the ring (csrc/lstm_seq_wgmma.cu, kStream; the streamed backward takes H <= 2048)."""
+    None when neither fits, with ``coresident`` CTAs of the backward kernel co-resident in its clusters (``_coresident_ctas``).
+    H / 16 CTAs per batch tile (pair); all of them must be co-resident (dataflow sync between CTAs), in clusters for the
+    backward pass.  Two tiles per CTA need the resident weight slice (H <= 1024); larger H streams it through the ring
+    (csrc/lstm_seq_wgmma.cu, kStream; the streamed backward takes H <= 2048)."""
     if H > 2048:
         return None
     tiles_m = (B + 127) // 128
-    n = _coresident_ctas(device, _bwd_cluster(H))
-    if tiles_m * (H // 16) <= n:
+    if tiles_m * (H // 16) <= coresident:
         return 1
-    if H <= 1024 and tiles_m % 2 == 0 and (tiles_m // 2) * (H // 16) <= n:
+    if H <= 1024 and tiles_m % 2 == 0 and (tiles_m // 2) * (H // 16) <= coresident:
         return 2
     return None
+
+
+def _tiles_per_cta(B: int, H: int, device) -> Optional[int]:
+    return tiles_per_cta(B, H, _coresident_ctas(device, _bwd_cluster(H)))
+
+
+def fwd_tiles_per_cta(B: int, H: int, sms: int, coresident) -> Optional[int]:
+    """Batch tiles per CTA of a forward recurrence that has the GPU to itself, on a device with ``sms`` SMs;
+    ``coresident(cluster)``: CTAs co-resident in thread-block clusters of that size (``_coresident_ctas``).
+    ``tiles_per_cta`` picks the tile count from the backward kernel's clusters of 4, which an H100 co-schedules on only 120
+    of its 132 SMs: at B = 256, H = 1024 that means two tiles on 64 CTAs.  The forward kernel runs without clusters (or in
+    clusters of 2 with its K-split), so its 128 one-tile CTAs fit, and each then has half the MMA work per step and no second
+    tile to wait behind.  1 where ``tiles_m * H / 16`` one-tile CTAs fit the forward kernel's own co-residency, else what
+    ``tiles_per_cta`` returns."""
+    tiles = tiles_per_cta(B, H, coresident(_bwd_cluster(H)))
+    if tiles != 2:
+        return tiles
+    fsplit = ext().lstm_seq_config(False, H, B, SEQ_VARIANT & ~15)[3]      # the one-tile launch's K-split (no device needed)
+    return 1 if (B + 127) // 128 * (H // 16) <= (coresident(2) if fsplit else sms) else 2
 
 
 def _seq_variant(B: int, H: int, device) -> int:
     if SEQ_VARIANT & 15 or _tiles_per_cta(B, H, device) != 2:
         return SEQ_VARIANT
     return SEQ_VARIANT | 2
+
+
+def _fwd_full_width(B: int, H: int, device) -> bool:
+    """Does a forward recurrence that runs alone take one batch tile per CTA where ``_seq_variant`` (which the backward
+    pass needs) takes two?  Decided from the device's SM count and cluster co-residency up front, not by a failed launch."""
+    if SEQ_VARIANT & 15 or _tiles_per_cta(B, H, device) != 2:
+        return False
+    return fwd_tiles_per_cta(B, H, _sms(device), lambda c: _coresident_ctas(device, c)) == 1
+
+
+def _fwd_variant(B: int, H: int, device) -> int:
+    """Variant of a forward recurrence with nothing co-resident beside it (``_fwd_full_width``)."""
+    return SEQ_VARIANT if _fwd_full_width(B, H, device) else _seq_variant(B, H, device)
 
 
 def fast_path_supported(B: int, H: int, dtype: torch.dtype, device) -> bool:
@@ -275,13 +307,17 @@ class _LSTMSeqFn(torch.autograd.Function):
         drop = _drop_args(dropout, x_seq.device)
         h_drop = None
         if fast:
-            outs = E.lstm_seq_fwd(gx, w_h_c, bias_f, h0c, c0f, _sync_ws(x_seq.device), _seq_variant(B, H, x_seq.device),
+            # the only recurrence on the GPU: the forward kernel's own co-residency decides its tile count (_fwd_full_width)
+            full = _fwd_full_width(B, H, x_seq.device)
+            outs = E.lstm_seq_fwd(gx, w_h_c, bias_f, h0c, c0f, _sync_ws(x_seq.device), _fwd_variant(B, H, x_seq.device),
                                   lengths=lengths, reverse=reverse, **drop)
             h_seq, c_seq, act = outs[:3]
             if drop:
                 h_drop = outs[3]                                          # written next to h_seq by the recurrence kernel
             STATS["fast_fwd"] += 1
             STATS["kernels"] += 1
+            if full:
+                count("fwd_full_width")
         else:
             h_seq = torch.empty(T + 1, B, H, dtype=cd, device=x_seq.device)
             c_seq = torch.empty(T + 1, B, H, dtype=torch.float32, device=x_seq.device)
@@ -460,7 +496,8 @@ def _pair_ws(device, tag: str, n_done: int):
 
 def pair_schedule(T: int, B: int, D: int, h_a: int, h_b: int, sms: int, coresident: int) -> Optional[str]:
     """How two stacked layers run as one op on a device with ``sms`` SMs, ``coresident`` of which hold backward-kernel CTAs in
-    clusters of 4 (``_coresident_ctas``).  Every recurrence runs two batch tiles per CTA, H/16 CTAs.  Both schedules need
+    clusters of 4 (``_coresident_ctas``).  Every recurrence runs two batch tiles per CTA, H/16 CTAs (except the pipelined
+    L_b forward, which runs alone: one tile per CTA where that fits, ``_fwd_full_width``).  Both schedules need
     B = 256 (one GEMM tile row per time step), resident weights (H <= 1024) and 256-aligned widths.
       "wavefront": both recurrences co-resident, the gated GEMM on the SMs they leave free (H_a/16 + H_b/16 + 8 SMs).
       "pipelined": the recurrences run one after the other, GEMMs next to them (forward: L_a with its own gx_a and with gx_b;
@@ -611,7 +648,15 @@ class _LSTMPairFn(torch.autograd.Function):
                 gate=ws_a[_gate_off(var):], gate_cfg=_gate_cfg(var, 2, Ha // 64, 4, 4 * Ha // 64, 2, 1, B, False), done=done,
                 gate_err=ws_a[SYNC_WORDS - 1:], pdl=True)
         if pipelined:
-            E.lstm_seq_fwd_into(gx_b, whb, bb_f, h0b_c, c0b_f, h_seq_b, c_seq_b, act_b, til_b, ws_b, var, None, 0, False, 0, 1, lengths,
+            # L_b is an ordinary launch after gx_a / gx_b are complete: nothing runs beside it, so it takes one batch tile per CTA
+            # where that fits (128 CTAs at B = 256, H_b = 1024; _fwd_full_width).  Its counters stay per k-block (sync mode 0 of
+            # the pipelined variant), and til_b is sized per batch tile, whatever the tiles per CTA.  No warm-up is needed for
+            # this instantiation (_warm_wavefront_kernels): its first launch comes after its producers have finished.
+            var_b = var
+            if _fwd_full_width(B, Hb, dev):
+                var_b = var & ~15
+                count("fwd_full_width")
+            E.lstm_seq_fwd_into(gx_b, whb, bb_f, h0b_c, c0b_f, h_seq_b, c_seq_b, act_b, til_b, ws_b, var_b, None, 0, False, 0, 1, lengths,
                                 h_drop=h_drop_b, **drb)
         STATS["fast_fwd"] += 2
         STATS["kernels"] += 3
