@@ -64,6 +64,8 @@ class Config:
     embedding_dropout: float = 0.0      # in training, whole rows of the embedding table are dropped for the lookup, one mask per step
     locked_dropout: bool = False        # --dropout / --output_dropout / --input_dropout draw one mask per sequence and training step,
                                         # shared by every time step (AWD-LSTM's LockedDropout), not a new mask per step
+    activation_reg: float = 0.0         # AWD-LSTM's AR: training adds ALPHA * mean(out^2) of the top layer's output as the head reads it
+    temporal_activation_reg: float = 0.0  # AWD-LSTM's TAR: training adds BETA * mean((h_t - h_{t-1})^2) of its raw output
     per_step_labels: bool = False       # sequence labelling: a label at every time step ([B,T]), the head scores the top layer's
                                         # output at each step (nn.LSTM -> nn.Linear -> cross_entropy over the real positions); a CSV
                                         # row is k*in_features values followed by k labels
@@ -249,6 +251,14 @@ class Config:
             raise ValueError("--output_dropout needs a head that reads the top layer's output sequence (--per_step_labels, "
                              "--next_token or --pooling mean | max | attention): with --pooling last the head reads only the "
                              "final state, and there is no sequence to drop")
+        for flag in ("activation_reg", "temporal_activation_reg"):
+            c = getattr(self, flag)
+            if not (math.isfinite(c) and c >= 0):
+                raise ValueError(f"--{flag} must be a finite number >= 0 (0 = off), got {c}")
+            if c > 0 and self.pooling == "last" and not self.per_step_labels:
+                raise ValueError(f"--{flag} needs a head that reads the top layer's output sequence (--per_step_labels, "
+                                 "--next_token or --pooling mean | max | attention): with --pooling last the head reads only the "
+                                 "final state, and there is no sequence to regularise")
         if self.locked_dropout and not (self.dropout > 0 or self.output_dropout > 0 or self.input_dropout > 0):
             warnings.warn("--locked_dropout has no effect without --dropout, --output_dropout or --input_dropout > 0: it shares "
                           "their masks across time steps")
@@ -365,6 +375,13 @@ _HELP = {
     "locked_dropout": "Locked (variational) dropout: --dropout, --output_dropout and --input_dropout draw one mask per sequence "
                       "and training step, shared by every time step (AWD-LSTM's LockedDropout; Gal & Ghahramani 2016), instead "
                       "of a new mask at every step",
+    "activation_reg": "AWD-LSTM's activation regularisation (AR): in training, the loss backward runs on gains ALPHA times the "
+                      "mean square of the top layer's output as the head reads it (after --output_dropout) over the real "
+                      "positions; the reported loss stays the cross-entropy, and AR is logged as `ar`.  Needs --per_step_labels, "
+                      "--next_token or --pooling mean | max | attention.  0 = off",
+    "temporal_activation_reg": "AWD-LSTM's temporal activation regularisation (TAR): in training, the loss backward runs on gains "
+                               "BETA times the mean square of h_t - h_{t-1} of the top layer's raw output (before dropout) over "
+                               "the real steps t >= 1 of each sequence; logged as `tar`.  Same head rule as --activation_reg.  0 = off",
     "per_step_labels": "Label every time step (sequence labelling): labels [B,T], loss and accuracy over the real positions; "
                        "a CSV row is k*in_features values followed by k labels",
 }

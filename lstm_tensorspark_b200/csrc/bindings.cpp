@@ -75,6 +75,10 @@ int ts_lstm_seq_bwd(const void*, const void*, const void*, const float*, const v
                     const int*, const unsigned int*);
 int ts_dropout(const void*, void*, int, int, int, int, int, const int*, const unsigned int*, cudaStream_t);
 int ts_weight_drop_grad(const float*, float*, int, int, int, const int*, const unsigned int*, cudaStream_t);
+long long ts_act_reg_scratch(int, int, int, int);
+int ts_act_reg_fwd(const void*, const void*, const int*, int, int, int, int, double*, float*, cudaStream_t);
+int ts_act_reg_bwd(const void*, const void*, const void*, const int*, const float*, int, int, int, int, const int*, const unsigned int*,
+                   void*, cudaStream_t);
 int ts_lstm_seq_prologue(const void*, const float*, void*, float*, void*, unsigned int*, int, int, cudaStream_t);
 int ts_seq_pool_fwd(const void*, int, const int*, const float*, int, int, int, int, float*, int*, cudaStream_t);
 int ts_seq_pool_attn_scores(float*, const float*, const float*, const int*, int, int, int, float*, int, cudaStream_t);
@@ -255,6 +259,55 @@ Tensor dropout(const Tensor& x, const Tensor& step, const std::vector<int64_t>& 
   auto y = torch::empty_like(x);
   check(ts_dropout(x.data_ptr(), y.data_ptr(), (int)steps, (int)B, (int)H, (int)t0, is_bf16(x), ds, dd, stream()), "dropout");
   return y;
+}
+
+// Activation regularisation (csrc/activation_reg.cu).  h: the top layer's raw output [T,B,H] (bf16 / fp32, time order), out: the
+// sequence the head reads when it is not h (output dropout), lengths: optional int32 [B].  -> fp32 [2] = {sum out^2,
+// sum (h_t - h_{t-1})^2} over the counted positions.  scratch: float64 [act_reg_scratch(T, B, H, bf16)], zero before its first
+// use (every call leaves it zero).
+void act_reg_same_shape(const std::optional<Tensor>& t, const Tensor& h, const char* n) {
+  if (!t.has_value()) return;
+  chk_cuda(*t, n);
+  TORCH_CHECK(t->sizes() == h.sizes() && t->scalar_type() == h.scalar_type() && t->device() == h.device(), n,
+              " must have h's shape, dtype and device");
+}
+
+Tensor act_reg_fwd(const std::optional<Tensor>& out, const Tensor& h, const std::optional<Tensor>& lengths, Tensor scratch) {
+  chk_cuda(h, "h");
+  TORCH_CHECK(h.dim() == 3, "act_reg_fwd: h must be [T,B,H]");
+  act_reg_same_shape(out, h, "out");
+  const int64_t T = h.size(0), B = h.size(1), H = h.size(2);
+  chk_cuda(scratch, "scratch");
+  TORCH_CHECK(scratch.scalar_type() == torch::kFloat64 && scratch.device() == h.device() &&
+              scratch.numel() >= ts_act_reg_scratch((int)T, (int)B, (int)H, is_bf16(h)), "act_reg_fwd: scratch float64 [act_reg_scratch(T, B, H, bf16)]");
+  c10::cuda::CUDAGuard g(h.device());
+  auto sums = torch::empty({2}, h.options().dtype(torch::kFloat32));
+  check(ts_act_reg_fwd(out.has_value() ? out->data_ptr() : nullptr, h.data_ptr(), lengths_ptr(lengths, B, h), (int)T, (int)B, (int)H,
+                       is_bf16(h), scratch.data_ptr<double>(), sums.data_ptr<float>(), stream()), "act_reg_fwd");
+  return sums;
+}
+
+// The gradient into the top layer's raw output: keep * s * (dh + 2 g0 out) + 2 g1 (the TAR stencil of h) at counted positions,
+// keep * s * dh elsewhere, in h's dtype.  dh: the head's gradient with respect to the sequence it reads (None: zero); g: fp32 [2] d loss / d sums;
+// drop_step / drop_desc: the output dropout's mask (None: none; out must then be None too).
+Tensor act_reg_bwd(const std::optional<Tensor>& dh, const std::optional<Tensor>& out, const Tensor& h, const std::optional<Tensor>& lengths,
+                   const Tensor& g, const std::optional<Tensor>& drop_step, const std::vector<int64_t>& drop_desc) {
+  chk_cuda(h, "h");
+  TORCH_CHECK(h.dim() == 3, "act_reg_bwd: h must be [T,B,H]");
+  act_reg_same_shape(dh, h, "dh");
+  act_reg_same_shape(out, h, "out");
+  chk_cuda(g, "g");
+  TORCH_CHECK(g.scalar_type() == torch::kFloat32 && g.numel() == 2 && g.device() == h.device(), "act_reg_bwd: g must be fp32 [2]");
+  TORCH_CHECK(out.has_value() == drop_step.has_value(), "act_reg_bwd: out is the dropped sequence: pass it with the dropout and only then");
+  const int64_t T = h.size(0), B = h.size(1), H = h.size(2);
+  c10::cuda::CUDAGuard guard(h.device());
+  unsigned int dd[5];
+  const int* ds = drop_args(drop_step, drop_desc, h, dd);
+  auto dst = torch::empty_like(h);
+  check(ts_act_reg_bwd(dh.has_value() ? dh->data_ptr() : nullptr, out.has_value() ? out->data_ptr() : nullptr, h.data_ptr(),
+                       lengths_ptr(lengths, B, h), g.data_ptr<float>(), (int)T, (int)B, (int)H, is_bf16(h), ds, dd, dst.data_ptr(),
+                       stream()), "act_reg_bwd");
+  return dst;
 }
 
 // Weight drop's gradient: dst (+)= src * mask * scale over fp32 [R, H] (R = 4H rows of W_h), the mask of `desc` at time 0, as
@@ -1108,6 +1161,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("lstm_seq_bwd", &lstm_seq_bwd, py::arg("dh_seq"), py::arg("w_hT"), py::arg("act"), py::arg("c_seq"), py::arg("dhT"),
         py::arg("dcT"), py::arg("sync_ws"), py::arg("variant") = 0, py::arg("dbg") = py::none(), py::arg("in_gate") = py::none(),
         py::arg("in_gate_tiles_n") = 0, py::arg("extra_signal") = false, py::arg("lengths") = py::none(), py::arg("reverse") = false,
+        py::arg("drop_step") = py::none(), py::arg("drop_desc") = std::vector<int64_t>{});
+  m.def("act_reg_scratch", [](int64_t T, int64_t B, int64_t H, bool bf16) { return ts_act_reg_scratch((int)T, (int)B, (int)H, bf16 ? 1 : 0); });
+  m.def("act_reg_fwd", &act_reg_fwd, py::arg("out"), py::arg("h"), py::arg("lengths"), py::arg("scratch"));
+  m.def("act_reg_bwd", &act_reg_bwd, py::arg("dh"), py::arg("out"), py::arg("h"), py::arg("lengths"), py::arg("g"),
         py::arg("drop_step") = py::none(), py::arg("drop_desc") = std::vector<int64_t>{});
   m.def("dropout", &dropout, py::arg("x"), py::arg("step"), py::arg("desc"), py::arg("t0") = 0);
   m.def("weight_drop_grad", &weight_drop_grad, py::arg("src"), py::arg("dst"), py::arg("step"), py::arg("desc"),

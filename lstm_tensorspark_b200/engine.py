@@ -6,6 +6,7 @@ This is what ``bench.py``, ``__graft_entry__.smoke`` and the per-replica trainer
     loss = eng.step(x, y)            # forward, backward, (fused allreduce +) optimizer update
     loss = eng.step(x, y, lengths)   # variable-length batch: int32 [B] per-sample lengths, x right-padded
     norm = eng.grad_norm()           # --clip_grad_norm: the last step's gradient norm before clipping (None without)
+    ar_tar = eng.activation_penalties()  # --activation_reg / --temporal_activation_reg: the last step's (AR, TAR) (None without)
     loss = eng.step(x, y, reset=k == 0)  # --stateful: batch k of a pass continues every stream from the state batch k-1 ended in
 
 One step replaces the reference's ``sess.run([train_op, loss], feed_dict=...)`` (original src/rnn.py:264-267):
@@ -98,6 +99,9 @@ class TrainEngine:
             bs = cfg.batch_size if batch_size is None else batch_size
             self.state = rnn.zero_state(bs, dtype, device)
             self.state_prev = rnn.zero_state(bs, dtype, device)
+        # --activation_reg / --temporal_activation_reg: the coefficients, and a static [2] buffer of the last step's (AR, TAR)
+        self.act_reg = (float(getattr(cfg, "activation_reg", 0.0)), float(getattr(cfg, "temporal_activation_reg", 0.0)))
+        self._act_pen = torch.zeros(2, dtype=torch.float32, device=device) if any(self.act_reg) else None
 
     # ---------------------------------------------------------------------------------------------------
     def _make_bucket_plan(self):
@@ -169,14 +173,20 @@ class TrainEngine:
         loss, _logits, _correct = self.model(x, y, lengths, state=self.state_prev)
         if self._wd_autograd:
             loss = loss + torch.stack([fn(v) * wd for (v, fn, wd) in self._wd_autograd]).sum()
+        train_loss = loss
+        if self._act_pen is not None:          # AR / TAR weigh into what backward runs on, not into the reported loss
+            pen = self.model.rnn.activation_penalties
+            with torch.no_grad():
+                self._act_pen.copy_(pen)
+            train_loss = loss + self.act_reg[0] * pen[0] + self.act_reg[1] * pen[1]
         l2 = None
         if self._wd_in_kernel:                 # reported total loss includes the L2 value (of the weights this step used); its
             with torch.no_grad():              # gradient is applied by the update kernel
                 l2 = torch.stack([fn(v) * wd for (v, fn, wd) in self._wd_in_kernel]).sum()
         if self._bucket_plan:
-            self._backward_with_buckets(loss)      # backward + per-bucket fused allreduce / update, overlapped with backward
+            self._backward_with_buckets(train_loss)  # backward + per-bucket fused allreduce / update, overlapped with backward
         else:
-            loss.backward()
+            train_loss.backward()
             self.flat.finalize_grads()
             if self.sync_grads:
                 self.comm.grad_step_(self.flat, self.optimizer)
@@ -248,6 +258,12 @@ class TrainEngine:
         if self.optimizer.clip_norm <= 0:
             return None
         return self.optimizer.clip_out[0].clone()
+
+    def activation_penalties(self) -> Optional[torch.Tensor]:
+        """``--activation_reg`` / ``--temporal_activation_reg``: the unweighted ``(AR, TAR)`` of the last training step, a device
+        fp32 ``[2]`` tensor (the static buffer every step, and every replay of a captured one, rewrites; copy it to keep it), else
+        None."""
+        return self._act_pen
 
     def carried_state(self):
         """``--stateful``: ``[(h [B,H], c [B,H]) per layer]``, the buffers the next step starts from (None without the flag)."""

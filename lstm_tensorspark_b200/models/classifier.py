@@ -89,6 +89,8 @@ class SequenceClassifier(nn.Module):
         self.rnn = RNN(settings, dropout=cfg.dropout, weight_drop=getattr(cfg, "weight_drop", 0.0),
                        output_dropout=getattr(cfg, "output_dropout", 0.0), input_dropout=getattr(cfg, "input_dropout", 0.0),
                        embedding_dropout=getattr(cfg, "embedding_dropout", 0.0),
+                       activation_reg=getattr(cfg, "activation_reg", 0.0),
+                       temporal_activation_reg=getattr(cfg, "temporal_activation_reg", 0.0),
                        locked=getattr(cfg, "locked_dropout", False), learn_initial_state=cfg.resolved_learn_initial_state(), init_std=cfg.init_std,
                        init=cfg.init, weight_decay=(cfg.weight_decay or None), device=device, generator=generator)
         # --tie_embeddings: the softmax reads the embedding table (head_weights); Dense1/weights is drawn and discarded

@@ -161,21 +161,23 @@ class LSTMLayer(nn.Module):
 
     # ---- whole-sequence path (the thing the persistent kernel implements) ----------------------
     def fit_sequence(self, x_seq: torch.Tensor, lengths: Optional[torch.Tensor] = None, dropout=None,
-                     weight_drop=None) -> torch.Tensor:
+                     weight_drop=None, activation_sums: bool = False):
         """``x_seq [T,B,D]`` -> ``h_seq [T,B,H]``; final (ht, Ct) stored on the layer.  ``lengths`` (int32 ``[B]``, right
         padding): the final state is each row's state after its own last step; padded positions of ``h_seq`` carry it.
         A reverse layer runs from the last step to the first: its final state is the one after step 0, and its padded
         positions hold the initial state.  ``dropout``: optional ``ops.reference.DropoutSpec``; the returned sequence is then
         the dropped one (the final state is not dropped).  ``weight_drop``: optional weight-drop ``DropoutSpec``: every step reads
-        ``W_h * M * s`` (``ops.reference.weight_drop``) and ``w_h`` gets the masked gradient."""
+        ``W_h * M * s`` (``ops.reference.weight_drop``) and ``w_h`` gets the masked gradient.  ``activation_sums``: ->
+        ``(h_seq, sums)``, ``sums`` the layer's unnormalised AR / TAR sums ``[2]`` (``ops.reference.activation_sums``)."""
         B = x_seq.shape[1]
         if B != self.ht.shape[0]:
             self.reset_state(B)
-        h_seq, h_T, c_T = F.lstm_layer_sequence(x_seq, self.ht, self.Ct, self.w_x, self.w_h, self.bias, lengths=lengths,
-                                                reverse=self.reverse, dropout=dropout, weight_drop=weight_drop)
+        outs = F.lstm_layer_sequence(x_seq, self.ht, self.Ct, self.w_x, self.w_h, self.bias, lengths=lengths,
+                                     reverse=self.reverse, dropout=dropout, weight_drop=weight_drop, activation_sums=activation_sums)
+        h_seq, h_T, c_T = outs[:3]
         self._set_state(h_T, c_T)
         self.state.append((h_T, c_T))
-        return h_seq
+        return (h_seq, outs[3]) if activation_sums else h_seq
 
     def named_reference_variables(self):
         """(reference variable name, tensor) in the §2.7 checkpoint naming."""

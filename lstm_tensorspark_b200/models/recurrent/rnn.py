@@ -11,16 +11,19 @@ recurrent weights ``W_h`` in training mode, one mask per training step (AWD-LSTM
 ``output_dropout`` drops the top layer's output sequence, ``input_dropout`` the embedding output and ``embedding_dropout``
 whole rows of the embedding table (the model's embedding reads ``input_dropout_spec`` / ``embedding_dropout_spec``);
 ``locked`` shares one mask of ``dropout``, ``output_dropout`` and ``input_dropout`` across every time step (AWD-LSTM's
-``LockedDropout``).
+``LockedDropout``).  ``activation_reg`` / ``temporal_activation_reg`` (AWD-LSTM's AR / TAR coefficients): when either is
+non-zero, a forward pass in training mode asks the op of the top layer for its activation sums and leaves the normalised
+``(AR, TAR)`` in ``activation_penalties`` (``ops.reference.activation_penalties``) for the training step to weigh into its loss.
 """
 from __future__ import annotations
 
+import math
 from typing import Dict, Iterable, List, Optional
 
 import torch
 from torch import nn
 
-from ...ops.reference import DropoutSpec
+from ...ops.reference import DropoutSpec, activation_penalties
 from .lstm import LSTMLayer
 
 EXPORT_KEYS = ("wf", "wi", "wo", "wc", "bf", "bi", "bc", "bo")
@@ -28,12 +31,16 @@ EXPORT_KEYS = ("wf", "wi", "wo", "wc", "bf", "bi", "bc", "bo")
 
 class RNN(nn.Module):
     def __init__(self, settings: Iterable[dict], dropout: float = 0.0, weight_drop: float = 0.0, output_dropout: float = 0.0,
-                 input_dropout: float = 0.0, embedding_dropout: float = 0.0, locked: bool = False, **layer_kw):
+                 input_dropout: float = 0.0, embedding_dropout: float = 0.0, locked: bool = False, activation_reg: float = 0.0,
+                 temporal_activation_reg: float = 0.0, **layer_kw):
         super().__init__()
         for name, p in (("dropout", dropout), ("weight_drop", weight_drop), ("output_dropout", output_dropout),
                         ("input_dropout", input_dropout), ("embedding_dropout", embedding_dropout)):
             if not 0.0 <= p < 1.0:
                 raise ValueError(f"{name} must satisfy 0 <= P < 1, got {p}")
+        for name, c in (("activation_reg", activation_reg), ("temporal_activation_reg", temporal_activation_reg)):
+            if not (math.isfinite(c) and c >= 0):
+                raise ValueError(f"{name} must be a finite number >= 0, got {c}")
         self.layers = nn.ModuleList()
         self.reverse_layers = nn.ModuleList()      # empty, or one reverse-time layer per entry of ``layers``
         self._layer_kw = layer_kw
@@ -43,6 +50,9 @@ class RNN(nn.Module):
         self.input_dropout = float(input_dropout)
         self.embedding_dropout = float(embedding_dropout)
         self.locked = bool(locked)
+        self.activation_reg = float(activation_reg)
+        self.temporal_activation_reg = float(temporal_activation_reg)
+        self.activation_penalties: Optional[torch.Tensor] = None      # [2] (AR, TAR) of the last training forward pass, or None
         # the mask's key (seed, partition) and step counter (training steps completed: an int32 [1] device tensor on the GPU,
         # an int on the CPU); a TrainEngine sets and advances them
         self.dropout_key = (0, 0)
@@ -70,6 +80,11 @@ class RNN(nn.Module):
         if not self.training or self.embedding_dropout == 0:
             return None
         return DropoutSpec(self.embedding_dropout, self.dropout_key, 0, False, self.dropout_step, site="rows")
+
+    @property
+    def wants_activation_sums(self) -> bool:
+        """Does this forward pass compute AR / TAR (training mode, a coefficient above 0)?"""
+        return self.training and (self.activation_reg > 0 or self.temporal_activation_reg > 0)
 
     @property
     def draws_masks(self) -> bool:
@@ -123,6 +138,9 @@ class RNN(nn.Module):
 
     # --------------------------------------------------------------------------------------------
     def reset_state(self, batch_size: Optional[int] = None):
+        # the last pass's penalties hold its autograd graph, and with it the parameters' gradient accumulators: let them go before
+        # the next pass builds its own (a captured step must not reuse accumulators created on another stream)
+        self.activation_penalties = None
         for layer in self.directions():
             layer.reset_state(batch_size)
 
@@ -177,14 +195,26 @@ class RNN(nn.Module):
         wavefront with both recurrences co-resident, or, where they do not fit side by side, the recurrences one after the other
         with the upper layer's GEMMs next to them), single layers otherwise.  Bidirectional: both
         directions of a layer run one after the other on the same input, and their outputs are joined into ``[T,B,2H]``
-        (one concatenation) for the next layer; no wavefront."""
+        (one concatenation) for the next layer; no wavefront.
+        ``wants_activation_sums``: the top layer's op (both directions, or the pair whose upper layer is the top one) also
+        returns its sums; their total, over the output's width, gives ``activation_penalties``."""
         from ...ops import functional as F
+        T, B = seq.shape[0], seq.shape[1]
+        n = len(self.layers)
+        want = self.wants_activation_sums
+        self.activation_penalties = None
+        parts = []
         if self.bidirectional:
             for i, (la, lr) in enumerate(zip(self.layers, self.reverse_layers)):
-                seq = torch.cat([la.fit_sequence(seq, lengths, self.dropout_spec(i), self.weight_drop_spec(i)),
-                                 lr.fit_sequence(seq, lengths, self.dropout_spec(i, True), self.weight_drop_spec(i, True))], 2)
-            return seq
-        i, n = 0, len(self.layers)
+                act = want and i == n - 1
+                outs = [l.fit_sequence(seq, lengths, self.dropout_spec(i, r), self.weight_drop_spec(i, r), activation_sums=act)
+                        for l, r in ((la, False), (lr, True))]
+                if act:
+                    parts = [o[1] for o in outs]
+                    outs = [o[0] for o in outs]
+                seq = torch.cat(outs, 2)
+            return self._penalties(seq, parts, T, B, lengths)
+        i = 0
         while i < n:
             la = self.layers[i]
             if i + 1 < n and F.lstm_pair_supported(seq, la.num_hidden, self.layers[i + 1].num_hidden):
@@ -193,17 +223,31 @@ class RNN(nn.Module):
                 for l in (la, lb):
                     if B != l.ht.shape[0]:
                         l.reset_state(B)
-                seq, hT_a, cT_a, hT_b, cT_b = F.lstm_pair_sequence(seq, (la.ht, la.Ct, la.w_x, la.w_h, la.bias),
-                                                                     (lb.ht, lb.Ct, lb.w_x, lb.w_h, lb.bias), lengths=lengths,
-                                                                     dropouts=(self.dropout_spec(i), self.dropout_spec(i + 1)),
-                                                                     weight_drops=(self.weight_drop_spec(i),
-                                                                                   self.weight_drop_spec(i + 1)))
+                act = want and i + 1 == n - 1
+                outs = F.lstm_pair_sequence(seq, (la.ht, la.Ct, la.w_x, la.w_h, la.bias), (lb.ht, lb.Ct, lb.w_x, lb.w_h, lb.bias),
+                                            lengths=lengths, dropouts=(self.dropout_spec(i), self.dropout_spec(i + 1)),
+                                            weight_drops=(self.weight_drop_spec(i), self.weight_drop_spec(i + 1)),
+                                            activation_sums=act)
+                seq, hT_a, cT_a, hT_b, cT_b = outs[:5]
+                if act:
+                    parts = [outs[5]]
                 la._set_state(hT_a, cT_a); la.state.append((hT_a, cT_a))
                 lb._set_state(hT_b, cT_b); lb.state.append((hT_b, cT_b))
                 i += 2
             else:
-                seq = la.fit_sequence(seq, lengths, self.dropout_spec(i), self.weight_drop_spec(i))
+                act = want and i == n - 1
+                seq = la.fit_sequence(seq, lengths, self.dropout_spec(i), self.weight_drop_spec(i), activation_sums=act)
+                if act:
+                    seq, sums = seq
+                    parts = [sums]
                 i += 1
+        return self._penalties(seq, parts, T, B, lengths)
+
+    def _penalties(self, seq: torch.Tensor, parts: list, T: int, B: int, lengths) -> torch.Tensor:
+        """Sets ``activation_penalties`` from the top op's sums ``parts`` (none: left None) -> ``seq``."""
+        if parts:
+            sums = parts[0] if len(parts) == 1 else parts[0] + parts[1]
+            self.activation_penalties = activation_penalties(sums, seq.shape[2], T, B, lengths)
         return seq
 
     # --------------------------------------------------------------------------------------------

@@ -14,8 +14,8 @@ _ERR = None
 LAUNCHES = {"n": 0}          # number of OUR kernels launched through the extension (bench.py "gpu_launches")
 # which paths the ops took (also read as ``cuda_lstm.STATS``): fixed keys are incremented in place, the others through ``count``
 STATS = {"fast_fwd": 0, "fast_bwd": 0, "generic_fwd": 0, "generic_bwd": 0, "tc_gemm": 0, "kernels": 0, "weight_drop": 0,
-         "weight_drop_grad": 0, "embed_fwd_dropout": 0, "embed_bwd_dropout": 0}
-_NO_KERNEL = {"ar_max_blocks", "ar_flag_words", "ar_slots"}
+         "weight_drop_grad": 0, "embed_fwd_dropout": 0, "embed_bwd_dropout": 0, "act_reg_fwd": 0, "act_reg_bwd": 0}
+_NO_KERNEL = {"ar_max_blocks", "ar_flag_words", "ar_slots", "act_reg_scratch"}
 
 
 def count(key: str, n: int = 1) -> None:

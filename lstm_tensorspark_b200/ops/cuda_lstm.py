@@ -288,9 +288,36 @@ def dropout(x: torch.Tensor, spec, t0: int = 0) -> torch.Tensor:
     return _DropoutFn.apply(x, spec, t0)
 
 
+_ACT_SCRATCH = {}
+
+
+def _activation_sums(out: Optional[torch.Tensor], h: torch.Tensor, lengths) -> torch.Tensor:
+    """fp32 ``[2]`` = (sum out^2, sum (h_t - h_{t-1})^2) over the counted positions of the top layer's output (csrc/activation_reg.cu):
+    ``h`` the raw output ``[T,B,H]`` in time order, ``out`` the dropped one the head reads (None: ``h`` itself)."""
+    T, B, H = h.shape
+    n = ext().act_reg_scratch(T, B, H, h.dtype == torch.bfloat16)
+    key = (h.device.index, n)
+    if key not in _ACT_SCRATCH:          # one buffer per size, never freed: a captured graph keeps its address
+        _ACT_SCRATCH[key] = torch.zeros(n, dtype=torch.float64, device=h.device)   # (every launch leaves its ticket 0)
+    STATS["act_reg_fwd"] += 1
+    STATS["kernels"] += 1
+    return ext().act_reg_fwd(out, h, lengths, _ACT_SCRATCH[key])
+
+
+def _activation_grad(dh: Optional[torch.Tensor], out: Optional[torch.Tensor], h: torch.Tensor, lengths, g: torch.Tensor,
+                     drop: dict) -> torch.Tensor:
+    """The gradient into the top layer's raw output ``h``: the head's ``dh`` (w.r.t. ``out``, None: zero) and that of the two sums
+    (``g = d loss / d sums``), with the output dropout's mask ``drop`` (``_drop_args``) applied, in one pass; the recurrence's
+    backward then reads it unmasked."""
+    STATS["act_reg_bwd"] += 1
+    STATS["kernels"] += 1
+    return ext().act_reg_bwd(dh, out, h, lengths, g.float().contiguous(), **drop)
+
+
 class _LSTMSeqFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x_seq, h0, c0, w_x, w_h, bias, lengths=None, reverse=False, dropout=None, weight_drop=None, chunks=None):
+    def forward(ctx, x_seq, h0, c0, w_x, w_h, bias, lengths=None, reverse=False, dropout=None, weight_drop=None, chunks=None,
+                act_sums=False):
         E = ext()
         T, B, D = x_seq.shape
         H = w_h.shape[1]
@@ -340,7 +367,9 @@ class _LSTMSeqFn(torch.autograd.Function):
                 h_drop = E.dropout(h_seq[:T] if reverse else h_seq[1:], drop["drop_step"], drop["drop_desc"], 0)
                 STATS["kernels"] += 1
         ctx.drop = drop
-        ctx.save_for_backward(x2d, h_seq, c_seq, act, w_x_c, w_h_c)
+        h_out = h_seq[:T] if reverse else h_seq[1:]
+        ctx.act_sums = act_sums
+        ctx.save_for_backward(x2d, h_seq, c_seq, act, w_x_c, w_h_c, h_drop if act_sums else None)
         ctx.set_materialize_grads(False)       # an unused output must arrive as None, not as a zero-filled [T,B,H] tensor
         ctx.fast = fast
         ctx.lengths = lengths
@@ -351,20 +380,27 @@ class _LSTMSeqFn(torch.autograd.Function):
         ctx.in_dtypes = (h0.dtype, c0.dtype)
         # h_T is its own output (not a slice of the first one taken by the caller): a consumer of the final state only - the
         # classifier on top of the stack - then sends back a [B,H] gradient instead of a zero-filled [T,B,H] one
-        if reverse:
-            return (h_seq[:T] if h_drop is None else h_drop), h_seq[0], c_seq[0]
-        return (h_seq[1:] if h_drop is None else h_drop), h_seq[T], c_seq[T]
+        outs = (h_out if h_drop is None else h_drop), h_seq[0 if reverse else T], c_seq[0 if reverse else T]
+        if act_sums:                           # AR / TAR: the sums over this op's rows and positions, one more output
+            return outs + (_activation_sums(h_drop, h_out, lengths),)
+        return outs
 
     @staticmethod
-    def backward(ctx, dh_seq, dh_T, dc_T):
+    def backward(ctx, dh_seq, dh_T, dc_T, d_sums=None):
         E = ext()
-        x2d, h_seq, c_seq, act, w_x_c, w_h_c = ctx.saved_tensors
+        x2d, h_seq, c_seq, act, w_x_c, w_h_c, h_drop = ctx.saved_tensors
         T, B, D, H = ctx.dims
         cd = act.dtype
         dev = act.device
         drop = ctx.drop if dh_seq is not None else {}          # (the mask only matters where a gradient arrives)
         if dh_seq is not None:
             dh_seq = dh_seq.to(cd).contiguous()
+        if ctx.act_sums and d_sums is not None:
+            # the sums' gradient joins the head's and the output dropout's mask is applied to both in one pass: the recurrence
+            # below (and the generic path) then reads dh_seq unmasked
+            dh_seq = _activation_grad(dh_seq, h_drop, h_seq[:T] if ctx.reverse else h_seq[1:], ctx.lengths, d_sums, ctx.drop)
+            drop = {}
+        if dh_seq is not None:
             if drop and not ctx.fast:
                 dh_seq = E.dropout(dh_seq, drop["drop_step"], drop["drop_desc"], 0)
                 STATS["kernels"] += 1
@@ -413,17 +449,21 @@ class _LSTMSeqFn(torch.autograd.Function):
             STATS["kernels"] += 1
             rel(a[0])
         h0_dt, c0_dt = ctx.in_dtypes
-        return dx, dh0.to(h0_dt), dc0.to(c0_dt), dw_x, dw_h, db, None, None, None, None, None
+        return dx, dh0.to(h0_dt), dc0.to(c0_dt), dw_x, dw_h, db, None, None, None, None, None, None
 
 
-def lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths=None, reverse=False, dropout=None, weight_drop=None):
+def lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths=None, reverse=False, dropout=None, weight_drop=None,
+                        activation_sums=False):
     """``x_seq [T,B,D]`` (bf16 or fp32) -> ``(h_seq [T,B,H], h_T, c_T)``.  ``lengths``: optional int32 ``[B]`` on the batch's
     device, right padding (``ops/reference.py``); the persistent kernels then run their masked instantiations.  ``reverse``:
     the reverse-time direction (time T-1 down to 0; ``h_T`` / ``c_T`` are then the state after time 0).  ``dropout``: a
     ``reference.DropoutSpec``; the first output is then the dropped sequence (the persistent kernels store it next to h_seq
     and mask the incoming gradient as they load it; other shapes run the standalone dropout kernel).  ``weight_drop``: a weight-drop
     ``reference.DropoutSpec``: the kernels read the masked image ``W_h * M * s`` in place of ``W_h`` and the weight gradient is
-    masked on its way into the sink (one mask for every batch chunk)."""
+    masked on its way into the sink (one mask for every batch chunk).  ``activation_sums``: one more output, fp32 ``[2]`` =
+    (sum out^2, sum (h_t - h_{t-1})^2) over the counted positions, ``out`` the first output and ``h`` the undropped one
+    (``reference.activation_sums``; csrc/activation_reg.cu); its gradient is combined with the first output's by one more kernel
+    ahead of the backward recurrence."""
     if (not x_seq.is_contiguous() and not x_seq.requires_grad and x_seq.transpose(0, 1).is_contiguous()
             and (x_seq.shape[2] * x_seq.element_size()) % 16 == 0):
         x_seq = ext().transpose01(x_seq.transpose(0, 1))     # batch-major feed -> time-major, a row permutation at copy speed
@@ -439,12 +479,18 @@ def lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths=None, reverse=Fal
         chunks = Countdown((B + chunk - 1) // chunk)
         outs = [_LSTMSeqFn.apply(x_seq[:, b0:b0 + chunk].contiguous(), h0[b0:b0 + chunk], c0[b0:b0 + chunk], w_x, w_h, bias,
                                  None if lengths is None else lengths[b0:b0 + chunk], reverse,
-                                 None if dropout is None else dropout.at_rows(b0), weight_drop, chunks)
+                                 None if dropout is None else dropout.at_rows(b0), weight_drop, chunks, activation_sums)
                 for b0 in range(0, B, chunk)]
         count("batch_chunks", len(outs))
-        return (torch.cat([o[0] for o in outs], dim=1), torch.cat([o[1] for o in outs], dim=0),
-                torch.cat([o[2] for o in outs], dim=0))
-    return _LSTMSeqFn.apply(x_seq.contiguous(), h0, c0, w_x, w_h, bias, lengths, reverse, dropout, weight_drop)
+        cat = (torch.cat([o[0] for o in outs], dim=1), torch.cat([o[1] for o in outs], dim=0),
+               torch.cat([o[2] for o in outs], dim=0))
+        if activation_sums:                  # unnormalised: the chunks' parts add up, in chunk order
+            sums = outs[0][3]
+            for o in outs[1:]:
+                sums = sums + o[3]
+            cat = cat + (sums,)
+        return cat
+    return _LSTMSeqFn.apply(x_seq.contiguous(), h0, c0, w_x, w_h, bias, lengths, reverse, dropout, weight_drop, None, activation_sums)
 
 
 # =====================================================================================================================
@@ -577,7 +623,7 @@ def _gate_cfg(var: int, tiles_m: int, nkb: int, per_kb_step: int, ctas_per_tile:
 class _LSTMPairFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x_seq, h0a, c0a, w_xa, w_ha, b_a, h0b, c0b, w_xb, w_hb, b_b, lengths=None, schedule="wavefront", drop_a=None,
-                drop_b=None, wdrop_a=None, wdrop_b=None):
+                drop_b=None, wdrop_a=None, wdrop_b=None, act_sums=False):
         E = ext()
         pipelined = schedule == "pipelined"
         dev = x_seq.device
@@ -661,8 +707,10 @@ class _LSTMPairFn(torch.autograd.Function):
         STATS["fast_fwd"] += 2
         STATS["kernels"] += 3
         count(schedule + "_fwd")
-        ctx.save_for_backward(x2d, h_seq_a, c_seq_a, act_a, h_seq_b, c_seq_b, act_b, wxa, wha, wxb, whb, hin_b)
+        ctx.save_for_backward(x2d, h_seq_a, c_seq_a, act_a, h_seq_b, c_seq_b, act_b, wxa, wha, wxb, whb, hin_b,
+                              h_drop_b if act_sums else None)
         ctx.set_materialize_grads(False)
+        ctx.act_sums = act_sums
         ctx.drop = (dra, drb)
         ctx.dims = (T, B, D, Ha, Hb)
         ctx.lengths = lengths
@@ -670,12 +718,15 @@ class _LSTMPairFn(torch.autograd.Function):
         ctx.x_folded = x_bm is not None
         ctx.addrs = (w_xa.data_ptr(), w_ha.data_ptr(), b_a.data_ptr(), w_xb.data_ptr(), w_hb.data_ptr(), b_b.data_ptr())
         ctx.in_dtypes = (h0a.dtype, c0a.dtype, h0b.dtype, c0b.dtype)
-        return (h_seq_b[1:] if h_drop_b is None else h_drop_b), h_seq_a[T], c_seq_a[T], h_seq_b[T], c_seq_b[T]
+        outs = (h_seq_b[1:] if h_drop_b is None else h_drop_b), h_seq_a[T], c_seq_a[T], h_seq_b[T], c_seq_b[T]
+        if act_sums:                          # AR / TAR of layer b, the top layer (an ordinary launch: L_b has finished)
+            return outs + (_activation_sums(h_drop_b, h_seq_b[1:], lengths),)
+        return outs
 
     @staticmethod
-    def backward(ctx, dh_seq_b, dhT_a, dcT_a, dhT_b, dcT_b):
+    def backward(ctx, dh_seq_b, dhT_a, dcT_a, dhT_b, dcT_b, d_sums=None):
         E = ext()
-        x2d, h_seq_a, c_seq_a, act_a, h_seq_b, c_seq_b, act_b, wxa, wha, wxb, whb, hin_b = ctx.saved_tensors
+        x2d, h_seq_a, c_seq_a, act_a, h_seq_b, c_seq_b, act_b, wxa, wha, wxb, whb, hin_b, h_drop_b = ctx.saved_tensors
         dra, drb = ctx.drop
         wda, wdb = ctx.wdrop
         if dh_seq_b is None:
@@ -684,6 +735,10 @@ class _LSTMPairFn(torch.autograd.Function):
         cd, dev = act_a.dtype, act_a.device
         if dh_seq_b is not None:
             dh_seq_b = dh_seq_b.to(cd).contiguous()
+        if ctx.act_sums and d_sums is not None:
+            # the sums' gradient joins the head's, masked by layer b's output dropout in the same pass: L_b reads it unmasked
+            dh_seq_b = _activation_grad(dh_seq_b, h_drop_b, h_seq_b[1:], ctx.lengths, d_sums, ctx.drop[1])
+            drb = {}
         f32 = dict(dtype=torch.float32, device=dev)
         z = lambda g, H: g.float().contiguous().clone() if g is not None else torch.zeros(B, H, **f32)
         dh0a, dc0a, dh0b, dc0b = z(dhT_a, Ha), z(dcT_a, Ha), z(dhT_b, Hb), z(dcT_b, Hb)
@@ -767,16 +822,18 @@ class _LSTMPairFn(torch.autograd.Function):
             release(a[0])
         t = ctx.in_dtypes
         return (dx, dh0a.to(t[0]), dc0a.to(t[1]), dw_xa, dw_ha, db_a, dh0b.to(t[2]), dc0b.to(t[3]), dw_xb, dw_hb, db_b, None, None,
-                None, None, None, None)
+                None, None, None, None, None)
 
 
-def lstm_pair_sequence(x_seq, la, lb, lengths=None, schedule=None, dropouts=(None, None), weight_drops=(None, None)):
+def lstm_pair_sequence(x_seq, la, lb, lengths=None, schedule=None, dropouts=(None, None), weight_drops=(None, None),
+                       activation_sums=False):
     """Two stacked layers as one op.  ``la`` / ``lb`` = (h0, c0, w_x, w_h, bias).  -> (h_seq_b, hT_a, cT_a, hT_b, cT_b).
     ``lengths``: optional int32 ``[B]`` per-row lengths (both layers run their masked kernels; the gated GEMM is unchanged).
     ``schedule``: "wavefront" or "pipelined" (see ``pair_schedule``); None = the one ``pair_schedule`` picks for the device.
     ``dropouts``: ``reference.DropoutSpec`` (or None) of layer a's output (the input of layer b) and of layer b's output (the
     first result).  ``weight_drops``: weight-drop ``reference.DropoutSpec`` (or None) of layer a's and layer b's ``W_h``: the
-    recurrences read the masked images, and each ``dW_h`` is masked on its way into the sink."""
+    recurrences read the masked images, and each ``dW_h`` is masked on its way into the sink.  ``activation_sums``: one more
+    output, layer b's sums of ``lstm_layer_sequence``."""
     _check_lengths_arg(lengths, x_seq.shape[1], x_seq.device)
     if schedule is None:
         schedule = _pair_schedule_of(x_seq, la[3].shape[1], lb[3].shape[1])
@@ -786,7 +843,8 @@ def lstm_pair_sequence(x_seq, la, lb, lengths=None, schedule=None, dropouts=(Non
     if (not x_seq.is_contiguous() and not x_seq.requires_grad and x_seq.transpose(0, 1).is_contiguous()
             and (x_seq.shape[2] * x_seq.element_size()) % 16 == 0):
         if FOLDED_FEED and G.folded_ok(x_seq.transpose(0, 1)):
-            return _LSTMPairFn.apply(x_seq, *la, *lb, lengths, schedule, *dropouts, *weight_drops)  # read in place (see forward)
+            return _LSTMPairFn.apply(x_seq, *la, *lb, lengths, schedule, *dropouts, *weight_drops,   # read in place (see forward)
+                                     activation_sums)
         x_seq = ext().transpose01(x_seq.transpose(0, 1))
         STATS["kernels"] += 1
-    return _LSTMPairFn.apply(x_seq.contiguous(), *la, *lb, lengths, schedule, *dropouts, *weight_drops)
+    return _LSTMPairFn.apply(x_seq.contiguous(), *la, *lb, lengths, schedule, *dropouts, *weight_drops, activation_sums)

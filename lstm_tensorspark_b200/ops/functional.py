@@ -46,17 +46,19 @@ def lstm_cell_step(x, h, c, w_x, w_h, bias, weight_drop=None):
     return ref.lstm_cell_step(x, h, c, w_x, ref.weight_drop(w_h, weight_drop), bias)
 
 
-def lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths=None, reverse=False, dropout=None, weight_drop=None):
+def lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths=None, reverse=False, dropout=None, weight_drop=None,
+                        activation_sums=False):
     """``lengths``: optional int32 ``[B]`` per-row sequence lengths (right padding, see ``reference.lstm_layer_sequence``).
     ``reverse``: the reverse-time direction of a bidirectional layer (same reference).  ``dropout``: optional
     ``reference.DropoutSpec``: the first output is then the dropped sequence.  ``weight_drop``: optional weight-drop
-    ``reference.DropoutSpec``: every step reads ``W_h * M * s`` and ``W_h`` gets the masked gradient."""
+    ``reference.DropoutSpec``: every step reads ``W_h * M * s`` and ``W_h`` gets the masked gradient.  ``activation_sums``: one
+    more output, the unnormalised AR / TAR sums ``[2]`` of the layer's output (``reference.activation_sums``)."""
     if _use_ext(x_seq):
         from . import cuda_lstm
         return cuda_lstm.lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths=lengths, reverse=reverse, dropout=dropout,
-                                             weight_drop=weight_drop)
+                                             weight_drop=weight_drop, activation_sums=activation_sums)
     return ref.lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths=lengths, reverse=reverse, dropout=dropout,
-                                   weight_drop=weight_drop)
+                                   weight_drop=weight_drop, activation_sums=activation_sums)
 
 
 def dropout(x, spec, t0: int = 0):
@@ -191,6 +193,8 @@ def lstm_pair_supported(x_seq, h_a: int, h_b: int) -> bool:
     return cuda_lstm.wavefront_supported(x_seq, h_a, h_b)
 
 
-def lstm_pair_sequence(x_seq, la, lb, lengths=None, dropouts=(None, None), weight_drops=(None, None)):
+def lstm_pair_sequence(x_seq, la, lb, lengths=None, dropouts=(None, None), weight_drops=(None, None), activation_sums=False):
+    """``activation_sums``: one more output, layer b's AR / TAR sums (``lstm_layer_sequence``)."""
     from . import cuda_lstm
-    return cuda_lstm.lstm_pair_sequence(x_seq, la, lb, lengths=lengths, dropouts=dropouts, weight_drops=weight_drops)
+    return cuda_lstm.lstm_pair_sequence(x_seq, la, lb, lengths=lengths, dropouts=dropouts, weight_drops=weight_drops,
+                                        activation_sums=activation_sums)

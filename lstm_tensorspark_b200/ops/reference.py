@@ -198,7 +198,7 @@ def weight_drop(w_h: torch.Tensor, spec: Optional[DropoutSpec]) -> torch.Tensor:
 
 
 def lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths: Optional[torch.Tensor] = None, reverse: bool = False,
-                        dropout: Optional[DropoutSpec] = None, weight_drop: Optional[DropoutSpec] = None):
+                        dropout: Optional[DropoutSpec] = None, weight_drop: Optional[DropoutSpec] = None, activation_sums: bool = False):
     """Unrolled layer: ``x_seq [T,B,D]`` -> ``(h_seq [T,B,H], h_T, c_T)``.
 
     ``lengths`` (int32 ``[B]``, right padding): at a step ``t >= lengths[b]`` row ``b`` holds its state (``h_t = h_{t-1}``,
@@ -214,7 +214,9 @@ def lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths: Optional[torch.T
     not dropped.
 
     ``weight_drop``: a ``weight`` ``DropoutSpec``; every step and row reads ``weight_drop(w_h, spec)`` in place of ``w_h``, built
-    inside autograd, so ``w_h`` gets the masked gradient."""
+    inside autograd, so ``w_h`` gets the masked gradient.
+
+    ``activation_sums``: a fourth output, ``activation_sums(first output, undropped h_seq, lengths)``."""
     T = x_seq.shape[0]
     w_h = _weight_drop(w_h, weight_drop)
     keep = None
@@ -238,7 +240,42 @@ def lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths: Optional[torch.T
         outs.append(h)
     if reverse:
         outs.reverse()
-    return _dropout(torch.stack(outs, 0), dropout), h, c
+    raw = torch.stack(outs, 0)
+    out = _dropout(raw, dropout)
+    if activation_sums:
+        return out, h, c, _activation_sums(out, raw, lengths)
+    return out, h, c
+
+
+def activation_sums(out: torch.Tensor, h: torch.Tensor, lengths: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """AWD-LSTM's activation regularisation, unnormalised: ``[2]`` = (sum of ``out[t,b,j]^2`` over the counted positions
+    ``t < len_b``, sum of ``(h[t,b,j] - h[t-1,b,j])^2`` over ``1 <= t < len_b``).  ``out`` is the top layer's output as the head
+    reads it (after ``--output_dropout``), ``h`` the raw output in time order, both ``[T,B,W]``; ``len_b = T`` without
+    ``lengths``.  AR = sums[0] / (W sum_b len_b), TAR = sums[1] / (W sum_b max(len_b - 1, 0)): ``activation_penalties``.  fp32
+    (fp64 for fp64 inputs), through autograd."""
+    T, B, _ = h.shape
+    dt = torch.float64 if h.dtype == torch.float64 else torch.float32
+    keep = step_mask(lengths, B, T, device=h.device).t().unsqueeze(2)                       # [T,B,1]
+    zero = torch.zeros((), dtype=dt, device=h.device)
+    ar = torch.where(keep, out.to(dt), zero).square().sum()
+    d = h[1:].to(dt) - h[:-1].to(dt)
+    tar = torch.where(keep[1:], d, zero).square().sum()
+    return torch.stack([ar, tar])
+
+
+_activation_sums = activation_sums
+
+
+def activation_penalties(sums: torch.Tensor, width: int, T: int, B: int, lengths: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """``[2]`` = (AR, TAR) from the summed ``activation_sums`` of an output ``width`` units wide: each sum over its count of terms,
+    ``N_ar = width * sum_b len_b`` and ``N_tar = width * sum_b max(len_b - 1, 0)`` (``len_b = T`` without ``lengths``), and 0 where
+    that count is 0.  Computed on the sums' device from ``lengths`` without reading it on the host."""
+    if lengths is None:                       # (host numbers: no copy to the device, which a captured graph could not hold)
+        return torch.stack([sums[i] / n if n > 0 else torch.zeros_like(sums[i]) for i, n in enumerate((width * B * T,
+                                                                                                     width * B * (T - 1)))])
+    lg = lengths.to(sums.device).long()
+    n = torch.stack([lg.sum(), (lg - 1).clamp(min=0).sum()]).to(sums.dtype) * width
+    return torch.where(n > 0, sums / n.clamp(min=1), torch.zeros((), dtype=sums.dtype, device=sums.device))
 
 
 _dropout = dropout          # (lstm_layer_sequence's arguments shadow these functions)

@@ -225,6 +225,8 @@ def train_rnn(partition, cfg: Config, rank: int = 0, world_size: int = 1, comm: 
         if is_eval:
             t_loss = float(loss.detach().float().item())
             g_norm = float(eng.grad_norm().item()) if cfg.clip_grad_norm > 0 else None
+            ar_tar = eng.activation_penalties()
+            ar_tar = None if ar_tar is None else [float(v) for v in ar_tar.tolist()]
         elif use_bar:
             t_loss = bar_loss.push(loss)         # CUDA: the previous step's loss, read back asynchronously (no host sync)
         if use_bar:
@@ -252,6 +254,10 @@ def train_rnn(partition, cfg: Config, rank: int = 0, world_size: int = 1, comm: 
                 if g_norm is not None:                               # the pre-clip norm of this step's gradient
                     sink.add("grad_norm", g_norm)
                     extra["grad_norm"] = g_norm
+                if ar_tar is not None:                               # this step's unweighted AR and TAR
+                    for k, v in zip(("ar", "tar"), ar_tar):
+                        sink.add(k, v)
+                        extra[k] = v
                 if cfg.next_token:
                     extra["perplexity"] = math.exp(t_loss)
                     sink.add("perplexity", extra["perplexity"])
