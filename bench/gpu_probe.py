@@ -448,8 +448,21 @@ def check_tiles2_tune():
     for v, nm in ((0, "ksplit_default"), (524288, "nosplit")):
         ms = _time_ms(lambda: E.lstm_seq_fwd(gx, whb, bias, h0, c0, ws, v), iters=5, warm=2)
         _emit("tiles1_fwd", variant=nm, us_per_step=ms * 1e3 / T)
-    ms = _time_ms(lambda: E.lstm_seq_bwd(dh, whT, act, cseq, z, z, ws, 0), iters=5, warm=2)
-    _emit("tiles1_bwd", us_per_step=ms * 1e3 / (T + 1))
+    # the backward at one tile per CTA on 128 CTAs without a cluster (K-split reduce-scattered through L2, kXchgL2), by ring
+    # depth (0 = the default), alternating with the two-tile clustered kernel the headline runs, in three rounds
+    xchg = cuda_lstm._xchg_buffer(B, H, dev)
+    for rnd in range(3):
+        for st in (0, 4, 5, 6):
+            ms = _time_ms(lambda: E.lstm_seq_bwd(dh, whT, act, cseq, z, z, ws, 16 * st, xchg=xchg), iters=5, warm=2)
+            cuda_lstm.check_kernel_errors(dev)
+            _emit("tiles1_l2_bwd", round=rnd, stages=st or E.lstm_seq_config(True, H, B, 0, True)[0], us_per_step=ms * 1e3 / (T + 1))
+        ms = _time_ms(lambda: E.lstm_seq_bwd(dh, whT, act, cseq, z, z, ws, 2), iters=5, warm=2)
+        _emit("tiles2_bwd", round=rnd, stages=E.lstm_seq_config(True, H, B, 2)[0], sync=0, us_per_step=ms * 1e3 / (T + 1))
+    try:                                              # clusters of 4: 128 CTAs are not co-resident on a 132-SM H100
+        ms = _time_ms(lambda: E.lstm_seq_bwd(dh, whT, act, cseq, z, z, ws, 0), iters=5, warm=2)
+        _emit("tiles1_bwd", us_per_step=ms * 1e3 / (T + 1))
+    except RuntimeError as e:
+        _emit("tiles1_bwd", error=repr(e)[:200])
 
 
 def check_tiles2_phase():
@@ -475,8 +488,12 @@ def check_tiles2_phase():
     _, cseq, act = E.lstm_seq_fwd(gx, whb, bias, h0, c0, ws, 2)
     dh = (torch.randn(T, B, H, device=dev) * 0.1).bfloat16()
     z = torch.zeros(B, H, device=dev)
+    xchg = cuda_lstm._xchg_buffer(B, H, dev)
     runs = {"fwd": lambda v, dbg=None: E.lstm_seq_fwd(gx, whb, bias, h0, c0, ws, v, dbg),
-            "bwd": lambda v, dbg=None: E.lstm_seq_bwd(dh, whT, act, cseq, z, z, ws, v, dbg)}
+            "bwd": lambda v, dbg=None: E.lstm_seq_bwd(dh, whT, act, cseq, z, z, ws, v, dbg),
+            # one tile per CTA, L2 exchange (128 CTAs): stamp 3 = the group's exchange counter seen, so accumulator ready ->
+            # stamp 3 is the partial's store, release and wait
+            "bwd_l2": lambda v, dbg=None: E.lstm_seq_bwd(dh, whT, act, cseq, z, z, ws, v & ~15, dbg, xchg=xchg)}
     for direction, run in runs.items():
         steps = T if direction == "fwd" else T + 1
         first = 8 if direction == "fwd" else 9              # skip the first steps (the backward pass stamps from s = 1)
@@ -495,6 +512,11 @@ def check_tiles2_phase():
 
                 def us(x):
                     return float(x.double().mean()) / 1e3
+                if direction == "bwd_l2":
+                    _emit("tiles2_phase", direction=direction, debug_mode=mode, us_per_step=ms * 1e3 / steps,
+                          load_mma_us=us(accum - waited), epi_us=us(sig - accum), sync_us=us(waited[1:] - sig[:-1]),
+                          xchg_us=us(d[:, 3] - accum), xchg_to_signal_us=us(sig - d[:, 3]))
+                    continue
                 overlap = (torch.minimum(d1[:, 1], d[:, 2]) - torch.maximum(d1[:, 3], d[:, 1])).clamp(min=0)
                 _emit("tiles2_phase", direction=direction, debug_mode=mode, us_per_step=ms * 1e3 / steps,
                       load_mma_us=us(accum - waited), epi_us=us(sig - accum), sync_us=us(waited[1:] - sig[:-1]),

@@ -20,7 +20,7 @@ int ts_lstm_pointwise_fwd(const void*, const float*, const float*, void*, float*
                           const int*, int);
 int ts_transpose01_rows(const void*, void*, int, int, long long, cudaStream_t);
 int ts_lstm_seq_cluster_probe(int);
-int ts_lstm_seq_config(int, int, int, int, int*);
+int ts_lstm_seq_config(int, int, int, int, int*, int);
 int ts_transpose2d_b16(const void*, void*, int, int, cudaStream_t);
 int ts_colsum_bf16(const void*, float*, void*, int, int, int, int, int, int, cudaStream_t);
 long long ts_colsum_scratch_bytes(int, int);
@@ -72,7 +72,7 @@ int ts_lstm_seq_fwd(const void*, const void*, const float*, const void*, const f
                     void*, const int*, const unsigned int*);
 int ts_lstm_seq_bwd(const void*, const void*, const void*, const float*, const void*, float*, float*, void*, void*, int,
                     int, int, unsigned int*, int, cudaStream_t, const unsigned int*, int, int, int, const int*, int,
-                    const int*, const unsigned int*);
+                    const int*, const unsigned int*, void*);
 int ts_dropout(const void*, void*, int, int, int, int, int, const int*, const unsigned int*, cudaStream_t);
 int ts_weight_drop_grad(const float*, float*, int, int, int, const int*, const unsigned int*, cudaStream_t);
 long long ts_act_reg_scratch(int, int, int, int);
@@ -859,7 +859,7 @@ Tensor gemm2(const Tensor& A, const Tensor& B, const std::optional<Tensor>& bias
              bool out_fp32, bool accumulate, int64_t ctas, int64_t bn, int64_t max_ctas, const std::optional<Tensor>& gate,
              const std::vector<int64_t>& gate_cfg, const std::optional<Tensor>& done, const std::optional<Tensor>& gate_err,
              int64_t stream_handle, bool pdl, int64_t a_fold, int64_t b_fold, int64_t fold_cols, const std::optional<Tensor>& rowsum,
-             bool rowsum_acc) {
+             bool rowsum_acc, bool reverse_m) {
   // a_fold / b_fold: the operand is the 2-D storage view [fold, T * fold_cols] of a batch-major [fold, T, fold_cols] array that
   // is read as the time-major matrix [T * fold, fold_cols] (A: K-major, K = fold_cols;  B: MN-major, N = fold_cols)
   TORCH_CHECK(A.is_cuda() && B.is_cuda(), "gemm2: CUDA tensors");
@@ -891,6 +891,7 @@ Tensor gemm2(const Tensor& A, const Tensor& B, const std::optional<Tensor>& bias
     gp = (const unsigned int*)gate->data_ptr<int>();
     for (int i = 0; i < 7; ++i) gcfg[i] = (int)gate_cfg[i];
   }
+  if (reverse_m) gcfg[6] = 1;           // walk the M tiles from the last to the first (also ungated)
   float* rp = nullptr;
   if (rowsum.has_value()) {
     TORCH_CHECK(rowsum->is_cuda() && rowsum->scalar_type() == torch::kFloat32 && rowsum->is_contiguous() && rowsum->numel() == M &&
@@ -968,6 +969,16 @@ std::vector<Tensor> lstm_seq_fwd(const Tensor& gx, const Tensor& w_h, const Tens
   return {h_seq, c_seq, act};
 }
 
+// xchg (backward): the exchange buffer of the one-tile kernel that reduce-scatters through L2 instead of a cluster's DSMEM,
+// >= 2 x tiles_m x H/16 x [128 x 64] bf16 (csrc/lstm_seq_wgmma.cu, kXchgL2); None = the clustered kernel.
+void* xchg_ptr(const std::optional<Tensor>& xchg, int B, int H, const Tensor& like) {
+  if (!xchg.has_value()) return nullptr;
+  chk_cuda(*xchg, "xchg");
+  TORCH_CHECK(xchg->scalar_type() == torch::kBFloat16 && xchg->is_contiguous() && xchg->device() == like.device() &&
+              xchg->numel() >= (int64_t)2 * ((B + 127) / 128) * (H / 16) * 128 * 64, "xchg: contiguous bf16 [2 x tiles_m x H/16 x 128 x 64]");
+  return xchg->data_ptr();
+}
+
 // dh_seq [T,B,H] bf16 (grad wrt every h_t from above; None when only h_T is used downstream), w_hT [H,4H] bf16 (transposed recurrent weights),
 // act/c_seq from forward, dhT fp32 [B,H] / dcT fp32 [B,H] extra grads into the final state (may be zeros)
 // -> dpre [T,B,4H] bf16, dh0 fp32 [B,H], dc0 fp32 [B,H]
@@ -975,7 +986,7 @@ std::vector<Tensor> lstm_seq_bwd(const std::optional<Tensor>& dh_seq, const Tens
                                  const Tensor& dhT, const Tensor& dcT, Tensor sync_ws, int64_t variant,
                                  std::optional<Tensor> dbg, std::optional<Tensor> in_gate, int64_t in_gate_tiles_n, bool extra_signal,
                                  const std::optional<Tensor>& lengths, bool reverse, const std::optional<Tensor>& drop_step,
-                                 const std::vector<int64_t>& drop_desc) {
+                                 const std::vector<int64_t>& drop_desc, const std::optional<Tensor>& xchg) {
   if (dh_seq.has_value()) chk_cuda(*dh_seq, "dh_seq");
   chk_cuda(w_hT, "w_hT"); chk_cuda(act, "act"); chk_cuda(c_seq, "c_seq");
   c10::cuda::CUDAGuard gd(act.device());
@@ -993,7 +1004,7 @@ std::vector<Tensor> lstm_seq_bwd(const std::optional<Tensor>& dh_seq, const Tens
                         dh0.data_ptr<float>(), dc0.data_ptr<float>(), dbg.has_value() ? dbg->data_ptr() : nullptr, tiled.data_ptr(), T, B, H,
                         (unsigned int*)sync_ws.data_ptr<int>(), (int)variant, stream(),
                         in_gate.has_value() ? (const unsigned int*)in_gate->data_ptr<int>() : nullptr, (int)in_gate_tiles_n,
-                        extra_signal ? 1 : 0, 0, lp, rev, ds, dd), "lstm_seq_bwd");
+                        extra_signal ? 1 : 0, 0, lp, rev, ds, dd, xchg_ptr(xchg, B, H, act)), "lstm_seq_bwd");
   return {dpre, dh0, dc0};
 }
 
@@ -1044,7 +1055,7 @@ void lstm_seq_bwd_into(const std::optional<Tensor>& dh_seq, const Tensor& w_hT, 
                        Tensor dh0, Tensor dc0, Tensor tiled, Tensor sync_ws, int64_t variant, std::optional<Tensor> in_gate,
                        int64_t in_gate_tiles_n, bool extra_signal, int64_t stream_handle, int64_t launch_flags,
                        const std::optional<Tensor>& lengths, bool reverse, const std::optional<Tensor>& drop_step,
-                       const std::vector<int64_t>& drop_desc) {
+                       const std::vector<int64_t>& drop_desc, const std::optional<Tensor>& xchg) {
   chk_cuda(w_hT, "w_hT"); chk_cuda(act, "act"); chk_cuda(c_seq, "c_seq"); chk_cuda(dpre, "dpre"); chk_cuda(dh0, "dh0"); chk_cuda(dc0, "dc0");
   c10::cuda::CUDAGuard gd(act.device());
   int T = act.size(0), B = act.size(1), H = act.size(2) / 4;
@@ -1058,7 +1069,7 @@ void lstm_seq_bwd_into(const std::optional<Tensor>& dh_seq, const Tensor& w_hT, 
                         dh0.data_ptr<float>(), dc0.data_ptr<float>(), nullptr, tiled.data_ptr(), T, B, H, (unsigned int*)sync_ws.data_ptr<int>(),
                         (int)variant, stream_handle ? (cudaStream_t)stream_handle : stream(),
                         in_gate.has_value() ? (const unsigned int*)in_gate->data_ptr<int>() : nullptr, (int)in_gate_tiles_n,
-                        extra_signal ? 1 : 0, (int)launch_flags, lp, rev, ds, dd), "lstm_seq_bwd_into");
+                        extra_signal ? 1 : 0, (int)launch_flags, lp, rev, ds, dd, xchg_ptr(xchg, B, H, act)), "lstm_seq_bwd_into");
 }
 
 }  // namespace
@@ -1074,11 +1085,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("col0") = 0, py::arg("ncols") = 0, py::arg("max_ctas") = 0);
   m.def("lstm_seq_cluster_probe", [](int64_t c) { return ts_lstm_seq_cluster_probe((int)c); });
   // (ring stages, batch tiles per CTA, streamed weights, forward K-split) of the persistent kernel for these arguments
-  m.def("lstm_seq_config", [](bool bwd, int64_t H, int64_t B, int64_t variant) {
+  // xchg_l2: the backward kernel that reduce-scatters through L2 (what an xchg buffer selects)
+  m.def("lstm_seq_config", [](bool bwd, int64_t H, int64_t B, int64_t variant, bool xchg_l2) {
     int out[4];
-    check(ts_lstm_seq_config(bwd ? 1 : 0, (int)H, (int)B, (int)variant, out), "lstm_seq_config");
+    check(ts_lstm_seq_config(bwd ? 1 : 0, (int)H, (int)B, (int)variant, out, xchg_l2 ? 1 : 0), "lstm_seq_config");
     return std::make_tuple(out[0], out[1], out[2] != 0, out[3] != 0);
-  }, py::arg("bwd"), py::arg("H"), py::arg("B"), py::arg("variant") = 0);
+  }, py::arg("bwd"), py::arg("H"), py::arg("B"), py::arg("variant") = 0, py::arg("xchg_l2") = false);
   m.def("lstm_pointwise_bwd", &lstm_pointwise_bwd, py::arg("dh_a"), py::arg("dh_b"), py::arg("dc_in"), py::arg("act"), py::arg("c_prev"),
         py::arg("c_new"), py::arg("lengths") = py::none(), py::arg("t") = 0);
   m.def("xent_rows", &xent_rows);
@@ -1141,7 +1153,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("b_mn") = false, py::arg("out_fp32") = false, py::arg("accumulate") = false, py::arg("ctas") = 2, py::arg("bn") = 256,
         py::arg("max_ctas") = 0, py::arg("gate") = py::none(), py::arg("gate_cfg") = std::vector<int64_t>{}, py::arg("done") = py::none(),
         py::arg("gate_err") = py::none(), py::arg("stream") = 0, py::arg("pdl") = false, py::arg("a_fold") = 0, py::arg("b_fold") = 0,
-        py::arg("fold_cols") = 0, py::arg("rowsum") = py::none(), py::arg("rowsum_acc") = false);
+        py::arg("fold_cols") = 0, py::arg("rowsum") = py::none(), py::arg("rowsum_acc") = false, py::arg("reverse_m") = false);
   m.def("lstm_seq_fwd", &lstm_seq_fwd, py::arg("gx"), py::arg("w_h"), py::arg("bias"), py::arg("h0"), py::arg("c0"),
         py::arg("sync_ws"), py::arg("variant") = 0, py::arg("dbg") = py::none(), py::arg("in_gate") = py::none(),
         py::arg("in_gate_tiles_n") = 0, py::arg("extra_signal") = false, py::arg("lengths") = py::none(), py::arg("reverse") = false,
@@ -1157,11 +1169,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("dh0"), py::arg("dc0"), py::arg("tiled"), py::arg("sync_ws"), py::arg("variant"), py::arg("in_gate") = py::none(),
         py::arg("in_gate_tiles_n") = 0, py::arg("extra_signal") = false, py::arg("stream") = 0, py::arg("launch_flags") = 0,
         py::arg("lengths") = py::none(), py::arg("reverse") = false, py::arg("drop_step") = py::none(),
-        py::arg("drop_desc") = std::vector<int64_t>{});
+        py::arg("drop_desc") = std::vector<int64_t>{}, py::arg("xchg") = py::none());
   m.def("lstm_seq_bwd", &lstm_seq_bwd, py::arg("dh_seq"), py::arg("w_hT"), py::arg("act"), py::arg("c_seq"), py::arg("dhT"),
         py::arg("dcT"), py::arg("sync_ws"), py::arg("variant") = 0, py::arg("dbg") = py::none(), py::arg("in_gate") = py::none(),
         py::arg("in_gate_tiles_n") = 0, py::arg("extra_signal") = false, py::arg("lengths") = py::none(), py::arg("reverse") = false,
-        py::arg("drop_step") = py::none(), py::arg("drop_desc") = std::vector<int64_t>{});
+        py::arg("drop_step") = py::none(), py::arg("drop_desc") = std::vector<int64_t>{}, py::arg("xchg") = py::none());
   m.def("act_reg_scratch", [](int64_t T, int64_t B, int64_t H, bool bf16) { return ts_act_reg_scratch((int)T, (int)B, (int)H, bf16 ? 1 : 0); });
   m.def("act_reg_fwd", &act_reg_fwd, py::arg("out"), py::arg("h"), py::arg("lengths"), py::arg("scratch"));
   m.def("act_reg_bwd", &act_reg_bwd, py::arg("dh"), py::arg("out"), py::arg("h"), py::arg("lengths"), py::arg("g"),

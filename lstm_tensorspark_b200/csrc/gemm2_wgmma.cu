@@ -357,7 +357,8 @@ int launch_major(const void* A, const void* B, const Gemm2Params& p, int lda, in
 
 // A: K-major [M, K] (lda = row pitch) or MN-major [K, M];  B: K-major [N, K] or MN-major [K, N];  C [M, N] row pitch ldc.
 // out_mode: 0 bf16, 1 fp32, 2 fp32 accumulate (C += A·B).  ctas: 1 or 2 (cluster sharing the B tile).  bn: 128 or 256.
-// gate_cfg[7] = {count, stride (u32 words), base, per_step, rows_per_step, use_last, reverse_m} (see Gemm2Params); max_ctas > 0 caps the grid.
+// gate_cfg[7] = {count, stride (u32 words), base, per_step, rows_per_step, use_last, reverse_m} (see Gemm2Params; reverse_m also
+// applies without a gate); max_ctas > 0 caps the grid.
 // rowsum (fp32 [M], or null): also rowsum[m] (=|+= with rowsum_acc) the sum over K of op(A)[m, :] (fp32 output only).
 extern "C" int ts_gemm2(const void* A, const void* B, void* C, const float* bias, int M, int N, int K, int lda, int ldb, int ldc,
                         int a_mn, int b_mn, int out_mode, int ctas, int bn, int dev, int max_ctas, const unsigned int* gate,
@@ -382,8 +383,9 @@ extern "C" int ts_gemm2(const void* A, const void* B, void* C, const float* bias
   p.gate = gate; p.gate_err = gate_err; p.done = done; p.pdl = pdl;
   if (gate != nullptr) {
     p.gate_count = gate_cfg[0]; p.gate_stride = gate_cfg[1]; p.gate_base = gate_cfg[2]; p.gate_per_step = gate_cfg[3];
-    p.gate_rows_per_step = gate_cfg[4] > 0 ? gate_cfg[4] : 1; p.gate_use_last = gate_cfg[5]; p.reverse_m = gate_cfg[6];
+    p.gate_rows_per_step = gate_cfg[4] > 0 ? gate_cfg[4] : 1; p.gate_use_last = gate_cfg[5];
   }
+  p.reverse_m = gate_cfg[6];
   p.gate_spin_limit = 6000000000LL;
   if (ctas == 2) {
     if (bn == 128) return launch_major<2, 128>(A, B, p, lda, ldb, a_mn, b_mn, out_mode, dev, max_ctas, st);

@@ -15,7 +15,8 @@
 //     the whole cell with one thread per batch row (the cell state never leaves its registers).  With one batch tile per
 //     CTA the two warpgroups split its rows; with two (kTiles = 2) they PING-PONG: each warpgroup owns one tile for the whole
 //     launch, so one tile's cell epilogue, exchange and dataflow signal run while the other tile's MMAs do.  At H = 1024
-//     with two batch tiles per CTA the ring holds 6 stages forward, 4 backward; with one, 4 forward (pick_stages).
+//     with two batch tiles per CTA the ring holds 6 stages forward, 4 backward; with one, 4 forward and 4 backward with the
+//     L2 exchange (pick_stages).
 //   * The forward pass can split K across a cluster of 2 CTAs and the backward pass does across 4 (one gate-column quarter
 //     each); the partial accumulators are reduce-scattered through DISTRIBUTED SHARED MEMORY with st.async (bytes are
 //     counted on the receiver's mbarrier: no release/acquire fences).  Every member then owns 16 hidden units.
@@ -179,6 +180,22 @@ TC_DEVICE bool wait_in_gate(const unsigned int* ctr, int lane, volatile int* abo
   ok = __shfl_sync(0xffffffffu, ok, 0);
   return ok != 0;
 }
+// Wait (one lane polls, the warp follows) until an arrival counter has reached `target` (kXchgL2 exchange).
+TC_DEVICE bool wait_count(const unsigned int* ctr, unsigned int target, int lane, volatile int* abort_flag) {
+  int ok = 1;
+  if (lane == 0) {
+    long long t0 = clock64();
+    int n = 0;
+    while ((int)(ld_acquire_gpu(ctr) - target) < 0) {
+      if ((++n & 63) == 0) {
+        if (*abort_flag) { ok = 0; break; }
+        if (clock64() - t0 > kSpinLimit) { *abort_flag = 1; ok = 0; break; }
+      }
+    }
+  }
+  ok = __shfl_sync(0xffffffffu, ok, 0);
+  return ok != 0;
+}
 TC_DEVICE void stg16(void* p, uint4 v) {
   asm volatile("st.global.v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
 }
@@ -232,12 +249,16 @@ struct SeqParams {
   // drop applied to the stored bf16 h), the backward pass applies the same mask to dh_seq as it loads it.
   __nv_bfloat16* h_drop;
   ts::DropSpec drop;
+  // kXchgL2 (backward, one tile, resident weights): the K-split's exchange buffer in global memory, [2 step parities][tiles_m]
+  // [H/64 groups nb][4 sources ks][4 chunks q][128 rows][16] bf16 - a source's 16 KB partial, chunk q = hidden [16 q, +16)
+  __nv_bfloat16* xchg;
 };
 
 // Work decomposition
 //   forward : CTA (mb, nb)      -> gate columns [64 nb, +64) = hidden [16 nb, +16) of batch tile mb, K = H.
 //   backward: CTA (mb, nb2, ks) -> partial dh columns [64 nb2, +64) over gate-column quarter ks (K = H); the 4 ks form a
-//                                 cluster; after the DSMEM reduce-scatter member ks owns hidden [64 nb2 + 16 ks, +16).
+//                                 cluster (kXchgL2: 4 consecutive CTAs); after the reduce-scatter member ks owns hidden
+//                                 [64 nb2 + 16 ks, +16).
 //             streamed weights (kNarrow): columns [32 nb2, +32) over gate-column half ks (K = 2H), clusters of 2; member ks
 //                                 then owns hidden [32 nb2 + 16 ks, +16) - the same 16 hidden units per CTA.
 // Warps: 0 = producer, 1..2 = idle, 3 = watchdog, 4..11 = two consumer warpgroups, `half` = (warp-4)/4, warp q = warp % 4.
@@ -270,6 +291,18 @@ struct SeqParams {
 //     tile-step land - earlier items again, and it holds no stage while it waits.
 //   A warpgroup never holds a stage while it waits on anything outside its own 4 warps, so no cycle can form and every
 //   item is eventually filled and released.  (The bounded spins and the watchdog remain as the safety net.)
+// kXchgL2 (backward, one tile per CTA, resident weights): the same work split without a cluster - member ks of group
+// (mb, nb) is CTA 4 (mb tiles_n / 4 + nb) + ks - and the reduce-scatter goes through L2 instead of DSMEM.  Clusters of 4
+// co-schedule only 120 CTAs on an H100, so at B = 256, H = 1024 the clustered backward needs two tiles on 64 CTAs; without
+// the cluster the 128 one-tile CTAs fit the 132 SMs.  Per step every member writes its [128 x 64] bf16 partial to slot
+// [step & 1][mb][nb][ks] of SeqParams::xchg (the same packed values the DSMEM path sends), the CTA barrier orders the
+// stores, and one red.release.gpu raises the group's counter (sync word kSyncKb + 32 (counters + mb H / 64 + nb), one 128 B
+// line after the k-block counters).  Each warp then waits (lane 0 acquire-polls) until the counter reaches 4 s and loads its
+// 16-column chunk of all four slots through L2 (ld.cg), summed in source order 0..3 exactly like the DSMEM path: given the
+// same partials, dh has the same bits.  Two parities suffice, with no "buffer free" handshake: a member writes step s + 2
+// into step s's slot only after its own wait at step s + 1, which needs all four members' step s + 1 writes, and each
+// member issues those (and the release that publishes them) after it has read step s.  The wait is entered after the
+// borrowed ring stages are released, like the DSMEM wait, so the deadlock argument above holds unchanged.
 // kStream = true (H too large for a resident slice, e.g. H = 2048: W_h alone is 32 MB): the weight k-block travels through
 // the ring next to its operand k-block (24 KB stages, W comes out of L2 every step); everything else is unchanged.
 // kFSplit (forward): a cluster of 2 CTAs splits K.  Each member contracts over HALF of h_{t-1} (8 instead of 16 operand
@@ -290,17 +323,18 @@ struct SeqParams {
 // dropped units of dh_seq are zeroed as it is loaded (before the MMAs of the step) and the kept ones scaled in fp32 where dh
 // joins the carry.  A separate instantiation: the kernels without it are those of a build without dropout.
 template <bool kBwd, int kStages, int kTiles, bool kStream, bool kFSplit = false, bool kMasked = false, bool kRev = false,
-          bool kDrop = false>
+          bool kDrop = false, bool kXchgL2 = false>
 __global__ void __launch_bounds__(384, 1)
 lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
   static_assert(!(kFSplit && (kBwd || kStream || kTiles != 1)), "forward K-split: one tile, resident weights");
+  static_assert(!kXchgL2 || (kBwd && !kStream && kTiles == 1), "L2 exchange: backward, one tile, resident weights");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   // kNarrow (streamed backward): a cluster of 2 splits K = 4H in halves, 32 accumulator columns per CTA.  Clusters of 2 pack
   // onto the GPCs where clusters of 4 do not: at H = 2048 an H100 co-schedules only 120 of the 128 CTAs in clusters of 4.
   constexpr bool kNarrow = kBwd && kStream;
   constexpr int kSplit = kBwd ? (kNarrow ? 2 : 4) : (kFSplit ? 2 : 1);     // cluster size = K-split factor
-  constexpr bool kCluster = kSplit > 1;
+  constexpr bool kCluster = kSplit > 1 && !kXchgL2;
   constexpr int kBNm = kFSplit ? 2 * BN : (kNarrow ? BN / 2 : BN);        // accumulator columns per CTA
   constexpr int kCW = kNarrow ? 16 : 32;                     // backward: accumulator columns per epilogue thread ([kCW chalf, +kCW))
   constexpr int kWBlk = kBNm * BK * 2;                       // bytes of one weight k-block
@@ -337,7 +371,7 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
   const int in_mb = blockIdx.x % p.tiles_n;
   const uint32_t crank = kCluster ? cluster_ctarank() : 0;
   const int nb = in_mb / kSplit;                              // weight-row block of the cluster (64 rows; kFSplit: 128 rows)
-  const int ks = (int)crank;                                  // K-split member
+  const int ks = kXchgL2 ? in_mb % kSplit : (int)crank;       // K-split member
   volatile int* abort_flag = &ss->abort_flag;
   const int steps = kBwd ? p.T + 1 : p.T;                    // backward runs one extra GEMM to produce dh_0
 
@@ -994,39 +1028,68 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
             }
           }
           acc_release();
-          // A member only needs the dG blocks of ITS K-quarter, so nothing in the dataflow stops a fast member from being a
-          // whole step ahead of a slow one: explicit back-pressure before overwriting anybody's exchange buffer.
-          if (s > 1) {
-            ok = xwait(&ss->xchg_free[xt], (uint32_t)(s & 1), abort_flag);
-            if (!ok) break;
-          }
-          // reduce-scatter over the kSplit K parts: column chunk q (16 wide, bf16) goes to member q's slot [ks] (DSMEM)
-#pragma unroll
-          for (int u = 0; u < kPass; ++u) {
+          if constexpr (kXchgL2) {
+            // reduce-scatter through L2: this member's partial to its slot of the step's parity, one release per CTA, then
+            // every warp waits for the group's four arrivals (see kXchgL2 at the top)
+            uint8_t* slots = reinterpret_cast<uint8_t*>(p.xchg) + ((size_t)((s & 1) * p.tiles_m + mb) * (H / BN) + nb) * (kSplit * kABytes);
+            unsigned int* xctr = p.sync + kSyncKb + ((size_t)p.tiles_m * (4 * H / BK) + (size_t)mb * (H / BN) + nb) * 32;
 #pragma unroll
             for (int qq = 0; qq < kCW / 16; ++qq) {
-              const uint32_t q = (uint32_t)((kCW / 16) * ch(u) + qq);
-              const uint32_t dst = mapa(xbase + (uint32_t)((ks * BM + rloc) * 32), q);
-              const uint32_t* a = pk[u] + 8 * qq;
-              const uint32_t dbar = mapa(xbar, q);
-              st_async_u4(dst, make_uint4(a[0], a[1], a[2], a[3]), dbar);
-              st_async_u4(dst + 16, make_uint4(a[4], a[5], a[6], a[7]), dbar);
+              const uint32_t* a = pk[0] + 8 * qq;
+              stg32(slots + (size_t)ks * kABytes + ((kCW / 16) * chalf + qq) * (BM * 32) + rloc * 32, a[0], a[1], a[2], a[3], a[4],
+                    a[5], a[6], a[7]);
             }
-          }
-          ok = xwait(&ss->xchg_full[xt], xphase, abort_flag);
-          if (!ok) break;
-#pragma unroll
-          for (int u = 0; u < kPass; ++u) {
+            epi_bar();
+            if (gtid == 0) signal_counter(xctr);
+            ok = wait_count(xctr, 4u * (unsigned)s, lane, abort_flag);
+            if (!ok) break;
+            if (dbg_wg) dbg_stamp(s, 3);                          // group counter seen (stamp 1 -> 3: partial out, exchange wait)
             if (!prev_pad) {
 #pragma unroll
-              for (int i = 0; i < 8; ++i) dh[u][i] = 0.f;
+              for (int i = 0; i < 8; ++i) dh[0][i] = 0.f;
             }
 #pragma unroll
             for (int src = 0; src < kSplit; ++src) {
-              const uint4 x4 = *reinterpret_cast<const uint4*>(xbuf + (size_t)(src * BM + rloc) * 32 + 16 * ch(u));
+              const uint4 x4 = ldg_cg16(slots + (size_t)src * kABytes + ks * (BM * 32) + rloc * 32 + 16 * chalf);
               const uint32_t w[4] = {x4.x, x4.y, x4.z, x4.w};
 #pragma unroll
-              for (int i = 0; i < 4; ++i) { dh[u][2 * i] += bf_lo(w[i]); dh[u][2 * i + 1] += bf_hi(w[i]); }
+              for (int i = 0; i < 4; ++i) { dh[0][2 * i] += bf_lo(w[i]); dh[0][2 * i + 1] += bf_hi(w[i]); }
+            }
+          } else {
+            // A member only needs the dG blocks of ITS K-quarter, so nothing in the dataflow stops a fast member from being a
+            // whole step ahead of a slow one: explicit back-pressure before overwriting anybody's exchange buffer.
+            if (s > 1) {
+              ok = xwait(&ss->xchg_free[xt], (uint32_t)(s & 1), abort_flag);
+              if (!ok) break;
+            }
+            // reduce-scatter over the kSplit K parts: column chunk q (16 wide, bf16) goes to member q's slot [ks] (DSMEM)
+#pragma unroll
+            for (int u = 0; u < kPass; ++u) {
+#pragma unroll
+              for (int qq = 0; qq < kCW / 16; ++qq) {
+                const uint32_t q = (uint32_t)((kCW / 16) * ch(u) + qq);
+                const uint32_t dst = mapa(xbase + (uint32_t)((ks * BM + rloc) * 32), q);
+                const uint32_t* a = pk[u] + 8 * qq;
+                const uint32_t dbar = mapa(xbar, q);
+                st_async_u4(dst, make_uint4(a[0], a[1], a[2], a[3]), dbar);
+                st_async_u4(dst + 16, make_uint4(a[4], a[5], a[6], a[7]), dbar);
+              }
+            }
+            ok = xwait(&ss->xchg_full[xt], xphase, abort_flag);
+            if (!ok) break;
+#pragma unroll
+            for (int u = 0; u < kPass; ++u) {
+              if (!prev_pad) {
+#pragma unroll
+                for (int i = 0; i < 8; ++i) dh[u][i] = 0.f;
+              }
+#pragma unroll
+              for (int src = 0; src < kSplit; ++src) {
+                const uint4 x4 = *reinterpret_cast<const uint4*>(xbuf + (size_t)(src * BM + rloc) * 32 + 16 * ch(u));
+                const uint32_t w[4] = {x4.x, x4.y, x4.z, x4.w};
+#pragma unroll
+                for (int i = 0; i < 4; ++i) { dh[u][2 * i] += bf_lo(w[i]); dh[u][2 * i + 1] += bf_hi(w[i]); }
+              }
             }
           }
         }
@@ -1099,7 +1162,7 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
           if (dbg_wg) dbg_stamp(s, 2);
         }
         // (the barrier above also means every thread of the tile is done reading this step's exchange buffer)
-        if (s > 0) {
+        if (!kXchgL2 && s > 0) {
           if (gtid == 32) tc::mbar_expect_tx_u32(xbar, kXchgRecv);    // arm the next phase, THEN free the buffer
           __syncwarp();
           if (gtid >= 32 && gtid < 32 + kSplit) mbar_arrive_remote_relaxed(mapa(tc::smem_u32(&ss->xchg_free[xt]), (uint32_t)(gtid - 32)));
@@ -1154,7 +1217,7 @@ __global__ void seq_prologue_kernel(const __nv_bfloat16* __restrict__ h0, const 
     for (int i = threadIdx.x; i < kSyncErr; i += blockDim.x) sync[i] = 0u;
 }
 
-size_t smem_bytes(int H, bool bwd, int stages, int tiles, bool stream = false, bool fsplit = false) {
+size_t smem_bytes(int H, bool bwd, int stages, int tiles, bool stream = false, bool fsplit = false, bool xl2 = false) {
   const bool narrow = bwd && stream;                       // streamed backward: 32 accumulator columns per CTA (kNarrow)
   const size_t ring = (size_t)stages * (stream ? kABytes + (narrow ? kWBlockBytes / 2 : kWBlockBytes) : kABytes);
   // resident weights: H/64 blocks of [64 x 64] (forward K-split: H/128 blocks of [128 x 64] = the same bytes)
@@ -1163,15 +1226,17 @@ size_t smem_bytes(int H, bool bwd, int stages, int tiles, bool stream = false, b
   // dedicated fp32 buffer of [128 x columns] per tile being staged at once (lstm_seq_kernel, ring_acc).
   const bool dedicated = fsplit || (!narrow && H / BK < 2 && !(tiles == 2 && bwd));
   const size_t acc_stage = dedicated ? (size_t)tiles * BM * (fsplit ? 2 * BN : BN) * sizeof(float) : 0;
-  return (stream ? 0 : (size_t)(H / BK) * kWBlockBytes) + ring + ((bwd || fsplit) ? tiles * kXchgBytes : 0) + acc_stage + sizeof(SeqSmem) + 1024;
+  // (the backward's DSMEM exchange buffer: not with the L2 exchange, xl2)
+  return (stream ? 0 : (size_t)(H / BK) * kWBlockBytes) + ring + (((bwd && !xl2) || fsplit) ? tiles * kXchgBytes : 0) + acc_stage +
+         sizeof(SeqSmem) + 1024;
 }
 
 template <bool kBwd, int kStages, int kTiles, bool kStream = false, bool kFSplit = false, bool kMasked = false, bool kRev = false,
-          bool kDrop = false>
+          bool kDrop = false, bool kXchgL2 = false>
 int launch_cfg(const CUtensorMap& tw, const SeqParams& p, int grid, cudaStream_t st) {
-  auto kern = lstm_seq_kernel<kBwd, kStages, kTiles, kStream, kFSplit, kMasked, kRev, kDrop>;
-  const size_t smem = smem_bytes(p.H, kBwd, kStages, kTiles, kStream, kFSplit);
-  constexpr int kClusterDim = kBwd ? (kStream ? 2 : 4) : (kFSplit ? 2 : 1);
+  auto kern = lstm_seq_kernel<kBwd, kStages, kTiles, kStream, kFSplit, kMasked, kRev, kDrop, kXchgL2>;
+  const size_t smem = smem_bytes(p.H, kBwd, kStages, kTiles, kStream, kFSplit, kXchgL2);
+  constexpr int kClusterDim = kBwd ? (kStream ? 2 : (kXchgL2 ? 1 : 4)) : (kFSplit ? 2 : 1);
   if (smem > 227 * 1024) return -4;
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return (int)e;
@@ -1198,6 +1263,16 @@ int launch_cfg(const CUtensorMap& tw, const SeqParams& p, int grid, cudaStream_t
 
 template <bool kBwd, bool kMasked, bool kRev, bool kDrop>
 int dispatch(const CUtensorMap& tw, const SeqParams& p, int grid, int stages, int tiles, bool stream, bool fsplit, cudaStream_t st) {
+  if constexpr (kBwd) {
+    if (p.xchg != nullptr) {                       // one tile per CTA, K-split reduce-scattered through L2 (no cluster)
+      switch (stages) {
+        case 4: return launch_cfg<true, 4, 1, false, false, kMasked, kRev, kDrop, true>(tw, p, grid, st);
+        case 5: return launch_cfg<true, 5, 1, false, false, kMasked, kRev, kDrop, true>(tw, p, grid, st);
+        case 6: return launch_cfg<true, 6, 1, false, false, kMasked, kRev, kDrop, true>(tw, p, grid, st);
+      }
+      return -5;
+    }
+  }
   if constexpr (!kBwd) {
     if (fsplit) {                                  // forward K-split (cluster of 2), one batch tile per CTA
       switch (stages) {
@@ -1246,13 +1321,15 @@ int dispatch_dir(const CUtensorMap& tw, const SeqParams& p, int grid, int stages
                               : dispatch<kBwd, false, false, kDrop>(tw, p, grid, stages, tiles, stream, fsplit, st));
 }
 
-int pick_stages(int H, bool bwd, int tiles) {
+int pick_stages(int H, bool bwd, int tiles, bool xl2 = false) {
   // One tile per CTA forward with H >= 1024 (>= 16 k-blocks per step, the resident slice takes >= 128 KB): 4 stages, not the
   // deepest ring that fits.  At B = 256, H = 1024 on an H100 80GB HBM3 (700 W) a step took 10.9-11.5 us with 4 stages against
   // 11.3-12.1 us with 6 (11.3-11.8 with 5, 12.1-12.4 with 3), eight runs each; 4 was the fastest within every set of runs.
-  if (!bwd && tiles == 1 && H / BK >= 16 && smem_bytes(H, false, 4, 1) <= 227 * 1024) return 4;
+  // The one-tile backward with the L2 exchange (xl2) likewise, at H = 1024 and B = 256 on the same card: 13.80-13.90 us per step
+  // with 4 stages, 14.67-14.74 with 5 and 14.45-14.67 with 6, three runs each, 4 the fastest in every run.
+  if ((!bwd || xl2) && tiles == 1 && H / BK >= 16 && smem_bytes(H, bwd, 4, 1, false, false, xl2) <= 227 * 1024) return 4;
   for (int s = 6; s >= 2; --s)
-    if (smem_bytes(H, bwd, s, tiles) <= 227 * 1024) return s;
+    if (smem_bytes(H, bwd, s, tiles, false, false, xl2) <= 227 * 1024) return s;
   return 0;
 }
 
@@ -1268,7 +1345,8 @@ struct SeqCfg {
 
 // The launch configuration seq_common() uses for H, B and variant (no device needed): 0, or a negative code with the error
 // message set.
-static int seq_config(bool bwd, int H, int B, int variant, SeqCfg& c) {
+// xl2: the backward kernel with the L2 exchange (kXchgL2; one tile per CTA, resident weights).
+static int seq_config(bool bwd, int H, int B, int variant, SeqCfg& c, bool xl2 = false) {
   if (H % 64 != 0) { ts::set_last_error("lstm_seq: H must be a multiple of 64"); return -2; }
   const int tiles_m = (B + BM - 1) / BM;
   int stages = (variant >> 4) & 15, tiles = variant & 15;
@@ -1278,9 +1356,14 @@ static int seq_config(bool bwd, int H, int B, int variant, SeqCfg& c) {
   const bool stream = H > (bwd ? 1024 : 1152) || ((variant >> 8) & 1);
   if (stream) tiles = 1;
   if (bwd && stream && 4 * H / (2 * BK) > 64) { ts::set_last_error("lstm_seq: streamed backward needs H <= 2048"); return -2; }
-  // one arrival counter per operand k-block of every batch tile, at word kSyncKb + 32 i: the last one must stay below the
-  // sticky error word (a layout with more counters would count its arrivals into the error flag)
-  const int counters = tiles_m * (bwd ? 4 * H : H) / BK;
+  if (xl2 && (!bwd || stream || tiles != 1)) {
+    ts::set_last_error("lstm_seq: the L2 exchange needs the backward pass at one tile per CTA with resident weights");
+    return -2;
+  }
+  // one arrival counter per operand k-block of every batch tile, at word kSyncKb + 32 i, then (xl2) one exchange counter per
+  // group of 4 CTAs: the last one must stay below the sticky error word (a layout with more counters would count its
+  // arrivals into the error flag)
+  const int counters = tiles_m * (bwd ? 4 * H : H) / BK + (xl2 ? tiles_m * H / BN : 0);
   if (kSyncKb + 32 * (counters - 1) >= kSyncErr) {
     ts::set_last_error("lstm_seq: the k-block arrival counters of this layout do not fit in the sync workspace");
     return -2;
@@ -1296,8 +1379,9 @@ static int seq_config(bool bwd, int H, int B, int variant, SeqCfg& c) {
       while (stages > 3 && smem_bytes(H, false, stages, 1, false, true) > 227 * 1024) --stages;
     }
   } else {
-    if (stages == 0) stages = pick_stages(H, bwd, tiles);
-    if (stages < 2 || smem_bytes(H, bwd, stages, tiles) > 227 * 1024) { ts::set_last_error("lstm_seq: weight slice does not fit in shared memory"); return -4; }
+    if (stages == 0) stages = pick_stages(H, bwd, tiles, xl2);
+    if (stages < 2 || smem_bytes(H, bwd, stages, tiles, false, false, xl2) > 227 * 1024) { ts::set_last_error("lstm_seq: weight slice does not fit in shared memory"); return -4; }
+    if (xl2 && (stages < 4 || stages > 6)) { ts::set_last_error("lstm_seq: the L2 exchange runs 4 to 6 ring stages"); return -4; }
   }
   c = SeqCfg{stages, tiles, stream, fsplit};
   return 0;
@@ -1311,7 +1395,7 @@ static int seq_common(SeqParams& p, const void* w_base, int variant, cudaStream_
     return -2;
   }
   SeqCfg cfg;
-  if (int rc = seq_config(kBwd, H, B, variant, cfg)) return rc;
+  if (int rc = seq_config(kBwd, H, B, variant, cfg, p.xchg != nullptr)) return rc;
   const int stages = cfg.stages, tiles = cfg.tiles;
   const bool stream = cfg.stream, fsplit = cfg.fsplit;
   const int tiles_m = (B + BM - 1) / BM, tiles_n = kBwd ? (H / BN) * 4 : 4 * H / BN;
@@ -1360,10 +1444,11 @@ extern "C" int ts_lstm_seq_fwd(const void* gx, const void* w_h, const float* bia
 }
 
 // The launch configuration ts_lstm_seq_fwd / _bwd choose for H, B and variant, without a device: out = {ring stages, batch
-// tiles per CTA, streamed weights, forward K-split}.  0, or a negative code with ts_last_error set.
-extern "C" int ts_lstm_seq_config(int bwd, int H, int B, int variant, int* out) {
+// tiles per CTA, streamed weights, forward K-split}; xchg_l2: the backward with the L2 exchange (an xchg buffer passed).  0,
+// or a negative code with ts_last_error set.
+extern "C" int ts_lstm_seq_config(int bwd, int H, int B, int variant, int* out, int xchg_l2) {
   SeqCfg c;
-  if (int rc = seq_config(bwd != 0, H, B, variant, c)) return rc;
+  if (int rc = seq_config(bwd != 0, H, B, variant, c, xchg_l2 != 0)) return rc;
   out[0] = c.stages; out[1] = c.tiles; out[2] = c.stream; out[3] = c.fsplit;
   return 0;
 }
@@ -1381,7 +1466,7 @@ extern "C" int ts_lstm_seq_prologue(const void* h0, const float* c0, void* h_seq
 extern "C" int ts_lstm_seq_bwd(const void* dh_seq, const void* w_hT, const void* act, const float* c_seq, const void* dpre,
                                float* dh0, float* dc0, void* dbg, void* a_tiled, int T, int B, int H, unsigned int* sync_ws, int variant,
                                cudaStream_t st, const unsigned int* in_gate, int in_gate_tiles_n, int extra_signal, int launch_flags,
-                               const int* lengths, int reverse, const int* drop_step, const unsigned int* drop_desc) {
+                               const int* lengths, int reverse, const int* drop_step, const unsigned int* drop_desc, void* xchg) {
   if (!(launch_flags & 1)) cudaMemsetAsync(sync_ws, 0, kSyncErr * sizeof(unsigned int), st);      // arrival counters restart at 0 every launch
   SeqParams p{};
   p.a_tiled = (__nv_bfloat16*)a_tiled;
@@ -1391,6 +1476,7 @@ extern "C" int ts_lstm_seq_bwd(const void* dh_seq, const void* w_hT, const void*
   p.pdl_wait = (launch_flags >> 1) & 1;
   p.lengths = lengths;
   p.drop = ts::make_drop_spec(drop_step, drop_desc);
+  p.xchg = (__nv_bfloat16*)xchg;      // non-null: one tile per CTA, reduce-scatter through L2 (kXchgL2)
   return seq_common<true>(p, w_hT, variant, st, reverse != 0);
 }
 

@@ -199,6 +199,33 @@ def _fwd_variant(B: int, H: int, device) -> int:
     return SEQ_VARIANT if _fwd_full_width(B, H, device) else _seq_variant(B, H, device)
 
 
+def bwd_tiles_per_cta(B: int, H: int, sms: int, coresident: int) -> Optional[int]:
+    """Batch tiles per CTA of a backward recurrence that has the GPU to itself, on a device with ``sms`` SMs, ``coresident`` of
+    which hold backward CTAs in clusters of 4 (``_coresident_ctas``).  ``tiles_per_cta`` needs those clusters for the DSMEM
+    reduce-scatter of the K-split, and an H100 co-schedules only 120 such CTAs: at B = 256, H = 1024 that means two tiles on
+    64 CTAs.  With the reduce-scatter through L2 instead (csrc/lstm_seq_wgmma.cu, kXchgL2) the kernel needs no cluster, so its
+    128 one-tile CTAs fit the 132 SMs.  1 where ``tiles_m * H / 16`` cluster-free one-tile CTAs fit ``sms`` (resident weights,
+    H <= 1024), else what ``tiles_per_cta`` returns."""
+    tiles = tiles_per_cta(B, H, coresident)
+    if tiles != 2:
+        return tiles
+    return 1 if (B + 127) // 128 * (H // 16) <= sms else 2
+
+
+def _bwd_full_width(B: int, H: int, device) -> bool:
+    """Does a backward recurrence that runs alone take one batch tile per CTA with the L2 exchange where ``_seq_variant``
+    takes two?  Decided from the device's SM count and cluster co-residency up front, not by a failed launch."""
+    if SEQ_VARIANT & 15 or _tiles_per_cta(B, H, device) != 2:
+        return False
+    return bwd_tiles_per_cta(B, H, _sms(device), _coresident_ctas(device, _bwd_cluster(H))) == 1
+
+
+def _xchg_buffer(B: int, H: int, device) -> torch.Tensor:
+    """Exchange buffer of the one-tile backward kernel that reduce-scatters through L2: two step parities x H / 16 CTAs per
+    batch tile x a [128 x 64] bf16 partial (4 MiB at B = 256, H = 1024)."""
+    return torch.empty(2 * ((B + 127) // 128) * (H // 16) * 128 * 64, dtype=torch.bfloat16, device=device)
+
+
 def fast_path_supported(B: int, H: int, dtype: torch.dtype, device) -> bool:
     if FORCE_GENERIC or dtype != torch.bfloat16 or H % 64 != 0:
         return False
@@ -410,11 +437,16 @@ class _LSTMSeqFn(torch.autograd.Function):
         dhT = (dh_T.float().contiguous() if dh_T is not None else torch.zeros(B, H, dtype=torch.float32, device=dev))
         if ctx.fast:
             w_hT = _transposed(w_h_c)
+            # the only recurrence on the GPU: one tile per CTA with the L2 exchange where that fits (_bwd_full_width)
+            full = _bwd_full_width(B, H, dev)
             big_launch_begin()
-            dpre, dh0, dc0 = E.lstm_seq_bwd(dh_seq, w_hT, act, c_seq, dhT, dcT, _sync_ws(dev), _seq_variant(B, H, dev),
-                                            lengths=ctx.lengths, reverse=ctx.reverse, **drop)
+            dpre, dh0, dc0 = E.lstm_seq_bwd(dh_seq, w_hT, act, c_seq, dhT, dcT, _sync_ws(dev),
+                                            SEQ_VARIANT if full else _seq_variant(B, H, dev), lengths=ctx.lengths,
+                                            reverse=ctx.reverse, xchg=_xchg_buffer(B, H, dev) if full else None, **drop)
             STATS["fast_bwd"] += 1
             STATS["kernels"] += 1
+            if full:
+                count("bwd_full_width")
             after_big_launch()                   # finished gradient buckets of the layers above: sync them under this recurrence
         else:
             dpre = torch.empty_like(act)
@@ -505,6 +537,7 @@ def lstm_layer_sequence(x_seq, h0, c0, w_x, w_h, bias, lengths=None, reverse=Fal
 # projection gx_a too: L_a waits for it block by block)
 #     forward :  L_a  || gx_a, gx_b (gated)              ->  L_b
 #     backward:  L_b  || dx_b (gated)                    ->  L_a  || dW_xb, dW_hb, db_b
+#            or  L_b alone, one tile per CTA             ->  L_a  || dx_b, dW_xb, dW_hb, db_b   (where that fits: _bwd_full_width)
 # =====================================================================================================================
 FOLDED_FEED = os.environ.get("LSTM_TS_FOLDED_FEED", "1") != "0"   # batch-major input read in place by the first layer's GEMMs
 WAVEFRONT = os.environ.get("LSTM_TS_WAVEFRONT", "1") == "1"
@@ -547,7 +580,8 @@ def pair_schedule(T: int, B: int, D: int, h_a: int, h_b: int, sms: int, coreside
     B = 256 (one GEMM tile row per time step), resident weights (H <= 1024) and 256-aligned widths.
       "wavefront": both recurrences co-resident, the gated GEMM on the SMs they leave free (H_a/16 + H_b/16 + 8 SMs).
       "pipelined": the recurrences run one after the other, GEMMs next to them (forward: L_a with its own gx_a and with gx_b;
-                   backward: L_b with dx_b, then L_a with dW_xb, dW_hb and db_b).  Needs max(H)/16 + 8 SMs.
+                   backward: L_b with dx_b, then L_a with dW_xb, dW_hb and db_b; where L_b's backward fits one tile per
+                   CTA, L_b alone, then L_a with dx_b too).  Needs max(H)/16 + 8 SMs.
       None: two separate layers."""
     if B != 256 or T < 2 or D % 8 != 0 or any(h % 256 != 0 or h > 1024 for h in (h_a, h_b)):
         return None
@@ -569,6 +603,21 @@ def pipelined_fwd_split(sms: int, d: int, h_a: int, h_b: int) -> tuple:
     free = max(2, sms - h_a // 16)
     n_a = min(free - 1, max(1, round(free * d / (d + h_b)))) if d > 0 else 0     # d = 0: gx_a computed before L_a
     return n_a, free - n_a
+
+
+def pipelined_bwd_split(sms: int, h_a: int, h_b: int) -> tuple:
+    """SMs of the pipelined pair's backward side GEMMs when L_b's backward runs alone at one tile per CTA -> (dx_b CTAs, CTAs of
+    each of dW_xb and dW_hb).  All three run next to L_a's backward on the ``sms - h_a / 16 - _COLSUM_SMS`` SMs its CTAs and
+    the bias column sums leave free, one single-CTA 128 x 256 tile per SM.  Their work is 2·T·B·4h_b·h_a (dx_b),
+    2·T·B·4h_b·h_a (dW_xb) and 2·T·B·4h_b·h_b (dW_hb) FLOP.  L_a waits for dx_b(t) at its step t, while dW_xb and dW_hb only
+    have to end with it, so dx_b gets a third more than its share of the work: the free SMs are split in the ratio
+    4h_a : 3h_a : 3h_b, 26 + 19 + 19 at the headline 2 x 1024 on a 132-SM H100.  There a step of L_a's backward takes about
+    20 us, and 26 SMs compute a step's 2.1 GFLOP of dx_b (eight 128 x 256 tiles) in about 16 us at 5.2 TFLOP/s per SM
+    (bench/side_gemms.py).  On an H100 80GB HBM3 at 700 W the headline step took 9.84 ms with 26 dx_b CTAs, against 9.87-9.88
+    with 21 (the plain work ratio), 9.87-9.88 with 30 and 9.92-9.96 with 34, two runs each."""
+    free = max(3, sms - h_a // 16 - _COLSUM_SMS)
+    n_dx = min(free - 2, max(1, round(free * 4 * h_a / (7 * h_a + 3 * h_b))))
+    return n_dx, (free - n_dx) // 2
 
 
 def _pair_schedule_of(x_seq: torch.Tensor, h_a: int, h_b: int) -> Optional[str]:
@@ -753,17 +802,36 @@ class _LSTMPairFn(torch.autograd.Function):
         # programmatic-dependent-launch chain on one stream (see forward): L_b -> L_a -> gated dX GEMM.  Pipelined: L_b -> gated
         # dX GEMM -> L_a (ordinary launch: dx_b is complete when it starts)
         pipelined = ctx.pipelined
+        # pipelined, where L_b's backward fits one tile per CTA with the L2 exchange (_bwd_full_width): it runs alone on 128 SMs,
+        # and dx_b moves next to L_a's backward, which waits for it block by block (as L_a's forward does for gx_a)
+        full_b = pipelined and _bwd_full_width(B, Hb, dev)
         # dropout: each recurrence masks the gradient into its output sequence as it loads it (dx_b stays the raw dL/dh_drop_a)
-        E.lstm_seq_bwd_into(dh_seq_b, whT_b, act_b, c_seq_b, dpre_b, dh0b, dc0b, til_b, ws_b, var, None, 0, True, 0, 1, ctx.lengths, **drb)
-        if not pipelined:
-            E.lstm_seq_bwd_into(dx_b, whT_a, act_a, c_seq_a, dpre_a, dh0a, dc0a, til_a, ws_a, var, done, tn, False, 0, 3, ctx.lengths,
+        if full_b:
+            # L_b: an ordinary launch.  L_a: the chain head, gated on dx_b's 128 x 256 blocks.  dx_b: its programmatic dependent,
+            # ungated (L_b is complete) on its capped grid, walking the M tiles (time steps) from the last, the order in which L_a
+            # consumes them.  dW_xb, dW_hb and db_b follow as programmatic dependents (below).
+            n_dx, side = pipelined_bwd_split(_sms(dev), Ha, Hb)
+            E.lstm_seq_bwd_into(dh_seq_b, whT_b, act_b, c_seq_b, dpre_b, dh0b, dc0b, til_b, ws_b, var & ~15, None, 0, False, 0, 1,
+                                ctx.lengths, xchg=_xchg_buffer(B, Hb, dev), **drb)
+            E.lstm_seq_bwd_into(dx_b, whT_a, act_a, c_seq_a, dpre_a, dh0a, dc0a, til_a, ws_a, var, done, tn, False, 0, 1, ctx.lengths,
                                 **dra)
-        free_ctas = max(1, _sms(dev) - Hb // 16 - (0 if pipelined else Ha // 16))
-        E.gemm2(dpre_b.view(T * B, 4 * Hb), wxb, out=dx_b.view(T * B, Ha), b_mn=True, ctas=1, bn=256, max_ctas=free_ctas,
-                gate=ws_b[_gate_off(var):], gate_cfg=_gate_cfg(var, 2, 4 * Hb // 64, 1, 4 * Hb // 64, T + 1, -1, B, True), done=done,
-                gate_err=ws_b[SYNC_WORDS - 1:], pdl=True)
-        if pipelined:
-            E.lstm_seq_bwd_into(dx_b, whT_a, act_a, c_seq_a, dpre_a, dh0a, dc0a, til_a, ws_a, var, None, 0, False, 0, 1, ctx.lengths, **dra)
+            E.gemm2(dpre_b.view(T * B, 4 * Hb), wxb, out=dx_b.view(T * B, Ha), b_mn=True, ctas=1, bn=256, max_ctas=n_dx, done=done,
+                    pdl=True, reverse_m=True)
+            count("bwd_full_width")
+        else:
+            E.lstm_seq_bwd_into(dh_seq_b, whT_b, act_b, c_seq_b, dpre_b, dh0b, dc0b, til_b, ws_b, var, None, 0, True, 0, 1, ctx.lengths,
+                                **drb)
+            if not pipelined:
+                E.lstm_seq_bwd_into(dx_b, whT_a, act_a, c_seq_a, dpre_a, dh0a, dc0a, til_a, ws_a, var, done, tn, False, 0, 3,
+                                    ctx.lengths, **dra)
+            free_ctas = max(1, _sms(dev) - Hb // 16 - (0 if pipelined else Ha // 16))
+            E.gemm2(dpre_b.view(T * B, 4 * Hb), wxb, out=dx_b.view(T * B, Ha), b_mn=True, ctas=1, bn=256, max_ctas=free_ctas,
+                    gate=ws_b[_gate_off(var):], gate_cfg=_gate_cfg(var, 2, 4 * Hb // 64, 1, 4 * Hb // 64, T + 1, -1, B, True), done=done,
+                    gate_err=ws_b[SYNC_WORDS - 1:], pdl=True)
+            if pipelined:
+                E.lstm_seq_bwd_into(dx_b, whT_a, act_a, c_seq_a, dpre_a, dh0a, dc0a, til_a, ws_a, var, None, 0, False, 0, 1, ctx.lengths,
+                                    **dra)
+            side = max(1, (_sms(dev) - Ha // 16 - _COLSUM_SMS) // 2)
         STATS["fast_bwd"] += 2
         STATS["kernels"] += 5
         a = ctx.addrs
@@ -779,8 +847,7 @@ class _LSTMPairFn(torch.autograd.Function):
             # ordinary launch (dW_xa), not under these: a programmatic dependent may start before the kernels ahead of it in
             # the stream are complete.
             # Weight drop: dW_hb's mask is an ordinary launch behind the column sums (it runs after L_a, before dW_xa), and W_hb is
-            # released only from then on.
-            side = max(1, (_sms(dev) - Ha // 16 - _COLSUM_SMS) // 2)
+            # released only from then on.  With dx_b beside L_a too (full_b), they share what dx_b leaves (pipelined_bwd_split).
             dw_xb = _accumulate_grad(a[3], dg_b.t(), hin_b.reshape(T * B, Ha), pdl=True, max_ctas=side)
             release(a[3])
             part, out, dw_hb = _grad_gemm(a[4], dg_b.t(), h_seq_b[:T].reshape(T * B, Hb), pdl=True, max_ctas=side, masked=bool(wdb))
