@@ -89,7 +89,11 @@ class Config:
     dtype: str = "auto"                 # auto: bf16 on cuda, fp32 on cpu
     device: str = "auto"                # auto | cpu | cuda
     backend: str = "auto"               # auto | cuda_ext (hand-written sm_90a kernels) | torch
-    optimizer: str = "adam"             # adam (TF formulation) | sgd
+    optimizer: str = "adam"             # adam (TF formulation) | sgd | asgd (SGD + the average of the iterates, evaluated and
+                                        # exported) | ntasgd (sgd until the non-monotone trigger fires, then asgd: AWD-LSTM)
+    nonmono: int = 5                    # ntasgd: fire when the validation loss exceeds the best of all but the last N validations
+    valid_path: str = ""                # held-out set in --training_path's format, scored at every evaluation step
+    valid_synthetic: int = 0            # >0: N held-out samples (--stateful: a stream of N segments) of the --synthetic task
     sync_mode: str = "param_avg"        # param_avg (reference) | grad_allreduce | none
     sync_every: int = 0                 # 0 => once at the end of training (reference); N => every N steps
     average_scope: str = "lstm"         # lstm (reference: map_data_by_key set) | all
@@ -268,8 +272,26 @@ class Config:
             raise ValueError(f"--clip_grad_norm must be a finite number >= 0 (0 = off), got {self.clip_grad_norm}")
         if self.clips_synced_grads() and self.comm == "fused":
             raise ValueError(FUSED_CLIP_ERROR)
-        if self.optimizer not in ("adam", "sgd"):
-            raise ValueError(f"unknown --optimizer {self.optimizer}")
+        if self.optimizer not in ("adam", "sgd", "asgd", "ntasgd"):
+            raise ValueError(f"unknown --optimizer {self.optimizer}: one of adam, sgd, asgd, ntasgd")
+        if self.nonmono < 1:
+            raise ValueError(f"--nonmono must be >= 1 (the validations the trigger looks past), got {self.nonmono}")
+        if self.valid_synthetic < 0:
+            raise ValueError(f"--valid_synthetic must be >= 0 (0 = off), got {self.valid_synthetic}")
+        if self.valid_path and self.valid_synthetic:
+            raise ValueError("--valid_path and --valid_synthetic both give a validation set: pass one of them")
+        if self.mode == "train" and self.valid_synthetic and not self.synthetic:
+            raise ValueError("--valid_synthetic draws held-out samples of the --synthetic task: add --synthetic N, or give the "
+                             "held-out file with --valid_path")
+        has_valid = bool(self.valid_path or self.valid_synthetic)
+        if self.mode == "train" and self.optimizer == "ntasgd" and not has_valid:
+            raise ValueError("--optimizer ntasgd switches averaging on when the validation loss stops improving: give a validation "
+                             "set with --valid_path or --valid_synthetic")
+        if self.nonmono != 5 and self.optimizer != "ntasgd":
+            warnings.warn(f"--nonmono {self.nonmono} has no effect without --optimizer ntasgd")
+        if has_valid and self.mode != "train":
+            warnings.warn(f"--valid_path / --valid_synthetic have no effect with --mode {self.mode}: the validation set is scored "
+                          "during training")
         if self.average_scope not in ("lstm", "all"):
             raise ValueError(f"unknown --average_scope {self.average_scope}")
         if self.steps_mode not in ("compat", "epochs"):
@@ -382,6 +404,16 @@ _HELP = {
     "temporal_activation_reg": "AWD-LSTM's temporal activation regularisation (TAR): in training, the loss backward runs on gains "
                                "BETA times the mean square of h_t - h_{t-1} of the top layer's raw output (before dropout) over "
                                "the real steps t >= 1 of each sequence; logged as `tar`.  Same head rule as --activation_reg.  0 = off",
+    "optimizer": "adam (TF formulation), sgd, asgd (SGD that also keeps the running average of its iterates, as "
+                 "torch.optim.ASGD(t0=0, lambd=0); evaluation, checkpoint scoring and the export use the average) or ntasgd "
+                 "(AWD-LSTM's non-monotonically triggered ASGD: sgd until the validation loss exceeds the best of all but the last "
+                 "--nonmono validations, then asgd from a fresh average; needs --valid_path or --valid_synthetic)",
+    "nonmono": "--optimizer ntasgd: the trigger looks past the last N validations (>= 1; AWD-LSTM's default 5)",
+    "valid_path": "Held-out set in the format of --training_path under the same flags (rows, or one token stream with "
+                  "--stateful), scored with the model in eval mode at every evaluation step (--evaluate_every and the last step); "
+                  "logged as val_loss, val_accuracy and, with --next_token, val_perplexity",
+    "valid_synthetic": "N held-out samples of the --synthetic task (the same chain or class centres, drawn by a generator of "
+                       "their own; --stateful: a stream of N segments), scored as --valid_path",
     "per_step_labels": "Label every time step (sequence labelling): labels [B,T], loss and accuracy over the real positions; "
                        "a CSV row is k*in_features values followed by k labels",
 }

@@ -30,6 +30,9 @@ int ts_xent_rows(const float*, const long long*, float*, float*, float*, int*, i
 int ts_flat_adam(float*, const float*, float*, float*, void*, long long, float, float, float, float, float, float,
                  cudaStream_t, int*, long long, const float*);
 int ts_flat_sgd(float*, const float*, void*, long long, float, float, float, cudaStream_t, long long, const float*);
+int ts_flat_asgd(float*, const float*, float*, int*, void*, long long, float, float, float, cudaStream_t, long long, const float*);
+int ts_flat_average(const float*, float*, int*, long long, cudaStream_t);
+int ts_flat_swap(float*, float*, void*, long long, cudaStream_t);
 long long ts_flat_grad_norm_scratch(long long);
 int ts_flat_grad_norm(const float*, const float*, long long, float, float, long long, float, double*, float*, cudaStream_t);
 int ts_cast_bf16(const float*, void*, long long, cudaStream_t);
@@ -812,6 +815,37 @@ void flat_sgd(Tensor p, const Tensor& g, std::optional<Tensor> shadow, double lr
   check(ts_flat_sgd(p.data_ptr<float>(), g.data_ptr<float>(), shadow.has_value() ? shadow->data_ptr() : nullptr,
                     p.numel(), lr, wd, gscale, stream(), (long long)wd_numel, clip_ptr(clip, p)), "flat_sgd");
 }
+static int* avg_ptr(Tensor& avg, const Tensor& p) {
+  TORCH_CHECK(avg.is_cuda() && avg.scalar_type() == torch::kInt32 && avg.numel() == 2 && avg.is_contiguous() &&
+              avg.device() == p.device(), "avg must be a contiguous int32 [2] {on, k} tensor on p's device");
+  return avg.data_ptr<int>();
+}
+// flat_sgd's update of p and the shadow, then, when avg[0] (on) is set, k = ++avg[1] and ax += (p - ax) * mu_k (ASGD, t0 = 0)
+void flat_asgd(Tensor p, const Tensor& g, Tensor ax, Tensor avg, std::optional<Tensor> shadow, double lr, double wd, double gscale,
+               int64_t wd_numel, std::optional<Tensor> clip) {
+  chk_cuda(p, "p"); chk_cuda(g, "g"); chk_cuda(ax, "ax");
+  c10::cuda::CUDAGuard gd(p.device());
+  TORCH_CHECK(p.numel() == g.numel() && p.numel() == ax.numel(), "numel mismatch");
+  check(ts_flat_asgd(p.data_ptr<float>(), g.data_ptr<float>(), ax.data_ptr<float>(), avg_ptr(avg, p),
+                     shadow.has_value() ? shadow->data_ptr() : nullptr, p.numel(), lr, wd, gscale, stream(), (long long)wd_numel,
+                     clip_ptr(clip, p)), "flat_asgd");
+}
+// the averaging half of flat_asgd alone (p already updated)
+void flat_average(const Tensor& p, Tensor ax, Tensor avg) {
+  chk_cuda(p, "p"); chk_cuda(ax, "ax");
+  c10::cuda::CUDAGuard gd(p.device());
+  TORCH_CHECK(p.numel() == ax.numel(), "numel mismatch");
+  check(ts_flat_average(p.data_ptr<float>(), ax.data_ptr<float>(), avg_ptr(avg, p), p.numel(), stream()), "flat_average");
+}
+// p <-> ax in place, shadow = bf16(new p)
+void flat_swap(Tensor p, Tensor ax, std::optional<Tensor> shadow) {
+  chk_cuda(p, "p"); chk_cuda(ax, "ax");
+  c10::cuda::CUDAGuard gd(p.device());
+  TORCH_CHECK(p.numel() == ax.numel(), "numel mismatch");
+  TORCH_CHECK(!shadow.has_value() || (shadow->scalar_type() == torch::kBFloat16 && shadow->numel() == p.numel()), "shadow");
+  check(ts_flat_swap(p.data_ptr<float>(), ax.data_ptr<float>(), shadow.has_value() ? shadow->data_ptr() : nullptr, p.numel(),
+                     stream()), "flat_swap");
+}
 // out = {||g_total||_2, min(max_norm / (norm + 1e-6), 1)} with g_total = g * gscale + wd * p over [0, wd_numel) (-1: all) and
 // g * gscale beyond; scratch: float64 [flat_grad_norm_scratch(n)], zeroed before its first use (each call leaves its ticket 0).
 void flat_grad_norm(const Tensor& g, const Tensor& p, Tensor out, Tensor scratch, double max_norm, double wd, double gscale,
@@ -1130,6 +1164,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("wd_numel") = -1, py::arg("clip") = py::none());
   m.def("flat_sgd", &flat_sgd, py::arg("p"), py::arg("g"), py::arg("shadow"), py::arg("lr"), py::arg("wd"), py::arg("gscale"),
         py::arg("wd_numel") = -1, py::arg("clip") = py::none());
+  m.def("flat_asgd", &flat_asgd, py::arg("p"), py::arg("g"), py::arg("ax"), py::arg("avg"), py::arg("shadow"), py::arg("lr"),
+        py::arg("wd"), py::arg("gscale"), py::arg("wd_numel") = -1, py::arg("clip") = py::none());
+  m.def("flat_average", &flat_average, py::arg("p"), py::arg("ax"), py::arg("avg"));
+  m.def("flat_swap", &flat_swap, py::arg("p"), py::arg("ax"), py::arg("shadow"));
   m.def("flat_grad_norm", &flat_grad_norm, py::arg("g"), py::arg("p"), py::arg("out"), py::arg("scratch"), py::arg("max_norm"),
         py::arg("wd") = 0.0, py::arg("gscale") = 1.0, py::arg("wd_numel") = -1);
   m.def("flat_grad_norm_scratch", [](int64_t n) { return ts_flat_grad_norm_scratch((long long)n); });

@@ -1,5 +1,5 @@
-// K-OPT: ONE launch over the flat fp32 master buffer (Adam, TF-1.0 "epsilon-hat" formulation, or SGD) that
-// also refreshes the bf16 shadow the tensor-core kernels read.  Replaces the reference's one ApplyAdam
+// K-OPT: ONE launch over the flat fp32 master buffer (Adam, TF-1.0 "epsilon-hat" formulation, SGD, or SGD with the ASGD
+// average of the iterates) that also refreshes the bf16 shadow the tensor-core kernels read.  Replaces the reference's one ApplyAdam
 // kernel per variable (14*L+2 launches per step; original src/rnn.py:207,224).
 // Memory-bound: 16 B vector loads/stores, grid = 132 SMs (H100) x 8 resident CTAs, grid-stride.
 #include "ts_common.cuh"
@@ -66,6 +66,17 @@ __global__ void __launch_bounds__(256) flat_adam_kernel(float4* __restrict__ p, 
   }
 }
 
+// p -= lr * coef * (g * gscale + wd * p): the one SGD expression of flat_sgd_kernel and flat_asgd_kernel (inlined into both, so
+// the compiler contracts it the same way in each)
+template <bool CLIP>
+TS_DEVICE float4 sgd_update(float4 pv, float4 gv, float lr, float wdi, float gscale, float coef) {
+  pv.x -= lr * clipped<CLIP>(gv.x * gscale + wdi * pv.x, coef);
+  pv.y -= lr * clipped<CLIP>(gv.y * gscale + wdi * pv.y, coef);
+  pv.z -= lr * clipped<CLIP>(gv.z * gscale + wdi * pv.z, coef);
+  pv.w -= lr * clipped<CLIP>(gv.w * gscale + wdi * pv.w, coef);
+  return pv;
+}
+
 template <bool CLIP>
 __global__ void __launch_bounds__(256) flat_sgd_kernel(float4* __restrict__ p, const float4* __restrict__ g,
                                                        uint2* __restrict__ shadow, size_t n4, float lr, float wd,
@@ -74,14 +85,75 @@ __global__ void __launch_bounds__(256) flat_sgd_kernel(float4* __restrict__ p, c
   float coef = 1.f;
   if constexpr (CLIP) coef = clip[1];
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += stride) {
-    float4 pv = p[i], gv = g[i];
-    const float wdi = i < wd_n4 ? wd : 0.f;
-    pv.x -= lr * clipped<CLIP>(gv.x * gscale + wdi * pv.x, coef);
-    pv.y -= lr * clipped<CLIP>(gv.y * gscale + wdi * pv.y, coef);
-    pv.z -= lr * clipped<CLIP>(gv.z * gscale + wdi * pv.z, coef);
-    pv.w -= lr * clipped<CLIP>(gv.w * gscale + wdi * pv.w, coef);
+    const float4 pv = sgd_update<CLIP>(p[i], g[i], lr, i < wd_n4 ? wd : 0.f, gscale, coef);
     p[i] = pv;
     if (shadow) shadow[i] = pack_bf16x4(pv);
+  }
+}
+
+// ---- ASGD (torch.optim.ASGD with lambd = 0, t0 = 0): ax, the running average of the iterates -----------------------------
+// avg = device int32 {on, k}.  bump_avg_kernel runs right before every averaging kernel (k counts the averaged updates, so a
+// captured graph stays exact across replays; switching on is a fill_ of {1, 0} outside the graph).  The k-th averaged update
+// uses torch's indexing mu_k = 1 / max(1, k - 1): k <= 2 copies ax = p, then ax = ax + (p - ax) * mu_k with each operation
+// rounded on its own (torch's order, no FMA), mu_k = fp32(1.0 / (k - 1)) as torch rounds the Python double.
+__global__ void bump_avg_kernel(int* avg) {
+  if (avg[0]) avg[1] += 1;
+}
+
+TS_DEVICE float average_mu(int k) { return k <= 2 ? 1.f : (float)(1.0 / (double)(k - 1)); }
+
+TS_DEVICE float4 average_step(float4 a, float4 pv, int k, float mu) {
+  if (k <= 2) return pv;
+  a.x = __fadd_rn(a.x, __fmul_rn(__fsub_rn(pv.x, a.x), mu));
+  a.y = __fadd_rn(a.y, __fmul_rn(__fsub_rn(pv.y, a.y), mu));
+  a.z = __fadd_rn(a.z, __fmul_rn(__fsub_rn(pv.z, a.z), mu));
+  a.w = __fadd_rn(a.w, __fmul_rn(__fsub_rn(pv.w, a.w), mu));
+  return a;
+}
+
+// flat_sgd_kernel's p and shadow (bit for bit: the same sgd_update), plus the average when on; with on == 0 ax is neither
+// read nor written.  22 B per element against SGD's 14 B.
+template <bool CLIP>
+__global__ void __launch_bounds__(256) flat_asgd_kernel(float4* __restrict__ p, const float4* __restrict__ g,
+                                                        float4* __restrict__ ax, const int* __restrict__ avg,
+                                                        uint2* __restrict__ shadow, size_t n4, float lr, float wd,
+                                                        float gscale, size_t wd_n4, const float* __restrict__ clip) {
+  size_t stride = (size_t)gridDim.x * blockDim.x;
+  float coef = 1.f;
+  if constexpr (CLIP) coef = clip[1];
+  const bool on = avg[0] != 0;
+  const int k = avg[1];
+  const float mu = average_mu(k);
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += stride) {
+    const float4 pv = sgd_update<CLIP>(p[i], g[i], lr, i < wd_n4 ? wd : 0.f, gscale, coef);
+    p[i] = pv;
+    if (shadow) shadow[i] = pack_bf16x4(pv);
+    if (on) ax[i] = average_step(k <= 2 ? pv : ax[i], pv, k, mu);
+  }
+}
+
+// The averaging half alone, for updates that ran elsewhere (the fused allreduce's bucket kernels): 12 B per element.
+__global__ void __launch_bounds__(256) flat_average_kernel(const float4* __restrict__ p, float4* __restrict__ ax,
+                                                           const int* __restrict__ avg, size_t n4) {
+  if (!avg[0]) return;
+  const int k = avg[1];
+  const float mu = average_mu(k);
+  size_t stride = (size_t)gridDim.x * blockDim.x;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += stride) {
+    const float4 pv = p[i];
+    ax[i] = average_step(k <= 2 ? pv : ax[i], pv, k, mu);
+  }
+}
+
+// p <-> ax in place, shadow = bf16(new p): evaluating the average is swap, score, swap (two swaps restore all three bit for bit).
+__global__ void __launch_bounds__(256) flat_swap_kernel(float4* __restrict__ p, float4* __restrict__ ax, uint2* __restrict__ shadow,
+                                                        size_t n4) {
+  size_t stride = (size_t)gridDim.x * blockDim.x;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += stride) {
+    const float4 a = ax[i], pv = p[i];
+    p[i] = a;
+    ax[i] = pv;
+    if (shadow) shadow[i] = pack_bf16x4(a);
   }
 }
 
@@ -179,6 +251,32 @@ extern "C" int ts_flat_sgd(float* p, const float* g, void* shadow, long long n, 
   auto kern = clip ? flat_sgd_kernel<true> : flat_sgd_kernel<false>;
   kern<<<grid_for(n4), 256, 0, st>>>((float4*)p, (const float4*)g, (uint2*)shadow, n4, lr, wd, gscale,
                                      wd_n < 0 ? n4 : (size_t)wd_n / 4, clip);
+  return (int)cudaGetLastError();
+}
+
+extern "C" int ts_flat_asgd(float* p, const float* g, float* ax, int* avg, void* shadow, long long n, float lr, float wd,
+                            float gscale, cudaStream_t st, long long wd_n, const float* clip) {
+  if (n % 4 || (wd_n >= 0 && wd_n % 4)) return -2;
+  size_t n4 = (size_t)n / 4;
+  bump_avg_kernel<<<1, 1, 0, st>>>(avg);
+  auto kern = clip ? flat_asgd_kernel<true> : flat_asgd_kernel<false>;
+  kern<<<grid_for(n4), 256, 0, st>>>((float4*)p, (const float4*)g, (float4*)ax, avg, (uint2*)shadow, n4, lr, wd, gscale,
+                                     wd_n < 0 ? n4 : (size_t)wd_n / 4, clip);
+  return (int)cudaGetLastError();
+}
+
+extern "C" int ts_flat_average(const float* p, float* ax, int* avg, long long n, cudaStream_t st) {
+  if (n % 4) return -2;
+  size_t n4 = (size_t)n / 4;
+  bump_avg_kernel<<<1, 1, 0, st>>>(avg);
+  flat_average_kernel<<<grid_for(n4), 256, 0, st>>>((const float4*)p, (float4*)ax, avg, n4);
+  return (int)cudaGetLastError();
+}
+
+extern "C" int ts_flat_swap(float* p, float* ax, void* shadow, long long n, cudaStream_t st) {
+  if (n % 4) return -2;
+  size_t n4 = (size_t)n / 4;
+  flat_swap_kernel<<<grid_for(n4), 256, 0, st>>>((float4*)p, (float4*)ax, (uint2*)shadow, n4);
   return (int)cudaGetLastError();
 }
 

@@ -319,15 +319,25 @@ def next_batch(train_x, train_y, batch_size: int = 10, shuffle: bool = True,
 # ------------------------------------------------------------------------------------------------
 # synthetic sequences (benchmark configs of BASELINE.json)
 # ------------------------------------------------------------------------------------------------
+# the generator key that draws a held-out set (``valid_of`` below) instead of a training set: same task, other samples
+VALID_DRAWS = 0x76616C
+
+
 def synthetic_sequences(n: int, seq_len: int, in_features: int, num_classes: int, seed: int = 0,
-                        dtype=np.float32, variable_length: bool = False):
+                        dtype=np.float32, variable_length: bool = False, valid_of: int = 0):
     """Class-dependent gaussian sequences (learnable, so loss curves are meaningful).  -> ``(x, y)``.
+
+    ``valid_of = m > 0``: ``n`` held-out samples of the task ``m`` training samples were drawn from (the same class centres),
+    labels and noise from a generator of their own.
 
     ``variable_length``: -> ``(x, y, lengths)``, the same ``x`` / ``y`` with per-sample lengths drawn uniformly from
     ``[max(1, seq_len // 4), seq_len]`` (int32) by a generator of their own, and the padded steps zeroed."""
     rng = np.random.default_rng(seed)
-    y = rng.integers(0, num_classes, size=n).astype(np.int64)
+    y = rng.integers(0, num_classes, size=valid_of or n).astype(np.int64)
     centers = rng.standard_normal((num_classes, in_features)).astype(np.float32)
+    if valid_of:
+        rng = np.random.default_rng([seed, VALID_DRAWS])
+        y = rng.integers(0, num_classes, size=n).astype(np.int64)
     if seq_len > 1:
         x = rng.standard_normal((n, seq_len, in_features), dtype=np.float32) * 0.5 + centers[y][:, None, :]
     else:
@@ -336,13 +346,13 @@ def synthetic_sequences(n: int, seq_len: int, in_features: int, num_classes: int
         return x.astype(dtype), y
     if seq_len < 2:
         raise ValueError("variable-length sequences need seq_len >= 2")
-    lengths = synthetic_lengths(n, seq_len, seed)
+    lengths = synthetic_lengths(n, seq_len, seed, valid=bool(valid_of))
     x[np.arange(seq_len)[None, :] >= lengths[:, None]] = 0.0
     return x.astype(dtype), y, lengths
 
 
 def synthetic_per_step(n: int, seq_len: int, in_features: int, num_classes: int, seed: int = 0, dtype=np.float32,
-                       variable_length: bool = False):
+                       variable_length: bool = False, valid_of: int = 0):
     """A learnable sequence-labelling task (``--per_step_labels``): every step has its own class, and its input is drawn around
     that class's centre.  -> ``(x [n, T, D], y int64 [n, T])``, plus ``lengths`` with ``variable_length`` (the lengths of
     ``synthetic_lengths``, padded steps zeroed and labelled 0).  Drawn by a generator of its own: the draws of
@@ -351,11 +361,13 @@ def synthetic_per_step(n: int, seq_len: int, in_features: int, num_classes: int,
         raise ValueError("per-step labels need seq_len >= 2")
     rng = np.random.default_rng([seed, 0x737465])
     centers = rng.standard_normal((num_classes, in_features)).astype(np.float32)
+    if valid_of:                                       # held out: the same centres, other samples
+        rng = np.random.default_rng([seed, 0x737465, VALID_DRAWS])
     y = rng.integers(0, num_classes, size=(n, seq_len)).astype(np.int64)
     x = rng.standard_normal((n, seq_len, in_features), dtype=np.float32) * 0.5 + centers[y]
     if not variable_length:
         return x.astype(dtype), y
-    lengths = synthetic_lengths(n, seq_len, seed)
+    lengths = synthetic_lengths(n, seq_len, seed, valid=bool(valid_of))
     pad = np.arange(seq_len)[None, :] >= lengths[:, None]
     x[pad] = 0.0
     y[pad] = 0
@@ -363,7 +375,7 @@ def synthetic_per_step(n: int, seq_len: int, in_features: int, num_classes: int,
 
 
 def synthetic_tokens(n: int, seq_len: int, vocab_size: int, num_classes: int, seed: int = 0, variable_length: bool = False,
-                     per_step_labels: bool = False, p_class: float = 0.5, ids_per_class: int = 8):
+                     per_step_labels: bool = False, p_class: float = 0.5, ids_per_class: int = 8, valid_of: int = 0):
     """A learnable token task (``--vocab_size``): every class owns ``ids_per_class`` indicative ids (distinct while the vocabulary
     allows); a step draws from its class's ids with probability ``p_class`` and from a Zipf(1.1) background over the whole
     vocabulary otherwise.  The class of a step is its sample's label, or with ``per_step_labels`` the step's own label.
@@ -376,6 +388,8 @@ def synthetic_tokens(n: int, seq_len: int, vocab_size: int, num_classes: int, se
     own = rng.permutation(vocab_size)[:num_classes * ids_per_class] if vocab_size >= num_classes * ids_per_class \
         else rng.integers(0, vocab_size, size=num_classes * ids_per_class)
     own = own.reshape(num_classes, ids_per_class)
+    if valid_of:                                       # held out: the same indicative ids, other samples
+        rng = np.random.default_rng([seed, 0x746F6B, VALID_DRAWS])
     if per_step_labels:
         y = rng.integers(0, num_classes, size=(n, seq_len)).astype(np.int64)
         cls = y
@@ -389,7 +403,7 @@ def synthetic_tokens(n: int, seq_len: int, vocab_size: int, num_classes: int, se
     if variable_length:
         if seq_len < 2:
             raise ValueError("variable-length sequences need seq_len >= 2")
-        lengths = synthetic_lengths(n, seq_len, seed)
+        lengths = synthetic_lengths(n, seq_len, seed, valid=bool(valid_of))
         pad = np.arange(seq_len)[None, :] >= lengths[:, None]
         x[pad] = 0
         if per_step_labels:
@@ -417,7 +431,7 @@ def next_token_chain(vocab_size: int, seed: int = 0) -> np.ndarray:
     return ((base[:, None] + np.arange(4)[None, :] * step[:, None]) % vocab_size).astype(np.int64)
 
 
-def synthetic_next_token(n: int, seq_len: int, vocab_size: int, seed: int = 0, variable_length: bool = False):
+def synthetic_next_token(n: int, seq_len: int, vocab_size: int, seed: int = 0, variable_length: bool = False, valid_of: int = 0):
     """A learnable language (``--next_token``): a fixed sparse first-order Markov chain over the ids (``next_token_chain``), so
     the achievable loss is known in closed form (``NEXT_TOKEN_ENTROPY``).  ``n`` walks of ``seq_len + 1`` ids from a uniform
     start -> ``(x int32 [n, T] = ids 0..T-1, y int64 [n, T] = ids 1..T)``, plus ``lengths`` with ``variable_length`` (those of
@@ -426,7 +440,7 @@ def synthetic_next_token(n: int, seq_len: int, vocab_size: int, seed: int = 0, v
     if seq_len < 2:
         raise ValueError("next-token sequences need seq_len >= 2")
     succ = next_token_chain(vocab_size, seed)
-    rng = np.random.default_rng([seed, 0x6E7874, 1])
+    rng = np.random.default_rng([seed, 0x6E7874, 1] + ([VALID_DRAWS] if valid_of else []))   # held out: the same chain
     tok = np.empty((n, seq_len + 1), dtype=np.int64)
     tok[:, 0] = rng.integers(0, vocab_size, size=n)
     pick = rng.choice(4, size=(n, seq_len), p=NEXT_TOKEN_PROBS)
@@ -435,7 +449,7 @@ def synthetic_next_token(n: int, seq_len: int, vocab_size: int, seed: int = 0, v
     x, y = tok[:, :-1].astype(np.int32), tok[:, 1:].copy()
     if not variable_length:
         return x, y
-    lengths = synthetic_lengths(n, seq_len, seed)
+    lengths = synthetic_lengths(n, seq_len, seed, valid=bool(valid_of))
     pad = np.arange(seq_len)[None, :] >= lengths[:, None]
     x[pad] = 0
     y[pad] = 0
@@ -511,13 +525,13 @@ def token_stream(rows: Sequence[Sequence[str]], vocab_size: int) -> np.ndarray:
     return np.asarray(ids, dtype=np.int64)
 
 
-def synthetic_stream(n: int, seq_len: int, vocab_size: int, seed: int = 0) -> np.ndarray:
+def synthetic_stream(n: int, seq_len: int, vocab_size: int, seed: int = 0, valid: bool = False) -> np.ndarray:
     """``--stateful --synthetic n``: one walk of ``n * seq_len + 1`` ids of the chain of ``synthetic_next_token``
     (``next_token_chain``) from a uniform start -> int64.  Drawn by a generator of its own: the other synthetic tasks are
-    untouched."""
+    untouched.  ``valid``: a held-out walk of the same chain, from a generator of its own."""
     succ = next_token_chain(vocab_size, seed)
     m = n * seq_len + 1
-    rng = np.random.default_rng([seed, 0x6E7874, 2])
+    rng = np.random.default_rng([seed, 0x6E7874, 2] + ([VALID_DRAWS] if valid else []))
     tok = np.empty(m, dtype=np.int64)
     tok[0] = rng.integers(0, vocab_size)
     pick = rng.choice(4, size=m - 1, p=NEXT_TOKEN_PROBS)
@@ -571,27 +585,44 @@ def load_stream(cfg, n_synthetic: int = 0) -> np.ndarray:
     return token_stream(read_dataset_from_path(cfg.training_path), cfg.vocab_size)
 
 
-def synthetic_lengths(n: int, seq_len: int, seed: int = 0) -> np.ndarray:
-    """Per-sample lengths, uniform in ``[max(1, seq_len // 4), seq_len]``, int32, from a generator seeded apart from the data's."""
-    rng = np.random.default_rng([seed, 0x6C656E])
+def synthetic_lengths(n: int, seq_len: int, seed: int = 0, valid: bool = False) -> np.ndarray:
+    """Per-sample lengths, uniform in ``[max(1, seq_len // 4), seq_len]``, int32, from a generator seeded apart from the data's
+    (``valid``: the lengths of a held-out set, from a generator of their own)."""
+    rng = np.random.default_rng([seed, 0x6C656E] + ([VALID_DRAWS] if valid else []))
     return rng.integers(max(1, seq_len // 4), seq_len + 1, size=n).astype(np.int32)
 
 
-def synthetic(cfg, n: int, seed: int):
+def synthetic(cfg, n: int, seed: int, valid_of: int = 0):
     """``n`` synthetic samples of the task the flags of ``cfg`` select -> ``(x, y, lengths)``; ``lengths`` is None unless
-    ``cfg.variable_length``."""
+    ``cfg.variable_length``.  ``valid_of = m > 0``: ``n`` held-out samples of the task ``synthetic(cfg, m, seed)`` draws from."""
     if getattr(cfg, "next_token", False):
-        x, y, *lengths = synthetic_next_token(n, cfg.seq_len, cfg.vocab_size, seed=seed, variable_length=cfg.variable_length)
+        x, y, *lengths = synthetic_next_token(n, cfg.seq_len, cfg.vocab_size, seed=seed, variable_length=cfg.variable_length,
+                                              valid_of=valid_of)
     elif cfg.vocab_size > 0:
         x, y, *lengths = synthetic_tokens(n, cfg.seq_len, cfg.vocab_size, cfg.num_classes, seed=seed,
-                                          variable_length=cfg.variable_length, per_step_labels=cfg.per_step_labels)
+                                          variable_length=cfg.variable_length, per_step_labels=cfg.per_step_labels,
+                                          valid_of=valid_of)
     elif cfg.per_step_labels:
         x, y, *lengths = synthetic_per_step(n, cfg.seq_len, cfg.in_features, cfg.num_classes, seed=seed,
-                                            variable_length=cfg.variable_length)
+                                            variable_length=cfg.variable_length, valid_of=valid_of)
     else:
         x, y, *lengths = synthetic_sequences(n, cfg.seq_len, cfg.in_features, cfg.num_classes, seed=seed,
-                                             variable_length=cfg.variable_length)
+                                             variable_length=cfg.variable_length, valid_of=valid_of)
     return x, y, (lengths[0] if lengths else None)
+
+
+def load_validation(cfg, n_train: int):
+    """The held-out set of ``--valid_path`` / ``--valid_synthetic``, or None: a token stream with ``--stateful``, else
+    ``(x, y, lengths)`` as ``parse_rows`` gives them.  ``--valid_synthetic`` draws from the task of the first training shard
+    (``n_train`` samples of ``--synthetic`` at ``--seed``)."""
+    if cfg.valid_synthetic:
+        if cfg.stateful:
+            return synthetic_stream(cfg.valid_synthetic, cfg.seq_len, cfg.vocab_size, cfg.seed, valid=True)
+        return synthetic(cfg, cfg.valid_synthetic, cfg.seed, valid_of=max(1, n_train))
+    if cfg.valid_path:
+        rows = read_dataset_from_path(cfg.valid_path)
+        return token_stream(rows, cfg.vocab_size) if cfg.stateful else parse_rows(rows, cfg)
+    return None
 
 
 # ------------------------------------------------------------------------------------------------

@@ -8,6 +8,8 @@ This is what ``bench.py``, ``__graft_entry__.smoke`` and the per-replica trainer
     norm = eng.grad_norm()           # --clip_grad_norm: the last step's gradient norm before clipping (None without)
     ar_tar = eng.activation_penalties()  # --activation_reg / --temporal_activation_reg: the last step's (AR, TAR) (None without)
     loss = eng.step(x, y, reset=k == 0)  # --stateful: batch k of a pass continues every stream from the state batch k-1 ended in
+    with eng.averaged_weights(): ...     # --optimizer asgd / ntasgd: score the average of the iterates, then train on
+    eng.finish_averaging()               # end of training: the average becomes the weights, before the replica average / export
 
 One step replaces the reference's ``sess.run([train_op, loss], feed_dict=...)`` (original src/rnn.py:264-267):
 H2D feed, forward, backward, 14·L+2 ApplyAdam launches, D2H loss.  With ``cuda_graph=True`` the whole step is
@@ -15,6 +17,7 @@ captured once and replayed (launch-bound inner loops belong in CUDA graphs, not 
 """
 from __future__ import annotations
 
+import contextlib
 from typing import Optional
 
 import torch
@@ -83,6 +86,7 @@ class TrainEngine:
         self._bound = {}                        # (x ptr, y ptr, lengths ptr, shape) -> (graph captured on those buffers, its loss)
         self._bound_keepalive = []
         self.steps_done = 0
+        self._averaging_finished = False
         # every dropout (between layers, output, input, embedding rows, weight drop): the masks are keyed on (seed, partition)
         # and on the number of training steps this engine has completed - a counter of its own, device-resident on the GPU (a
         # captured graph advances it; the optimizer's step_dev is bumped before backward by the fused allreduce and never by
@@ -162,6 +166,8 @@ class TrainEngine:
         params.after_big_launch(flush=True)                 # queued, but no big kernel followed (generic path / last layer)
         for b in plan[state["next"]:]:
             comm.launch_bucket(b["lo"], b["hi"])
+        if getattr(self.optimizer, "ax", None) is not None:
+            self.optimizer.average_()                       # asgd / ntasgd: the buckets updated p; every rank averages all of it
 
     def _step_eager(self, x: torch.Tensor, y: torch.Tensor, lengths: Optional[torch.Tensor] = None) -> torch.Tensor:
         if self.stateful:
@@ -290,6 +296,31 @@ class TrainEngine:
         if force or (cfg.sync_every and self.steps_done % cfg.sync_every == 0):
             self.comm.average_params_(self.flat, cfg.average_scope)
 
+    @contextlib.contextmanager
+    def averaged_weights(self):
+        """``--optimizer asgd / ntasgd``: inside the block the model holds the average of the iterates (``ax``), once averaging
+        is on and has averaged at least one update; the raw weights are back, bit for bit, when it exits.  A no-op otherwise."""
+        opt = self.optimizer
+        swap = opt.ax is not None and opt.has_average()
+        if swap:
+            opt.swap_average()
+        try:
+            yield swap
+        finally:
+            if swap:
+                opt.swap_average()
+
+    def finish_averaging(self) -> bool:
+        """End of training with ``--optimizer asgd / ntasgd``: put the average into the weights (once; the raw last iterate
+        goes to ``ax``), so the replica average, the export and the returned variables are those of the averaged model.  -> whether
+        it swapped."""
+        opt = self.optimizer
+        if opt.ax is None or not opt.has_average() or self._averaging_finished:
+            return False
+        opt.swap_average()
+        self._averaging_finished = True
+        return True
+
     # ---------------------------------------------------------------------------------------------------
     def capture(self, x: torch.Tensor, y: torch.Tensor, warmup: int = 3, bind=(), lengths: Optional[torch.Tensor] = None):
         """Capture fwd+bwd+update into one CUDA graph (static shapes).  Adam's bias correction is derived in-kernel from
@@ -311,6 +342,7 @@ class TrainEngine:
         snap = {"data": self.flat.data.clone(), "step_count": opt.step_count,
                 "m": None if opt.m is None else opt.m.clone(), "v": None if opt.v is None else opt.v.clone(),
                 "step_dev": None if opt.step_dev is None else opt.step_dev.clone(),
+                "ax": None if opt.ax is None else opt.ax.clone(), "avg": None if opt.avg is None else opt.avg.clone(),
                 "dropout_step": self.model.rnn.dropout_step.clone(),
                 "state": None if not self.stateful else [(h.clone(), c.clone()) for h, c in self.state + self.state_prev]}
         s = torch.cuda.Stream()
@@ -339,6 +371,8 @@ class TrainEngine:
                 opt.m.copy_(snap["m"]); opt.v.copy_(snap["v"])
             if snap["step_dev"] is not None:
                 opt.step_dev.copy_(snap["step_dev"])
+            if snap["ax"] is not None:                      # capturing does not advance the average either
+                opt.ax.copy_(snap["ax"]); opt.avg.copy_(snap["avg"])
             self.model.rnn.dropout_step.copy_(snap["dropout_step"])
             if snap["state"] is not None:                   # capturing does not advance the carry
                 for (h, c), (h1, c1) in zip(self.state + self.state_prev, snap["state"]):

@@ -19,6 +19,8 @@ def flat_step(opt, grad_scale: float = 1.0) -> None:
     if opt.kind == "adam":
         E.flat_adam(fl.data, fl.grad, opt.m, opt.v, shadow, opt.lr, opt.beta1, opt.beta2, opt.eps,
                     opt.weight_decay, grad_scale, opt.step_dev, opt.wd_numel, clip)
+    elif opt.ax is not None:                # asgd / ntasgd: the SGD update and the average in one pass
+        E.flat_asgd(fl.data, fl.grad, opt.ax, opt.avg, shadow, opt.lr, opt.weight_decay, grad_scale, opt.wd_numel, clip)
     else:
         E.flat_sgd(fl.data, fl.grad, shadow, opt.lr, opt.weight_decay, grad_scale, opt.wd_numel, clip)
 

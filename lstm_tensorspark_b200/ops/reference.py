@@ -576,3 +576,13 @@ def sgd_step_(p, g, lr: float, weight_decay: float = 0.0, grad_scale: float = 1.
         gg = gg * clip_coef
     p.add_(gg, alpha=-lr)
     return p
+
+
+def asgd_average_(ax, p, k: int):
+    """The k-th (k = 1, 2, ...) averaging step of ``torch.optim.ASGD(lambd=0, t0=0)``, in torch's indexing and order: k <= 2
+    copies ``ax = p``; after that ``ax += (p - ax) * mu_k`` with ``mu_k = fp32(1 / (k - 1))``, each operation rounded on its own
+    (no fused multiply-add).  So ``ax_k = mean(p_2 .. p_k)`` for k >= 2."""
+    if k <= 2:
+        return ax.copy_(p)
+    mu = torch.tensor(1.0 / (k - 1), dtype=torch.float32, device=ax.device)
+    return ax.add_(p.sub(ax).mul_(mu))

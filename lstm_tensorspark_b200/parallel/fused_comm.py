@@ -172,6 +172,7 @@ class FusedComm(TorchDistComm):
         """Whole-message gradient sync + update in one launch (no overlap)."""
         self.begin_grad_step(flat, optimizer)
         self.launch_bucket(0, flat.padded_numel, force=force)
+        optimizer.average_()            # asgd / ntasgd: the bucket kernel updated p (all of it on every rank); average it
 
     # -- bucketed gradient sync: a bucket's allreduce + update is launched as soon as its gradients are final ----------
     def begin_grad_step(self, flat: FlatParams, optimizer):

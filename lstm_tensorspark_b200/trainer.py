@@ -28,7 +28,7 @@ from .models.classifier import SequenceClassifier
 from .models.recurrent.lstm import clear_weight_decay_collection
 from .ops import functional as F
 from .ops.loss import report_accuracy, report_loss
-from .ops.optim import FlatOptimizer
+from .ops.optim import FlatOptimizer, nonmono_trigger
 from .parallel.comm import Communicator, make_communicator
 from .utils import checkpoint as ckpt
 from .utils import metrics as M
@@ -82,11 +82,61 @@ def _check_device_errors(device: torch.device, comm) -> None:
         comm.check_errors()
 
 
+def score_rows(model, xs: torch.Tensor, ys: torch.Tensor, ls: Optional[torch.Tensor], bs: int) -> Tuple[float, float, int]:
+    """Loss and accuracy of the rows ``xs`` / ``ys`` (per-sample lengths ``ls`` or None) with ``model`` in eval mode, in batches of
+    ``bs`` rows: the full batches (static shapes for the kernels), then the tail as the last ``bs`` rows, counting only the ones
+    not seen yet; --per_step_labels weighs each batch by its number of counted positions.  -> (loss, accuracy, count)."""
+    n = xs.shape[0]
+    windows = [(lo, 0) for lo in range(0, n - bs + 1, bs)] + ([(n - bs, bs - n % bs)] if n % bs else [])
+    loss_sum, correct, count = 0.0, 0, 0
+    for lo, first in windows:
+        loss, ok, cnt = model.score(xs[lo:lo + bs], ys[lo:lo + bs], None if ls is None else ls[lo:lo + bs], first)
+        loss_sum += float(loss) * int(cnt); correct += int(ok); count += int(cnt)
+    return loss_sum / count, correct / count, count
+
+
+def score_stream(model, xs: torch.Tensor, ys: torch.Tensor, B: int, tail: int, dtype: torch.dtype) -> Tuple[float, float, int]:
+    """--stateful: loss and accuracy of a stream laid out by ``data.stream_layout(..., tail=True)`` as ``B`` parallel streams,
+    with ``model`` in eval mode, the state carried from segment to segment from zero (``tail``: the length of the last, short
+    segment in every row, 0 = none).  Uses the model's own state buffers only.  -> (loss, accuracy, positions)."""
+    device = xs.device
+    segs = xs.shape[0] // B
+    tail_lengths = torch.full((B,), tail, dtype=torch.int32, device=device) if tail else None
+    state = model.rnn.zero_state(B, dtype, device)
+    loss_sum, correct, count = 0.0, 0, 0
+    for k in range(segs):
+        lengths = tail_lengths if (tail and k == segs - 1) else None
+        loss, ok, cnt = model.score(xs[k * B:(k + 1) * B], ys[k * B:(k + 1) * B], lengths, state=state)
+        state = model.rnn.final_state()
+        loss_sum += float(loss) * int(cnt); correct += int(ok); count += int(cnt)
+    return loss_sum / count, correct / count, count
+
+
+def validation_scorer(valid, cfg: Config, batch_size: int, device: torch.device, dtype: torch.dtype):
+    """The held-out set ``valid`` (``data.load_validation``) copied to the device once -> ``score(model) -> (loss, accuracy,
+    count)`` in batches of ``batch_size`` (``score_rows`` / ``score_stream``), or None without a set."""
+    if valid is None:
+        return None
+    if cfg.stateful:
+        x, y, tail = D.stream_layout(valid, batch_size, cfg.seq_len, tail=True)
+        xs = torch.as_tensor(x).to(device=device, dtype=D.input_dtype(cfg))
+        ys = torch.as_tensor(y).to(device)
+        return lambda model: score_stream(model, xs, ys, batch_size, tail, dtype)
+    x, y, lengths = valid
+    if x.shape[0] < batch_size:
+        raise ValueError(f"the validation set has {x.shape[0]} samples, fewer than the batch size {batch_size} it is scored in")
+    xs = torch.as_tensor(x).to(device=device, dtype=D.input_dtype(cfg))
+    ys = torch.as_tensor(y).to(device)
+    ls = None if lengths is None else torch.as_tensor(lengths).to(device=device, dtype=torch.int32)
+    return lambda model: score_rows(model, xs, ys, ls, batch_size)
+
+
 def train_rnn(partition, cfg: Config, rank: int = 0, world_size: int = 1, comm: Optional[Communicator] = None,
               train_optimizer: Optional[Callable] = None, standalone: bool = False,
-              run_stamp: Optional[str] = None, defer_average: bool = False) -> Optional[ReplicaResult]:
+              run_stamp: Optional[str] = None, defer_average: bool = False, valid=None) -> Optional[ReplicaResult]:
     """Train one replica on one shard.  ``partition`` = ``(key, rows)`` (distributed) or a list of rows
-    (standalone) or ``(key, (x ndarray, y ndarray))`` for pre-parsed / synthetic data."""
+    (standalone) or ``(key, (x ndarray, y ndarray))`` for pre-parsed / synthetic data.  ``valid``: the held-out set
+    (``data.load_validation``), scored at every evaluation step, or None."""
     comm = comm or Communicator(0, 1)
     prefix_name = "lstm_no_spark" if standalone else "spark_lstm"
     tag = "RNN-LSTM"
@@ -176,6 +226,8 @@ def train_rnn(partition, cfg: Config, rank: int = 0, world_size: int = 1, comm: 
                                    "a checkpoint is missing or stale on some rank")
 
     max_steps = compute_max_steps(cfg, batch_size, loader.per_epoch)
+    score_valid = validation_scorer(valid, cfg, batch_size, device, dtype)
+    averages = optimizer.ax is not None
 
     use_bar = (trange is not None) and (rank == 0) and not cfg.quiet
     total_steps = trange(start_step, max_steps) if use_bar else range(start_step, max_steps)
@@ -234,12 +286,30 @@ def train_rnn(partition, cfg: Config, rank: int = 0, world_size: int = 1, comm: 
 
         if is_eval:
             _check_device_errors(device, comm)       # sticky in-kernel timeout flags (dead peer / stalled grid barrier)
+            val = None
+            if score_valid is not None:
+                with M.nvtx_range("validate", cfg.nvtx), torch.no_grad(), eng.averaged_weights():
+                    model.eval()                                     # no dropout, raw W_h; the average once there is one
+                    try:
+                        val = score_valid(model)
+                    finally:
+                        model.train()
+                if cfg.optimizer == "ntasgd":
+                    fire = nonmono_trigger(optimizer.nonmono_history, val[0], cfg.nonmono, optimizer.averaging)
+                    if world_size > 1:                               # every replica switches at the same step
+                        fire = comm.max_scalar(1.0 if fire else 0.0) > 0
+                    optimizer.nonmono_history.append(val[0])
+                    if fire:
+                        optimizer.start_averaging()
+                        if rank == 0 and not cfg.quiet:
+                            print(f"{tag} - NT-ASGD: validation loss {val[0]:.6f} did not improve on the best before the last "
+                                  f"{cfg.nonmono} validations: averaging the weights from step {step + 1} on")
             with M.nvtx_range("eval_ckpt", cfg.nvtx):
                 saver.save(model.reference_state_dict(), global_step=step,
                            extra={"rank": rank, "world_size": world_size, "partition_key": partition_key,
                                   "loss": t_loss, "config": cfg.__dict__},
                            opt_state={"optimizer": comm.optimizer_state(optimizer), "loader": loader.state_dict(),
-                                      "stateful": cfg.stateful,
+                                      "stateful": cfg.stateful, "batch_size": batch_size,
                                       "state": None if not cfg.stateful else
                                       [(h.detach().cpu().clone(), c.detach().cpu().clone()) for h, c in eng.carried_state()]})
                 model.eval()                                         # no dropout while scoring
@@ -261,6 +331,15 @@ def train_rnn(partition, cfg: Config, rank: int = 0, world_size: int = 1, comm: 
                 if cfg.next_token:
                     extra["perplexity"] = math.exp(t_loss)
                     sink.add("perplexity", extra["perplexity"])
+                if val is not None:                                  # the held-out set, scored before this checkpoint
+                    extra.update(val_loss=val[0], val_accuracy=val[1])
+                    if cfg.next_token:
+                        extra["val_perplexity"] = math.exp(val[0]) if val[0] < 700 else float("inf")
+                if averages:
+                    extra.update(averaging=int(optimizer.averaging), averaged_steps=optimizer.averaged_steps)
+                for k in ("val_loss", "val_accuracy", "val_perplexity", "averaging", "averaged_steps"):
+                    if k in extra:
+                        sink.add(k, extra[k])
                 sink.flush(step)
                 jlog.write(step=step, loss=t_loss, acc=t_acc, rank=rank, **extra)
             if use_bar:
@@ -269,6 +348,7 @@ def train_rnn(partition, cfg: Config, rank: int = 0, world_size: int = 1, comm: 
 
     # ---- the cross-replica average (src/rnn.py:393-407) ------------------------------------------------
     with M.nvtx_range("final_param_avg", cfg.nvtx):
+        averaged = eng.finish_averaging()       # asgd / ntasgd: the average is the model that is averaged and exported
         if not defer_average:                   # oversubscribed ranks average all their replicas at once (_rank_main)
             eng.maybe_average(force=True)
     device_ms = timer.stop_ms()
@@ -283,7 +363,7 @@ def train_rnn(partition, cfg: Config, rank: int = 0, world_size: int = 1, comm: 
     records = [(k, [[t.detach().float().cpu().clone() for t in layer] if isinstance(layer, list)
                     else layer.detach().float().cpu().clone() for layer in v])
                for k, v in model.rnn.map_data_by_key()]
-    result = ReplicaResult(partition_key=partition_key, rank=rank, records=records,
+    result = ReplicaResult(partition_key=partition_key, rank=rank, records=records, averaged=averaged,
                            variables=model.reference_state_dict(), loss=t_loss, acc=t_acc, steps=n_steps,
                            seconds=end_time, device_ms=device_ms, samples=samples, model_save_dir=model_save_dir)
     if defer_average:
@@ -299,7 +379,7 @@ def train_rnn(partition, cfg: Config, rank: int = 0, world_size: int = 1, comm: 
 # ====================================================================================================
 # job driver
 # ====================================================================================================
-def _rank_main(rank: int, world_size: int, cfg: Config, shards, standalone: bool):
+def _rank_main(rank: int, world_size: int, cfg: Config, shards, standalone: bool, valid=None):
     device = resolve_device(cfg, rank)
     comm = make_communicator(cfg.comm, rank, world_size, device, cfg.timeout_s, clip_synced_grads=cfg.clips_synced_grads())
     try:
@@ -307,9 +387,9 @@ def _rank_main(rank: int, world_size: int, cfg: Config, shards, standalone: bool
         mine = list(shards[rank::world_size]) if shards is not None else [None]
         if len(shards or []) <= world_size:
             shard = shards[rank] if shards is not None else None
-            res = train_rnn(shard, cfg, rank, world_size, comm, standalone=standalone, run_stamp=stamp)
+            res = train_rnn(shard, cfg, rank, world_size, comm, standalone=standalone, run_stamp=stamp, valid=valid)
         else:
-            res = _train_oversubscribed(mine, len(shards), cfg, rank, world_size, comm, stamp)
+            res = _train_oversubscribed(mine, len(shards), cfg, rank, world_size, comm, stamp, valid)
         comm.barrier()
         if res is not None and rank != 0:
             # only rank 0's records are needed by the driver (all replicas hold the same average)
@@ -319,14 +399,14 @@ def _rank_main(rank: int, world_size: int, cfg: Config, shards, standalone: bool
         comm.close()
 
 
-def _train_oversubscribed(mine, n_partitions: int, cfg: Config, rank: int, world_size: int, comm, stamp: str):
+def _train_oversubscribed(mine, n_partitions: int, cfg: Config, rank: int, world_size: int, comm, stamp: str, valid=None):
     """More partitions than workers (the reference runs ``--partitions`` tasks on ``local[workers]`` executor threads,
     original src/rnn.py:355-358: each worker takes its tasks in turn).  Every partition is still its own replica
     with its own checkpoint directory; a rank trains its partitions one after the other and the one-shot average at the
     end of the job (src/rnn.py:393-407) runs over ALL partitions: local sum -> cross-rank sum -> / partitions."""
     results = []
     for shard in mine:
-        results.append(train_rnn(shard, cfg, rank, 1, None, standalone=False, run_stamp=stamp, defer_average=True))
+        results.append(train_rnn(shard, cfg, rank, 1, None, standalone=False, run_stamp=stamp, defer_average=True, valid=valid))
     results = [r for r in results if r is not None]
     if not results:
         return None
@@ -389,10 +469,25 @@ def load_shards(cfg: Config, world_size: int, standalone: bool):
     return D.text_to_partitions(cfg.training_path, world_size, shuffle=True, seed=cfg.seed, remainder=cfg.remainder)
 
 
+def _averaged_variables(cfg: Config, variables, ax: torch.Tensor, batch_size: int):
+    """The variables (reference names) of the model whose flat buffer is ``ax``: ``variables`` laid out as training laid them
+    out (at its ``batch_size``), with every value taken from ``ax``."""
+    model = SequenceClassifier(cfg, batch_size=batch_size, device="cpu")
+    model.load_reference_state_dict(variables, strict=False)
+    flat = model.build_flat()
+    if flat.data.numel() != ax.numel():
+        raise ValueError(f"the checkpoint's weight average holds {ax.numel()} values, the model it belongs to {flat.data.numel()}: "
+                         "give the flags it was trained with")
+    with torch.no_grad():
+        flat.data.copy_(ax)
+    return model.reference_state_dict()
+
+
 def _find_trained_model(cfg: Config, standalone: bool):
     """--resume <file | dir>, else <output_path>/averaged_model.pt (distributed job), else the latest checkpoint under
     --checkpoint_path.  -> (variables in the reference's names, description, the flags the file records
-    (``utils.checkpoint.recorded_settings``))."""
+    (``utils.checkpoint.recorded_settings``), "averaged" | "raw").  A training checkpoint whose optimizer state holds a weight
+    average (--optimizer asgd / ntasgd, averaging on, k >= 1) gives the average's variables, as training evaluates it."""
     src = cfg.resume
     if not src and not standalone and cfg.output_path and os.path.isfile(os.path.join(cfg.output_path, "averaged_model.pt")):
         src = os.path.join(cfg.output_path, "averaged_model.pt")
@@ -402,14 +497,19 @@ def _find_trained_model(cfg: Config, standalone: bool):
         src = os.path.join(src, "averaged_model.pt")
     if src and os.path.isfile(src) and src.endswith(".pt"):
         blob = torch.load(src, map_location="cpu", weights_only=False)
-        return blob["variables"], src, ckpt.recorded_settings(blob.get("meta") or {})
+        meta = blob.get("meta") or {}
+        return blob["variables"], src, ckpt.recorded_settings(meta), meta.get("weights", "raw")
     if src and os.path.isdir(src):
         if ckpt.latest_checkpoint(src) is None and os.path.isdir(os.path.join(src, "0")):
             src = os.path.join(src, "0")
         last = ckpt.latest_checkpoint(src)
         if last:
-            variables, meta, _ = ckpt.load(last)
-            return variables, last, ckpt.recorded_settings(meta)
+            variables, meta, opt_state = ckpt.load(last)
+            sd = (opt_state or {}).get("optimizer") or {}
+            if sd.get("ax") is not None and int(sd.get("on", 0)) and int(sd.get("k", 0)) >= 1:
+                variables = _averaged_variables(cfg, variables, sd["ax"], int(opt_state.get("batch_size") or cfg.batch_size))
+                return variables, last, ckpt.recorded_settings(meta), "averaged"
+            return variables, last, ckpt.recorded_settings(meta), "raw"
     raise FileNotFoundError(f"--mode {cfg.mode}: no trained model found (give --resume <averaged_model.pt | checkpoint dir>)")
 
 
@@ -418,7 +518,7 @@ def _load_trained_model(cfg: Config, found, batch_size: int, device: torch.devic
     (``SequenceClassifier.check_compatible``).  The reference's trainable initial state is one row PER BATCH ROW
     ([batch_size, H], src/models/recurrent/lstm.py:24-33): at another batch size every row starts from the mean learned row."""
     from .engine import TrainEngine
-    variables, src, settings = found
+    variables, src, settings, _weights = found
     eng = TrainEngine(cfg, 0, 1, Communicator(0, 1), batch_size=batch_size, device=device, dtype=dtype)
     eng.model.eval()                                    # no dropout
     shapes = {k: tuple(v.shape) for k, v in eng.model.named_reference_variables()}
@@ -452,18 +552,12 @@ def evaluate_job(cfg: Config, standalone: bool = False) -> Dict:
     xs = torch.as_tensor(x).to(device=device, dtype=D.input_dtype(cfg))
     ys = torch.as_tensor(y).to(device)
     ls = None if lengths is None else torch.as_tensor(lengths).to(device=device, dtype=torch.int32)
-    # full batches (static shapes for the kernels), then the tail as the last `bs` rows, counting only the ones not seen yet;
-    # --per_step_labels weighs each batch by its number of counted positions
-    windows = [(lo, 0) for lo in range(0, n - bs + 1, bs)] + ([(n - bs, bs - n % bs)] if n % bs else [])
-    loss_sum, correct, count = 0.0, 0, 0
     start = time.time()
-    for lo, first in windows:
-        loss, ok, cnt = eng.model.score(xs[lo:lo + bs], ys[lo:lo + bs], None if ls is None else ls[lo:lo + bs], first)
-        loss_sum += float(loss) * int(cnt); correct += int(ok); count += int(cnt)
+    loss, accuracy, count = score_rows(eng.model, xs, ys, ls, bs)
     out = {"mode": "eval", "model": src, "samples": n}
     if eng.model.per_step:
         out["positions"] = count
-    out.update(loss=loss_sum / count, accuracy=correct / count, seconds=time.time() - start)
+    out.update(loss=loss, accuracy=accuracy, seconds=time.time() - start, weights=found[3])
     if cfg.next_token:
         out["perplexity"] = math.exp(out["loss"])
     if not cfg.quiet:
@@ -490,18 +584,10 @@ def _evaluate_stream(cfg: Config, found) -> Dict:
     model = eng.model
     xs = torch.as_tensor(x).to(device=device, dtype=D.input_dtype(cfg))
     ys = torch.as_tensor(y).to(device)
-    segs = x.shape[0] // B
-    tail_lengths = torch.full((B,), tail, dtype=torch.int32, device=device) if tail else None
-    state = model.rnn.zero_state(B, eng.dtype, device)
-    loss_sum, correct, count = 0.0, 0, 0
     start = time.time()
-    for k in range(segs):
-        lengths = tail_lengths if (tail and k == segs - 1) else None
-        loss, ok, cnt = model.score(xs[k * B:(k + 1) * B], ys[k * B:(k + 1) * B], lengths, state=state)
-        state = model.rnn.final_state()
-        loss_sum += float(loss) * int(cnt); correct += int(ok); count += int(cnt)
+    loss, accuracy, count = score_stream(model, xs, ys, B, tail, eng.dtype)
     out = {"mode": "eval", "model": src, "stream": int(len(stream)), "streams": B, "positions": count,
-           "loss": loss_sum / count, "accuracy": correct / count, "seconds": time.time() - start}
+           "loss": loss, "accuracy": accuracy, "seconds": time.time() - start, "weights": found[3]}
     out["perplexity"] = math.exp(out["loss"])
     if not cfg.quiet:
         print(("RNN-LSTM - eval: model {model}, a stream of {stream} ids in {streams} streams, {positions} positions, "
@@ -552,7 +638,7 @@ def generate_job(cfg: Config, standalone: bool = False) -> Dict:
     path = os.path.join(cfg.output_path or ".", "generated.csv")
     with open(path, "w") as f:
         f.writelines(",".join(str(int(v)) for v in row) + "\n" for row in tokens)
-    out = {"mode": "generate", "model": src, "prompts": n, "tokens": int(tokens.size), "seconds": seconds,
+    out = {"mode": "generate", "model": src, "weights": found[3], "prompts": n, "tokens": int(tokens.size), "seconds": seconds,
            "tokens_per_s": tokens.size / max(seconds, 1e-9), "mean_logprob": float(logprob.mean()), "temperature": cfg.temperature,
            "top_k": cfg.top_k, "top_p": cfg.top_p, "output": path}
     if cfg.synthetic:
@@ -582,13 +668,18 @@ def run_job(cfg: Config, standalone: bool = False) -> Dict:
         if cfg.sync_mode == "grad_allreduce" or (cfg.sync_mode == "param_avg" and cfg.sync_every):
             raise ValueError(f"--partitions {cfg.partitions} > {world_size} workers needs the one-shot parameter average "
                              "(--sync_mode param_avg --sync_every 0): replicas that take turns cannot sync every step")
+        if cfg.optimizer == "ntasgd":
+            raise ValueError(f"--optimizer ntasgd with --partitions {cfg.partitions} > {world_size} workers: replicas that take "
+                             "turns cannot decide together when averaging starts (use --optimizer asgd, or one worker per partition)")
         sys.stderr.write(f"RNN-LSTM - warning: {n_shards} partitions on {world_size} workers: each worker trains its "
                          "partitions in turn (round-robin), the final average runs over all partitions\n")
     if not cfg.quiet:
         print("Total workers: ", f"[{world_size}]")
     shards = load_shards(cfg, n_shards, standalone)
+    # the held-out set: every rank scores the same one (--valid_synthetic: of the first shard's task)
+    valid = D.load_validation(cfg, cfg.synthetic // n_shards if cfg.synthetic else 0)
     start = time.time()
-    results = launch(_rank_main, world_size, args=(cfg, shards, standalone))
+    results = launch(_rank_main, world_size, args=(cfg, shards, standalone, valid))
     total = time.time() - start
     res0 = next((r for r in results if r is not None and "records" in r), None)
     if res0 is not None and cfg.output_path:
@@ -597,7 +688,8 @@ def run_job(cfg: Config, standalone: bool = False) -> Dict:
                                   "hidden_units": cfg.hidden_units, "pooling": cfg.pooling,
                                   "attention_units": cfg.attention_units, "vocab_size": cfg.vocab_size,
                                   "next_token": cfg.next_token, "stateful": cfg.stateful,
-                                  "tie_embeddings": cfg.tie_embeddings, "seconds": total})
+                                  "tie_embeddings": cfg.tie_embeddings, "seconds": total,
+                                  "weights": "averaged" if cfg.optimizer in ("asgd", "ntasgd") and res0.get("averaged") else "raw"})
     if not cfg.quiet:
         print("RNN-LSTM - Total Processing Time {}s".format(total))
     return {"results": results, "seconds": total, "world_size": world_size, "partitions": n_shards}
