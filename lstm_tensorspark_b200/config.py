@@ -26,6 +26,9 @@ ATTENTION_UNITS_DEFAULT = 128
 NUM_CLASSES_DEFAULT = 3
 MAX_NEW_TOKENS_DEFAULT = 32
 TEMPERATURE_DEFAULT = 1.0
+# AWD-LSTM's pointer.py defaults (tuned there for WikiText-2)
+CACHE_THETA_DEFAULT = 0.6625523432485668
+CACHE_LAMBDA_DEFAULT = 0.12785920428335693
 
 
 @dataclass
@@ -86,6 +89,10 @@ class Config:
     temperature: float = TEMPERATURE_DEFAULT      # --mode generate: sample from softmax(logits / temperature); 0 = greedy
     top_k: int = 0                      # --mode generate: sample from the k most likely classes only (ties at the k-th kept); 0 = off
     top_p: float = 1.0                  # --mode generate: then from the smallest top set of tempered mass >= P (nucleus); 1 = off
+    cache_window: int = 0               # --mode eval --next_token --stateful: mix a continuous cache pointer over each stream's last
+                                        # W hidden states into the scored probability (Grave et al. 2017); 0 = off
+    cache_theta: float = CACHE_THETA_DEFAULT    # the cache's score scale: s_j = theta (h_p . h_j)
+    cache_lambda: float = CACHE_LAMBDA_DEFAULT  # the cache's mixture weight: p = (1 - lambda) p_model + lambda p_cache
     dtype: str = "auto"                 # auto: bf16 on cuda, fp32 on cpu
     device: str = "auto"                # auto | cpu | cuda
     backend: str = "auto"               # auto | cuda_ext (hand-written sm_90a kernels) | torch
@@ -324,7 +331,29 @@ class Config:
                 if getattr(self, flag) != default:
                     warnings.warn(f"--{flag} {getattr(self, flag)} has no effect with --temperature 0: greedy decoding takes the "
                                   "arg-max, which every filter keeps")
+        self._validate_cache()
         return self
+
+    def _validate_cache(self) -> None:
+        if self.cache_window < 0:
+            raise ValueError(f"--cache_window must be an integer >= 0 (0 = off), got {self.cache_window}")
+        if not (math.isfinite(self.cache_theta) and self.cache_theta >= 0):
+            raise ValueError(f"--cache_theta must be a finite number >= 0, got {self.cache_theta}")
+        if not (0 <= self.cache_lambda < 1):
+            raise ValueError(f"--cache_lambda must be in [0, 1), got {self.cache_lambda}: at 1 a label absent from the window "
+                             "would cost an infinite loss")
+        coefs = [f"--{f} {getattr(self, f)}" for f, d in (("cache_theta", CACHE_THETA_DEFAULT), ("cache_lambda", CACHE_LAMBDA_DEFAULT))
+                 if getattr(self, f) != d]
+        if self.mode != "eval":
+            if self.cache_window > 0 or coefs:
+                warnings.warn(f"{', '.join(([f'--cache_window {self.cache_window}'] if self.cache_window > 0 else []) + coefs)} "
+                              f"has no effect with --mode {self.mode}: the cache pointer scores --mode eval --stateful only")
+            return
+        if self.cache_window > 0 and not (self.next_token and self.stateful):
+            raise ValueError(f"--cache_window {self.cache_window} needs --next_token --stateful: the cache holds the earlier "
+                             "positions of each token stream")
+        if self.cache_window == 0 and coefs:
+            warnings.warn(f"{', '.join(coefs)} has no effect without --cache_window W > 0")
 
 
 def _str2bool(v) -> bool:
@@ -362,6 +391,12 @@ _HELP = {
     "top_p": "--mode generate: nucleus sampling, after --top_k: sample only from the classes with the largest logits whose "
              "share of softmax(logits / temperature) first reaches P (ties at the cut are kept); 1 = off.  The reported "
              "log-probabilities stay under the full softmax",
+    "cache_window": "--mode eval --next_token --stateful: score with a continuous cache pointer (Grave et al. 2017, AWD-LSTM's "
+                    "pointer.py): p(y) = (1 - lambda) p_model(y) + lambda p_cache(y), p_cache the softmax of theta (h_p . h_j) over "
+                    "the stream's last W positions j, summed over those whose next id is y; loss and perplexity are then the "
+                    "mixture's and loss_model / perplexity_model the model's alone.  0 = off",
+    "cache_theta": "--cache_window: the scale theta of the cache's scores (finite, >= 0; pointer.py's default)",
+    "cache_lambda": "--cache_window: the cache's mixture weight lambda, in [0, 1) (pointer.py's default)",
     "checkpoint_path": "Directory where to save network model and logs",
     "clip_grad_norm": "Clip the gradient by its global L2 norm to this value before the update, as "
                       "torch.nn.utils.clip_grad_norm_ (0 = off); the norm includes the --weight_decay term and, with "

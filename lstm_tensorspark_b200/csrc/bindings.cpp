@@ -95,6 +95,14 @@ int ts_embed_bwd(const void*, int, const int*, const int*, int, int, int, int, f
                  const unsigned int*, const int*, const unsigned int*, cudaStream_t);
 int ts_embed_bwd_launches();
 const char* ts_last_error();
+int ts_cache_key_tile();
+int ts_cache_chunks(int, int, int, int);
+int ts_cache_combine_blocks(int);
+int ts_cache_pointer(const void*, const void*, const int*, const long long*, const float*, const int*, int, int, int, int, int, long long,
+                     float, float, int, int, void*, void*, unsigned int*, float*, float*, cudaStream_t);
+int ts_cache_append(const void*, void*, int*, const long long*, int, int, long long, int, long long, cudaStream_t);
+int ts_cache_label_logprob_parts(const void*, const float*, const long long*, float*, int, int, int, int, cudaStream_t);
+int ts_cache_label_logprob_logits(const float*, const long long*, float*, int, int, int, cudaStream_t);
 }
 
 namespace {
@@ -311,6 +319,85 @@ Tensor act_reg_bwd(const std::optional<Tensor>& dh, const std::optional<Tensor>&
                        lengths_ptr(lengths, B, h), g.data_ptr<float>(), (int)T, (int)B, (int)H, is_bf16(h), ds, dd, dst.data_ptr(),
                        stream()), "act_reg_bwd");
   return dst;
+}
+
+// ---- continuous cache pointer (csrc/cache_pointer.cu) -----------------------------------------------------------------
+// h [T,B,H] the segment's top-layer outputs (bf16 / fp32, packed), keys [B,Cap,H] the per-stream ring in h's dtype (the segment
+// already appended), klab int32 [B,Cap], labels int64 [B,T], logp_model fp32 [T·B] (time-major rows), lengths int32 [B] or None;
+// P0: positions of each stream before this segment.  tc: the tensor-core kernel (bf16, H % 64 == 0), else the generic one.
+// -> logp fp32 [T·B] (the mixture's log p(y), 0 at uncounted positions), sums fp32 [2] {sum -log p, sum -log p_model}.
+void cache_ring_check(const Tensor& h, const Tensor& keys, const Tensor& klab, const Tensor& labels) {
+  chk_cuda(h, "h"); chk_cuda(keys, "keys"); chk_cuda(klab, "klab"); chk_cuda(labels, "labels");
+  TORCH_CHECK(h.dim() == 3 && keys.dim() == 3 && keys.size(0) == h.size(1) && keys.size(2) == h.size(2) &&
+              keys.scalar_type() == h.scalar_type() && keys.device() == h.device(), "cache: keys [B,Cap,H] in h's dtype");
+  is_bf16(h);
+  TORCH_CHECK(keys.size(1) % ts_cache_key_tile() == 0, "cache: the ring's capacity must be a multiple of ", ts_cache_key_tile());
+  TORCH_CHECK(klab.scalar_type() == torch::kInt32 && klab.dim() == 2 && klab.size(0) == keys.size(0) && klab.size(1) == keys.size(1),
+              "cache: klab int32 [B,Cap]");
+  TORCH_CHECK(labels.scalar_type() == torch::kInt64 && labels.dim() == 2 && labels.size(0) == h.size(1) && labels.size(1) == h.size(0),
+              "cache: labels int64 [B,T]");
+  TORCH_CHECK(keys.numel() < (int64_t(1) << 40) && h.size(0) * h.size(1) < (int64_t(1) << 31), "cache: too large");
+}
+
+std::vector<Tensor> cache_pointer(const Tensor& h, const Tensor& keys, const Tensor& klab, const Tensor& labels, const Tensor& logp_model,
+                                  const std::optional<Tensor>& lengths, int64_t W, int64_t P0, double theta, double lambda, bool tc) {
+  cache_ring_check(h, keys, klab, labels);
+  const int64_t T = h.size(0), B = h.size(1), H = h.size(2), Cap = keys.size(1);
+  chk_cuda(logp_model, "logp_model");
+  TORCH_CHECK(logp_model.scalar_type() == torch::kFloat32 && logp_model.numel() == T * B, "cache: logp_model fp32 [T*B]");
+  TORCH_CHECK(W >= 1 && Cap >= W + T && P0 >= 0, "cache: W >= 1, Cap >= W + T, P0 >= 0");
+  TORCH_CHECK(std::isfinite(theta) && theta >= 0 && lambda >= 0 && lambda < 1, "cache: theta finite >= 0, lambda in [0, 1)");
+  TORCH_CHECK(!tc || (h.scalar_type() == torch::kBFloat16 && H % 64 == 0), "cache: the tensor-core path needs bf16 and H % 64 == 0");
+  c10::cuda::CUDAGuard g(h.device());
+  auto fo = h.options().dtype(torch::kFloat32);
+  const int nch = ts_cache_chunks((int)T, (int)B, (int)H, (int)W);
+  auto part = torch::empty({B * T * nch * 4}, fo);
+  auto block_sums = torch::empty({ts_cache_combine_blocks((int)(T * B)) * 2}, fo);
+  auto ticket = torch::zeros({1}, fo.dtype(torch::kInt32));
+  auto logp = torch::empty({T * B}, fo), sums = torch::empty({2}, fo);
+  check(ts_cache_pointer(h.data_ptr(), keys.data_ptr(), klab.data_ptr<int>(), (const long long*)labels.data_ptr<int64_t>(),
+                         logp_model.data_ptr<float>(), lengths_ptr(lengths, B, h), (int)T, (int)B, (int)H, (int)W, (int)Cap, (long long)P0,
+                         (float)theta, (float)lambda, is_bf16(h), tc ? 1 : 0, part.data_ptr(), block_sums.data_ptr(),
+                         (unsigned int*)ticket.data_ptr<int>(), logp.data_ptr<float>(), sums.data_ptr<float>(), stream()), "cache_pointer");
+  return {logp, sums};
+}
+
+// Write the segment h [T,B,H] / labels [B,T] into the ring at positions P0 .. P0 + T - 1 (slot = position % Cap).
+void cache_append(const Tensor& h, Tensor keys, Tensor klab, const Tensor& labels, int64_t P0) {
+  cache_ring_check(h, keys, klab, labels);
+  TORCH_CHECK(P0 >= 0 && keys.size(1) >= h.size(0), "cache_append: P0 >= 0 and a ring of at least T slots");
+  c10::cuda::CUDAGuard g(h.device());
+  check(ts_cache_append(h.data_ptr(), keys.data_ptr(), klab.data_ptr<int>(), (const long long*)labels.data_ptr<int64_t>(), (int)h.size(0),
+                        (int)h.size(1), (long long)(h.size(2) * h.element_size()), (int)keys.size(1), (long long)P0, stream()), "cache_append");
+}
+
+// log p_model(y) fp32 [T·B] at every position (time-major rows) from the large-vocabulary head's forward: part (its float4
+// [T·B, vocab_head_parts(C)] scratch) and lse [T·B].  Labels outside [0, C) give 0 (padded positions).
+Tensor cache_label_logprob_parts(const Tensor& part, const Tensor& lse, const Tensor& labels, int64_t C) {
+  chk_cuda(part, "part"); chk_cuda(lse, "lse"); chk_cuda(labels, "labels");
+  TORCH_CHECK(labels.scalar_type() == torch::kInt64 && labels.dim() == 2, "labels int64 [B,T]");
+  const int64_t B = labels.size(0), T = labels.size(1), nt = ts_vocab_head_parts((int)C);
+  TORCH_CHECK(lse.scalar_type() == torch::kFloat32 && lse.numel() == T * B && part.scalar_type() == torch::kFloat32 &&
+              part.numel() >= T * B * nt * 4, "cache_label_logprob_parts: lse fp32 [T*B], part float4 [T*B, parts]");
+  c10::cuda::CUDAGuard g(lse.device());
+  auto logp = torch::empty({T * B}, lse.options());
+  check(ts_cache_label_logprob_parts(part.data_ptr(), lse.data_ptr<float>(), (const long long*)labels.data_ptr<int64_t>(), logp.data_ptr<float>(),
+                                     (int)T, (int)B, (int)C, (int)nt, stream()), "cache_label_logprob_parts");
+  return logp;
+}
+
+// The same from stored fp32 logits [B,T,C] (the per-step head's).
+Tensor cache_label_logprob_logits(const Tensor& logits, const Tensor& labels) {
+  chk_cuda(logits, "logits"); chk_cuda(labels, "labels");
+  TORCH_CHECK(logits.scalar_type() == torch::kFloat32 && logits.dim() == 3, "logits fp32 [B,T,C]");
+  TORCH_CHECK(labels.scalar_type() == torch::kInt64 && labels.dim() == 2 && labels.size(0) == logits.size(0) && labels.size(1) == logits.size(1),
+              "labels int64 [B,T]");
+  const int64_t B = logits.size(0), T = logits.size(1), C = logits.size(2);
+  c10::cuda::CUDAGuard g(logits.device());
+  auto logp = torch::empty({T * B}, logits.options());
+  check(ts_cache_label_logprob_logits(logits.data_ptr<float>(), (const long long*)labels.data_ptr<int64_t>(), logp.data_ptr<float>(), (int)T,
+                                      (int)B, (int)C, stream()), "cache_label_logprob_logits");
+  return logp;
 }
 
 // Weight drop's gradient: dst (+)= src * mask * scale over fp32 [R, H] (R = 4H rows of W_h), the mask of `desc` at time 0, as
@@ -1128,6 +1215,13 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("lstm_pointwise_bwd", &lstm_pointwise_bwd, py::arg("dh_a"), py::arg("dh_b"), py::arg("dc_in"), py::arg("act"), py::arg("c_prev"),
         py::arg("c_new"), py::arg("lengths") = py::none(), py::arg("t") = 0);
   m.def("xent_rows", &xent_rows);
+  m.def("cache_key_tile", []() { return ts_cache_key_tile(); });
+  m.def("cache_chunks", [](int64_t T, int64_t B, int64_t H, int64_t W) { return ts_cache_chunks((int)T, (int)B, (int)H, (int)W); });
+  m.def("cache_pointer", &cache_pointer, py::arg("h"), py::arg("keys"), py::arg("klab"), py::arg("labels"), py::arg("logp_model"),
+        py::arg("lengths"), py::arg("W"), py::arg("P0"), py::arg("theta"), py::arg("lambda_"), py::arg("tc"));
+  m.def("cache_append", &cache_append, py::arg("h"), py::arg("keys"), py::arg("klab"), py::arg("labels"), py::arg("P0"));
+  m.def("cache_label_logprob_parts", &cache_label_logprob_parts, py::arg("part"), py::arg("lse"), py::arg("labels"), py::arg("C"));
+  m.def("cache_label_logprob_logits", &cache_label_logprob_logits, py::arg("logits"), py::arg("labels"));
   m.def("head_fwd", &head_fwd);
   m.def("seq_pool_fwd", &seq_pool_fwd, py::arg("h"), py::arg("lengths"), py::arg("T"), py::arg("mode"), py::arg("alpha"));
   m.def("seq_pool_attn_scores", &seq_pool_attn_scores, py::arg("u"), py::arg("b_a"), py::arg("v"), py::arg("lengths"), py::arg("T"),

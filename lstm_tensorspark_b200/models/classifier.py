@@ -238,14 +238,26 @@ class SequenceClassifier(nn.Module):
         return loss, logits, correct
 
     @torch.no_grad()
-    def score(self, x: torch.Tensor, labels: torch.Tensor, lengths: Optional[torch.Tensor] = None, first: int = 0, state=None):
+    def score(self, x: torch.Tensor, labels: torch.Tensor, lengths: Optional[torch.Tensor] = None, first: int = 0, state=None,
+              cache: Optional[F.CacheHistory] = None):
         """Evaluation without gradients (call in eval mode): -> (mean loss, correct count, count) over rows ``first:`` of the
         batch, device tensors (no host sync); ``state`` as in ``forward``.  The count is of the counted positions with ``--per_step_labels``, of the rows
-        otherwise.  The whole batch runs through the stack, so a tail can be scored in a batch of the usual static shape."""
+        otherwise.  The whole batch runs through the stack, so a tail can be scored in a batch of the usual static shape.
+
+        ``cache``: the continuous cache pointer's history of the batch's streams (``ops.functional.cache_pointer``; a segment of
+        a --stateful stream, ``first = 0``): the segment is appended to it and the loss is the cache mixture's; -> (mean loss,
+        correct count, count, the model's own mean loss).  The correct count stays the model's arg-max."""
         from ..ops import reference as ref
         self.check_labels(labels)
+        if cache is not None and (not self.per_step or first):
+            raise ValueError("the cache pointer scores whole segments of a token stream (--next_token --stateful)")
         if self.per_step:
             h_seq = self.sequence_features(x, lengths, state)
+            if cache is not None:
+                w, class_major = self.head_weights()
+                _loss, correct, n, logp = F.vocab_xent_logprob(h_seq, w, self.head.bias, labels, lengths, class_major=class_major)
+                _lp, sums = F.cache_pointer(h_seq, labels, logp, cache, lengths)
+                return sums[0] / n, correct, n, sums[1] / n
             if F.vocab_head_supported(h_seq, self.cfg.num_classes):
                 # the tail is a mask, not a slice: rows before `first` get length 0, and no [rows, C] array is ever built
                 if first > 0:

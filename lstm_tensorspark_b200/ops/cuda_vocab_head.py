@@ -42,23 +42,30 @@ def _weights_lowp(weights: torch.Tensor, class_major: bool) -> torch.Tensor:
     return wb
 
 
+def _forward(h_seq, weights, bias, labels, lengths, class_major):
+    """The forward launches -> (operands h2, wb, b, lab, ln; the per-tile partials ``part``; lse, loss, correct, N)."""
+    E = ext()
+    T, B, H = h_seq.shape
+    hc = h_seq.detach()
+    h2 = hc.reshape(T * B, H) if hc.is_contiguous() else hc.contiguous().view(T * B, H)
+    wb = _weights_lowp(weights, class_major)
+    b = bias.detach().float().contiguous()
+    lab = labels.long().contiguous()
+    ln = None if lengths is None else lengths.contiguous()
+    C = wb.shape[0 if class_major else 1]
+    part = torch.empty(T * B * E.vocab_head_parts(C) * 4, dtype=torch.float32, device=h2.device)
+    lse, loss, correct, n = E.vocab_head_fwd(h2, wb, bool(class_major), b, lab, ln, T, part)
+    count("vocab_head_fwd")
+    if class_major:
+        count("vocab_head_fwd_tied")
+    return (h2, wb, b, lab, ln), part, (lse, loss, correct, n)
+
+
 class _VocabXentFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, h_seq, weights, bias, labels, lengths, class_major=False):
-        E = ext()
         T, B, H = h_seq.shape
-        hc = h_seq.detach()
-        h2 = hc.reshape(T * B, H) if hc.is_contiguous() else hc.contiguous().view(T * B, H)
-        wb = _weights_lowp(weights, class_major)
-        b = bias.detach().float().contiguous()
-        lab = labels.long().contiguous()
-        ln = None if lengths is None else lengths.contiguous()
-        C = wb.shape[0 if class_major else 1]
-        part = torch.empty(T * B * E.vocab_head_parts(C) * 4, dtype=torch.float32, device=h2.device)
-        lse, loss, correct, n = E.vocab_head_fwd(h2, wb, bool(class_major), b, lab, ln, T, part)
-        count("vocab_head_fwd")
-        if class_major:
-            count("vocab_head_fwd_tied")
+        (h2, wb, b, lab, ln), _part, (lse, loss, correct, n) = _forward(h_seq, weights, bias, labels, lengths, class_major)
         ctx.save_for_backward(h2, wb, b, lab, ln, lse, n)
         ctx.shape, ctx.class_major = (T, B, H), bool(class_major)
         ctx.addrs = (weights.data_ptr(), bias.data_ptr())
@@ -97,6 +104,16 @@ class _VocabXentFn(torch.autograd.Function):
 def vocab_xent_per_step(h_seq, weights, bias, labels, lengths=None, class_major=False):
     """-> (mean loss over the counted positions, correct count, N); see ``ops.functional.vocab_xent_per_step``."""
     return _VocabXentFn.apply(h_seq, weights, bias, labels, lengths, bool(class_major))
+
+
+@torch.no_grad()
+def vocab_xent_logprob(h_seq, weights, bias, labels, lengths=None, class_major=False):
+    """The forward of ``vocab_xent_per_step`` (no gradients) that also gives the model's log-probability at the label of every
+    position, ``log p(y) [T·B]`` in time-major row order, read from the same launch's partials and lse (csrc/cache_pointer.cu)
+    -> (loss, correct, N, log p(y))."""
+    (_h2, wb, _b, lab, _ln), part, (lse, loss, correct, n) = _forward(h_seq, weights, bias, labels, lengths, class_major)
+    logp = ext().cache_label_logprob_parts(part, lse, lab, wb.shape[0 if class_major else 1])
+    return loss.squeeze(0), correct.squeeze(0), n.squeeze(0), logp
 
 
 def _device_int(v, device):

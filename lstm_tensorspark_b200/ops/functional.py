@@ -113,6 +113,84 @@ def vocab_xent_per_step(h_seq, weights, bias, labels, lengths=None, class_major:
     return ref.vocab_xent_per_step(h_seq, w, bias, labels, lengths)
 
 
+@torch.no_grad()
+def vocab_xent_logprob(h_seq, weights, bias, labels, lengths=None, class_major: bool = False):
+    """Evaluation through the per-step head (``vocab_xent_per_step``'s loss, correct count and N, no gradients) that also gives
+    the model's log-probability at the label of every position, ``[T·B]`` fp32 in time-major row order (row t·B + b), for the
+    continuous cache pointer.  The large-vocabulary head reads it from its own forward's partials; the per-step head's
+    path from the logits it stores."""
+    C = weights.shape[0 if class_major else 1]
+    if vocab_head_supported(h_seq, C):
+        from . import cuda_vocab_head
+        return cuda_vocab_head.vocab_xent_logprob(h_seq, weights, bias, labels, lengths, class_major)
+    w = weights.t().contiguous() if class_major else weights
+    logits, loss, correct, n = head_xent_per_step(h_seq, w, bias, labels, lengths)
+    if _use_ext(h_seq):
+        from . import cuda_cache
+        return loss, correct, n, cuda_cache.label_logprob_logits(logits, labels)
+    return loss, correct, n, ref.label_logprob(logits, labels).float()
+
+
+CACHE_KEY_TILE = 128       # keys per tile of csrc/cache_pointer.cu: the ring's capacity is a multiple of it
+
+
+class CacheHistory:
+    """The continuous cache pointer of ``B`` parallel streams (``ops.reference.cache_pointer`` holds the definition): the scale
+    ``theta``, the mixture weight ``lam``, the ``window`` W, and each stream's history, a ring of its last positions' top-layer
+    outputs ``keys [B, Cap, H]`` in the compute dtype and their labels ``key_labels [B, Cap]`` int32 (position j in slot
+    j % Cap), with ``seen`` positions scored so far.  ``Cap`` is ``W + T`` rounded up to 128 (a segment of ``T`` positions is
+    appended before it is scored), so the ring takes ``B · Cap · (H · element size + 4)`` bytes: about 2.1 GB at B = 256,
+    W = 3785, T = 128, H = 1024 in bf16.  An append writes the segment's ``T·B`` rows only; the window never moves."""
+
+    def __init__(self, window: int, theta: float, lam: float, B: int, T: int, H: int, dtype: torch.dtype, device):
+        if window < 1:
+            raise ValueError(f"the cache window must be >= 1, got {window}")
+        self.window, self.theta, self.lam, self.T = int(window), float(theta), float(lam), int(T)
+        cap = -(-(self.window + self.T) // CACHE_KEY_TILE) * CACHE_KEY_TILE
+        self.keys = torch.zeros(B, cap, H, dtype=dtype, device=device)
+        self.key_labels = torch.zeros(B, cap, dtype=torch.int32, device=device)
+        self.seen = 0
+
+    def reset(self) -> None:
+        """Start the streams again: no history."""
+        self.seen = 0
+
+    def append(self, h_seq, labels) -> None:
+        """Write the segment ``h_seq [T,B,H]`` / ``labels [B,T]`` at positions ``seen .. seen + T - 1`` (``seen`` unchanged)."""
+        T = h_seq.shape[0]
+        if T > self.T or tuple(h_seq.shape[1:]) != (self.keys.shape[0], self.keys.shape[2]) or h_seq.dtype != self.keys.dtype:
+            raise ValueError(f"the cache holds segments of at most {self.T} x {self.keys.shape[0]} x {self.keys.shape[2]} "
+                             f"{self.keys.dtype}, got {tuple(h_seq.shape)} {h_seq.dtype}")
+        if _use_ext(h_seq):
+            from . import cuda_cache
+            cuda_cache.append(h_seq, labels, self.keys, self.key_labels, self.seen)
+            return
+        slots = (self.seen + torch.arange(T, device=h_seq.device)) % self.keys.shape[1]
+        self.keys[:, slots] = h_seq.detach().transpose(0, 1)
+        self.key_labels[:, slots] = labels.to(h_seq.device).to(torch.int32)
+
+
+@torch.no_grad()
+def cache_pointer(h_seq, labels, logp_model, history: CacheHistory, lengths=None):
+    """Score one segment of every stream with the continuous cache pointer: append ``h_seq [T,B,H]`` (the top layer's outputs,
+    the queries) and ``labels [B,T]`` to ``history``, mix the model's ``logp_model [T·B]`` (``vocab_xent_logprob``) with the
+    cache's distribution over each position's last ``window`` positions, and advance ``history.seen`` by T.  ``lengths``:
+    optional int32 ``[B]`` counted positions per stream (a tail segment).  -> (log p(y) ``[T·B]``, 0 at uncounted positions;
+    ``[2]`` {sum -log p, sum -log p_model} over the counted positions, both reduced in the same order, so at ``lam = 0`` they
+    are equal).  On the GPU bf16 with ``H % 64 == 0`` runs on the tensor cores, everything else on the generic kernel."""
+    history.append(h_seq, labels)
+    args = (history.keys, history.key_labels, history.seen, history.window, history.theta, history.lam)
+    if _use_ext(h_seq):
+        from . import cuda_cache
+        out = cuda_cache.cache_pointer(h_seq, labels, logp_model, *args, lengths=lengths)
+    else:
+        lp, keep = ref.cache_pointer(h_seq, labels, logp_model, *args, lengths=lengths)
+        lv = logp_model.to(lp.dtype)
+        out = lp, torch.stack([-(lp[keep]).sum(), -(lv[keep]).sum()])
+    history.seen += h_seq.shape[0]
+    return out
+
+
 def vocab_sample(h, weights, bias, temperature: float, seed: int, step, tokens=None, record=None, row0=0, class_major: bool = False,
                  top_k: int = 0, top_p: float = 1.0):
     """Sample the next token of every row from the head's logits ``l = h W + bias`` (``h [B,H]``, ``W [H,C]``) without a host

@@ -451,6 +451,60 @@ def softmax_xent_per_step(logits, labels, lengths=None):
     return torch.nn.functional.cross_entropy(lg, lab, reduction="sum") / n, (lg.argmax(1) == lab).sum(), n
 
 
+def label_logprob(logits, labels):
+    """``logits [B,T,C]``, ``labels [B,T]`` -> ``log softmax(logits)[label]`` ``[T·B]`` in time-major row order (row t·B + b)."""
+    lp = torch.log_softmax(logits, dim=2).gather(2, labels.to(logits.device).long().unsqueeze(2)).squeeze(2)
+    return lp.transpose(0, 1).reshape(-1)
+
+
+# ---- continuous cache pointer (Grave et al. 2017) ----------------------------------------------------------------------
+# The definition is shared with the CUDA kernels (csrc/cache_pointer.cu): change both or neither.
+def cache_ring_positions(capacity: int, end: int, device=None) -> torch.Tensor:
+    """The stream position each ring slot holds once positions ``0 .. end - 1`` have been written to slot ``position % capacity``:
+    the largest ``q < end`` with ``q % capacity == slot``, -1 where none is."""
+    slot = torch.arange(capacity, device=device, dtype=torch.int64)
+    last = end - 1
+    q = last - ((last - slot) % capacity)
+    return torch.where(q >= 0, q, torch.full_like(q, -1))
+
+
+def cache_pointer(h_seq, labels, logp_model, keys, key_labels, seen: int, window: int, theta: float, lam: float, lengths=None):
+    """The continuous cache pointer's log p(y) of one segment of ``B`` streams, in the dtype of ``h_seq`` / ``keys``.
+
+    ``h_seq [T,B,H]``: the segment's top-layer outputs (queries), ``labels [B,T]``: y_p, the id after position p,
+    ``logp_model [T·B]``: the model's log p_v(y_p) in time-major row order, ``keys [B,Cap,H]`` / ``key_labels [B,Cap]``: each
+    stream's ring with the segment already written (position j in slot j % Cap, Cap >= window + T), ``seen``: positions of each
+    stream before the segment, ``lengths``: optional ``[B]`` counted positions per stream (a tail segment).  For the query at
+    absolute position p, J(p) = {j : max(0, p - window) <= j < p}, s_j = theta (h_p . h_j), and
+
+        log p(y_p) = logaddexp(log1p(-lam) + log p_v(y_p), log lam + log sum_{j in J, y_j = y_p} e^{s_j} - log sum_{j in J} e^{s_j})
+
+    (J empty: log p_v(y_p)).  -> (log p ``[T·B]``, 0 at uncounted positions; counted mask ``[T·B]``)."""
+    T, B, _ = h_seq.shape
+    dev = h_seq.device
+    cap = keys.shape[1]
+    if cap < window + T:
+        raise ValueError(f"the ring holds {cap} positions, fewer than the window {window} plus the segment {T}")
+    pos = cache_ring_positions(cap, seen + T, dev)                                       # [Cap]
+    p = seen + torch.arange(T, device=dev, dtype=torch.int64)                             # [T]
+    valid = (pos.view(1, -1) >= (p.view(-1, 1) - window).clamp(min=0)) & (pos.view(1, -1) < p.view(-1, 1))   # [T,Cap]
+    s = theta * torch.einsum("tbh,bch->btc", h_seq, keys.to(h_seq.dtype))                # [B,T,Cap]
+    s = s.masked_fill(~valid.unsqueeze(0), float("-inf"))
+    same = key_labels.to(dev).long().unsqueeze(1) == labels.to(dev).long().unsqueeze(2)  # [B,T,Cap]
+    lz = torch.logsumexp(s, dim=2)                                                        # [B,T]
+    lm = torch.logsumexp(s.masked_fill(~same, float("-inf")), dim=2)
+    lv = logp_model.to(h_seq.dtype).view(T, B).t()
+    empty = ~valid.any(1).view(1, T).expand(B, T)
+    neg_inf = torch.full_like(lv, float("-inf"))
+    a = math.log1p(-lam) + lv
+    c = (math.log(lam) + (lm - lz)) if lam > 0 else neg_inf
+    c = torch.where(torch.isfinite(c), c, neg_inf)
+    lp = torch.where(empty, lv, torch.where(torch.isinf(c), a, torch.logaddexp(a, c)))
+    keep = step_mask(lengths, B, T, device=dev)
+    lp = torch.where(keep, lp, torch.zeros_like(lp))
+    return lp.t().reshape(-1), keep.t().reshape(-1)
+
+
 POOLING_MODES = ("last", "mean", "max", "attention")
 
 

@@ -95,20 +95,32 @@ def score_rows(model, xs: torch.Tensor, ys: torch.Tensor, ls: Optional[torch.Ten
     return loss_sum / count, correct / count, count
 
 
-def score_stream(model, xs: torch.Tensor, ys: torch.Tensor, B: int, tail: int, dtype: torch.dtype) -> Tuple[float, float, int]:
+def score_stream(model, xs: torch.Tensor, ys: torch.Tensor, B: int, tail: int, dtype: torch.dtype,
+                 cache: Optional[F.CacheHistory] = None) -> Tuple[float, ...]:
     """--stateful: loss and accuracy of a stream laid out by ``data.stream_layout(..., tail=True)`` as ``B`` parallel streams,
     with ``model`` in eval mode, the state carried from segment to segment from zero (``tail``: the length of the last, short
-    segment in every row, 0 = none).  Uses the model's own state buffers only.  -> (loss, accuracy, positions)."""
+    segment in every row, 0 = none).  Uses the model's own state buffers only.  -> (loss, accuracy, positions).
+
+    ``cache``: score with the continuous cache pointer (``SequenceClassifier.score``); the history is reset here, so it holds
+    this stream only.  -> (the mixture's loss, accuracy, positions, the model's own loss over the same positions)."""
     device = xs.device
     segs = xs.shape[0] // B
     tail_lengths = torch.full((B,), tail, dtype=torch.int32, device=device) if tail else None
     state = model.rnn.zero_state(B, dtype, device)
-    loss_sum, correct, count = 0.0, 0, 0
+    if cache is not None:
+        cache.reset()
+    loss_sum, model_sum, correct, count = 0.0, 0.0, 0, 0
     for k in range(segs):
         lengths = tail_lengths if (tail and k == segs - 1) else None
-        loss, ok, cnt = model.score(xs[k * B:(k + 1) * B], ys[k * B:(k + 1) * B], lengths, state=state)
+        out = model.score(xs[k * B:(k + 1) * B], ys[k * B:(k + 1) * B], lengths, state=state,
+                          **({} if cache is None else {"cache": cache}))
+        loss, ok, cnt = out[:3]
         state = model.rnn.final_state()
         loss_sum += float(loss) * int(cnt); correct += int(ok); count += int(cnt)
+        if cache is not None:
+            model_sum += float(out[3]) * int(cnt)
+    if cache is not None:
+        return loss_sum / count, correct / count, count, model_sum / count
     return loss_sum / count, correct / count, count
 
 
@@ -584,14 +596,25 @@ def _evaluate_stream(cfg: Config, found) -> Dict:
     model = eng.model
     xs = torch.as_tensor(x).to(device=device, dtype=D.input_dtype(cfg))
     ys = torch.as_tensor(y).to(device)
+    cache = None
+    if cfg.cache_window > 0:
+        H = cfg.hidden_list()[-1] * (2 if cfg.bidirectional else 1)
+        cache = F.CacheHistory(cfg.cache_window, cfg.cache_theta, cfg.cache_lambda, B, T, H, eng.dtype, device)
     start = time.time()
-    loss, accuracy, count = score_stream(model, xs, ys, B, tail, eng.dtype)
+    scored = score_stream(model, xs, ys, B, tail, eng.dtype, cache=cache)
+    loss, accuracy, count = scored[:3]
     out = {"mode": "eval", "model": src, "stream": int(len(stream)), "streams": B, "positions": count,
            "loss": loss, "accuracy": accuracy, "seconds": time.time() - start, "weights": found[3]}
     out["perplexity"] = math.exp(out["loss"])
+    line = ("RNN-LSTM - eval: model {model}, a stream of {stream} ids in {streams} streams, {positions} positions, "
+            "loss {loss:.6f}, accuracy {accuracy:.4f}, perplexity {perplexity:.4f}")
+    if cache is not None:
+        out.update(loss_model=scored[3], perplexity_model=math.exp(scored[3]), cache_window=cfg.cache_window,
+                   cache_theta=cfg.cache_theta, cache_lambda=cfg.cache_lambda)
+        line += (" with the cache pointer (window {cache_window}, theta {cache_theta:g}, lambda {cache_lambda:g}); the model "
+                 "alone: loss {loss_model:.6f}, perplexity {perplexity_model:.4f}")
     if not cfg.quiet:
-        print(("RNN-LSTM - eval: model {model}, a stream of {stream} ids in {streams} streams, {positions} positions, "
-               "loss {loss:.6f}, accuracy {accuracy:.4f}, perplexity {perplexity:.4f}").format(**out))
+        print(line.format(**out))
     if cfg.json_log:
         jl = M.JsonLog(cfg.json_log); jl.write(**out); jl.close()
     return out
