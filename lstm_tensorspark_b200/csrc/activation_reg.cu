@@ -15,6 +15,7 @@
 // squares of its fp32 values (differences of two bf16 values are exact in fp32) in fp64, each CTA sums in a fixed tree, and
 // the last CTA to take a ticket sums the CTA partials in a fixed order and leaves the ticket 0 (flat_grad_norm_kernel's
 // pattern, csrc/multi_tensor_opt.cu).
+#include "launchers.h"
 #include "ts_common.cuh"
 
 namespace {

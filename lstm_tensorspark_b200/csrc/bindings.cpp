@@ -1,7 +1,7 @@
 // Python bindings for the sm_90a kernels (the only translation unit that sees torch headers).
 // Every function validates device / dtype / contiguity, takes the CURRENT torch CUDA stream (so the kernels
 // are stream-ordered with the rest of the step and capturable in CUDA graphs) and forwards raw pointers to the
-// C-ABI launchers defined next to the kernels.
+// C-ABI launchers defined next to the kernels and declared in launchers.h.
 #include <torch/extension.h>
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
@@ -13,97 +13,9 @@
 #include <string>
 #include <vector>
 
-using torch::Tensor;
+#include "launchers.h"
 
-extern "C" {
-int ts_lstm_pointwise_fwd(const void*, const float*, const float*, void*, float*, void*, int, int, int, cudaStream_t, const void*,
-                          const int*, int);
-int ts_transpose01_rows(const void*, void*, int, int, long long, cudaStream_t);
-int ts_lstm_seq_cluster_probe(int);
-int ts_lstm_seq_config(int, int, int, int, int*, int);
-int ts_transpose2d_b16(const void*, void*, int, int, cudaStream_t);
-int ts_colsum_bf16(const void*, float*, void*, int, int, int, int, int, int, cudaStream_t);
-long long ts_colsum_scratch_bytes(int, int);
-int ts_lstm_pointwise_bwd(const void*, const float*, const float*, const void*, const float*, const float*, void*,
-                          float*, int, int, int, cudaStream_t, const int*, int, float*);
-int ts_xent_rows(const float*, const long long*, float*, float*, float*, int*, int, int, int, cudaStream_t);
-int ts_flat_adam(float*, const float*, float*, float*, void*, long long, float, float, float, float, float, float,
-                 cudaStream_t, int*, long long, const float*);
-int ts_flat_sgd(float*, const float*, void*, long long, float, float, float, cudaStream_t, long long, const float*);
-int ts_flat_asgd(float*, const float*, float*, int*, void*, long long, float, float, float, cudaStream_t, long long, const float*);
-int ts_flat_average(const float*, float*, int*, long long, cudaStream_t);
-int ts_flat_swap(float*, float*, void*, long long, cudaStream_t);
-long long ts_flat_grad_norm_scratch(long long);
-int ts_flat_grad_norm(const float*, const float*, long long, float, float, long long, float, double*, float*, cudaStream_t);
-int ts_cast_bf16(const float*, void*, long long, cudaStream_t);
-int ts_fused_allreduce(const unsigned long long*, unsigned long long, unsigned long long, unsigned long long, float*,
-                       float*, unsigned int*, int*, long long, int, int, int, int, int, int, float, float, float, float,
-                       float, double, cudaStream_t, int*, long long, int, int);
-int ts_ar_bump_step(int*, cudaStream_t);
-int ts_ar_max_blocks();
-int ts_ar_flag_words();
-int ts_ar_slots();
-int ts_head_fwd_tc(const void*, int, const float*, const float*, const long long*, float*, float*, float*, int*, int, int, int, cudaStream_t);
-int ts_head_logits_generic(const void*, const float*, const float*, float*, int, int, int, int, cudaStream_t);
-int ts_head_bwd(const void*, const float*, const float*, const float*, void*, float*, float*, int, int, int, int, int, int, cudaStream_t);
-int ts_head_step_fwd_generic_parts(int);
-int ts_head_step_fwd(const void*, int, int, const float*, const float*, const long long*, const int*, float*, float*, float*, int*,
-                     unsigned int*, float*, int*, int*, int, int, int, int, int*, cudaStream_t);
-long long ts_head_step_bwd_scratch(int, int, int);
-int ts_head_step_bwd_tickets(int);
-int ts_head_step_bwd(const void*, const float*, const float*, const float*, void*, float*, float*, float*, unsigned int*, int, int, int,
-                     int, int, int, cudaStream_t);
-int ts_vocab_head_parts(int);
-int ts_vocab_head_blocks(int);
-int ts_vocab_head_fwd(const void*, const void*, int, const float*, const long long*, const int*, void*, float*, float*, int*, unsigned int*,
-                      float*, int*, int*, int, int, int, int, int, cudaStream_t);
-int ts_vocab_head_dlogits(const void*, const void*, int, const float*, const long long*, const int*, const float*, const float*, const int*,
-                          void*, int, int, int, int, int, int, int, cudaStream_t);
-int ts_vocab_head_colsum(const void*, float*, int, int, int, cudaStream_t);
-int ts_vocab_sample(const void*, const void*, int, const float*, float, unsigned int, int*, const int*, void*, int*, unsigned int*, int*,
-                    float*, int*, float*, int, int, int, int, int, int, cudaStream_t);
-int ts_vocab_sample_logits(const float*, const float*, float, unsigned int, int*, const int*, void*, int*, unsigned int*, int*, float*, int*,
-                           float*, int, int, int, int, cudaStream_t);
-int ts_vocab_head_logits(const void*, const void*, int, const float*, float*, int, int, int, int, cudaStream_t);
-int ts_vocab_threshold(const float*, int, int, int, double, float, float*, cudaStream_t);
-int ts_gemm_generic(const void*, const void*, void*, const float*, int, int, int, long long, long long, long long, long long, long long,
-                    int, int, int, float, cudaStream_t);
-int ts_gemm2(const void*, const void*, void*, const float*, int, int, int, int, int, int, int, int, int, int, int, int, int,
-             const unsigned int*, const int*, unsigned int*, int*, int, int, int, int, float*, int, cudaStream_t);
-int ts_lstm_seq_fwd(const void*, const void*, const float*, const void*, const float*, void*, const float*, void*, void*, int,
-                    int, int, unsigned int*, int, cudaStream_t, const void*, const unsigned int*, int, int, int, const int*, int,
-                    void*, const int*, const unsigned int*);
-int ts_lstm_seq_bwd(const void*, const void*, const void*, const float*, const void*, float*, float*, void*, void*, int,
-                    int, int, unsigned int*, int, cudaStream_t, const unsigned int*, int, int, int, const int*, int,
-                    const int*, const unsigned int*, void*);
-int ts_dropout(const void*, void*, int, int, int, int, int, const int*, const unsigned int*, cudaStream_t);
-int ts_weight_drop_grad(const float*, float*, int, int, int, const int*, const unsigned int*, cudaStream_t);
-long long ts_act_reg_scratch(int, int, int, int);
-int ts_act_reg_fwd(const void*, const void*, const int*, int, int, int, int, double*, float*, cudaStream_t);
-int ts_act_reg_bwd(const void*, const void*, const void*, const int*, const float*, int, int, int, int, const int*, const unsigned int*,
-                   void*, cudaStream_t);
-int ts_lstm_seq_prologue(const void*, const float*, void*, float*, void*, unsigned int*, int, int, cudaStream_t);
-int ts_seq_pool_fwd(const void*, int, const int*, const float*, int, int, int, int, float*, int*, cudaStream_t);
-int ts_seq_pool_attn_scores(float*, const float*, const float*, const int*, int, int, int, float*, int, cudaStream_t);
-int ts_seq_pool_attn_bwd(const void*, int, const float*, const float*, const float*, const float*, const int*, int, int, int, int,
-                         float*, void*, float*, unsigned int*, float*, float*, int, int, cudaStream_t);
-int ts_seq_pool_bwd(const float*, const int*, const int*, const float*, const float*, int, int, int, int, void*, int, cudaStream_t);
-void ts_embed_scratch_numel(long long, long long, long long, long long*);
-int ts_embed_fwd(const void*, int, const int*, const int*, int, int, int, int, void*, const int*, const unsigned int*, const int*,
-                 const unsigned int*, cudaStream_t);
-int ts_embed_bwd(const void*, int, const int*, const int*, int, int, int, int, float*, int, int*, int*, float*, const int*,
-                 const unsigned int*, const int*, const unsigned int*, cudaStream_t);
-int ts_embed_bwd_launches();
-const char* ts_last_error();
-int ts_cache_key_tile();
-int ts_cache_chunks(int, int, int, int);
-int ts_cache_combine_blocks(int);
-int ts_cache_pointer(const void*, const void*, const int*, const long long*, const float*, const int*, int, int, int, int, int, long long,
-                     float, float, int, int, void*, void*, unsigned int*, float*, float*, cudaStream_t);
-int ts_cache_append(const void*, void*, int*, const long long*, int, int, long long, int, long long, cudaStream_t);
-int ts_cache_label_logprob_parts(const void*, const float*, const long long*, float*, int, int, int, int, cudaStream_t);
-int ts_cache_label_logprob_logits(const float*, const long long*, float*, int, int, int, cudaStream_t);
-}
+using torch::Tensor;
 
 namespace {
 

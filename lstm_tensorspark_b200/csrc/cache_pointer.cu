@@ -27,6 +27,7 @@
 #include <stdint.h>
 
 #include "hopper.cuh"
+#include "launchers.h"
 #include "tmap.h"
 #include "ts_common.cuh"
 

@@ -18,6 +18,7 @@
 //     3. sum     one CTA per id plus one per further piece of a long segment: sums its rows of dx in fp32 in row order.  An id
 //                with several pieces writes per-piece partials, and the last piece to take the id's ticket sums them in piece
 //                order (and leaves the ticket 0).  A single id at every position costs T·B / kSeg CTAs, not one.
+#include "launchers.h"
 #include "ts_common.cuh"
 
 namespace {

@@ -20,6 +20,8 @@
 //              end bit-identical, optimizer state is touched for 1/N of the elements per rank.
 // Cross-GPU barrier: per-CTA flag slots in a symmetric pad, monotonically increasing epochs (never reset),
 // st.release.sys / ld.acquire.sys, bounded spin -> error flag instead of a hang if a peer died.
+#include "hopper.cuh"
+#include "launchers.h"
 #include "ts_common.cuh"
 
 namespace {
@@ -82,11 +84,6 @@ TS_DEVICE uint2 pack_bf16x4(float4 v) {
   r.y = *reinterpret_cast<uint32_t*>(&hi);
   return r;
 }
-TS_DEVICE unsigned long long globaltimer_ns() {
-  unsigned long long t;
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-  return t;
-}
 
 // All CTAs with the same blockIdx on every rank meet here.  Writes made by any thread of this CTA before the
 // call are visible to the peers after their wait returns (bar.sync + cumulative release / acquire, sys scope).
@@ -97,13 +94,13 @@ TS_DEVICE void cross_rank_barrier(const ARArgs& a, uint32_t epoch) {
     uint32_t* remote = a.flags[t] + blockIdx.x * kMaxRanks + a.rank;
     asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(remote), "r"(epoch) : "memory");
     const uint32_t* mine = a.flags[a.rank] + blockIdx.x * kMaxRanks + t;
-    unsigned long long t0 = globaltimer_ns();
+    unsigned long long t0 = tc::globaltimer();
     uint32_t seen;
     int spins = 0;
     while (true) {
       asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(seen) : "l"(mine) : "memory");
       if ((int32_t)(seen - epoch) >= 0) break;
-      if ((++spins & 1023) == 0 && globaltimer_ns() - t0 > a.timeout_ns) {
+      if ((++spins & 1023) == 0 && tc::globaltimer() - t0 > a.timeout_ns) {
         atomicExch(a.err, 1);
         break;
       }
@@ -150,7 +147,7 @@ __global__ void ar_inc_step_kernel(int* step) { *step += 1; }
 
 template <int kMode, bool kMulticast>
 __global__ void __launch_bounds__(kThreads) ar_two_shot_kernel(const __grid_constant__ ARArgs a) {
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");      // the next bucket may start next to this one
+  tc::pdl_launch_dependents();      // the next bucket may start next to this one
   const float lr = kMode == MODE_ADAM ? effective_lr(a) : a.lr;
   uint32_t epoch = a.epochs[blockIdx.x];
   cross_rank_barrier(a, ++epoch);              // every rank's inputs are final
@@ -191,7 +188,7 @@ __global__ void __launch_bounds__(kThreads) ar_two_shot_kernel(const __grid_cons
   }
   cross_rank_barrier(a, ++epoch);              // every replica holds every slice
   if (threadIdx.x == 0) a.epochs[blockIdx.x] = epoch;
-  if (a.pdl) asm volatile("griddepcontrol.wait;" ::: "memory");
+  if (a.pdl) tc::pdl_wait();
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -199,7 +196,7 @@ __global__ void __launch_bounds__(kThreads) ar_two_shot_kernel(const __grid_cons
 // ---------------------------------------------------------------------------------------------------------
 template <int kMode>
 __global__ void __launch_bounds__(kThreads) ar_one_shot_kernel(const __grid_constant__ ARArgs a) {
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  tc::pdl_launch_dependents();
   const float lr = kMode == MODE_ADAM ? effective_lr(a) : a.lr;
   uint32_t epoch = a.epochs[blockIdx.x];
   long long stride = (long long)gridDim.x * kThreads;
@@ -227,7 +224,7 @@ __global__ void __launch_bounds__(kThreads) ar_one_shot_kernel(const __grid_cons
   }
   cross_rank_barrier(a, ++epoch);              // peers are done reading my input: it may be overwritten
   if (threadIdx.x == 0) a.epochs[blockIdx.x] = epoch;
-  if (a.pdl) asm volatile("griddepcontrol.wait;" ::: "memory");
+  if (a.pdl) tc::pdl_wait();
 }
 
 // pdl: programmatic dependent launch - the kernel may start while the PREVIOUS kernel of the stream is still running (as soon

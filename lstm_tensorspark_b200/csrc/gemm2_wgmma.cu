@@ -25,6 +25,7 @@
 #include <string.h>
 
 #include "hopper.cuh"
+#include "launchers.h"
 #include "tmap.h"
 
 namespace {
@@ -45,20 +46,6 @@ template <int kCtas, int BN> struct Cfg2 {
   static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align*/ + 1024 /*barriers, padded to 1 KB*/
                                      + 1024 /*all-ones B block*/;
 };
-
-TC_DEVICE uint32_t cluster_ctarank2() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
-TC_DEVICE void cluster_sync2() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-TC_DEVICE uint32_t mapa2(uint32_t local_smem_addr, uint32_t cta) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_smem_addr), "r"(cta));
-  return r;
-}
-TC_DEVICE void mbar_arrive_cluster(uint32_t cluster_bar_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_bar_addr) : "memory");
-}
 
 struct Gemm2Params {
   void* C;
@@ -101,8 +88,8 @@ gemm2_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__
   const int lane = threadIdx.x & 31;
   // A kernel queued behind this one with the programmatic-dependent-launch attribute (a finished gradient bucket's fused
   // allreduce + update) may start once this grid is resident: it shares the SMs instead of waiting for the GEMM to drain.
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-  const uint32_t crank = kCtas == 2 ? cluster_ctarank2() : 0u;
+  tc::pdl_launch_dependents();
+  const uint32_t crank = kCtas == 2 ? tc::cluster_ctarank() : 0u;
   constexpr int TM = BM * kCtas;                              // tile rows per cluster
   const int tiles_n = (p.N + BN - 1) / BN;
   const int tiles_m = (p.M + TM - 1) / TM;
@@ -121,7 +108,7 @@ gemm2_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__
     tc::fence_barrier_init();
   }
   __syncthreads();
-  if (kCtas == 2) cluster_sync2();               // the peer's barriers are initialised before anything arrives on them
+  if (kCtas == 2) tc::cluster_sync();            // the peer's barriers are initialised before anything arrives on them
 
   if (warp == 0) {
     // ===================================================================== TMA producer (every CTA loads its own rows)
@@ -142,9 +129,8 @@ gemm2_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__
           const long long t0 = clock64();
           for (int g = lane; g < p.gate_count; g += 32) {
             const unsigned int* c = p.gate + (size_t)g * p.gate_stride;
-            unsigned int v;
             while (true) {
-              asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(c) : "memory");
+              const unsigned int v = tc::ld_relaxed_gpu(c);
               if ((int)v - target >= 0) break;
               if (clock64() - t0 > p.gate_spin_limit) { if (p.gate_err) atomicExch(p.gate_err, 1); ok = false; break; }
             }
@@ -200,7 +186,7 @@ gemm2_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__
     const int wg = (warp - kConsWarp0) >> 2;             // rows [64 wg, +64) of the CTA's 128
     const int wq = warp & 3;                              // warp within the warpgroup
     const uint32_t full0 = tc::smem_u32(full), empty0 = tc::smem_u32(empty);
-    const uint32_t empty0_peer = kCtas == 2 ? mapa2(empty0, crank ^ 1u) : 0u;
+    const uint32_t empty0_peer = kCtas == 2 ? tc::mapa(empty0, crank ^ 1u) : 0u;
     const uint64_t da0 = kAMN ? tc::desc_mnmajor_sw128(tc::smem_u32(smem_a) + wg * 8192) : tc::desc_kmajor_sw128(tc::smem_u32(smem_a) + wg * 8192);
     const uint64_t db0 = kBMN ? tc::desc_mnmajor_sw128(tc::smem_u32(smem_b)) : tc::desc_kmajor_sw128(tc::smem_u32(smem_b));
     constexpr uint64_t kAStep = kAMN ? (2048 >> 4) : (32 >> 4);     // descriptor advance per k16
@@ -208,7 +194,7 @@ gemm2_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__
     auto release = [&](uint32_t st) {                     // this warp has finished reading stage st (in every CTA of the cluster)
       if (lane == 0) {
         tc::mbar_arrive_u32(empty0 + 8 * st);
-        if (kCtas == 2) mbar_arrive_cluster(empty0_peer + 8 * st);
+        if (kCtas == 2) tc::mbar_arrive_cluster(empty0_peer + 8 * st);
       }
     };
     uint32_t stage = 0, phase = 0;
@@ -281,15 +267,14 @@ gemm2_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__
       if (p.done != nullptr) {                     // publish this CTA's 128 x BN output block to the gated consumer kernel
         asm volatile("bar.sync 1, 256;" ::: "memory");           // both consumer warpgroups have issued their stores
         if (warp == kConsWarp0 && lane == 0)
-          asm volatile("red.release.gpu.global.add.u32 [%0], 1;"
-                       ::"l"(p.done + ((size_t)tile_m_of(tile) * kCtas + crank) * tiles_n + (tile % tiles_n)) : "memory");
+          tc::signal_counter(p.done + ((size_t)tile_m_of(tile) * kCtas + crank) * tiles_n + (tile % tiles_n));
       }
     }
   }
 
   __syncthreads();
-  if (kCtas == 2) cluster_sync2();               // nobody leaves while the peer may still multicast into / arrive on its smem
-  if (p.pdl) asm volatile("griddepcontrol.wait;" ::: "memory");
+  if (kCtas == 2) tc::cluster_sync();            // nobody leaves while the peer may still multicast into / arrive on its smem
+  if (p.pdl) tc::pdl_wait();
 }
 
 template <int kCtas, int BN, bool kAMN, bool kBMN, int kOut>

@@ -4,6 +4,7 @@
 // in_features = 4, hidden 16, batch 10, ONE time step (original src/rnn.py:312-321, lstm.py:88-91) - and the fp32
 // parity path.  Performance target: none; these products are a few kFLOP.  Keeping them on our own kernel means the
 // product path never calls a library GEMM.
+#include "launchers.h"
 #include "ts_common.cuh"
 
 namespace {

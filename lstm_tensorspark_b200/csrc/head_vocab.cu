@@ -32,6 +32,7 @@
 #include <cuda_runtime.h>
 
 #include "hopper.cuh"
+#include "launchers.h"
 #include "tmap.h"
 #include "ts_common.cuh"
 
@@ -124,20 +125,6 @@ TC_DEVICE void sample_take(float& best, int& arg, float& lbest, float b2, int a2
   if (b2 > best || (b2 == best && a2 < arg)) { best = b2; arg = a2; lbest = l2; }
 }
 
-TC_DEVICE uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
-TC_DEVICE void cluster_sync() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-TC_DEVICE uint32_t mapa(uint32_t local_smem_addr, uint32_t cta) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_smem_addr), "r"(cta));
-  return r;
-}
-TC_DEVICE void mbar_arrive_cluster(uint32_t cluster_bar_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_bar_addr) : "memory");
-}
-
 // tile -> (cluster tile row, class tile): bands of kBandTiles cluster tiles, class tile outer inside a band
 TC_DEVICE void tile_coords(int tile, int tiles_m, int tiles_n, int& tm, int& tn) {
   const int per_band = kBandTiles * tiles_n;
@@ -161,7 +148,7 @@ vocab_head_gemm_kernel(const __grid_constant__ CUtensorMap tmap_h, const __grid_
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const uint32_t crank = cluster_ctarank();
+  const uint32_t crank = tc::cluster_ctarank();
   const int tiles_n = (p.C + BN - 1) / BN;
   const int tiles_m = (p.rows + TM - 1) / TM;
   const int num_tiles = tiles_m * tiles_n;
@@ -178,7 +165,7 @@ vocab_head_gemm_kernel(const __grid_constant__ CUtensorMap tmap_h, const __grid_
     tc::fence_barrier_init();
   }
   __syncthreads();
-  cluster_sync();                                // the peer's barriers are initialised before anything arrives on them
+  tc::cluster_sync();                            // the peer's barriers are initialised before anything arrives on them
 
   // The consumers hold 128 accumulator registers per thread and the epilogue works on all of them: setmaxnreg moves registers
   // from warpgroup 0 (producer and idle warps) to them, (168 - 56) * 128 = (224 - 168) * 256.  All four warps of a warpgroup
@@ -220,14 +207,14 @@ vocab_head_gemm_kernel(const __grid_constant__ CUtensorMap tmap_h, const __grid_
     const int wg = (warp - kConsWarp0) >> 2;             // rows [64 wg, +64) of the CTA's 128
     const int wq = warp & 3;
     const uint32_t full0 = tc::smem_u32(full), empty0 = tc::smem_u32(empty);
-    const uint32_t empty0_peer = mapa(empty0, crank ^ 1u);
+    const uint32_t empty0_peer = tc::mapa(empty0, crank ^ 1u);
     const uint64_t da0 = tc::desc_kmajor_sw128(tc::smem_u32(smem_a) + wg * 8192);
     const uint64_t db0 = kBK ? tc::desc_kmajor_sw128(tc::smem_u32(smem_b)) : tc::desc_mnmajor_sw128(tc::smem_u32(smem_b));
     constexpr uint32_t kBStep = kBK ? (32 >> 4) : (2048 >> 4);   // per k16: 32 B along a K-major row, 16 rows of the MN-major tile
     auto release = [&](uint32_t st) {                     // this warp has finished reading stage st (in both CTAs)
       if (lane == 0) {
         tc::mbar_arrive_u32(empty0 + 8 * st);
-        mbar_arrive_cluster(empty0_peer + 8 * st);
+        tc::mbar_arrive_cluster(empty0_peer + 8 * st);
       }
     };
     float scale = 0.f;
@@ -397,7 +384,7 @@ vocab_head_gemm_kernel(const __grid_constant__ CUtensorMap tmap_h, const __grid_
   }
 
   __syncthreads();
-  cluster_sync();                                // nobody leaves while the peer may still multicast into / arrive on its smem
+  tc::cluster_sync();                            // nobody leaves while the peer may still multicast into / arrive on its smem
 }
 
 // ---- combine ----------------------------------------------------------------------------------------------------------------

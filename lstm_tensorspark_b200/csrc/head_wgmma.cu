@@ -20,6 +20,7 @@
 #include <cuda_runtime.h>
 
 #include "hopper.cuh"
+#include "launchers.h"
 #include "tmap.h"
 #include "ts_common.cuh"
 

@@ -2,6 +2,7 @@
 // the tensor-core head of head_wgmma.cu does not take: fp32 activations, more than 256 classes).  One warp per batch row.
 // Reference: sparse_softmax_cross_entropy_with_logits -> reduce_mean -> argmax/equal/cast/reduce_mean
 // (original src/rnn.py:55-63, 84-92).
+#include "launchers.h"
 #include "ts_common.cuh"
 
 namespace {

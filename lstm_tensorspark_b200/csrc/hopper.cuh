@@ -1,6 +1,7 @@
 // Inline-PTX wrappers for the Hopper (sm_90a) async machinery used by the tensor-core kernels:
-// mbarrier, TMA (cp.async.bulk[.tensor]), wgmma (warpgroup MMA, fp32 accumulators in registers) and its shared-memory
-// matrix descriptors.  Bit layouts follow the PTX ISA "wgmma matrix descriptor" table.
+// mbarrier, TMA (cp.async.bulk[.tensor]), thread-block clusters, programmatic dependent launch, GPU-scope dataflow counters,
+// wgmma (warpgroup MMA, fp32 accumulators in registers) and its shared-memory matrix descriptors.  Bit layouts follow the
+// PTX ISA "wgmma matrix descriptor" table.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -88,6 +89,63 @@ TC_DEVICE void tma_load_2d_mc(uint32_t smem_dst, const CUtensorMap* map, uint32_
                " [%0], [%1, {%3, %4}], [%2], %5;"
                ::"r"(smem_dst), "l"((uint64_t)map), "r"(bar), "r"(c0), "r"(c1), "h"(cta_mask) : "memory");
 }
+
+// ---------------------------------------------------------------------------------------- thread-block clusters
+TC_DEVICE uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
+TC_DEVICE void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
+  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+// The address of the same shared-memory location in cluster member `cta`.
+TC_DEVICE uint32_t mapa(uint32_t local_smem_addr, uint32_t cta) {
+  uint32_t r;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_smem_addr), "r"(cta));
+  return r;
+}
+// Arrive on a cluster member's mbarrier (address from mapa), releasing this thread's prior writes at cluster scope.
+TC_DEVICE void mbar_arrive_cluster(uint32_t cluster_bar_addr) {
+  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_bar_addr) : "memory");
+}
+// "Buffer consumed" notifications carry no data: the reads they order were complete (their values used) before the CTA
+// barrier that precedes the arrive.  The .release form compiles to MEMBAR.ALL.GPU + ERRBAR + CGAERRBAR - a second
+// GPU-scope fence per step that competes with the one the dataflow signal needs.
+TC_DEVICE void mbar_arrive_remote_relaxed(uint32_t remote_bar_addr) {
+  asm volatile("mbarrier.arrive.relaxed.cluster.shared::cluster.b64 _, [%0];" ::"r"(remote_bar_addr) : "memory");
+}
+
+// ---------------------------------------------------------------------------------------- programmatic dependent launch
+// A kernel launched behind this one with cudaLaunchAttributeProgrammaticStreamSerialization may start once every CTA of this
+// grid has called pdl_launch_dependents (or exited); pdl_wait blocks until the grid this one was launched behind has completed
+// and its writes are visible.
+TC_DEVICE void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+TC_DEVICE void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+
+// ---------------------------------------------------------------------------------------- GPU-scope dataflow counters
+// Counters in global memory through which kernels that run at the same time hand on data: the producer publishes its prior
+// writes with a release store or reduction, the consumer polls with an acquire load, or with relaxed loads and a fence.
+TC_DEVICE unsigned int ld_acquire_gpu(const unsigned int* ctr) {
+  unsigned int v;
+  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(ctr) : "memory");
+  return v;
+}
+TC_DEVICE uint2 ld_relaxed_gpu_v2(const unsigned int* ctr) {
+  uint2 v;
+  asm volatile("ld.relaxed.gpu.global.v2.u32 {%0,%1}, [%2];" : "=r"(v.x), "=r"(v.y) : "l"(ctr) : "memory");
+  return v;
+}
+TC_DEVICE void st_release_gpu(unsigned int* ctr, unsigned int v) {
+  asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(ctr), "r"(v) : "memory");
+}
+TC_DEVICE unsigned int ld_relaxed_gpu(const unsigned int* ctr) {      // coalesces across lanes (a divergent ld.acquire does not)
+  unsigned int v;
+  asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(ctr) : "memory");
+  return v;
+}
+TC_DEVICE void signal_counter(unsigned int* ctr) {
+  asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(ctr) : "memory");
+}
+// Nanoseconds, one clock for every SM of the GPU.
+TC_DEVICE unsigned long long globaltimer() { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
 
 // ---------------------------------------------------------------------------------------- wgmma
 // Warpgroup MMA: the four warps of an aligned warpgroup issue it together; D (64 x N fp32) lives in their registers.

@@ -9,6 +9,8 @@
 // Layout: pre/act/dpre are [B, 4H] with column n = 4*j + g, g: 0=i 1=f 2=g(candidate) 3=o. c is fp32.
 // kMasked (per-row lengths, right padding): at step t >= lengths[b] row b holds its state - forward h_t = h_{t-1}, c_t = c_{t-1};
 // backward dpre = 0, dc passes through and the total dh is handed on (dh_out) instead of going through W_h.
+#include "hopper.cuh"
+#include "launchers.h"
 #include "ts_common.cuh"
 
 namespace {
@@ -300,7 +302,7 @@ __global__ void colsum_bf16_kernel(const uint4* __restrict__ src, float* __restr
                                    int pitch_cols, int nx, int ny) {
   __shared__ float red[8][256];
   __shared__ unsigned int ticket_s;
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  tc::pdl_launch_dependents();
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int vec_per_row = pitch_cols / 8;                      // (src / out already point at the first column of this launch)
   for (int vb = blockIdx.x; vb < nx * ny; vb += gridDim.x) {
@@ -347,7 +349,7 @@ __global__ void colsum_bf16_kernel(const uint4* __restrict__ src, float* __restr
   }
   // launched as a programmatic dependent of a weight-gradient GEMM (it runs on the SMs that GEMM leaves idle and reads the same
   // dG): do not let anything behind us start before that GEMM has completed
-  if (pdl) asm volatile("griddepcontrol.wait;" ::: "memory");
+  if (pdl) tc::pdl_wait();
 }
 }  // namespace
 

@@ -35,6 +35,7 @@
 #include <stdio.h>
 
 #include "hopper.cuh"
+#include "launchers.h"
 #include "tmap.h"
 #include "ts_common.cuh"
 
@@ -72,27 +73,11 @@ struct SeqSmem {
   float bias[64];
 };
 
-TC_DEVICE uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
-TC_DEVICE void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-TC_DEVICE uint32_t mapa(uint32_t local_smem_addr, uint32_t cta) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_smem_addr), "r"(cta));
-  return r;
-}
 // 16 B into a cluster member's shared memory; the bytes are accounted on ITS mbarrier (complete_tx), so the receiver needs
 // no release/acquire round trip: it arms the barrier with expect_tx and waits, exactly as for a TMA load.
 TC_DEVICE void st_async_u4(uint32_t remote_addr, uint4 v, uint32_t remote_bar) {
   asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.v4.b32 [%0], {%1,%2,%3,%4}, [%5];"
                ::"r"(remote_addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w), "r"(remote_bar) : "memory");
-}
-// "Buffer consumed" notifications carry no data: the reads they order were complete (their values used) before the CTA
-// barrier that precedes the arrive.  The .release form compiles to MEMBAR.ALL.GPU + ERRBAR + CGAERRBAR - a second
-// GPU-scope fence per step that competes with the one the dataflow signal needs.
-TC_DEVICE void mbar_arrive_remote_relaxed(uint32_t remote_bar_addr) {
-  asm volatile("mbarrier.arrive.relaxed.cluster.shared::cluster.b64 _, [%0];" ::"r"(remote_bar_addr) : "memory");
 }
 TC_DEVICE bool mbar_try_wait_cluster(uint64_t* bar, uint32_t parity) {
   uint32_t ok;
@@ -119,30 +104,8 @@ TC_DEVICE bool wait_bar(uint64_t* bar, uint32_t parity, volatile int* abort_flag
   return true;
 }
 
-TC_DEVICE unsigned int ld_acquire_gpu(const unsigned int* ctr) {
-  unsigned int v;
-  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(ctr) : "memory");
-  return v;
-}
-TC_DEVICE uint2 ld_relaxed_gpu_v2(const unsigned int* ctr) {
-  uint2 v;
-  asm volatile("ld.relaxed.gpu.global.v2.u32 {%0,%1}, [%2];" : "=r"(v.x), "=r"(v.y) : "l"(ctr) : "memory");
-  return v;
-}
-TC_DEVICE void st_release_gpu(unsigned int* ctr, unsigned int v) {
-  asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(ctr), "r"(v) : "memory");
-}
-TC_DEVICE unsigned int ld_relaxed_gpu(const unsigned int* ctr) {      // coalesces across lanes (a divergent ld.acquire does not)
-  unsigned int v;
-  asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(ctr) : "memory");
-  return v;
-}
-TC_DEVICE void signal_counter(unsigned int* ctr) {
-  asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(ctr) : "memory");
-}
 // Two-tile kernels: the second tile's per-step stamps follow the first tile's [T + 2][4] and the single-step / per-CTA stamps.
 TC_DEVICE size_t dbg_tile1(int T) { return 4 * (size_t)(T + 2) + 64 + 512; }
-TC_DEVICE unsigned long long gtime() { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
 
 TC_DEVICE uint4 ldg_nc16(const void* p) {
   uint4 r;
@@ -170,7 +133,7 @@ TC_DEVICE bool wait_in_gate(const unsigned int* ctr, int lane, volatile int* abo
   if (lane == 0) {
     long long t0 = clock64();
     int n = 0;
-    while (ld_acquire_gpu(ctr) == 0u) {
+    while (tc::ld_acquire_gpu(ctr) == 0u) {
       if ((++n & 63) == 0) {
         if (*abort_flag) { ok = 0; break; }
         if (clock64() - t0 > kSpinLimit) { *abort_flag = 1; ok = 0; break; }
@@ -186,7 +149,7 @@ TC_DEVICE bool wait_count(const unsigned int* ctr, unsigned int target, int lane
   if (lane == 0) {
     long long t0 = clock64();
     int n = 0;
-    while ((int)(ld_acquire_gpu(ctr) - target) < 0) {
+    while ((int)(tc::ld_acquire_gpu(ctr) - target) < 0) {
       if ((++n & 63) == 0) {
         if (*abort_flag) { ok = 0; break; }
         if (clock64() - t0 > kSpinLimit) { *abort_flag = 1; ok = 0; break; }
@@ -366,10 +329,10 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
   // Programmatic dependent launch: a kernel queued behind this one WITH the PDL attribute (the fused allreduce + update of a
   // gradient bucket that is already complete) may start once every CTA of this grid is resident - it then runs on the SMs
   // this persistent grid leaves idle instead of after it.  No effect on ordinary launches.
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  tc::pdl_launch_dependents();
   const int mb0 = (blockIdx.x / p.tiles_n) * kTiles;          // first batch tile of this CTA
   const int in_mb = blockIdx.x % p.tiles_n;
-  const uint32_t crank = kCluster ? cluster_ctarank() : 0;
+  const uint32_t crank = kCluster ? tc::cluster_ctarank() : 0;
   const int nb = in_mb / kSplit;                              // weight-row block of the cluster (64 rows; kFSplit: 128 rows)
   const int ks = kXchgL2 ? in_mb % kSplit : (int)crank;       // K-split member
   volatile int* abort_flag = &ss->abort_flag;
@@ -393,7 +356,7 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
   }
   if (!kBwd && threadIdx.x >= 64 && threadIdx.x < 128) ss->bias[threadIdx.x - 64] = p.bias[in_mb * BN + threadIdx.x - 64];
   __syncthreads();
-  if (kCluster) cluster_sync_all();             // peers' mbarriers are initialised before anyone arrives remotely
+  if (kCluster) tc::cluster_sync();            // peers' mbarriers are initialised before anyone arrives remotely
 
   // The consumers of the two-tile and K-split kernels hold 64 accumulator registers per thread: setmaxnreg moves registers
   // from warpgroup 0 to them.  All four warps of a warpgroup execute it at one place (warpgroup 0: idle warps too), at the
@@ -482,18 +445,18 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
             uint64_t ready = pending;
             if (s > 0) {
               if (p.sync_mode == 1) {
-                const unsigned int v = p.poll_acquire ? ld_acquire_gpu(p.sync + mb) : ld_relaxed_gpu(p.sync + mb);
+                const unsigned int v = p.poll_acquire ? tc::ld_acquire_gpu(p.sync + mb) : tc::ld_relaxed_gpu(p.sync + mb);
                 ready = ((int)(v - (unsigned)s * (unsigned)p.tiles_n) >= 0) ? pending : 0ull;
               } else if (p.sync_mode == 2) {
                 const unsigned int* fl = p.sync + kSyncFlags + (size_t)mb * p.tiles_n;
                 if (kBwd) {                                       // k-block kb_base + lane is written by CTA kb_base + lane
                   bool r0 = false;
-                  if (lane < num_kb) r0 = (int)(ld_relaxed_gpu(fl + kb_base + lane) - (unsigned)s) >= 0;
+                  if (lane < num_kb) r0 = (int)(tc::ld_relaxed_gpu(fl + kb_base + lane) - (unsigned)s) >= 0;
                   ready = (uint64_t)__ballot_sync(0xffffffffu, r0);
                 } else {                                          // k-block j is written by CTAs 4j..4j+3; lane L reads flags 2L, 2L+1
                   bool r0 = false;
                   if (2 * lane < p.tiles_n) {
-                    const uint2 v2 = ld_relaxed_gpu_v2(fl + 2 * lane);
+                    const uint2 v2 = tc::ld_relaxed_gpu_v2(fl + 2 * lane);
                     r0 = ((int)(v2.x - (unsigned)s) >= 0) && ((int)(v2.y - (unsigned)s) >= 0);
                   }
                   const unsigned int b = __ballot_sync(0xffffffffu, r0);
@@ -504,8 +467,8 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
                 }
               } else {
                 bool r0 = false, r1 = false;
-                if (lane < num_kb) r0 = (int)(ld_relaxed_gpu(ctr + lane * 32) - target) >= 0;
-                if (lane + 32 < num_kb) r1 = (int)(ld_relaxed_gpu(ctr + (lane + 32) * 32) - target) >= 0;
+                if (lane < num_kb) r0 = (int)(tc::ld_relaxed_gpu(ctr + lane * 32) - target) >= 0;
+                if (lane + 32 < num_kb) r1 = (int)(tc::ld_relaxed_gpu(ctr + (lane + 32) * 32) - target) >= 0;
                 ready = (uint64_t)__ballot_sync(0xffffffffu, r0) | ((uint64_t)__ballot_sync(0xffffffffu, r1) << 32);
               }
               ready &= pending;
@@ -528,7 +491,7 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
               asm volatile("fence.proxy.async.global;" ::: "memory");
             }
             if (p.dbg && blockIdx.x == 0 && lane == 0 && (tile == 0 || kPP) && !stamped) {
-              p.dbg[(tile ? dbg_tile1(p.T) : 0) + 4 * s + 0] = gtime();
+              p.dbg[(tile ? dbg_tile1(p.T) : 0) + 4 * s + 0] = tc::globaltimer();
               stamped = true;
             }
             pending &= ~ready;
@@ -612,7 +575,7 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
     auto wg_bar = [&]() { asm volatile("bar.sync %0, 128;" ::"r"(3 + half) : "memory"); };
     // per-step stamps of CTA 0: slot 0 first block ready (producer), 1 accumulator ready, 2 signal sent, 3 MMA start
     const bool dbg_wg = p.dbg && blockIdx.x == 0 && gtid == 0;
-    auto dbg_stamp = [&](int step, int slot) { p.dbg[(kPP && half ? dbg_tile1(p.T) : 0) + 4 * step + slot] = gtime(); };
+    auto dbg_stamp = [&](int step, int slot) { p.dbg[(kPP && half ? dbg_tile1(p.T) : 0) + 4 * step + slot] = tc::globaltimer(); };
     auto mma_tile = [&](int dstep) -> bool {
       // kPP computes the TRANSPOSED product, D[64 gate columns][128 batch rows] = W_slice x tile^T: one m64n128k16 per k16 with
       // the weight block as A and the operand stage as B reads 6 KB of shared memory instead of the 8 KB of two m64n64k16 with
@@ -756,7 +719,7 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
       uint32_t xphase = 0;
       const uint32_t xbase = tc::smem_u32(smem_x);
       const uint32_t xbar = tc::smem_u32(&ss->xchg_full[0]), fbar = tc::smem_u32(&ss->xchg_free[0]);
-      const uint32_t pbar = kFSplit ? mapa(xbar, (uint32_t)(1 - ks)) : 0u;      // the peer's exchange barrier
+      const uint32_t pbar = kFSplit ? tc::mapa(xbar, (uint32_t)(1 - ks)) : 0u;      // the peer's exchange barrier
       float cst[kPass][8];
       const size_t init_row = kRev ? (size_t)p.T * B : 0;     // the prologue wrote h0 / c0 to row 0 (forward) or row T (kRev)
 #pragma unroll
@@ -803,7 +766,7 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
         ok = mma_tile(t);
         if (!ok) break;
         unsigned long long t_acc = 0;
-        if (p.dbg && t == 8 && etid == 0) t_acc = gtime();
+        if (p.dbg && t == 8 && etid == 0) t_acc = tc::globaltimer();
         if (dbg_wg) dbg_stamp(t, 1);
         const bool pad = kMasked && tt >= len;        // padded step: the cell holds (the activations are computed but unused)
         float cn[kPass][8];
@@ -821,7 +784,7 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
               ok = xwait(&ss->xchg_free[0], (uint32_t)((t - 1) & 1), abort_flag);
               if (!ok) break;
             }
-            const uint32_t drow = mapa(xbase + (uint32_t)(rloc * 128), (uint32_t)(1 - ks));
+            const uint32_t drow = tc::mapa(xbase + (uint32_t)(rloc * 128), (uint32_t)(1 - ks));
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
               uint32_t pk[4];
@@ -846,7 +809,7 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
             acc_ld32(32 * ch(u), v);
             if (u == kPass - 1) acc_release();          // every pass has read its columns
           }
-          if (dbg_thread && t == 8 && u == 0) p.dbg[4 * (p.T + 2) + 0] = gtime();
+          if (dbg_thread && t == 8 && u == 0) p.dbg[4 * (p.T + 2) + 0] = tc::globaltimer();
           const float* bs = ss->bias + 32 * ch(u);
           float hv[8];
 #pragma unroll
@@ -883,24 +846,24 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
           }
         }
         if (!ok) break;
-        if (dbg_thread && t == 8) p.dbg[4 * (p.T + 2) + 1] = gtime();
+        if (dbg_thread && t == 8) p.dbg[4 * (p.T + 2) + 1] = tc::globaltimer();
         epi_bar();
         if (gtid == 0) {
-          if (dbg_thread && t == 8) p.dbg[4 * (p.T + 2) + 2] = gtime();
+          if (dbg_thread && t == 8) p.dbg[4 * (p.T + 2) + 2] = tc::globaltimer();
           if (p.dbg && t == 8 && etid == 0) {                // per-CTA stamps (skew study): accumulator ready / about to signal
             p.dbg[4 * (p.T + 2) + 64 + 2 * blockIdx.x] = t_acc;
-            p.dbg[4 * (p.T + 2) + 64 + 2 * blockIdx.x + 1] = gtime();
+            p.dbg[4 * (p.T + 2) + 64 + 2 * blockIdx.x + 1] = tc::globaltimer();
           }
           // this CTA's 16 hidden units = a quarter of k-block nb/4
-          if (p.sync_mode == 1) signal_counter(p.sync + mb);
-          else if (p.sync_mode == 2) st_release_gpu(p.sync + kSyncFlags + (size_t)mb * p.tiles_n + in_mb, (unsigned)(t + 1));
-          else signal_counter(p.sync + kSyncKb + ((size_t)mb * (H / BK) + (in_mb >> 2)) * 32);
+          if (p.sync_mode == 1) tc::signal_counter(p.sync + mb);
+          else if (p.sync_mode == 2) tc::st_release_gpu(p.sync + kSyncFlags + (size_t)mb * p.tiles_n + in_mb, (unsigned)(t + 1));
+          else tc::signal_counter(p.sync + kSyncKb + ((size_t)mb * (H / BK) + (in_mb >> 2)) * 32);
           if (dbg_wg) dbg_stamp(t, 2);
         }
         // (after the CTA barrier every epilogue thread is done with this step's exchange buffer)
         if (kFSplit && etid == 32) {
           tc::mbar_expect_tx_u32(xbar, (uint32_t)kXchgBytes);        // arm the next phase, THEN let the peer overwrite the buffer
-          mbar_arrive_remote_relaxed(mapa(fbar, (uint32_t)(1 - ks)));
+          tc::mbar_arrive_remote_relaxed(tc::mapa(fbar, (uint32_t)(1 - ks)));
         }
         signal_sent_bar();
         if (valid && p.debug_mode != 5) {              // everything below is off the critical path
@@ -926,8 +889,8 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
       if (p.extra_signal && ok) {                 // the last step's h_seq rows (natural layout) are visible to the gated GEMM
         epi_bar();
         if (gtid == 0) {
-          if (p.sync_mode == 1) signal_counter(p.sync + mb);
-          else signal_counter(p.sync + kSyncKb + ((size_t)mb * (H / BK) + (in_mb >> 2)) * 32);
+          if (p.sync_mode == 1) tc::signal_counter(p.sync + mb);
+          else tc::signal_counter(p.sync + kSyncKb + ((size_t)mb * (H / BK) + (in_mb >> 2)) * 32);
         }
       }
     } else {
@@ -1040,7 +1003,7 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
                     a[5], a[6], a[7]);
             }
             epi_bar();
-            if (gtid == 0) signal_counter(xctr);
+            if (gtid == 0) tc::signal_counter(xctr);
             ok = wait_count(xctr, 4u * (unsigned)s, lane, abort_flag);
             if (!ok) break;
             if (dbg_wg) dbg_stamp(s, 3);                          // group counter seen (stamp 1 -> 3: partial out, exchange wait)
@@ -1068,9 +1031,9 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
 #pragma unroll
               for (int qq = 0; qq < kCW / 16; ++qq) {
                 const uint32_t q = (uint32_t)((kCW / 16) * ch(u) + qq);
-                const uint32_t dst = mapa(xbase + (uint32_t)((ks * BM + rloc) * 32), q);
+                const uint32_t dst = tc::mapa(xbase + (uint32_t)((ks * BM + rloc) * 32), q);
                 const uint32_t* a = pk[u] + 8 * qq;
-                const uint32_t dbar = mapa(xbar, q);
+                const uint32_t dbar = tc::mapa(xbar, q);
                 st_async_u4(dst, make_uint4(a[0], a[1], a[2], a[3]), dbar);
                 st_async_u4(dst + 16, make_uint4(a[4], a[5], a[6], a[7]), dbar);
               }
@@ -1106,8 +1069,8 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
           if (p.extra_signal) {                   // dpre[0] (natural layout, written after the last per-step signal) is visible to the gated GEMM
             epi_bar();
             if (gtid == 0) {
-              if (p.sync_mode == 1) signal_counter(p.sync + mb);
-              else signal_counter(p.sync + kSyncKb + ((size_t)mb * (4 * H / BK) + in_mb) * 32);
+              if (p.sync_mode == 1) tc::signal_counter(p.sync + mb);
+              else tc::signal_counter(p.sync + kSyncKb + ((size_t)mb * (4 * H / BK) + in_mb) * 32);
             }
           }
           break;
@@ -1156,16 +1119,16 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
         epi_bar();
         if (gtid == 0) {
           // this CTA's 64 gate columns = dG k-block 4 nb + ks
-          if (p.sync_mode == 1) signal_counter(p.sync + mb);
-          else if (p.sync_mode == 2) st_release_gpu(p.sync + kSyncFlags + (size_t)mb * p.tiles_n + in_mb, (unsigned)(s + 1));
-          else signal_counter(p.sync + kSyncKb + ((size_t)mb * (4 * H / BK) + in_mb) * 32);
+          if (p.sync_mode == 1) tc::signal_counter(p.sync + mb);
+          else if (p.sync_mode == 2) tc::st_release_gpu(p.sync + kSyncFlags + (size_t)mb * p.tiles_n + in_mb, (unsigned)(s + 1));
+          else tc::signal_counter(p.sync + kSyncKb + ((size_t)mb * (4 * H / BK) + in_mb) * 32);
           if (dbg_wg) dbg_stamp(s, 2);
         }
         // (the barrier above also means every thread of the tile is done reading this step's exchange buffer)
         if (!kXchgL2 && s > 0) {
           if (gtid == 32) tc::mbar_expect_tx_u32(xbar, kXchgRecv);    // arm the next phase, THEN free the buffer
           __syncwarp();
-          if (gtid >= 32 && gtid < 32 + kSplit) mbar_arrive_remote_relaxed(mapa(tc::smem_u32(&ss->xchg_free[xt]), (uint32_t)(gtid - 32)));
+          if (gtid >= 32 && gtid < 32 + kSplit) tc::mbar_arrive_remote_relaxed(tc::mapa(tc::smem_u32(&ss->xchg_free[xt]), (uint32_t)(gtid - 32)));
           xphase ^= 1;
         }
         signal_sent_bar();
@@ -1188,8 +1151,8 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
     if (lane == 0) atomicAdd(&ss->roles_done, 1);
   }
   __syncthreads();
-  if (kCluster) cluster_sync_all();              // nobody exits while a peer may still write into / arrive on its smem
-  if (p.pdl_wait) asm volatile("griddepcontrol.wait;" ::: "memory");
+  if (kCluster) tc::cluster_sync();             // nobody exits while a peer may still write into / arrive on its smem
+  if (p.pdl_wait) tc::pdl_wait();
   if (threadIdx.x == 0 && ss->abort_flag) atomicExch(reinterpret_cast<int*>(p.sync + kSyncErr), 1);
 }
 

@@ -2,6 +2,7 @@
 // average of the iterates) that also refreshes the bf16 shadow the tensor-core kernels read.  Replaces the reference's one ApplyAdam
 // kernel per variable (14*L+2 launches per step; original src/rnn.py:207,224).
 // Memory-bound: 16 B vector loads/stores, grid = 132 SMs (H100) x 8 resident CTAs, grid-stride.
+#include "launchers.h"
 #include "ts_common.cuh"
 
 namespace {

@@ -16,6 +16,7 @@
 //                       dh_t = alpha_t ds + (dU W_a^T)_t, the second term from the GEMM in fp32, summed and rounded once here.
 //                       dv = sum de_t u_t and db_a = sum dU_t (fp32 dU) come from per-CTA partials that the last CTA to take
 //                       a ticket sums in batch-row order.
+#include "launchers.h"
 #include "ts_common.cuh"
 
 namespace {

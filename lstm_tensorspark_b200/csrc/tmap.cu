@@ -1,4 +1,5 @@
 #include "tmap.h"
+#include "launchers.h"
 
 #include <mutex>
 #include <stdio.h>
