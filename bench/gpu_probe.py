@@ -377,8 +377,8 @@ def check_seq_tune():
         bias = torch.zeros(4 * H, device=dev)
         h0 = torch.zeros(B, H, device=dev).bfloat16(); c0 = torch.zeros(B, H, device=dev)
         ws = cuda_lstm._sync_ws(dev)
-        for (tiles, st, mode, sync, acq, nosplit) in ((1, 0, 0, 1, 0, 1), (1, 0, 0, 0, 0, 1), (1, 0, 0, 1, 0, 0), (1, 0, 0, 0, 0, 0), (1, 4, 0, 0, 0, 0), (1, 0, 5, 0, 0, 0)):
-            v = tiles + 16 * st + 4096 * mode + 65536 * sync + 262144 * acq + 524288 * nosplit
+        for (tiles, st) in ((1, 0), (1, 4)):
+            v = tiles + 16 * st
             try:
                 ms = _time_ms(lambda: E.lstm_seq_fwd(gx, whb, bias, h0, c0, ws, v), iters=5, warm=2)
                 dbg = torch.zeros(4 * (T + 2) + 64 + 512, dtype=torch.int64, device=dev)
@@ -398,7 +398,7 @@ def check_seq_tune():
                 mma_total = [(int(x) >> 40) & 0xFFFFF for x in w3]
                 e = dbg[4 * (T + 2):4 * (T + 2) + 3].cpu()
                 acc8, sig8 = int(d[0, 1]), int(d[0, 2])
-                _emit("fwd_variant", T=T, B=B, H=H, tiles=tiles, stages=st, debug_mode=mode, sync=sync, acq=acq, nosplit=nosplit, us_per_step=ms * 1e3 / T,
+                _emit("fwd_variant", T=T, B=B, H=H, tiles=tiles, stages=st, us_per_step=ms * 1e3 / T,
                       mma_first_wait_cyc=sum(mma_first) / 16, mma_later_wait_cyc=sum(mma_wait) / 16, mma_step_cyc=sum(mma_total) / 16,
                       epi_ld_ns=int(e[0]) - acc8, epi_math_store_ns=int(e[1]) - int(e[0]), epi_bar_ns=int(e[2]) - int(e[1]), epi_signal_ns=sig8 - int(e[2]),
                       load_mma_us=float((accum - waited).float().mean()) / 1e3, epi_us=float((sig - accum).float().mean()) / 1e3,
@@ -427,7 +427,7 @@ def check_tiles2_tune():
     dh = torch.randn(T, B, H, device=dev).bfloat16()
     z = torch.zeros(B, H, device=dev)
     for st in (0, 4, 5, 6):
-        for sync in (0, 1, 2):
+        for sync in (0, 1):
             v = 2 + 16 * st + 65536 * sync
             try:
                 ms = _time_ms(lambda: E.lstm_seq_fwd(gx, whb, bias, h0, c0, ws, v), iters=5, warm=2)
@@ -436,7 +436,7 @@ def check_tiles2_tune():
             except Exception as e:        # noqa: BLE001
                 _emit("tiles2_fwd", stages=st, sync=sync, error=repr(e)[:200])
     for st in (0, 3, 4):
-        for sync in (0, 1, 2):
+        for sync in (0, 1):
             v = 2 + 16 * st + 65536 * sync
             try:
                 ms = _time_ms(lambda: E.lstm_seq_bwd(dh, whT, act, cseq, z, z, ws, v), iters=5, warm=2)
@@ -445,9 +445,8 @@ def check_tiles2_tune():
             except Exception as e:        # noqa: BLE001
                 _emit("tiles2_bwd", stages=st, sync=sync, error=repr(e)[:200])
     # one tile per CTA on 128 CTAs (the single-layer default), for reference
-    for v, nm in ((0, "ksplit_default"), (524288, "nosplit")):
-        ms = _time_ms(lambda: E.lstm_seq_fwd(gx, whb, bias, h0, c0, ws, v), iters=5, warm=2)
-        _emit("tiles1_fwd", variant=nm, us_per_step=ms * 1e3 / T)
+    ms = _time_ms(lambda: E.lstm_seq_fwd(gx, whb, bias, h0, c0, ws, 0), iters=5, warm=2)
+    _emit("tiles1_fwd", variant="ksplit_default", us_per_step=ms * 1e3 / T)
     # the backward at one tile per CTA on 128 CTAs without a cluster (K-split reduce-scattered through L2, kXchgL2), by ring
     # depth (0 = the default), alternating with the two-tile clustered kernel the headline runs, in three rounds
     xchg = cuda_lstm._xchg_buffer(B, H, dev)
@@ -468,8 +467,7 @@ def check_tiles2_tune():
 def check_tiles2_phase():
     """Per-step phase split of the two-tiles-per-CTA kernels (64 CTAs per layer, the headline's recurrences), from the time
     stamps of CTA 0's first tile: first operand block ready -> accumulator ready (load_mma_us), accumulator ready -> dataflow
-    signal sent (epi_us), signal -> next step's first block ready (sync_us).  debug_mode 1 skips the operand loads (garbage
-    results): how much of the step the operand stream costs.
+    signal sent (epi_us), signal -> next step's first block ready (sync_us).
     Per warpgroup (= tile, ping-pong schedule): MMA start -> accumulator ready (wgN_mma_us), accumulator ready -> signal
     (wgN_epi_us), and how much of warpgroup 1's MMA window falls inside warpgroup 0's epilogue (wg1_mma_in_wg0_epi_us)."""
     import torch
@@ -497,34 +495,32 @@ def check_tiles2_phase():
     for direction, run in runs.items():
         steps = T if direction == "fwd" else T + 1
         first = 8 if direction == "fwd" else 9              # skip the first steps (the backward pass stamps from s = 1)
-        for mode in (0, 1):
-            v = 2 + 4096 * mode
-            try:
-                ms = _time_ms(lambda: run(v), iters=5, warm=2)
-                tile1 = 4 * (T + 2) + 64 + 512                # the second tile's [steps][4] stamps start here
-                dbg = torch.zeros(tile1 + 4 * (T + 2), dtype=torch.int64, device=dev)
-                run(v, dbg)
-                torch.cuda.synchronize()
-                cuda_lstm.check_kernel_errors(dev)
-                d = dbg[:4 * (T + 2)].view(-1, 4)[first:steps - 8].cpu()
-                d1 = dbg[tile1:].view(-1, 4)[first:steps - 8].cpu()
-                waited, accum, sig = d[:, 0], d[:, 1], d[:, 2]
+        try:
+            ms = _time_ms(lambda: run(2), iters=5, warm=2)
+            tile1 = 4 * (T + 2) + 64 + 512                # the second tile's [steps][4] stamps start here
+            dbg = torch.zeros(tile1 + 4 * (T + 2), dtype=torch.int64, device=dev)
+            run(2, dbg)
+            torch.cuda.synchronize()
+            cuda_lstm.check_kernel_errors(dev)
+            d = dbg[:4 * (T + 2)].view(-1, 4)[first:steps - 8].cpu()
+            d1 = dbg[tile1:].view(-1, 4)[first:steps - 8].cpu()
+            waited, accum, sig = d[:, 0], d[:, 1], d[:, 2]
 
-                def us(x):
-                    return float(x.double().mean()) / 1e3
-                if direction == "bwd_l2":
-                    _emit("tiles2_phase", direction=direction, debug_mode=mode, us_per_step=ms * 1e3 / steps,
-                          load_mma_us=us(accum - waited), epi_us=us(sig - accum), sync_us=us(waited[1:] - sig[:-1]),
-                          xchg_us=us(d[:, 3] - accum), xchg_to_signal_us=us(sig - d[:, 3]))
-                    continue
-                overlap = (torch.minimum(d1[:, 1], d[:, 2]) - torch.maximum(d1[:, 3], d[:, 1])).clamp(min=0)
-                _emit("tiles2_phase", direction=direction, debug_mode=mode, us_per_step=ms * 1e3 / steps,
+            def us(x):
+                return float(x.double().mean()) / 1e3
+            if direction == "bwd_l2":
+                _emit("tiles2_phase", direction=direction, us_per_step=ms * 1e3 / steps,
                       load_mma_us=us(accum - waited), epi_us=us(sig - accum), sync_us=us(waited[1:] - sig[:-1]),
-                      wg0_mma_us=us(d[:, 1] - d[:, 3]), wg0_epi_us=us(d[:, 2] - d[:, 1]),
-                      wg1_mma_us=us(d1[:, 1] - d1[:, 3]), wg1_epi_us=us(d1[:, 2] - d1[:, 1]),
-                      wg1_mma_start_after_wg0_acc_us=us(d1[:, 3] - d[:, 1]), wg1_mma_in_wg0_epi_us=us(overlap))
-            except Exception as e:                     # noqa: BLE001
-                _emit("tiles2_phase", direction=direction, debug_mode=mode, error=repr(e)[:300])
+                      xchg_us=us(d[:, 3] - accum), xchg_to_signal_us=us(sig - d[:, 3]))
+                continue
+            overlap = (torch.minimum(d1[:, 1], d[:, 2]) - torch.maximum(d1[:, 3], d[:, 1])).clamp(min=0)
+            _emit("tiles2_phase", direction=direction, us_per_step=ms * 1e3 / steps,
+                  load_mma_us=us(accum - waited), epi_us=us(sig - accum), sync_us=us(waited[1:] - sig[:-1]),
+                  wg0_mma_us=us(d[:, 1] - d[:, 3]), wg0_epi_us=us(d[:, 2] - d[:, 1]),
+                  wg1_mma_us=us(d1[:, 1] - d1[:, 3]), wg1_epi_us=us(d1[:, 2] - d1[:, 1]),
+                  wg1_mma_start_after_wg0_acc_us=us(d1[:, 3] - d[:, 1]), wg1_mma_in_wg0_epi_us=us(overlap))
+        except Exception as e:                     # noqa: BLE001
+            _emit("tiles2_phase", direction=direction, error=repr(e)[:300])
 
 
 def check_bwd_tune():
@@ -545,27 +541,25 @@ def check_bwd_tune():
     dh_seq = (torch.randn(T, B, H, device=dev) * 0.1).bfloat16()
     w_hT = whb.t().contiguous()
     z = torch.zeros(B, H, device=dev)
-    for (mode, sync) in ((0, 0), (0, 1), (1, 0), (2, 0)):
-        v = 4096 * mode + 65536 * sync
-        try:
-            ms = _time_ms(lambda: E.lstm_seq_bwd(dh_seq, w_hT, act, c_seq, z, z, ws, v), iters=5, warm=2)
-            dbg = torch.zeros(4 * (T + 2) + 64 + 512, dtype=torch.int64, device=dev)
-            E.lstm_seq_bwd(dh_seq, w_hT, act, c_seq, z, z, ws, v, dbg)
-            torch.cuda.synchronize()
-            cuda_lstm.check_kernel_errors(dev)
-            d = dbg[:4 * (T + 2)].view(-1, 4)[8:40].cpu()
-            waited, accum, sig = d[:, 0], d[:, 1], d[:, 2]
-            w3 = d[:, 3]
-            mma_first = [int(x) & 0xFFFFF for x in w3]
-            mma_wait = [(int(x) >> 20) & 0xFFFFF for x in w3]
-            mma_total = [(int(x) >> 40) & 0xFFFFF for x in w3]
-            n = len(mma_first)
-            _emit("bwd_variant", debug_mode=mode, sync=sync, us_per_step=ms * 1e3 / (T + 1),
-                  mma_first_wait_us=sum(mma_first) / n / 1965, mma_later_wait_us=sum(mma_wait) / n / 1965, mma_step_us=sum(mma_total) / n / 1965,
-                  load_mma_us=float((accum - waited).float().mean()) / 1e3, epi_us=float((sig - accum).float().mean()) / 1e3,
-                  sync_us=float((waited[1:] - sig[:-1]).float().mean()) / 1e3)
-        except Exception as e:                     # noqa: BLE001
-            _emit("bwd_variant", debug_mode=mode, sync=sync, error=repr(e)[:300])
+    try:
+        ms = _time_ms(lambda: E.lstm_seq_bwd(dh_seq, w_hT, act, c_seq, z, z, ws, 0), iters=5, warm=2)
+        dbg = torch.zeros(4 * (T + 2) + 64 + 512, dtype=torch.int64, device=dev)
+        E.lstm_seq_bwd(dh_seq, w_hT, act, c_seq, z, z, ws, 0, dbg)
+        torch.cuda.synchronize()
+        cuda_lstm.check_kernel_errors(dev)
+        d = dbg[:4 * (T + 2)].view(-1, 4)[8:40].cpu()
+        waited, accum, sig = d[:, 0], d[:, 1], d[:, 2]
+        w3 = d[:, 3]
+        mma_first = [int(x) & 0xFFFFF for x in w3]
+        mma_wait = [(int(x) >> 20) & 0xFFFFF for x in w3]
+        mma_total = [(int(x) >> 40) & 0xFFFFF for x in w3]
+        n = len(mma_first)
+        _emit("bwd_variant", us_per_step=ms * 1e3 / (T + 1),
+              mma_first_wait_us=sum(mma_first) / n / 1965, mma_later_wait_us=sum(mma_wait) / n / 1965, mma_step_us=sum(mma_total) / n / 1965,
+              load_mma_us=float((accum - waited).float().mean()) / 1e3, epi_us=float((sig - accum).float().mean()) / 1e3,
+              sync_us=float((waited[1:] - sig[:-1]).float().mean()) / 1e3)
+    except Exception as e:                     # noqa: BLE001
+        _emit("bwd_variant", error=repr(e)[:300])
 
 
 def check_skew():

@@ -52,12 +52,10 @@ constexpr int kXchgBytes = 4 * BM * 16 * 2;   // backward: 4 source slots of [12
 constexpr long long kSpinLimit = 6000000000LL;   // ~3 s of SM clocks: a bug surfaces as an error, not a hung GPU
 constexpr long long kAbortGrace = 1000000000LL;  // ~0.5 s for the role loops to drain after an abort before the watchdog traps
 
-// sync workspace (u32 words): [0,16) grid-barrier counters, [64,320) per-CTA step flags, [512 + 32 i) k-block arrival
-// counters (one 128 B line each, i < tiles_m * 4H/64; seq_config rejects layouts that reach the last word), [kSyncWords-1]
-// sticky error flag
+// sync workspace (u32 words): [0,16) grid-barrier counters, [512 + 32 i) k-block arrival counters (one 128 B line each,
+// i < tiles_m * 4H/64; seq_config rejects layouts that reach the last word), [kSyncWords-1] sticky error flag
 constexpr int kSyncWords = 8192;
 constexpr int kSyncErr = kSyncWords - 1;
-constexpr int kSyncFlags = 64;
 constexpr int kSyncKb = 512;
 
 struct SeqSmem {
@@ -79,23 +77,11 @@ TC_DEVICE void st_async_u4(uint32_t remote_addr, uint4 v, uint32_t remote_bar) {
   asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.v4.b32 [%0], {%1,%2,%3,%4}, [%5];"
                ::"r"(remote_addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w), "r"(remote_bar) : "memory");
 }
-TC_DEVICE bool mbar_try_wait_cluster(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok) : "r"(tc::smem_u32(bar)), "r"(parity) : "memory");
-  return ok != 0;
-}
-
-template <bool kClusterScope>
 TC_DEVICE bool wait_bar(uint64_t* bar, uint32_t parity, volatile int* abort_flag) {
-  auto probe = [&]() { return kClusterScope ? mbar_try_wait_cluster(bar, parity) : tc::mbar_try_wait(bar, parity); };
-  if (probe()) return true;
+  if (tc::mbar_try_wait(bar, parity)) return true;
   long long t0 = clock64();
   int n = 0;
-  while (!probe()) {
+  while (!tc::mbar_try_wait(bar, parity)) {
     if ((++n & 255) == 0) {
       if (*abort_flag) return false;
       if (clock64() - t0 > kSpinLimit) { *abort_flag = 1; return false; }
@@ -188,21 +174,19 @@ struct SeqParams {
   float* dc0;                  // [B,H] in: dL/dc_T, out: dL/dc_0
   __nv_bfloat16* a_tiled;      // streamed operand as pre-swizzled SMEM images: [time][tiles_m][K/64][128 rows][64] (16 KB blocks)
   int tiles_m;
-  int debug_mode;              // timing experiments only: 1 = skip operand loads, 2 = skip MMAs, 4 = half-size loads (garbage results), 3 = in-order stream
+  int in_order;                // operand k-blocks issued (and accumulated) in index order, not arrival order: repeatable bits
   unsigned int* sync;          // [63] error flag; [64 + mb * nkb + kb] arrival counter of operand k-block kb of batch tile mb
   unsigned long long* dbg;     // optional [steps][4] timestamps of CTA 0's first tile (ns); two-tile kernels: the second
                                // tile's from word dbg_tile1(T)
   int T, B, H;
   int tiles_n;                 // CTAs per batch tile
-  int sync_mode;               // 0 = k-block arrival counters (dataflow), 1 = one counter per batch tile (grid barrier), 2 = per-CTA flags
-  int poll_acquire;            // experiment: ld.acquire polls instead of relaxed
+  int sync_mode;               // 0 = k-block arrival counters (dataflow), 1 = one counter per batch tile (grid barrier)
   // Layer wavefront (two layers' recurrences co-resident, chained through a dataflow-gated GEMM on the idle SMs):
   const unsigned int* in_gate; // completion counters of the GEMM that produces gx (fwd) / dh_seq (bwd) tile by tile while this kernel
                                // runs: [(row / 128) * in_gate_tiles_n + col / 256]; null = the operand is complete
   int in_gate_tiles_n;
   int pdl_wait;                // launched as a programmatic dependent: before exiting, wait for the grids launched before this one
                                // (completion of the chain's LAST kernel then implies completion of all of them)
-  int no_trap;                 // debugging: the watchdog only records the abort (variant bit 20) instead of killing the kernel
   int extra_signal;            // one more arrival on this CTA's k-block counter after the LAST step's bookkeeping stores (a gated
                                // GEMM consumes h_seq / dpre in the natural layout, which is written after the per-step signal)
   const int* lengths;          // [B] valid steps per row (right padding, 1 <= len <= T); null = every row runs all T steps.  Read
@@ -388,14 +372,13 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
       auto issue = [&](uint32_t st_, const __nv_bfloat16* src, int kb) {   // elected lane: fill ring stage st_ with k-block kb
         const uint32_t fb = full0 + 8 * st_;
         ss->kb_idx[st_] = (uint32_t)kb;                         // published by the release of the expect_tx arrive below
-        if (p.debug_mode == 1) { tc::mbar_arrive(&ss->full[st_]); return; }
         tc::mbar_expect_tx_u32(fb, a_bytes + (kStream ? kWBlk : 0));
         tc::bulk_load_1d_u32(a0 + st_ * kStageBytes, src + (size_t)kb * (BM * BK), a_bytes, fb);
         if (kStream) tc::tma_load_2d_u32(a0 + st_ * kStageBytes + kABytes, &tmap_w, fb, wc0 + kb * BK, wc1);
       };
       auto load_block = [&](const __nv_bfloat16* src, int kb) -> bool {
         if (!tc::mbar_try_wait_u32(empty0 + 8 * stage, phase ^ 1)) {
-          if (!wait_bar<false>(&ss->empty[stage], phase ^ 1, abort_flag)) return false;
+          if (!wait_bar(&ss->empty[stage], phase ^ 1, abort_flag)) return false;
         }
         if (tc::elect_one()) issue(stage, src, kb);
         __syncwarp();
@@ -408,8 +391,8 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
         if (s1 == kStages) { s1 = 0; ph1 ^= 1; }
         const bool r0 = tc::mbar_try_wait_u32(empty0 + 8 * stage, phase ^ 1);
         const bool r1 = tc::mbar_try_wait_u32(empty0 + 8 * s1, ph1 ^ 1);
-        if (!r0 && !wait_bar<false>(&ss->empty[stage], phase ^ 1, abort_flag)) return false;
-        if (!r1 && !wait_bar<false>(&ss->empty[s1], ph1 ^ 1, abort_flag)) return false;
+        if (!r0 && !wait_bar(&ss->empty[stage], phase ^ 1, abort_flag)) return false;
+        if (!r1 && !wait_bar(&ss->empty[s1], ph1 ^ 1, abort_flag)) return false;
         if (tc::elect_one()) {
           issue(stage, src, kb_a);
           issue(s1, src, kb_b);
@@ -432,11 +415,8 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
           const __nv_bfloat16* src = p.a_tiled + (((size_t)tsl * p.tiles_m + mb) * nkb_all + kb_base) * (BM * BK);
           const unsigned int* ctr = p.sync + kSyncKb + ((size_t)mb * nkb_all + kb_base) * 32;
           const unsigned int target = (unsigned)s * per_step;
-          {
-            const int rows = p.B - mb * BM;                     // rows beyond B are never read back from the accumulator
-            a_bytes = rows >= BM ? kABytes : (uint32_t)(((rows + 7) / 8) * 8 * BK * 2);
-            if (p.debug_mode == 4) a_bytes = kABytes / 2;       // experiment: half the operand traffic (results are garbage)
-          }
+          const int rows = p.B - mb * BM;                       // rows beyond B are never read back from the accumulator
+          a_bytes = rows >= BM ? kABytes : (uint32_t)(((rows + 7) / 8) * 8 * BK * 2);
           uint64_t pending = all_kb;
           const long long t0 = clock64();
           int spins = 0;
@@ -445,26 +425,8 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
             uint64_t ready = pending;
             if (s > 0) {
               if (p.sync_mode == 1) {
-                const unsigned int v = p.poll_acquire ? tc::ld_acquire_gpu(p.sync + mb) : tc::ld_relaxed_gpu(p.sync + mb);
+                const unsigned int v = tc::ld_relaxed_gpu(p.sync + mb);
                 ready = ((int)(v - (unsigned)s * (unsigned)p.tiles_n) >= 0) ? pending : 0ull;
-              } else if (p.sync_mode == 2) {
-                const unsigned int* fl = p.sync + kSyncFlags + (size_t)mb * p.tiles_n;
-                if (kBwd) {                                       // k-block kb_base + lane is written by CTA kb_base + lane
-                  bool r0 = false;
-                  if (lane < num_kb) r0 = (int)(tc::ld_relaxed_gpu(fl + kb_base + lane) - (unsigned)s) >= 0;
-                  ready = (uint64_t)__ballot_sync(0xffffffffu, r0);
-                } else {                                          // k-block j is written by CTAs 4j..4j+3; lane L reads flags 2L, 2L+1
-                  bool r0 = false;
-                  if (2 * lane < p.tiles_n) {
-                    const uint2 v2 = tc::ld_relaxed_gpu_v2(fl + 2 * lane);
-                    r0 = ((int)(v2.x - (unsigned)s) >= 0) && ((int)(v2.y - (unsigned)s) >= 0);
-                  }
-                  const unsigned int b = __ballot_sync(0xffffffffu, r0);
-                  unsigned int pr = b & (b >> 1) & 0x55555555u;   // bit 2j set <=> k-block j complete
-                  pr = (pr | (pr >> 1)) & 0x33333333u; pr = (pr | (pr >> 2)) & 0x0f0f0f0fu;
-                  pr = (pr | (pr >> 4)) & 0x00ff00ffu; pr = (pr | (pr >> 8)) & 0x0000ffffu;
-                  ready = pr >> kb_base;
-                }
               } else {
                 bool r0 = false, r1 = false;
                 if (lane < num_kb) r0 = (int)(tc::ld_relaxed_gpu(ctr + lane * 32) - target) >= 0;
@@ -472,7 +434,7 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
                 ready = (uint64_t)__ballot_sync(0xffffffffu, r0) | ((uint64_t)__ballot_sync(0xffffffffu, r1) << 32);
               }
               ready &= pending;
-              if (p.debug_mode == 3) {                            // experiment: in-order issue (lowest pending block first)
+              if (p.in_order) {                                   // lowest pending block first
                 const uint64_t low = pending & (~pending + 1ull);
                 ready = (ready & low) ? low : 0ull;
               }
@@ -524,8 +486,7 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
           else if (clock64() - t_abort > kAbortGrace) {
             if (lane == 0) atomicExch(reinterpret_cast<int*>(p.sync + kSyncErr), 2);
             __threadfence_system();
-            if (!p.no_trap) __trap();
-            break;
+            __trap();
           }
         }
       }
@@ -587,13 +548,13 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
       // has seen those of step n: every earlier item of the ring has then landed.  (Bounded wait: mbarrier, not bar.sync.)
       const int turn = kBwd ? dstep - 1 : dstep;       // this warpgroup's tile-steps before this one
       if (kPP && (half == 1 || turn > 0) &&
-          !wait_bar<false>(&ss->mma_turn[half], (uint32_t)((half ? turn : turn - 1) & 1), abort_flag))
+          !wait_bar(&ss->mma_turn[half], (uint32_t)((half ? turn : turn - 1) & 1), abort_flag))
         return false;
       // ring staging: the last kAccPieces stages of the tile stay borrowed (no empty arrival) until acc_release
       const int borrow = ring_acc ? kAccPieces : 0;
       uint32_t prev = 0;
       for (int kb = 0; kb < num_kb; ++kb) {
-        if (!tc::mbar_try_wait_u32(full0 + 8 * stage, phase) && !wait_bar<false>(&ss->full[stage], phase, abort_flag)) {
+        if (!tc::mbar_try_wait_u32(full0 + 8 * stage, phase) && !wait_bar(&ss->full[stage], phase, abort_flag)) {
           tc::wgmma_wait<0>();                           // no MMA may still be writing the accumulator when it goes out of scope
           return false;
         }
@@ -694,12 +655,8 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
       if constexpr (kPP) wg_bar();
       else asm volatile("bar.sync 1, 256;" ::: "memory");
     };
-    // exchange-buffer barriers: filled by st.async (async proxy, like a TMA load) / freed by relaxed arrives, so a CTA-scope
-    // wait is enough; the cluster-scope acquire form (debug_mode 7, the earlier default) adds a CCTL.IVALL per wait
-    const bool cluster_acquire = p.debug_mode == 7;
-    auto xwait = [&](uint64_t* bar, uint32_t parity, volatile int* af) {
-      return cluster_acquire ? wait_bar<true>(bar, parity, af) : wait_bar<false>(bar, parity, af);
-    };
+    // (exchange-buffer barriers: filled by st.async (async proxy, like a TMA load) / freed by relaxed arrives, so wait_bar's
+    // CTA-scope wait is enough for them)
     // MEMBAR.ALL.GPU (the release of the dataflow signal) drains EVERY outstanding store of the SM, not just the signalling
     // thread's: if the other threads of the tile start their bookkeeping stores (h_seq / c_seq / activations) meanwhile, the
     // signal - the only thing the other CTAs wait for - is held back by 1-3 us (measured).  They wait for it instead.
@@ -759,7 +716,7 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
           for (int u = 0; u < kPass; ++u) {
             const __nv_bfloat16* gp = p.gx + ((size_t)tt * B + row) * (4 * H) + n0(u);
             gxw[u][0] = ldg_nc32(gp); gxw[u][1] = ldg_nc32(gp + 16);
-            if (t + 2 < p.T && p.debug_mode != 6)      // the x-projection comes from HBM: pull it into L2 early
+            if (t + 2 < p.T)                           // the x-projection comes from HBM: pull it into L2 early
               prefetch_l2(kRev ? gp - (size_t)2 * B * (4 * H) : gp + (size_t)2 * B * (4 * H));
           }
         }
@@ -781,7 +738,7 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
             acc_ld32(32 * chalf + 64 * (1 - ks), w32);
             acc_ld32(32 * chalf + 64 * ks, v);
             if (t > 0) {                                               // the peer has consumed last step's partial
-              ok = xwait(&ss->xchg_free[0], (uint32_t)((t - 1) & 1), abort_flag);
+              ok = wait_bar(&ss->xchg_free[0], (uint32_t)((t - 1) & 1), abort_flag);
               if (!ok) break;
             }
             const uint32_t drow = tc::mapa(xbase + (uint32_t)(rloc * 128), (uint32_t)(1 - ks));
@@ -792,7 +749,7 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
               for (int k = 0; k < 4; ++k) pk[k] = pack_bf2(__uint_as_float(w32[8 * i + 2 * k]), __uint_as_float(w32[8 * i + 2 * k + 1]));
               st_async_u4(drow + (uint32_t)((((4 * chalf + i) ^ (rloc & 7))) * 16), make_uint4(pk[0], pk[1], pk[2], pk[3]), pbar);
             }
-            ok = xwait(&ss->xchg_full[0], xphase, abort_flag);
+            ok = wait_bar(&ss->xchg_full[0], xphase, abort_flag);
             if (!ok) break;
             xphase ^= 1;
 #pragma unroll
@@ -856,7 +813,6 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
           }
           // this CTA's 16 hidden units = a quarter of k-block nb/4
           if (p.sync_mode == 1) tc::signal_counter(p.sync + mb);
-          else if (p.sync_mode == 2) tc::st_release_gpu(p.sync + kSyncFlags + (size_t)mb * p.tiles_n + in_mb, (unsigned)(t + 1));
           else tc::signal_counter(p.sync + kSyncKb + ((size_t)mb * (H / BK) + (in_mb >> 2)) * 32);
           if (dbg_wg) dbg_stamp(t, 2);
         }
@@ -866,7 +822,7 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
           tc::mbar_arrive_remote_relaxed(tc::mapa(fbar, (uint32_t)(1 - ks)));
         }
         signal_sent_bar();
-        if (valid && p.debug_mode != 5) {              // everything below is off the critical path
+        if (valid) {                                   // everything below is off the critical path
           const size_t srow = kRev ? (size_t)tt : (size_t)(t + 1);      // state row written by this step
 #pragma unroll
           for (int u = 0; u < kPass; ++u) {
@@ -1022,7 +978,7 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
             // A member only needs the dG blocks of ITS K-quarter, so nothing in the dataflow stops a fast member from being a
             // whole step ahead of a slow one: explicit back-pressure before overwriting anybody's exchange buffer.
             if (s > 1) {
-              ok = xwait(&ss->xchg_free[xt], (uint32_t)(s & 1), abort_flag);
+              ok = wait_bar(&ss->xchg_free[xt], (uint32_t)(s & 1), abort_flag);
               if (!ok) break;
             }
             // reduce-scatter over the kSplit K parts: column chunk q (16 wide, bf16) goes to member q's slot [ks] (DSMEM)
@@ -1038,7 +994,7 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
                 st_async_u4(dst + 16, make_uint4(a[4], a[5], a[6], a[7]), dbar);
               }
             }
-            ok = xwait(&ss->xchg_full[xt], xphase, abort_flag);
+            ok = wait_bar(&ss->xchg_full[xt], xphase, abort_flag);
             if (!ok) break;
 #pragma unroll
             for (int u = 0; u < kPass; ++u) {
@@ -1120,7 +1076,6 @@ lstm_seq_kernel(const __grid_constant__ CUtensorMap tmap_w, const SeqParams p) {
         if (gtid == 0) {
           // this CTA's 64 gate columns = dG k-block 4 nb + ks
           if (p.sync_mode == 1) tc::signal_counter(p.sync + mb);
-          else if (p.sync_mode == 2) tc::st_release_gpu(p.sync + kSyncFlags + (size_t)mb * p.tiles_n + in_mb, (unsigned)(s + 1));
           else tc::signal_counter(p.sync + kSyncKb + ((size_t)mb * (4 * H / BK) + in_mb) * 32);
           if (dbg_wg) dbg_stamp(s, 2);
         }
@@ -1299,8 +1254,12 @@ int pick_stages(int H, bool bwd, int tiles, bool xl2 = false) {
 }  // namespace
 
 // sync_ws: kSyncWords u32 (layout above); everything but the sticky error flag in the last word is zeroed before every launch.
-// variant (tuning knob, 0 = defaults) = tiles_per_cta + 16*stages + 4096*debug_mode:  tiles_per_cta 0 -> 1 (set 2 to let a
-// CTA alternate two batch tiles);  stages 0 -> deepest ring that fits next to the resident weight slice.
+// variant (tuning knob, 0 = defaults), bit fields:
+//   [0:4)    batch tiles per CTA: 2 lets a CTA alternate two batch tiles, any other value means 1;
+//   [4:8)    ring stages: 0 = the deepest ring that fits next to the resident weight slice (pick_stages);
+//   [12:15)  3 = in-order operand stream (SeqParams::in_order), 0 = arrival order;
+//   bit 16   one arrival counter per batch tile instead of one per operand k-block (SeqParams::sync_mode).
+// seq_config refuses a variant with any other bit set or another value in [12:15).
 struct SeqCfg {
   int stages, tiles;
   bool stream, fsplit;
@@ -1311,12 +1270,17 @@ struct SeqCfg {
 // xl2: the backward kernel with the L2 exchange (kXchgL2; one tile per CTA, resident weights).
 static int seq_config(bool bwd, int H, int B, int variant, SeqCfg& c, bool xl2 = false) {
   if (H % 64 != 0) { ts::set_last_error("lstm_seq: H must be a multiple of 64"); return -2; }
+  const int order = (variant >> 12) & 7;
+  if ((variant & ~(0xff | (7 << 12) | (1 << 16))) != 0 || (order != 0 && order != 3)) {
+    ts::set_last_error("lstm_seq: unsupported variant (fields: [0:8) tiles and stages, [12:15) 0 or 3 = in order, bit 16 counter per tile)");
+    return -2;
+  }
   const int tiles_m = (B + BM - 1) / BM;
   int stages = (variant >> 4) & 15, tiles = variant & 15;
   if (tiles != 2 || tiles_m % 2 != 0) tiles = 1;
   // resident weight slice up to H = 1152 (forward) / 1024 (backward; cuda_lstm._bwd_cluster and _tiles_per_cta assume this
   // boundary), else stream the weights through the ring
-  const bool stream = H > (bwd ? 1024 : 1152) || ((variant >> 8) & 1);
+  const bool stream = H > (bwd ? 1024 : 1152);
   if (stream) tiles = 1;
   if (bwd && stream && 4 * H / (2 * BK) > 64) { ts::set_last_error("lstm_seq: streamed backward needs H <= 2048"); return -2; }
   if (xl2 && (!bwd || stream || tiles != 1)) {
@@ -1331,8 +1295,8 @@ static int seq_config(bool bwd, int H, int B, int variant, SeqCfg& c, bool xl2 =
     ts::set_last_error("lstm_seq: the k-block arrival counters of this layout do not fit in the sync workspace");
     return -2;
   }
-  // forward: 2-way K split (cluster of 2) unless disabled by variant bit 19
-  const bool fsplit = !bwd && !stream && tiles == 1 && H % 128 == 0 && !((variant >> 19) & 1) &&
+  // forward: 2-way K split (cluster of 2)
+  const bool fsplit = !bwd && !stream && tiles == 1 && H % 128 == 0 &&
                       smem_bytes(H, false, 3, 1, false, true) <= 227 * 1024;
   if (stream) {
     if (stages != 4 && stages != 6 && stages != 8) stages = smem_bytes(H, bwd, 8, 1, true) <= 227 * 1024 ? 8 : 6;
@@ -1362,10 +1326,8 @@ static int seq_common(SeqParams& p, const void* w_base, int variant, cudaStream_
   const int stages = cfg.stages, tiles = cfg.tiles;
   const bool stream = cfg.stream, fsplit = cfg.fsplit;
   const int tiles_m = (B + BM - 1) / BM, tiles_n = kBwd ? (H / BN) * 4 : 4 * H / BN;
-  p.debug_mode = (variant >> 12) & 7;
-  p.sync_mode = (variant >> 16) & 3;
-  p.poll_acquire = (variant >> 18) & 1;
-  p.no_trap = (variant >> 20) & 1;
+  p.in_order = ((variant >> 12) & 7) == 3;
+  p.sync_mode = (variant >> 16) & 1;
   int dev = 0;
   cudaGetDevice(&dev);
   const int grid = (tiles_m / tiles) * tiles_n;

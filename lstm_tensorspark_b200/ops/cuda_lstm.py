@@ -24,11 +24,10 @@ from . import cuda_gemm as G
 _SYNC_WS = {}
 _SM_COUNT = {}
 FORCE_GENERIC = os.environ.get("LSTM_TS_FORCE_GENERIC", "0") == "1"
-# Tuning / experiment knob of the persistent kernels (0 = defaults), bit fields as decoded in csrc/lstm_seq_wgmma.cu seq_common():
-#   [0:4) batch tiles per CTA (2 = one CTA alternates two tiles), [4:8) ring stages, bit 8 force streamed weights,
-#   [12:15) timing-only debug mode (1 skip loads, 2 skip MMAs, 3 in-order stream, 4 half-size loads, 5 no bookkeeping stores,
-#   6 no L2 prefetch, 7 cluster-scope acquire on the exchange barriers), [16:18) sync mode (0 per-k-block dataflow counters,
-#   1 one counter per batch tile = grid barrier, 2 per-CTA flags), bit 18 acquire polls, bit 19 no forward K-split.
+# Tuning knob of the persistent kernels (0 = defaults), bit fields as decoded in csrc/lstm_seq_wgmma.cu seq_config():
+#   [0:4) batch tiles per CTA (2 = one CTA alternates two tiles), [4:8) ring stages (0 = auto), [12:15) 3 = in-order operand
+#   stream (--deterministic), bit 16 sync mode (0 per-k-block dataflow counters, 1 one counter per batch tile = grid barrier).
+#   The kernels refuse any other bit, and any other value in [12:15).
 SEQ_VARIANT = int(os.environ.get("LSTM_TS_SEQ_VARIANT", "0"))
 
 

@@ -1,9 +1,10 @@
 """A backward recurrence that has the GPU to itself runs one batch tile per CTA with its K-split reduce-scattered through L2
 instead of a cluster's DSMEM (csrc/lstm_seq_wgmma.cu kXchgL2; ops/cuda_lstm.py bwd_tiles_per_cta): at B = 256, H = 1024 that
 is 128 CTAs on an H100 instead of the 64 two-tile CTAs its clusters of 4 fit.  The tile choice, the side-GEMM split of the
-pipelined pair and the ring depths are host logic (no GPU).  On the GPU (`pytest -m gpu`) the L2 exchange is held bit for
-bit against the clustered one-tile kernel where both fit, and the single-layer op and the pipelined layer pair that take
-the path against fp64 within the bf16 budget of tests/lstm_numerics.py."""
+pipelined pair, the ring depths and the variant fields the kernels accept are host logic (no GPU).  On the GPU
+(`pytest -m gpu`) the L2 exchange is held bit for bit against the clustered one-tile kernel where both fit, and the
+single-layer op and the pipelined layer pair that take the path against fp64 within the bf16 budget of
+tests/lstm_numerics.py."""
 import pytest
 import torch
 
@@ -64,6 +65,16 @@ def test_l2_exchange_configs():
     assert E.lstm_seq_config(True, 768, 640, 0)[1] == 1
     with pytest.raises(RuntimeError, match="sync workspace"):
         E.lstm_seq_config(True, 768, 640, 0, True)
+    # the variant's fields: [0:4) tiles per CTA, [4:8) ring stages, [12:15) = 3 the in-order stream, bit 16 one counter per
+    # batch tile.  Any other bit, or another value in [12:15), is refused.
+    for bwd, want in ((False, {3 << 12: (4, 1, False, False), 1 << 16: (4, 1, False, False), 2 + 16 * 4: (4, 2, False, False)}),
+                      (True, {3 << 12: (5, 1, False, False), 1 << 16: (5, 1, False, False), 2 + 16 * 4: (4, 2, False, False)})):
+        for var, cfg in want.items():
+            assert E.lstm_seq_config(bwd, 1024, 256, var) == cfg, (bwd, var)
+        refused = [m << 12 for m in (1, 2, 4, 5, 6, 7)] + [2 << 16, 3 << 16] + [1 << b for b in (8, 9, 15, 18, 19, 20, 21, 30)]
+        for var in refused + [2 + 16 * 4 + (1 << 19), (3 << 12) | (1 << 20), -1]:
+            with pytest.raises(RuntimeError, match="unsupported variant"):
+                E.lstm_seq_config(bwd, 1024, 256, var)
 
 
 # ---- on the GPU ------------------------------------------------------------------------------------------------------------
